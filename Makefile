@@ -1,6 +1,6 @@
-# Builds dgraph_b200/libdgx.so (sm_100a only) and the CPU oracle.
+# Builds dgraph_b200/libdgx.so (sm_90a only: H100) and the CPU oracle.
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS ?= -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-maybe-uninitialized -Xptxas -v
 CSRC := dgraph_b200/csrc
 HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.hpp) include/dgx.h

@@ -1,12 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the posting-list set-op hot path on B200.
+"""bench.py -- headline benchmark of the posting-list set-op hot path on H100.
 
 Workload (BASELINE.json configs[1]): k-way algo.IntersectSorted, k = 8 Zipf-gap lists of ~1e6 UIDs each
 (independent thinnings, p = 0.25, of a shared 4e6 master), as a batch of Q independent queries per GPU per
-step so that one step's inputs (Q x 64 MB) exceed the 126 MB L2.  Metric: input UIDs intersected per
+step so that one step's inputs (Q x 64 MB) exceed the 50 MB L2.  Metric: input UIDs intersected per
 second, bit-exact vs the CPU oracle (every query of the step is checked).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c2dense]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c2dense] [--dump-outputs DIR]
+
+--dump-outputs DIR writes what the last timed step returned to its caller -- the per-query result offsets and the
+intersected UIDs -- as DIR/<name>.npy (float64), so that two builds can be compared output for output on the same
+seeded inputs.
 
 value   device-resident: lists already in HBM, one batched launch per step, CUDA events on the launching stream.
 e2e     the same step through the host-pointer C ABI, HOST buffers, copies inside the timed region.  The
@@ -132,7 +136,7 @@ def workload_config(q: int, world: int, workload: str = "c2"):
         "workload": f"configs[1]: k-way IntersectSorted, k=8 Zipf-gap lists of ~1e6 UIDs ({desc}), "
                     f"batch of {q} independent queries per GPU per step",
         "k": K_LISTS, "list_len": LIST_LEN, "queries_per_gpu": q, "parallelism": f"queries sharded over {world} GPU(s)",
-        "l2": f"inputs {q * K_LISTS * LIST_LEN * 8 / 1e9:.2f} GB per GPU per step > 126 MB L2 (no flush needed)",
+        "l2": f"inputs {q * K_LISTS * LIST_LEN * 8 / 1e9:.2f} GB per GPU per step > 50 MB L2 (no flush needed)",
         "lists": "resident in HBM and declared so to the lane (dgx_lane_set_resident_inputs): the plan pre-pass of a step overlaps the previous step's kernel",
     }
 
@@ -338,6 +342,30 @@ def run_e2e_legs(args, lib, queries, want, uids_all, uids_per_step, rank, world,
     return e2e, e2e_cached, e2e_raw, bool(ok_packed and ok_cached and ok_raw)
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, buf, q: int, rank: int, world: int) -> None:
+    """The last timed step's results as a caller of dgx_dev_filter_batch receives them: `offsets` (Q + 1 result
+    offsets) and `uids` (the concatenated intersections), float64.  UIDs above 2^53 would not survive the
+    conversion, so they are refused.  Past 64 MB the UIDs are a fixed sample (seed 0, sorted positions, stored as
+    `uids_index`)."""
+    host = buf.cpu().numpy().view(np.uint64)
+    off = host[: q + 1]
+    uids = host[q + 1: q + 1 + int(off[q])]
+    if uids.size and int(uids.max()) > (1 << 53):
+        raise SystemExit("--dump-outputs: UIDs above 2^53 cannot be written as float64")
+    arrays = {"offsets": off.astype(np.float64)}
+    room = (DUMP_BYTES - arrays["offsets"].nbytes) // 8
+    if uids.size > room:
+        idx = np.sort(np.random.default_rng(0).choice(uids.size, size=room // 2, replace=False))
+        arrays["uids_index"], uids = idx.astype(np.float64), uids[idx]
+    arrays["uids"] = uids.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    suffix = "" if world == 1 else f"_rank{rank}"
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}{suffix}.npy"), a)
+
 
 def main():
     ap = argparse.ArgumentParser()
@@ -353,7 +381,13 @@ def main():
     ap.add_argument("--no-dense", action="store_true", help="skip the p=0.9 variant of the headline step")
     ap.add_argument("--no-resident", action="store_true", help="do not declare the lists resident (no pre-pass / pipeline overlap across steps)")
     ap.add_argument("--no-e2e", action="store_true", help="kernel iteration runs only: skip the end-to-end legs (the line then has no e2e)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results (offsets, uids) to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the device path's results; the reference arm has none to write")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
 
     rank = int(os.environ.get("RANK", "0"))
@@ -504,6 +538,10 @@ def main():
     torch.cuda.synchronize()
     sampler.active = False
     rc_sync = lib.dgx_lane_sync(lane)                        # DGX_ERR_CAP here = some step overflowed out_cap
+    if args.dump_outputs:
+        if rc_sync != 0:   # a step overflowed out_cap: the buffers hold truncated results, which are not written
+            raise SystemExit(f"--dump-outputs: the timed steps failed ({lib.dgx_last_error().decode()}); nothing written")
+        dump_outputs(args.dump_outputs, bufs[(args.steps - 1) % NBUF], Q, rank, world)
     if world > 1:
         dist.barrier()
     clocks = sampler.stop()
@@ -531,7 +569,7 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
     algo_bytes = 8.0 * (uids_per_step + out_uids)  # 8*(sum|L_i| + |Out|), SURVEY 8(d)
     kern_ms = float(np.median(step_ms)) if world == 1 else ms_per_step
     achieved = algo_bytes / (kern_ms * 1e-3) / 1e9

@@ -1,4 +1,4 @@
-"""dgraph_b200: B200-native (sm_100a CUDA) posting-list set operations and
+"""dgraph_b200: H100-native (sm_90a CUDA) posting-list set operations and
 UidPack decode -- the drop-in for dgraph's algo/ + codec/ hot path.
 
 The product is dgraph_b200/libdgx.so behind include/dgx.h; the modules here are

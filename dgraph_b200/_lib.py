@@ -1,4 +1,4 @@
-"""ctypes loader for libdgx.so (the sm_100a CUDA library behind include/dgx.h).
+"""ctypes loader for libdgx.so (the sm_90a CUDA library behind include/dgx.h).
 
 There is deliberately NO fallback: if the shared library is missing or CUDA is
 unavailable, every product entry point raises.  Build with `make` or

@@ -1,4 +1,4 @@
-"""Host-side mirror of dgraph's `algo` package over libdgx (sm_100a CUDA).
+"""Host-side mirror of dgraph's `algo` package over libdgx (sm_90a CUDA).
 
 Same function names, argument meaning and result shapes as
 /root/reference/algo/uidlist.go; every body is one C-ABI call into libdgx.so

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the dgx kernels (sm_100a only).
+// common.cuh -- shared device helpers for the dgx kernels (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// decode_kernel.cuh -- group-varint UidPack decode for sm_100a.
+// decode_kernel.cuh -- group-varint UidPack decode for sm_90a.
 //
 // codec.Decode / Decoder.UnpackBlock (codec/codec.go:154-200, 444-452): block b
 // yields Base, then running sums of its group-varint u32 deltas, truncated to

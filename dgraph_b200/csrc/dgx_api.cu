@@ -1,4 +1,4 @@
-// dgx_api.cu -- libdgx.so: C ABI (include/dgx.h) over the sm_100a kernels.
+// dgx_api.cu -- libdgx.so: C ABI (include/dgx.h) over the sm_90a kernels.
 //
 // Host responsibilities only: lane (stream + workspace) management, building the
 // small task / list descriptor tables the kernels read, host<->device copies for
@@ -82,18 +82,18 @@ constexpr u32 kScapMin = 8192, kScapMax = 65536;  // bytes
 static int g_filter_pipe = 1;          // DGX_FILTER=v4 selects the non-persistent kernel
 static int g_merge_multi = 1;          // DGX_MERGE=tree forces the pairwise merge tree
 static int g_merge_lag = 0;            // DGX_MERGE_LAG: a merge CTA moves the tile this many tiles back to the output; 0 = scan + compact kernels
-                                       // (default: measured faster, 1.655 vs 1.69 ms at 888 on C5 -- the copy is not hidden under the merging)
+                                       // (default: the copy phase is not hidden under the merging, so the separate kernels are no slower)
 static int g_merge_ahead = -1;         // DGX_MERGE_AHEAD: L2 prefetch distance in tiles (-1 = 3 x SM count, the resident CTAs; 0 = off)
 static int g_merge_t32 = 1;            // DGX_MERGE=levels: the round-1 pipeline (64-bit levels engine, boundary-major bounds)
 static u32 g_merge_stride = 0;         // DGX_MERGE_STRIDE: sample gaps per multiway-merge tile (tile ~ 512 x stride values); 0 = 10 for the
                                        // 32-bit engine (7680-slot rounds), 6 for DGX_MERGE=levels (4096-slot rounds)
-static int g_zero_copy = 0;            // DGX_ZERO_COPY=1: decode pinned packs in place over PCIe (measured slower than DMA: 35 vs 43 GB/s)
+static int g_zero_copy = 0;            // DGX_ZERO_COPY=1: decode pinned packs in place over PCIe (off: DMA copies move the bytes faster)
 static size_t g_merge_multi_min = size_t(1) << 18;  // totals below this stay on the tree (fewer launches)
 static size_t g_pre_throttle_smem = 0;  // DGX_PRE_THROTTLE: dynamic smem asked for by an ahead-of-time pre-pass (0 = unthrottled)
 static u32 g_reserve_ctas = 0;         // DGX_RESERVE_CTAS: pipeline CTAs left out of the persistent grid
 static uint64_t g_pipe_min_values = 0;  // DGX_PIPE_MIN_VALUES: batches driving fewer values than this use filter_kernel
 static size_t g_pipe_min_k = 2;        // DGX_PIPE_MIN_K: batches whose widest query has fewer lists use filter_kernel
-static int g_num_sms = 148;
+static int g_num_sms = 132;
 constexpr size_t kPipeSmemMax = 220 * 1024;
 
 // ---------------------------------------------------------------------------
@@ -258,8 +258,9 @@ extern "C" int dgx_init(int device) {
     CK(cudaSetDevice(device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10)
-        return fail(DGX_ERR_NODEV, "libdgx is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+    // the library carries sm_90a code only (no PTX), which loads on compute capability 9.0 and nothing else
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(DGX_ERR_NODEV, "libdgx is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
     CK(cudaFuncSetAttribute(decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)(sizeof(DWarpSmem) * D_WARPS)));
     CK(cudaFuncSetAttribute(decode_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -299,7 +300,7 @@ extern "C" int dgx_describe(char* buf, size_t n) {
     if (rc != DGX_OK) return rc;
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, g_device));
-    snprintf(buf, n, "libdgx sm_100a | device %d: %s, %d SMs, %.1f GB | filter tile %d, merge tile %d",
+    snprintf(buf, n, "libdgx sm_90a | device %d: %s, %d SMs, %.1f GB | filter tile %d, merge tile %d",
              g_device, prop.name, prop.multiProcessorCount, prop.totalGlobalMem / 1e9, F_TA, M_T);
     return DGX_OK;
 }
@@ -617,8 +618,8 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
         if (rc) return rc;
         CK(cudaMemcpyAsync(d_pb, h_pb, nq * sizeof(u64), cudaMemcpyHostToDevice, pre));
         // DGX_PRE_THROTTLE: dynamic shared memory an ahead-of-time pre-pass asks for (16 KB would limit it to one CTA on
-        // an SM that holds two pipeline CTAs).  Measured: no effect (0.3559 vs 0.3565 ms) -- what the overlap costs the
-        // pipeline is L2 / DRAM interference, not issue slots -- so the default is 0.
+        // an SM that holds two pipeline CTAs).  What the overlap costs the pipeline is L2 / DRAM interference, not issue
+        // slots, so throttling the pre-pass does not help and the default is 0.
         const size_t pre_smem = ahead ? g_pre_throttle_smem : 0;
         filter_tiles_kernel<<<(unsigned)((ntiles + 255) / 256), 256, pre_smem, pre>>>(P.tasks, P.lists, (const u64*)d_pb, P.ntasks,
                                                                                       P.ntiles, (PTileEntry*)d_tiles, (u32)tile_sz);
@@ -639,8 +640,8 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
         PP.plan_base = (const u64*)d_pb;
         PP.plan = (const PPlanEntry*)d_plan;
         PP.tiles = (const PTileEntry*)d_tiles;
-        // wide queries: one tile per ticket keeps the look-back order tight (measured 0.476 vs 0.50 ms on
-        // C2); 2-list batches have tiny tiles and amortise the metadata chain over two (measured +4 %)
+        // wide queries: one tile per ticket keeps the look-back order tight; 2-list batches have tiny tiles and
+        // amortise the metadata chain over two
         PP.grp = kmax >= 4 ? 1u : 2u;
         const size_t nl = std::min<size_t>(std::max<size_t>(kmax - 1, 1), P_MAXL);
         const size_t TA = (size_t)tile_sz;
@@ -1725,7 +1726,7 @@ static std::mutex g_cache_mu;
 static std::unordered_map<CacheKey, CacheEntry*, CacheKeyHash> g_cache;
 static std::list<CacheEntry*> g_cache_lru;  // front = most recently used
 static size_t g_cache_bytes = 0;
-static size_t g_cache_max = size_t(32) << 30;  // DGX_CACHE_BYTES / dgx_cache_configure
+static size_t g_cache_max = size_t(16) << 30;  // DGX_CACHE_BYTES / dgx_cache_configure (a fifth of an 80 GB H100)
 static bool g_cache_env_read = false;
 static dgx_cache_stats g_cache_stats = {0, 0, 0, 0, 0, 0};
 

@@ -1,4 +1,4 @@
-// filter_kernel.cuh -- batched "A-driven" sorted-set filter for sm_100a.
+// filter_kernel.cuh -- batched "A-driven" sorted-set filter for sm_90a.
 //
 // One kernel covers algo.IntersectWith (algo/uidlist.go:142), the whole chain of
 // algo.IntersectSorted (:297-329, k lists in ONE pass), algo.Difference (:332)

@@ -2,7 +2,7 @@
 //
 // Same contract as filter_kernel.cuh (IntersectWith / IntersectSorted chain /
 // Difference over a batch of queries, bit-exact incl. duplicate semantics), built
-// as a Blackwell pipeline:
+// as a TMA / mbarrier pipeline (Hopper's bulk copies, no register staging):
 //
 //   filter_tiles_kernel  one thread per tile: owning task, driving offset, plan index,
 //                        predecessor value -> a tile table in HBM.
@@ -39,7 +39,7 @@ namespace dgx {
 
 // Tile geometry is a template parameter of the kernel: VA candidate rows per consumer warp, 32 VA candidates per
 // warp, 8 consumer warps, 256 VA candidates per tile.  Wide queries (k >= 3) run VA = 2 (512-value tiles: more
-// tiles in flight per byte of shared memory, measured best on C2); 2-list batches run VA = 4 (1024-value tiles:
+// tiles in flight per byte of shared memory); 2-list batches run VA = 4 (1024-value tiles:
 // their per-tile costs -- metadata, TMA issue, look-back, delivery -- are spread over twice the values).
 constexpr int P_CW = 8;                  // consumer warps
 constexpr int P_CT = P_CW * 32;          // consumer threads
@@ -53,12 +53,12 @@ constexpr int p_tile_size(int va) { return P_CW * 32 * va; }
 #ifndef DGX_P_OS
 #define DGX_P_OS 6
 #endif
-constexpr int P_OS = DGX_P_OS;           // output slots in flight (6 vs 4: 2-list batches +4.5 %, C2 unchanged)
+constexpr int P_OS = DGX_P_OS;           // output slots in flight (more slots let 2-list batches, whose tiles finish fast, run ahead of the look-back)
 #ifndef DGX_P_ST
 #define DGX_P_ST 2
 #endif
 #ifndef DGX_PLAN_4ARY
-#define DGX_PLAN_4ARY 0   // 1: 4-ary plan searches (half the dependent latencies, 1.5x the probes) -- measured 2.4 % SLOWER on C2
+#define DGX_PLAN_4ARY 0   // 1: 4-ary plan searches (half the dependent latencies, 1.5x the probes; off: the extra probes cost more)
 #endif
 #ifndef DGX_P_PAIR2
 #define DGX_P_PAIR2 1   // two-row warps search two lists per iteration (four chains) once past the first list
@@ -73,7 +73,7 @@ constexpr int P_GRP = 4;                 // most tiles the metadata warp can res
 constexpr u32 P_END = 0xffffffffu;
 // Back-off between polls of a waiting helper warp (ns): TMA warp / metadata + output warps / look-back.
 // The helpers share schedulers with consumer warps and every poll is an issue slot taken from them
-// (polling was 14 % of the issued instructions at 128 ns); measured -0.8 % (C2) / -2 % (C1 batch).
+// (with short sleeps, polling takes a visible share of the issued instructions).
 #ifndef DGX_P_SLEEP_T
 #define DGX_P_SLEEP_T 600
 #endif
@@ -684,8 +684,7 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
 #if DGX_P_PAIR2
                     // (only after the first list: a warp that still fills two rows then has lost less than half of its
                     //  candidates, so the second search is rarely wasted; sparse workloads drop to one row and take
-                    //  the three-list path below -- measured: always pairing costs C2 6 %, never pairing costs the
-                    //  dense variant 24 %)
+                    //  the three-list path below; always pairing slows sparse queries, never pairing slows dense ones)
                     if (rows == 2 && t >= 1 && t + 1 < km1 && G.n[t] != 0 && G.n[t + 1] != 0 &&
                         (G.n[t] > G.n[t + 1] ? G.n[t] : G.n[t + 1]) <= 3u << (31 - __clz(G.n[t] < G.n[t + 1] ? G.n[t] : G.n[t + 1]))) {
                         // ---- two rows against TWO lists at once (four chains; the second list is searched for

@@ -1,4 +1,4 @@
-// merge_kernel.cuh -- batched 2-way sorted union with de-duplication (sm_100a).
+// merge_kernel.cuh -- batched 2-way sorted union with de-duplication (sm_90a).
 //
 // Building block of algo.MergeSorted (algo/uidlist.go:448-542): the reference
 // pops a k-way heap and drops a value equal to the last one written (:409-412),

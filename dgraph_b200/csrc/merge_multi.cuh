@@ -1,4 +1,4 @@
-// merge_multi.cuh -- single-pass multiway MergeSorted (k <= 64 runs) for sm_100a.
+// merge_multi.cuh -- single-pass multiway MergeSorted (k <= 64 runs) for sm_90a.
 //
 // algo.MergeSorted (algo/uidlist.go:448-542) pops a k-way heap and drops values equal
 // to the last one written: a sorted union with global de-duplication.  A pairwise

@@ -13,8 +13,8 @@
 //                   instructions of the 64-bit levels per slot.  Tiles whose span does not fit 32 bits use the 64-bit
 //                   engine of merge_multi.cuh (mm_levels_tile) in the same kernel.
 // An LSD radix sort of the tile (8-bit digits, match.any ranking) and a decoupled look-back straight to the final
-// position were built and measured first (profiles/README.md): ~3 warp-instructions per value and pass for the sort,
-// and in-order retirement behind the slowest tile for the look-back; both slower than this.
+// position were built first: ~3 warp-instructions per value and pass for the sort, and in-order retirement behind
+// the slowest tile for the look-back; both slower than this.
 // algo.MergeSorted: algo/uidlist.go:448-542.
 #pragma once
 
@@ -30,7 +30,7 @@ constexpr size_t T_SMEM_32 = (size_t)2 * T_C * sizeof(u32);
 constexpr size_t T_SMEM_64 = (size_t)2 * MM_CP * sizeof(u64);
 constexpr size_t T_SMEM = T_SMEM_32 > T_SMEM_64 ? T_SMEM_32 : T_SMEM_64;
 #ifndef DGX_T_PIECE
-#define DGX_T_PIECE 128  // 256 measured slower (1.677 vs 1.642 ms on C5)
+#define DGX_T_PIECE 128  // slots per load piece (256-slot pieces balance the runs less evenly)
 #endif
 constexpr int T_PIECE = DGX_T_PIECE;         // slots per load piece (T_PIECE / 32 independent loads per lane)
 constexpr int T_NCH = T_VT * (T_NT / 32);   // 32-position chunks of a round (de-duplication scan)
@@ -349,12 +349,12 @@ __device__ __noinline__ u32 t32_tile(u32* s_k, const u64* const* s_ptr, u64* s_c
 
 // ---- lagged compaction (optional: DGX_MERGE_LAG > 0; default is mscan_kernel + mcompact_kernel) --------------------
 // A tile's place in the output is the sum of the counts of the tiles before it, known only when they are all done.
-// Waiting for it at the end of a tile retires the CTAs in order (measured: half the kernel's time spent waiting behind
+// Waiting for it at the end of a tile retires the CTAs in order (much of the kernel's time is then spent waiting behind
 // the slowest tile).  Here a tile writes its keys to scratch, publishes its count, and the CTA that starts P.lag tiles
 // LATER -- when the tile and its predecessors have long finished -- resolves the offset with a decoupled look-back that
 // finds everything already published, and moves the values to their final position before it begins its own tile;
-// mtail_kernel moves the last P.lag tiles.  Bit-exact, no waiting at lag >= 6 x SMs, but measured no faster than the
-// two extra kernels (C5: 1.69 vs 1.655 ms): the merge kernel is bound by its phases' latencies, not by issue slots, so
+// mtail_kernel moves the last P.lag tiles.  Bit-exact, no waiting at lag >= 6 x SMs, but no faster than the
+// two extra kernels: the merge kernel is bound by its phases' latencies, not by issue slots, so
 // the copy phase costs what the compaction kernel costs.
 constexpr u32 kTileWide = 0x80000000u;  // tile_cnt flag: the tile's scratch holds u64 values, not u32 offsets from tile_lo
 

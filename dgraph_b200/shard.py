@@ -115,8 +115,8 @@ def gatherv_exact(dist, parts, local_out, local_off, device=None):
     base = np.concatenate([[0], np.cumsum(tot)]).astype(np.int64)
     out_g = torch.empty(max(int(base[-1]), 1), dtype=torch.int64, device=dev)
     if dist.get_backend() == "nccl" and world > 2 and 8 * int(base[-1]) >= (64 << 20):
-        # Bandwidth regime on many GPUs: NCCL's point-to-point transfers to 7 peers ran at ~240 GB/s per rank on an
-        # 8-GPU box, its all_gather collective (ring / NVLS) runs at several times that.  The collective needs equal
+        # Bandwidth regime on many GPUs: NCCL's point-to-point transfers to many peers run well below the link rate,
+        # its all_gather collective (ring / NVLS) runs closer to it.  The collective needs equal
         # shard sizes, so shards travel padded to the largest one (contiguous_partition balances by bytes: the padding
         # is a few percent) and are then moved to their final, compact positions at HBM speed.
         max_t = max(tot)
@@ -128,9 +128,8 @@ def gatherv_exact(dist, parts, local_out, local_off, device=None):
             if tot[r]:
                 out_g[int(base[r]): int(base[r]) + tot[r]].copy_(buf[r * max_t: r * max_t + tot[r]])
         return out_g[: int(base[-1])], torch.from_numpy(off_host).to(dev)
-    # grouped point-to-point transfers of the exact sizes (ncclGroupStart/End under NCCL), one per peer.  Measured on
-    # 2 GPUs, 0.96 GB per peer: 3.9 ms this way; cut into 8 or 64 MiB pieces 8.4 ms; NCCL's uneven all_gather (one
-    # broadcast per rank) 6.5 ms.
+    # grouped point-to-point transfers of the exact sizes (ncclGroupStart/End under NCCL), one per peer: one large
+    # transfer per peer beats cutting it into pieces, and beats NCCL's uneven all_gather (one broadcast per rank).
     piece = int(os.environ.get("DGX_GATHER_PIECE", str(1 << 40)))  # values per transfer (default: one per peer)
     ops = []
     for r in range(world):

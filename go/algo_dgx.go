@@ -1,7 +1,7 @@
 //go:build dgx
 
 // Package algo -- cgo shim that routes dgraph's posting-list set operations to
-// libdgx (B200, sm_100a).  Drop this file next to algo/uidlist.go and build alpha
+// libdgx (H100, sm_90a).  Drop this file next to algo/uidlist.go and build alpha
 // with `-tags dgx`; uidlist.go's bodies are renamed to *Go (intersectWithGo, ...) by
 // the companion patch in INTEGRATION.md and stay as the fallback.
 //

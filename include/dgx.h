@@ -1,5 +1,5 @@
 /*
- * dgx.h -- C ABI of libdgx.so: B200-native (sm_100a) sorted-uint64 posting-list
+ * dgx.h -- C ABI of libdgx.so: H100-native (sm_90a) sorted-uint64 posting-list
  * set operations and UidPack decode, the drop-in for dgraph's algo/ + codec/
  * hot path.
  *
@@ -145,7 +145,7 @@ int dgx_intersect_compressed(const dgx_pack_view* p, uint64_t after_uid, const u
  *   version     : commit timestamp of the immutable layer the pack was built from (List.minTs);
  *                 (key, version) must name immutable bytes -- a rollup produces a new version.
  * On a hit nothing is copied; on a miss the pack is uploaded and kept, least-recently-used packs
- * making room (capacity: DGX_CACHE_BYTES, default 32 GiB, or dgx_cache_configure). */
+ * making room (capacity: DGX_CACHE_BYTES, default 16 GiB, or dgx_cache_configure). */
 typedef struct dgx_pack_ref {
     const dgx_pack_view* pack;
     uint64_t key;

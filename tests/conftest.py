@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `-m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with `-m gpu`)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -23,7 +23,7 @@ def pytest_collection_modifyitems(config, items):
         have = False
     if have:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200); run under gpurun with -m gpu")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

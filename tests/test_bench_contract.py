@@ -58,6 +58,65 @@ def test_reference_arm_other_ranks_exit_quietly():
     assert r.returncode == 0 and r.stdout.strip() == ""
 
 
+def test_reference_arm_refuses_dump_outputs(tmp_path):
+    r = run("--impl", "reference", "--queries", "2", "--steps", "1", "--dump-outputs", str(tmp_path / "d"))
+    assert r.returncode != 0 and "--dump-outputs" in r.stderr
+    assert not (tmp_path / "d").exists()
+
+
+def _bench_module():
+    import importlib.util
+
+    spec = importlib.util.spec_from_file_location("bench_under_test", os.path.join(ROOT, "bench.py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+def _result_buffer(q, values):
+    """bench.py's result buffer layout: [out_off (q+1 words) | values | 2 words of slack], int64."""
+    import numpy as np
+    import torch
+
+    rng = np.random.default_rng(7)
+    cuts = np.sort(rng.integers(0, values.size + 1, q - 1))
+    off = np.concatenate([[0], cuts, [values.size]]).astype(np.uint64)
+    host = np.concatenate([off, values, np.array([123, 456], np.uint64)])
+    return torch.from_numpy(host.view(np.int64)), off
+
+
+def test_dump_outputs_writes_offsets_and_uids(tmp_path):
+    import numpy as np
+
+    bench = _bench_module()
+    vals = np.cumsum(np.arange(1, 1001, dtype=np.uint64))
+    buf, off = _result_buffer(5, vals)
+    bench.dump_outputs(str(tmp_path), buf, 5, 0, 1)
+    assert sorted(p.name for p in tmp_path.iterdir()) == ["offsets.npy", "uids.npy"]
+    o, u = np.load(tmp_path / "offsets.npy"), np.load(tmp_path / "uids.npy")
+    assert o.dtype == np.float64 and u.dtype == np.float64
+    assert np.array_equal(o, off.astype(np.float64)) and np.array_equal(u, vals.astype(np.float64))
+
+
+def test_dump_outputs_samples_past_the_budget(tmp_path, monkeypatch):
+    import numpy as np
+
+    bench = _bench_module()
+    monkeypatch.setattr(bench, "DUMP_BYTES", 8 * 1024)
+    vals = np.cumsum(np.arange(1, 5001, dtype=np.uint64))
+    buf, off = _result_buffer(3, vals)
+    for d in ("a", "b"):
+        bench.dump_outputs(str(tmp_path / d), buf, 3, 0, 1)
+    a = {n: np.load(tmp_path / "a" / f"{n}.npy") for n in ("offsets", "uids", "uids_index")}
+    b = {n: np.load(tmp_path / "b" / f"{n}.npy") for n in ("offsets", "uids", "uids_index")}
+    assert all(np.array_equal(a[n], b[n]) for n in a)          # the sample is fixed
+    assert sum(x.nbytes for x in a.values()) <= 8 * 1024
+    idx = a["uids_index"].astype(np.int64)
+    assert idx.size > 0 and np.all(np.diff(idx) > 0)
+    assert np.array_equal(a["uids"], vals[idx].astype(np.float64))
+    assert np.array_equal(a["offsets"], off.astype(np.float64))
+
+
 def test_product_arm_needs_cuda():
     import torch
     if torch.cuda.is_available():

@@ -1,6 +1,6 @@
 """GPU parity: libdgx (through the C ABI) vs the CPU oracle, bit-exact.
 
-Runs on a B200 only (`pytest -m gpu`).  Known-answer cases transcribe the
+Runs on an H100 only (`pytest -m gpu`).  Known-answer cases transcribe the
 reference's own tests; randomized cases compare with oracle/ on the same seeded
 inputs; large cases use size-independent properties plus the oracle.
 """

@@ -1,5 +1,5 @@
 """GPU parity, round-2 entry points and BASELINE-size configs: libdgx (through the C ABI) vs the CPU
-oracle, bit-exact.  Runs on a B200 only (`pytest -m gpu`).
+oracle, bit-exact.  Runs on an H100 only (`pytest -m gpu`).
 
  - IntersectSorted over packs (dgx_intersect_sorted_packed) with and without the HBM pack cache
  - IndexOf batch, shared-list batch
@@ -119,7 +119,7 @@ def test_pack_cache(dgx, orc):
     eq(dgx.algo.IntersectSortedPacks(packs, keys).Uids, want, "cache disabled")
     one(C.byref(st))
     assert st.entries == 0
-    _lib.check(lib.dgx_cache_configure(32 << 30))
+    _lib.check(lib.dgx_cache_configure(16 << 30))
 
 
 def test_pack_cache_concurrent(dgx, orc):

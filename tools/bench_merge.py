@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""MergeSorted alone (BASELINE config 5: k=64 lists, lengths ~ 1/rank, 1e8 UIDs in total) on one B200, device-resident,
+"""MergeSorted alone (BASELINE config 5: k=64 lists, lengths ~ 1/rank, 1e8 UIDs in total) on one H100, device-resident,
 CUDA-event timed, checked against torch.unique.  tools/bench_ops.py holds the same row; this script exists to iterate
 on the merge kernels without paying for the other configs.  --dense adds a densely allocated variant (gaps 1..3)."""
 import argparse, json, os, sys

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-operation device-resident benchmarks of libdgx on one B200 (BASELINE configs C1-C5).
+"""Per-operation device-resident benchmarks of libdgx on one H100 (BASELINE configs C1-C5).
 
 Complements bench.py (which times the headline config C2): every row reports CUDA-event
 time, input UIDs/s, algorithmic GB/s (SURVEY.md 8d formulas) and the fraction of the
@@ -33,7 +33,7 @@ def peak_gbs():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 def zipf_gaps_gpu(n, gen, a=1.5, clip=1 << 20):
