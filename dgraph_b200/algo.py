@@ -192,6 +192,27 @@ def _refs_of(packs, keys=None):
     return refs, keep
 
 
+def IntersectCompressedWithRows(packs, afterUID: int, v, keys=None):
+    """algo.IntersectCompressedWith(packs[i], afterUID, v, o_i) for every i in ONE call
+    (dgx_intersect_compressed_rows): the handleUidPostings loop (worker/task.go:783-987) over a task's keys.
+
+    v: ascending, duplicate-free uids (a pb.List or an array).  keys: optional [(key, version)] naming each pack for
+    the HBM-resident cache (0 = anonymous).  A nil / empty pack gives an empty row.  Returns (out, out_off):
+    row i is out[out_off[i]:out_off[i+1]]."""
+    vv = v.Uids if isinstance(v, List) else v
+    vv = np.zeros(0, np.uint64) if vv is None else _u64(vv)
+    nrows = len(packs)
+    if nrows == 0:
+        return np.zeros(0, np.uint64), np.zeros(1, np.uint64)
+    lib = _lib.load()
+    refs, keep = _refs_of(packs, keys)
+    cap = sum(min(vv.size, _exact(p)) for p in packs if p is not None)
+    out = np.empty(max(cap, 1), dtype=np.uint64)
+    out_off = np.zeros(nrows + 1, dtype=np.uint64)
+    _lib.check(lib.dgx_intersect_compressed_rows(refs, nrows, afterUID, _p(vv), vv.size, _p(out), _p(out_off), cap))
+    return out[: int(out_off[-1])], out_off
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -65,6 +65,56 @@ __global__ void __launch_bounds__(256) icw_ranges_by_block_kernel(const IcwParam
     if (hi > lo) { P.vlo[b] = (u32)lo; P.vhi[b] = (u32)hi; }
 }
 
+// Block i of the warp's batch, its group offsets already in column i of S.goff, expanded into S.stage[0, NumUids):
+// Base, then the 64-bit running sums of its group-varint deltas.  Called by the whole warp.
+__device__ __forceinline__ void icw_expand_block(DWarpSmem& S, int i, u32 ng_i, u64 base_i, int lane) {
+    const u32* pl32 = reinterpret_cast<const u32*>(S.payload);
+    if (lane == 0) S.stage[0] = base_i;
+    u64 carry = 0;
+    for (u32 g0 = 0; g0 < ng_i; g0 += 32) {
+        const u32 g = g0 + lane;
+        u32 d0 = 0, d1 = 0, d2 = 0, d3 = 0;
+        if (g < ng_i) {
+            const u32 off = S.goff[g * D_TSTRIDE + i];
+            const u32 tag = S.payload[off];
+            const u32 a = off + 1;
+            const u32 wb = a >> 2, sh = (a & 3u) * 8u;
+            const u32 w0 = pl32[wb], w1 = pl32[wb + 1], w2 = pl32[wb + 2], w3 = pl32[wb + 3], w4 = pl32[wb + 4];
+            const u32 D0 = __funnelshift_r(w0, w1, sh), D1 = __funnelshift_r(w1, w2, sh);
+            const u32 D2 = __funnelshift_r(w2, w3, sh), D3 = __funnelshift_r(w3, w4, sh);
+            const u32 l0 = (tag & 3u) + 1u, l1 = ((tag >> 2) & 3u) + 1u;
+            const u32 l2 = ((tag >> 4) & 3u) + 1u, l3 = (tag >> 6) + 1u;
+            auto extract = [&](u32 s, u32 l) -> u32 {
+                const u32 wi = s >> 2, sh2 = (s & 3u) * 8u;
+                const u32 lo_ = wi == 0 ? D0 : (wi == 1 ? D1 : (wi == 2 ? D2 : D3));
+                const u32 hi_ = wi == 0 ? D1 : (wi == 1 ? D2 : (wi == 2 ? D3 : 0u));
+                return __funnelshift_r(lo_, hi_, sh2) & (0xffffffffu >> (32u - 8u * l));
+            };
+            d0 = extract(0, l0);
+            d1 = extract(l0, l1);
+            d2 = extract(l0 + l1, l2);
+            d3 = extract(l0 + l1 + l2, l3);
+        }
+        const u64 p1 = d0, p2 = p1 + d1, p3 = p2 + d2, p4 = p3 + d3;
+        u64 inc = p4;
+#pragma unroll
+        for (int dlt = 1; dlt < 32; dlt <<= 1) {
+            u64 t = __shfl_up_sync(0xffffffffu, inc, dlt);
+            if (lane >= dlt) inc += t;
+        }
+        const u64 ex = base_i + carry + inc - p4;
+        if (g < ng_i) {
+            const u32 idx = 1u + 4u * g;
+            S.stage[idx] = ex + p1;
+            S.stage[idx + 1] = ex + p2;
+            S.stage[idx + 2] = ex + p3;
+            S.stage[idx + 3] = ex + p4;
+        }
+        carry += __shfl_sync(0xffffffffu, inc, 31);
+    }
+    __syncwarp();
+}
+
 __global__ void __launch_bounds__(D_NT) icw_probe_kernel(const IcwParams P) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -158,57 +208,13 @@ __global__ void __launch_bounds__(D_NT) icw_probe_kernel(const IcwParams P) {
         }
         __syncwarp();
 
-        const u32* pl32 = reinterpret_cast<const u32*>(S.payload);
         for (unsigned rest = want; rest; rest &= rest - 1) {
             const int i = __ffs(rest) - 1;
             const u32 n_i = __shfl_sync(0xffffffffu, num, i);
             const u64 base_i = __shfl_sync(0xffffffffu, base, i);
             const u32 ng_i = __shfl_sync(0xffffffffu, ngroups, i);
             const u32 lo_i = __shfl_sync(0xffffffffu, lo, i), hi_i = __shfl_sync(0xffffffffu, hi, i);
-            if (lane == 0) S.stage[0] = base_i;
-            u64 carry = 0;
-            for (u32 g0 = 0; g0 < ng_i; g0 += 32) {
-                const u32 g = g0 + lane;
-                u32 d0 = 0, d1 = 0, d2 = 0, d3 = 0;
-                if (g < ng_i) {
-                    const u32 off = S.goff[g * D_TSTRIDE + i];
-                    const u32 tag = S.payload[off];
-                    const u32 a = off + 1;
-                    const u32 wb = a >> 2, sh = (a & 3u) * 8u;
-                    const u32 w0 = pl32[wb], w1 = pl32[wb + 1], w2 = pl32[wb + 2], w3 = pl32[wb + 3], w4 = pl32[wb + 4];
-                    const u32 D0 = __funnelshift_r(w0, w1, sh), D1 = __funnelshift_r(w1, w2, sh);
-                    const u32 D2 = __funnelshift_r(w2, w3, sh), D3 = __funnelshift_r(w3, w4, sh);
-                    const u32 l0 = (tag & 3u) + 1u, l1 = ((tag >> 2) & 3u) + 1u;
-                    const u32 l2 = ((tag >> 4) & 3u) + 1u, l3 = (tag >> 6) + 1u;
-                    auto extract = [&](u32 s, u32 l) -> u32 {
-                        const u32 wi = s >> 2, sh2 = (s & 3u) * 8u;
-                        const u32 lo_ = wi == 0 ? D0 : (wi == 1 ? D1 : (wi == 2 ? D2 : D3));
-                        const u32 hi_ = wi == 0 ? D1 : (wi == 1 ? D2 : (wi == 2 ? D3 : 0u));
-                        return __funnelshift_r(lo_, hi_, sh2) & (0xffffffffu >> (32u - 8u * l));
-                    };
-                    d0 = extract(0, l0);
-                    d1 = extract(l0, l1);
-                    d2 = extract(l0 + l1, l2);
-                    d3 = extract(l0 + l1 + l2, l3);
-                }
-                const u64 p1 = d0, p2 = p1 + d1, p3 = p2 + d2, p4 = p3 + d3;
-                u64 inc = p4;
-#pragma unroll
-                for (int dlt = 1; dlt < 32; dlt <<= 1) {
-                    u64 t = __shfl_up_sync(0xffffffffu, inc, dlt);
-                    if (lane >= dlt) inc += t;
-                }
-                const u64 ex = base_i + carry + inc - p4;
-                if (g < ng_i) {
-                    const u32 idx = 1u + 4u * g;
-                    S.stage[idx] = ex + p1;
-                    S.stage[idx + 1] = ex + p2;
-                    S.stage[idx + 2] = ex + p3;
-                    S.stage[idx + 3] = ex + p4;
-                }
-                carry += __shfl_sync(0xffffffffu, inc, 31);
-            }
-            __syncwarp();
+            icw_expand_block(S, i, ng_i, base_i, lane);
             // ---- probe: the shorter side searches the longer one ----------------------------------
             const u32 cnt = hi_i - lo_i;
             if (cnt <= 4u * n_i) {
@@ -278,6 +284,278 @@ __global__ void __launch_bounds__(CP_NT) compact_kernel(const CompactParams P) {
             if (w < P.out_cap) P.out[w] = P.v[e0 + i];
             ++w;
         }
+}
+
+// ---- many packs, one v, one afterUID: the rows of a task's uid matrix -----------------------------
+// handleUidPostings (worker/task.go:783-987) intersects every key's pack with the same v from the same afterUID.
+// The blocks of all non-empty packs form ONE flat block space (pack after pack) and the batch runs a fixed number
+// of launches whatever the row count; the workspace is a few words per flat block plus one slot buffer:
+//   icw_rows_ranges_kernel  per-block v-ranges of every pack, the shorter side searched per row (as above)
+//   icw_rows_slots_kernel   slot of block b = min(vhi - vlo, NumUids_b): at most that many of its v match
+//   scan_u64_kernel         slot offsets (flat block order = row order, then block order)
+//   icw_rows_probe_kernel   icw_probe_kernel's warp-per-64-blocks walk; matches go in order to the block's slot
+//                           (warp ballot + popc) with a per-block count
+//   scan_u64_kernel         counts -> final positions; out_off[i] = position of row i's first block
+//   icw_rows_gather_kernel  slots -> out, CSR
+// Slots of one row sum to at most min(m, ExactLen): their total stays within the caller's out_cap bound.
+struct IcwJob {              // one non-empty pack
+    DPack pk;
+    u64 blk_base;            // its first block in the flat block space
+    u64 thr_base;            // its first thread in the ranges launch
+    u64 warp_base;           // its first warp in the probe launch
+    u32 by_v;                // nblocks > m: ranges from v's side (m threads) instead of the blocks' (nblocks threads)
+};
+struct IcwRowsParams {
+    const IcwJob* jobs;
+    u32 njobs;
+    const u64* v;
+    u64 m;
+    u64 after;
+    u64 nblocks;             // flat blocks
+    u64 nthreads;            // ranges launch
+    u64 nwarps;              // probe launch
+    u32* vlo;                // per flat block, zero-initialised (vlo == vhi: not touched)
+    u32* vhi;
+    u64* slot;               // per flat block: slot size; scanned into slot_off (nblocks + 1)
+    u64* slot_off;
+    u64* cnt;                // per flat block: matches; scanned into cnt_off (nblocks + 1)
+    u64* cnt_off;
+    u64* slots;              // slots_cap values
+    u64 slots_cap;
+    const u64* row_blk;      // nrows + 1: first flat block of each row (row_blk[nrows] = nblocks)
+    u64 nrows;
+    u64* out;
+    u64 out_cap;
+    u64* out_off;            // nrows + 1
+    int* err;
+};
+
+// Last job whose field F is <= x (F ascends over the jobs).
+template <u64 IcwJob::*F>
+__device__ __forceinline__ u32 icw_job_of(const IcwJob* __restrict__ jobs, u32 njobs, u64 x) {
+    u32 lo = 0, hi = njobs;
+    while (hi - lo > 1) {
+        const u32 mid = (lo + hi) >> 1;
+        if (jobs[mid].*F <= x) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(256) icw_rows_ranges_kernel(const IcwRowsParams P) {
+    const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= P.nthreads) return;
+    const IcwJob& J = P.jobs[icw_job_of<&IcwJob::thr_base>(P.jobs, P.njobs, t)];
+    const u64 k = t - J.thr_base;
+    const u64 nb = J.pk.nblocks;
+    const u64* base = J.pk.base;
+    u32* vlo = P.vlo + J.blk_base;
+    u32* vhi = P.vhi + J.blk_base;
+    if (!J.by_v) {  // thread per block: [lower_bound(v, max(base[b], after)), lower_bound(v, base[b+1]))
+        const u64 first = base[k];
+        const u64 lo = lower_bound_g(P.v, P.m, first > P.after ? first : P.after);
+        const u64 hi = (k + 1 < nb) ? lower_bound_g(P.v, P.m, base[k + 1]) : P.m;
+        if (hi > lo) { vlo[k] = (u32)lo; vhi[k] = (u32)hi; }
+        return;
+    }
+    // thread per element of v: the block whose range holds v[k]; run boundaries write vlo / vhi
+    const u64 x = P.v[k];
+    if (x < P.after || x < base[0]) return;  // before the pack's range
+    auto block_of = [&](u64 y) -> long long {  // last b with base[b] <= y
+        u64 lo = 0, hi = nb;
+        while (lo < hi) {
+            const u64 mid = lo + ((hi - lo) >> 1);
+            if (ld_probe(base + mid) <= y) lo = mid + 1; else hi = mid;
+        }
+        return (long long)lo - 1;
+    };
+    const long long b = block_of(x);
+    long long bp = -2, bn = -2;
+    if (k > 0) { const u64 xp = P.v[k - 1]; if (xp >= P.after) bp = block_of(xp); }
+    if (k + 1 < P.m) bn = block_of(P.v[k + 1]);
+    if (bp != b) vlo[b] = (u32)k;
+    if (bn != b) vhi[b] = (u32)(k + 1);
+}
+
+__global__ void __launch_bounds__(256) icw_rows_slots_kernel(const IcwRowsParams P) {
+    const u64 fb = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (fb >= P.nblocks) return;
+    const IcwJob& J = P.jobs[icw_job_of<&IcwJob::blk_base>(P.jobs, P.njobs, fb)];
+    const u32 lo = P.vlo[fb], hi = P.vhi[fb];
+    const u32 num = J.pk.num[fb - J.blk_base];
+    const u32 n = hi > lo ? hi - lo : 0u;
+    P.slot[fb] = n < num ? n : num;
+    P.cnt[fb] = 0;
+}
+
+__global__ void __launch_bounds__(D_NT) icw_rows_probe_kernel(const IcwRowsParams P) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    DWarpSmem& S = reinterpret_cast<DWarpSmem*>(smem_raw)[wid];
+    const u64 gw = (u64)blockIdx.x * D_WARPS + wid;
+    // slots beyond the buffer only arise from a pack whose bases do not ascend: nothing is written then
+    if (gw >= P.nwarps || P.slot_off[P.nblocks] > P.slots_cap) return;
+    const IcwJob& J = P.jobs[icw_job_of<&IcwJob::warp_base>(P.jobs, P.njobs, gw)];
+    const DPack pk = J.pk;
+    const u32* vlo = P.vlo + J.blk_base;
+    const u32* vhi = P.vhi + J.blk_base;
+    const u64* slot_off = P.slot_off + J.blk_base;
+    u64* cnt = P.cnt + J.blk_base;
+    u64 b = (gw - J.warp_base) * D_BPW;
+    const u64 bend = (b + D_BPW < pk.nblocks) ? b + D_BPW : pk.nblocks;
+    const u32 bar = smem_u32(&S.mbar);
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    u32 parity = 0;
+
+    while (b < bend) {
+        const u64 bi = b + lane;
+        const bool in = bi < bend;
+        const u32 lo = in ? vlo[bi] : 0u, hi = in ? vhi[bi] : 0u;
+        const bool tch = in && hi > lo;
+        const unsigned touched = __ballot_sync(0xffffffffu, tch);
+        if (touched == 0) { b += 32; continue; }
+        const int f = __ffs(touched) - 1;
+        const u64 doff = in ? pk.delta_off[bi] : 0;
+        const u64 dnext = in ? pk.delta_off[bi + 1] : 0;
+        const u64 s0 = tch ? slot_off[bi] : 0;
+        const u64 scap = tch ? slot_off[bi + 1] - s0 : 0;
+        const u64 win0 = __shfl_sync(0xffffffffu, doff, f) & ~15ull;
+        const bool fits = in && lane >= f && (dnext - win0 <= (u64)D_WB);
+        const unsigned fm = __ballot_sync(0xffffffffu, fits) >> f;
+        int run = __ffs(~fm) - 1;
+        if (fm == (0xffffffffu >> f)) run = 32 - f;
+        const u32 num = in ? pk.num[bi] : 0;
+        const bool oversize = run == 0 || (num > 256u && lane >= f && lane < f + (run ? run : 1));
+        if (__any_sync(0xffffffffu, oversize)) {
+            // non-reference BlockSize: lane-serial walk from global memory, matches written in uid order
+            const int r = run ? run : 1;
+            if (tch && lane >= f && lane < f + r) {
+                const unsigned char* p = pk.deltas + doff;
+                u64 last = pk.base[bi];
+                u32 produced = 1;
+                u64 w = 0;
+                auto probe = [&](u64 y) {
+                    const u64 pos = lo + lower_bound_g(P.v + lo, (u64)(hi - lo), y);
+                    if (pos < hi && ld_probe(P.v + pos) == y) {
+                        if (w < scap) P.slots[s0 + w] = y;
+                        ++w;
+                    }
+                };
+                probe(last);
+                while (produced < num) {
+                    const u32 tag = p[0];
+                    const unsigned char* d = p + 1;
+                    for (int j = 0; j < 4 && produced < num; ++j) {
+                        const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
+                        u32 v32 = 0;
+                        for (u32 k = 0; k < l; ++k) v32 |= (u32)d[k] << (8 * k);
+                        d += l;
+                        last += v32;
+                        ++produced;
+                        probe(last);
+                    }
+                    p += gv_bytes_used(tag);
+                }
+                cnt[bi] = w < scap ? w : scap;
+            }
+            b += f + r;
+            continue;
+        }
+        const unsigned in_run = (run >= 32 ? 0xffffffffu : ((1u << run) - 1u)) << f;
+        const unsigned want = touched & in_run;
+        const int last_t = 31 - __clz(want);
+        const u64 wend = __shfl_sync(0xffffffffu, dnext, last_t);
+        const u64 base = in ? pk.base[bi] : 0;
+        const u32 ngroups = num > 1 ? (num + 2) / 4 : 0;
+
+        const u32 bytes = (u32)(((wend - win0) + 15ull) & ~15ull);
+        if (lane == 0) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            mbar_expect_tx(bar, bytes);
+            tma_bulk_g2s(smem_u32(S.payload), pk.deltas + win0, bytes, bar);
+        }
+        mbar_wait(bar, parity);
+        parity ^= 1u;
+
+        if ((want >> lane) & 1u) {
+            u32 off = (u32)(doff - win0);
+            const u32 off_end = (u32)(dnext - win0);
+            for (u32 g = 0; g < ngroups; ++g) {
+                S.goff[g * D_TSTRIDE + lane] = (unsigned short)off;
+                off += gv_bytes_used(S.payload[off]);
+                off = off < off_end ? off : off_end;
+            }
+        }
+        __syncwarp();
+
+        const unsigned below = (1u << lane) - 1u;
+        for (unsigned rest = want; rest; rest &= rest - 1) {
+            const int i = __ffs(rest) - 1;
+            const u32 n_i = __shfl_sync(0xffffffffu, num, i);
+            const u64 base_i = __shfl_sync(0xffffffffu, base, i);
+            const u32 ng_i = __shfl_sync(0xffffffffu, ngroups, i);
+            const u32 lo_i = __shfl_sync(0xffffffffu, lo, i), hi_i = __shfl_sync(0xffffffffu, hi, i);
+            const u64 s0_i = __shfl_sync(0xffffffffu, s0, i), scap_i = __shfl_sync(0xffffffffu, scap, i);
+            icw_expand_block(S, i, ng_i, base_i, lane);
+            // ---- probe, the shorter side searching the longer; hits leave in ascending order -----------
+            u64 w = 0;
+            const u32 c = hi_i - lo_i;
+            if (c <= 4u * n_i) {
+                for (u32 j0 = lo_i; j0 < hi_i; j0 += 32) {
+                    const u32 j = j0 + lane;
+                    u64 x = 0;
+                    bool hit = false;
+                    if (j < hi_i) {
+                        x = ld_stream(P.v + j);
+                        const int pos = lower_bound_s(S.stage, 0, (int)n_i, x);
+                        hit = pos < (int)n_i && S.stage[pos] == x;
+                    }
+                    const unsigned hm = __ballot_sync(0xffffffffu, hit);
+                    const u64 k = w + __popc(hm & below);
+                    if (hit && k < scap_i) P.slots[s0_i + k] = x;
+                    w += __popc(hm);
+                }
+            } else {
+                for (u32 e0 = 0; e0 < n_i; e0 += 32) {
+                    const u32 e = e0 + lane;
+                    u64 y = 0;
+                    bool hit = false;
+                    if (e < n_i) {
+                        y = S.stage[e];
+                        const u64 pos = lo_i + lower_bound_g(P.v + lo_i, (u64)c, y);
+                        hit = pos < hi_i && ld_probe(P.v + pos) == y;
+                    }
+                    const unsigned hm = __ballot_sync(0xffffffffu, hit);
+                    const u64 k = w + __popc(hm & below);
+                    if (hit && k < scap_i) P.slots[s0_i + k] = y;
+                    w += __popc(hm);
+                }
+            }
+            if (lane == 0) cnt[b + i] = w < scap_i ? w : scap_i;
+            __syncwarp();
+        }
+        b += f + run;
+    }
+}
+
+// Thread t <= nrows writes out_off[t]; warp w moves block w's matches from its slot to their final place.
+__global__ void __launch_bounds__(256) icw_rows_gather_kernel(const IcwRowsParams P) {
+    const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t <= P.nrows) P.out_off[t] = P.cnt_off[P.row_blk[t]];
+    const bool bad = P.cnt_off[P.nblocks] > P.out_cap || P.slot_off[P.nblocks] > P.slots_cap;
+    if (bad) {
+        if (t == 0) atomicExch(P.err, 1);
+        return;  // past out_cap nothing is written
+    }
+    const u64 fb = t >> 5;
+    if (fb >= P.nblocks) return;
+    const u64 c = P.cnt[fb];
+    const u64* src = P.slots + P.slot_off[fb];
+    u64* dst = P.out + P.cnt_off[fb];
+    for (u64 k = t & 31; k < c; k += 32) dst[k] = src[k];
 }
 
 // ---- Decoder seeks on the device (codec/codec.go:219-384) --------------------------------------

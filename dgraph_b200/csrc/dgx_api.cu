@@ -2342,6 +2342,168 @@ extern "C" int dgx_intersect_batch_shared(const uint64_t* a, const uint64_t* a_o
 }
 
 // ---------------------------------------------------------------------------
+// IntersectCompressedWith over many packs (handleUidPostings)
+// ---------------------------------------------------------------------------
+// Row i = algo.IntersectCompressedWith(packs[i], after, v) for every row with six launches whatever nrows is
+// (compressed_kernel.cuh): ranges, slot sizes, slot scan, probe, count scan, gather.  Workspace: ~44 bytes per
+// block of the batch plus a slot buffer of sum_i min(m, ExactLen_i) values.
+static int icw_rows_impl(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows, uint64_t after, const uint64_t* d_v,
+                         size_t m, uint64_t* d_out, size_t out_cap, uint64_t* d_out_off) {
+    if (m >= (size_t(1) << 32)) return fail(DGX_ERR_ARG, "v has %zu uids: per-block v-ranges are 32-bit", m);
+    size_t nj = 0;
+    uint64_t nb = 0, thr = 0, warps = 0, exact = 0, slots_cap = 0;
+    for (size_t i = 0; i < nrows; ++i)
+        if (packs[i] && packs[i]->pk.nblocks) ++nj;
+    const size_t b_jobs = (nj * sizeof(IcwJob) + 15) & ~size_t(15), b_rows = (nrows + 1) * sizeof(uint64_t);
+    void* h_raw;
+    int rc = l->host.alloc(b_jobs + b_rows, &h_raw);
+    if (rc) return rc;
+    IcwJob* hj = (IcwJob*)h_raw;
+    uint64_t* h_rows = (uint64_t*)((char*)h_raw + b_jobs);
+    size_t j = 0;
+    for (size_t i = 0; i < nrows; ++i) {
+        h_rows[i] = nb;
+        const dgx_dev_pack* p = packs[i];
+        if (!p || p->pk.nblocks == 0) continue;
+        const uint64_t pnb = p->pk.nblocks;
+        IcwJob& J = hj[j++];
+        J.pk = p->pk;
+        J.blk_base = nb;
+        J.thr_base = thr;
+        J.warp_base = warps;
+        J.by_v = pnb > m;
+        nb += pnb;
+        thr += J.by_v ? m : pnb;
+        warps += (pnb + D_BPW - 1) / D_BPW;
+        exact += p->exact_len;
+        slots_cap += std::min<uint64_t>(m, p->exact_len);
+    }
+    h_rows[nrows] = nb;
+    g_stats.uids_in += exact + m;
+    if (nb == 0 || m == 0) {
+        CK(cudaMemsetAsync(d_out_off, 0, (nrows + 1) * sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    const uint64_t kMaxGrid = 0x7fffffffull;
+    const uint64_t g_rng = (thr + 255) / 256, g_blk = (nb + 255) / 256, tiles = (nb + EN_TILE - 1) / EN_TILE;
+    const uint64_t g_probe = (warps + D_WARPS - 1) / D_WARPS, g_gather = (std::max<uint64_t>(nb * 32, nrows + 1) + 255) / 256;
+    if (std::max({g_rng, g_blk, tiles, g_probe, g_gather}) > kMaxGrid || nj > 0xffffffffull)
+        return fail(DGX_ERR_ARG, "batch too large for one launch (%llu blocks, %zu rows)", (unsigned long long)nb, nrows);
+    // workspace: [table | zeroed: vlo vhi, scan status + tickets | slot | slot_off | cnt | cnt_off | slots]
+    const size_t b_tab = b_jobs + b_rows;
+    const size_t b_rng = (2 * nb * sizeof(u32) + 15) & ~size_t(15), b_stat = 2 * tiles * sizeof(u64) + 16;
+    const size_t b_zero = b_rng + b_stat;
+    const size_t b_words = (4 * nb + 2) * sizeof(u64);
+    void* d_raw;
+    rc = l->ws.alloc(b_tab + b_zero + b_words + slots_cap * sizeof(u64), &d_raw);
+    if (rc) return rc;
+    char* d = (char*)d_raw;
+    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
+    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
+    g_stats.h2d += b_tab;
+    IcwRowsParams P;
+    P.jobs = (const IcwJob*)d;
+    P.njobs = (u32)nj;
+    P.v = (const u64*)d_v;
+    P.m = m;
+    P.after = after;
+    P.nblocks = nb;
+    P.nthreads = thr;
+    P.nwarps = warps;
+    P.row_blk = (const u64*)(d + b_jobs);
+    P.vlo = (u32*)(d + b_tab);
+    P.vhi = P.vlo + nb;
+    u64* status = (u64*)(d + b_tab + b_rng);
+    u32* tickets = (u32*)(status + 2 * tiles);
+    P.slot = (u64*)(d + b_tab + b_zero);
+    P.slot_off = P.slot + nb;
+    P.cnt = P.slot_off + nb + 1;
+    P.cnt_off = P.cnt + nb;
+    P.slots = P.cnt_off + nb + 1;
+    P.slots_cap = slots_cap;
+    P.nrows = nrows;
+    P.out = (u64*)d_out;
+    P.out_cap = out_cap;
+    P.out_off = (u64*)d_out_off;
+    P.err = l->d_err;
+    const u64* d_nb = P.row_blk + nrows;  // the block count as a device word (scan length)
+    icw_rows_ranges_kernel<<<(unsigned)g_rng, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    icw_rows_slots_kernel<<<(unsigned)g_blk, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)tiles, EN_NT, 0, l->stream>>>(P.slot, P.slot_off, d_nb, nb, status, tickets, nullptr);
+    CK(cudaGetLastError());
+    icw_rows_probe_kernel<<<(unsigned)g_probe, D_NT, sizeof(DWarpSmem) * D_WARPS, l->stream>>>(P);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)tiles, EN_NT, 0, l->stream>>>(P.cnt, P.cnt_off, d_nb, nb, status + tiles, tickets + 1, nullptr);
+    CK(cudaGetLastError());
+    icw_rows_gather_kernel<<<(unsigned)g_gather, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    l->launches += 6;
+    g_stats.launches += 6;
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_intersect_compressed_rows(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows,
+                                                 uint64_t after_uid, const uint64_t* d_v, size_t m, uint64_t* d_out,
+                                                 size_t out_cap, uint64_t* d_out_off) {
+    if (!l || !d_out_off || (nrows && !packs) || (m && !d_v)) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    const int rc = icw_rows_impl(l, packs, nrows, after_uid, d_v, m, d_out, out_cap, d_out_off);
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    return rc;
+}
+
+extern "C" int dgx_intersect_compressed_rows(const dgx_pack_ref* refs, size_t nrows, uint64_t after_uid,
+                                             const uint64_t* v, size_t m, uint64_t* out, uint64_t* out_off,
+                                             size_t out_cap) {
+    if (!out_off) return fail(DGX_ERR_ARG, "null out_off");
+    if (nrows == 0) { out_off[0] = 0; return DGX_OK; }
+    if (!refs || (m && !v)) return fail(DGX_ERR_ARG, "null argument");
+    if (m >= (size_t(1) << 32)) return fail(DGX_ERR_ARG, "v has %zu uids: per-block v-ranges are 32-bit", m);
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    std::vector<PackLease> pls(nrows);
+    std::vector<const dgx_pack_view*> oneshot(nrows, nullptr);
+    int rc = DGX_OK;
+    size_t got = 0;
+    for (; got < nrows && rc == DGX_OK; ++got) {
+        const dgx_pack_ref& r = refs[got];
+        if (!r.pack || r.pack->nblocks == 0) continue;  // nil / empty pack: empty row
+        bool deferred = false;
+        rc = pack_acquire(l, r, &pls[got], &deferred);
+        if (deferred) oneshot[got] = r.pack;
+    }
+    if (rc == DGX_OK) {  // the one-shot packs cross PCIe together (one transfer when they are back-to-back images)
+        std::vector<dgx_dev_pack> up(nrows);
+        rc = packs_upload_ws(l, oneshot.data(), nrows, up.data());
+        for (size_t i = 0; i < nrows && rc == DGX_OK; ++i)
+            if (oneshot[i]) pls[i].pk = up[i];
+    }
+    std::vector<const dgx_dev_pack*> rows(nrows, nullptr);
+    size_t cap = 0;
+    for (size_t i = 0; i < nrows && rc == DGX_OK; ++i)
+        if (refs[i].pack && refs[i].pack->nblocks) {
+            rows[i] = &pls[i].pk;
+            cap += std::min<size_t>(m, pls[i].pk.exact_len);
+        }
+    uint64_t* d_v = nullptr;
+    void *d_out = nullptr, *d_off = nullptr;
+    if (rc == DGX_OK) rc = upload_list(l, v, m, &d_v);
+    if (rc == DGX_OK) rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
+    if (rc == DGX_OK) rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
+    if (rc == DGX_OK) rc = icw_rows_impl(l, rows.data(), nrows, after_uid, d_v, m, (uint64_t*)d_out, cap, (uint64_t*)d_off);
+    if (rc == DGX_OK) rc = batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap);
+    else cudaStreamSynchronize(l->stream);  // nothing queued may outlive the references released below
+    for (size_t i = 0; i < got; ++i) pack_release(pls[i]);
+    return rc;
+}
+
+// ---------------------------------------------------------------------------
 // protobuf wire-format adjacency (host only; see include/dgx.h and wire.hpp)
 // ---------------------------------------------------------------------------
 extern "C" int dgx_wire_posting_list_pack(const uint8_t* buf, size_t len, const uint8_t** pack, size_t* pack_len) {

@@ -161,6 +161,116 @@ func IntersectCompressedWithRef(ref PackRef, afterUID uint64, v, o *pb.List) boo
 	return true
 }
 
+// IntersectCompressedWithRows is algo.IntersectCompressedWith(refs[i].Pack, afterUID, v, o_i) for every i in ONE
+// library call: the loop handleUidPostings (worker/task.go:783-987) runs over a task's keys with one ListOptions
+// (posting/list.go:1795-1800).  Row i of the result is o_i; a nil pack leaves its row as &pb.List{} (the reference
+// leaves o untouched).  Anonymous packs (Key 0) are flattened back to back into one C staging buffer in the
+// library's flat-image layout, so they cross PCIe as one transfer; named packs use the HBM cache.  The rows are
+// slices of one result buffer.  The size threshold applies to the batch total, not to each row: a task of many
+// small lists is what pays off.  Returns false when the caller must run the Go path.
+func IntersectCompressedWithRows(refs []PackRef, afterUID uint64, v *pb.List) ([]*pb.List, bool) {
+	n := len(refs)
+	if n == 0 {
+		return []*pb.List{}, true
+	}
+	total, capOut, img := len(v.Uids), 0, 0
+	for _, r := range refs {
+		if r.Pack == nil || len(r.Pack.Blocks) == 0 {
+			continue
+		}
+		total += ApproxLen(r.Pack)
+		if e := ExactLen(r.Pack); e < len(v.Uids) {
+			capOut += e
+		} else {
+			capOut += len(v.Uids)
+		}
+		if r.Key == 0 {
+			img += int(C.dgx_pack_image_size(C.size_t(len(r.Pack.Blocks)), C.size_t(deltaBytes(r.Pack))))
+		}
+	}
+	if total < dgxMinDecode || uint64(len(v.Uids)) >= 1<<32 {
+		return nil, false
+	}
+	crefs := (*[1 << 28]C.dgx_pack_ref)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(C.dgx_pack_ref{}))))
+	views := (*[1 << 28]C.dgx_pack_view)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(C.dgx_pack_view{}))))
+	stage := C.malloc(C.size_t(img + 64))
+	frees := []func(){}
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+		C.free(unsafe.Pointer(crefs))
+		C.free(unsafe.Pointer(views))
+		C.free(stage)
+	}()
+	o := 0
+	for i, r := range refs {
+		crefs[i] = C.dgx_pack_ref{key: C.uint64_t(r.Key), version: C.uint64_t(r.Version)}
+		if r.Pack == nil || len(r.Pack.Blocks) == 0 {
+			continue // empty row
+		}
+		if r.Key != 0 {
+			view, free := flatten(r.Pack)
+			frees = append(frees, free)
+			views[i] = view
+		} else {
+			nb, db := len(r.Pack.Blocks), deltaBytes(r.Pack)
+			if C.dgx_pack_image_view(unsafe.Add(stage, o), C.uint32_t(r.Pack.BlockSize), C.size_t(nb), C.size_t(db), &views[i]) != C.DGX_OK {
+				return nil, false
+			}
+			fillImage(&views[i], r.Pack)
+			o += int(C.dgx_pack_image_size(C.size_t(nb), C.size_t(db)))
+		}
+		crefs[i].pack = &views[i]
+	}
+	out := make([]uint64, capOut+1)
+	off := make([]uint64, n+1)
+	var vp *C.uint64_t
+	if len(v.Uids) > 0 {
+		vp = (*C.uint64_t)(unsafe.Pointer(&v.Uids[0]))
+	}
+	if C.dgx_intersect_compressed_rows(&crefs[0], C.size_t(n), C.uint64_t(afterUID), vp, C.size_t(len(v.Uids)),
+		(*C.uint64_t)(unsafe.Pointer(&out[0])), (*C.uint64_t)(unsafe.Pointer(&off[0])), C.size_t(capOut)) != C.DGX_OK {
+		return nil, false
+	}
+	rows := make([]*pb.List, n)
+	for i, r := range refs {
+		if r.Pack == nil {
+			rows[i] = &pb.List{}
+			continue
+		}
+		rows[i] = &pb.List{Uids: out[off[i]:off[i+1]:off[i+1]]}
+	}
+	return rows, true
+}
+
+func deltaBytes(pack *pb.UidPack) int {
+	t := 0
+	for _, b := range pack.Blocks {
+		t += len(b.Deltas)
+	}
+	return t
+}
+
+// fillImage writes pack's blocks into the arrays dgx_pack_image_view pointed v at.
+func fillImage(v *C.dgx_pack_view, pack *pb.UidPack) {
+	nb := len(pack.Blocks)
+	base := (*[1 << 28]C.uint64_t)(unsafe.Pointer(v.base))[:nb:nb]
+	num := (*[1 << 28]C.uint32_t)(unsafe.Pointer(v.num_uids))[:nb:nb]
+	off := (*[1 << 28]C.uint64_t)(unsafe.Pointer(v.delta_off))[: nb+1 : nb+1]
+	o := 0
+	for i, b := range pack.Blocks {
+		base[i] = C.uint64_t(b.Base)
+		num[i] = C.uint32_t(b.NumUids)
+		off[i] = C.uint64_t(o)
+		if len(b.Deltas) > 0 {
+			C.memcpy(unsafe.Add(unsafe.Pointer(v.deltas), o), unsafe.Pointer(&b.Deltas[0]), C.size_t(len(b.Deltas)))
+		}
+		o += len(b.Deltas)
+	}
+	off[nb] = C.uint64_t(o)
+}
+
 // IntersectSortedPacks is algo.IntersectSorted over lists still held as packs: every pack is decoded on the
 // device (codec.Decode(p, 0)) and the k-way intersection runs there; ~1.5 B/UID cross PCIe instead of 8.
 func IntersectSortedPacks(refs []PackRef) (*pb.List, bool) {

@@ -202,6 +202,16 @@ int dgx_merge_sorted_packed(const dgx_pack_ref* refs, size_t k, uint32_t block_s
 int dgx_intersect_compressed_ref(const dgx_pack_ref* ref, uint64_t after_uid, const uint64_t* v, size_t m,
                                  uint64_t* out, size_t out_cap, size_t* out_len);
 
+/* algo.IntersectCompressedWith(pack_i, afterUID, v, o_i) for every row i, one call: the handleUidPostings loop
+ * (worker/task.go:783-987 -> posting/list.go:1795-1800) with its one ListOptions.  Row i of the CSR result is
+ * out[out_off[i] .. out_off[i+1]) (nrows + 1 offsets).  refs[i] as in dgx_intersect_sorted_packed (named packs use the
+ * HBM cache, anonymous ones cross PCIe together); a NULL / empty pack is an empty row.  v is ascending and
+ * duplicate-free, m < 2^32 (DGX_ERR_ARG otherwise).  out_cap >= sum_i min(m, ExactLen(pack_i)).  The batch runs a fixed
+ * number of kernel launches whatever nrows is. */
+int dgx_intersect_compressed_rows(const dgx_pack_ref* refs, size_t nrows, uint64_t after_uid,
+                                  const uint64_t* v, size_t m,
+                                  uint64_t* out, uint64_t* out_off, size_t out_cap);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -340,6 +350,12 @@ size_t dgx_dev_pack_bytes(const dgx_dev_pack* pk);      /* bytes of the pack in 
 /* Decode(pack, seek) into d_out; d_out_len: one device uint64. */
 int dgx_dev_decode(dgx_lane* lane, const dgx_dev_pack* pk, uint64_t seek,
                    uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
+/* Device-resident form of dgx_intersect_compressed_rows: packs already in HBM (dgx_dev_pack_upload; NULL = empty
+ * row), d_v / d_out / d_out_off (nrows + 1 values) device pointers.  Asynchronous on the lane; past out_cap nothing is
+ * written and the next dgx_lane_sync returns DGX_ERR_CAP. */
+int dgx_dev_intersect_compressed_rows(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t nrows,
+                                      uint64_t after_uid, const uint64_t* d_v, size_t m,
+                                      uint64_t* d_out, size_t out_cap, uint64_t* d_out_off);
 
 #ifdef __cplusplus
 }

@@ -131,8 +131,15 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--small", action="store_true", help="1/10 sizes (quick functional pass)")
+    ap.add_argument("--c6-only", action="store_true", help="only the C6 handleUidPostings rows")
     args = ap.parse_args()
-    rows = run(Lane(), 10 if args.small else 1, quick=False)
+    rows = c6_rows(Lane()) if args.c6_only else run(Lane(), 10 if args.small else 1, quick=False)
+    if args.c6_only:  # the card and its power limit, read in the same run as the numbers
+        import subprocess
+
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True).stdout.strip()
+        rows = {"device": torch.cuda.get_device_name(0), "nvidia_smi_name_power_limit": q, "rows": rows}
     if args.out:
         with open(args.out, "w") as f:
             json.dump(rows, f, indent=1)
@@ -375,7 +382,145 @@ def run(L, S, quick):
                     {"speedup_vs_cpu_1thread": (t_dec + t_int) / t_pin, "cpu_oracle_ms": (t_dec + t_int) * 1e3}))
     for ptr in pins:
         L.lib.dgx_host_free(ptr)
+    rows += c6_rows(L)
     return rows
+
+
+def c6_rows(L, threads: int = 4):
+    """C6 "handleUidPostings": one task's 10 000 posting lists (UidPacks, BlockSize 256) each intersected with the same
+    v from the same afterUID (worker/task.go:783-987 -> algo.IntersectCompressedWith).  Five legs on the same inputs,
+    each checked row by row against the oracle: (1) dgx_dev_intersect_compressed_rows on resident packs (CUDA events),
+    (2) the host form with named packs in steady state, (3) the host form with anonymous packs flattened back to back
+    into one pinned buffer (every pack crosses PCIe each step), (4) dgx_intersect_compressed_ref per row from
+    `threads` host threads, (5) the oracle row loop on one thread and on every host thread."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    import gen_rows
+    from oracle import pyoracle as orc
+
+    lib = L.lib
+    master, rows_u, v = gen_rows.c6_inputs()
+    nrows, m = len(rows_u), v.size
+    ops = [orc.encode(r, 256) for r in rows_u]
+    arrs = [(op.base, op.num_uids, op.delta_off, op.deltas) for op in ops]
+    exact = sum(r.size for r in rows_u)
+    del rows_u
+    # flat images of all packs back to back in one pinned buffer (what the shim's flatten writes)
+    sizes = [lib.dgx_pack_image_size(a[0].size, a[3].size) for a in arrs]
+    blob = lib.dgx_host_alloc(sum(sizes) + 64)
+    assert blob
+    views, o = [], 0
+    for (base, num, doff, deltas), sz in zip(arrs, sizes):
+        pv = _lib.PackView()
+        _lib.check(lib.dgx_pack_image_view(C.c_void_p(blob + o), 256, base.size, deltas.size, C.byref(pv)))
+        C.memmove(pv.base, base.ctypes.data, base.nbytes)
+        C.memmove(pv.delta_off, doff.ctypes.data, doff.nbytes)
+        C.memmove(pv.num_uids, num.ctypes.data, num.nbytes)
+        C.memmove(pv.deltas, deltas.ctypes.data, deltas.nbytes)
+        views.append(pv)
+        o += sz
+
+    def refs_of(named: bool):
+        refs = (_lib.PackRef * nrows)()
+        for i in range(nrows):
+            refs[i].pack = C.pointer(views[i])
+            refs[i].key, refs[i].version = ((900_000 + i) if named else 0), 1
+        return refs
+
+    named, anon = refs_of(True), refs_of(False)
+    hv = np.ascontiguousarray(v)
+    cap = sum(min(m, int(a[1].sum(dtype=np.uint64))) for a in arrs)
+    hout = np.empty(max(cap, 1), np.uint64)
+    hoff = np.zeros(nrows + 1, np.uint64)
+
+    def host_rows(refs, after):
+        _lib.check(lib.dgx_intersect_compressed_rows(refs, nrows, after, hv.ctypes.data_as(C.c_void_p), m,
+                                                      hout.ctypes.data_as(C.c_void_p), hoff.ctypes.data_as(C.c_void_p), cap))
+
+    def wall(fn, reps):
+        fn()
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            fn()
+        return (time.perf_counter() - t0) / reps * 1e3
+
+    # device-resident packs for leg 1
+    handles = []
+    for pv in views:
+        h = C.c_void_p()
+        _lib.check(lib.dgx_dev_pack_upload(L.h, C.byref(pv), C.byref(h)))
+        handles.append(h)
+    tab = (C.c_void_p * nrows)(*[h.value for h in handles])
+    d_v = torch.from_numpy(hv.view(np.int64)).to(DEV)
+    d_out = torch.empty(cap + 8, dtype=torch.int64, device=DEV)
+    d_off = torch.zeros(nrows + 1, dtype=torch.int64, device=DEV)
+    lib.dgx_cache_clear()
+    _lib.check(lib.dgx_cache_configure(16 << 30))
+    out_rows = []
+    try:
+        for after in (0, int(master[master.size // 2])):
+            t0 = time.perf_counter()
+            want = [orc.intersect_compressed_with(op, after, v) for op in ops]
+            t_orc1 = time.perf_counter() - t0
+            ncpu = os.cpu_count() or 1
+            t0 = time.perf_counter()
+            with ThreadPoolExecutor(max_workers=ncpu) as ex:   # ctypes releases the GIL
+                list(ex.map(lambda op: orc.intersect_compressed_with(op, after, v), ops))
+            t_orcn = time.perf_counter() - t0
+            want_off = np.concatenate([[0], np.cumsum([w.size for w in want])]).astype(np.uint64)
+            want_all = np.concatenate(want) if want_off[-1] else np.zeros(0, np.uint64)
+            nout = int(want_off[-1])
+            abytes = gen_rows.algorithmic_bytes([(a[0], a[2]) for a in arrs], after, hv, nout)
+
+            def same(out, off):
+                return bool(np.array_equal(off, want_off) and np.array_equal(out[:nout], want_all))
+
+            def dev():
+                _lib.check(lib.dgx_dev_intersect_compressed_rows(L.h, tab, nrows, after, C.c_void_p(d_v.data_ptr()), m,
+                                                                 C.c_void_p(d_out.data_ptr()), cap, C.c_void_p(d_off.data_ptr())))
+            ms1, _ = timeit(dev, warm=3, reps=10)
+            L.sync()
+            ok1 = same(d_out[:nout].cpu().numpy().view(np.uint64), d_off.cpu().numpy().view(np.uint64))
+            ms2 = wall(lambda: host_rows(named, after), 5)
+            ok2 = same(hout, hoff)
+            hoff[:] = 0
+            ms3 = wall(lambda: host_rows(anon, after), 5)
+            ok3 = same(hout, hoff)
+            single_out = [np.empty(max(min(m, int(a[1].sum(dtype=np.uint64))), 1), np.uint64) for a in arrs]
+            single_n = [C.c_size_t(0) for _ in range(nrows)]
+
+            def one(i):
+                _lib.check(lib.dgx_intersect_compressed_ref(C.byref(named[i]), after, hv.ctypes.data_as(C.c_void_p), m,
+                                                            single_out[i].ctypes.data_as(C.c_void_p), single_out[i].size,
+                                                            C.byref(single_n[i])))
+
+            def per_row():
+                with ThreadPoolExecutor(max_workers=threads) as ex:
+                    list(ex.map(one, range(nrows)))
+            ms4 = wall(per_row, 2)
+            ok4 = all(np.array_equal(single_out[i][: single_n[i].value], want[i]) for i in range(nrows))
+            cfg = (f"C6 handleUidPostings: {nrows} UidPacks (BlockSize 256, sizes ~ power law alpha=2 on [1e3,1e6], samples of a "
+                   f"2e7 Zipf-gap master, {exact} UIDs) each ∩ one v ({m} UIDs, thinning p=0.05), afterUID={after}")
+            uids_in = exact + m
+            extra = {"rows": nrows, "out": nout, "after": after,
+                     "bytes_note": "algorithmic bytes count every v element inside a touched block's range once per row; "
+                                   "slices longer than 4x the block are probed by binary search, so the kernel reads far "
+                                   "fewer and the GB/s figure is not an HBM rate"}
+            for name, ms, ok, note in (
+                ("IntersectCompressedWithRows (device, resident packs)", ms1, ok1, "dgx_dev_intersect_compressed_rows, CUDA events"),
+                ("IntersectCompressedWithRows (host, named packs, cache hits)", ms2, ok2, "dgx_intersect_compressed_rows, wall clock incl. D2H"),
+                ("IntersectCompressedWithRows (host, anonymous packs over PCIe)", ms3, ok3, "one pinned flat-image buffer per step, wall clock"),
+                (f"IntersectCompressedWith per row ({threads} host threads)", ms4, ok4, "dgx_intersect_compressed_ref per row, named packs, wall clock"),
+                ("oracle row loop (1 thread)", t_orc1 * 1e3, True, "algo.IntersectCompressedWith restated in C, one row after another"),
+                (f"oracle row loop ({ncpu} threads)", t_orcn * 1e3, True, "same, rows spread over every host thread"),
+            ):
+                out_rows.append(row(name, cfg, ms, uids_in, abytes, ok, dict(extra, rows_per_s=nrows / (ms * 1e-3), note=note)))
+    finally:
+        for h in handles:
+            lib.dgx_dev_pack_free(h)
+        lib.dgx_cache_clear()
+        lib.dgx_host_free(C.c_void_p(blob))
+    return out_rows
 
 
 if __name__ == "__main__":
