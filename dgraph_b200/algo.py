@@ -124,30 +124,14 @@ def IntersectSortedPacks(packs, keys=None) -> List:
     PCIe compressed and are decoded on the device (codec.Decode(p, 0) for each, codec/codec.go:444).
 
     keys: optional [(key, version)] naming each pack for the HBM-resident cache (0 = anonymous)."""
-    from .codec import ExactLen, view_of
-
     if len(packs) == 0:
         return List(None)
     lib = _lib.load()
-    k = len(packs)
-    refs = (_lib.PackRef * k)()
-    keep = []
-    cap = None
-    for i, p in enumerate(packs):
-        if p is None or p.nblocks == 0:
-            refs[i].pack = None
-            cap = 0
-        else:
-            p = p.normalized()
-            v = view_of(p)
-            keep.append((p, v))
-            refs[i].pack = C.pointer(v)
-            n = ExactLen(p)
-            cap = n if cap is None else min(cap, n)
-        refs[i].key, refs[i].version = (keys[i] if keys is not None else (0, 0))
-    out = np.empty(max(cap or 0, 1), dtype=np.uint64)
+    refs, keep = _refs_of(packs, keys)
+    cap = min(_exact(p) for p in packs)
+    out = np.empty(max(cap, 1), dtype=np.uint64)
     n = C.c_size_t(0)
-    _lib.check(lib.dgx_intersect_sorted_packed(refs, k, _p(out), cap or 0, C.byref(n)))
+    _lib.check(lib.dgx_intersect_sorted_packed(refs, len(packs), _p(out), cap, C.byref(n)))
     return List(out[: n.value])
 
 

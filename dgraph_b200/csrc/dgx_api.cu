@@ -1016,27 +1016,61 @@ static PackLayout pack_layout(const dgx_pack_view* v) {
     L.dpad = ((L.dbytes + 15) & ~size_t(15)) + 48;
     return L;
 }
-// Writes the metadata image at h (L.meta_bytes) and validates the block table.
-static int pack_fill_meta(const dgx_pack_view* v, const PackLayout& L, char* h, uint64_t* exact_len, uint32_t* max_num_out) {
-    const size_t nb = L.nb;
-    uint64_t* h_uoff = (uint64_t*)(h + L.o_uoff);
+// The block-table walk of every staging route: writes uid_off[0..nb] (exclusive prefix of NumUids, every block's
+// output offset) and returns ExactLen and the largest NumUids.  The kernels trust the block table: offsets must
+// ascend and every block must hold at least the 5-byte minimum of each group its NumUids needs (ceil((n-1)/4),
+// codec.go:76-96).  A pack that fails this is refused (the shim stays on the Go path) instead of being walked.
+static int walk_block_table(const dgx_pack_view* v, uint64_t* uid_off, uint64_t* exact_len, uint32_t* max_num_out) {
+    const size_t nb = v ? v->nblocks : 0;
     uint64_t acc = 0;
     uint32_t max_num = 0;
     for (size_t i = 0; i < nb; ++i) {
-        h_uoff[i] = acc;  // uid_off: exclusive prefix of NumUids, every block's output offset
+        uid_off[i] = acc;
         const uint32_t num = v->num_uids[i];
         acc += num;
         max_num = std::max(max_num, num);
-        // The kernels trust the block table: offsets must ascend and every block must hold at least
-        // the 5-byte minimum of each group its NumUids needs (ceil((n-1)/4), codec.go:76-96).  A pack
-        // that fails this is refused (the shim stays on the Go path) instead of being walked.
         const uint64_t b0 = v->delta_off[i], b1 = v->delta_off[i + 1];
         const uint64_t need = num > 1 ? 5ull * ((uint64_t)(num + 2) / 4) : 0;
         if (b1 < b0 || b1 - b0 < need)
             return fail(DGX_ERR_ARG, "malformed UidPack: block %zu has %lld delta bytes, NumUids %u needs >= %llu",
                         i, (long long)(b1 - b0), num, (unsigned long long)need);
     }
-    h_uoff[nb] = acc;
+    uid_off[nb] = acc;
+    *exact_len = acc;
+    *max_num_out = max_num;
+    return DGX_OK;
+}
+
+// The pack v (nullptr: the empty pack) at the device addresses of its arrays.  sysmem: the arrays other than uid_off
+// are mapped pinned host memory.  d_mem: the allocation the pack owns (nullptr: workspace or host memory).
+static dgx_dev_pack dev_pack(const dgx_pack_view* v, uint64_t exact_len, uint32_t max_num, const void* base,
+                             const void* delta_off, const void* num, const void* deltas, const void* uid_off, bool sysmem,
+                             size_t bytes, void* d_mem) {
+    dgx_dev_pack P;
+    P.pk.nblocks = v ? v->nblocks : 0;
+    P.pk.base = (const u64*)base;
+    P.pk.delta_off = (const u64*)delta_off;
+    P.pk.uid_off = (const u64*)uid_off;
+    P.pk.num = (const u32*)num;
+    P.pk.deltas = (const unsigned char*)deltas;
+    P.pk.max_num = max_num;
+    P.pk.sysmem = sysmem ? 1 : 0;
+    P.d_mem = d_mem;
+    P.bytes = bytes;
+    P.exact_len = exact_len;
+    P.block_size = v ? v->block_size : 0;
+    return P;
+}
+
+// Writes v's metadata image at h (L.meta_bytes) and sets *out to the pack it becomes once that image is copied to
+// d_meta and the delta bytes to d_deltas.
+static int pack_fill_meta(const dgx_pack_view* v, const PackLayout& L, char* h, char* d_meta, char* d_deltas,
+                          void* d_mem, dgx_dev_pack* out) {
+    const size_t nb = L.nb;
+    uint64_t exact = 0;
+    uint32_t max_num = 0;
+    int rc = walk_block_table(v, (uint64_t*)(h + L.o_uoff), &exact, &max_num);
+    if (rc) return rc;
     if (nb) {
         memcpy(h, v->base, nb * 8);
         memcpy(h + L.o_doff, v->delta_off, (nb + 1) * 8);
@@ -1044,53 +1078,28 @@ static int pack_fill_meta(const dgx_pack_view* v, const PackLayout& L, char* h, 
     } else {
         memset(h + L.o_doff, 0, 8);
     }
-    *exact_len = acc;
-    *max_num_out = max_num;
+    *out = dev_pack(v, exact, max_num, d_meta, d_meta + L.o_doff, d_meta + L.o_num, d_deltas, d_meta + L.o_uoff, false,
+                    L.meta_bytes + L.dpad, d_mem);
     return DGX_OK;
 }
-static void pack_point(dgx_dev_pack* out, const dgx_pack_view* v, const PackLayout& L, char* d_meta, char* d_deltas,
-                       uint64_t exact_len, uint32_t max_num) {
-    out->pk.nblocks = L.nb;
-    out->pk.base = (const u64*)d_meta;
-    out->pk.delta_off = (const u64*)(d_meta + L.o_doff);
-    out->pk.uid_off = (const u64*)(d_meta + L.o_uoff);
-    out->pk.num = (const u32*)(d_meta + L.o_num);
-    out->pk.deltas = (const unsigned char*)d_deltas;
-    out->pk.max_num = max_num;
-    out->pk.sysmem = 0;
-    out->bytes = L.meta_bytes + L.dpad;
-    out->exact_len = exact_len;
-    out->block_size = v ? v->block_size : 0;
-}
 
-// One pack -> one device allocation (cudaMalloc when arena == nullptr: the caller owns out->d_mem).
-static int pack_upload_impl(dgx_lane* l, const dgx_pack_view* v, void* d_mem_or_null, DevArena* arena,
-                            dgx_dev_pack* out) {
+// One pack -> its own cudaMalloc allocation (cache entries, dgx_dev_pack_upload).
+static int pack_upload_owned(dgx_lane* l, const dgx_pack_view* v, dgx_dev_pack* out) {
     const PackLayout L = pack_layout(v);
     const size_t total = L.meta_bytes + L.dpad;
-    void* d_mem = d_mem_or_null;
-    int rc;
-    if (!d_mem) {
-        if (arena) { rc = arena->alloc(total, &d_mem); if (rc) return rc; }
-        else {
-            cudaError_t e = cudaMalloc(&d_mem, total);
-            if (e != cudaSuccess) return fail(DGX_ERR_OOM, "cudaMalloc(%zu) failed: %s", total, cudaGetErrorString(e));
-            out->d_mem = d_mem;  // owned by *out from here on, also when a later step fails
-        }
-    }
+    void* d_mem = nullptr;
+    cudaError_t e = cudaMalloc(&d_mem, total);
+    if (e != cudaSuccess) return fail(DGX_ERR_OOM, "cudaMalloc(%zu) failed: %s", total, cudaGetErrorString(e));
+    out->d_mem = d_mem;  // owned by *out from here on, also when a later step fails
     void* h_raw;
-    rc = l->host.alloc(L.meta_bytes, &h_raw);
-    if (rc) return rc;
-    uint64_t exact = 0;
-    uint32_t max_num = 0;
-    rc = pack_fill_meta(v, L, (char*)h_raw, &exact, &max_num);
+    int rc = l->host.alloc(L.meta_bytes, &h_raw);
     if (rc) return rc;
     char* d = (char*)d_mem;
+    rc = pack_fill_meta(v, L, (char*)h_raw, d, d + L.meta_bytes, d_mem, out);
+    if (rc) return rc;
     CK(cudaMemcpyAsync(d, h_raw, L.meta_bytes, cudaMemcpyHostToDevice, l->stream));
     if (L.dbytes) CK(cudaMemcpyAsync(d + L.meta_bytes, v->deltas, L.dbytes, cudaMemcpyHostToDevice, l->stream));
     g_stats.h2d += L.meta_bytes + L.dbytes;
-    pack_point(out, v, L, d, d + L.meta_bytes, exact, max_num);
-    out->d_mem = d_mem;
     return DGX_OK;
 }
 
@@ -1135,34 +1144,12 @@ static int packs_map_ws(dgx_lane* l, const dgx_pack_view* const* views, size_t k
         const dgx_pack_view* v = views[i];
         if (!v) continue;
         const size_t nb = v->nblocks;
-        uint64_t* h_uoff = (uint64_t*)((char*)h_raw + o);
-        uint64_t acc = 0;
+        uint64_t exact = 0;
         uint32_t max_num = 0;
-        for (size_t b = 0; b < nb; ++b) {
-            h_uoff[b] = acc;
-            const uint32_t num = v->num_uids[b];
-            acc += num;
-            max_num = std::max(max_num, num);
-            const uint64_t b0 = v->delta_off[b], b1 = v->delta_off[b + 1];
-            const uint64_t need = num > 1 ? 5ull * ((uint64_t)(num + 2) / 4) : 0;
-            if (b1 < b0 || b1 - b0 < need)
-                return fail(DGX_ERR_ARG, "malformed UidPack: block %zu has %lld delta bytes, NumUids %u needs >= %llu",
-                            b, (long long)(b1 - b0), num, (unsigned long long)need);
-        }
-        h_uoff[nb] = acc;
-        dgx_dev_pack& P = outs[i];
-        P.pk.nblocks = nb;
-        P.pk.base = (const u64*)dv[i].base;
-        P.pk.num = (const u32*)dv[i].num;
-        P.pk.delta_off = (const u64*)dv[i].doff;
-        P.pk.deltas = (const unsigned char*)dv[i].del;
-        P.pk.uid_off = (const u64*)((char*)d_raw + o);
-        P.pk.max_num = max_num;
-        P.pk.sysmem = 1;
-        P.d_mem = nullptr;
-        P.bytes = 0;
-        P.exact_len = acc;
-        P.block_size = v->block_size;
+        rc = walk_block_table(v, (uint64_t*)((char*)h_raw + o), &exact, &max_num);
+        if (rc) return rc;
+        outs[i] = dev_pack(v, exact, max_num, dv[i].base, dv[i].doff, dv[i].num, dv[i].del, (char*)d_raw + o, true, 0,
+                           nullptr);
         o += (nb + 1) * sizeof(uint64_t);
         // the bytes still cross PCIe, as reads issued by the decode kernel
         g_stats.h2d += nb * 20 + (nb + 1) * 8 + (size_t)v->delta_off[nb];
@@ -1172,8 +1159,6 @@ static int packs_map_ws(dgx_lane* l, const dgx_pack_view* const* views, size_t k
     return DGX_OK;
 }
 
-// The k packs of one call into the lane's workspace: one copy for all metadata images, one per pack
-// for its delta bytes (straight from the caller's memory).  views[i] == nullptr entries are skipped.
 // Flat image of a pack (dgx_pack_image_size / dgx_pack_image_view): [base u64 x nb | delta_off u64 x (nb+1) |
 // num_uids u32 x nb | pad to 16 | deltas | pad to 16].  A shim that flattens pb.UidPack.Blocks into pinned staging
 // memory writes this directly; images written back to back travel as ONE DMA transfer.
@@ -1217,35 +1202,13 @@ static int packs_upload_run(dgx_lane* l, const dgx_pack_view* const* views, size
         const dgx_pack_view* v = views[i];
         if (!v) continue;
         const size_t nb = v->nblocks;
-        uint64_t* hu = (uint64_t*)((char*)h_uoff + uo);
-        uint64_t acc = 0;
+        uint64_t exact = 0;
         uint32_t max_num = 0;
-        for (size_t b = 0; b < nb; ++b) {
-            hu[b] = acc;
-            const uint32_t num = v->num_uids[b];
-            acc += num;
-            max_num = std::max(max_num, num);
-            const uint64_t b0 = v->delta_off[b], b1 = v->delta_off[b + 1];
-            const uint64_t need = num > 1 ? 5ull * ((uint64_t)(num + 2) / 4) : 0;
-            if (b1 < b0 || b1 - b0 < need)
-                return fail(DGX_ERR_ARG, "malformed UidPack: block %zu has %lld delta bytes, NumUids %u needs >= %llu",
-                            b, (long long)(b1 - b0), num, (unsigned long long)need);
-        }
-        hu[nb] = acc;
-        char* d = (char*)d_img + ((const char*)v->base - start);
-        dgx_dev_pack& P = outs[i];
-        P.pk.nblocks = nb;
-        P.pk.base = (const u64*)d;
-        P.pk.delta_off = (const u64*)(d + nb * 8);
-        P.pk.num = (const u32*)(d + nb * 8 + (nb + 1) * 8);
-        P.pk.deltas = (const unsigned char*)(d + image_meta_bytes(nb));
-        P.pk.uid_off = (const u64*)((char*)d_uoff + uo);
-        P.pk.max_num = max_num;
-        P.pk.sysmem = 0;
-        P.d_mem = nullptr;
-        P.bytes = view_image_bytes(v);
-        P.exact_len = acc;
-        P.block_size = v->block_size;
+        rc = walk_block_table(v, (uint64_t*)((char*)h_uoff + uo), &exact, &max_num);
+        if (rc) return rc;
+        const char* d = (const char*)d_img + ((const char*)v->base - start);
+        outs[i] = dev_pack(v, exact, max_num, d, d + nb * 8, d + nb * 8 + (nb + 1) * 8, d + image_meta_bytes(nb),
+                           (char*)d_uoff + uo, false, view_image_bytes(v), nullptr);
         uo += (nb + 1) * sizeof(uint64_t);
     }
     CK(cudaMemcpyAsync(d_img, start, run, cudaMemcpyHostToDevice, l->stream));
@@ -1255,6 +1218,9 @@ static int packs_upload_run(dgx_lane* l, const dgx_pack_view* const* views, size
     return DGX_OK;
 }
 
+// The one way one-shot packs reach the lane's workspace: the k packs of one call, as one run of images when they
+// are laid out that way, else one copy for all metadata images and one per pack for its delta bytes (straight
+// from the caller's memory).  views[i] == nullptr entries are skipped.
 static int packs_upload_ws(dgx_lane* l, const dgx_pack_view* const* views, size_t k, dgx_dev_pack* outs) {
     {
         bool done = false;
@@ -1281,12 +1247,8 @@ static int packs_upload_ws(dgx_lane* l, const dgx_pack_view* const* views, size_
     size_t mo = 0, dof = 0;
     for (size_t i = 0; i < k; ++i) {
         if (!views[i]) continue;
-        uint64_t exact = 0;
-        uint32_t max_num = 0;
-        rc = pack_fill_meta(views[i], Ls[i], h + mo, &exact, &max_num);
+        rc = pack_fill_meta(views[i], Ls[i], h + mo, d_meta + mo, d_del + dof, nullptr, &outs[i]);
         if (rc) return rc;
-        pack_point(&outs[i], views[i], Ls[i], d_meta + mo, d_del + dof, exact, max_num);
-        outs[i].d_mem = nullptr;  // workspace memory: not owned
         mo += Ls[i].meta_bytes;
         dof += Ls[i].dpad;
     }
@@ -1303,7 +1265,7 @@ extern "C" int dgx_dev_pack_upload(dgx_lane* l, const dgx_pack_view* v, dgx_dev_
     if (!l || !out) return fail(DGX_ERR_ARG, "null argument");
     CK(cudaSetDevice(l->device));
     dgx_dev_pack* pk = new dgx_dev_pack();
-    int rc = pack_upload_impl(l, v, nullptr, nullptr, pk);
+    int rc = pack_upload_owned(l, v, pk);
     // the pinned uid_off staging must outlive the async copy
     if (rc == DGX_OK && cudaStreamSynchronize(l->stream) != cudaSuccess) rc = fail(DGX_ERR_CUDA, "pack upload failed");
     if (rc) { dgx_dev_pack_free(pk); return rc; }
@@ -1433,6 +1395,23 @@ static int finish_to_host(dgx_lane* l, const uint64_t* d_len, const uint64_t* d_
     return DGX_OK;
 }
 
+// CSR result of a batch to the host: the npairs + 1 offsets, then the values they count.
+static int batch_to_host(dgx_lane* l, const void* d_out, const void* d_off, size_t npairs, uint64_t* out,
+                         uint64_t* out_off, size_t out_cap) {
+    CK(cudaMemcpyAsync(out_off, d_off, (npairs + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    int rc = dgx_lane_sync(l);
+    if (rc) return rc;
+    const uint64_t n = out_off[npairs];
+    if (n > out_cap) return fail(DGX_ERR_CAP, "batch result (%llu) does not fit out_cap (%zu)", (unsigned long long)n, out_cap);
+    if (n) {
+        CK(cudaMemcpyAsync(out, d_out, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+        CK(cudaStreamSynchronize(l->stream));
+    }
+    g_stats.d2h += (n + npairs + 1) * sizeof(uint64_t);
+    g_stats.uids_out += n;
+    return DGX_OK;
+}
+
 static int filter_host(int op, const uint64_t* const* lists, const size_t* lens, size_t k, uint64_t* out,
                        size_t out_cap, size_t* out_len) {
     LaneLease lease;
@@ -1541,18 +1520,7 @@ extern "C" int dgx_intersect_batch(const uint64_t* a, const uint64_t* a_off, con
     if (rc) return rc;
     rc = filter_batch_impl(l, DGX_OP_INTERSECT, ld.data(), k_off.data(), npairs, (uint64_t*)d_out, cap, (uint64_t*)d_off);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(out_off, d_off, (npairs + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
-    rc = dgx_lane_sync(l);
-    if (rc) return rc;
-    const uint64_t n = out_off[npairs];
-    if (n > out_cap) return fail(DGX_ERR_CAP, "batch result (%llu) does not fit out_cap (%zu)", (unsigned long long)n, out_cap);
-    if (n) {
-        CK(cudaMemcpyAsync(out, d_out, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
-        CK(cudaStreamSynchronize(l->stream));
-    }
-    g_stats.d2h += (n + npairs + 1) * sizeof(uint64_t);
-    g_stats.uids_out += n;
-    return DGX_OK;
+    return batch_to_host(l, d_out, d_off, npairs, out, out_off, out_cap);
 }
 
 extern "C" int dgx_decode(const dgx_pack_view* p, uint64_t seek, uint64_t* out, size_t out_cap, size_t* out_len) {
@@ -1565,7 +1533,7 @@ extern "C" int dgx_decode(const dgx_pack_view* p, uint64_t seek, uint64_t* out, 
     dgx_lane* l = lease.l;
     g_stats.calls += 1;
     dgx_dev_pack pk;
-    int rc = pack_upload_impl(l, p, nullptr, &l->ws, &pk);
+    int rc = packs_upload_ws(l, &p, 1, &pk);
     if (rc) return rc;
     g_stats.uids_in += pk.exact_len;
     void *d_out, *d_len;
@@ -1601,7 +1569,7 @@ extern "C" int dgx_decode_intersect_sorted(const dgx_pack_view* p, uint64_t seek
     size_t exact = 0;
     if (p && p->nblocks) {
         dgx_dev_pack pk;
-        rc = pack_upload_impl(l, p, nullptr, &l->ws, &pk);
+        rc = packs_upload_ws(l, &p, 1, &pk);
         if (rc) return rc;
         exact = pk.exact_len;
         rc = l->ws.alloc((exact + 2) * sizeof(uint64_t), &d_dec);
@@ -1677,7 +1645,6 @@ static int icw_impl(dgx_lane* l, const dgx_dev_pack& pk, uint64_t after, const u
     return DGX_OK;
 }
 
-struct PackLease;
 static int intersect_compressed_host(const dgx_pack_ref& ref, uint64_t after_uid, const uint64_t* v, size_t m,
                                      uint64_t* out, size_t out_cap, size_t* out_len);
 
@@ -1774,22 +1741,51 @@ extern "C" void dgx_cache_get_stats(dgx_cache_stats* out) {
     out->max_bytes = g_cache_max;
 }
 
-// A pack made available to lane `l`: from the cache (entry != nullptr, one reference held) or copied
-// into the lane's workspace for this call only.
-struct PackLease {
-    dgx_dev_pack pk;
-    CacheEntry* entry = nullptr;
-};
-static void pack_release(PackLease& pl) {
-    if (!pl.entry) return;
-    std::lock_guard<std::mutex> lk(g_cache_mu);
-    pl.entry->refs -= 1;
-    pl.entry = nullptr;
-}
-static int pack_acquire(dgx_lane* l, const dgx_pack_ref& ref, PackLease* out, bool* deferred) {
-    *deferred = false;
-    const dgx_pack_view* v = ref.pack;
-    if (ref.key != 0) {
+// The packs of one host-pointer call on lane `l`.  pk[i] is refs[i]'s pack: the empty pack for a nil or empty ref,
+// the cached copy for a named ref (one reference held until the set is destroyed), else copied into the lane's
+// workspace together with the call's other one-shot packs.  Declared after the call's LaneLease, so that it is
+// destroyed first: unless the call reported synced() after its final host sync, the destructor synchronises the
+// lane stream before it drops the references, since queued work may still read the cached packs.
+struct PackSet {
+    std::vector<dgx_dev_pack> pk;
+    int rc = DGX_OK;
+    // zero_copy: pinned one-shot packs are decoded in place when DGX_ZERO_COPY=1 (packs_map_ws)
+    PackSet(dgx_lane* lane, const dgx_pack_ref* refs, size_t k, bool zero_copy = false) : pk(k), l(lane) {
+        std::vector<const dgx_pack_view*> oneshot(k, nullptr);
+        for (size_t i = 0; i < k; ++i) {
+            const dgx_pack_view* v = refs[i].pack;
+            if (!v || v->nblocks == 0) continue;
+            CacheEntry* e = nullptr;
+            if (refs[i].key) rc = acquire(refs[i], &e);
+            if (rc) return;
+            if (e) pk[i] = e->pk;
+            else oneshot[i] = v;
+        }
+        bool mapped = false;
+        if (zero_copy) rc = packs_map_ws(l, oneshot.data(), k, pk.data(), &mapped);
+        if (rc == DGX_OK && !mapped) rc = packs_upload_ws(l, oneshot.data(), k, pk.data());
+    }
+    // rc of the call's final step, which ends in a host sync when it succeeds
+    int synced(int call_rc) {
+        finished = call_rc == DGX_OK;
+        return call_rc;
+    }
+    ~PackSet() {
+        if (!finished) cudaStreamSynchronize(l->stream);
+        if (held.empty()) return;
+        std::lock_guard<std::mutex> lk(g_cache_mu);
+        for (CacheEntry* e : held) e->refs -= 1;
+    }
+
+  private:
+    dgx_lane* l;
+    std::vector<CacheEntry*> held;
+    bool finished = false;
+
+    // *out: the cache entry holding ref's pack, one reference taken; nullptr when the pack does not fit (cache
+    // disabled, pack larger than the cache, everything pinned) and is copied for this call only.
+    int acquire(const dgx_pack_ref& ref, CacheEntry** out) {
+        const dgx_pack_view* v = ref.pack;
         std::lock_guard<std::mutex> lk(g_cache_mu);
         if (!g_cache_env_read) {
             g_cache_env_read = true;
@@ -1800,52 +1796,47 @@ static int pack_acquire(dgx_lane* l, const dgx_pack_ref& ref, PackLease* out, bo
         if (it != g_cache.end()) {
             CacheEntry* e = it->second;
             e->refs += 1;
+            held.push_back(e);
             g_cache_lru.erase(e->lru);
             g_cache_lru.push_front(e);
             e->lru = g_cache_lru.begin();
             g_cache_stats.hits += 1;
             CK(cudaStreamWaitEvent(l->stream, e->ready, 0));
-            out->pk = e->pk;
-            out->entry = e;
+            *out = e;
             return DGX_OK;
         }
         g_cache_stats.misses += 1;
         const size_t bytes = pack_device_bytes(v);
-        if (v && bytes <= g_cache_max) {
-            cache_make_room(bytes);
-            if (g_cache_bytes + bytes <= g_cache_max) {
-                CacheEntry* e = new CacheEntry();
-                e->id = id;
-                // the enqueue (a handful of async copies) happens under the lock so that a second caller
-                // asking for the same pack finds the recorded event, never a half-built entry
-                int rc = pack_upload_impl(l, v, nullptr, nullptr, &e->pk);
-                if (rc == DGX_OK && (cudaEventCreateWithFlags(&e->ready, cudaEventDisableTiming) != cudaSuccess ||
-                                     cudaEventRecord(e->ready, l->stream) != cudaSuccess))
-                    rc = fail(DGX_ERR_CUDA, "cache event failed");
-                if (rc) {
-                    if (e->pk.d_mem) cudaFree(e->pk.d_mem);
-                    if (e->ready) cudaEventDestroy(e->ready);
-                    delete e;
-                    return rc;
-                }
-                e->refs = 1;
-                g_cache_bytes += e->pk.bytes;
-                g_cache_lru.push_front(e);
-                e->lru = g_cache_lru.begin();
-                g_cache.emplace(id, e);
-                out->pk = e->pk;
-                out->entry = e;
-                return DGX_OK;
-            }
+        if (bytes > g_cache_max) return DGX_OK;
+        cache_make_room(bytes);
+        if (g_cache_bytes + bytes > g_cache_max) return DGX_OK;
+        CacheEntry* e = new CacheEntry();
+        e->id = id;
+        // the enqueue (a handful of async copies) happens under the lock so that a second caller
+        // asking for the same pack finds the recorded event, never a half-built entry
+        int rc = pack_upload_owned(l, v, &e->pk);
+        if (rc == DGX_OK && (cudaEventCreateWithFlags(&e->ready, cudaEventDisableTiming) != cudaSuccess ||
+                             cudaEventRecord(e->ready, l->stream) != cudaSuccess))
+            rc = fail(DGX_ERR_CUDA, "cache event failed");
+        if (rc) {
+            if (e->pk.d_mem) cudaFree(e->pk.d_mem);
+            if (e->ready) cudaEventDestroy(e->ready);
+            delete e;
+            return rc;
         }
-        // does not fit (cache disabled, pack larger than the cache, everything pinned): one-shot copy
+        e->refs = 1;
+        held.push_back(e);
+        g_cache_bytes += e->pk.bytes;
+        g_cache_lru.push_front(e);
+        e->lru = g_cache_lru.begin();
+        g_cache.emplace(id, e);
+        *out = e;
+        return DGX_OK;
     }
-    *deferred = true;  // copied into the lane's workspace together with the call's other one-shot packs
-    return DGX_OK;
-}
+};
 
-// Decode every pack of `pls` in full, side by side, with one launch; d_lists[i] receives pack i.
-static int decode_batch_impl(dgx_lane* l, const PackLease* pls, size_t k, uint64_t** d_lists) {
+// Decode every pack of `pks` in full, side by side, with one launch; d_lists[i] receives pack i.
+static int decode_batch_impl(dgx_lane* l, const dgx_dev_pack* pks, size_t k, uint64_t** d_lists) {
     void *h_raw, *d_raw;
     int rc = l->host.alloc(k * sizeof(DJob), &h_raw);
     if (rc) return rc;
@@ -1856,16 +1847,16 @@ static int decode_batch_impl(dgx_lane* l, const PackLease* pls, size_t k, uint64
     u32 nj = 0;
     for (size_t i = 0; i < k; ++i) {
         void* d;
-        rc = l->ws.alloc((pls[i].pk.exact_len + 2) * sizeof(uint64_t), &d);
+        rc = l->ws.alloc((pks[i].exact_len + 2) * sizeof(uint64_t), &d);
         if (rc) return rc;
         d_lists[i] = (uint64_t*)d;
-        if (pls[i].pk.pk.nblocks == 0) continue;
-        hj[nj].pk = pls[i].pk.pk;
+        if (pks[i].pk.nblocks == 0) continue;
+        hj[nj].pk = pks[i].pk;
         hj[nj].out = (u64*)d;
         hj[nj].warp_base = warps;
-        warps += (pls[i].pk.pk.nblocks + D_BPW - 1) / D_BPW;
+        warps += (pks[i].pk.nblocks + D_BPW - 1) / D_BPW;
         ++nj;
-        g_stats.uids_in += pls[i].pk.exact_len;
+        g_stats.uids_in += pks[i].exact_len;
     }
     if (nj == 0) return DGX_OK;
     CK(cudaMemcpyAsync(d_raw, h_raw, nj * sizeof(DJob), cudaMemcpyHostToDevice, l->stream));
@@ -1889,42 +1880,26 @@ extern "C" int dgx_intersect_sorted_packed(const dgx_pack_ref* refs, size_t k, u
     if (lease.rc) return lease.rc;
     dgx_lane* l = lease.l;
     g_stats.calls += 1;
-    std::vector<PackLease> pls(k);
+    PackSet ps(l, refs, k, /*zero_copy=*/true);
+    if (ps.rc) return ps.rc;
     std::vector<uint64_t*> d_lists(k, nullptr);
-    int rc = DGX_OK;
-    size_t got = 0;
-    std::vector<const dgx_pack_view*> oneshot(k, nullptr);
-    for (; got < k && rc == DGX_OK; ++got) {
-        bool deferred = false;
-        rc = pack_acquire(l, refs[got], &pls[got], &deferred);
-        if (deferred) oneshot[got] = refs[got].pack;
-    }
-    if (rc == DGX_OK) {
-        std::vector<dgx_dev_pack> up(k);
-        bool mapped = false;
-        rc = packs_map_ws(l, oneshot.data(), k, up.data(), &mapped);  // pinned packs are decoded in place (zero-copy)
-        if (rc == DGX_OK && !mapped) rc = packs_upload_ws(l, oneshot.data(), k, up.data());
-        for (size_t i = 0; i < k && rc == DGX_OK; ++i)
-            if (oneshot[i]) pls[i].pk = up[i];
-    }
-    if (rc == DGX_OK) rc = decode_batch_impl(l, pls.data(), k, d_lists.data());
+    int rc = decode_batch_impl(l, ps.pk.data(), k, d_lists.data());
+    if (rc) return rc;
+    std::vector<ListDesc> ld(k);
     size_t cap = SIZE_MAX;
-    void *d_out = nullptr, *d_off = nullptr;
-    if (rc == DGX_OK) {
-        std::vector<ListDesc> ld(k);
-        for (size_t i = 0; i < k; ++i) {
-            ld[i] = {d_lists[i], pls[i].pk.exact_len, nullptr};
-            cap = std::min(cap, pls[i].pk.exact_len);
-        }
-        rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-        if (rc == DGX_OK) rc = l->ws.alloc(2 * sizeof(uint64_t), &d_off);
-        const size_t k_off[2] = {0, k};
-        if (rc == DGX_OK) rc = filter_batch_impl(l, DGX_OP_INTERSECT, ld.data(), k_off, 1, (uint64_t*)d_out, cap, (uint64_t*)d_off);
+    for (size_t i = 0; i < k; ++i) {
+        ld[i] = {d_lists[i], ps.pk[i].exact_len, nullptr};
+        cap = std::min(cap, ps.pk[i].exact_len);
     }
-    if (rc == DGX_OK) rc = finish_to_host(l, (uint64_t*)d_off + 1, (uint64_t*)d_out, cap, out, out_cap, out_len);
-    else cudaStreamSynchronize(l->stream);  // nothing queued may outlive the references released below
-    for (size_t i = 0; i < got; ++i) pack_release(pls[i]);
-    return rc;
+    void *d_out, *d_off;
+    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc(2 * sizeof(uint64_t), &d_off);
+    if (rc) return rc;
+    const size_t k_off[2] = {0, k};
+    rc = filter_batch_impl(l, DGX_OP_INTERSECT, ld.data(), k_off, 1, (uint64_t*)d_out, cap, (uint64_t*)d_off);
+    if (rc) return rc;
+    return ps.synced(finish_to_host(l, (uint64_t*)d_off + 1, (uint64_t*)d_out, cap, out, out_cap, out_len));
 }
 
 static int intersect_compressed_host(const dgx_pack_ref& ref, uint64_t after_uid, const uint64_t* v, size_t m,
@@ -1940,20 +1915,19 @@ static int intersect_compressed_host(const dgx_pack_ref& ref, uint64_t after_uid
     if (lease.rc) return lease.rc;
     dgx_lane* l = lease.l;
     g_stats.calls += 1;
-    PackLease pl;
-    bool deferred = false;
-    int rc = pack_acquire(l, ref, &pl, &deferred);
-    if (rc == DGX_OK && deferred) rc = pack_upload_impl(l, ref.pack, nullptr, &l->ws, &pl.pk);
-    uint64_t* d_v = nullptr;
-    void *d_out = nullptr, *d_len = nullptr;
-    if (rc == DGX_OK) rc = upload_list(l, v, m, &d_v);
-    if (rc == DGX_OK) rc = l->ws.alloc((m + 2) * sizeof(uint64_t), &d_out);
-    if (rc == DGX_OK) rc = l->ws.alloc(64, &d_len);
-    if (rc == DGX_OK) rc = icw_impl(l, pl.pk, after_uid, d_v, m, (uint64_t*)d_out, m, (uint64_t*)d_len);
-    if (rc == DGX_OK) rc = finish_to_host(l, (uint64_t*)d_len, (uint64_t*)d_out, m, out, out_cap, out_len);
-    else cudaStreamSynchronize(l->stream);
-    pack_release(pl);
-    return rc;
+    PackSet ps(l, &ref, 1);
+    if (ps.rc) return ps.rc;
+    uint64_t* d_v;
+    int rc = upload_list(l, v, m, &d_v);
+    if (rc) return rc;
+    void *d_out, *d_len;
+    rc = l->ws.alloc((m + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc(64, &d_len);
+    if (rc) return rc;
+    rc = icw_impl(l, ps.pk[0], after_uid, d_v, m, (uint64_t*)d_out, m, (uint64_t*)d_len);
+    if (rc) return rc;
+    return ps.synced(finish_to_host(l, (uint64_t*)d_len, (uint64_t*)d_out, m, out, out_cap, out_len));
 }
 
 // Decoder.Seek / SeekToBlock / LinearSeek / Next / UnpackBlock for one call (codec/codec.go:154-384), on the device.
@@ -1968,7 +1942,7 @@ extern "C" int dgx_pack_seek(const dgx_pack_view* p, int kind, uint64_t uid, int
     dgx_lane* l = lease.l;
     g_stats.calls += 1;
     dgx_dev_pack pk;
-    int rc = pack_upload_impl(l, p, nullptr, &l->ws, &pk);
+    int rc = packs_upload_ws(l, &p, 1, &pk);
     if (rc) return rc;
     void *d_out, *d_meta;
     const size_t cap = std::max<size_t>(pk.pk.max_num, 1);
@@ -2171,69 +2145,44 @@ static int packed_op_host(int kind /*0 intersect, 1 difference, 2 merge*/, const
     if (lease.rc) return lease.rc;
     dgx_lane* l = lease.l;
     g_stats.calls += 1;
-    std::vector<PackLease> pls(k);
+    PackSet ps(l, refs, k);
+    if (ps.rc) return ps.rc;
     std::vector<uint64_t*> d_lists(k, nullptr);
-    std::vector<const dgx_pack_view*> oneshot(k, nullptr);
-    int rc = DGX_OK;
-    size_t got = 0;
-    static const dgx_pack_view kEmpty = {0, 0, nullptr, nullptr, nullptr, nullptr};
-    for (; got < k && rc == DGX_OK; ++got) {
-        dgx_pack_ref r = refs[got];
-        if (!r.pack || r.pack->nblocks == 0) { r.pack = &kEmpty; r.key = 0; }
-        bool deferred = false;
-        rc = pack_acquire(l, r, &pls[got], &deferred);
-        if (deferred) oneshot[got] = r.pack;
+    int rc = decode_batch_impl(l, ps.pk.data(), k, d_lists.data());
+    if (rc) return rc;
+    std::vector<ListDesc> ld(k);
+    size_t mn = SIZE_MAX, total = 0;
+    for (size_t i = 0; i < k; ++i) {
+        ld[i] = {d_lists[i], ps.pk[i].exact_len, nullptr};
+        mn = std::min(mn, ps.pk[i].exact_len);
+        total += ps.pk[i].exact_len;
     }
-    if (rc == DGX_OK) {
-        for (size_t i = 0; i < k; ++i)  // an empty view has no delta_off array: give the layout code a zero
-            if (oneshot[i] == &kEmpty) oneshot[i] = nullptr;
-        std::vector<dgx_dev_pack> up(k);
-        rc = packs_upload_ws(l, oneshot.data(), k, up.data());
-        for (size_t i = 0; i < k && rc == DGX_OK; ++i)
-            if (oneshot[i]) pls[i].pk = up[i];
-            else if (!pls[i].entry) { pls[i].pk = dgx_dev_pack(); pls[i].pk.pk = DPack(); pls[i].pk.pk.nblocks = 0; pls[i].pk.exact_len = 0; }
+    const size_t cap = kind == 0 ? (k ? mn : 0) : (kind == 1 ? (k ? ps.pk[0].exact_len : 0) : total);
+    void *d_out, *d_off, *d_len;
+    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc(64, &d_off);
+    if (rc) return rc;
+    if (kind == 2) {
+        d_len = d_off;
+        rc = merge_sorted_impl(l, ld.data(), k, (uint64_t*)d_out, cap, (uint64_t*)d_len);
+    } else if (k == 0) {
+        d_len = d_off;
+        CK(cudaMemsetAsync(d_len, 0, 8, l->stream));
+    } else {
+        const size_t k_off[2] = {0, k};
+        rc = filter_batch_impl(l, kind == 0 ? DGX_OP_INTERSECT : DGX_OP_DIFFERENCE, ld.data(), k_off, 1,
+                               (uint64_t*)d_out, cap, (uint64_t*)d_off);
+        d_len = (uint64_t*)d_off + 1;
     }
-    if (rc == DGX_OK) rc = decode_batch_impl(l, pls.data(), k, d_lists.data());
-    size_t cap = 0;
-    void *d_out = nullptr, *d_len = nullptr;
-    if (rc == DGX_OK) {
-        std::vector<ListDesc> ld(k);
-        size_t mn = SIZE_MAX, total = 0;
-        for (size_t i = 0; i < k; ++i) {
-            ld[i] = {d_lists[i], pls[i].pk.exact_len, nullptr};
-            mn = std::min(mn, pls[i].pk.exact_len);
-            total += pls[i].pk.exact_len;
-        }
-        cap = kind == 0 ? (k ? mn : 0) : (kind == 1 ? (k ? pls[0].pk.exact_len : 0) : total);
-        rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-        void* d_off = nullptr;
-        if (rc == DGX_OK) rc = l->ws.alloc(64, &d_off);
-        if (rc == DGX_OK) {
-            if (kind == 2) {
-                d_len = d_off;
-                rc = merge_sorted_impl(l, ld.data(), k, (uint64_t*)d_out, cap, (uint64_t*)d_len);
-            } else if (k == 0) {
-                d_len = d_off;
-                CK(cudaMemsetAsync(d_len, 0, 8, l->stream));
-            } else {
-                const size_t k_off[2] = {0, k};
-                rc = filter_batch_impl(l, kind == 0 ? DGX_OP_INTERSECT : DGX_OP_DIFFERENCE, ld.data(), k_off, 1,
-                                       (uint64_t*)d_out, cap, (uint64_t*)d_off);
-                d_len = (uint64_t*)d_off + 1;
-            }
-        }
-    }
+    if (rc) return rc;
+    size_t nb_cap, db_cap;
+    dgx_encode_bound(cap, block_size, &nb_cap, &db_cap);
+    nb_cap = std::max(nb_cap, std::min(*nblocks, cap));  // a larger capacity from the caller is honoured
     EncOut E;
-    if (rc == DGX_OK) {
-        size_t nb_cap, db_cap;
-        dgx_encode_bound(cap, block_size, &nb_cap, &db_cap);
-        nb_cap = std::max(nb_cap, std::min(*nblocks, cap));  // a larger capacity from the caller is honoured
-        rc = encode_impl(l, (const uint64_t*)d_out, cap, (const uint64_t*)d_len, block_size, nb_cap, db_cap, &E);
-    }
-    if (rc == DGX_OK) rc = encode_to_host(l, E, block_size, base, num_uids, delta_off, deltas, nblocks, delta_bytes, view);
-    else cudaStreamSynchronize(l->stream);
-    for (size_t i = 0; i < got; ++i) pack_release(pls[i]);
-    return rc;
+    rc = encode_impl(l, (const uint64_t*)d_out, cap, (const uint64_t*)d_len, block_size, nb_cap, db_cap, &E);
+    if (rc) return rc;
+    return ps.synced(encode_to_host(l, E, block_size, base, num_uids, delta_off, deltas, nblocks, delta_bytes, view));
 }
 
 extern "C" int dgx_intersect_packed(const dgx_pack_ref* u, const dgx_pack_ref* v, uint32_t block_size, uint64_t* base,
@@ -2288,22 +2237,6 @@ extern "C" int dgx_index_of_batch(const uint64_t* u, size_t n, const uint64_t* u
     CK(cudaMemcpyAsync(idx, d_idx, m * sizeof(int64_t), cudaMemcpyDeviceToHost, l->stream));
     g_stats.d2h += m * sizeof(int64_t);
     return dgx_lane_sync(l);
-}
-
-static int batch_to_host(dgx_lane* l, const void* d_out, const void* d_off, size_t npairs, uint64_t* out,
-                         uint64_t* out_off, size_t out_cap) {
-    CK(cudaMemcpyAsync(out_off, d_off, (npairs + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
-    int rc = dgx_lane_sync(l);
-    if (rc) return rc;
-    const uint64_t n = out_off[npairs];
-    if (n > out_cap) return fail(DGX_ERR_CAP, "batch result (%llu) does not fit out_cap (%zu)", (unsigned long long)n, out_cap);
-    if (n) {
-        CK(cudaMemcpyAsync(out, d_out, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
-        CK(cudaStreamSynchronize(l->stream));
-    }
-    g_stats.d2h += (n + npairs + 1) * sizeof(uint64_t);
-    g_stats.uids_out += n;
-    return DGX_OK;
 }
 
 extern "C" int dgx_intersect_batch_shared(const uint64_t* a, const uint64_t* a_off, size_t npairs, const uint64_t* b,
@@ -2467,40 +2400,25 @@ extern "C" int dgx_intersect_compressed_rows(const dgx_pack_ref* refs, size_t nr
     if (lease.rc) return lease.rc;
     dgx_lane* l = lease.l;
     g_stats.calls += 1;
-    std::vector<PackLease> pls(nrows);
-    std::vector<const dgx_pack_view*> oneshot(nrows, nullptr);
-    int rc = DGX_OK;
-    size_t got = 0;
-    for (; got < nrows && rc == DGX_OK; ++got) {
-        const dgx_pack_ref& r = refs[got];
-        if (!r.pack || r.pack->nblocks == 0) continue;  // nil / empty pack: empty row
-        bool deferred = false;
-        rc = pack_acquire(l, r, &pls[got], &deferred);
-        if (deferred) oneshot[got] = r.pack;
-    }
-    if (rc == DGX_OK) {  // the one-shot packs cross PCIe together (one transfer when they are back-to-back images)
-        std::vector<dgx_dev_pack> up(nrows);
-        rc = packs_upload_ws(l, oneshot.data(), nrows, up.data());
-        for (size_t i = 0; i < nrows && rc == DGX_OK; ++i)
-            if (oneshot[i]) pls[i].pk = up[i];
-    }
-    std::vector<const dgx_dev_pack*> rows(nrows, nullptr);
+    PackSet ps(l, refs, nrows);  // nil / empty packs are packs of no blocks: empty rows
+    if (ps.rc) return ps.rc;
+    std::vector<const dgx_dev_pack*> rows(nrows);
     size_t cap = 0;
-    for (size_t i = 0; i < nrows && rc == DGX_OK; ++i)
-        if (refs[i].pack && refs[i].pack->nblocks) {
-            rows[i] = &pls[i].pk;
-            cap += std::min<size_t>(m, pls[i].pk.exact_len);
-        }
-    uint64_t* d_v = nullptr;
-    void *d_out = nullptr, *d_off = nullptr;
-    if (rc == DGX_OK) rc = upload_list(l, v, m, &d_v);
-    if (rc == DGX_OK) rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-    if (rc == DGX_OK) rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
-    if (rc == DGX_OK) rc = icw_rows_impl(l, rows.data(), nrows, after_uid, d_v, m, (uint64_t*)d_out, cap, (uint64_t*)d_off);
-    if (rc == DGX_OK) rc = batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap);
-    else cudaStreamSynchronize(l->stream);  // nothing queued may outlive the references released below
-    for (size_t i = 0; i < got; ++i) pack_release(pls[i]);
-    return rc;
+    for (size_t i = 0; i < nrows; ++i) {
+        rows[i] = &ps.pk[i];
+        cap += std::min<size_t>(m, ps.pk[i].exact_len);
+    }
+    uint64_t* d_v;
+    int rc = upload_list(l, v, m, &d_v);
+    if (rc) return rc;
+    void *d_out, *d_off;
+    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
+    if (rc) return rc;
+    rc = icw_rows_impl(l, rows.data(), nrows, after_uid, d_v, m, (uint64_t*)d_out, cap, (uint64_t*)d_off);
+    if (rc) return rc;
+    return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
 }
 
 // ---------------------------------------------------------------------------

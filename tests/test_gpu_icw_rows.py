@@ -12,7 +12,7 @@ import pytest
 sys.path.insert(0, os.path.dirname(__file__))
 import gen  # noqa: E402
 import gen_rows  # noqa: E402
-from test_gpu_parity import eq, to_pack  # noqa: E402
+from test_gpu_parity import eq, generic_bytes, image_bytes, pack_images, to_pack  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -224,6 +224,15 @@ def test_rows_cap_and_malformed(dgx, orc):
     with pytest.raises(_lib.DgxError) as ei:
         dgx.algo.IntersectCompressedWithRows([packs[0], bad_named], 0, v, [(7001, 1), (7002, 1)])
     assert ei.value.code == ERR_ARG
+    # the references the failed calls took on good named packs are released: entries still referenced are never
+    # evicted, so a leaked one would survive the clear
+    with pytest.raises(_lib.DgxError) as ei:
+        dgx.algo.IntersectCompressedWithRows([packs[0], packs[1], bad], 0, v, [(7003, 1), (7004, 1), (0, 0)])
+    assert ei.value.code == ERR_ARG
+    lib.dgx_cache_clear()
+    st = _lib.CacheStats()
+    lib.dgx_cache_get_stats(C.byref(st))
+    assert st.entries == 0
     # v of 2^32 or more uids is refused (the per-block v-ranges are 32-bit); nothing of v is read
     rc = lib.dgx_intersect_compressed_rows(refs, 2, 0, _p(v), 1 << 32, _p(out), _p(off), need)
     assert rc == ERR_ARG
@@ -231,6 +240,48 @@ def test_rows_cap_and_malformed(dgx, orc):
     out2, off2 = dgx.algo.IntersectCompressedWithRows(packs, 0, v)
     for i, g in enumerate(rows_of(out2, off2)):
         eq(g, want_row(orc, ops[i], 0, v), f"after errors row {i}")
+
+
+def test_rows_pack_images(dgx, orc):
+    """Anonymous packs written back to back as flat images into one pinned buffer (what bench.py and the C6 rows of
+    tools/bench_ops.py send) cross PCIe as one transfer; a gap between two images sends the call down the route for
+    separate arrays; a malformed image among good ones is refused."""
+    from dgraph_b200 import _lib
+
+    lib = _lib.load()
+    rng = np.random.default_rng(79)
+    master = gen.zipf_gaps(rng, 600_000)
+    lists = [gen.thin(rng, master, 0.3), gen.thin(rng, master, 0.001), None, gen.thin(rng, master, 0.5), master[:1]]
+    ops = [None if l is None else orc.encode(l, bs) for l, bs in zip(lists, (256, 256, 0, 7, 256))]
+    packs = [None if op is None else to_pack(dgx, op) for op in ops]
+    v = gen.thin(rng, master, 0.05)
+    after = int(master[1000])
+    wants = [want_row(orc, op, after, v) for op in ops]
+    cap = sum(w.size for w in wants)
+    out, off = np.empty(cap + 1, np.uint64), np.zeros(len(packs) + 1, np.uint64)
+
+    def call(refs):
+        h0 = _lib.stats()["h2d_bytes"]
+        _lib.check(lib.dgx_intersect_compressed_rows(refs, len(packs), after, _p(v), v.size, _p(out), _p(off), cap))
+        return [r.copy() for r in rows_of(out, off)], _lib.stats()["h2d_bytes"] - h0
+
+    refs, keep = dgx.algo._refs_of(packs)
+    separate, h2d_separate = call(refs)
+    for i, g in enumerate(separate):
+        eq(g, wants[i], f"separate arrays row {i}")
+    real = [p for p in packs if p is not None]
+    for gaps, extra in (((), sum(image_bytes(p) - generic_bytes(p) for p in real)), ((3,), 0)):
+        with pack_images(packs, gaps) as img_refs:
+            got, h2d = call(img_refs)
+        for i, g in enumerate(got):
+            eq(g, wants[i], f"images gaps {gaps} row {i}")
+            eq(g, separate[i], f"images gaps {gaps} row {i} vs separate arrays")
+        assert h2d == h2d_separate + extra, f"gaps {gaps}: staged through the wrong route"
+    bad = dgx.pb.UidPack(packs[3].block_size, packs[3].base, packs[3].num_uids, packs[3].delta_off.copy(), packs[3].deltas)
+    bad.delta_off[3] = bad.delta_off[2] + 2
+    with pack_images(packs[:3] + [bad] + packs[4:]) as img_refs:
+        rc = lib.dgx_intersect_compressed_rows(img_refs, len(packs), after, _p(v), v.size, _p(out), _p(off), cap)
+    assert rc == ERR_ARG
 
 
 def test_rows_device_form(dgx, orc):

@@ -4,6 +4,8 @@ Runs on an H100 only (`pytest -m gpu`).  Known-answer cases transcribe the
 reference's own tests; randomized cases compare with oracle/ on the same seeded
 inputs; large cases use size-independent properties plus the oracle.
 """
+import contextlib
+import ctypes as C
 import os
 import sys
 import threading
@@ -50,6 +52,49 @@ def to_pack(dgx, op):
     if op.is_nil:
         return None
     return dgx.pb.UidPack(op.block_size, op.base, op.num_uids, op.delta_off, op.deltas)
+
+
+@contextlib.contextmanager
+def pack_images(packs, gaps=()):
+    """The packs written back to back as flat images (dgx_pack_image_size / dgx_pack_image_view) into one pinned
+    dgx_host_alloc buffer, as a shim's flatten writes them; 16 unused bytes precede pack i for every i in `gaps`.
+    Yields a PackRef array over them (a NULL pack for None)."""
+    from dgraph_b200 import _lib
+
+    lib = _lib.load()
+    sizes = [0 if p is None else lib.dgx_pack_image_size(p.nblocks, p.deltas.size) for p in packs]
+    blob = lib.dgx_host_alloc(sum(sizes) + 16 * len(gaps) + 64)
+    assert blob
+    try:
+        refs = (_lib.PackRef * len(packs))()
+        views, o = [], 0
+        for i, (p, sz) in enumerate(zip(packs, sizes)):
+            if p is None:
+                continue
+            o += 16 if i in gaps else 0
+            p = p.normalized()
+            pv = _lib.PackView()
+            _lib.check(lib.dgx_pack_image_view(C.c_void_p(blob + o), p.block_size, p.nblocks, p.deltas.size, C.byref(pv)))
+            for dst, src in ((pv.base, p.base), (pv.delta_off, p.delta_off), (pv.num_uids, p.num_uids), (pv.deltas, p.deltas)):
+                C.memmove(dst, src.ctypes.data, src.nbytes)
+            views.append(pv)
+            refs[i].pack = C.pointer(pv)
+            o += sz
+        yield refs
+    finally:
+        lib.dgx_host_free(C.c_void_p(blob))
+
+
+def generic_bytes(p):
+    """h2d_bytes a pack given as separate arrays counts when it is copied: its metadata image, then its deltas."""
+    return ((28 * p.nblocks + 31) & ~15) + p.deltas.size
+
+
+def image_bytes(p):
+    """h2d_bytes a pack given as a flat image counts when it is copied: the image, then its uid_off table."""
+    from dgraph_b200 import _lib
+
+    return _lib.load().dgx_pack_image_size(p.nblocks, p.deltas.size) + 8 * (p.nblocks + 1)
 
 
 # ---- known answers from algo/uidlist_test.go ------------------------------------

@@ -1,7 +1,8 @@
 """GPU parity, round-2 entry points and BASELINE-size configs: libdgx (through the C ABI) vs the CPU
 oracle, bit-exact.  Runs on an H100 only (`pytest -m gpu`).
 
- - IntersectSorted over packs (dgx_intersect_sorted_packed) with and without the HBM pack cache
+ - IntersectSorted over packs (dgx_intersect_sorted_packed) with and without the HBM pack cache, as flat images in
+   pinned memory and decoded in place (DGX_ZERO_COPY=1)
  - IndexOf batch, shared-list batch
  - malformed packs are refused, not walked
  - BASELINE configs[2] (1e8-UID pack -> decode -> IntersectSorted), configs[3] (10k pairs, power-law sizes),
@@ -17,7 +18,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(__file__))
 import gen  # noqa: E402
-from test_gpu_parity import L, eq, to_pack  # noqa: E402
+from test_gpu_parity import L, eq, generic_bytes, image_bytes, pack_images, to_pack  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -59,6 +60,8 @@ def same(got, want, what):
 # ---- IntersectSorted over packs, pack cache -------------------------------------------------------
 
 def test_intersect_sorted_packed(dgx, orc):
+    from dgraph_b200 import _lib
+
     rng = np.random.default_rng(31)
     master = gen.zipf_gaps(rng, 400_000)
     for k, p, bs in ((1, 0.5, 256), (2, 0.5, 256), (3, 0.3, 10), (8, 0.25, 256), (8, 0.9, 256), (12, 0.8, 64)):
@@ -77,6 +80,81 @@ def test_intersect_sorted_packed(dgx, orc):
     a, b = hi[rng.random(hi.size) < 0.7], hi[rng.random(hi.size) < 0.7]
     got = dgx.algo.IntersectSortedPacks([to_pack(dgx, orc.encode(a, 256)), to_pack(dgx, orc.encode(b, 256))])
     eq(got.Uids, orc.intersect_sorted([a, b]), "packed full-range")
+    # flat images back to back in one pinned buffer cross PCIe as one transfer; a gap between two images sends the
+    # call down the route for separate arrays; a malformed image among good ones is refused
+    lists = [gen.thin(rng, master, p) for p in (0.5, 0.6, 0.7)]
+    packs = [to_pack(dgx, orc.encode(l, bs)) for l, bs in zip(lists, (256, 10, 256))]
+    want = orc.intersect_sorted(lists)
+    eq(dgx.algo.IntersectSortedPacks(packs).Uids, want, "separate arrays")
+    for gaps, staged in (((), sum(image_bytes(p) for p in packs)), ((1,), sum(generic_bytes(p) for p in packs))):
+        with pack_images(packs, gaps) as refs:
+            got, h2d = sorted_packed(refs, len(packs), want.size)
+        eq(got, want, f"images gaps {gaps}")
+        assert h2d == staged, f"gaps {gaps}: staged through the wrong route"
+    bad = dgx.pb.UidPack(packs[1].block_size, packs[1].base, packs[1].num_uids, packs[1].delta_off.copy(), packs[1].deltas)
+    bad.delta_off[3] = bad.delta_off[2] + 2
+    with pack_images([packs[0], bad, packs[2]]) as refs:
+        with pytest.raises(_lib.DgxError) as ei:
+            sorted_packed(refs, 3, want.size)
+    assert ei.value.code == -3
+
+
+def sorted_packed(refs, k, cap):
+    """dgx_intersect_sorted_packed over a PackRef array: the result and the h2d_bytes the call counted."""
+    from dgraph_b200 import _lib
+
+    lib = _lib.load()
+    out = np.empty(max(cap, 1), np.uint64)
+    n = C.c_size_t(0)
+    h0 = _lib.stats()["h2d_bytes"]
+    _lib.check(lib.dgx_intersect_sorted_packed(refs, k, out.ctypes.data_as(C.c_void_p), cap, C.byref(n)))
+    return out[: n.value], _lib.stats()["h2d_bytes"] - h0
+
+
+def test_intersect_sorted_packed_zero_copy(orc):
+    """DGX_ZERO_COPY=1, in a subprocess because libdgx reads its knobs once: pinned packs are decoded in place over
+    PCIe, a pageable pack in the same call sends every pack through DMA copies, a malformed pinned pack is refused."""
+    import subprocess
+    code = r'''
+import os, sys
+import numpy as np
+sys.path.insert(0, os.getcwd()); sys.path.insert(0, os.path.join(os.getcwd(), "tests"))
+import gen
+import dgraph_b200
+from dgraph_b200 import _lib
+from oracle import pyoracle as orc
+from test_gpu_parity import eq, generic_bytes, pack_images, to_pack
+from test_gpu_round2 import sorted_packed
+rng = np.random.default_rng(37)
+master = gen.zipf_gaps(rng, 300_000)
+lists = [gen.thin(rng, master, p) for p in (0.5, 0.6, 0.7)]
+packs = [to_pack(dgraph_b200, orc.encode(l, bs)) for l, bs in zip(lists, (256, 10, 256))]
+want = orc.intersect_sorted(lists)
+with pack_images(packs) as refs:
+    got, h2d = sorted_packed(refs, 3, want.size)
+    eq(got, want, "pinned")
+    # only uid_off is copied; the decode kernel's reads over PCIe are counted: base, NumUids, delta_off, deltas
+    assert h2d == sum(28 * p.nblocks + 8 + p.deltas.size for p in packs), h2d
+    mixed = (_lib.PackRef * 3)()
+    pageable, keep = dgraph_b200.algo._refs_of([packs[1]])
+    mixed[0], mixed[1], mixed[2] = refs[0], pageable[0], refs[2]
+    got, h2d = sorted_packed(mixed, 3, want.size)
+    eq(got, want, "pinned and pageable")
+    assert h2d == sum(generic_bytes(p) for p in packs), h2d
+bad = dgraph_b200.pb.UidPack(packs[1].block_size, packs[1].base, packs[1].num_uids, packs[1].delta_off.copy(), packs[1].deltas)
+bad.delta_off[3] = bad.delta_off[2] + 2
+with pack_images([packs[0], bad, packs[2]]) as refs:
+    try:
+        sorted_packed(refs, 3, want.size)
+        raise AssertionError("malformed pinned pack accepted")
+    except _lib.DgxError as e:
+        assert e.code == -3, e.code
+print("ZERO_COPY_OK")
+'''
+    env = dict(os.environ, DGX_ZERO_COPY="1")
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600, env=env,
+                       cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+    assert "ZERO_COPY_OK" in r.stdout, r.stdout[-2000:] + r.stderr[-4000:]
 
 
 def test_pack_cache(dgx, orc):
@@ -162,6 +240,17 @@ def test_malformed_pack_refused(dgx, orc):
     bad2.delta_off[5] = bad2.delta_off[4] - 1        # offsets go backwards
     with pytest.raises(_lib.DgxError):
         dgx.codec.Decode(bad2, 0)
+    # a call refused on a malformed pack, named or not, releases the cache references it took on the good named
+    # packs before it: entries still referenced are never evicted, so a leaked one would survive the clear
+    lib = _lib.load()
+    for keys in ([(9001, 1), (9002, 1), (9003, 1)], [(9001, 1), (9002, 1), (0, 0)]):
+        with pytest.raises(_lib.DgxError) as ei:
+            dgx.algo.IntersectSortedPacks([good, good, bad], keys)
+        assert ei.value.code == -3
+    lib.dgx_cache_clear()
+    st = _lib.CacheStats()
+    lib.dgx_cache_get_stats(C.byref(st))
+    assert st.entries == 0
     # tags that claim more bytes than the block holds: memory-safe, library usable afterwards
     evil = dgx.pb.UidPack(good.block_size, good.base, good.num_uids, good.delta_off, np.full_like(good.deltas, 0xFF))
     out = dgx.codec.Decode(evil, 0)
