@@ -197,6 +197,34 @@ def IntersectCompressedWithRows(packs, afterUID: int, v, keys=None):
     return out[: int(out_off[-1])], out_off
 
 
+def IntersectCompressedWithMatrix(pack, rows, key=None):
+    """algo.IntersectCompressedWith(pack, 0, rows[i], o_i) for every row i in ONE call
+    (dgx_intersect_compressed_matrix): the intersectBucket loop (worker/sort.go:605-700) of one index bucket over a
+    uid matrix.
+
+    rows: strictly ascending uid lists (pb.List values or arrays).  key: optional (key, version) naming the pack for the
+    HBM-resident cache.  A nil / empty pack gives empty rows.  Returns (out, out_off): row i is
+    out[out_off[i]:out_off[i+1]]."""
+    arrs = []
+    for r in rows:
+        u = r.Uids if isinstance(r, List) else r
+        arrs.append(np.zeros(0, np.uint64) if u is None else _u64(u))
+    nrows = len(arrs)
+    out_off = np.zeros(nrows + 1, dtype=np.uint64)
+    if nrows == 0:
+        return np.zeros(0, np.uint64), out_off
+    v_off = np.zeros(nrows + 1, dtype=np.uint64)
+    np.cumsum([a.size for a in arrs], out=v_off[1:])
+    v = np.concatenate(arrs) if int(v_off[-1]) else np.zeros(1, np.uint64)
+    lib = _lib.load()
+    refs, keep = _refs_of([pack], [key] if key is not None else None)
+    exact = _exact(pack)
+    cap = sum(min(a.size, exact) for a in arrs)
+    out = np.empty(max(cap, 1), dtype=np.uint64)
+    _lib.check(lib.dgx_intersect_compressed_matrix(refs, _p(v), _p(v_off), nrows, _p(out), _p(out_off), cap))
+    return out[: int(out_off[-1])], out_off
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -558,6 +558,242 @@ __global__ void __launch_bounds__(256) icw_rows_gather_kernel(const IcwRowsParam
     for (u64 k = t & 31; k < c; k += 32) dst[k] = src[k];
 }
 
+// ---- one pack, many v: the rows of a uid matrix against one posting list -------------------------
+// intersectBucket (worker/sort.go:605-700) intersects every row of a uid matrix with the same index bucket's pack
+// (afterUID 0).  The rows are the concatenation v[0 .. M), row i = v[v_off[i] .. v_off[i+1]).  A UNIT is the run of
+// one row's elements inside one block's value range.  Membership of v[j] in the pack is all the result needs: keep[j]
+// is set on a match, and the CSR result is v compacted by keep (row i starts at the count of matches before v_off[i]).
+//   icw_mx_locate_kernel  thread per element: its row (search of v_off), the rows-ascend check, its block (search of
+//                         the bases); the first element of a unit finds the unit's end by a search of its row and
+//                         counts the unit for its block
+//   scan_u64_kernel       units per block -> each block's first position in block order
+//   icw_mx_place_kernel   thread per element: every unit takes a position in its block's range (block order)
+//   icw_mx_probe_kernel   warp per 32 positions: one TMA window over the touched blocks, each distinct block expanded
+//                         ONCE into shared memory and probed by all of its units in the warp; blocks of more than
+//                         256 uids are walked lane-serially from global memory, one unit per lane
+//   scan_u64_kernel       keep -> output positions
+//   icw_mx_gather_kernel  out_off and out
+// Work and workspace are linear in M + units + nrows + nblocks (units <= M); a block touched by every row is cut into
+// pieces of 32 units, one per warp.  Every row must ascend strictly; the locate pass checks it (each thread reads its
+// predecessor anyway), and a violation sets kLaneErrOrder in the lane's error flag and empties the result.
+constexpr int kLaneErrOrder = 2;  // lane error flag bit: a row of a matrix call does not ascend (DGX_ERR_ARG at sync);
+                                  // the flag's value 1 (result past out_cap, DGX_ERR_CAP) is unchanged
+constexpr u32 MX_SERIAL = 8;      // units of at most this many elements are probed by their own lane
+struct IcwMatrixParams {
+    DPack pk;
+    const u64* v;            // m values, rows concatenated
+    u64 m;
+    const u64* v_off;        // nrows + 1
+    u64 nrows;
+    u64* head;               // per element: (block << 32 | unit end) where a unit starts, else kU64Max
+    u64* bcount;             // per block: units; zero-initialised
+    u32* bfill;              // per block: units placed so far; zero-initialised
+    u64* boff;               // nblocks + 1: first position of each block's units
+    u64* unit;               // per position: lo | hi << 32 (v indices)
+    u32* ublk;               // per position: block
+    u64 unit_cap;            // positions allocated (= sum_i min(|row i|, nblocks) units of ascending rows)
+    u64* keep;               // per element: 1 when in the pack
+    u64* kex;                // m + 1: exclusive scan of keep
+    u64* out;
+    u64 out_cap;
+    u64* out_off;            // nrows + 1
+    int* bad;                // workspace word, zero-initialised: some row does not ascend
+    int* err;
+};
+
+__device__ __forceinline__ long long icw_block_of(const DPack& pk, u64 x) {  // last b with base[b] <= x, or -1
+    u64 lo = 0, hi = pk.nblocks;
+    while (lo < hi) {
+        const u64 mid = lo + ((hi - lo) >> 1);
+        if (ld_probe(pk.base + mid) <= x) lo = mid + 1; else hi = mid;
+    }
+    return (long long)lo - 1;
+}
+
+__global__ void __launch_bounds__(256) icw_mx_locate_kernel(const IcwMatrixParams P) {
+    const u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= P.m) return;
+    P.keep[k] = 0;
+    u64 lo = 1, hi = P.nrows;  // row: last r with v_off[r] <= k (first r >= 1 with v_off[r] > k, minus one)
+    while (lo < hi) {
+        const u64 mid = lo + ((hi - lo) >> 1);
+        if (ld_probe(P.v_off + mid) <= k) lo = mid + 1; else hi = mid;
+    }
+    const u64 s = ld_probe(P.v_off + lo - 1), e = ld_probe(P.v_off + lo);
+    const u64 x = P.v[k];
+    const u64 xp = k > s ? P.v[k - 1] : 0;
+    if (k > s && xp >= x) {
+        *P.bad = 1;
+        atomicOr(P.err, kLaneErrOrder);
+    }
+    u64 hd = kU64Max;
+    const long long b = icw_block_of(P.pk, x);
+    if (b >= 0 && (k == s || xp < ld_probe(P.pk.base + b))) {  // the row's first element in block b
+        const u64 end = (u64)b + 1 < P.pk.nblocks ? k + lower_bound_g(P.v + k, e - k, ld_probe(P.pk.base + b + 1)) : e;
+        hd = ((u64)b << 32) | end;
+        atomicAdd(P.bcount + b, 1ull);
+    }
+    P.head[k] = hd;
+}
+
+__global__ void __launch_bounds__(256) icw_mx_place_kernel(const IcwMatrixParams P) {
+    const u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= P.m) return;
+    const u64 hd = P.head[k];
+    if (hd == kU64Max) return;
+    const u32 b = (u32)(hd >> 32);
+    const u64 pos = P.boff[b] + atomicAdd(P.bfill + b, 1u);
+    if (pos >= P.unit_cap) return;  // only when a row does not ascend: the result is discarded then
+    P.unit[pos] = k | (hd << 32);
+    P.ublk[pos] = b;
+}
+
+__global__ void __launch_bounds__(D_NT) icw_mx_probe_kernel(const IcwMatrixParams P) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    DWarpSmem& S = reinterpret_cast<DWarpSmem*>(smem_raw)[wid];
+    const DPack& pk = P.pk;
+    const u64 nu = min(P.boff[pk.nblocks], P.unit_cap);
+    const u64 p0 = ((u64)blockIdx.x * D_WARPS + wid) * 32;
+    if (p0 >= nu) return;
+    const int nin = (int)min(nu - p0, (u64)32);
+    const bool in = lane < nin;
+    const u64 lh = in ? P.unit[p0 + lane] : 0;
+    const u32 blk = in ? P.ublk[p0 + lane] : 0u;
+    const u32 lo = (u32)lh, hi = (u32)(lh >> 32);
+    const u64 doff = in ? pk.delta_off[blk] : 0, dnext = in ? pk.delta_off[blk + 1] : 0;
+    const u32 num = in ? pk.num[blk] : 0u;
+    const u64 base = in ? pk.base[blk] : 0;
+    const u32 ngroups = num > 1 ? (num + 2) / 4 : 0;
+    const u32 bup = __shfl_up_sync(0xffffffffu, blk, 1);
+    const u32 bar = smem_u32(&S.mbar);
+    if (lane == 0) {
+        mbar_init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    u32 parity = 0;
+
+    int f = 0;  // lanes [0, f) are done; positions are in block order, so a block's units are adjacent lanes
+    while (f < nin) {
+        const u64 win0 = __shfl_sync(0xffffffffu, doff, f) & ~15ull;
+        const bool ok = in && lane >= f && num <= 256u && (dnext - win0 <= (u64)D_WB);
+        const unsigned om = __ballot_sync(0xffffffffu, ok) >> f;
+        const int run = om == (0xffffffffu >> f) ? 32 - f : __ffs(~om) - 1;  // leading lanes whose blocks fit the window
+        if (run == 0) {
+            // block of more than 256 uids (non-reference BlockSize): every unit of it walks it from global memory
+            const u32 bf = __shfl_sync(0xffffffffu, blk, f);
+            const unsigned grp = __ballot_sync(0xffffffffu, in && lane >= f && blk == bf);
+            if ((grp >> lane) & 1u) {
+                const unsigned char* p = pk.deltas + doff;
+                u64 y = base;
+                u32 produced = 1, q = lo;
+                auto probe = [&](u64 uid) {  // merge step: both sides ascend
+                    while (q < hi && ld_probe(P.v + q) < uid) ++q;
+                    if (q < hi && ld_probe(P.v + q) == uid) P.keep[q] = 1;
+                };
+                probe(y);
+                while (produced < num && q < hi) {
+                    const u32 tag = p[0];
+                    const unsigned char* d = p + 1;
+                    for (int j = 0; j < 4 && produced < num; ++j) {
+                        const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
+                        u32 v32 = 0;
+                        for (u32 t = 0; t < l; ++t) v32 |= (u32)d[t] << (8 * t);
+                        d += l;
+                        y += v32;
+                        ++produced;
+                        probe(y);
+                    }
+                    p += gv_bytes_used(tag);
+                }
+            }
+            f += __popc(grp);
+            continue;
+        }
+        const int rend = f + run;
+        const bool mine = lane >= f && lane < rend;
+        // one leader per distinct block of the run; it walks the block's tags into its goff column
+        const bool lead = mine && (lane == f || bup != blk);
+        const unsigned leaders = __ballot_sync(0xffffffffu, lead);
+        const u64 wend = __shfl_sync(0xffffffffu, dnext, rend - 1);
+        const u32 bytes = (u32)(((wend - win0) + 15ull) & ~15ull);
+        if (lane == 0) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            mbar_expect_tx(bar, bytes);
+            if (bytes) tma_bulk_g2s(smem_u32(S.payload), pk.deltas + win0, bytes, bar);
+        }
+        mbar_wait(bar, parity);
+        parity ^= 1u;
+        if (lead) {
+            u32 off = (u32)(doff - win0);
+            const u32 off_end = (u32)(dnext - win0);
+            for (u32 g = 0; g < ngroups; ++g) {
+                S.goff[g * D_TSTRIDE + lane] = (unsigned short)off;
+                off += gv_bytes_used(S.payload[off]);
+                off = off < off_end ? off : off_end;
+            }
+        }
+        __syncwarp();
+
+        for (unsigned rest = leaders; rest; rest &= rest - 1) {
+            const int i = __ffs(rest) - 1;
+            const unsigned later = (rest & (rest - 1));
+            const int iend = later ? __ffs(later) - 1 : rend;  // units of this block: lanes [i, iend)
+            const u32 n_i = __shfl_sync(0xffffffffu, num, i);
+            const u64 base_i = __shfl_sync(0xffffffffu, base, i);
+            const u32 ng_i = __shfl_sync(0xffffffffu, ngroups, i);
+            icw_expand_block(S, i, ng_i, base_i, lane);
+            const bool grp = lane >= i && lane < iend;
+            const u32 c = hi - lo;
+            if (grp && c <= MX_SERIAL) {  // short units, side by side: each lane searches the block with its own
+                for (u32 j = lo; j < hi; ++j) {
+                    const u64 x = ld_probe(P.v + j);
+                    const int pos = lower_bound_s(S.stage, 0, (int)n_i, x);
+                    if (pos < (int)n_i && S.stage[pos] == x) P.keep[j] = 1;
+                }
+            }
+            // longer units one after another with the whole warp, the shorter side searching the longer one
+            for (unsigned big = __ballot_sync(0xffffffffu, grp && c > MX_SERIAL); big; big &= big - 1) {
+                const int t = __ffs(big) - 1;
+                const u32 lo_t = __shfl_sync(0xffffffffu, lo, t), hi_t = __shfl_sync(0xffffffffu, hi, t);
+                const u32 c_t = hi_t - lo_t;
+                if (c_t <= 4u * n_i) {
+                    for (u32 j = lo_t + lane; j < hi_t; j += 32) {
+                        const u64 x = ld_stream(P.v + j);
+                        const int pos = lower_bound_s(S.stage, 0, (int)n_i, x);
+                        if (pos < (int)n_i && S.stage[pos] == x) P.keep[j] = 1;
+                    }
+                } else {
+                    for (u32 e = lane; e < n_i; e += 32) {
+                        const u64 y = S.stage[e];
+                        const u64 pos = lo_t + lower_bound_g(P.v + lo_t, (u64)c_t, y);
+                        if (pos < hi_t && ld_probe(P.v + pos) == y) P.keep[pos] = 1;
+                    }
+                }
+            }
+            __syncwarp();  // the next block's expansion overwrites S.stage
+        }
+        f = rend;
+    }
+}
+
+// Thread t < m moves v[t] to its place when kept; thread t <= nrows writes out_off[t].  A row that does not ascend
+// empties the result (out untouched, every offset 0); past out_cap nothing of out is written.
+__global__ void __launch_bounds__(256) icw_mx_gather_kernel(const IcwMatrixParams P) {
+    const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+    if (*P.bad) {
+        if (t <= P.nrows) P.out_off[t] = 0;
+        return;
+    }
+    if (t <= P.nrows) P.out_off[t] = P.kex[P.v_off[t]];
+    if (P.kex[P.m] > P.out_cap) {
+        if (t == 0) atomicExch(P.err, 1);
+        return;
+    }
+    if (t < P.m && P.keep[t]) P.out[P.kex[t]] = P.v[t];
+}
+
 // ---- Decoder seeks on the device (codec/codec.go:219-384) --------------------------------------
 // One thread restates the control flow of the reference's iterator for ONE call and expands the block it
 // lands on; what comes back is what the Go call returns: the uid slice and the decoder's new block index.

@@ -451,9 +451,10 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
     l->ws.release_retired();
     l->outs.clear();
     l->outs_overflow = false;
-    if (*l->h_err) {
+    if (const int flag = *l->h_err) {
         *l->h_err = 0;
         CK(cudaMemsetAsync(l->d_err, 0, sizeof(int), l->stream));
+        if (flag & kLaneErrOrder) return fail(DGX_ERR_ARG, "a row of the uid matrix is not strictly ascending");
         return fail(DGX_ERR_CAP, "result does not fit out_cap");
     }
     return DGX_OK;
@@ -2417,6 +2418,149 @@ extern "C" int dgx_intersect_compressed_rows(const dgx_pack_ref* refs, size_t nr
     rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
     if (rc) return rc;
     rc = icw_rows_impl(l, rows.data(), nrows, after_uid, d_v, m, (uint64_t*)d_out, cap, (uint64_t*)d_off);
+    if (rc) return rc;
+    return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
+}
+
+// ---------------------------------------------------------------------------
+// IntersectCompressedWith of one pack against every row of a uid matrix (intersectBucket)
+// ---------------------------------------------------------------------------
+// v_off (host) must start at 0, never decrease and end below 2^32: checked before anything of v is read.
+static int check_v_off(const uint64_t* v_off, size_t nrows) {
+    if (v_off[0] != 0) return fail(DGX_ERR_ARG, "v_off[0] is %llu, not 0", (unsigned long long)v_off[0]);
+    for (size_t r = 0; r < nrows; ++r)
+        if (v_off[r + 1] < v_off[r]) return fail(DGX_ERR_ARG, "v_off decreases at row %zu", r);
+    if (v_off[nrows] >= (uint64_t(1) << 32))
+        return fail(DGX_ERR_ARG, "the matrix has %llu uids: unit ranges are 32-bit", (unsigned long long)v_off[nrows]);
+    return DGX_OK;
+}
+
+// Row i = algo.IntersectCompressedWith(pk, 0, v[v_off[i] .. v_off[i+1])) with six launches whatever nrows, M and the
+// block count are (compressed_kernel.cuh): locate, unit scan, place, probe, keep scan, gather.  Workspace: at most 36
+// bytes per element of v plus about 20 per block and 8 per row.  v_off is host memory, already checked.
+static int icw_matrix_impl(dgx_lane* l, const dgx_dev_pack& pk, const uint64_t* d_v, const uint64_t* v_off, size_t nrows,
+                           uint64_t* d_out, size_t out_cap, uint64_t* d_out_off) {
+    const uint64_t m = v_off[nrows], nb = pk.pk.nblocks;
+    g_stats.uids_in += pk.exact_len + m;
+    if (nb == 0 || m == 0) {  // nothing can match: every row is empty
+        CK(cudaMemsetAsync(d_out_off, 0, (nrows + 1) * sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (nb > 0xffffffffull) return fail(DGX_ERR_ARG, "pack of %llu blocks: block indices are 32-bit", (unsigned long long)nb);
+    uint64_t units = 0;  // units of ascending rows: each row touches at most min(|row|, nb) blocks
+    for (size_t r = 0; r < nrows; ++r) units += std::min<uint64_t>(v_off[r + 1] - v_off[r], nb);
+    const uint64_t kMaxGrid = 0x7fffffffull;
+    const uint64_t g_elem = (m + 255) / 256, g_gather = (std::max<uint64_t>(m, nrows + 1) + 255) / 256;
+    const uint64_t t_blk = (nb + EN_TILE - 1) / EN_TILE, t_elem = (m + EN_TILE - 1) / EN_TILE;
+    const uint64_t g_probe = ((units + 31) / 32 + D_WARPS - 1) / D_WARPS;
+    if (std::max({g_elem, g_gather, g_probe}) > kMaxGrid)
+        return fail(DGX_ERR_ARG, "matrix too large for one launch (%llu uids, %zu rows)", (unsigned long long)m, nrows);
+    // table (copied): [v_off | nb | m];  zeroed: [bcount | bfill | scan status + tickets | bad];  then head, boff,
+    // unit, ublk, keep, kex
+    const size_t b_tab = (nrows + 3) * sizeof(uint64_t);
+    const size_t b_zero = nb * sizeof(u64) + ((nb * sizeof(u32) + 15) & ~size_t(15)) + (t_blk + t_elem) * sizeof(u64) + 16;
+    const size_t b_rest = (m + (nb + 1) + units + m + (m + 1)) * sizeof(u64) + ((units * sizeof(u32) + 15) & ~size_t(15));
+    void *h_raw, *d_raw;
+    int rc = l->host.alloc(b_tab, &h_raw);
+    if (rc) return rc;
+    rc = l->ws.alloc(b_tab + b_zero + b_rest, &d_raw);
+    if (rc) return rc;
+    uint64_t* h_tab = (uint64_t*)h_raw;
+    memcpy(h_tab, v_off, (nrows + 1) * sizeof(uint64_t));
+    h_tab[nrows + 1] = nb;
+    h_tab[nrows + 2] = m;
+    char* d = (char*)d_raw;
+    CK(cudaMemcpyAsync(d, h_tab, b_tab, cudaMemcpyHostToDevice, l->stream));
+    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
+    g_stats.h2d += b_tab;
+    IcwMatrixParams P;
+    P.pk = pk.pk;
+    P.v = (const u64*)d_v;
+    P.m = m;
+    P.v_off = (const u64*)d;
+    P.nrows = nrows;
+    const u64* d_nb = P.v_off + nrows + 1;  // scan lengths as device words
+    const u64* d_m = P.v_off + nrows + 2;
+    char* z = d + b_tab;
+    P.bcount = (u64*)z;
+    P.bfill = (u32*)(P.bcount + nb);
+    u64* status = (u64*)((char*)P.bfill + ((nb * sizeof(u32) + 15) & ~size_t(15)));
+    u32* tickets = (u32*)(status + t_blk + t_elem);
+    P.bad = (int*)(tickets + 2);
+    P.head = (u64*)(z + b_zero);
+    P.boff = P.head + m;
+    P.unit = P.boff + nb + 1;
+    P.keep = P.unit + units;
+    P.kex = P.keep + m;
+    P.ublk = (u32*)(P.kex + m + 1);
+    P.unit_cap = units;
+    P.out = (u64*)d_out;
+    P.out_cap = out_cap;
+    P.out_off = (u64*)d_out_off;
+    P.err = l->d_err;
+    icw_mx_locate_kernel<<<(unsigned)g_elem, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)t_blk, EN_NT, 0, l->stream>>>(P.bcount, P.boff, d_nb, nb, status, tickets, nullptr);
+    CK(cudaGetLastError());
+    icw_mx_place_kernel<<<(unsigned)g_elem, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    icw_mx_probe_kernel<<<(unsigned)g_probe, D_NT, sizeof(DWarpSmem) * D_WARPS, l->stream>>>(P);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)t_elem, EN_NT, 0, l->stream>>>(P.keep, P.kex, d_m, m, status + t_blk, tickets + 1, nullptr);
+    CK(cudaGetLastError());
+    icw_mx_gather_kernel<<<(unsigned)g_gather, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    l->launches += 6;
+    g_stats.launches += 6;
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_intersect_compressed_matrix(dgx_lane* l, const dgx_dev_pack* pk, const uint64_t* d_v,
+                                                   const uint64_t* v_off, size_t nrows, uint64_t* d_out, size_t out_cap,
+                                                   uint64_t* d_out_off) {
+    if (!l || !d_out_off || (nrows && !v_off)) return fail(DGX_ERR_ARG, "null argument");
+    static const uint64_t zero_off = 0;
+    if (nrows == 0) v_off = &zero_off;
+    if (int rc = check_v_off(v_off, nrows)) return rc;
+    if (v_off[nrows] && !d_v) return fail(DGX_ERR_ARG, "null d_v");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    const dgx_dev_pack empty = dev_pack(nullptr, 0, 0, nullptr, nullptr, nullptr, nullptr, nullptr, false, 0, nullptr);
+    const int rc = icw_matrix_impl(l, pk ? *pk : empty, d_v, v_off, nrows, d_out, out_cap, d_out_off);
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    return rc;
+}
+
+extern "C" int dgx_intersect_compressed_matrix(const dgx_pack_ref* ref, const uint64_t* v, const uint64_t* v_off,
+                                               size_t nrows, uint64_t* out, uint64_t* out_off, size_t out_cap) {
+    if (!out_off) return fail(DGX_ERR_ARG, "null out_off");
+    if (nrows == 0) { out_off[0] = 0; return DGX_OK; }
+    if (!ref || !v_off) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = check_v_off(v_off, nrows)) return rc;
+    const size_t m = v_off[nrows];
+    if (m && !v) return fail(DGX_ERR_ARG, "null v");
+    if (!ref->pack || ref->pack->nblocks == 0) {  // nil / empty pack: every row is empty, nothing runs
+        memset(out_off, 0, (nrows + 1) * sizeof(uint64_t));
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    PackSet ps(l, ref, 1);
+    if (ps.rc) return ps.rc;
+    size_t cap = 0;
+    for (size_t r = 0; r < nrows; ++r) cap += std::min<size_t>(v_off[r + 1] - v_off[r], ps.pk[0].exact_len);
+    uint64_t* d_v;
+    int rc = upload_list(l, v, m, &d_v);
+    if (rc) return rc;
+    void *d_out, *d_off;
+    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
+    if (rc) return rc;
+    rc = icw_matrix_impl(l, ps.pk[0], d_v, v_off, nrows, (uint64_t*)d_out, cap, (uint64_t*)d_off);
     if (rc) return rc;
     return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
 }

@@ -244,6 +244,72 @@ func IntersectCompressedWithRows(refs []PackRef, afterUID uint64, v *pb.List) ([
 	return rows, true
 }
 
+// dgxMinMatrix: below this many uids (ApproxLen of the bucket + all rows) IntersectCompressedWithMatrix stays on the
+// Go path.  Set from the C7 record (profiles/h100_c7_sort_buckets.json, H100 80GB HBM3, 400 W): the host form took
+// 0.62 ms for the whole tiny-bucket call, and the row loop on one CPU thread spent 0.64 us per matrix uid there, so
+// a matrix of about 1 000 uids costs the Go loop what one library call costs.
+const dgxMinMatrix = 1 << 10
+
+// IntersectCompressedWithMatrix is algo.IntersectCompressedWith(ref.Pack, 0, rows[i], o_i) for every row of a uid
+// matrix in ONE library call: the loop intersectBucket (worker/sort.go:605-700) runs for each index bucket of a sort,
+// reaching algo.IntersectCompressedWith through posting/list.go:1795-1800.  Every row must be strictly ascending (a
+// uid matrix row is).  The rows travel as one CSR allocation in C memory; the result rows are slices of one buffer.
+// A nil / empty pack gives empty rows.  Returns false when the caller must keep pl.Uids: on any error, when the call
+// is too small to pay off (dgxMinMatrix), or when the matrix holds 2^32 uids or more.
+func IntersectCompressedWithMatrix(ref PackRef, rows []*pb.List) ([]*pb.List, bool) {
+	n := len(rows)
+	if n == 0 {
+		return []*pb.List{}, true
+	}
+	m, capOut := 0, 0
+	exact := ExactLen(ref.Pack)
+	for _, r := range rows {
+		m += len(r.Uids)
+		if len(r.Uids) < exact {
+			capOut += len(r.Uids)
+		} else {
+			capOut += exact
+		}
+	}
+	if ApproxLen(ref.Pack)+m < dgxMinMatrix || uint64(m) >= 1<<32 {
+		return nil, false
+	}
+	// [v_off: n + 1 values | v: m values]
+	csr := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(n+1+m) * 8))
+	defer C.free(unsafe.Pointer(csr))
+	voff, o := csr[:n+1:n+1], 0
+	v := csr[n+1 : n+1+m : n+1+m]
+	for i, r := range rows {
+		voff[i] = C.uint64_t(o)
+		if len(r.Uids) > 0 {
+			C.memcpy(unsafe.Pointer(&v[o]), unsafe.Pointer(&r.Uids[0]), C.size_t(len(r.Uids)*8))
+		}
+		o += len(r.Uids)
+	}
+	voff[n] = C.uint64_t(o)
+	cref := C.dgx_pack_ref{key: C.uint64_t(ref.Key), version: C.uint64_t(ref.Version)}
+	if ref.Pack != nil && len(ref.Pack.Blocks) > 0 {
+		view, free := flatten(ref.Pack)
+		defer free()
+		cref.pack = &view
+	}
+	out := make([]uint64, capOut+1)
+	off := make([]uint64, n+1)
+	var vp *C.uint64_t
+	if m > 0 {
+		vp = &v[0]
+	}
+	if C.dgx_intersect_compressed_matrix(&cref, vp, &voff[0], C.size_t(n), (*C.uint64_t)(unsafe.Pointer(&out[0])),
+		(*C.uint64_t)(unsafe.Pointer(&off[0])), C.size_t(capOut)) != C.DGX_OK {
+		return nil, false
+	}
+	res := make([]*pb.List, n)
+	for i := range rows {
+		res[i] = &pb.List{Uids: out[off[i]:off[i+1]:off[i+1]]}
+	}
+	return res, true
+}
+
 func deltaBytes(pack *pb.UidPack) int {
 	t := 0
 	for _, b := range pack.Blocks {

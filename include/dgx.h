@@ -212,6 +212,17 @@ int dgx_intersect_compressed_rows(const dgx_pack_ref* refs, size_t nrows, uint64
                                   const uint64_t* v, size_t m,
                                   uint64_t* out, uint64_t* out_off, size_t out_cap);
 
+/* algo.IntersectCompressedWith(pack, 0, v_i, o_i) for every row i of a uid matrix, one call: the intersectBucket loop
+ * (worker/sort.go:605-700 -> posting/list.go:1795-1800).  Row i of the input is v[v_off[i] .. v_off[i+1]) (host
+ * offsets, nrows + 1 values, v_off[0] == 0); row i of the result is out[out_off[i] .. out_off[i+1]).  ref as in
+ * dgx_intersect_compressed_ref (named packs use the HBM cache).  out_cap >= sum_i min(|v_i|, ExactLen(pack)).
+ * Every row must ascend strictly; a row that does not is DGX_ERR_ARG and nothing is written to out.  v_off[0] != 0,
+ * decreasing offsets, v_off[nrows] >= 2^32 and malformed packs are DGX_ERR_ARG before anything is copied.  A NULL /
+ * empty pack gives empty rows and nrows == 0 gives out_off[0] = 0; neither needs a device.  The call runs a fixed
+ * number of kernel launches whatever nrows, the number of uids and the pack's size are. */
+int dgx_intersect_compressed_matrix(const dgx_pack_ref* ref, const uint64_t* v, const uint64_t* v_off, size_t nrows,
+                                    uint64_t* out, uint64_t* out_off, size_t out_cap);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -356,6 +367,13 @@ int dgx_dev_decode(dgx_lane* lane, const dgx_dev_pack* pk, uint64_t seek,
 int dgx_dev_intersect_compressed_rows(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t nrows,
                                       uint64_t after_uid, const uint64_t* d_v, size_t m,
                                       uint64_t* d_out, size_t out_cap, uint64_t* d_out_off);
+/* Device form of dgx_intersect_compressed_matrix: pack resident (dgx_dev_pack_upload; NULL = empty rows), d_v / d_out
+ * / d_out_off (nrows + 1 values) device pointers, v_off in HOST memory (checked and staged by the call).  Asynchronous
+ * on the lane: past out_cap nothing is written and the next dgx_lane_sync returns DGX_ERR_CAP; a row that does not
+ * ascend strictly leaves d_out untouched, zeroes d_out_off and makes the next dgx_lane_sync return DGX_ERR_ARG. */
+int dgx_dev_intersect_compressed_matrix(dgx_lane* lane, const dgx_dev_pack* pk, const uint64_t* d_v,
+                                        const uint64_t* v_off, size_t nrows,
+                                        uint64_t* d_out, size_t out_cap, uint64_t* d_out_off);
 
 #ifdef __cplusplus
 }

@@ -132,9 +132,15 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--small", action="store_true", help="1/10 sizes (quick functional pass)")
     ap.add_argument("--c6-only", action="store_true", help="only the C6 handleUidPostings rows")
+    ap.add_argument("--c7-only", action="store_true", help="only the C7 sort-bucket rows")
     args = ap.parse_args()
-    rows = c6_rows(Lane()) if args.c6_only else run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only:
+        rows = c6_rows(Lane())
+    elif args.c7_only:
+        rows = c7_rows(Lane())
+    else:
+        rows = run(Lane(), 10 if args.small else 1, quick=False)
+    if args.c6_only or args.c7_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -383,6 +389,7 @@ def run(L, S, quick):
     for ptr in pins:
         L.lib.dgx_host_free(ptr)
     rows += c6_rows(L)
+    rows += c7_rows(L)
     return rows
 
 
@@ -520,6 +527,115 @@ def c6_rows(L, threads: int = 4):
             lib.dgx_dev_pack_free(h)
         lib.dgx_cache_clear()
         lib.dgx_host_free(C.c_void_p(blob))
+    return out_rows
+
+
+def c7_rows(L, threads: int = 4):
+    """C7 "sort buckets": one uid matrix of 10 000 rows (sizes ~ power law alpha=2 on [10, 1e4]) intersected with each
+    of three index-bucket packs (BlockSize 256: 1e6, 1e4 and 100 uids), the intersectBucket loop of an indexed sort
+    (worker/sort.go:605-700 -> algo.IntersectCompressedWith(pack, 0, row)).  Four legs per bucket, each checked row by
+    row against the oracle: (1) dgx_dev_intersect_compressed_matrix with the pack and the matrix resident (CUDA
+    events), (2) dgx_intersect_compressed_matrix with a named pack that hits the cache, the matrix crossing PCIe every
+    call (wall clock), (3) dgx_intersect_compressed_ref per row from `threads` host threads, (4) the oracle row loop on
+    one thread, as the reference's single goroutine runs it."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    import gen_sort
+    from dgraph_b200 import codec, pb
+    from oracle import pyoracle as orc
+
+    lib = L.lib
+    master, rows_u, buckets = gen_sort.c7_inputs()
+    nrows = len(rows_u)
+    v_off = np.zeros(nrows + 1, np.uint64)
+    np.cumsum([r.size for r in rows_u], out=v_off[1:])
+    hv = np.ascontiguousarray(np.concatenate(rows_u))
+    m = hv.size
+    d_v = torch.from_numpy(hv.view(np.int64)).to(DEV)
+    pv_off = v_off.ctypes.data_as(C.c_void_p)
+
+    def wall(fn, reps):
+        fn()
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            fn()
+        return (time.perf_counter() - t0) / reps * 1e3
+
+    lib.dgx_cache_clear()
+    _lib.check(lib.dgx_cache_configure(16 << 30))
+    out_rows = []
+    for bi, (bname, uids) in enumerate(buckets.items()):
+        op = orc.encode(uids, 256)
+        pk = pb.UidPack(op.block_size, op.base, op.num_uids, op.delta_off, op.deltas).normalized()
+        view = codec.view_of(pk)  # pk stays alive for the whole bucket
+        ref = _lib.PackRef(C.pointer(view), 700_000 + bi, 1)
+        t0 = time.perf_counter()
+        want = [orc.intersect_compressed_with(op, 0, r) for r in rows_u]
+        t_orc = time.perf_counter() - t0
+        want_off = np.concatenate([[0], np.cumsum([w.size for w in want])]).astype(np.uint64)
+        want_all = np.concatenate(want) if want_off[-1] else np.zeros(0, np.uint64)
+        nout = int(want_off[-1])
+        cap = int(np.minimum(np.diff(v_off), uids.size).sum())
+        abytes = gen_sort.matrix_algorithmic_bytes(pk.base, pk.delta_off, rows_u, nout)
+
+        def same(out, off):
+            return bool(np.array_equal(off, want_off) and np.array_equal(out[:nout], want_all))
+
+        h = C.c_void_p()
+        _lib.check(lib.dgx_dev_pack_upload(L.h, C.byref(view), C.byref(h)))
+        try:
+            d_out = torch.empty(cap + 8, dtype=torch.int64, device=DEV)
+            d_off = torch.zeros(nrows + 1, dtype=torch.int64, device=DEV)
+
+            def dev():
+                _lib.check(lib.dgx_dev_intersect_compressed_matrix(L.h, h, C.c_void_p(d_v.data_ptr()), pv_off, nrows,
+                                                                   C.c_void_p(d_out.data_ptr()), cap,
+                                                                   C.c_void_p(d_off.data_ptr())))
+            ms1, _ = timeit(dev, warm=3, reps=20)
+            L.sync()
+            ok1 = same(d_out[:nout].cpu().numpy().view(np.uint64), d_off.cpu().numpy().view(np.uint64))
+        finally:
+            lib.dgx_dev_pack_free(h)
+        hout = np.empty(max(cap, 1), np.uint64)
+        hoff = np.zeros(nrows + 1, np.uint64)
+
+        def host():
+            _lib.check(lib.dgx_intersect_compressed_matrix(C.byref(ref), hv.ctypes.data_as(C.c_void_p), pv_off, nrows,
+                                                           hout.ctypes.data_as(C.c_void_p),
+                                                           hoff.ctypes.data_as(C.c_void_p), cap))
+        ms2 = wall(host, 10)
+        ok2 = same(hout, hoff)
+        single_out = [np.empty(max(r.size, 1), np.uint64) for r in rows_u]
+        single_n = [C.c_size_t(0) for _ in range(nrows)]
+
+        def one(i):
+            r = rows_u[i]
+            _lib.check(lib.dgx_intersect_compressed_ref(C.byref(ref), 0, r.ctypes.data_as(C.c_void_p), r.size,
+                                                        single_out[i].ctypes.data_as(C.c_void_p), single_out[i].size,
+                                                        C.byref(single_n[i])))
+
+        def per_row():
+            with ThreadPoolExecutor(max_workers=threads) as ex:
+                list(ex.map(one, range(nrows)))
+        ms3 = wall(per_row, 2)
+        ok3 = all(np.array_equal(single_out[i][: single_n[i].value], want[i]) for i in range(nrows))
+        cfg = (f"C7 sort buckets: bucket '{bname}' ({uids.size} UIDs, {op.base.size} blocks of BlockSize 256, a sample "
+               f"of a 2e7 Zipf-gap master) against a uid matrix of {nrows} rows ({m} UIDs, sizes ~ power law alpha=2 "
+               f"on [10,1e4], samples of the master), afterUID 0")
+        extra = {"bucket": bname, "rows": nrows, "matrix_uids": m, "out": nout}
+        for name, ms, ok, note in (
+            ("IntersectCompressedWithMatrix (device, resident pack and matrix)", ms1, ok1,
+             "dgx_dev_intersect_compressed_matrix, CUDA events"),
+            ("IntersectCompressedWithMatrix (host, named pack, cache hit)", ms2, ok2,
+             "dgx_intersect_compressed_matrix, the matrix crosses PCIe every call, wall clock incl. D2H"),
+            (f"IntersectCompressedWith per row ({threads} host threads)", ms3, ok3,
+             "dgx_intersect_compressed_ref per row, named pack, wall clock"),
+            ("oracle row loop (1 thread)", t_orc * 1e3, True,
+             "algo.IntersectCompressedWith restated in C, one row after another"),
+        ):
+            out_rows.append(row(name, cfg, ms, uids.size + m, abytes, ok,
+                                dict(extra, rows_per_s=nrows / (ms * 1e-3), note=note)))
+    lib.dgx_cache_clear()
     return out_rows
 
 
