@@ -225,6 +225,28 @@ def IntersectCompressedWithMatrix(pack, rows, key=None):
     return out[: int(out_off[-1])], out_off
 
 
+def MergeSortedMatrix(rows) -> List:
+    """algo.MergeSorted(rows) over the rows of a uid matrix in ONE call (dgx_merge_sorted_matrix):
+    sg.DestUIDs = algo.MergeSorted(result.UidMatrix) (query/query.go:2290).
+
+    rows: ascending uid lists (pb.List values or arrays); duplicates inside and across rows are removed.  The rows
+    cross PCIe as one CSR copy, and the launch count does not depend on the number of rows."""
+    arrs = []
+    for r in rows:
+        u = r.Uids if isinstance(r, List) else r
+        arrs.append(np.zeros(0, np.uint64) if u is None else _u64(u))
+    nrows = len(arrs)
+    v_off = np.zeros(nrows + 1, dtype=np.uint64)
+    if nrows:
+        np.cumsum([a.size for a in arrs], out=v_off[1:])
+    m = int(v_off[-1])
+    v = np.concatenate(arrs) if m else np.zeros(1, np.uint64)
+    out = np.empty(max(m, 1), dtype=np.uint64)
+    n = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_merge_sorted_matrix(_p(v), _p(v_off), nrows, _p(out), m, C.byref(n)))
+    return List(out[: n.value])
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

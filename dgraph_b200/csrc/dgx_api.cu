@@ -31,6 +31,7 @@
 #include "merge_kernel.cuh"
 #include "merge_multi.cuh"
 #include "merge_tile32.cuh"
+#include "merge_matrix.cuh"
 #include "probe_kernel.cuh"
 #include "compressed_kernel.cuh"
 #include "encode_kernel.cuh"
@@ -70,6 +71,7 @@ struct Stats {
     std::atomic<uint64_t> calls{0}, uids_in{0}, uids_out{0}, h2d{0}, d2h{0}, launches{0};
 };
 static Stats g_stats;
+static std::atomic<uint64_t> g_xm_overflows{0};  // chunks of dgx_*merge_sorted_matrix sorted in global memory
 static std::mutex g_mu;
 static int g_device = -1;
 static std::vector<dgx_lane*> g_pool;  // idle lanes for the host-pointer entry points
@@ -195,6 +197,7 @@ struct dgx_lane {
     uint64_t* h_word = nullptr;  // pinned scratch for lengths (8 words)
     uint64_t* h_head = nullptr;  // pinned landing zone for the head of a result (kSpecHead values)
     uint64_t launches = 0;
+    uint64_t xm_overflows = 0;  // overflow-path chunks of the matrix merges this lane ran, as of its last sync
     // "resident lists" mode (dgx_lane_set_resident_inputs): the plan pre-pass of batch i+1 runs on a side stream while
     // the pipeline kernel of batch i is still running; its tables live in two alternating workspaces
     bool resident_inputs = false;
@@ -445,12 +448,17 @@ extern "C" uint64_t dgx_lane_launches(const dgx_lane* l) { return l ? l->launche
 extern "C" int dgx_lane_sync(dgx_lane* l) {
     if (!l) return fail(DGX_ERR_ARG, "null lane");
     CK(cudaSetDevice(l->device));
-    CK(cudaMemcpyAsync(l->h_err, l->d_err, sizeof(int), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(l->h_err, l->d_err, (kLaneOverflowWord + 1) * sizeof(u32), cudaMemcpyDeviceToHost, l->stream));
     CK(cudaStreamSynchronize(l->stream));
     l->host.reset();
     l->ws.release_retired();
     l->outs.clear();
     l->outs_overflow = false;
+    if (const u32 ovf = reinterpret_cast<const u32*>(l->h_err)[kLaneOverflowWord]) {
+        l->xm_overflows += ovf;
+        g_xm_overflows += ovf;
+        CK(cudaMemsetAsync(reinterpret_cast<u32*>(l->d_err) + kLaneOverflowWord, 0, sizeof(u32), l->stream));
+    }
     if (const int flag = *l->h_err) {
         *l->h_err = 0;
         CK(cudaMemsetAsync(l->d_err, 0, sizeof(int), l->stream));
@@ -2564,6 +2572,136 @@ extern "C" int dgx_intersect_compressed_matrix(const dgx_pack_ref* ref, const ui
     if (rc) return rc;
     return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
 }
+
+// ---------------------------------------------------------------------------
+// MergeSorted over the rows of a uid matrix (sg.DestUIDs = algo.MergeSorted(result.UidMatrix))
+// ---------------------------------------------------------------------------
+// Sample sort of merge_matrix.cuh: 7 launches plus ceil(log2 ntiles) levels of the sample tree, whatever nrows is.
+// Workspace: about 22 bytes per value of v_cap (tile runs 8, keys 4, bucketed values 8, samples, splitters and
+// bucket tables about 2.3), plus 24 per chunk of XM_H values.  v_off is read on the device only: no per-row host work.
+static int merge_matrix_impl(dgx_lane* l, const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows, uint64_t v_cap,
+                             uint64_t* d_out, size_t out_cap, uint64_t* d_out_len) {
+    if (nrows == 0 || v_cap == 0) {
+        CK(cudaMemsetAsync(d_out_len, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    const uint64_t ntiles = (v_cap + XM_T - 1) / XM_T, ns_cap = ntiles * XM_SPR, nk_cap = 2 * ns_cap + 1;
+    const uint64_t nchunks = (v_cap + XM_H - 1) / XM_H;
+    const uint64_t t_keys = (nk_cap + EN_TILE - 1) / EN_TILE, t_chunks = (nchunks + EN_TILE - 1) / EN_TILE;
+    // zeroed: [kcnt | kfill | scan status | tickets];  then runs, samples, soff, split, words, koff, bucketed, cstart,
+    // ccount, cpos, rlen (u32), key (u32)
+    const size_t b_zero = (2 * nk_cap + t_keys + t_chunks + 2) * sizeof(u64);
+    const size_t w_rest = ntiles * XM_T + ns_cap + 2 * ntiles + ns_cap + 4 + (nk_cap + 1) + v_cap + 3 * nchunks + 1;
+    const size_t b_u32 = ((ntiles + ntiles * XM_T) * sizeof(u32) + 15) & ~size_t(15);
+    void* d_raw;
+    int rc = l->ws.alloc(b_zero + w_rest * sizeof(u64) + b_u32, &d_raw);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(d_raw, 0, b_zero, l->stream));
+    XmParams P;
+    P.v = (const u64*)d_v;
+    P.v_off = (const u64*)d_v_off;
+    P.nrows = nrows;
+    P.v_cap = v_cap;
+    P.kcnt = (u64*)d_raw;
+    P.kfill = P.kcnt + nk_cap;
+    u64* status = P.kfill + nk_cap;
+    u32* tickets = (u32*)(status + t_keys + t_chunks);
+    P.runs = (u64*)((char*)d_raw + b_zero);
+    P.samples = P.runs + ntiles * XM_T;
+    P.soff = P.samples + ns_cap;
+    u64* split = P.soff + 2 * ntiles;
+    u64* words = split + ns_cap;  // nsplit, nkeys, nchunks
+    P.split = split;
+    P.nsplit = words;
+    P.nkeys = words + 1;
+    P.nch = words + 2;
+    P.koff = words + 4;
+    P.bucketed = P.koff + nk_cap + 1;
+    P.cstart = P.bucketed + v_cap;
+    P.ccount = P.cstart + nchunks;
+    P.cpos = P.ccount + nchunks;
+    P.rlen = (u32*)(P.cpos + nchunks + 1);
+    P.key = P.rlen + ntiles;
+    P.ntiles = (u32)ntiles;
+    P.nchunks = (u32)nchunks;
+    P.out = (u64*)d_out;
+    P.out_cap = out_cap;
+    P.err = l->d_err;
+    xm_tile_kernel<<<(unsigned)ntiles, XM_NT, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    l->launches += 1;
+    g_stats.launches += 1;
+    // the sample runs are sorted: the merge tree (with de-duplication) yields the distinct splitters
+    std::vector<MRef> sruns(ntiles);
+    std::vector<uint64_t> sub(ntiles, XM_SPR);
+    for (uint64_t t = 0; t < ntiles; ++t) sruns[t] = MRef{P.samples, P.soff + 2 * t, (u64)XM_SPR};
+    rc = merge_tree_impl(l, std::move(sruns), std::move(sub), ns_cap, (uint64_t*)split, ns_cap, (uint64_t*)words);
+    if (rc) return rc;
+    xm_count_kernel<<<(unsigned)ntiles, XM_NT, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)t_keys, EN_NT, 0, l->stream>>>(P.kcnt, P.koff, P.nkeys, nk_cap, status, tickets, nullptr);
+    CK(cudaGetLastError());
+    xm_scatter_kernel<<<(unsigned)ntiles, XM_NT, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    xm_chunk_kernel<<<(unsigned)nchunks, XM_CNT, 0, l->stream>>>(P, (u32*)l->d_err + kLaneOverflowWord);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)t_chunks, EN_NT, 0, l->stream>>>(P.ccount, P.cpos, P.nch, nchunks, status + t_keys,
+                                                                  tickets + 1, (u64*)d_out_len);
+    CK(cudaGetLastError());
+    xm_gather_kernel<<<(unsigned)nchunks, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    l->launches += 6;
+    g_stats.launches += 6;
+    return DGX_OK;
+}
+
+// Values are counted per 32-bit key and position: 2^32 values or more are refused before anything runs.
+constexpr uint64_t kMergeMatrixMax = (uint64_t(1) << 32) - 1;
+
+extern "C" int dgx_dev_merge_sorted_matrix(dgx_lane* l, const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows,
+                                           size_t v_cap, uint64_t* d_out, size_t out_cap, uint64_t* d_out_len) {
+    if (!l || !d_out_len || (nrows && !d_v_off) || (nrows && v_cap && !d_v)) return fail(DGX_ERR_ARG, "null argument");
+    if (v_cap > kMergeMatrixMax) return fail(DGX_ERR_ARG, "v_cap of %zu values: positions are 32-bit", v_cap);
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    const int rc = merge_matrix_impl(l, d_v, d_v_off, nrows, v_cap, d_out, out_cap, d_out_len);
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_len, sizeof(uint64_t));
+    return rc;
+}
+
+extern "C" int dgx_merge_sorted_matrix(const uint64_t* v, const uint64_t* v_off, size_t nrows, uint64_t* out,
+                                       size_t out_cap, size_t* out_len) {
+    if (nrows == 0) { if (out_len) *out_len = 0; return DGX_OK; }
+    if (!v_off) return fail(DGX_ERR_ARG, "null v_off");
+    if (v_off[0] != 0) return fail(DGX_ERR_ARG, "v_off[0] is %llu, not 0", (unsigned long long)v_off[0]);
+    for (size_t r = 0; r < nrows; ++r)
+        if (v_off[r + 1] < v_off[r]) return fail(DGX_ERR_ARG, "v_off decreases at row %zu", r);
+    const uint64_t m = v_off[nrows];
+    if (m > kMergeMatrixMax) return fail(DGX_ERR_ARG, "the matrix has %llu uids: positions are 32-bit", (unsigned long long)m);
+    if (m == 0) { if (out_len) *out_len = 0; return DGX_OK; }  // every row empty: nothing runs
+    if (!v || (out_cap && !out)) return fail(DGX_ERR_ARG, "null argument");
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += m;
+    uint64_t *d_v, *d_off;
+    int rc = upload_list(l, v, m, &d_v);  // one copy of the values, one of the offsets
+    if (rc) return rc;
+    rc = upload_list(l, v_off, nrows + 1, &d_off);
+    if (rc) return rc;
+    void *d_out, *d_len;
+    rc = l->ws.alloc((m + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc(64, &d_len);
+    if (rc) return rc;
+    rc = merge_matrix_impl(l, d_v, d_off, nrows, m, (uint64_t*)d_out, m, (uint64_t*)d_len);
+    if (rc) return rc;
+    return finish_to_host(l, (uint64_t*)d_len, (uint64_t*)d_out, m, out, out_cap, out_len);
+}
+
+extern "C" uint64_t dgx_merge_matrix_overflows(const dgx_lane* l) { return l ? l->xm_overflows : g_xm_overflows.load(); }
 
 // ---------------------------------------------------------------------------
 // protobuf wire-format adjacency (host only; see include/dgx.h and wire.hpp)

@@ -136,6 +136,43 @@ func MergeSorted(lists []*pb.List) *pb.List {
 	return &pb.List{Uids: out[:int(outLen)]}
 }
 
+// dgxMinMergeMatrix: below this many uids MergeSortedMatrix stays on the Go path.  Set from the C8 record
+// (profiles/h100_c8_merge_matrix.json, H100 80GB HBM3, 700 W): the host form took 1.1-1.4 ms for the C8a matrix
+// (6.49e5 uids in 10 000 rows) and the reference's 10-thread MergeSorted spent 78 ns per uid on it, so about 16 000
+// uids cost the Go merge what one library call costs.
+const dgxMinMergeMatrix = 1 << 14
+
+// MergeSortedMatrix is algo.MergeSorted(matrix) in ONE library call for the rows of a uid matrix:
+// sg.DestUIDs = algo.MergeSorted(result.UidMatrix) (query/query.go:2290, 2505; query/recurse.go:134;
+// worker/task.go:1629, 1706; worker/match.go:100).  The rows travel as one CSR allocation in C memory, written in one
+// pass; the library's launch count does not depend on the number of rows.  Rows must ascend (a uid matrix row does);
+// on any error, or when the call is too small to pay off, the result is mergeSortedGo's.
+func MergeSortedMatrix(matrix []*pb.List) *pb.List {
+	n, m := len(matrix), totalUids(matrix)
+	if m < dgxMinMergeMatrix || uint64(m) >= 1<<32 {
+		return mergeSortedGo(matrix)
+	}
+	// [v_off: n + 1 values | v: m values]
+	csr := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(n+1+m) * 8))
+	defer C.free(unsafe.Pointer(csr))
+	voff, o := csr[:n+1:n+1], 0
+	v := csr[n+1 : n+1+m : n+1+m]
+	for i, r := range matrix {
+		voff[i] = C.uint64_t(o)
+		if r != nil && len(r.Uids) > 0 {
+			C.memcpy(unsafe.Pointer(&v[o]), unsafe.Pointer(&r.Uids[0]), C.size_t(len(r.Uids)*8))
+			o += len(r.Uids)
+		}
+	}
+	voff[n] = C.uint64_t(o)
+	out := make([]uint64, m)
+	var outLen C.size_t
+	if rc := C.dgx_merge_sorted_matrix(&v[0], &voff[0], C.size_t(n), u64ptr(out), C.size_t(m), &outLen); rc != C.DGX_OK {
+		return mergeSortedGo(matrix)
+	}
+	return &pb.List{Uids: out[:int(outLen)]}
+}
+
 // Difference: algo/uidlist.go:332.  nil u or v -> non-nil empty list.
 func Difference(u, v *pb.List) *pb.List {
 	if u == nil || v == nil {

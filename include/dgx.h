@@ -223,6 +223,17 @@ int dgx_intersect_compressed_rows(const dgx_pack_ref* refs, size_t nrows, uint64
 int dgx_intersect_compressed_matrix(const dgx_pack_ref* ref, const uint64_t* v, const uint64_t* v_off, size_t nrows,
                                     uint64_t* out, uint64_t* out_off, size_t out_cap);
 
+/* algo.MergeSorted(rows) over the rows of a uid matrix, one call: sg.DestUIDs = algo.MergeSorted(result.UidMatrix)
+ * (query/query.go:2290, 2505; query/recurse.go:134; worker/task.go:1629, 1706; worker/match.go:100).
+ * Row i is v[v_off[i] .. v_off[i+1]) (host offsets, nrows + 1 values, v_off[0] == 0).  Rows ascend; duplicates
+ * inside a row and across rows are allowed and removed, as MergeSorted does (TestMergeSorted9 {1,1,1} -> {1}).
+ * out_cap >= the result length (v_off[nrows] always suffices), else DGX_ERR_CAP.  v_off[0] != 0, decreasing offsets
+ * and v_off[nrows] >= 2^32 are DGX_ERR_ARG before anything is copied; a row that descends is DGX_ERR_ARG and nothing is
+ * written to out.  nrows == 0 or all rows empty gives *out_len = 0 and needs no device.  v and v_off cross PCIe as one
+ * copy each; the number of kernel launches does not depend on nrows. */
+int dgx_merge_sorted_matrix(const uint64_t* v, const uint64_t* v_off, size_t nrows,
+                            uint64_t* out, size_t out_cap, size_t* out_len);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -374,6 +385,16 @@ int dgx_dev_intersect_compressed_rows(dgx_lane* lane, const dgx_dev_pack* const*
 int dgx_dev_intersect_compressed_matrix(dgx_lane* lane, const dgx_dev_pack* pk, const uint64_t* d_v,
                                         const uint64_t* v_off, size_t nrows,
                                         uint64_t* d_out, size_t out_cap, uint64_t* d_out_off);
+/* Device form of dgx_merge_sorted_matrix: d_v and d_v_off (nrows + 1 values) are DEVICE pointers, so the
+ * (d_out, d_out_off) of dgx_dev_intersect_compressed_rows / dgx_dev_filter_batch feed it directly.  v_cap >=
+ * d_v_off[nrows] sizes the workspace (v_cap >= 2^32 is DGX_ERR_ARG).  d_out_len: one device uint64, the result length.
+ * Asynchronous on the lane: past out_cap nothing is written and the next dgx_lane_sync returns DGX_ERR_CAP, as it does
+ * when d_v_off[nrows] > v_cap; a row that descends makes the next dgx_lane_sync return DGX_ERR_ARG. */
+int dgx_dev_merge_sorted_matrix(dgx_lane* lane, const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows,
+                                size_t v_cap, uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
+/* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
+ * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
+uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);
 
 #ifdef __cplusplus
 }

@@ -133,14 +133,17 @@ def main():
     ap.add_argument("--small", action="store_true", help="1/10 sizes (quick functional pass)")
     ap.add_argument("--c6-only", action="store_true", help="only the C6 handleUidPostings rows")
     ap.add_argument("--c7-only", action="store_true", help="only the C7 sort-bucket rows")
+    ap.add_argument("--c8-only", action="store_true", help="only the C8 DestUIDs (MergeSorted of a uid matrix) rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
     elif args.c7_only:
         rows = c7_rows(Lane())
+    elif args.c8_only:
+        rows = c8_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -390,6 +393,7 @@ def run(L, S, quick):
         L.lib.dgx_host_free(ptr)
     rows += c6_rows(L)
     rows += c7_rows(L)
+    rows += c8_rows(L)
     return rows
 
 
@@ -636,6 +640,109 @@ def c7_rows(L, threads: int = 4):
             out_rows.append(row(name, cfg, ms, uids.size + m, abytes, ok,
                                 dict(extra, rows_per_s=nrows / (ms * 1e-3), note=note)))
     lib.dgx_cache_clear()
+    return out_rows
+
+
+def c8_rows(L, reps: int = 10):
+    """C8 "DestUIDs": sg.DestUIDs = algo.MergeSorted(result.UidMatrix) (query/query.go:2290) over three uid matrices
+    (tests/gen_merge.py): C8a the C7 matrix, C8b the C6 rows, C8c 200 000 rows of 1-32 uids plus one hub uid in every
+    row.  Legs on the same inputs, every output compared with the oracle's in full: (1) dgx_dev_merge_sorted_matrix with
+    the matrix resident (CUDA events), (2) dgx_merge_sorted_matrix from pinned and (3) from pageable host memory (wall
+    clock incl. D2H), (4) dgx_dev_merge_sorted with one device pointer per row (CUDA events), (5) dgx_merge_sorted with
+    one host pointer per row (wall clock), (6) the oracle's MergeSorted with the reference's 10-thread split."""
+    import gen_merge
+    from oracle import pyoracle as orc
+
+    lib = L.lib
+
+    def wall(fn, n):
+        fn()
+        t0 = time.perf_counter()
+        for _ in range(n):
+            fn()
+        return (time.perf_counter() - t0) / n * 1e3
+
+    out_rows = []
+    for name, make in gen_merge.C8.items():
+        hv, v_off = make()
+        nrows, m = v_off.size - 1, hv.size
+        rows_u = gen_merge.rows_of(hv, v_off)
+        t0 = time.perf_counter()
+        want = orc.merge_sorted(rows_u)
+        t_orc = (time.perf_counter() - t0) * 1e3
+        t_orc = min(t_orc, wall(lambda: orc.merge_sorted(rows_u), 2))
+        nout = want.size
+        abytes = gen_merge.algorithmic_bytes(m, nout)
+        d_v = torch.from_numpy(hv.view(np.int64)).to(DEV)
+        d_off = torch.from_numpy(v_off.view(np.int64)).to(DEV)
+        d_out = torch.empty(m + 8, dtype=torch.int64, device=DEV)
+        d_len = torch.zeros(1, dtype=torch.int64, device=DEV)
+
+        def dev_got():
+            L.sync()
+            return d_out[: int(d_len.item())].cpu().numpy().view(np.uint64)
+
+        l0, o0 = lib.dgx_lane_launches(L.h), lib.dgx_merge_matrix_overflows(None)
+
+        def dev():
+            _lib.check(lib.dgx_dev_merge_sorted_matrix(L.h, C.c_void_p(d_v.data_ptr()), C.c_void_p(d_off.data_ptr()), nrows,
+                                                       m, C.c_void_p(d_out.data_ptr()), m, C.c_void_p(d_len.data_ptr())))
+        dev()
+        L.sync()
+        launches = lib.dgx_lane_launches(L.h) - l0
+        ms1, _ = timeit(dev, warm=3, reps=reps)
+        ok1 = bool(np.array_equal(dev_got(), want))
+        overflows = lib.dgx_merge_matrix_overflows(None) - o0
+        # today's device path: one device pointer per row
+        ptrs = (C.c_void_p * nrows)(*[d_v.data_ptr() + 8 * int(v_off[i]) for i in range(nrows)])
+        lens = (C.c_size_t * nrows)(*np.diff(v_off).tolist())
+
+        def dev_rows():
+            _lib.check(lib.dgx_dev_merge_sorted(L.h, ptrs, lens, nrows, C.c_void_p(d_out.data_ptr()), m,
+                                                C.c_void_p(d_len.data_ptr())))
+        ms4, _ = timeit(dev_rows, warm=2, reps=max(3, reps // 2))
+        ok4 = bool(np.array_equal(dev_got(), want))
+        hout = np.empty(max(m, 1), np.uint64)
+        n = C.c_size_t(0)
+        pin_v = lib.dgx_host_alloc(max(m, 1) * 8)
+        pin_off = lib.dgx_host_alloc((nrows + 1) * 8)
+        try:
+            pv = np.ctypeslib.as_array(C.cast(pin_v, C.POINTER(C.c_uint64)), (max(m, 1),))
+            po = np.ctypeslib.as_array(C.cast(pin_off, C.POINTER(C.c_uint64)), (nrows + 1,))
+            pv[:m], po[:] = hv, v_off
+            res = {}
+            for leg, (va, oa) in (("pinned", (pin_v, pin_off)), ("pageable", (hv.ctypes.data, v_off.ctypes.data))):
+                def host(va=va, oa=oa):
+                    _lib.check(lib.dgx_merge_sorted_matrix(C.c_void_p(va), C.c_void_p(oa), nrows,
+                                                           hout.ctypes.data_as(C.c_void_p), m, C.byref(n)))
+                res[leg] = wall(host, reps)
+                res[leg + "_ok"] = bool(np.array_equal(hout[: n.value], want))
+        finally:
+            lib.dgx_host_free(pin_v)
+            lib.dgx_host_free(pin_off)
+        hptrs = (C.c_void_p * nrows)(*[hv.ctypes.data + 8 * int(v_off[i]) for i in range(nrows)])
+
+        def host_rows():
+            _lib.check(lib.dgx_merge_sorted(hptrs, lens, nrows, hout.ctypes.data_as(C.c_void_p), m, C.byref(n)))
+        ms5 = wall(host_rows, max(2, reps // 2))
+        ok5 = bool(np.array_equal(hout[: n.value], want))
+        cfg = (f"C8 DestUIDs {name}: MergeSorted of a uid matrix of {nrows} rows, {m} UIDs -> {nout} distinct "
+               f"({gen_merge.C8[name].__doc__.split(chr(10))[0]})")
+        extra = {"matrix": name, "rows": nrows, "matrix_uids": m, "out": nout}
+        for op, ms, ok, note in (
+            ("MergeSortedMatrix (device, resident matrix)", ms1, ok1,
+             f"dgx_dev_merge_sorted_matrix, CUDA events; {launches} launches per call, {overflows} overflow-path chunks"),
+            ("MergeSortedMatrix (host, pinned)", res["pinned"], res["pinned_ok"],
+             "dgx_merge_sorted_matrix from pinned memory, wall clock incl. H2D and D2H"),
+            ("MergeSortedMatrix (host, pageable)", res["pageable"], res["pageable_ok"],
+             "dgx_merge_sorted_matrix from pageable memory, wall clock incl. H2D and D2H"),
+            ("MergeSorted, one device pointer per row", ms4, ok4, "dgx_dev_merge_sorted, CUDA events"),
+            ("MergeSorted, one host pointer per row", ms5, ok5, "dgx_merge_sorted, wall clock incl. H2D and D2H"),
+            ("oracle MergeSorted (10-thread split)", t_orc, True, "algo.MergeSorted restated in C, wall clock"),
+        ):
+            out_rows.append(row(op, cfg, ms, m, abytes, ok, dict(extra, note=note, launches_per_call=launches,
+                                                                 overflow_chunks=overflows)))
+        del d_v, d_off, d_out
     return out_rows
 
 
