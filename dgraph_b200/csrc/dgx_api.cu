@@ -82,15 +82,8 @@ static u32 g_stream_ratio = 16;
 static u32 g_scap_override = 0;       // DGX_SCAP: force the filter kernel's slice staging capacity
 constexpr u32 kScapMin = 8192, kScapMax = 65536;  // bytes
 static int g_filter_pipe = 1;          // DGX_FILTER=v4 selects the non-persistent kernel
-static int g_merge_multi = 1;          // DGX_MERGE=tree forces the pairwise merge tree
-static int g_merge_lag = 0;            // DGX_MERGE_LAG: a merge CTA moves the tile this many tiles back to the output; 0 = scan + compact kernels
-                                       // (default: the copy phase is not hidden under the merging, so the separate kernels are no slower)
-static int g_merge_ahead = -1;         // DGX_MERGE_AHEAD: L2 prefetch distance in tiles (-1 = 3 x SM count, the resident CTAs; 0 = off)
-static int g_merge_t32 = 1;            // DGX_MERGE=levels: the round-1 pipeline (64-bit levels engine, boundary-major bounds)
-static u32 g_merge_stride = 0;         // DGX_MERGE_STRIDE: sample gaps per multiway-merge tile (tile ~ 512 x stride values); 0 = 10 for the
-                                       // 32-bit engine (7680-slot rounds), 6 for DGX_MERGE=levels (4096-slot rounds)
 static int g_zero_copy = 0;            // DGX_ZERO_COPY=1: decode pinned packs in place over PCIe (off: DMA copies move the bytes faster)
-static size_t g_merge_multi_min = size_t(1) << 18;  // totals below this stay on the tree (fewer launches)
+constexpr size_t g_merge_multi_min = size_t(1) << 18;  // MergeSorted totals below this stay on the tree (fewer launches)
 static size_t g_pre_throttle_smem = 0;  // DGX_PRE_THROTTLE: dynamic smem asked for by an ahead-of-time pre-pass (0 = unthrottled)
 static u32 g_reserve_ctas = 0;         // DGX_RESERVE_CTAS: pipeline CTAs left out of the persistent grid
 static uint64_t g_pipe_min_values = 0;  // DGX_PIPE_MIN_VALUES: batches driving fewer values than this use filter_kernel
@@ -274,16 +267,11 @@ extern "C" int dgx_init(int device) {
                             (int)(2 * F_TA * sizeof(u64) + kScapMax)));
     CK(cudaFuncSetAttribute(filter_pipe_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmemMax));
     CK(cudaFuncSetAttribute(filter_pipe_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmemMax));
-    CK(cudaFuncSetAttribute(mmerge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * MM_CP * sizeof(u64))));
     g_num_sms = prop.multiProcessorCount;
     numa_probe(device);
     if (const char* s = getenv("DGX_FILTER")) g_filter_pipe = (strcmp(s, "v4") != 0);
     CK(cudaFuncSetAttribute(mmerge3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T_SMEM));
-    if (const char* s = getenv("DGX_MERGE")) { g_merge_multi = (strcmp(s, "tree") != 0); g_merge_t32 = (strcmp(s, "levels") != 0); }
     if (const char* s = getenv("DGX_ZERO_COPY")) g_zero_copy = atoi(s) != 0;
-    if (const char* s = getenv("DGX_MERGE_AHEAD")) g_merge_ahead = atoi(s);
-    if (const char* s = getenv("DGX_MERGE_LAG")) g_merge_lag = atoi(s);
-    if (const char* s = getenv("DGX_MERGE_STRIDE")) { const int v = atoi(s); if (v >= 1 && v <= 16) g_merge_stride = (u32)v; }
     g_device = device;
     return DGX_OK;
 }
@@ -738,11 +726,11 @@ static int merge_sorted_impl(dgx_lane* l, const ListDesc* lists, size_t k, uint6
 static int merge_runs_impl(dgx_lane* l, const std::vector<MRef>& cur, const std::vector<uint64_t>& ub, uint64_t total,
                            uint64_t* d_out, size_t out_cap, uint64_t* d_out_len) {
     const size_t k = cur.size();
-    if (g_merge_multi && k >= 3 && k <= (size_t)MM_K && total >= g_merge_multi_min)
+    if (k >= 3 && k <= (size_t)MM_K && total >= g_merge_multi_min)
         return merge_multi_impl(l, cur, ub, total, d_out, out_cap, d_out_len);
     const size_t ngroups = (k + MM_K - 1) / MM_K;
     // a multiway call is a dozen launches: grouping pays only when every group is a few times the multiway minimum
-    if (!g_merge_multi || k <= (size_t)MM_K || total / ngroups < 4 * g_merge_multi_min)
+    if (k <= (size_t)MM_K || total / ngroups < 4 * g_merge_multi_min)
         return merge_tree_impl(l, cur, ub, total, d_out, out_cap, d_out_len);
     const size_t gsz = (k + ngroups - 1) / ngroups;
     void *d_tmp, *d_pairs;
@@ -868,14 +856,12 @@ static int merge_tree_impl(dgx_lane* l, std::vector<MRef> cur, std::vector<uint6
     return DGX_OK;
 }
 
-// Single-pass multiway merge (merge_multi.cuh) for 3..64 runs.
+// Single-pass multiway merge (merge_multi.cuh) for 3..64 runs: msample -> merge tree over the samples -> mplan2 ->
+// mmerge3 -> mscan -> mcompact.
 static int merge_multi_impl(dgx_lane* l, const std::vector<MRef>& runs, const std::vector<uint64_t>& ub, uint64_t total,
                             uint64_t* d_out, size_t out_cap, uint64_t* d_out_len) {
     const size_t k = runs.size();
-    // Samples per run proportional to its length.  Every 4th distinct sample becomes a splitter, so a
-    // tile is the sum of 4 sample gaps (~2K values on average, Gamma-distributed instead of
-    // exponential) and rarely overflows the 4096-value shared-memory chunk.
-    const u32 stride = g_merge_stride ? (g_merge_t32 ? g_merge_stride : std::min<u32>(g_merge_stride, 7)) : (g_merge_t32 ? 10u : 6u);
+    // about one sample per 512 values, shared among the runs in proportion to their lengths
     const uint64_t ntarget = std::min<uint64_t>(std::max<uint64_t>(total / 512, 1), uint64_t(1) << 24);
     std::vector<u32> soff(k + 1, 0);
     for (size_t j = 0; j < k; ++j) soff[j + 1] = soff[j] + (u32)((unsigned __int128)ub[j] * ntarget / total);
@@ -894,8 +880,7 @@ static int merge_multi_impl(dgx_lane* l, const std::vector<MRef>& runs, const st
     const size_t a_tout = a_tin + (size_t)(nsamp + 2) * 8;
     const size_t a_tcnt = a_tout + (size_t)(nsamp + 3) * 8;
     const size_t a_tlo = ((a_tcnt + (size_t)(nsamp + 2) * 4 + 255) & ~size_t(255));
-    const size_t a_status = a_tlo + (size_t)(nsamp + 2) * 8;
-    const size_t a_end = a_status + (size_t)(nsamp + 3) * 8 + 256;  // look-back words + ticket (merge_tile32.cuh, DGX_MERGE_LAG)
+    const size_t a_end = a_tlo + (size_t)(nsamp + 2) * 8;
     rc = l->ws.alloc(a_end, &d_raw);
     if (rc) return rc;
     void* d_scratch;
@@ -908,26 +893,22 @@ static int merge_multi_impl(dgx_lane* l, const std::vector<MRef>& runs, const st
     P.k = (u32)k;
     P.samp_off = (const u32*)(d + runs_b);
     P.nsamp = nsamp;
-    P.stride = stride;
     P.samples = (u64*)(d + a_samples);
     P.splitters = (u64*)(d + a_split);
     P.nsplit = (const u64*)(d + a_nsplit);
+    const u32 max_tiles = nsamp / MM_STRIDE + 1;
     P.bounds = (u64*)(d + a_bounds);
+    P.nbs = max_tiles + 1;
     P.tile_in = (u64*)(d + a_tin);
-    P.tile_out = (u64*)(d + a_tout);
     P.tile_cnt = (u32*)(d + a_tcnt);
+    P.tile_out = (u64*)(d + a_tout);
+    P.tile_lo = (u64*)(d + a_tlo);
     P.scratch = (u64*)d_scratch;
     P.out = (u64*)d_out;
     P.out_cap = out_cap;
     P.out_len = (u64*)d_out_len;
     P.err = l->d_err;
-    const u32 max_tiles = nsamp / stride + 1;
-    P.nbs = max_tiles + 1;
-    P.tile_lo = (u64*)(d + a_tlo);
-    P.lag = !g_merge_t32 || g_merge_lag < 0 ? 0u : (u32)g_merge_lag;
-    P.ahead = g_merge_ahead < 0 ? 3u * (u32)g_num_sms : (u32)g_merge_ahead;
-    P.status = (u64*)(d + a_status);
-    P.ticket = (u32*)(d + a_status + (size_t)(nsamp + 3) * 8);
+    P.ahead = 3u * (u32)g_num_sms;  // the tile the same SM slot most likely runs next: 3 resident CTAs per SM
     if (nsamp) {
         msample_kernel<<<(nsamp + 255) / 256, 256, 0, l->stream>>>(P);
         CK(cudaGetLastError());
@@ -947,31 +928,10 @@ static int merge_multi_impl(dgx_lane* l, const std::vector<MRef>& runs, const st
     } else {
         CK(cudaMemsetAsync(d + a_nsplit, 0, 8, l->stream));
     }
-    const uint64_t nb = (uint64_t)(max_tiles + 1) * k;
-    if (g_merge_t32) {
-        mplan2_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, l->stream>>>(P);
-        CK(cudaGetLastError());
-        if (P.lag) CK(cudaMemsetAsync(d + a_status, 0, (size_t)(nsamp + 3) * 8 + 256, l->stream));
-        mmerge3_kernel<<<max_tiles, T_NT, T_SMEM, l->stream>>>(P);
-        CK(cudaGetLastError());
-        if (P.lag) {
-            mtail_kernel<<<std::min<u32>(P.lag, max_tiles), T_NT, 0, l->stream>>>(P);
-            CK(cudaGetLastError());
-            l->launches += 3;
-            g_stats.launches += 3;
-            return DGX_OK;
-        }
-        mscan_kernel<<<1, 1024, 0, l->stream>>>(P);
-        CK(cudaGetLastError());
-        mcompact_kernel<<<max_tiles, 256, 0, l->stream>>>(P);
-        CK(cudaGetLastError());
-        l->launches += 4;
-        g_stats.launches += 4;
-        return DGX_OK;
-    }
-    mplan_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, l->stream>>>(P);
+    const uint64_t nb = (uint64_t)P.nbs * k;
+    mplan2_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, l->stream>>>(P);
     CK(cudaGetLastError());
-    mmerge_kernel<<<max_tiles, MM_NT, 2 * MM_CP * sizeof(u64), l->stream>>>(P);
+    mmerge3_kernel<<<max_tiles, T_NT, T_SMEM, l->stream>>>(P);
     CK(cudaGetLastError());
     mscan_kernel<<<1, 1024, 0, l->stream>>>(P);
     CK(cudaGetLastError());

@@ -7,19 +7,21 @@
 //   msample_kernel   evenly spaced samples of every run (count proportional to its length)
 //   (merge tree)     the k sample runs are themselves sorted, so the existing pairwise
 //                    merge tree (merge_kernel, with de-duplication) turns them into the
-//                    sorted distinct splitters; splitters b-1 .. b bound tile b.
-//   mplan_kernel     one thread per (boundary, run): lower_bound of the splitter in the run
-//   mmerge_kernel    one CTA per tile: the k slices of the tile's value range are merged in
-//                    shared memory by log2(k) rounds of pairwise merge-path merges, values
-//                    equal to their predecessor are dropped, the result goes to a scratch
-//                    buffer at the tile's INPUT offset (output <= input, so regions never
-//                    overlap) and the tile's count is recorded.  A tile larger than the
-//                    shared-memory chunk is processed in rounds: every run contributes a
-//                    quota, only values <= the smallest "last loaded value of a run that has
-//                    more" are final in that round (classic block-wise k-way merge), so no
-//                    distribution of the input can overflow shared memory.
+//                    sorted distinct splitters; every MM_STRIDE-th one is a tile boundary.
+//   mplan2_kernel    (merge_tile32.cuh) position of every boundary in every run
+//   mmerge3_kernel   (merge_tile32.cuh) one CTA per tile: the k slices of the tile's value
+//                    range are merged in shared memory, values equal to their predecessor
+//                    are dropped, the result goes to a scratch buffer at the tile's INPUT
+//                    offset (output <= input, so regions never overlap) and the tile's count
+//                    is recorded.  A tile larger than the shared-memory chunk is processed in
+//                    rounds: every run contributes a quota, only values <= the smallest "last
+//                    loaded value of a run that has more" are final in that round (classic
+//                    block-wise k-way merge), so no distribution of the input can overflow
+//                    shared memory.
 //   mscan_kernel     exclusive scan of the tile counts (one CTA)
 //   mcompact_kernel  moves every tile's output to its final, compact position.
+// This file holds the sampling, the scan and the compaction, and the 64-bit merge engine
+// (mm_levels_tile) that mmerge3_kernel runs for tiles whose value span does not fit 32 bits.
 #pragma once
 
 #include "common.cuh"
@@ -37,6 +39,10 @@ constexpr int MM_VT = MM_C / MM_NT;
 // 64-bit accesses.
 __device__ __forceinline__ int mm_pad(int i) { return i + (i >> 4); }
 constexpr int MM_CP = MM_C + MM_C / 16 + 2;  // padded buffer length
+// Every MM_STRIDE-th distinct sample is a splitter: a tile is the sum of MM_STRIDE sample gaps (~5 K values on average,
+// Gamma-distributed instead of exponential), so most tiles fit one round of the 32-bit engine (7680 slots).
+constexpr u32 MM_STRIDE = 10;
+constexpr u32 kTileWide = 0x80000000u;  // tile_cnt flag: the tile's scratch holds u64 values, not u32 offsets from tile_lo
 
 struct MMParams {
     const MRef* runs;       // k run references (plain arrays or CSR slices of a previous level)
@@ -46,23 +52,18 @@ struct MMParams {
     u64* samples;           // nsamp
     u64* splitters;         // <= nsamp
     const u64* nsplit;      // device word: number of distinct sample values
-    u32 stride;             // every stride-th distinct sample is a splitter (evens out tile sizes)
-    u64* bounds;            // (nsamp + 2) * k: boundary b, run j -> position in run j
+    u64* bounds;            // k * nbs, run-major: bounds[j * nbs + b] = position of boundary b in run j
+    u32 nbs;                // boundaries per run
     u64* tile_in;           // nsamp + 1: input offset of every tile (= scratch offset)
-    u32* tile_cnt;          // nsamp + 1: values the tile produced
+    u32* tile_cnt;          // nsamp + 1: values the tile produced, | kTileWide
     u64* tile_out;          // nsamp + 2: exclusive scan of tile_cnt
+    u64* tile_lo;           // nsamp + 2: base of a tile's 32-bit scratch keys
     u64* scratch;           // sum of run lengths
     u64* out;
     u64 out_cap;
     u64* out_len;
     int* err;
-    // merge_tile32.cuh
-    u32 nbs;                // boundaries per run in the run-major bounds table (bounds[j * nbs + b])
-    u64* status;            // look-back words, one per tile, zeroed
-    u32* ticket;            // zeroed
-    u32 ahead;              // merge_tile32.cuh: prefetch the tile this many tiles on into L2 (0 = off)
-    u32 lag;                // merge_tile32.cuh: a CTA moves the tile `lag` tiles before its own to the output (0 = scan + compact kernels)
-    u64* tile_lo;           // nsamp + 2: base of a tile's 32-bit scratch keys
+    u32 ahead;              // mmerge3_kernel prefetches the tile this many tiles on into L2
 };
 
 // ---- samples ---------------------------------------------------------------------------
@@ -81,22 +82,6 @@ __global__ void __launch_bounds__(256) msample_kernel(const MMParams P) {
     u64 v = kU64Max;  // an empty (fully de-duplicated) run contributes "+inf" samples
     if (n > 0) v = ld_probe(p + (u64)(((unsigned __int128)(r + 1) * n) / (s + 1)));
     P.samples[i] = v;
-}
-
-// ---- boundaries: position of every splitter in every run ----------------------------------
-__global__ void __launch_bounds__(256) mplan_kernel(const MMParams P) {
-    const u32 ns = (u32)(*P.nsplit / P.stride);
-    const u64 idx = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    const u64 nb = (u64)ns + 2;  // boundaries 0 .. ns+1
-    if (idx >= nb * P.k) return;
-    const u32 b = (u32)(idx / P.k), j = (u32)(idx % P.k);
-    const u64* p; u64 n;
-    mref_resolve(P.runs[j], p, n);
-    u64 pos;
-    if (b == 0) pos = 0;
-    else if (b == ns + 1) pos = n;
-    else pos = lower_bound_g(p, n, P.splitters[(u64)b * P.stride - 1]);
-    P.bounds[idx] = pos;
 }
 
 // ---- the merge -----------------------------------------------------------------------------
@@ -138,11 +123,11 @@ __device__ __forceinline__ void mm_merge_level(const u64* src, u64* dst, const i
 #undef MM_B
 }
 
-// The levels engine for ONE tile: the slices [s_cur[r], s_end[r]) of the k runs s_ptr[r] are merged in rounds of at
+// The 64-bit engine for ONE tile: the slices [s_cur[r], s_end[r]) of the k runs s_ptr[r] are merged in rounds of at
 // most MM_C values (two ping-pong buffers of MM_CP values in s_mm), values equal to their predecessor are dropped and
 // the rest is appended to dst.  Called by all MM_NT threads of the CTA; returns the number of values written.
 __device__ __noinline__ u32 mm_levels_tile(u64* s_mm, const u64* const* s_ptr, u64* s_cur, const u64* s_end, int k,
-                                           u64* dst, bool have_last, u64 last) {
+                                           u64* dst) {
     u64* s_x = s_mm;
     u64* s_y = s_mm + MM_CP;
     __shared__ int s_off[2][MM_K + 2];
@@ -152,6 +137,10 @@ __device__ __noinline__ u32 mm_levels_tile(u64* s_mm, const u64* const* s_ptr, u
     __shared__ u32 s_scan[MM_NT / 32 + 1];
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     u32 produced = 0;
+    // A value equal to a round's bound can have more copies waiting in runs that had loaded only part of them, so the
+    // last value written is remembered across rounds.
+    bool have_last = false;
+    u64 last = 0;
 
     for (;;) {
         // ---- how much of every run enters this round -------------------------------------------
@@ -302,63 +291,14 @@ __device__ __noinline__ u32 mm_levels_tile(u64* s_mm, const u64* const* s_ptr, u
     return produced;
 }
 
-__global__ void __launch_bounds__(MM_NT, 3) mmerge_kernel(const MMParams P) {
-    extern __shared__ __align__(16) u64 s_mm[];  // two ping-pong buffers of MM_C values
-    __shared__ u64 s_cur[MM_K], s_end[MM_K];
-    __shared__ const u64* s_ptr[MM_K];
-    __shared__ u64 s_red[8];
-
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const u32 b = blockIdx.x;
-    const u32 ns = (u32)(*P.nsplit / P.stride);
-    if (b > ns) return;
-    const int k = (int)P.k;
-
-    // ---- the tile's slice of every run, its input offset and its predecessor value ------------
-    u64 my_c = 0;
-    u64 my_pred = 0;
-    bool my_has = false;
-    if (tid < k) {
-        const u64* p; u64 n;
-        mref_resolve(P.runs[tid], p, n);
-        const u64 c = P.bounds[(u64)b * k + tid], e = P.bounds[(u64)(b + 1) * k + tid];
-        s_ptr[tid] = p; s_cur[tid] = c; s_end[tid] = e;
-        my_c = c;
-        if (c > 0) { my_pred = ld_probe(p + c - 1); my_has = true; }
-    }
-    // block reductions over the first 64 threads (two warps): sum of starts, max predecessor
-    {
-        u64 sum = my_c, mx = my_has ? my_pred : 0;
-        u32 any = my_has ? 1u : 0u;
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) {
-            sum += __shfl_xor_sync(0xffffffffu, sum, d);
-            const u64 o = __shfl_xor_sync(0xffffffffu, mx, d);
-            mx = o > mx ? o : mx;
-            any |= __shfl_xor_sync(0xffffffffu, any, d);
-        }
-        if (lane == 0 && wid < 2) { s_red[wid] = sum; s_red[2 + wid] = mx; s_red[4 + wid] = any; }
-    }
-    __syncthreads();
-    const u64 inbase = s_red[0] + s_red[1];
-    const bool have_last = (s_red[4] | s_red[5]) != 0;
-    const u64 last = s_red[2] > s_red[3] ? s_red[2] : s_red[3];
-    __syncthreads();
-    const u32 produced = mm_levels_tile(s_mm, s_ptr, s_cur, s_end, k, P.scratch + inbase, have_last, last);
-    if (tid == 0) {
-        P.tile_in[b] = inbase;
-        P.tile_cnt[b] = produced | 0x80000000u;  // scratch holds u64 values (mcompact_kernel)
-    }
-}
-
 // ---- scan of the tile counts (one CTA) --------------------------------------------------------
 __global__ void __launch_bounds__(1024) mscan_kernel(const MMParams P) {
     __shared__ u32 s_warp[1024 / 32 + 1];
-    const u32 ntiles = (u32)(*P.nsplit / P.stride) + 1;
+    const u32 ntiles = (u32)(*P.nsplit / MM_STRIDE) + 1;
     u64 base = 0;
     for (u32 start = 0; start < ntiles; start += 1024) {
         const u32 i = start + threadIdx.x;
-        const u32 v = i < ntiles ? (P.tile_cnt[i] & 0x7fffffffu) : 0u;
+        const u32 v = i < ntiles ? (P.tile_cnt[i] & ~kTileWide) : 0u;
         u32 total;
         const u32 off = block_exclusive_scan<1024>(v, s_warp, &total);
         if (i < ntiles) P.tile_out[i] = base + off;
@@ -374,14 +314,14 @@ __global__ void __launch_bounds__(1024) mscan_kernel(const MMParams P) {
 
 // ---- compaction: scratch (tile-local offsets) -> out (final offsets) ------------------------------
 __global__ void __launch_bounds__(256) mcompact_kernel(const MMParams P) {
-    const u32 ntiles = (u32)(*P.nsplit / P.stride) + 1;
+    const u32 ntiles = (u32)(*P.nsplit / MM_STRIDE) + 1;
     const u32 b = blockIdx.x;
     if (b >= ntiles) return;
     const u64 o = P.tile_out[b];
-    const u32 cnt = P.tile_cnt[b] & 0x7fffffffu;
+    const u32 cnt = P.tile_cnt[b] & ~kTileWide;
     if (o + cnt > P.out_cap) return;  // error already flagged by mscan_kernel
     u64* dst = P.out + o;
-    if (P.tile_cnt[b] & 0x80000000u) {  // u64 values
+    if (P.tile_cnt[b] & kTileWide) {  // u64 values
         const u64* src = P.scratch + P.tile_in[b];
         for (u32 i = threadIdx.x; i < cnt; i += 256) st_stream(dst + i, ld_stream(src + i));
     } else {                            // 32-bit offsets from tile_lo (merge_tile32.cuh)

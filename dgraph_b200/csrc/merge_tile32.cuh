@@ -1,7 +1,5 @@
-// merge_tile32.cuh -- the tile engine of the single-pass multiway MergeSorted, second version.
+// merge_tile32.cuh -- bounds and tile merge of the single-pass multiway MergeSorted (pipeline: merge_multi.cuh).
 //
-// Same decomposition as merge_multi.cuh (samples -> distinct splitters -> per-(boundary, run) bounds -> one CTA per
-// tile -> scan of the tile counts -> compaction), with two changes:
 //   mplan2_kernel   bounds, run-major (threads of a warp search neighbouring splitters in the SAME run, so their
 //                   probes share sectors), each search confined to the gap between two samples of the run (the
 //                   samples are already in HBM/L2: 9 steps instead of 24).
@@ -10,11 +8,13 @@
 //                   run on u32 keys: one-instruction compares and selects, half the shared-memory bytes (so a
 //                   round holds 7680 slots instead of 4096), T_VT = 15 consecutive slots per thread -- an odd stride,
 //                   so the threads of a warp hit different banks without index padding.  About a third of the
-//                   instructions of the 64-bit levels per slot.  Tiles whose span does not fit 32 bits use the 64-bit
+//                   instructions of the 64-bit engine per slot.  Tiles whose span does not fit 32 bits use the 64-bit
 //                   engine of merge_multi.cuh (mm_levels_tile) in the same kernel.
 // An LSD radix sort of the tile (8-bit digits, match.any ranking) and a decoupled look-back straight to the final
 // position were built first: ~3 warp-instructions per value and pass for the sort, and in-order retirement behind
-// the slowest tile for the look-back; both slower than this.
+// the slowest tile for the look-back; both slower than this.  Moving a finished tile to the output from inside the
+// merge kernel, a fixed number of tiles later, was no faster than the scan and compaction kernels either: the merge
+// kernel is bound by its phases' latencies, not by issue slots, so such a copy phase costs what the compaction costs.
 // algo.MergeSorted: algo/uidlist.go:448-542.
 #pragma once
 
@@ -29,17 +29,15 @@ constexpr u32 T_INF = 0xFFFFFFFFu;          // padding key; real keys are < T_IN
 constexpr size_t T_SMEM_32 = (size_t)2 * T_C * sizeof(u32);
 constexpr size_t T_SMEM_64 = (size_t)2 * MM_CP * sizeof(u64);
 constexpr size_t T_SMEM = T_SMEM_32 > T_SMEM_64 ? T_SMEM_32 : T_SMEM_64;
-#ifndef DGX_T_PIECE
-#define DGX_T_PIECE 128  // slots per load piece (256-slot pieces balance the runs less evenly)
-#endif
-constexpr int T_PIECE = DGX_T_PIECE;         // slots per load piece (T_PIECE / 32 independent loads per lane)
+// slots per load piece (T_PIECE / 32 independent loads per lane; 256-slot pieces balance the runs less evenly)
+constexpr int T_PIECE = 128;
 constexpr int T_NCH = T_VT * (T_NT / 32);   // 32-position chunks of a round (de-duplication scan)
 static_assert(T_NCH <= 256, "chunk scan handles 8 chunks per lane");
 static_assert(MM_K == 64, "six merge levels");
 
 // ---- bounds, run-major: bounds[j * nbs + b] = position of boundary b in run j ---------------------------------
 __global__ void __launch_bounds__(256) mplan2_kernel(const MMParams P) {
-    const u32 ns = (u32)(*P.nsplit / P.stride);
+    const u32 ns = (u32)(*P.nsplit / MM_STRIDE);
     const u64 idx = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     const u32 j = (u32)(idx / P.nbs), b = (u32)(idx % P.nbs);
     if (j >= P.k || b > ns + 1) return;
@@ -49,7 +47,7 @@ __global__ void __launch_bounds__(256) mplan2_kernel(const MMParams P) {
     if (b == 0 || n == 0) pos = 0;
     else if (b == ns + 1) pos = n;
     else {
-        const u64 S = P.splitters[(u64)b * P.stride - 1];
+        const u64 S = P.splitters[(u64)b * MM_STRIDE - 1];
         // the samples of run j sit at positions q(r) = (r + 1) * n / (s + 1) (msample_kernel): the samples below S
         // and the first one not below S fence the answer in
         const u64* sm = P.samples + P.samp_off[j];
@@ -347,82 +345,17 @@ __device__ __noinline__ u32 t32_tile(u32* s_k, const u64* const* s_ptr, u64* s_c
     return produced;
 }
 
-// ---- lagged compaction (optional: DGX_MERGE_LAG > 0; default is mscan_kernel + mcompact_kernel) --------------------
-// A tile's place in the output is the sum of the counts of the tiles before it, known only when they are all done.
-// Waiting for it at the end of a tile retires the CTAs in order (much of the kernel's time is then spent waiting behind
-// the slowest tile).  Here a tile writes its keys to scratch, publishes its count, and the CTA that starts P.lag tiles
-// LATER -- when the tile and its predecessors have long finished -- resolves the offset with a decoupled look-back that
-// finds everything already published, and moves the values to their final position before it begins its own tile;
-// mtail_kernel moves the last P.lag tiles.  Bit-exact, no waiting at lag >= 6 x SMs, but no faster than the
-// two extra kernels: the merge kernel is bound by its phases' latencies, not by issue slots, so
-// the copy phase costs what the compaction kernel costs.
-constexpr u32 kTileWide = 0x80000000u;  // tile_cnt flag: the tile's scratch holds u64 values, not u32 offsets from tile_lo
-
-__device__ __forceinline__ u64 t32_ldcg64(const u64* p) {
-    u64 v;
-    asm volatile("ld.global.cg.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ u32 t32_ldcg32(const u32* p) {
-    u32 v;
-    asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-
-// One warp: output offset of tile t (its count must be, or is about to be, published in P.status[t]).
-// Returns the exclusive prefix; *agg gets the tile's count.
-__device__ __forceinline__ u64 t32_tile_offset(const MMParams& P, u32 t, int lane, u64* agg) {
-    u64 w = 0;
-    if (lane == 0) {
-        while (((w = ld_relaxed(P.status + t)) >> 62) == 0) __nanosleep(200);
-    }
-    w = __shfl_sync(0xffffffffu, w, 0);
-    *agg = w & kValMask;
-    const u64 base = lookback_exclusive<true, 100>(P.status, t, *agg, lane);
-    __threadfence();  // what the tile wrote before publishing its count is visible to the loads that follow
-    return base;
-}
-
-// All threads of the CTA: move tile t's values from scratch to out[base ..).
-template <int NT>
-__device__ __forceinline__ void t32_copy_tile(const MMParams& P, u32 t, u64 base, int tid) {
-    const u64 inb = t32_ldcg64(P.tile_in + t);
-    const u64 lo = t32_ldcg64(P.tile_lo + t);
-    const u32 c = t32_ldcg32(P.tile_cnt + t);
-    const u32 cnt = c & ~kTileWide;
-    if (c & kTileWide) {
-        const u64* src = P.scratch + inb;
-        for (u32 i = tid; i < cnt; i += NT)
-            if (base + i < P.out_cap) st_stream(P.out + base + i, t32_ldcg64(src + i));
-    } else {
-        const u32* src = (const u32*)(P.scratch + inb);
-        for (u32 i = tid; i < cnt; i += NT)
-            if (base + i < P.out_cap) st_stream(P.out + base + i, lo + t32_ldcg32(src + i));
-    }
-}
-
 __global__ void __launch_bounds__(T_NT, 3) mmerge3_kernel(const MMParams P) {
     extern __shared__ __align__(16) unsigned char s_raw[];
     __shared__ u64 s_cur[MM_K], s_end[MM_K];
     __shared__ const u64* s_ptr[MM_K];
     __shared__ u64 s_r[2][4];
-    __shared__ u64 s_cbase;
-    __shared__ u32 s_tile;
 
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    // tiles are numbered in the order their CTAs start, so every tile before a running one has started (look-back)
-    if (tid == 0) s_tile = P.lag ? atomicAdd(P.ticket, 1u) : blockIdx.x;
-    __syncthreads();
-    const u32 b = s_tile;
-    const u32 ns = (u32)(*P.nsplit / P.stride);
+    const u32 b = blockIdx.x;
+    const u32 ns = (u32)(*P.nsplit / MM_STRIDE);
     if (b > ns) return;
     const int k = (int)P.k;
-    const bool docopy = P.lag != 0 && b >= P.lag;
-    if (docopy && wid == 2) {  // warps 0 and 1 read the tile's bounds meanwhile
-        u64 agg;
-        const u64 base = t32_tile_offset(P, b - P.lag, lane, &agg);
-        if (lane == 0) s_cbase = base;
-    }
 
     // ---- the tile's slice of every run; input offset, size, smallest and largest value ---------------------
     // An interior tile holds the values in [S(b), S(b+1)) (S(b) = splitter of boundary b), which bounds its span without
@@ -431,8 +364,8 @@ __global__ void __launch_bounds__(T_NT, 3) mmerge3_kernel(const MMParams P) {
     u64 lo = 0, hi = 0;
     bool exact = !interior;  // read the runs' end values (also when the splitters are too far apart for 32-bit keys
     if (interior) {          // although the values between them may not be)
-        lo = P.splitters[(u64)b * P.stride - 1];
-        hi = P.splitters[(u64)(b + 1) * P.stride - 1] - 1;  // splitters are distinct and ascending: hi >= lo
+        lo = P.splitters[(u64)b * MM_STRIDE - 1];
+        hi = P.splitters[(u64)(b + 1) * MM_STRIDE - 1] - 1;  // splitters are distinct and ascending: hi >= lo
         exact = hi - lo >= (u64)T_INF;
     }
     {
@@ -469,12 +402,11 @@ __global__ void __launch_bounds__(T_NT, 3) mmerge3_kernel(const MMParams P) {
 
     // Pull the slices of the tile this SM slot will most likely run next (P.ahead tiles on) into L2 while this one is
     // merged: its loads then pay an L2 hit instead of a DRAM round trip.
-    if (P.ahead && tid < k && b + P.ahead <= ns) {
+    if (tid < k && b + P.ahead <= ns) {
         const u64 c2 = P.bounds[(u64)tid * P.nbs + b + P.ahead], e2 = P.bounds[(u64)tid * P.nbs + b + P.ahead + 1];
         const u64* q = s_ptr[tid];
         for (u64 i = c2 & ~(u64)15; i < e2; i += 16) asm volatile("prefetch.global.L2 [%0];" ::"l"(q + i));
     }
-    if (docopy) t32_copy_tile<T_NT>(P, b - P.lag, s_cbase, tid);
 
     // Equal values always fall into the same tile (every run is cut at lower_bound of the same splitter), so a tile
     // never has to look at its predecessor's last value.
@@ -482,40 +414,13 @@ __global__ void __launch_bounds__(T_NT, 3) mmerge3_kernel(const MMParams P) {
     const bool wide = hi - lo >= (u64)T_INF;
     if (total != 0) {
         if (!wide) produced = t32_tile((u32*)s_raw, s_ptr, s_cur, s_end, k, (u32*)(P.scratch + inbase), lo);
-        else produced = mm_levels_tile((u64*)s_raw, s_ptr, s_cur, s_end, k, P.scratch + inbase, false, 0);
+        else produced = mm_levels_tile((u64*)s_raw, s_ptr, s_cur, s_end, k, P.scratch + inbase);
     }
-    __syncthreads();  // every thread's scratch writes precede the fence below
     if (tid == 0) {
         P.tile_in[b] = inbase;
         P.tile_lo[b] = lo;
         P.tile_cnt[b] = produced | (wide ? kTileWide : 0u);
-        if (P.lag) {
-            __threadfence();
-            st_relaxed(P.status + b, kFlagAgg | (u64)produced);
-        }
     }
-}
-
-// The tiles no later CTA moves: tile ns - i for CTA i < min(lag, ns + 1).  The CTA of tile ns also reports the length.
-__global__ void __launch_bounds__(T_NT) mtail_kernel(const MMParams P) {
-    __shared__ u64 s_cbase;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const u32 ns = (u32)(*P.nsplit / P.stride);
-    if (blockIdx.x > ns) return;
-    const u32 t = ns - blockIdx.x;
-    if (wid == 0) {
-        u64 agg;
-        const u64 base = t32_tile_offset(P, t, lane, &agg);
-        if (lane == 0) {
-            s_cbase = base;
-            if (t == ns) {
-                *P.out_len = base + agg;
-                if (base + agg > P.out_cap) atomicExch(P.err, 1);
-            }
-        }
-    }
-    __syncthreads();
-    t32_copy_tile<T_NT>(P, t, s_cbase, tid);
 }
 
 }  // namespace dgx

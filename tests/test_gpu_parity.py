@@ -426,61 +426,131 @@ def test_properties_at_scale(dgx):
     eq(m2.Uids, np.union1d(a, b), "union")
 
 
-@pytest.mark.parametrize("knobs", [{}, {"DGX_MERGE_STRIDE": "16"}, {"DGX_MERGE_LAG": "3"}, {"DGX_MERGE_LAG": "700"},
-                                   {"DGX_MERGE": "levels"}],
-                         ids=["default", "stride16", "lag3", "lag700", "levels"])
-def test_merge_multiway_forced(orc, knobs):
-    """The multiway MergeSorted path with its size threshold removed (DGX_MERGE_MULTI_MIN=0), in a
-    subprocess because libdgx reads its knobs once: known answers, random k, adversarial shapes that
-    force the block-wise rounds (identical lists, one dense cluster, long duplicate runs).  Variants: tiles so large
-    that most need several rounds (stride 16), compaction inside the merge kernel at a lag smaller and larger than
-    the number of resident CTAs, and the round-1 pipeline (64-bit tile keys)."""
-    import subprocess
-    code = r'''
-import os, sys
-import numpy as np
-sys.path.insert(0, os.getcwd()); sys.path.insert(0, os.path.join(os.getcwd(), "tests"))
-import gen
-from dgraph_b200 import algo, pb
-from oracle import pyoracle as orc
-from test_oracle_algo import MERGE_CASES
-def L(x): return pb.List(np.asarray(x, dtype=np.uint64))
-def chk(lists, what):
-    got = algo.MergeSorted([L(l) for l in lists]).Uids
-    want = orc.merge_sorted(lists)
-    assert got.size == want.size and np.array_equal(got, want), (what, got.size, want.size)
-for lists, want in MERGE_CASES:
-    got = algo.MergeSorted([L(l) for l in lists])
-    assert got.tolist() == want, (lists, got.tolist())
-rng = np.random.default_rng(77)
-for k in (3, 4, 5, 17, 33, 63, 64):
-    chk([np.sort(rng.integers(0, 50000, int(rng.integers(0, 3000)), dtype=np.uint64)) for _ in range(k)], f"small k={k}")
-# more than 64 lists: groups of <= 64 merged multiway into intermediate runs (device-side lengths), then merged again
-for k in (65, 130, 257):
-    chk([np.sort(rng.integers(0, 200000, int(rng.integers(0, 4000)), dtype=np.uint64)) for _ in range(k)], f"grouped k={k}")
-wide = gen.zipf_gaps(rng, 1500000)
-chk([gen.thin(rng, wide, float(rng.uniform(0.002, 0.03))) for _ in range(200)], "grouped k=200, 3e6 values")
-chk([np.zeros(0, np.uint64)] * 70 + [wide[::5], wide[1::7]] + [np.zeros(0, np.uint64)] * 70, "mostly empty, k=142")
-master = gen.zipf_gaps(rng, 400000)
-chk([master] * 64, "64 identical lists")
-chk([master[::3], master[1::3], master[2::3]] * 8, "interleaved x8")
-dense = np.arange(10**6, 10**6 + 300000, dtype=np.uint64)
-chk([dense] + [gen.thin(rng, master, 0.01) for _ in range(40)], "one dense cluster")
-runs = np.sort(np.concatenate([np.full(50000, 7), np.full(70000, 9), rng.integers(0, 100, 5000)]).astype(np.uint64))
-chk([runs, runs[::2], np.arange(0, 200, dtype=np.uint64)] * 5, "long duplicate runs")
-lens = (2_000_000 / np.arange(1, 65)).astype(int)
-big = gen.zipf_gaps(rng, 4_000_000)
-chk([gen.thin(rng, big, min(1.0, l / big.size)) for l in lens], "config-5 shape")
-chk([np.array([2**64 - 1, 2**64 - 1], dtype=np.uint64), np.array([0, 2**64 - 1], dtype=np.uint64), np.array([5], dtype=np.uint64)], "max values")
-# key widths: tiles whose value span fits 32 bits merge on u32 keys, wide ones on u64 -- cover both and the mix
-chk([np.sort(rng.integers(0, 2**64 - 1, 20000, dtype=np.uint64)) for _ in range(9)], "full-range 64-bit values")
-far = (np.arange(30000, dtype=np.uint64) << np.uint64(33)) + np.uint64(12345)
-chk([far[::2], far[1::3], np.arange(5 * 10**9, 5 * 10**9 + 40000, dtype=np.uint64), far[::7]], "wide gaps around a dense cluster")
-edge = np.uint64(2**32 - 2) * np.arange(1, 20001, dtype=np.uint64)
-chk([edge, edge + np.uint64(1), edge[::2] + np.uint64(2**32 - 3)], "spans at the 32-bit boundary")
-print("MULTIWAY_OK")
-'''
-    env = dict(os.environ, DGX_MERGE_MULTI_MIN="0", **knobs)
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600, env=env,
-                       cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    assert "MULTIWAY_OK" in r.stdout, r.stdout[-2000:] + r.stderr[-4000:]
+# ---- MergeSorted: the multiway merge and its grouping --------------------------------------
+
+MERGE_MULTI_MIN = 1 << 18  # merge_runs_impl (dgx_api.cu): smallest total that leaves the pairwise tree
+MM_K = 64                  # largest fan-in of one multiway merge
+
+
+def _tree_launches(k):
+    """merge_tree_impl: one merge_kernel launch per level; a single run still takes one (in-run de-duplication)."""
+    levels = 0
+    while k > 1:
+        k, levels = (k + 1) // 2, levels + 1
+    return max(levels, 1)
+
+
+def _merge_plan(lens):
+    """(path, kernel launches) of merge_runs_impl for non-empty runs of these lengths."""
+    k, total = len(lens), sum(lens)
+    if 3 <= k <= MM_K and total >= MERGE_MULTI_MIN:
+        # merge_multi_impl: msample, the tree over the non-empty sample runs, mplan2, mmerge3, mscan, mcompact
+        ntarget = min(max(total // 512, 1), 1 << 24)
+        return "multiway", 5 + _tree_launches(sum(1 for n in lens if n * ntarget // total))
+    ngroups = -(-k // MM_K)
+    if k <= MM_K or total // ngroups < 4 * MERGE_MULTI_MIN:
+        return "tree", _tree_launches(k)
+    gsz = -(-k // ngroups)
+    groups = [lens[b:b + gsz] for b in range(0, k, gsz)]
+    return "grouped", sum(_merge_plan(g)[1] for g in groups) + _merge_plan([sum(g) for g in groups])[1]
+
+
+def _random_k(k, lo, hi):
+    return lambda rng: [np.sort(rng.integers(0, 1 << 22, int(rng.integers(lo, hi)), dtype=np.uint64)) for _ in range(k)]
+
+
+def _zipf_lists(k, lo, hi):
+    return lambda rng: [gen.zipf_gaps(rng, int(n)) for n in rng.integers(lo, hi, k)]
+
+
+def _wide_gaps(rng):
+    far = (np.arange(240_000, dtype=np.uint64) << np.uint64(33)) + np.uint64(12345)
+    return [far[::2], far[1::3], np.arange(5 * 10**9, 5 * 10**9 + 100_000, dtype=np.uint64), far[::7]]
+
+
+def _edges(rng):
+    edge = np.uint64(2**32 - 2) * np.arange(1, 120_001, dtype=np.uint64)
+    return [edge, edge + np.uint64(1), edge[::2] + np.uint64(2**32 - 3)]
+
+
+def _max_values(rng):
+    top = np.uint64(2**64 - 1) - np.arange(240_000, dtype=np.uint64)[::-1]
+    low = gen.thin(rng, gen.zipf_gaps(rng, 150_000), 0.7)
+    mx = np.full(2_000, 2**64 - 1, dtype=np.uint64)
+    return [top[::2], top[1::3], np.concatenate([low, mx]), np.full(5_000, 2**64 - 1, dtype=np.uint64),
+            np.array([0, 2**64 - 1], dtype=np.uint64)]
+
+
+def _identical(rng):
+    return [gen.zipf_gaps(rng, 200_000)] * 64
+
+
+def _interleaved(rng):
+    m = gen.zipf_gaps(rng, 400_000)
+    return [m[::3], m[1::3], m[2::3]] * 8
+
+
+def _dense_cluster(rng):
+    m = gen.zipf_gaps(rng, 400_000)
+    return [np.arange(10**6, 10**6 + 300_000, dtype=np.uint64)] + [gen.thin(rng, m, 0.01) for _ in range(40)]
+
+
+def _duplicate_runs(rng):
+    runs = np.sort(np.concatenate([np.full(50_000, 7), np.full(70_000, 9), rng.integers(0, 100, 5_000)]).astype(np.uint64))
+    return [runs, runs[::2], np.arange(0, 200, dtype=np.uint64)] * 5
+
+
+def _config5(rng):
+    big = gen.zipf_gaps(rng, 4_000_000)
+    return [gen.thin(rng, big, min(1.0, n / big.size)) for n in (2_000_000 / np.arange(1, 65)).astype(int)]
+
+
+def _mostly_empty(rng):
+    w, e = gen.zipf_gaps(rng, 1_500_000), np.zeros(0, np.uint64)
+    return [e] * 70 + [w[::5], w[1::7], w[2::11]] + [e] * 70
+
+
+# name -> (path, inputs).  Sizes are chosen for the path under the shipped thresholds: 3..64 non-empty runs and
+# >= 2^18 values for the multiway merge, more than 64 runs and >= 4 x 2^18 values per group for the grouping.
+MULTIWAY_CASES = {
+    "random k=3": ("multiway", _random_k(3, 100_000, 200_000)),
+    "random k=17": ("multiway", _random_k(17, 20_000, 40_000)),
+    "random k=64": ("multiway", _random_k(64, 5_000, 15_000)),
+    # tiles whose value span does not fit 32 bits take the 64-bit engine; mixed inputs put both kinds in one call
+    "full-range 64-bit values": ("multiway", lambda rng: [np.sort(rng.integers(0, 2**64 - 1, 40_000, dtype=np.uint64))
+                                                          for _ in range(9)]),
+    "wide gaps around a dense cluster": ("multiway", _wide_gaps),
+    "spans at multiples of 2^32": ("multiway", _edges),
+    "2^64-1 in a large input": ("multiway", _max_values),
+    # adversarial shapes: tiles that take several rounds, few distinct splitters
+    "64 identical lists": ("multiway", _identical),
+    "interleaved x8": ("multiway", _interleaved),
+    "one dense cluster": ("multiway", _dense_cluster),
+    "long duplicate runs": ("multiway", _duplicate_runs),
+    "config-5 shape": ("multiway", _config5),
+    "mostly empty": ("multiway", _mostly_empty),
+    # groups of <= 64 merged multiway into intermediate runs (device-side lengths), then merged again
+    "grouped k=65": ("grouped", _zipf_lists(65, 36_000, 44_000)),
+    "grouped k=200": ("grouped", _zipf_lists(200, 20_000, 52_000)),
+    "grouped k=257": ("grouped", _zipf_lists(257, 22_000, 28_000)),
+}
+
+
+@pytest.mark.parametrize("name", list(MULTIWAY_CASES))
+def test_merge_multiway_paths(dgx, orc, name):
+    """MergeSorted through the multiway merge or its grouping, bit-exact against the oracle.  The kernel launch count
+    shows which path ran, so a change of the thresholds fails here instead of sending the cases to the tree."""
+    from dgraph_b200 import _lib
+
+    path, make = MULTIWAY_CASES[name]
+    lists = make(np.random.default_rng(77))
+    lens = [int(x.size) for x in lists if x.size]
+    plan, want_launches = _merge_plan(lens)
+    assert plan == path, f"{name}: {len(lens)} runs of {sum(lens)} values take the {plan} path"
+    assert want_launches != _tree_launches(len(lens))
+    k0 = _lib.stats()["kernel_launches"]
+    got = dgx.algo.MergeSorted([L(dgx, x) for x in lists]).Uids
+    launches = _lib.stats()["kernel_launches"] - k0
+    print(f"{name}: k={len(lens)} values={sum(lens)} {path}, {launches} launches")
+    eq(got, orc.merge_sorted(lists), name)
+    assert launches == want_launches, f"{name}: {launches} launches, the {path} path makes {want_launches}"

@@ -8,7 +8,7 @@ timeout 200 python bench.py --no-resident --no-e2e --no-ops --steps 50 --warmup 
 timeout 600 python tools/bench_ops.py --out $o/${tag}_ops.json > $o/${tag}_ops.log 2>&1
 timeout 300 ncu --metrics gpu__time_duration.sum --clock-control none -c 400 --csv --log-file $o/${tag}_bench_launches.csv \
     python bench.py --steps 2 --warmup 3 --no-e2e --no-ops --no-dense > $o/${tag}_ncu_bench.log 2>&1
-timeout 200 ncu --metrics gpu__time_duration.sum --clock-control none -k regex:"mmerge|mplan|msample|merge_kernel|mscan|mcompact|mtail" -c 60 --csv --log-file $o/${tag}_merge_launches.csv python tools/bench_merge.py --reps 2 > $o/${tag}_ncu_merge.log 2>&1
+timeout 200 ncu --metrics gpu__time_duration.sum --clock-control none -k regex:"mmerge3|mplan2|msample|merge_kernel|mscan|mcompact" -c 60 --csv --log-file $o/${tag}_merge_launches.csv python tools/bench_merge.py --reps 2 > $o/${tag}_ncu_merge.log 2>&1
 timeout 300 ncu --set full --import-source on --clock-control none -k regex:mmerge3 -s 1 -c 1 -o $o/${tag}_mmerge3 -f python tools/bench_merge.py --reps 1 > $o/${tag}_ncu_merge2.log 2>&1
 timeout 120 python tools/bench_merge.py --dense > $o/${tag}_merge_cases.jsonl 2>/dev/null; cat $o/${tag}_merge_cases.jsonl
 timeout 900 python -m pytest tests -m gpu -q --durations=5 > $o/${tag}_tests.log 2>&1; tail -2 $o/${tag}_tests.log
