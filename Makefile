@@ -5,7 +5,7 @@ NVFLAGS ?= -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-maybe-un
 CSRC := dgraph_b200/csrc
 HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.hpp) include/dgx.h
 
-.PHONY: all prof clean variant
+.PHONY: all prof clean
 all: dgraph_b200/libdgx.so oracle/liboracle.so
 
 dgraph_b200/libdgx.so: $(CSRC)/dgx_api.cu $(HDRS)
@@ -21,7 +21,3 @@ oracle/liboracle.so: oracle/oracle.c oracle/oracle.h
 
 clean:
 	rm -f dgraph_b200/libdgx.so dgraph_b200/libdgx_prof.so oracle/liboracle.so
-
-# experimental builds for A/B runs: make variant NAME=nofast EXTRA="-DDGX_P_FAST=0" -> dgraph_b200/libdgx_nofast.so
-variant:
-	$(NVCC) $(NVFLAGS) $(EXTRA) -shared -o dgraph_b200/libdgx_$(NAME).so $(CSRC)/dgx_api.cu -lcudart

@@ -20,11 +20,6 @@ __device__ __forceinline__ u64 ld_stream(const u64* p) {
     asm volatile("ld.global.nc.L1::no_allocate.u64 %0, [%1];" : "=l"(v) : "l"(p));
     return v;
 }
-__device__ __forceinline__ ulonglong2 ld_stream2(const u64* p) {  // p must be 16-byte aligned
-    ulonglong2 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v2.u64 {%0, %1}, [%2];" : "=l"(v.x), "=l"(v.y) : "l"(p));
-    return v;
-}
 // Probe read (binary searches): cached, neighbouring probes share sectors.
 __device__ __forceinline__ u64 ld_probe(const u64* p) { return __ldg(p); }
 

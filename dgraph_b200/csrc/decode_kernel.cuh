@@ -121,10 +121,6 @@ __device__ __forceinline__ void mbar_wait(u32 bar, u32 parity) {
 // backs off with nanosleep, so a waiting warp does not compete with working warps for issue slots.
 template <unsigned kSleepNs = 128>
 __device__ __forceinline__ void mbar_wait_relaxed(u32 bar, u32 parity) {
-#ifdef DGX_HWWAIT
-    mbar_wait(bar, parity);   // experiment: leave the waiting to the hardware's try_wait suspension
-    return;
-#endif
     u32 done = 0;
     while (true) {
         asm volatile(

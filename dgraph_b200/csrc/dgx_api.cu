@@ -78,16 +78,8 @@ static std::vector<dgx_lane*> g_pool;  // idle lanes for the host-pointer entry 
 static std::condition_variable g_pool_cv;
 static size_t g_lanes_out = 0;     // lanes currently leased
 static size_t g_lanes_total = 0;   // lanes in existence (pooled + leased)
-static u32 g_stream_ratio = 16;
-static u32 g_scap_override = 0;       // DGX_SCAP: force the filter kernel's slice staging capacity
-constexpr u32 kScapMin = 8192, kScapMax = 65536;  // bytes
-static int g_filter_pipe = 1;          // DGX_FILTER=v4 selects the non-persistent kernel
 static int g_zero_copy = 0;            // DGX_ZERO_COPY=1: decode pinned packs in place over PCIe (off: DMA copies move the bytes faster)
 constexpr size_t g_merge_multi_min = size_t(1) << 18;  // MergeSorted totals below this stay on the tree (fewer launches)
-static size_t g_pre_throttle_smem = 0;  // DGX_PRE_THROTTLE: dynamic smem asked for by an ahead-of-time pre-pass (0 = unthrottled)
-static u32 g_reserve_ctas = 0;         // DGX_RESERVE_CTAS: pipeline CTAs left out of the persistent grid
-static uint64_t g_pipe_min_values = 0;  // DGX_PIPE_MIN_VALUES: batches driving fewer values than this use filter_kernel
-static size_t g_pipe_min_k = 2;        // DGX_PIPE_MIN_K: batches whose widest query has fewer lists use filter_kernel
 static int g_num_sms = 132;
 constexpr size_t kPipeSmemMax = 220 * 1024;
 
@@ -263,13 +255,10 @@ extern "C" int dgx_init(int device) {
                             (int)(sizeof(DWarpSmem) * D_WARPS)));
     CK(cudaFuncSetAttribute(icw_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)(sizeof(DWarpSmem) * D_WARPS)));
-    CK(cudaFuncSetAttribute(filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)(2 * F_TA * sizeof(u64) + kScapMax)));
     CK(cudaFuncSetAttribute(filter_pipe_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmemMax));
     CK(cudaFuncSetAttribute(filter_pipe_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPipeSmemMax));
     g_num_sms = prop.multiProcessorCount;
     numa_probe(device);
-    if (const char* s = getenv("DGX_FILTER")) g_filter_pipe = (strcmp(s, "v4") != 0);
     CK(cudaFuncSetAttribute(mmerge3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T_SMEM));
     if (const char* s = getenv("DGX_ZERO_COPY")) g_zero_copy = atoi(s) != 0;
     g_device = device;
@@ -291,8 +280,8 @@ extern "C" int dgx_describe(char* buf, size_t n) {
     if (rc != DGX_OK) return rc;
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, g_device));
-    snprintf(buf, n, "libdgx sm_90a | device %d: %s, %d SMs, %.1f GB | filter tile %d, merge tile %d",
-             g_device, prop.name, prop.multiProcessorCount, prop.totalGlobalMem / 1e9, F_TA, M_T);
+    snprintf(buf, n, "libdgx sm_90a | device %d: %s, %d SMs, %.1f GB | filter tiles %d / %d, merge tile %d",
+             g_device, prop.name, prop.multiProcessorCount, prop.totalGlobalMem / 1e9, p_tile_size(2), p_tile_size(4), M_T);
     return DGX_OK;
 }
 
@@ -506,25 +495,14 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
     uint64_t ntiles = 0, uids_in = 0;
     size_t li = 0, kmax = 1;
     for (size_t q = 0; q < nq; ++q) kmax = std::max(kmax, k_off[q + 1] - k_off[q]);
-    // Small batches take the single-launch kernel: the pipeline's plan pre-pass (two more launches, a second
-    // descriptor copy) costs more than it saves when the whole batch is a few hundred tiles (DGX_PIPE_MIN_VALUES).
-    uint64_t drive_total = 0;
-    for (size_t q = 0; q < nq; ++q) {
-        uint64_t mn = UINT64_MAX;
-        for (size_t i = k_off[q]; i < k_off[q + 1]; ++i) mn = std::min<uint64_t>(mn, lists[i].len);
-        if (op == DGX_OP_DIFFERENCE && k_off[q + 1] > k_off[q]) mn = lists[k_off[q]].len;
-        if (mn != UINT64_MAX) drive_total += mn;
-    }
-    const bool use_pipe = g_filter_pipe && kmax >= g_pipe_min_k && drive_total >= g_pipe_min_values;
-    // 2-list batches: 1024-value tiles (per-tile overheads over twice the values); wider queries: 512 (filter_pipe.cuh)
+    // 1- and 2-list batches: 1024-value tiles (per-tile overheads over twice the values); wider queries: 512 (filter_pipe.cuh)
     const int pipe_va = kmax <= 2 ? 4 : 2;
-    const uint64_t tile_sz = use_pipe ? (uint64_t)p_tile_size(pipe_va) : (uint64_t)F_TA;
+    const uint64_t tile_sz = (uint64_t)p_tile_size(pipe_va);
     std::vector<size_t> order;
     for (size_t q = 0; q < nq; ++q) {
         const size_t k0 = k_off[q], k1 = k_off[q + 1];
         const size_t k = k1 - k0;
         if (k == 0) return fail(DGX_ERR_ARG, "query %zu has no lists", q);
-        kmax = std::max(kmax, k);
         if (op == DGX_OP_DIFFERENCE && k != 2) return fail(DGX_ERR_ARG, "difference takes exactly two lists");
         order.resize(k);
         std::iota(order.begin(), order.end(), k0);
@@ -550,7 +528,7 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
     // Resident-inputs lanes: one of two alternating workspaces and the side stream -- descriptor copies, status
     // reset and the plan pre-pass of THIS batch then run while the pipeline kernel of the PREVIOUS batch is still
     // busy (the lists are immutable, so the pre-pass depends on nothing the main stream has queued).
-    const bool ahead = l->resident_inputs && use_pipe && l->side;
+    const bool ahead = l->resident_inputs && l->side;
     const int slot = l->fslot;
     DevArena* ar = &l->ws;
     cudaStream_t pre = l->stream;
@@ -579,97 +557,77 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
     P.ntasks = (u32)nq;
     P.ntiles = (u32)ntiles;
     P.op = op;
-    P.stream_ratio = g_stream_ratio;
-    // staging capacity (bytes): ~1.1 tile-widths of 32-bit keys for every filter list of the widest query
-    P.scap_bytes = g_scap_override ? g_scap_override
-                                   : (u32)std::min<size_t>(32768, std::max<size_t>(kScapMin, (kmax - 1) * 1152 * 4));
     P.out = (u64*)d_out;
     P.out_cap = out_cap;
     P.out_off = (u64*)d_out_off;
     P.status = (u64*)d_status;
     P.ticket = (u32*)(d_status + ntiles * sizeof(u64));
     P.err = l->d_err;
-    if (!use_pipe) {
-        filter_kernel<<<(unsigned)ntiles, F_NT, 2 * F_TA * sizeof(u64) + P.scap_bytes, l->stream>>>(P);
-        CK(cudaGetLastError());
-        l->launches += 1;
-        g_stats.launches += 1;
-    } else {
-        // ---- persistent TMA pipeline: plan pre-pass + filter_pipe_kernel ----------------
-        void* hp_raw;
-        rc = l->host.alloc(nq * sizeof(u64), &hp_raw);
-        if (rc) return rc;
-        u64* h_pb = (u64*)hp_raw;
-        u64 npairs = 0;
-        for (size_t q = 0; q < nq; ++q) {
-            h_pb[q] = npairs;
-            const u64 nt = (q + 1 < nq ? ht[q + 1].tile_base : ntiles) - ht[q].tile_base;
-            npairs += nt * (u64)(ht[q].k - 1);
-        }
-        void *d_pb, *d_plan, *d_tiles;
-        rc = ar->alloc(nq * sizeof(u64), &d_pb);
-        if (rc) return rc;
-        rc = ar->alloc(ntiles * sizeof(PTileEntry), &d_tiles);
-        if (rc) return rc;
-        rc = ar->alloc((npairs + 1) * sizeof(PPlanEntry), &d_plan);
-        if (rc) return rc;
-        CK(cudaMemcpyAsync(d_pb, h_pb, nq * sizeof(u64), cudaMemcpyHostToDevice, pre));
-        // DGX_PRE_THROTTLE: dynamic shared memory an ahead-of-time pre-pass asks for (16 KB would limit it to one CTA on
-        // an SM that holds two pipeline CTAs).  What the overlap costs the pipeline is L2 / DRAM interference, not issue
-        // slots, so throttling the pre-pass does not help and the default is 0.
-        const size_t pre_smem = ahead ? g_pre_throttle_smem : 0;
-        filter_tiles_kernel<<<(unsigned)((ntiles + 255) / 256), 256, pre_smem, pre>>>(P.tasks, P.lists, (const u64*)d_pb, P.ntasks,
-                                                                                      P.ntiles, (PTileEntry*)d_tiles, (u32)tile_sz);
-        CK(cudaGetLastError());
-        l->launches += 1;
-        g_stats.launches += 1;
-        if (npairs) {
-            const u64 blocks = (npairs + 255) / 256;
-            if (blocks > 0x7fffffffull) return fail(DGX_ERR_ARG, "batch too large");
-            filter_plan_kernel<<<(unsigned)blocks, 256, pre_smem, pre>>>(P.tasks, P.lists, (const u64*)d_pb, P.ntasks, npairs,
-                                                                         (PPlanEntry*)d_plan, (u32)tile_sz);
-            CK(cudaGetLastError());
-            l->launches += 1;
-            g_stats.launches += 1;
-        }
-        PParams PP;
-        PP.f = P;
-        PP.plan_base = (const u64*)d_pb;
-        PP.plan = (const PPlanEntry*)d_plan;
-        PP.tiles = (const PTileEntry*)d_tiles;
-        // wide queries: one tile per ticket keeps the look-back order tight; 2-list batches have tiny tiles and
-        // amortise the metadata chain over two
-        PP.grp = kmax >= 4 ? 1u : 2u;
-        const size_t nl = std::min<size_t>(std::max<size_t>(kmax - 1, 1), P_MAXL);
-        const size_t TA = (size_t)tile_sz;
-        // staged slices: ~1.125 tile-widths per filter list; a 2-list batch stages up to 2.25 tile-widths of its one
-        // filter list (size ratios beyond that probe the list in HBM, the reference's own Jump / Bin regimes)
-        size_t cap = (TA + TA / 8) * nl * (kmax <= 2 ? 2 : 1);
-        if (g_scap_override) cap = g_scap_override / 8;
-        cap = std::min<size_t>(std::max<size_t>(cap, TA + TA / 8), 9216) & ~size_t(1);
-        PP.slice_cap = (u32)cap;
-        const size_t smem = ((sizeof(PShared) + 127) & ~size_t(127)) + (1 + P_OS) * TA * sizeof(u64) +
-                            P_ST * ((TA + 2) + cap) * sizeof(u64);
-        if (smem > kPipeSmemMax) return fail(DGX_ERR_ARG, "pipeline stage too large");
-        auto kern = pipe_va == 4 ? filter_pipe_kernel<4> : filter_pipe_kernel<2>;
-        int per_sm = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, P_NT, smem));
-        if (per_sm < 1) return fail(DGX_ERR_CUDA, "filter_pipe_kernel does not fit on an SM");
-        u64 resident = (u64)per_sm * (u64)g_num_sms;
-        // DGX_RESERVE_CTAS: leave a few CTA slots free so that a collective queued on another stream (the result
-        // gather of the previous batch) finds an SM while the persistent pipeline runs
-        if (g_reserve_ctas && resident > 2 * (u64)g_reserve_ctas) resident -= g_reserve_ctas;
-        PP.nctas = (u32)std::min<u64>(resident, ntiles);
-        if (ahead) {
-            CK(cudaEventRecord(l->ev_plan[slot], l->side));
-            CK(cudaStreamWaitEvent(l->stream, l->ev_plan[slot], 0));
-        }
-        kern<<<PP.nctas, P_NT, smem, l->stream>>>(PP);
-        CK(cudaGetLastError());
-        l->launches += 1;
-        g_stats.launches += 1;
-        if (ahead) CK(cudaEventRecord(l->ev_pipe[slot], l->stream));
+    // ---- plan pre-pass + persistent TMA pipeline (filter_pipe_kernel) ----------------
+    void* hp_raw;
+    rc = l->host.alloc(nq * sizeof(u64), &hp_raw);
+    if (rc) return rc;
+    u64* h_pb = (u64*)hp_raw;
+    u64 npairs = 0;
+    for (size_t q = 0; q < nq; ++q) {
+        h_pb[q] = npairs;
+        const u64 nt = (q + 1 < nq ? ht[q + 1].tile_base : ntiles) - ht[q].tile_base;
+        npairs += nt * (u64)(ht[q].k - 1);
     }
+    void *d_pb, *d_plan, *d_tiles;
+    rc = ar->alloc(nq * sizeof(u64), &d_pb);
+    if (rc) return rc;
+    rc = ar->alloc(ntiles * sizeof(PTileEntry), &d_tiles);
+    if (rc) return rc;
+    rc = ar->alloc((npairs + 1) * sizeof(PPlanEntry), &d_plan);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(d_pb, h_pb, nq * sizeof(u64), cudaMemcpyHostToDevice, pre));
+    filter_tiles_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, pre>>>(P.tasks, P.lists, (const u64*)d_pb, P.ntasks,
+                                                                           P.ntiles, (PTileEntry*)d_tiles, (u32)tile_sz);
+    CK(cudaGetLastError());
+    l->launches += 1;
+    g_stats.launches += 1;
+    if (npairs) {  // a batch of one-list queries has no slices to bound
+        const u64 blocks = (npairs + 255) / 256;
+        if (blocks > 0x7fffffffull) return fail(DGX_ERR_ARG, "batch too large");
+        filter_plan_kernel<<<(unsigned)blocks, 256, 0, pre>>>(P.tasks, P.lists, (const u64*)d_pb, P.ntasks, npairs,
+                                                              (PPlanEntry*)d_plan, (u32)tile_sz);
+        CK(cudaGetLastError());
+        l->launches += 1;
+        g_stats.launches += 1;
+    }
+    PParams PP;
+    PP.f = P;
+    PP.plan_base = (const u64*)d_pb;
+    PP.plan = (const PPlanEntry*)d_plan;
+    PP.tiles = (const PTileEntry*)d_tiles;
+    // wide queries: one tile per ticket keeps the look-back order tight; 2-list batches have tiny tiles and
+    // amortise the metadata chain over two
+    PP.grp = kmax >= 4 ? 1u : 2u;
+    const size_t nl = std::min<size_t>(std::max<size_t>(kmax - 1, 1), P_MAXL);
+    const size_t TA = (size_t)tile_sz;
+    // staged slices: ~1.125 tile-widths per filter list; a 2-list batch stages up to 2.25 tile-widths of its one
+    // filter list (size ratios beyond that probe the list in HBM, the reference's own Jump / Bin regimes)
+    size_t cap = (TA + TA / 8) * nl * (kmax <= 2 ? 2 : 1);
+    cap = std::min<size_t>(std::max<size_t>(cap, TA + TA / 8), 9216) & ~size_t(1);
+    PP.slice_cap = (u32)cap;
+    const size_t smem = ((sizeof(PShared) + 127) & ~size_t(127)) + (1 + P_OS) * TA * sizeof(u64) +
+                        P_ST * ((TA + 2) + cap) * sizeof(u64);
+    if (smem > kPipeSmemMax) return fail(DGX_ERR_ARG, "pipeline stage too large");
+    auto kern = pipe_va == 4 ? filter_pipe_kernel<4> : filter_pipe_kernel<2>;
+    int per_sm = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, P_NT, smem));
+    if (per_sm < 1) return fail(DGX_ERR_CUDA, "filter_pipe_kernel does not fit on an SM");
+    PP.nctas = (u32)std::min<u64>((u64)per_sm * (u64)g_num_sms, ntiles);
+    if (ahead) {
+        CK(cudaEventRecord(l->ev_plan[slot], l->side));
+        CK(cudaStreamWaitEvent(l->stream, l->ev_plan[slot], 0));
+    }
+    kern<<<PP.nctas, P_NT, smem, l->stream>>>(PP);
+    CK(cudaGetLastError());
+    l->launches += 1;
+    g_stats.launches += 1;
+    if (ahead) CK(cudaEventRecord(l->ev_pipe[slot], l->stream));
     g_stats.uids_in += uids_in;
     return DGX_OK;
 }

@@ -1,8 +1,7 @@
-// filter_pipe.cuh -- persistent, TMA-fed version of the batched sorted-set filter.
-//
-// Same contract as filter_kernel.cuh (IntersectWith / IntersectSorted chain /
-// Difference over a batch of queries, bit-exact incl. duplicate semantics), built
-// as a TMA / mbarrier pipeline (Hopper's bulk copies, no register staging):
+// filter_pipe.cuh -- the batched sorted-set filter for sm_90a: IntersectWith /
+// IntersectSorted chain / Difference over a batch of queries (descriptors and
+// duplicate semantics in filter_kernel.cuh), bit-exact, built as a persistent
+// TMA / mbarrier pipeline (Hopper's bulk copies, no register staging):
 //
 //   filter_tiles_kernel  one thread per tile: owning task, driving offset, plan index,
 //                        predecessor value -> a tile table in HBM.
@@ -29,7 +28,8 @@
 //   tile i+1 and the look-back of tiles i-1.. overlap the searches of tile i.
 //
 // Lists that are not pre-staged (slice larger than the stage, or more than 8
-// filter lists) are binary-searched in HBM by the surviving candidates.
+// filter lists) are binary-searched in HBM by the surviving candidates.  A query
+// of one list (k = 1) has no plan entries and its tiles are copied through.
 #pragma once
 
 #include "decode_kernel.cuh"   // mbarrier / TMA helpers
@@ -50,23 +50,8 @@ constexpr int P_NT = P_CT + 96;          // + metadata warp + TMA warp + output 
     constexpr int P_TA = P_CW * 32 * (VA); /* candidates per tile */                      \
     static_assert(P_VA == 2 || P_VA == 4, "rows per consumer warp")
 constexpr int p_tile_size(int va) { return P_CW * 32 * va; }
-#ifndef DGX_P_OS
-#define DGX_P_OS 6
-#endif
-constexpr int P_OS = DGX_P_OS;           // output slots in flight (more slots let 2-list batches, whose tiles finish fast, run ahead of the look-back)
-#ifndef DGX_P_ST
-#define DGX_P_ST 2
-#endif
-#ifndef DGX_PLAN_4ARY
-#define DGX_PLAN_4ARY 0   // 1: 4-ary plan searches (half the dependent latencies, 1.5x the probes; off: the extra probes cost more)
-#endif
-#ifndef DGX_P_PAIR2
-#define DGX_P_PAIR2 1   // two-row warps search two lists per iteration (four chains) once past the first list
-#endif
-#ifndef DGX_P_FAST
-#define DGX_P_FAST 1   // 0: build without the 32-bit fast path (A/B measurements, fallback-path tests)
-#endif
-constexpr int P_ST = DGX_P_ST;           // data stages in flight
+constexpr int P_OS = 6;                  // output slots in flight (more slots let 2-list batches, whose tiles finish fast, run ahead of the look-back)
+constexpr int P_ST = 2;                  // data stages in flight
 constexpr int P_MAXL = 8;                // filter lists a stage can hold
 constexpr int P_RING = 8;                // tile descriptors in flight between M and T
 constexpr int P_GRP = 4;                 // most tiles the metadata warp can resolve per iteration (8 lanes each)
@@ -74,15 +59,9 @@ constexpr u32 P_END = 0xffffffffu;
 // Back-off between polls of a waiting helper warp (ns): TMA warp / metadata + output warps / look-back.
 // The helpers share schedulers with consumer warps and every poll is an issue slot taken from them
 // (with short sleeps, polling takes a visible share of the issued instructions).
-#ifndef DGX_P_SLEEP_T
-#define DGX_P_SLEEP_T 600
-#endif
-#ifndef DGX_P_SLEEP_MO
-#define DGX_P_SLEEP_MO 2000
-#endif
-#ifndef DGX_P_SLEEP_LB
-#define DGX_P_SLEEP_LB 1000
-#endif
+constexpr unsigned P_SLEEP_T = 600;
+constexpr unsigned P_SLEEP_MO = 2000;
+constexpr unsigned P_SLEEP_LB = 1000;
 
 struct PPlanEntry { u64 r0, r1; };
 struct PTileEntry {            // everything the metadata warp needs about a tile, resolved by filter_tiles_kernel
@@ -92,7 +71,7 @@ struct PTileEntry {            // everything the metadata warp needs about a til
 };
 
 struct PParams {
-    FParams f;                 // tasks, lists, op, outputs, look-back state (ticket unused)
+    FParams f;                 // tasks, lists, op, outputs, look-back state; the M warp claims tiles with f.ticket
     const u64* plan_base;      // per task: index of its first plan entry
     const PPlanEntry* plan;    // per (tile, filter list)
     const struct PTileEntry* tiles;  // per tile
@@ -104,8 +83,8 @@ struct PParams {
 // ---- plan ---------------------------------------------------------------------------
 // One THREAD per (tile, filter list): r0 = first i with L[i] >= tile first, r1 = first i
 // with L[i] > tile last, as two interleaved binary searches.  A binary search touches one
-// new 32-byte sector per level only near its end (~8 sectors), where the 32-ary warp
-// search of filter_kernel.cuh touches ~70: the plan must not cost a second pass over HBM.
+// new 32-byte sector per level only near its end (~8 sectors), where a 32-ary warp
+// search touches ~70: the plan must not cost a second pass over HBM.
 __global__ void __launch_bounds__(256) filter_plan_kernel(const FTask* __restrict__ tasks, const FList* __restrict__ lists,
                                                           const u64* __restrict__ plan_base, u32 ntasks, u64 npairs,
                                                           PPlanEntry* __restrict__ plan, u32 tile_sz) {
@@ -131,30 +110,6 @@ __global__ void __launch_bounds__(256) filter_plan_kernel(const FTask* __restric
         const FList Lj = lists[T.list_first + j];
         const u64* __restrict__ B = Lj.ptr;
         u64 l0 = 0, h0 = flist_len(Lj), l1 = 0, h1 = h0;
-#if DGX_PLAN_4ARY
-        // Both searches advance in lock step and 4-ary: three probes per search and level are in flight together, so
-        // the dependent chain is log4(n) memory latencies instead of log2(n) -- the kernel is a latency chain, not a
-        // bandwidth load (the extra probes touch ~1.5x the sectors of a binary search, a few MB per launch)
-        while (h0 - l0 > 3 || h1 - l1 > 3) {
-            const bool a = h0 - l0 > 3, c = h1 - l1 > 3;
-            const u64 q0 = (h0 - l0) >> 2, q1 = (h1 - l1) >> 2;
-            u64 a1 = 0, a2 = 0, a3 = 0, c1 = 0, c2 = 0, c3 = 0;
-            if (a) { a1 = ld_probe(B + l0 + q0); a2 = ld_probe(B + l0 + 2 * q0); a3 = ld_probe(B + l0 + 3 * q0); }
-            if (c) { c1 = ld_probe(B + l1 + q1); c2 = ld_probe(B + l1 + 2 * q1); c3 = ld_probe(B + l1 + 3 * q1); }
-            if (a) {
-                if (a3 < tlo) l0 = l0 + 3 * q0 + 1;
-                else if (a2 < tlo) { h0 = l0 + 3 * q0; l0 = l0 + 2 * q0 + 1; }
-                else if (a1 < tlo) { h0 = l0 + 2 * q0; l0 = l0 + q0 + 1; }
-                else h0 = l0 + q0;
-            }
-            if (c) {
-                if (c3 <= thi) l1 = l1 + 3 * q1 + 1;
-                else if (c2 <= thi) { h1 = l1 + 3 * q1; l1 = l1 + 2 * q1 + 1; }
-                else if (c1 <= thi) { h1 = l1 + 2 * q1; l1 = l1 + q1 + 1; }
-                else h1 = l1 + q1;
-            }
-        }
-#endif
         while (l0 < h0 || l1 < h1) {
             const u64 m0 = l0 + ((h0 - l0) >> 1), m1 = l1 + ((h1 - l1) >> 1);
             const bool a = l0 < h0, c = l1 < h1;
@@ -456,7 +411,7 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
             if (lane == 0) next_base = atomicAdd(P.ticket, grp);  // prefetch (harmless past the end)
             const bool act = (u32)h < grp;  // lane groups beyond grp idle
             PPROF_T()
-            if (act && u == 0) mbar_wait_relaxed<DGX_P_SLEEP_MO>(smem_u32(&S.freed[slot]), (use & 1u) ^ 1u);
+            if (act && u == 0) mbar_wait_relaxed<P_SLEEP_MO>(smem_u32(&S.freed[slot]), (use & 1u) ^ 1u);
             __syncwarp();
             PPROF_ACC(pp_w0)
             const u64 tile64 = (u64)base_ticket + h;
@@ -495,12 +450,12 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
         for (u32 seq = 0;; ++seq) {
             const u32 slot = seq % P_RING, use = seq / P_RING;
             PPROF_T()
-            mbar_wait_relaxed<DGX_P_SLEEP_T>(smem_u32(&S.ready[slot]), use & 1u);
+            mbar_wait_relaxed<P_SLEEP_T>(smem_u32(&S.ready[slot]), use & 1u);
             PPROF_ACC(pp_w0)
             const PDesc& D = S.ring[slot];
             const u32 st = seq % P_ST, suse = seq / P_ST;
             PPROF_T()
-            mbar_wait_relaxed<DGX_P_SLEEP_T>(smem_u32(&S.empty[st]), (suse & 1u) ^ 1u);
+            mbar_wait_relaxed<P_SLEEP_T>(smem_u32(&S.empty[st]), (suse & 1u) ^ 1u);
             PPROF_ACC(pp_w1)
             PStageInfo& G = S.st[st];
             const u32 tile = D.tile;
@@ -567,7 +522,7 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
         for (u32 it = 0;; ++it) {
             const u32 sl = it % P_OS, use = it / P_OS;
             PPROF_T()
-            mbar_wait_relaxed<DGX_P_SLEEP_MO>(smem_u32(&S.ofull[sl]), use & 1u);
+            mbar_wait_relaxed<P_SLEEP_MO>(smem_u32(&S.ofull[sl]), use & 1u);
             PPROF_ACC(pp_w0)
             const POutSlot& O = S.os[sl];
             const u32 tile = O.tile;
@@ -582,7 +537,7 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
             }
             const u32 total = __shfl_sync(0xffffffffu, incl, 31);
             PPROF_T()
-            const u64 base = lookback_exclusive<true, DGX_P_SLEEP_LB>(P.status, tile, (u64)total, lane);
+            const u64 base = lookback_exclusive<true, P_SLEEP_LB>(P.status, tile, (u64)total, lane);
             PPROF_ACC(pp_w1)
             if (lane == 0) {
                 if (O.first) P.out_off[q] = base;
@@ -667,7 +622,7 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
             PPROF_PHASE(0)
             // ---- fast path: one upper word for the whole tile, no repeated values in this warp's rows,
             //      every filter list staged -> 32-bit searches on the low words (see lift32) ----------
-            bool fast = DGX_P_FAST && !warp_dup && nstaged == km1 && na > 0;
+            bool fast = !warp_dup && nstaged == km1 && na > 0;
             u32 hiword = 0;
             if (fast) {
                 const u32 cb = smem_u32(cand);
@@ -681,7 +636,6 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
                 const u32 slb = smem_u32(sl);
                 const bool keep_hits = P.op == 0;
                 while (t < km1 && rows > 0) {
-#if DGX_P_PAIR2
                     // (only after the first list: a warp that still fills two rows then has lost less than half of its
                     //  candidates, so the second search is rarely wasted; sparse workloads drop to one row and take
                     //  the three-list path below; always pairing slows sparse queries, never pairing slows dense ones)
@@ -697,9 +651,7 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
                         lift32m<2, 2>(s2, n2, l2, x2, h2);
                         alive &= h2[0] & h2[1];   // intersect only: a difference has a single filter list
                         t += 2;
-                    } else
-#endif
-                    if (rows >= 2) {
+                    } else if (rows >= 2) {
                         // ---- every row of the warp against ONE list (rows chains) ----------------------
                         const u32 nn[1] = {G.n[t]};
                         unsigned hit[1] = {0};

@@ -631,6 +631,124 @@ def test_filter_fast_path_stress(dgx, orc):
         eq(out[int(off[i]): int(off[i + 1])], orc.intersect_with(rows_a[i], rows_b[i]), f"batch row {i}")
 
 
+def one_list(rng, n, where):
+    """n sorted values with runs of equal values across every multiple of 512 (both tile sizes), placed low, straddling
+    2^32, or ending at 2^64 - 1."""
+    i = np.arange(n)
+    gaps = rng.choice(np.array([0, 1, 7, 1000], np.uint64), n, p=[0.2, 0.4, 0.3, 0.1])
+    gaps[(i % 512 >= 506) | (i % 512 < 6)] = 0
+    span = int(gaps.sum(dtype=np.uint64))
+    lo = {"low": 3, "2^32": (1 << 32) - span // 2, "top": (1 << 64) - 1 - span}[where]
+    return np.uint64(lo) + np.cumsum(gaps, dtype=np.uint64)
+
+
+def test_filter_one_list_queries(dgx, orc):
+    """Queries of one list (IntersectSorted of one list is a copy) run the pipeline without a plan: alone in a batch
+    (tile table + pipeline, two launches), mixed with wider queries, over a capacity one short, and on a resident-inputs
+    lane reading the previous batch's output."""
+    import torch
+    from dgraph_b200 import _lib
+
+    lib = _lib.load()
+    rng = np.random.default_rng(90)
+    # ---- host form: one list around the 1024-value tile size, and a long one
+    for n in (1, 1023, 1024, 1025, 3_000_000):
+        for where in ("low", "2^32", "top"):
+            l = one_list(rng, n, where)
+            before = _lib.stats()["kernel_launches"]
+            got = dgx.algo.IntersectSorted([L(dgx, l)])
+            assert _lib.stats()["kernel_launches"] - before == 2, f"launches, n={n} {where}"
+            eq(got.Uids, orc.intersect_sorted([l]), f"IntersectSorted of one list, n={n} {where}")
+
+    dev = torch.device("cuda", 0)
+    stream = torch.cuda.Stream(device=dev)
+    with torch.cuda.stream(stream):
+        lane = lib.dgx_lane_create(0, C.c_void_p(stream.cuda_stream))
+        assert lane
+
+        def run(queries, cap, op=0, out=None):
+            """queries: lists of numpy lists, each copied into its own device buffer.  Returns (out, off, inputs);
+            the input tensors must stay alive until the lane is synchronised."""
+            flat = [torch.from_numpy(np.concatenate([l, np.zeros(2, np.uint64)]).view(np.int64)).to(dev)
+                    for q in queries for l in q]
+            lens = [l.size for q in queries for l in q]
+            koff = np.concatenate([[0], np.cumsum([len(q) for q in queries])])
+            if out is None:
+                out = torch.full((cap + 8,), -1, dtype=torch.int64, device=dev)
+            off = torch.zeros(len(queries) + 1, dtype=torch.int64, device=dev)
+            _lib.check(lib.dgx_dev_filter_batch(lane, op, (C.c_void_p * len(flat))(*[t.data_ptr() for t in flat]),
+                                                (C.c_size_t * len(lens))(*lens),
+                                                (C.c_size_t * len(koff))(*[int(x) for x in koff]), len(queries),
+                                                C.c_void_p(out.data_ptr()), cap, C.c_void_p(off.data_ptr())))
+            return out, off, flat
+
+        # ---- device form: ~1000 one-list queries, some empty: one tile-table launch + one pipeline launch
+        qs = []
+        for q in range(1000):
+            n = 0 if q % 9 == 0 else int(rng.integers(1, 3000))
+            qs.append([one_list(rng, n, ("low", "2^32", "top")[q % 3])])
+        total = sum(q[0].size for q in qs)
+        before = lib.dgx_lane_launches(lane)
+        out, off, keep = run(qs, total)
+        assert lib.dgx_lane_launches(lane) - before == 2
+        _lib.check(lib.dgx_lane_sync(lane))
+        ho, hoff = out.cpu().numpy().view(np.uint64), off.cpu().numpy().view(np.uint64)
+        eq(hoff, np.concatenate([[0], np.cumsum([q[0].size for q in qs])]), "out_off of one-list queries")
+        eq(ho[:total], np.concatenate([orc.intersect_sorted(q) for q in qs]), "out of one-list queries")
+
+        # ---- one batch mixing k = 1, 2 and 5 (512-value tiles, with a plan for the wider queries)
+        master = gen.zipf_gaps(rng, 200_000, start=(1 << 32) - 600_000)
+        mixed = []
+        for q in range(60):
+            k = (1, 2, 5)[q % 3]
+            lists = [gen.thin(rng, master, float(rng.choice([0.3, 0.9]))) for _ in range(k)]
+            if q % 7 == 0:
+                lists[0] = np.sort(np.concatenate([lists[0], lists[0][::5]]))   # repeated values
+            mixed.append(lists)
+        cap = sum(min(l.size for l in lists) for lists in mixed)
+        out, off, keep = run(mixed, cap)
+        _lib.check(lib.dgx_lane_sync(lane))
+        ho, hoff = out.cpu().numpy().view(np.uint64), off.cpu().numpy()
+        for qi, lists in enumerate(mixed):
+            eq(ho[int(hoff[qi]): int(hoff[qi + 1])], orc.intersect_sorted(lists), f"mixed batch query {qi} k={len(lists)}")
+
+        # ---- out_cap one short: the sync reports it and nothing lands past out_cap
+        qs = [[one_list(rng, n, "2^32")] for n in (700, 1024, 2500)]
+        total = sum(q[0].size for q in qs)
+        out, off, keep = run(qs, total - 1)
+        assert lib.dgx_lane_sync(lane) == -4  # DGX_ERR_CAP
+        assert (out[total - 1:].cpu() == -1).all(), "a value was written past out_cap"
+
+        # ---- resident-inputs lane: a one-list batch whose list is the previous batch's output on the lane
+        _lib.check(lib.dgx_lane_set_resident_inputs(lane, 1))
+        a, b = gen.thin(rng, master, 0.8), gen.thin(rng, master, 0.7)
+        want = orc.intersect_sorted([a, b])
+        da = torch.from_numpy(np.concatenate([a, np.zeros(2, np.uint64)]).view(np.int64)).to(dev)
+        db = torch.from_numpy(np.concatenate([b, np.zeros(2, np.uint64)]).view(np.int64)).to(dev)
+        garbage = torch.arange(a.size + 8, 0, -1, dtype=torch.int64, device=dev) * 977
+        mid = garbage.clone()
+        mid_off = torch.zeros(2, dtype=torch.int64, device=dev)
+        fin = torch.empty(a.size + 8, dtype=torch.int64, device=dev)
+        fin_off = torch.zeros(2, dtype=torch.int64, device=dev)
+        torch.cuda.synchronize()
+
+        def batch(lists, lens, o, o_off):
+            n = len(lists)
+            _lib.check(lib.dgx_dev_filter_batch(lane, 0, (C.c_void_p * n)(*[t.data_ptr() for t in lists]),
+                                                (C.c_size_t * n)(*lens), (C.c_size_t * 2)(0, n), 1,
+                                                C.c_void_p(o.data_ptr()), a.size, C.c_void_p(o_off.data_ptr())))
+
+        for rep in range(3):
+            if rep:
+                mid.copy_(garbage)
+            batch([da, db], [a.size, b.size], mid, mid_off)
+            batch([mid], [want.size], fin, fin_off)  # the length is known here only because the test knows the answer
+            _lib.check(lib.dgx_lane_sync(lane))
+            eq(fin[: int(fin_off[1].item())].cpu().numpy().view(np.uint64), want, f"intersect -> one-list batch, rep {rep}")
+        _lib.check(lib.dgx_lane_set_resident_inputs(lane, 0))
+        lib.dgx_lane_destroy(lane)
+
+
 # ---- resident-inputs lanes: the pre-pass of batch i+1 under the pipeline kernel of batch i -------------------------
 
 def test_resident_lane_batches(dgx, orc):
