@@ -6,13 +6,17 @@
 // Same idea here, data-parallel:
 //   icw_ranges_*     block b can only match v[j] with base[b] <= v[j] < base[b+1]: the v-range of every
 //                    block (searching the block bases with v, or v with the bases, whichever side is
-//                    shorter).  Blocks with an empty range are never touched again.
+//                    shorter: icw_range_by_v / icw_range_by_block, shared with the rows form).  Blocks with
+//                    an empty range are never touched again.
 //   icw_probe_kernel a warp owns 64 consecutive blocks (as in decode_kernel): per batch of 32 it TMA-copies
 //                    only the delta bytes between the first and last touched block, walks the tags of
 //                    touched blocks, expands each into the warp's shared-memory row and probes it with
 //                    the block's slice of v (or probes that slice with the row when the slice is the
-//                    longer side).  A match sets keep[j]; nothing decoded ever reaches HBM.
+//                    longer side).  A match sets keep[j]; nothing decoded ever reaches HBM.  The walk is
+//                    icw_probe_blocks, shared with the rows form, which differs only in where a match goes.
 //   compact_kernel   o.Uids = v[keep], order preserved, single pass (decoupled look-back).
+// The block format itself (window copy, tag walk, block expansion, lane-serial walk) is read through the helpers
+// of decode_kernel.cuh.
 // Defined, like the reference's own tests (algo/uidlist_test.go:607-681), for duplicate-free inputs.
 #pragma once
 
@@ -30,117 +34,142 @@ struct IcwParams {
     unsigned char* keep;  // per v element: 1 when present in the pack; zero-initialised
 };
 
-// Thread per element of v: the block whose range holds v[j]; run boundaries write vlo / vhi.
+// Element j of v: the block whose range holds v[j]; the first and the last element of a block's run write its
+// vlo / vhi.
+__device__ __forceinline__ void icw_range_by_v(const DPack& pk, const u64* v, u64 m, u64 after, u64 j, u32* vlo,
+                                               u32* vhi) {
+    const u64 x = v[j];
+    if (x < after) return;
+    const long long b = pack_block_of(pk, x);
+    if (b < 0) return;  // before the pack's range
+    long long bp = -2, bn = -2;
+    if (j > 0) { const u64 xp = v[j - 1]; if (xp >= after) bp = pack_block_of(pk, xp); }
+    if (j + 1 < m) bn = pack_block_of(pk, v[j + 1]);
+    if (bp != b) vlo[b] = (u32)j;
+    if (bn != b) vhi[b] = (u32)(j + 1);
+}
+
+// Block b: [lower_bound(v, max(base[b], after)), lower_bound(v, base[b+1])), written when not empty.
+__device__ __forceinline__ void icw_range_by_block(const DPack& pk, const u64* v, u64 m, u64 after, u64 b, u32* vlo,
+                                                   u32* vhi) {
+    const u64 first = pk.base[b];
+    const u64 lo = lower_bound_g(v, m, first > after ? first : after);
+    const u64 hi = (b + 1 < pk.nblocks) ? lower_bound_g(v, m, pk.base[b + 1]) : m;
+    if (hi > lo) { vlo[b] = (u32)lo; vhi[b] = (u32)hi; }
+}
+
 __global__ void __launch_bounds__(256) icw_ranges_by_v_kernel(const IcwParams P) {
     const u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= P.m) return;
-    const u64 x = P.v[j];
-    if (x < P.after) return;
-    const u64 nb = P.pk.nblocks;
-    // block of x: last b with base[b] <= x
-    auto block_of = [&](u64 y) -> long long {
-        u64 lo = 0, hi = nb;  // first b with base[b] > y
-        while (lo < hi) {
-            const u64 mid = lo + ((hi - lo) >> 1);
-            if (ld_probe(P.pk.base + mid) <= y) lo = mid + 1; else hi = mid;
-        }
-        return (long long)lo - 1;
-    };
-    const long long b = block_of(x);
-    if (b < 0) return;
-    long long bp = -2, bn = -2;
-    if (j > 0) { const u64 xp = P.v[j - 1]; if (xp >= P.after) bp = block_of(xp); }
-    if (j + 1 < P.m) bn = block_of(P.v[j + 1]);
-    if (bp != b) P.vlo[b] = (u32)j;
-    if (bn != b) P.vhi[b] = (u32)(j + 1);
+    if (j < P.m) icw_range_by_v(P.pk, P.v, P.m, P.after, j, P.vlo, P.vhi);
 }
 
-// Thread per block: [lower_bound(v, max(base[b], after)), lower_bound(v, base[b+1])).
 __global__ void __launch_bounds__(256) icw_ranges_by_block_kernel(const IcwParams P) {
     const u64 b = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= P.pk.nblocks) return;
-    const u64 first = P.pk.base[b];
-    const u64 lo = lower_bound_g(P.v, P.m, first > P.after ? first : P.after);
-    const u64 hi = (b + 1 < P.pk.nblocks) ? lower_bound_g(P.v, P.m, P.pk.base[b + 1]) : P.m;
-    if (hi > lo) { P.vlo[b] = (u32)lo; P.vhi[b] = (u32)hi; }
+    if (b < P.pk.nblocks) icw_range_by_block(P.pk, P.v, P.m, P.after, b, P.vlo, P.vhi);
 }
 
-// Block i of the warp's batch, its group offsets already in column i of S.goff, expanded into S.stage[0, NumUids):
-// Base, then the 64-bit running sums of its group-varint deltas.  Called by the whole warp.
-__device__ __forceinline__ void icw_expand_block(DWarpSmem& S, int i, u32 ng_i, u64 base_i, int lane) {
-    const u32* pl32 = reinterpret_cast<const u32*>(S.payload);
-    if (lane == 0) S.stage[0] = base_i;
-    u64 carry = 0;
-    for (u32 g0 = 0; g0 < ng_i; g0 += 32) {
-        const u32 g = g0 + lane;
-        u32 d0 = 0, d1 = 0, d2 = 0, d3 = 0;
-        if (g < ng_i) {
-            const u32 off = S.goff[g * D_TSTRIDE + i];
-            const u32 tag = S.payload[off];
-            const u32 a = off + 1;
-            const u32 wb = a >> 2, sh = (a & 3u) * 8u;
-            const u32 w0 = pl32[wb], w1 = pl32[wb + 1], w2 = pl32[wb + 2], w3 = pl32[wb + 3], w4 = pl32[wb + 4];
-            const u32 D0 = __funnelshift_r(w0, w1, sh), D1 = __funnelshift_r(w1, w2, sh);
-            const u32 D2 = __funnelshift_r(w2, w3, sh), D3 = __funnelshift_r(w3, w4, sh);
-            const u32 l0 = (tag & 3u) + 1u, l1 = ((tag >> 2) & 3u) + 1u;
-            const u32 l2 = ((tag >> 4) & 3u) + 1u, l3 = (tag >> 6) + 1u;
-            auto extract = [&](u32 s, u32 l) -> u32 {
-                const u32 wi = s >> 2, sh2 = (s & 3u) * 8u;
-                const u32 lo_ = wi == 0 ? D0 : (wi == 1 ? D1 : (wi == 2 ? D2 : D3));
-                const u32 hi_ = wi == 0 ? D1 : (wi == 1 ? D2 : (wi == 2 ? D3 : 0u));
-                return __funnelshift_r(lo_, hi_, sh2) & (0xffffffffu >> (32u - 8u * l));
-            };
-            d0 = extract(0, l0);
-            d1 = extract(l0, l1);
-            d2 = extract(l0 + l1, l2);
-            d3 = extract(l0 + l1 + l2, l3);
-        }
-        const u64 p1 = d0, p2 = p1 + d1, p3 = p2 + d2, p4 = p3 + d3;
-        u64 inc = p4;
-#pragma unroll
-        for (int dlt = 1; dlt < 32; dlt <<= 1) {
-            u64 t = __shfl_up_sync(0xffffffffu, inc, dlt);
-            if (lane >= dlt) inc += t;
-        }
-        const u64 ex = base_i + carry + inc - p4;
-        if (g < ng_i) {
-            const u32 idx = 1u + 4u * g;
-            S.stage[idx] = ex + p1;
-            S.stage[idx + 1] = ex + p2;
-            S.stage[idx + 2] = ex + p3;
-            S.stage[idx + 3] = ex + p4;
-        }
-        carry += __shfl_sync(0xffffffffu, inc, 31);
+// Where icw_probe_blocks puts a match.  Per batch, batch() reads what each lane's block needs; a block of more than 256
+// uids is walked by its own lane, which reports each match with walk_hit() and ends with walk_done(); any other
+// block is probed by the whole warp between open() and close(), which receives the matches of 32 probes at a time
+// through hit().
+template <class Flag>
+struct IcwKeepSink {  // a match sets keep[j]
+    Flag* keep;
+    __device__ __forceinline__ void batch(u64, bool) {}
+    __device__ __forceinline__ void walk_hit(u64 j, u64) { keep[j] = 1; }
+    __device__ __forceinline__ void walk_done(u64) {}
+    __device__ __forceinline__ void open(int) {}
+    __device__ __forceinline__ void hit(bool h, u64 j, u64) { if (h) keep[j] = 1; }
+    __device__ __forceinline__ void close(u64, int) {}
+};
+struct IcwSlotSink {  // rows form: matches go in ascending order to the block's slot, with a count per block
+    u64* slots;
+    const u64* slot_off;  // the pack's blocks: slot of block b = slots[slot_off[b], slot_off[b+1])
+    u64* cnt;             // the pack's blocks: matches written
+    unsigned below;       // lanes before this one
+    u64 s0, scap;         // the lane's block of the batch
+    u64 s0_i, scap_i;     // the block between open() and close()
+    u64 w;                // matches so far in the block
+    __device__ __forceinline__ void batch(u64 bi, bool touched) {
+        s0 = touched ? slot_off[bi] : 0;
+        scap = touched ? slot_off[bi + 1] - s0 : 0;
+        w = 0;
     }
-    __syncwarp();
+    __device__ __forceinline__ void walk_hit(u64, u64 y) {
+        if (w < scap) slots[s0 + w] = y;
+        ++w;
+    }
+    __device__ __forceinline__ void walk_done(u64 bi) { cnt[bi] = w < scap ? w : scap; }
+    __device__ __forceinline__ void open(int i) {
+        s0_i = __shfl_sync(0xffffffffu, s0, i);
+        scap_i = __shfl_sync(0xffffffffu, scap, i);
+        w = 0;
+    }
+    __device__ __forceinline__ void hit(bool h, u64, u64 x) {
+        const unsigned hm = __ballot_sync(0xffffffffu, h);
+        const u64 k = w + __popc(hm & below);
+        if (h && k < scap_i) slots[s0_i + k] = x;
+        w += __popc(hm);
+    }
+    __device__ __forceinline__ void close(u64 b, int lane) {
+        if (lane == 0) cnt[b] = w < scap_i ? w : scap_i;
+    }
+};
+
+// The block expanded in S.stage[0, n) probed with v[lo, hi) by the whole warp, the shorter side searching the longer
+// one; matches go to the sink 32 probes at a time.
+template <class Sink>
+__device__ __forceinline__ void icw_probe_slice(const DWarpSmem& S, u32 n, const u64* v, u32 lo, u32 hi, Sink& sink,
+                                                int lane) {
+    if (hi - lo <= 4u * n) {
+        for (u32 j0 = lo; j0 < hi; j0 += 32) {
+            const u32 j = j0 + lane;
+            u64 x = 0;
+            bool h = false;
+            if (j < hi) {
+                x = ld_stream(v + j);
+                const int pos = lower_bound_s(S.stage, 0, (int)n, x);
+                h = pos < (int)n && S.stage[pos] == x;
+            }
+            sink.hit(h, j, x);
+        }
+    } else {
+        for (u32 e0 = 0; e0 < n; e0 += 32) {
+            const u32 e = e0 + lane;
+            u64 y = 0, pos = 0;
+            bool h = false;
+            if (e < n) {
+                y = S.stage[e];
+                pos = lo + lower_bound_g(v + lo, (u64)(hi - lo), y);
+                h = pos < hi && ld_probe(v + pos) == y;
+            }
+            sink.hit(h, pos, y);
+        }
+    }
 }
 
-__global__ void __launch_bounds__(D_NT) icw_probe_kernel(const IcwParams P) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    DWarpSmem& S = reinterpret_cast<DWarpSmem*>(smem_raw)[wid];
-    const DPack& pk = P.pk;
-    const u64 gw = (u64)blockIdx.x * D_WARPS + wid;
-    u64 b = gw * D_BPW;
+// One warp probes blocks [b, b + D_BPW) of pk with their v-ranges [vlo, vhi): per batch of 32 blocks, one window
+// copy from the first touched block to the last one that fits, the tag walk of the touched blocks, then each touched
+// block expanded into S.stage and probed, the shorter side searching the longer one.
+template <class Sink>
+__device__ __forceinline__ void icw_probe_blocks(const DPack& pk, const u32* vlo, const u32* vhi, const u64* v, u64 b,
+                                                 Sink& sink, DWarpSmem& S, int lane) {
     const u64 bend = (b + D_BPW < pk.nblocks) ? b + D_BPW : pk.nblocks;
     if (b >= bend) return;
-    const u32 bar = smem_u32(&S.mbar);
-    if (lane == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
+    warp_mbar_init(S, lane);
     u32 parity = 0;
 
     while (b < bend) {
         const u64 bi = b + lane;
         const bool in = bi < bend;
-        const u32 lo = in ? P.vlo[bi] : 0u, hi = in ? P.vhi[bi] : 0u;
-        const unsigned touched = __ballot_sync(0xffffffffu, in && hi > lo);
+        const u32 lo = in ? vlo[bi] : 0u, hi = in ? vhi[bi] : 0u;
+        const bool tch = in && hi > lo;
+        const unsigned touched = __ballot_sync(0xffffffffu, tch);
         if (touched == 0) { b += 32; continue; }  // nothing of v falls into these 32 blocks
         const int f = __ffs(touched) - 1;          // first touched block of the batch
         const u64 doff = in ? pk.delta_off[bi] : 0;
         const u64 dnext = in ? pk.delta_off[bi + 1] : 0;
+        sink.batch(bi, tch);
         const u64 win0 = __shfl_sync(0xffffffffu, doff, f) & ~15ull;
         // blocks f .. l whose bytes fit the window together (l >= f: one block is at most 1088 B at BlockSize 256)
         const bool fits = in && lane >= f && (dnext - win0 <= (u64)D_WB);
@@ -153,29 +182,13 @@ __global__ void __launch_bounds__(D_NT) icw_probe_kernel(const IcwParams P) {
             // Generic slow path (non-reference BlockSize): lane-serial walk of the touched blocks from global
             // memory, every decoded uid binary-searched in the block's slice of v.
             const int r = run ? run : 1;
-            if (in && lane >= f && lane < f + r && hi > lo) {
-                const unsigned char* p = pk.deltas + doff;
-                u64 last = pk.base[bi];
-                u32 produced = 1;
-                auto probe = [&](u64 y) {
-                    const u64 pos = lo + lower_bound_g(P.v + lo, (u64)(hi - lo), y);
-                    if (pos < hi && ld_probe(P.v + pos) == y) P.keep[pos] = 1;
-                };
-                probe(last);
-                while (produced < num) {
-                    const u32 tag = p[0];
-                    const unsigned char* d = p + 1;
-                    for (int j = 0; j < 4 && produced < num; ++j) {
-                        const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
-                        u32 v32 = 0;
-                        for (u32 k = 0; k < l; ++k) v32 |= (u32)d[k] << (8 * k);
-                        d += l;
-                        last += v32;
-                        ++produced;
-                        probe(last);
-                    }
-                    p += gv_bytes_used(tag);
-                }
+            if (tch && lane >= f && lane < f + r) {
+                gv_walk_block(pk.deltas + doff, pk.base[bi], num, [&](u32, u64 y) {
+                    const u64 pos = lo + lower_bound_g(v + lo, (u64)(hi - lo), y);
+                    if (pos < hi && ld_probe(v + pos) == y) sink.walk_hit(pos, y);
+                    return true;
+                });
+                sink.walk_done(bi);
             }
             b += f + r;
             continue;
@@ -186,27 +199,9 @@ __global__ void __launch_bounds__(D_NT) icw_probe_kernel(const IcwParams P) {
         const int last_t = 31 - __clz(want);
         const u64 wend = __shfl_sync(0xffffffffu, dnext, last_t);
         const u64 base = in ? pk.base[bi] : 0;
-        const u32 ngroups = num > 1 ? (num + 2) / 4 : 0;
-
-        const u32 bytes = (u32)(((wend - win0) + 15ull) & ~15ull);
-        if (lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_expect_tx(bar, bytes);
-            tma_bulk_g2s(smem_u32(S.payload), pk.deltas + win0, bytes, bar);
-        }
-        mbar_wait(bar, parity);
-        parity ^= 1u;
-
-        if ((want >> lane) & 1u) {  // tag walk of the touched blocks only
-            u32 off = (u32)(doff - win0);
-            const u32 off_end = (u32)(dnext - win0);
-            for (u32 g = 0; g < ngroups; ++g) {
-                S.goff[g * D_TSTRIDE + lane] = (unsigned short)off;
-                off += gv_bytes_used(S.payload[off]);
-                off = off < off_end ? off : off_end;
-            }
-        }
-        __syncwarp();
+        const u32 ngroups = gv_groups(num);
+        warp_window_load(pk, win0, wend, S, parity, lane);
+        warp_tag_walk(S, (want >> lane) & 1u, doff, dnext, win0, ngroups, lane);  // touched blocks only
 
         for (unsigned rest = want; rest; rest &= rest - 1) {
             const int i = __ffs(rest) - 1;
@@ -214,26 +209,22 @@ __global__ void __launch_bounds__(D_NT) icw_probe_kernel(const IcwParams P) {
             const u64 base_i = __shfl_sync(0xffffffffu, base, i);
             const u32 ng_i = __shfl_sync(0xffffffffu, ngroups, i);
             const u32 lo_i = __shfl_sync(0xffffffffu, lo, i), hi_i = __shfl_sync(0xffffffffu, hi, i);
-            icw_expand_block(S, i, ng_i, base_i, lane);
-            // ---- probe: the shorter side searches the longer one ----------------------------------
-            const u32 cnt = hi_i - lo_i;
-            if (cnt <= 4u * n_i) {
-                for (u32 j = lo_i + lane; j < hi_i; j += 32) {
-                    const u64 x = ld_stream(P.v + j);
-                    const int pos = lower_bound_s(S.stage, 0, (int)n_i, x);
-                    if (pos < (int)n_i && S.stage[pos] == x) P.keep[j] = 1;
-                }
-            } else {
-                for (u32 e = lane; e < n_i; e += 32) {
-                    const u64 y = S.stage[e];
-                    const u64 pos = lo_i + lower_bound_g(P.v + lo_i, (u64)cnt, y);
-                    if (pos < hi_i && ld_probe(P.v + pos) == y) P.keep[pos] = 1;
-                }
-            }
+            sink.open(i);
+            expand_block(S, i, ng_i, base_i, lane);
+            icw_probe_slice(S, n_i, v, lo_i, hi_i, sink, lane);
+            sink.close(b + i, lane);
             __syncwarp();
         }
         b += f + run;
     }
+}
+
+__global__ void __launch_bounds__(D_NT) icw_probe_kernel(const IcwParams P) {
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    DWarpSmem& S = reinterpret_cast<DWarpSmem*>(smem_raw)[wid];
+    IcwKeepSink<unsigned char> sink{P.keep};
+    icw_probe_blocks(P.pk, P.vlo, P.vhi, P.v, ((u64)blockIdx.x * D_WARPS + wid) * D_BPW, sink, S, lane);
 }
 
 // ---- order-preserving compaction of v by keep[] (single pass, decoupled look-back) ------------
@@ -330,56 +321,22 @@ struct IcwRowsParams {
     int* err;
 };
 
-// Last job whose field F is <= x (F ascends over the jobs).
-template <u64 IcwJob::*F>
-__device__ __forceinline__ u32 icw_job_of(const IcwJob* __restrict__ jobs, u32 njobs, u64 x) {
-    u32 lo = 0, hi = njobs;
-    while (hi - lo > 1) {
-        const u32 mid = (lo + hi) >> 1;
-        if (jobs[mid].*F <= x) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 __global__ void __launch_bounds__(256) icw_rows_ranges_kernel(const IcwRowsParams P) {
     const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= P.nthreads) return;
-    const IcwJob& J = P.jobs[icw_job_of<&IcwJob::thr_base>(P.jobs, P.njobs, t)];
+    const IcwJob& J = P.jobs[job_of<IcwJob, &IcwJob::thr_base>(P.jobs, P.njobs, t)];
     const u64 k = t - J.thr_base;
-    const u64 nb = J.pk.nblocks;
-    const u64* base = J.pk.base;
+    const DPack pk = J.pk;  // in registers: the searches read base and nblocks again and again
     u32* vlo = P.vlo + J.blk_base;
     u32* vhi = P.vhi + J.blk_base;
-    if (!J.by_v) {  // thread per block: [lower_bound(v, max(base[b], after)), lower_bound(v, base[b+1]))
-        const u64 first = base[k];
-        const u64 lo = lower_bound_g(P.v, P.m, first > P.after ? first : P.after);
-        const u64 hi = (k + 1 < nb) ? lower_bound_g(P.v, P.m, base[k + 1]) : P.m;
-        if (hi > lo) { vlo[k] = (u32)lo; vhi[k] = (u32)hi; }
-        return;
-    }
-    // thread per element of v: the block whose range holds v[k]; run boundaries write vlo / vhi
-    const u64 x = P.v[k];
-    if (x < P.after || x < base[0]) return;  // before the pack's range
-    auto block_of = [&](u64 y) -> long long {  // last b with base[b] <= y
-        u64 lo = 0, hi = nb;
-        while (lo < hi) {
-            const u64 mid = lo + ((hi - lo) >> 1);
-            if (ld_probe(base + mid) <= y) lo = mid + 1; else hi = mid;
-        }
-        return (long long)lo - 1;
-    };
-    const long long b = block_of(x);
-    long long bp = -2, bn = -2;
-    if (k > 0) { const u64 xp = P.v[k - 1]; if (xp >= P.after) bp = block_of(xp); }
-    if (k + 1 < P.m) bn = block_of(P.v[k + 1]);
-    if (bp != b) vlo[b] = (u32)k;
-    if (bn != b) vhi[b] = (u32)(k + 1);
+    if (J.by_v) icw_range_by_v(pk, P.v, P.m, P.after, k, vlo, vhi);
+    else icw_range_by_block(pk, P.v, P.m, P.after, k, vlo, vhi);
 }
 
 __global__ void __launch_bounds__(256) icw_rows_slots_kernel(const IcwRowsParams P) {
     const u64 fb = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (fb >= P.nblocks) return;
-    const IcwJob& J = P.jobs[icw_job_of<&IcwJob::blk_base>(P.jobs, P.njobs, fb)];
+    const IcwJob& J = P.jobs[job_of<IcwJob, &IcwJob::blk_base>(P.jobs, P.njobs, fb)];
     const u32 lo = P.vlo[fb], hi = P.vhi[fb];
     const u32 num = J.pk.num[fb - J.blk_base];
     const u32 n = hi > lo ? hi - lo : 0u;
@@ -394,151 +351,10 @@ __global__ void __launch_bounds__(D_NT) icw_rows_probe_kernel(const IcwRowsParam
     const u64 gw = (u64)blockIdx.x * D_WARPS + wid;
     // slots beyond the buffer only arise from a pack whose bases do not ascend: nothing is written then
     if (gw >= P.nwarps || P.slot_off[P.nblocks] > P.slots_cap) return;
-    const IcwJob& J = P.jobs[icw_job_of<&IcwJob::warp_base>(P.jobs, P.njobs, gw)];
+    const IcwJob& J = P.jobs[job_of<IcwJob, &IcwJob::warp_base>(P.jobs, P.njobs, gw)];
     const DPack pk = J.pk;
-    const u32* vlo = P.vlo + J.blk_base;
-    const u32* vhi = P.vhi + J.blk_base;
-    const u64* slot_off = P.slot_off + J.blk_base;
-    u64* cnt = P.cnt + J.blk_base;
-    u64 b = (gw - J.warp_base) * D_BPW;
-    const u64 bend = (b + D_BPW < pk.nblocks) ? b + D_BPW : pk.nblocks;
-    const u32 bar = smem_u32(&S.mbar);
-    if (lane == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    u32 parity = 0;
-
-    while (b < bend) {
-        const u64 bi = b + lane;
-        const bool in = bi < bend;
-        const u32 lo = in ? vlo[bi] : 0u, hi = in ? vhi[bi] : 0u;
-        const bool tch = in && hi > lo;
-        const unsigned touched = __ballot_sync(0xffffffffu, tch);
-        if (touched == 0) { b += 32; continue; }
-        const int f = __ffs(touched) - 1;
-        const u64 doff = in ? pk.delta_off[bi] : 0;
-        const u64 dnext = in ? pk.delta_off[bi + 1] : 0;
-        const u64 s0 = tch ? slot_off[bi] : 0;
-        const u64 scap = tch ? slot_off[bi + 1] - s0 : 0;
-        const u64 win0 = __shfl_sync(0xffffffffu, doff, f) & ~15ull;
-        const bool fits = in && lane >= f && (dnext - win0 <= (u64)D_WB);
-        const unsigned fm = __ballot_sync(0xffffffffu, fits) >> f;
-        int run = __ffs(~fm) - 1;
-        if (fm == (0xffffffffu >> f)) run = 32 - f;
-        const u32 num = in ? pk.num[bi] : 0;
-        const bool oversize = run == 0 || (num > 256u && lane >= f && lane < f + (run ? run : 1));
-        if (__any_sync(0xffffffffu, oversize)) {
-            // non-reference BlockSize: lane-serial walk from global memory, matches written in uid order
-            const int r = run ? run : 1;
-            if (tch && lane >= f && lane < f + r) {
-                const unsigned char* p = pk.deltas + doff;
-                u64 last = pk.base[bi];
-                u32 produced = 1;
-                u64 w = 0;
-                auto probe = [&](u64 y) {
-                    const u64 pos = lo + lower_bound_g(P.v + lo, (u64)(hi - lo), y);
-                    if (pos < hi && ld_probe(P.v + pos) == y) {
-                        if (w < scap) P.slots[s0 + w] = y;
-                        ++w;
-                    }
-                };
-                probe(last);
-                while (produced < num) {
-                    const u32 tag = p[0];
-                    const unsigned char* d = p + 1;
-                    for (int j = 0; j < 4 && produced < num; ++j) {
-                        const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
-                        u32 v32 = 0;
-                        for (u32 k = 0; k < l; ++k) v32 |= (u32)d[k] << (8 * k);
-                        d += l;
-                        last += v32;
-                        ++produced;
-                        probe(last);
-                    }
-                    p += gv_bytes_used(tag);
-                }
-                cnt[bi] = w < scap ? w : scap;
-            }
-            b += f + r;
-            continue;
-        }
-        const unsigned in_run = (run >= 32 ? 0xffffffffu : ((1u << run) - 1u)) << f;
-        const unsigned want = touched & in_run;
-        const int last_t = 31 - __clz(want);
-        const u64 wend = __shfl_sync(0xffffffffu, dnext, last_t);
-        const u64 base = in ? pk.base[bi] : 0;
-        const u32 ngroups = num > 1 ? (num + 2) / 4 : 0;
-
-        const u32 bytes = (u32)(((wend - win0) + 15ull) & ~15ull);
-        if (lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_expect_tx(bar, bytes);
-            tma_bulk_g2s(smem_u32(S.payload), pk.deltas + win0, bytes, bar);
-        }
-        mbar_wait(bar, parity);
-        parity ^= 1u;
-
-        if ((want >> lane) & 1u) {
-            u32 off = (u32)(doff - win0);
-            const u32 off_end = (u32)(dnext - win0);
-            for (u32 g = 0; g < ngroups; ++g) {
-                S.goff[g * D_TSTRIDE + lane] = (unsigned short)off;
-                off += gv_bytes_used(S.payload[off]);
-                off = off < off_end ? off : off_end;
-            }
-        }
-        __syncwarp();
-
-        const unsigned below = (1u << lane) - 1u;
-        for (unsigned rest = want; rest; rest &= rest - 1) {
-            const int i = __ffs(rest) - 1;
-            const u32 n_i = __shfl_sync(0xffffffffu, num, i);
-            const u64 base_i = __shfl_sync(0xffffffffu, base, i);
-            const u32 ng_i = __shfl_sync(0xffffffffu, ngroups, i);
-            const u32 lo_i = __shfl_sync(0xffffffffu, lo, i), hi_i = __shfl_sync(0xffffffffu, hi, i);
-            const u64 s0_i = __shfl_sync(0xffffffffu, s0, i), scap_i = __shfl_sync(0xffffffffu, scap, i);
-            icw_expand_block(S, i, ng_i, base_i, lane);
-            // ---- probe, the shorter side searching the longer; hits leave in ascending order -----------
-            u64 w = 0;
-            const u32 c = hi_i - lo_i;
-            if (c <= 4u * n_i) {
-                for (u32 j0 = lo_i; j0 < hi_i; j0 += 32) {
-                    const u32 j = j0 + lane;
-                    u64 x = 0;
-                    bool hit = false;
-                    if (j < hi_i) {
-                        x = ld_stream(P.v + j);
-                        const int pos = lower_bound_s(S.stage, 0, (int)n_i, x);
-                        hit = pos < (int)n_i && S.stage[pos] == x;
-                    }
-                    const unsigned hm = __ballot_sync(0xffffffffu, hit);
-                    const u64 k = w + __popc(hm & below);
-                    if (hit && k < scap_i) P.slots[s0_i + k] = x;
-                    w += __popc(hm);
-                }
-            } else {
-                for (u32 e0 = 0; e0 < n_i; e0 += 32) {
-                    const u32 e = e0 + lane;
-                    u64 y = 0;
-                    bool hit = false;
-                    if (e < n_i) {
-                        y = S.stage[e];
-                        const u64 pos = lo_i + lower_bound_g(P.v + lo_i, (u64)c, y);
-                        hit = pos < hi_i && ld_probe(P.v + pos) == y;
-                    }
-                    const unsigned hm = __ballot_sync(0xffffffffu, hit);
-                    const u64 k = w + __popc(hm & below);
-                    if (hit && k < scap_i) P.slots[s0_i + k] = y;
-                    w += __popc(hm);
-                }
-            }
-            if (lane == 0) cnt[b + i] = w < scap_i ? w : scap_i;
-            __syncwarp();
-        }
-        b += f + run;
-    }
+    IcwSlotSink sink{P.slots, P.slot_off + J.blk_base, P.cnt + J.blk_base, (1u << lane) - 1u};
+    icw_probe_blocks(pk, P.vlo + J.blk_base, P.vhi + J.blk_base, P.v, (gw - J.warp_base) * D_BPW, sink, S, lane);
 }
 
 // Thread t <= nrows writes out_off[t]; warp w moves block w's matches from its slot to their final place.
@@ -601,15 +417,6 @@ struct IcwMatrixParams {
     int* err;
 };
 
-__device__ __forceinline__ long long icw_block_of(const DPack& pk, u64 x) {  // last b with base[b] <= x, or -1
-    u64 lo = 0, hi = pk.nblocks;
-    while (lo < hi) {
-        const u64 mid = lo + ((hi - lo) >> 1);
-        if (ld_probe(pk.base + mid) <= x) lo = mid + 1; else hi = mid;
-    }
-    return (long long)lo - 1;
-}
-
 __global__ void __launch_bounds__(256) icw_mx_locate_kernel(const IcwMatrixParams P) {
     const u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= P.m) return;
@@ -627,7 +434,7 @@ __global__ void __launch_bounds__(256) icw_mx_locate_kernel(const IcwMatrixParam
         atomicOr(P.err, kLaneErrOrder);
     }
     u64 hd = kU64Max;
-    const long long b = icw_block_of(P.pk, x);
+    const long long b = pack_block_of(P.pk, x);
     if (b >= 0 && (k == s || xp < ld_probe(P.pk.base + b))) {  // the row's first element in block b
         const u64 end = (u64)b + 1 < P.pk.nblocks ? k + lower_bound_g(P.v + k, e - k, ld_probe(P.pk.base + b + 1)) : e;
         hd = ((u64)b << 32) | end;
@@ -664,14 +471,10 @@ __global__ void __launch_bounds__(D_NT) icw_mx_probe_kernel(const IcwMatrixParam
     const u64 doff = in ? pk.delta_off[blk] : 0, dnext = in ? pk.delta_off[blk + 1] : 0;
     const u32 num = in ? pk.num[blk] : 0u;
     const u64 base = in ? pk.base[blk] : 0;
-    const u32 ngroups = num > 1 ? (num + 2) / 4 : 0;
+    const u32 ngroups = gv_groups(num);
     const u32 bup = __shfl_up_sync(0xffffffffu, blk, 1);
-    const u32 bar = smem_u32(&S.mbar);
-    if (lane == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
+    IcwKeepSink<u64> sink{P.keep};
+    warp_mbar_init(S, lane);
     u32 parity = 0;
 
     int f = 0;  // lanes [0, f) are done; positions are in block order, so a block's units are adjacent lanes
@@ -685,28 +488,12 @@ __global__ void __launch_bounds__(D_NT) icw_mx_probe_kernel(const IcwMatrixParam
             const u32 bf = __shfl_sync(0xffffffffu, blk, f);
             const unsigned grp = __ballot_sync(0xffffffffu, in && lane >= f && blk == bf);
             if ((grp >> lane) & 1u) {
-                const unsigned char* p = pk.deltas + doff;
-                u64 y = base;
-                u32 produced = 1, q = lo;
-                auto probe = [&](u64 uid) {  // merge step: both sides ascend
+                u32 q = lo;
+                gv_walk_block(pk.deltas + doff, base, num, [&](u32, u64 uid) {  // merge step: both sides ascend
                     while (q < hi && ld_probe(P.v + q) < uid) ++q;
                     if (q < hi && ld_probe(P.v + q) == uid) P.keep[q] = 1;
-                };
-                probe(y);
-                while (produced < num && q < hi) {
-                    const u32 tag = p[0];
-                    const unsigned char* d = p + 1;
-                    for (int j = 0; j < 4 && produced < num; ++j) {
-                        const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
-                        u32 v32 = 0;
-                        for (u32 t = 0; t < l; ++t) v32 |= (u32)d[t] << (8 * t);
-                        d += l;
-                        y += v32;
-                        ++produced;
-                        probe(y);
-                    }
-                    p += gv_bytes_used(tag);
-                }
+                    return q < hi;
+                });
             }
             f += __popc(grp);
             continue;
@@ -716,25 +503,8 @@ __global__ void __launch_bounds__(D_NT) icw_mx_probe_kernel(const IcwMatrixParam
         // one leader per distinct block of the run; it walks the block's tags into its goff column
         const bool lead = mine && (lane == f || bup != blk);
         const unsigned leaders = __ballot_sync(0xffffffffu, lead);
-        const u64 wend = __shfl_sync(0xffffffffu, dnext, rend - 1);
-        const u32 bytes = (u32)(((wend - win0) + 15ull) & ~15ull);
-        if (lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_expect_tx(bar, bytes);
-            if (bytes) tma_bulk_g2s(smem_u32(S.payload), pk.deltas + win0, bytes, bar);
-        }
-        mbar_wait(bar, parity);
-        parity ^= 1u;
-        if (lead) {
-            u32 off = (u32)(doff - win0);
-            const u32 off_end = (u32)(dnext - win0);
-            for (u32 g = 0; g < ngroups; ++g) {
-                S.goff[g * D_TSTRIDE + lane] = (unsigned short)off;
-                off += gv_bytes_used(S.payload[off]);
-                off = off < off_end ? off : off_end;
-            }
-        }
-        __syncwarp();
+        warp_window_load(pk, win0, __shfl_sync(0xffffffffu, dnext, rend - 1), S, parity, lane);
+        warp_tag_walk(S, lead, doff, dnext, win0, ngroups, lane);
 
         for (unsigned rest = leaders; rest; rest &= rest - 1) {
             const int i = __ffs(rest) - 1;
@@ -743,7 +513,7 @@ __global__ void __launch_bounds__(D_NT) icw_mx_probe_kernel(const IcwMatrixParam
             const u32 n_i = __shfl_sync(0xffffffffu, num, i);
             const u64 base_i = __shfl_sync(0xffffffffu, base, i);
             const u32 ng_i = __shfl_sync(0xffffffffu, ngroups, i);
-            icw_expand_block(S, i, ng_i, base_i, lane);
+            expand_block(S, i, ng_i, base_i, lane);
             const bool grp = lane >= i && lane < iend;
             const u32 c = hi - lo;
             if (grp && c <= MX_SERIAL) {  // short units, side by side: each lane searches the block with its own
@@ -757,20 +527,7 @@ __global__ void __launch_bounds__(D_NT) icw_mx_probe_kernel(const IcwMatrixParam
             for (unsigned big = __ballot_sync(0xffffffffu, grp && c > MX_SERIAL); big; big &= big - 1) {
                 const int t = __ffs(big) - 1;
                 const u32 lo_t = __shfl_sync(0xffffffffu, lo, t), hi_t = __shfl_sync(0xffffffffu, hi, t);
-                const u32 c_t = hi_t - lo_t;
-                if (c_t <= 4u * n_i) {
-                    for (u32 j = lo_t + lane; j < hi_t; j += 32) {
-                        const u64 x = ld_stream(P.v + j);
-                        const int pos = lower_bound_s(S.stage, 0, (int)n_i, x);
-                        if (pos < (int)n_i && S.stage[pos] == x) P.keep[j] = 1;
-                    }
-                } else {
-                    for (u32 e = lane; e < n_i; e += 32) {
-                        const u64 y = S.stage[e];
-                        const u64 pos = lo_t + lower_bound_g(P.v + lo_t, (u64)c_t, y);
-                        if (pos < hi_t && ld_probe(P.v + pos) == y) P.keep[pos] = 1;
-                    }
-                }
+                icw_probe_slice(S, n_i, P.v, lo_t, hi_t, sink, lane);
             }
             __syncwarp();  // the next block's expansion overwrites S.stage
         }
@@ -810,25 +567,10 @@ struct SeekParams {
 };
 __device__ __forceinline__ u32 sk_unpack(const DPack& pk, u64 b, u64* out) {  // Decoder.UnpackBlock (:154-200)
     if (b >= pk.nblocks) return 0;
-    const u32 num = pk.num[b];
-    const unsigned char* p = pk.deltas + pk.delta_off[b];
-    u64 last = pk.base[b];
-    u32 produced = 0;
-    if (num) out[produced++] = last; else return 0;
-    while (produced < num) {
-        const u32 tag = p[0];
-        const unsigned char* d = p + 1;
-        for (int j = 0; j < 4 && produced < num; ++j) {
-            const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
-            u32 v = 0;
-            for (u32 k = 0; k < l; ++k) v |= (u32)d[k] << (8 * k);
-            d += l;
-            last += v;
-            out[produced++] = last;
-        }
-        p += gv_bytes_used(tag);
-    }
-    return num;
+    return gv_walk_block(pk.deltas + pk.delta_off[b], pk.base[b], pk.num[b], [&](u32 i, u64 uid) {
+        out[i] = uid;
+        return true;
+    });
 }
 __global__ void pack_seek_kernel(const SeekParams P) {
     if (threadIdx.x != 0 || blockIdx.x != 0) return;

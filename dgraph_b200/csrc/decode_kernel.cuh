@@ -1,9 +1,15 @@
-// decode_kernel.cuh -- group-varint UidPack decode for sm_90a.
+// decode_kernel.cuh -- group-varint UidPack decode for sm_90a, and the block-format helpers every pack reader uses.
 //
 // codec.Decode / Decoder.UnpackBlock (codec/codec.go:154-200, 444-452): block b
 // yields Base, then running sums of its group-varint u32 deltas, truncated to
 // NumUids.  A group is 1 tag byte + 4 little-endian values of 1..4 bytes
 // (go-groupvarint; value j's length-1 in tag bits [2j+1:2j]).
+//
+// The block format is read in this file only; compressed_kernel.cuh calls the same helpers:
+//   gv_walk_block      one thread's walk of one block from global memory (blocks of more than 256 uids, seeks)
+//   pack_block_of      the block whose value range holds x
+//   warp_mbar_init / warp_window_load / warp_tag_walk / expand_block
+//                      the shared-memory path of one warp, below
 //
 // Mapping: a warp owns a run of consecutive blocks and streams it in batches of
 // up to 32 blocks.  Per batch: (1) ONE TMA bulk copy (cp.async.bulk + mbarrier)
@@ -47,6 +53,54 @@ struct DSeek {            // written by decode_seek_kernel
 __device__ __forceinline__ u32 gv_bytes_used(u32 t) {
     return 5u + (t & 3u) + ((t >> 2) & 3u) + ((t >> 4) & 3u) + (t >> 6);
 }
+// groups of a block of num uids: ceil((num-1)/4) carry data
+__device__ __forceinline__ u32 gv_groups(u32 num) { return num > 1 ? (num + 2) / 4 : 0; }
+
+// One block walked by one thread straight from global memory, from its Base `last`, NumUids `num` and delta bytes p:
+// fn(i, uid) for Base (i = 0), then for every running sum, i < num.  The sum is 64-bit like the reference's
+// `last + uint64(delta)` (codec.go:191-196): packs produced by the Encoder never carry more than 2^32 per block,
+// hand-built ones may.  fn returns false to stop.  Returns num.  (The callers pass what they have already loaded:
+// reloading it here costs decode_batch_kernel registers.)
+template <class Fn>
+__device__ __forceinline__ u32 gv_walk_block(const unsigned char* p, u64 last, u32 num, Fn&& fn) {
+    if (num == 0 || !fn(0u, last)) return num;
+    u32 produced = 1;
+    while (produced < num) {
+        const u32 tag = p[0];
+        const unsigned char* d = p + 1;
+        for (int j = 0; j < 4 && produced < num; ++j) {
+            const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
+            u32 v = 0;
+            for (u32 k = 0; k < l; ++k) v |= (u32)d[k] << (8 * k);
+            d += l;
+            last += v;
+            if (!fn(produced++, last)) return num;
+        }
+        p += gv_bytes_used(tag);
+    }
+    return num;
+}
+
+// Last block b with base[b] <= x, or -1 when x is below the first block.
+__device__ __forceinline__ long long pack_block_of(const DPack& pk, u64 x) {
+    u64 lo = 0, hi = pk.nblocks;  // first b with base[b] > x
+    while (lo < hi) {
+        const u64 mid = lo + ((hi - lo) >> 1);
+        if (ld_probe(pk.base + mid) <= x) lo = mid + 1; else hi = mid;
+    }
+    return (long long)lo - 1;
+}
+
+// Last job whose field F is <= x (F ascends over the jobs).
+template <class Job, u64 Job::*F>
+__device__ __forceinline__ u32 job_of(const Job* __restrict__ jobs, u32 njobs, u64 x) {
+    u32 lo = 0, hi = njobs;
+    while (hi - lo > 1) {
+        const u32 mid = (lo + hi) >> 1;
+        if (jobs[mid].*F <= x) lo = mid; else hi = mid;
+    }
+    return lo;
+}
 
 // Decoder.Seek(seek, SeekStart), codec/codec.go:279-337, restated for one thread.
 __global__ void decode_seek_kernel(const DPack pk, u64 seek, DSeek* out, u64* out_len_word, u64 out_cap, int* err) {
@@ -61,24 +115,11 @@ __global__ void decode_seek_kernel(const DPack pk, u64 seek, DSeek* out, u64* ou
             first = idx;
         } else {
             const u64 b = idx - 1;  // unpack the previous block, count uids < seek
-            const u32 num = pk.num[b];
-            const unsigned char* p = pk.deltas + pk.delta_off[b];
-            u64 last = pk.base[b];
-            u32 produced = 1, below = last < seek ? 1u : 0u;
-            while (produced < num) {
-                const u32 tag = p[0];
-                const unsigned char* d = p + 1;
-                for (int j = 0; j < 4 && produced < num; ++j) {
-                    const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
-                    u32 v = 0;
-                    for (u32 k = 0; k < l; ++k) v |= (u32)d[k] << (8 * k);
-                    d += l;
-                    last += v;
-                    ++produced;
-                    if (last < seek) ++below;
-                }
-                p += gv_bytes_used(tag);
-            }
+            u32 below = 0;
+            const u32 num = gv_walk_block(pk.deltas + pk.delta_off[b], pk.base[b], pk.num[b], [&](u32, u64 uid) {
+                below += uid < seek;
+                return true;
+            });
             if (below < num) { first = b; trim = below; }
             else { first = idx; }  // Next(): nothing >= seek in that block
         }
@@ -141,19 +182,108 @@ struct __align__(128) DWarpSmem {
     u64 mbar;
 };
 
+// ---- one warp's shared-memory path over a batch of blocks; every helper is called by the whole warp -----------
+
+__device__ __forceinline__ void warp_mbar_init(DWarpSmem& S, int lane) {
+    if (lane == 0) {
+        mbar_init(smem_u32(&S.mbar), 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+}
+
+// TMA bulk copy of delta bytes [win0, wend) of pk, win0 16-byte aligned, into S.payload (rounded up to 16 bytes);
+// returns when they are there.  parity is the phase of S.mbar the copy completes and flips with every copy.
+__device__ __forceinline__ void warp_window_load(const DPack& pk, u64 win0, u64 wend, DWarpSmem& S, u32& parity,
+                                                 int lane) {
+    const u32 bytes = (u32)(((wend - win0) + 15ull) & ~15ull);
+    const u32 bar = smem_u32(&S.mbar);
+    if (lane == 0) {
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        mbar_expect_tx(bar, bytes);
+        if (bytes) tma_bulk_g2s(smem_u32(S.payload), pk.deltas + win0, bytes, bar);  // blocks of one uid have none
+    }
+    mbar_wait(bar, parity);
+    parity ^= 1u;
+}
+
+// Every lane with `walk` set records the payload offsets of its block's ngroups groups in column `lane` of S.goff;
+// the block's delta bytes are [doff, dnext) of the pack, in the window that starts at win0.  A corrupt tag may claim
+// more bytes than the block holds: the walk stops at the block's end (the reference zero-pads a short tail,
+// codec.go:176-188; here the next block's bytes are read instead -- garbage in, garbage out, but never outside the
+// window).
+__device__ __forceinline__ void warp_tag_walk(DWarpSmem& S, bool walk, u64 doff, u64 dnext, u64 win0, u32 ngroups,
+                                              int lane) {
+    if (walk) {
+        u32 off = (u32)(doff - win0);
+        const u32 off_end = (u32)(dnext - win0);
+        for (u32 g = 0; g < ngroups; ++g) {
+            S.goff[g * D_TSTRIDE + lane] = (unsigned short)off;
+            off += gv_bytes_used(S.payload[off]);
+            off = off < off_end ? off : off_end;
+        }
+    }
+    __syncwarp();
+}
+
+// Block i of the batch, its ng_i group offsets in column i of S.goff, expanded into S.stage[0, NumUids): Base, then
+// the running sums of its deltas -- lane g decodes group g (unaligned 16-byte read, four extractions), and a 64-bit
+// warp prefix sum (`last + uint64(delta)`, codec.go:191-196) carries the sums across lanes and rounds of 32 groups.
+__device__ __forceinline__ void expand_block(DWarpSmem& S, int i, u32 ng_i, u64 base_i, int lane) {
+    const u32* pl32 = reinterpret_cast<const u32*>(S.payload);
+    if (lane == 0) S.stage[0] = base_i;
+    u64 carry = 0;
+    for (u32 g0 = 0; g0 < ng_i; g0 += 32) {
+        const u32 g = g0 + lane;
+        u32 d0 = 0, d1 = 0, d2 = 0, d3 = 0;
+        if (g < ng_i) {
+            const u32 off = S.goff[g * D_TSTRIDE + i];
+            const u32 tag = S.payload[off];
+            const u32 a = off + 1;
+            const u32 wb = a >> 2, sh = (a & 3u) * 8u;
+            const u32 w0 = pl32[wb], w1 = pl32[wb + 1], w2 = pl32[wb + 2], w3 = pl32[wb + 3], w4 = pl32[wb + 4];
+            const u32 D0 = __funnelshift_r(w0, w1, sh), D1 = __funnelshift_r(w1, w2, sh);
+            const u32 D2 = __funnelshift_r(w2, w3, sh), D3 = __funnelshift_r(w3, w4, sh);
+            const u32 l0 = (tag & 3u) + 1u, l1 = ((tag >> 2) & 3u) + 1u;
+            const u32 l2 = ((tag >> 4) & 3u) + 1u, l3 = (tag >> 6) + 1u;
+            auto extract = [&](u32 s, u32 l) -> u32 {
+                const u32 wi = s >> 2, sh2 = (s & 3u) * 8u;
+                const u32 lo = wi == 0 ? D0 : (wi == 1 ? D1 : (wi == 2 ? D2 : D3));
+                const u32 hi = wi == 0 ? D1 : (wi == 1 ? D2 : (wi == 2 ? D3 : 0u));
+                return __funnelshift_r(lo, hi, sh2) & (0xffffffffu >> (32u - 8u * l));
+            };
+            d0 = extract(0, l0);
+            d1 = extract(l0, l1);
+            d2 = extract(l0 + l1, l2);
+            d3 = extract(l0 + l1 + l2, l3);
+        }
+        const u64 p1 = d0, p2 = p1 + d1, p3 = p2 + d2, p4 = p3 + d3;
+        u64 inc = p4;
+#pragma unroll
+        for (int dlt = 1; dlt < 32; dlt <<= 1) {
+            u64 t = __shfl_up_sync(0xffffffffu, inc, dlt);
+            if (lane >= dlt) inc += t;
+        }
+        const u64 ex = base_i + carry + inc - p4;
+        if (g < ng_i) {
+            const u32 idx = 1u + 4u * g;  // uid index of this group's first value
+            S.stage[idx] = ex + p1;
+            S.stage[idx + 1] = ex + p2;
+            S.stage[idx + 2] = ex + p3;
+            S.stage[idx + 3] = ex + p4;
+        }
+        carry += __shfl_sync(0xffffffffu, inc, 31);
+    }
+    __syncwarp();
+}
+
 // One warp decodes blocks [first_block + gw*D_BPW, +D_BPW) of `pk` into out[uid_off - skip ...].
 __device__ __forceinline__ void decode_warp_run(const DPack& pk, u64 first_block, u64 skip, u64* __restrict__ out,
                                                 u64 gw, DWarpSmem& S, int lane) {
     u64 b = first_block + gw * D_BPW;
     const u64 bend = (b + D_BPW < pk.nblocks) ? b + D_BPW : pk.nblocks;
     if (b >= bend) return;  // whole warp
-
-    const u32 bar = smem_u32(&S.mbar);
-    if (lane == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
+    warp_mbar_init(S, lane);
     u32 parity = 0;
 
     while (b < bend) {
@@ -173,44 +303,27 @@ __device__ __forceinline__ void decode_warp_run(const DPack& pk, u64 first_block
         const u32 num = in ? pk.num[bi] : 0;
         const u64 base = in ? pk.base[bi] : 0;
         const u64 uoff = in ? pk.uid_off[bi] : 0;
-        const u32 ngroups = num > 1 ? (num + 2) / 4 : 0;  // ceil((num-1)/4) groups carry data
+        const u32 ngroups = gv_groups(num);
 
         const bool oversize = (wend - win0 > (u64)D_WB) || (num > 256u && lane < nb);
         if (__any_sync(0xffffffffu, oversize)) {
             // Generic slow path (BlockSize > 256 packs): lane-serial decode straight from
             // global memory, one block per lane.  Never taken at the reference's BlockSize 256.
-            if (lane < nb && in) {
-                const unsigned char* p = pk.deltas + doff;
-                u64 last = base;
-                u64 gi = uoff;
-                if (gi >= skip) st_stream(out + (gi - skip), last);
-                u32 produced = 1;
-                while (produced < num) {
-                    const u32 tag = p[0];
-                    const unsigned char* d = p + 1;
-                    for (int j = 0; j < 4 && produced < num; ++j) {
-                        const u32 l = ((tag >> (2 * j)) & 3u) + 1u;
-                        u32 v = 0;
-                        for (u32 k = 0; k < l; ++k) v |= (u32)d[k] << (8 * k);
-                        d += l;
-                        last += v;
-                        gi = uoff + produced;
-                        if (gi >= skip) st_stream(out + (gi - skip), last);
-                        ++produced;
-                    }
-                    p += gv_bytes_used(tag);
-                }
-            }
+            if (lane < nb && in)
+                gv_walk_block(pk.deltas + doff, base, num, [&](u32 i, u64 uid) {
+                    if (uoff + i >= skip) st_stream(out + (uoff + i - skip), uid);
+                    return true;
+                });
             b += nb;
             continue;
         }
 
         // ---- (1) TMA bulk copy of the batch's delta bytes ------------------------
-        const u32 bytes = (u32)(((wend - win0) + 15ull) & ~15ull);
         if (pk.sysmem) {
             // Zero-copy: the pack's bytes are read straight from pinned host memory by the lanes (16 bytes each,
             // all requests of the window in flight together); thousands of resident warps keep PCIe full without
             // the per-copy set-up a DMA of every small pack costs, and nothing compressed is staged in HBM.
+            const u32 bytes = (u32)(((wend - win0) + 15ull) & ~15ull);
             const uint4* src = reinterpret_cast<const uint4*>(pk.deltas + win0);
             uint4* dstw = reinterpret_cast<uint4*>(S.payload);
             for (u32 o = lane; o < bytes / 16u; o += 32) {
@@ -221,83 +334,19 @@ __device__ __forceinline__ void decode_warp_run(const DPack& pk, u64 first_block
             }
             __syncwarp();
         } else {
-            if (lane == 0) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                mbar_expect_tx(bar, bytes);
-                tma_bulk_g2s(smem_u32(S.payload), pk.deltas + win0, bytes, bar);
-            }
-            mbar_wait(bar, parity);
-            parity ^= 1u;
+            warp_window_load(pk, win0, wend, S, parity, lane);
         }
 
         // ---- (2) tag walk: lane i records the byte offset of every group of block i
-        if (lane < nb) {
-            // a corrupt tag may claim more bytes than the block holds: the walk stops at the block's
-            // end (the reference zero-pads a short tail, codec.go:176-188; here the next block's
-            // bytes are read instead -- garbage in, garbage out, but never outside the window)
-            u32 off = (u32)(doff - win0);
-            const u32 off_end = (u32)(dnext - win0);
-            for (u32 g = 0; g < ngroups; ++g) {
-                S.goff[g * D_TSTRIDE + lane] = (unsigned short)off;
-                off += gv_bytes_used(S.payload[off]);
-                off = off < off_end ? off : off_end;
-            }
-        }
-        __syncwarp();
+        warp_tag_walk(S, lane < nb, doff, dnext, win0, ngroups, lane);
 
         // ---- (3) cooperative decode, block by block --------------------------------
-        const u32* pl32 = reinterpret_cast<const u32*>(S.payload);
         for (int i = 0; i < nb; ++i) {
             const u32 n_i = __shfl_sync(0xffffffffu, num, i);
             const u64 base_i = __shfl_sync(0xffffffffu, base, i);
             const u64 uoff_i = __shfl_sync(0xffffffffu, uoff, i);
             const u32 ng_i = __shfl_sync(0xffffffffu, ngroups, i);
-            if (lane == 0) S.stage[0] = base_i;
-            u64 carry = 0;
-            for (u32 g0 = 0; g0 < ng_i; g0 += 32) {
-                const u32 g = g0 + lane;
-                u32 d0 = 0, d1 = 0, d2 = 0, d3 = 0;
-                if (g < ng_i) {
-                    const u32 off = S.goff[g * D_TSTRIDE + i];
-                    const u32 tag = S.payload[off];
-                    const u32 a = off + 1;
-                    const u32 wb = a >> 2, sh = (a & 3u) * 8u;
-                    const u32 w0 = pl32[wb], w1 = pl32[wb + 1], w2 = pl32[wb + 2], w3 = pl32[wb + 3], w4 = pl32[wb + 4];
-                    const u32 D0 = __funnelshift_r(w0, w1, sh), D1 = __funnelshift_r(w1, w2, sh);
-                    const u32 D2 = __funnelshift_r(w2, w3, sh), D3 = __funnelshift_r(w3, w4, sh);
-                    const u32 l0 = (tag & 3u) + 1u, l1 = ((tag >> 2) & 3u) + 1u;
-                    const u32 l2 = ((tag >> 4) & 3u) + 1u, l3 = (tag >> 6) + 1u;
-                    auto extract = [&](u32 s, u32 l) -> u32 {
-                        const u32 wi = s >> 2, sh2 = (s & 3u) * 8u;
-                        const u32 lo = wi == 0 ? D0 : (wi == 1 ? D1 : (wi == 2 ? D2 : D3));
-                        const u32 hi = wi == 0 ? D1 : (wi == 1 ? D2 : (wi == 2 ? D3 : 0u));
-                        return __funnelshift_r(lo, hi, sh2) & (0xffffffffu >> (32u - 8u * l));
-                    };
-                    d0 = extract(0, l0);
-                    d1 = extract(l0, l1);
-                    d2 = extract(l0 + l1, l2);
-                    d3 = extract(l0 + l1 + l2, l3);
-                }
-                // running sums are 64-bit like the reference's `last + uint64(delta)` (codec.go:191-196):
-                // packs produced by the Encoder never carry more than 2^32 per block, hand-built ones may
-                const u64 p1 = d0, p2 = p1 + d1, p3 = p2 + d2, p4 = p3 + d3;
-                u64 inc = p4;
-#pragma unroll
-                for (int dlt = 1; dlt < 32; dlt <<= 1) {
-                    u64 t = __shfl_up_sync(0xffffffffu, inc, dlt);
-                    if (lane >= dlt) inc += t;
-                }
-                const u64 ex = base_i + carry + inc - p4;
-                if (g < ng_i) {
-                    const u32 idx = 1u + 4u * g;  // uid index of this group's first value
-                    S.stage[idx] = ex + p1;
-                    S.stage[idx + 1] = ex + p2;
-                    S.stage[idx + 2] = ex + p3;
-                    S.stage[idx + 3] = ex + p4;
-                }
-                carry += __shfl_sync(0xffffffffu, inc, 31);
-            }
-            __syncwarp();
+            expand_block(S, i, ng_i, base_i, lane);
             // coalesced write-out of uids [e0, n_i) of the block
             const u64 e0 = skip > uoff_i ? skip - uoff_i : 0;  // trimmed head (first block only)
             if (e0 < (u64)n_i) {
@@ -340,13 +389,9 @@ __global__ void __launch_bounds__(D_NT) decode_batch_kernel(const DJob* __restri
     DWarpSmem& S = reinterpret_cast<DWarpSmem*>(smem_raw)[wid];
     const u64 gw = (u64)blockIdx.x * D_WARPS + wid;
     if (gw >= nwarps) return;
-    u32 lo = 0, hi = njobs;  // last job with warp_base <= gw
-    while (hi - lo > 1) {
-        const u32 mid = (lo + hi) >> 1;
-        if (jobs[mid].warp_base <= gw) lo = mid; else hi = mid;
-    }
-    const DPack pk = jobs[lo].pk;
-    decode_warp_run(pk, 0, 0, jobs[lo].out, gw - jobs[lo].warp_base, S, lane);
+    const u32 j = job_of<DJob, &DJob::warp_base>(jobs, njobs, gw);
+    const DPack pk = jobs[j].pk;
+    decode_warp_run(pk, 0, 0, jobs[j].out, gw - jobs[j].warp_base, S, lane);
 }
 
 }  // namespace dgx
