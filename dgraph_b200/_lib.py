@@ -107,6 +107,7 @@ SYMBOLS = {
     "dgx_dev_intersect_compressed_matrix": (_int, [_vp, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_merge_sorted_matrix": (_int, [_vp, _vp, _vp, _sz, _sz, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),
+    "dgx_filter_tail_queries": (_u64, [_vp]),
     "dgx_wire_posting_list_pack": (_int, [_vp, _sz, C.POINTER(_vp), _szp]),
     "dgx_wire_pack_measure": (_int, [_vp, _sz, _szp, _szp]),
     "dgx_wire_pack_parse": (_int, [_vp, _sz, _vp, _vp, _vp, _vp, _sz, _sz, C.POINTER(PackView)]),

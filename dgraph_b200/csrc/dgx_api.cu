@@ -72,6 +72,7 @@ struct Stats {
 };
 static Stats g_stats;
 static std::atomic<uint64_t> g_xm_overflows{0};  // chunks of dgx_*merge_sorted_matrix sorted in global memory
+static std::atomic<uint64_t> g_tail_queries{0};  // filter queries whose sparse tail filter_tail_kernel served
 static std::mutex g_mu;
 static int g_device = -1;
 static std::vector<dgx_lane*> g_pool;  // idle lanes for the host-pointer entry points
@@ -183,6 +184,7 @@ struct dgx_lane {
     uint64_t* h_head = nullptr;  // pinned landing zone for the head of a result (kSpecHead values)
     uint64_t launches = 0;
     uint64_t xm_overflows = 0;  // overflow-path chunks of the matrix merges this lane ran, as of its last sync
+    uint64_t tail_queries = 0;  // filter queries with deferred lists this lane ran, as of its last sync
     // "resident lists" mode (dgx_lane_set_resident_inputs): the plan pre-pass of batch i+1 runs on a side stream while
     // the pipeline kernel of batch i is still running; its tables live in two alternating workspaces
     bool resident_inputs = false;
@@ -425,7 +427,8 @@ extern "C" uint64_t dgx_lane_launches(const dgx_lane* l) { return l ? l->launche
 extern "C" int dgx_lane_sync(dgx_lane* l) {
     if (!l) return fail(DGX_ERR_ARG, "null lane");
     CK(cudaSetDevice(l->device));
-    CK(cudaMemcpyAsync(l->h_err, l->d_err, (kLaneOverflowWord + 1) * sizeof(u32), cudaMemcpyDeviceToHost, l->stream));
+    static_assert(kLaneTailWord == kLaneOverflowWord + 1, "the lane's counter words are read back in one copy");
+    CK(cudaMemcpyAsync(l->h_err, l->d_err, (kLaneTailWord + 1) * sizeof(u32), cudaMemcpyDeviceToHost, l->stream));
     CK(cudaStreamSynchronize(l->stream));
     l->host.reset();
     l->ws.release_retired();
@@ -435,6 +438,11 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
         l->xm_overflows += ovf;
         g_xm_overflows += ovf;
         CK(cudaMemsetAsync(reinterpret_cast<u32*>(l->d_err) + kLaneOverflowWord, 0, sizeof(u32), l->stream));
+    }
+    if (const u32 tq = reinterpret_cast<const u32*>(l->h_err)[kLaneTailWord]) {
+        l->tail_queries += tq;
+        g_tail_queries += tq;
+        CK(cudaMemsetAsync(reinterpret_cast<u32*>(l->d_err) + kLaneTailWord, 0, sizeof(u32), l->stream));
     }
     if (const int flag = *l->h_err) {
         *l->h_err = 0;
@@ -492,8 +500,9 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
     if (rc) return rc;
     FTask* ht = (FTask*)h_raw;
     FList* hl = (FList*)((char*)h_raw + tasks_b);
-    uint64_t ntiles = 0, uids_in = 0;
+    uint64_t ntiles = 0, uids_in = 0, mid_cap = 0;
     size_t li = 0, kmax = 1;
+    bool sample_any = false;
     for (size_t q = 0; q < nq; ++q) kmax = std::max(kmax, k_off[q + 1] - k_off[q]);
     // 1- and 2-list batches: 1024-value tiles (per-tile overheads over twice the values); wider queries: 512 (filter_pipe.cuh)
     const int pipe_va = kmax <= 2 ? 4 : 2;
@@ -521,14 +530,26 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
         }
         const uint64_t lenA = lists[order[0]].len;
         ntiles += std::max<uint64_t>(1, (lenA + tile_sz - 1) / tile_sz);
+        mid_cap += lenA;
+        sample_any |= k >= 3 && lenA >= P_SAMPLE_MIN_A;
     }
     if (ntiles > 0x7fffffffull) return fail(DGX_ERR_ARG, "batch too large (%llu tiles)", (unsigned long long)ntiles);
-    const size_t status_b = ntiles * sizeof(u64) + 64;
+    const bool ahead = l->resident_inputs && l->side;
+    // Intersections of 3+ lists on a resident-inputs lane, where the pre-pass runs under the previous batch's
+    // pipeline, are sampled and may defer their sparse tail to filter_tail_kernel (filter_pipe.cuh).  Elsewhere
+    // the sample would sit on the call's critical path, and driving lists under P_SAMPLE_MIN_A values (an upper
+    // bound here; the sample checks the exact length) are not worth sampling.
+    const bool deep = op == DGX_OP_INTERSECT && ahead && sample_any;
+    // zeroed per batch: pipeline status words | 64 B (pipeline ticket, deferral word, tail ticket) | deep batches:
+    // tail status words, the sample's hit words (P_SAMPLES per query) and its per-query CTA counts
+    const uint64_t tail_chunks = mid_cap / P_TAIL_NT + 1;
+    if (deep && tail_chunks > 0xffffffffull) return fail(DGX_ERR_ARG, "batch too large (%llu values)", (unsigned long long)mid_cap);
+    const size_t sample_b = nq * (P_SAMPLES + 1) * sizeof(u32);
+    const size_t status_b = ntiles * sizeof(u64) + 64 + (deep ? tail_chunks * sizeof(u64) + sample_b : 0);
     // Where the batch's tables live and which stream prepares them.  Normally: the lane's workspace and stream.
     // Resident-inputs lanes: one of two alternating workspaces and the side stream -- descriptor copies, status
     // reset and the plan pre-pass of THIS batch then run while the pipeline kernel of the PREVIOUS batch is still
     // busy (the lists are immutable, so the pre-pass depends on nothing the main stream has queued).
-    const bool ahead = l->resident_inputs && l->side;
     const int slot = l->fslot;
     DevArena* ar = &l->ws;
     cudaStream_t pre = l->stream;
@@ -563,6 +584,26 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
     P.status = (u64*)d_status;
     P.ticket = (u32*)(d_status + ntiles * sizeof(u64));
     P.err = l->d_err;
+    u32* d_defer = P.ticket + 1;
+    u32* d_tail_ticket = P.ticket + 2;
+    u64* d_tail_status = (u64*)(d_status + ntiles * sizeof(u64) + 64);
+    u32* d_hits = (u32*)(d_tail_status + (deep ? tail_chunks : 0));
+    u32* d_done = d_hits + nq * P_SAMPLES;
+    // ---- stream depth per query (deep batches): k_eff words, the intermediate and its offsets --------
+    void *d_keff = nullptr, *d_mid = nullptr, *d_mid_off = nullptr;
+    if (deep) {
+        rc = ar->alloc(nq * sizeof(u32), &d_keff);
+        if (rc) return rc;
+        rc = ar->alloc(std::max<uint64_t>(mid_cap, 1) * sizeof(u64), &d_mid);
+        if (rc) return rc;
+        rc = ar->alloc((nq + 1) * sizeof(u64), &d_mid_off);
+        if (rc) return rc;
+        const dim3 sgrid((unsigned)nq, (unsigned)std::min<size_t>(kmax - 2, P_SAMPLE_LISTS));
+        filter_sample_kernel<<<sgrid, P_SAMPLES, 0, pre>>>(P.tasks, P.lists, d_hits, d_done, (u32*)d_keff, d_defer);
+        CK(cudaGetLastError());
+        l->launches += 1;
+        g_stats.launches += 1;
+    }
     // ---- plan pre-pass + persistent TMA pipeline (filter_pipe_kernel) ----------------
     void* hp_raw;
     rc = l->host.alloc(nq * sizeof(u64), &hp_raw);
@@ -583,7 +624,8 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
     if (rc) return rc;
     CK(cudaMemcpyAsync(d_pb, h_pb, nq * sizeof(u64), cudaMemcpyHostToDevice, pre));
     filter_tiles_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, pre>>>(P.tasks, P.lists, (const u64*)d_pb, P.ntasks,
-                                                                           P.ntiles, (PTileEntry*)d_tiles, (u32)tile_sz);
+                                                                           P.ntiles, (PTileEntry*)d_tiles, (u32)tile_sz,
+                                                                           (const u32*)d_keff);
     CK(cudaGetLastError());
     l->launches += 1;
     g_stats.launches += 1;
@@ -591,7 +633,7 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
         const u64 blocks = (npairs + 255) / 256;
         if (blocks > 0x7fffffffull) return fail(DGX_ERR_ARG, "batch too large");
         filter_plan_kernel<<<(unsigned)blocks, 256, 0, pre>>>(P.tasks, P.lists, (const u64*)d_pb, P.ntasks, npairs,
-                                                              (PPlanEntry*)d_plan, (u32)tile_sz);
+                                                              (PPlanEntry*)d_plan, (u32)tile_sz, (const u32*)d_keff);
         CK(cudaGetLastError());
         l->launches += 1;
         g_stats.launches += 1;
@@ -601,6 +643,10 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
     PP.plan_base = (const u64*)d_pb;
     PP.plan = (const PPlanEntry*)d_plan;
     PP.tiles = (const PTileEntry*)d_tiles;
+    PP.defer = deep ? d_defer : nullptr;
+    PP.mid = (u64*)d_mid;
+    PP.mid_off = (u64*)d_mid_off;
+    PP.mid_cap = mid_cap;
     // wide queries: one tile per ticket keeps the look-back order tight; 2-list batches have tiny tiles and
     // amortise the metadata chain over two
     PP.grp = kmax >= 4 ? 1u : 2u;
@@ -627,6 +673,29 @@ static int filter_batch_impl(dgx_lane* l, int op, const ListDesc* lists, const s
     CK(cudaGetLastError());
     l->launches += 1;
     g_stats.launches += 1;
+    if (deep) {  // exits at once unless the sample deferred some query
+        PTailParams T;
+        T.tasks = P.tasks;
+        T.lists = P.lists;
+        T.ntasks = P.ntasks;
+        T.keff = (const u32*)d_keff;
+        T.defer = d_defer;
+        T.mid = (const u64*)d_mid;
+        T.mid_off = (const u64*)d_mid_off;
+        T.out = P.out;
+        T.out_cap = P.out_cap;
+        T.out_off = P.out_off;
+        T.status = d_tail_status;
+        T.ticket = d_tail_ticket;
+        T.err = l->d_err;
+        T.tail_queries = (u32*)l->d_err + kLaneTailWord;
+        const u64 ctas = std::min<u64>((u64)g_num_sms * (2048 / P_TAIL_NT), tail_chunks);
+        filter_tail_kernel<<<(unsigned)ctas, P_TAIL_NT, 0, l->stream>>>(T);
+        CK(cudaGetLastError());
+        l->launches += 1;
+        g_stats.launches += 1;
+    }
+    // the tail reads this workspace too: the pre-pass that reuses it waits for both
     if (ahead) CK(cudaEventRecord(l->ev_pipe[slot], l->stream));
     g_stats.uids_in += uids_in;
     return DGX_OK;
@@ -2620,6 +2689,7 @@ extern "C" int dgx_merge_sorted_matrix(const uint64_t* v, const uint64_t* v_off,
 }
 
 extern "C" uint64_t dgx_merge_matrix_overflows(const dgx_lane* l) { return l ? l->xm_overflows : g_xm_overflows.load(); }
+extern "C" uint64_t dgx_filter_tail_queries(const dgx_lane* l) { return l ? l->tail_queries : g_tail_queries.load(); }
 
 // ---------------------------------------------------------------------------
 // protobuf wire-format adjacency (host only; see include/dgx.h and wire.hpp)

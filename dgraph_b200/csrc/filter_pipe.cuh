@@ -30,6 +30,21 @@
 // Lists that are not pre-staged (slice larger than the stage, or more than 8
 // filter lists) are binary-searched in HBM by the surviving candidates.  A query
 // of one list (k = 1) has no plan entries and its tiles are copied through.
+//
+// Intersections of k >= 3 lists add two kernels around that chain:
+//   filter_sample_kernel one CTA per (query, filter list), first in the pre-pass: 256 evenly
+//                        spaced driving values are searched in the filter lists; after the
+//                        first list that leaves fewer than 1/32 of them alive (hits in every
+//                        list so far) the query's remaining lists are DEFERRED.  k_eff (lists
+//                        streamed, A included) goes into the tile table.
+// Both run only on resident-inputs lanes, where the pre-pass is hidden under the previous
+// batch's pipeline; elsewhere the sample would sit on the call's critical path.
+//   filter_tail_kernel   after the pipeline, which then writes the survivors of its k_eff
+//                        lists into an intermediate (mid / mid_off): one thread per survivor
+//                        searches the deferred lists in HBM, a block scan and a decoupled
+//                        look-back place the kept values in out.
+// A tile of 512 driving values costs ~4 KB of TMA traffic per streamed list however few
+// candidates still reach it; a deferred survivor costs a few scattered sectors per list.
 #pragma once
 
 #include "decode_kernel.cuh"   // mbarrier / TMA helpers
@@ -75,19 +90,104 @@ struct PParams {
     const u64* plan_base;      // per task: index of its first plan entry
     const PPlanEntry* plan;    // per (tile, filter list)
     const struct PTileEntry* tiles;  // per tile
+    const u32* defer;          // null, or the batch's "some query deferred" word: survivors then go to mid / mid_off
+    u64* mid;                  // the intermediate: sum of |A| values, an exact bound on it
+    u64* mid_off;              // ntasks + 1
+    u64 mid_cap;
     u32 slice_cap;             // stage capacity for slices, in u64 values
     u32 nctas;
     u32 grp;                   // tiles the metadata warp claims per ticket (1 .. P_GRP)
 };
 
+// ---- stream depth ---------------------------------------------------------------------
+// A filter list streamed by the pipeline costs 8 bytes per driving value whatever survives.
+// A deferred survivor costs one HBM binary search per deferred list it reaches: about 5 new
+// 32-byte sectors below the levels L2 holds, ~160 bytes.  The two break even when one driving
+// value in ~20-32 still reaches the list; 1/32 keeps the dense side of the estimate.
+// The sample itself costs ~160 bytes per (sampled value, list) whether or not anything is
+// deferred, and it shares HBM with the previous batch's pipeline: 256 values (a defer decision
+// two standard deviations from the threshold on both sides for C2's 1/16 and 1/64 survival),
+// and only for driving lists of at least P_SAMPLE_MIN_A values, where it costs under 8 % of one
+// streamed list (256 x 160 B against 8 B x 64 Ki).
+constexpr u32 P_SAMPLES = 256;         // sampled driving values per query, one per thread
+constexpr u32 P_DEFER_DIV = 32;        // defer the lists after the first that leaves < samples / 32 alive
+constexpr u64 P_SAMPLE_MIN_A = 65536;  // shorter driving lists stream every list
+constexpr int kLaneTailWord = 5;       // u32 index in the lane's error block (after kLaneOverflowWord): deferred queries
+constexpr u32 P_SAMPLE_LISTS = 31;     // filter lists searched by the sample (hit bits of a u32)
+
+// One CTA (P_SAMPLES threads) per (query, filter list j <= k - 2).  The last list is never a split
+// point: deferring after it would defer nothing.  The lists are searched side by side, not one after
+// another: the pre-pass shares the GPU with the previous batch's pipeline, where every dependent HBM
+// load waits microseconds, so the chain must be ONE search long.  A CTA sets bit j - 1 of its samples'
+// hit words (branch-free lower bound); the query's last CTA to finish counts, per j, the samples that
+// hit lists 1..j and sets k_eff = 1 + the first j with fewer than samples / P_DEFER_DIV of them, else
+// k.  Results never depend on k_eff.  hits (P_SAMPLES words per query) and done (one word per query)
+// are zeroed by the caller.
+__global__ void __launch_bounds__(P_SAMPLES) filter_sample_kernel(const FTask* __restrict__ tasks,
+                                                                  const FList* __restrict__ lists,
+                                                                  u32* __restrict__ hits, u32* __restrict__ done,
+                                                                  u32* __restrict__ keff, u32* defer) {
+    __shared__ u32 s_depth[P_SAMPLE_LISTS + 2];
+    __shared__ bool s_last;
+    const u32 q = blockIdx.x, j = blockIdx.y + 1, tid = threadIdx.x;
+    const FTask T = tasks[q];
+    const FList LA = lists[T.list_first];
+    const u64 lenA = flist_len(LA);
+    const u32 nj = (T.k < 3 || lenA < P_SAMPLE_MIN_A) ? 0u : (T.k - 2 < P_SAMPLE_LISTS ? T.k - 2 : P_SAMPLE_LISTS);
+    if (nj == 0) {  // not sampled: every list is streamed
+        if (j == 1 && tid == 0) keff[q] = T.k;
+        return;
+    }
+    if (j > nj) return;
+    u32* hq = hits + (size_t)q * P_SAMPLES;
+    {
+        const FList L = lists[T.list_first + j];
+        const u64* __restrict__ B = L.ptr;
+        const u64 n = flist_len(L);
+        const u64 x = ld_probe(LA.ptr + (u64)tid * lenA / P_SAMPLES);
+        if (n) {
+            u64 base = 0;
+            for (u64 len = n; len > 1;) {
+                const u64 half = len >> 1;
+                if (ld_probe(B + base + half) < x) base += half;
+                len -= half;
+            }
+            const u64 v = ld_probe(B + base);
+            const u64 p = base + (v < x ? 1u : 0u);
+            if (p < n && (p == base ? v : ld_probe(B + p)) == x) atomicOr(hq + tid, 1u << (j - 1));
+        }
+    }
+    // the last CTA of the query decides
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(done + q, 1u) == nj - 1;
+    if (tid < P_SAMPLE_LISTS + 2) s_depth[tid] = 0;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    atomicAdd(&s_depth[__ffs(~*(volatile const u32*)(hq + tid)) - 1], 1u);  // lists 1..depth all hit
+    __syncthreads();
+    if (tid == 0) {
+        u32 ke = T.k, alive = P_SAMPLES;  // samples that hit lists 1..j
+        for (u32 jj = 1; jj <= nj; ++jj) {
+            alive -= s_depth[jj - 1];
+            if (alive * P_DEFER_DIV < P_SAMPLES) { ke = 1 + jj; break; }
+        }
+        keff[q] = ke;
+        if (ke < T.k) atomicExch(defer, 1u);
+    }
+}
+
 // ---- plan ---------------------------------------------------------------------------
 // One THREAD per (tile, filter list): r0 = first i with L[i] >= tile first, r1 = first i
 // with L[i] > tile last, as two interleaved binary searches.  A binary search touches one
 // new 32-byte sector per level only near its end (~8 sectors), where a 32-ary warp
-// search touches ~70: the plan must not cost a second pass over HBM.
+// search touches ~70: the plan must not cost a second pass over HBM.  Deferred lists
+// (j >= keff[task]) are not streamed and need no bounds.
 __global__ void __launch_bounds__(256) filter_plan_kernel(const FTask* __restrict__ tasks, const FList* __restrict__ lists,
                                                           const u64* __restrict__ plan_base, u32 ntasks, u64 npairs,
-                                                          PPlanEntry* __restrict__ plan, u32 tile_sz) {
+                                                          PPlanEntry* __restrict__ plan, u32 tile_sz,
+                                                          const u32* __restrict__ keff) {
     const u64 p = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= npairs) return;
     u32 lo = 0, hi = ntasks;  // last task with plan_base <= p (the one that owns pair p)
@@ -100,6 +200,7 @@ __global__ void __launch_bounds__(256) filter_plan_kernel(const FTask* __restric
     const u32 km1 = T.k - 1;
     const u64 tl = local / km1;
     const u32 j = (u32)(local - tl * km1) + 1;
+    if (keff && j >= keff[lo]) return;
     const FList LA = lists[T.list_first];
     const u64 lenA = flist_len(LA);
     const u64 a0 = tl * (u64)tile_sz;
@@ -123,10 +224,13 @@ __global__ void __launch_bounds__(256) filter_plan_kernel(const FTask* __restric
     plan[p].r1 = r1;
 }
 
-// One thread per tile: which task it belongs to and where its driving values start.
+// One thread per tile: which task it belongs to and where its driving values start.  The tile's
+// k is the number of lists the pipeline streams (keff[task] when the batch was sampled); its plan
+// entries keep the stride k - 1 of the task.
 __global__ void __launch_bounds__(256) filter_tiles_kernel(const FTask* __restrict__ tasks, const FList* __restrict__ lists,
                                                            const u64* __restrict__ plan_base, u32 ntasks, u32 ntiles,
-                                                           PTileEntry* __restrict__ tiles, u32 tile_sz) {
+                                                           PTileEntry* __restrict__ tiles, u32 tile_sz,
+                                                           const u32* __restrict__ keff) {
     const u32 tile = blockIdx.x * blockDim.x + threadIdx.x;
     if (tile >= ntiles) return;
     u32 lo = 0, hi = ntasks;
@@ -138,7 +242,7 @@ __global__ void __launch_bounds__(256) filter_tiles_kernel(const FTask* __restri
     const FList LA = lists[T.list_first];
     const u64 lenA = flist_len(LA);
     PTileEntry e;
-    e.task = lo; e.list_first = T.list_first; e.k = T.k;
+    e.task = lo; e.list_first = T.list_first; e.k = keff ? keff[lo] : T.k;
     e.a0 = ((u64)tile - T.tile_base) * (u64)tile_sz;
     e.na = e.a0 < lenA ? (u32)((lenA - e.a0 < (u64)tile_sz) ? (lenA - e.a0) : (u64)tile_sz) : 0u;
     e.plan_idx = plan_base[lo] + ((u64)tile - T.tile_base) * (u64)(T.k - 1);
@@ -518,6 +622,11 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
         PPROF_FLUSH(4)
     } else if (wid == P_CW + 2) {
         // =========================== O: output warp =================================
+        // A batch with deferred queries ends in filter_tail_kernel: this pass fills the intermediate.
+        u64* out = P.out;
+        u64* out_off = P.out_off;
+        u64 out_cap = P.out_cap;
+        if (PP.defer && *PP.defer) { out = PP.mid; out_off = PP.mid_off; out_cap = PP.mid_cap; }
         PPROF_VARS
         for (u32 it = 0;; ++it) {
             const u32 sl = it % P_OS, use = it / P_OS;
@@ -540,16 +649,16 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
             const u64 base = lookback_exclusive<true, P_SLEEP_LB>(P.status, tile, (u64)total, lane);
             PPROF_ACC(pp_w1)
             if (lane == 0) {
-                if (O.first) P.out_off[q] = base;
-                if (tile == P.ntiles - 1) P.out_off[P.ntasks] = base + (u64)total;
+                if (O.first) out_off[q] = base;
+                if (tile == P.ntiles - 1) out_off[P.ntasks] = base + (u64)total;
             }
-            if (base + (u64)total > P.out_cap) {
+            if (base + (u64)total > out_cap) {
                 if (lane == 0) atomicExch(P.err, 1);
             } else if (total != 0) {
                 // a warp's segment holds at most P_WC survivors: P_VA predicated stores per segment,
                 // the shuffles of all segments independent of each other
                 const u64* data = s_out + (size_t)sl * P_TA;
-                u64* dst = P.out + base;
+                u64* dst = out + base;
 #pragma unroll
                 for (int w = 0; w < P_CW; ++w) {
                     const u32 nw = __shfl_sync(0xffffffffu, cw, w);
@@ -869,6 +978,101 @@ __global__ void __launch_bounds__(P_NT, 2) filter_pipe_kernel(const PParams PP) 
         }
         PPROF_FLUSH(0)
         PPROF_PHASE_FLUSH()
+    }
+}
+
+// ---- the deferred lists: one thread per survivor of the pipeline -----------------------------
+struct PTailParams {
+    const FTask* tasks;
+    const FList* lists;
+    u32 ntasks;
+    const u32* keff;          // per task: lists the pipeline streamed
+    const u32* defer;         // the batch's "some query deferred" word (0: the pipeline wrote out itself)
+    const u64* mid;           // the pipeline's survivors, queries back to back
+    const u64* mid_off;       // ntasks + 1
+    u64* out;
+    u64 out_cap;
+    u64* out_off;             // ntasks + 1
+    u64* status;              // per chunk of 256 survivors (mid_cap / 256 + 1 words), zeroed
+    u32* ticket;              // zeroed
+    int* err;
+    u32* tail_queries;        // the lane's counter of deferred queries (this kernel runs on the lane's stream)
+};
+constexpr int P_TAIL_NT = 256;
+
+// Persistent CTAs claim chunks of 256 intermediate values in order (atomic ticket, so the look-back never
+// waits on a chunk nobody runs).  Thread i: query q = the one whose range of mid holds i; the duplicate rank r
+// of x = mid[i] among the copies of x in that range (the pipeline keeps copies 0..m-1 of a value, so r is the
+// rank of the candidate in A, cand_rank's r); x survives deferred list L iff L[lower_bound(L, x) + r] == x,
+// the lists tested in order up to the first miss.  A block scan of the keep flags and a decoupled look-back
+// place the kept values; out_off[q] is the number kept before mid_off[q].  The thread of index mid_off[q]
+// writes it, so the chunk count covers index m = mid_off[ntasks] as well.  A chunk whose values would end
+// past out_cap writes none of them and raises err, as the pipeline's tiles do.  CTA 0 also counts the
+// deferred queries into the lane's counter.
+__global__ void __launch_bounds__(P_TAIL_NT) filter_tail_kernel(const PTailParams P) {
+    if (*P.defer == 0) return;
+    __shared__ u32 s_chunk;
+    __shared__ u32 s_sums[P_TAIL_NT / 32 + 1];
+    __shared__ u64 s_base;
+    const int tid = threadIdx.x, lane = tid & 31;
+    if (blockIdx.x == 0) {
+        u32 nd = 0;
+        for (u32 q = tid; q < P.ntasks; q += P_TAIL_NT) nd += P.keff[q] < P.tasks[q].k ? 1u : 0u;
+        for (int d = 16; d > 0; d >>= 1) nd += __shfl_xor_sync(0xffffffffu, nd, d);
+        if (lane == 0 && nd) atomicAdd(P.tail_queries, nd);
+    }
+    const u64 m = P.mid_off[P.ntasks];
+    const u64 nchunks = m / P_TAIL_NT + 1;
+    for (;;) {
+        if (tid == 0) s_chunk = atomicAdd(P.ticket, 1u);
+        __syncthreads();
+        const u32 c = s_chunk;
+        if ((u64)c >= nchunks) break;
+        const u64 i = (u64)c * P_TAIL_NT + tid;
+        bool keep = false;
+        u64 x = 0, s = 0;
+        u32 lo = 0;
+        if (i <= m) {
+            u32 hi = P.ntasks + 1;  // lo: last q with mid_off[q] <= i
+            while (hi - lo > 1) {
+                const u32 md = (lo + hi) >> 1;
+                if (ld_probe(P.mid_off + md) <= i) lo = md; else hi = md;
+            }
+            s = ld_probe(P.mid_off + lo);
+            if (i < m) {
+                x = P.mid[i];
+                keep = true;
+                const FTask T = P.tasks[lo];
+                const u32 ke = P.keff[lo];
+                if (ke < T.k) {
+                    u64 r = 0;
+                    if (i > s && P.mid[i - 1] == x) r = (i - s) - lower_bound_g(P.mid + s, i - s, x);
+                    for (u32 j = ke; j < T.k && keep; ++j) {
+                        const FList L = P.lists[T.list_first + j];
+                        const u64 len = flist_len(L);
+                        const u64 g = lower_bound_g(L.ptr, len, x) + r;
+                        keep = g < len && ld_probe(L.ptr + g) == x;
+                    }
+                }
+            }
+        }
+        u32 tot;
+        const u32 ex = block_exclusive_scan<P_TAIL_NT>(keep ? 1u : 0u, s_sums, &tot);
+        if (tid < 32) {
+            const u64 b = lookback_exclusive(P.status, c, (u64)tot, lane);
+            if (lane == 0) s_base = b;
+        }
+        __syncthreads();
+        const u64 base = s_base;
+        if (i <= m && s == i) {  // i opens query lo, and every empty query before it
+            for (long long q = lo; q >= 0 && ld_probe(P.mid_off + q) == i; --q) P.out_off[q] = base + ex;
+        }
+        if (base + (u64)tot > P.out_cap) {
+            if (tid == 0 && tot) atomicExch(P.err, 1);
+        } else if (keep) {
+            P.out[base + ex] = x;
+        }
+        __syncthreads();  // s_chunk / s_sums / s_base are rewritten by the next chunk
     }
 }
 

@@ -395,6 +395,10 @@ int dgx_dev_merge_sorted_matrix(dgx_lane* lane, const uint64_t* d_v, const uint6
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);
+/* Intersection queries of 3+ lists whose sparse tail of lists was searched after the streaming pass (on a lane with
+ * resident inputs, a sample of a driving list of at least 65536 values found few candidates reaching those lists): of
+ * this lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
+uint64_t dgx_filter_tail_queries(const dgx_lane* lane);
 
 #ifdef __cplusplus
 }
