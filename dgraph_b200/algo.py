@@ -197,6 +197,42 @@ def IntersectCompressedWithRows(packs, afterUID: int, v, keys=None):
     return out[: int(out_off[-1])], out_off
 
 
+UIDS_COMPRESSED, UIDS_PROBE, UIDS_ITERATE = 0, 1, 2  # List.Uids branch of a row (include/dgx.h DGX_UIDS_*)
+MUT_DEL, MUT_VALUE = 1, 2                             # flags of a resolved mutable entry (DGX_MUT_*)
+
+
+def ListUidsRows(packs, modes, muts, afterUID: int, v, keys=None):
+    """posting.List.Uids(opts) for every key of a task in ONE call (dgx_list_uids_rows), mutable layers included: the
+    handleUidPostings loop (worker/task.go:783-987) of a filtered read of unsplit lists.
+
+    packs[i]: the immutable layer (None for an empty one, or for a delete-all marker).  modes[i]: the branch of List.Uids
+    row i takes (UIDS_COMPRESSED / UIDS_PROBE / UIDS_ITERATE).  muts[i]: None or (uids, flags), the resolved mutable
+    entries of row i, strictly ascending, flags MUT_DEL / MUT_VALUE.  v: opts.Intersect, ascending and non-empty.
+    keys: optional [(key, version)] naming each pack for the HBM-resident cache.  Returns (out, out_off): row i is
+    out[out_off[i]:out_off[i+1]]."""
+    vv = v.Uids if isinstance(v, List) else v
+    vv = np.zeros(0, np.uint64) if vv is None else _u64(vv)
+    nrows = len(packs)
+    if nrows == 0:
+        return np.zeros(0, np.uint64), np.zeros(1, np.uint64)
+    mode = np.ascontiguousarray(np.asarray(modes, dtype=np.uint8))
+    mu = [np.zeros(0, np.uint64) if t is None else _u64(t[0]) for t in muts]
+    mf = [np.zeros(0, np.uint8) if t is None else np.ascontiguousarray(np.asarray(t[1], np.uint8)) for t in muts]
+    mut_off = np.zeros(nrows + 1, dtype=np.uint64)
+    np.cumsum([a.size for a in mu], out=mut_off[1:])
+    nmut = int(mut_off[-1])
+    mut_uids = np.concatenate(mu) if nmut else np.zeros(1, np.uint64)
+    mut_flags = np.concatenate(mf) if nmut else np.zeros(1, np.uint8)
+    lib = _lib.load()
+    refs, keep = _refs_of(packs, keys)
+    cap = sum(min(vv.size, (_exact(p) if p is not None else 0) + a.size) for p, a in zip(packs, mu))
+    out = np.empty(max(cap, 1), dtype=np.uint64)
+    out_off = np.zeros(nrows + 1, dtype=np.uint64)
+    _lib.check(lib.dgx_list_uids_rows(refs, _p(mode), nrows, _p(mut_uids), _p(mut_flags), _p(mut_off), afterUID,
+                                      _p(vv), vv.size, _p(out), _p(out_off), cap))
+    return out[: int(out_off[-1])], out_off
+
+
 def IntersectCompressedWithMatrix(pack, rows, key=None):
     """algo.IntersectCompressedWith(pack, 0, rows[i], o_i) for every row i in ONE call
     (dgx_intersect_compressed_matrix): the intersectBucket loop (worker/sort.go:605-700) of one index bucket over a

@@ -34,6 +34,7 @@
 #include "merge_matrix.cuh"
 #include "probe_kernel.cuh"
 #include "compressed_kernel.cuh"
+#include "list_uids_kernel.cuh"
 #include "encode_kernel.cuh"
 #include "wire.hpp"
 
@@ -448,6 +449,9 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
         *l->h_err = 0;
         CK(cudaMemsetAsync(l->d_err, 0, sizeof(int), l->stream));
         if (flag & kLaneErrOrder) return fail(DGX_ERR_ARG, "a row of the uid matrix is not strictly ascending");
+        if (flag & kLaneErrMut)
+            return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
+                                     "flags) or a probe / iterate row's pack starts at uid 0");
         return fail(DGX_ERR_CAP, "result does not fit out_cap");
     }
     return DGX_OK;
@@ -2556,6 +2560,196 @@ extern "C" int dgx_intersect_compressed_matrix(const dgx_pack_ref* ref, const ui
     rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
     if (rc) return rc;
     rc = icw_matrix_impl(l, ps.pk[0], d_v, v_off, nrows, (uint64_t*)d_out, cap, (uint64_t*)d_off);
+    if (rc) return rc;
+    return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
+}
+
+// ---------------------------------------------------------------------------
+// List.Uids over a task's keys, mutable layers included (handleUidPostings)
+// ---------------------------------------------------------------------------
+// The host-side checks of both forms, before anything is copied: modes, offsets, m, and the bounds that keep the
+// MaxInt32 cut of List.Uids (posting/list.go:1840, 1864-1870) from biting.  exact(i) is ExactLen of row i's pack.
+static_assert(LU_COMPRESSED == DGX_UIDS_COMPRESSED && LU_PROBE == DGX_UIDS_PROBE && LU_ITERATE == DGX_UIDS_ITERATE &&
+                  LU_DEL == DGX_MUT_DEL && LU_VALUE == DGX_MUT_VALUE,
+              "list_uids_kernel.cuh reads the modes and flags of include/dgx.h");
+template <class ExactLen>
+static int list_uids_check(const uint8_t* mode, size_t nrows, const uint64_t* mut_off, size_t m, ExactLen exact) {
+    const uint64_t k31 = uint64_t(1) << 31;
+    if (m == 0) return fail(DGX_ERR_ARG, "v is empty: an unfiltered read is not a List.Uids row call");
+    if (m >= k31) return fail(DGX_ERR_ARG, "v has %zu uids: at most 2^31 - 1", m);
+    if (mut_off[0] != 0) return fail(DGX_ERR_ARG, "mut_off[0] is %llu, not 0", (unsigned long long)mut_off[0]);
+    for (size_t r = 0; r < nrows; ++r) {
+        if (mode[r] > LU_ITERATE) return fail(DGX_ERR_ARG, "row %zu has mode %u", r, (unsigned)mode[r]);
+        if (mut_off[r + 1] < mut_off[r]) return fail(DGX_ERR_ARG, "mut_off decreases at row %zu", r);
+        const uint64_t nm = mut_off[r + 1] - mut_off[r];
+        if (mode[r] == LU_COMPRESSED && nm) return fail(DGX_ERR_ARG, "row %zu is compressed but has mutable entries", r);
+        if (mode[r] == LU_ITERATE && exact(r) + nm >= k31)
+            return fail(DGX_ERR_ARG, "iterate row %zu has %llu postings: at most 2^31 - 1", r,
+                        (unsigned long long)(exact(r) + nm));
+    }
+    if (mut_off[nrows] >= k31)
+        return fail(DGX_ERR_ARG, "the mutable layers have %llu entries: at most 2^31 - 1", (unsigned long long)mut_off[nrows]);
+    return DGX_OK;
+}
+
+// Row i = List.Uids of row i's branch (list_uids_kernel.cuh) with the six launches of icw_rows_impl (pack ∩ v, after 0)
+// and five of its own: classify, entry scan, rows, row scan, write.  When no row has a non-empty pack, icw_rows_impl
+// launches nothing and the call makes five.  mode and mut_off are host memory, already checked.
+static int list_uids_impl(dgx_lane* l, const dgx_dev_pack* const* packs, const uint8_t* mode, size_t nrows,
+                          const uint64_t* d_mut, const uint8_t* d_flags, const uint64_t* mut_off, uint64_t after,
+                          const uint64_t* d_v, size_t m, uint64_t* d_out, size_t out_cap, uint64_t* d_out_off) {
+    const uint64_t nmut = mut_off[nrows];
+    uint64_t a_cap = 0;
+    for (size_t i = 0; i < nrows; ++i)
+        if (packs[i]) a_cap += std::min<uint64_t>(m, packs[i]->exact_len);
+    const uint64_t kMaxGrid = 0x7fffffffull;
+    const uint64_t g_mut = std::max<uint64_t>((nmut + 255) / 256, 1), g_rows = (nrows + 255) / 256;
+    const uint64_t g_write = (std::max<uint64_t>(a_cap + nmut, nrows + 1) + 255) / 256;
+    const uint64_t t_mut = std::max<uint64_t>((nmut + EN_TILE - 1) / EN_TILE, 1), t_rows = (nrows + EN_TILE - 1) / EN_TILE;
+    if (std::max({g_mut, g_rows, g_write}) > kMaxGrid)
+        return fail(DGX_ERR_ARG, "batch too large for one launch (%llu uids, %zu rows)", (unsigned long long)(a_cap + nmut),
+                    nrows);
+    // table (copied): [mut_off | first | nmut | nrows | mode];  zeroed: [scan status + tickets | bad];  then a, a_off,
+    // cls, cls_ex, lo, cnt
+    const size_t b_tab = ((2 * nrows + 3) * sizeof(uint64_t) + nrows + 15) & ~size_t(15);
+    const size_t b_zero = (t_mut + t_rows) * sizeof(u64) + 16;
+    const size_t b_rest = (a_cap + 2 + (nrows + 1) + nmut + (nmut + 1) + 2 * nrows) * sizeof(u64);
+    void *h_raw, *d_raw;
+    int rc = l->host.alloc(b_tab, &h_raw);
+    if (rc) return rc;
+    rc = l->ws.alloc(b_tab + b_zero + b_rest, &d_raw);
+    if (rc) return rc;
+    uint64_t* h_tab = (uint64_t*)h_raw;
+    memcpy(h_tab, mut_off, (nrows + 1) * sizeof(uint64_t));
+    for (size_t i = 0; i < nrows; ++i) {
+        const bool reads_pack = mode[i] != LU_COMPRESSED && packs[i] && packs[i]->pk.nblocks;
+        h_tab[nrows + 1 + i] = reads_pack ? (uint64_t)(uintptr_t)packs[i]->pk.base : 0;
+    }
+    h_tab[2 * nrows + 1] = nmut;
+    h_tab[2 * nrows + 2] = nrows;
+    memcpy(h_tab + 2 * nrows + 3, mode, nrows);
+    char* d = (char*)d_raw;
+    CK(cudaMemcpyAsync(d, h_tab, b_tab, cudaMemcpyHostToDevice, l->stream));
+    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
+    g_stats.h2d += b_tab;
+    LuParams P;
+    P.mut_off = (const u64*)d;
+    P.first = (const u64* const*)(P.mut_off + nrows + 1);
+    const u64* d_nmut = P.mut_off + 2 * nrows + 1;  // scan lengths as device words
+    const u64* d_nrows = d_nmut + 1;
+    P.mode = (const unsigned char*)(d_nrows + 1);
+    P.nrows = nrows;
+    P.mut = (const u64*)d_mut;
+    P.flags = d_flags;
+    P.nmut = nmut;
+    P.after = after;
+    P.v = (const u64*)d_v;
+    P.m = m;
+    u64* status = (u64*)(d + b_tab);
+    u32* tickets = (u32*)(status + t_mut + t_rows);
+    P.bad = (int*)(tickets + 2);
+    u64* a = (u64*)(d + b_tab + b_zero);
+    u64* a_off = a + a_cap + 2;
+    P.a = a;
+    P.a_off = a_off;
+    P.a_cap = a_cap;
+    P.cls = a_off + nrows + 1;
+    P.cls_ex = P.cls + nmut;
+    P.lo = P.cls_ex + nmut + 1;
+    P.cnt = P.lo + nrows;
+    P.out = (u64*)d_out;
+    P.out_cap = out_cap;
+    P.out_off = (u64*)d_out_off;
+    P.err = l->d_err;
+    // pack ∩ v of every row from uid 0: each mode applies its own bound afterwards
+    rc = icw_rows_impl(l, packs, nrows, 0, d_v, m, (uint64_t*)a, a_cap, (uint64_t*)a_off);
+    if (rc) return rc;
+    lu_classify_kernel<<<(unsigned)g_mut, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)t_mut, EN_NT, 0, l->stream>>>(P.cls, P.cls_ex, d_nmut, nmut, status, tickets, nullptr);
+    CK(cudaGetLastError());
+    lu_rows_kernel<<<(unsigned)g_rows, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)t_rows, EN_NT, 0, l->stream>>>(P.cnt, P.out_off, d_nrows, nrows, status + t_mut,
+                                                                tickets + 1, nullptr);
+    CK(cudaGetLastError());
+    lu_write_kernel<<<(unsigned)g_write, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    l->launches += 5;
+    g_stats.launches += 5;
+    g_stats.uids_in += nmut;
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_list_uids_rows(dgx_lane* l, const dgx_dev_pack* const* packs, const uint8_t* mode, size_t nrows,
+                                      const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
+                                      uint64_t after_uid, const uint64_t* d_v, size_t m, uint64_t* d_out,
+                                      size_t out_cap, uint64_t* d_out_off) {
+    if (!l || !d_out_off) return fail(DGX_ERR_ARG, "null argument");
+    if (nrows == 0) {
+        if (int rc = lane_begin_op(l)) return rc;
+        CK(cudaMemsetAsync(d_out_off, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (!packs || !mode || !mut_off || !d_v) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = list_uids_check(mode, nrows, mut_off, m, [&](size_t r) -> uint64_t {
+            return packs[r] ? packs[r]->exact_len : 0;
+        }))
+        return rc;
+    if (mut_off[nrows] && (!d_mut_uids || !d_mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    const int rc = list_uids_impl(l, packs, mode, nrows, d_mut_uids, d_mut_flags, mut_off, after_uid, d_v, m, d_out,
+                                  out_cap, d_out_off);
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    return rc;
+}
+
+extern "C" int dgx_list_uids_rows(const dgx_pack_ref* refs, const uint8_t* mode, size_t nrows, const uint64_t* mut_uids,
+                                  const uint8_t* mut_flags, const uint64_t* mut_off, uint64_t after_uid, const uint64_t* v,
+                                  size_t m, uint64_t* out, uint64_t* out_off, size_t out_cap) {
+    if (!out_off) return fail(DGX_ERR_ARG, "null out_off");
+    if (nrows == 0) { out_off[0] = 0; return DGX_OK; }
+    if (!refs || !mode || !mut_off || !v) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = list_uids_check(mode, nrows, mut_off, m, [&](size_t r) -> uint64_t {
+            const dgx_pack_view* p = refs[r].pack;
+            uint64_t n = 0;
+            for (size_t b = 0; p && b < p->nblocks; ++b) n += p->num_uids[b];
+            return n;
+        }))
+        return rc;
+    const uint64_t nmut = mut_off[nrows];
+    if (nmut && (!mut_uids || !mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    PackSet ps(l, refs, nrows);  // nil / empty packs are packs of no blocks
+    if (ps.rc) return ps.rc;
+    std::vector<const dgx_dev_pack*> rows(nrows);
+    size_t cap = 0;
+    for (size_t i = 0; i < nrows; ++i) {
+        rows[i] = &ps.pk[i];
+        cap += std::min<size_t>(m, ps.pk[i].exact_len + (mut_off[i + 1] - mut_off[i]));
+    }
+    uint64_t *d_v, *d_mut;
+    int rc = upload_list(l, v, m, &d_v);
+    if (rc) return rc;
+    rc = upload_list(l, mut_uids, nmut, &d_mut);
+    if (rc) return rc;
+    void* d_flags;
+    rc = l->ws.alloc(nmut + 16, &d_flags);
+    if (rc) return rc;
+    if (nmut) CK(cudaMemcpyAsync(d_flags, mut_flags, nmut, cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += nmut;
+    void *d_out, *d_off;
+    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
+    if (rc) return rc;
+    rc = list_uids_impl(l, rows.data(), mode, nrows, d_mut, (const uint8_t*)d_flags, mut_off, after_uid, d_v, m,
+                        (uint64_t*)d_out, cap, (uint64_t*)d_off);
     if (rc) return rc;
     return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
 }

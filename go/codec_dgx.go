@@ -409,3 +409,112 @@ func EncodeDevice(uids []uint64, blockSize int) (*pb.UidPack, bool) {
 	}
 	return nil, false
 }
+
+// MutRow is a key's mutable layer as List.Uids sees it, resolved by the caller under l.RLock (INTEGRATION §2): one
+// entry per uid, strictly ascending, Flags[i] = DGX_MUT_DEL (Op == Del) | DGX_MUT_VALUE (PostingType != REF).
+type MutRow struct {
+	Uids  []uint64
+	Flags []uint8
+}
+
+// ListUidsRows is posting.List.Uids(opts) (posting/list.go:1758-1874) for every key of a task in ONE library call:
+// the handleUidPostings loop (worker/task.go:783-987) of a filtered read (opts.Intersect = v, non-empty) of unsplit
+// lists, mutable layers included.  modes[i] is the branch List.Uids takes for key i (DGX_UIDS_COMPRESSED without a
+// mutable layer, DGX_UIDS_PROBE when len(v) < ApproxLen, DGX_UIDS_ITERATE otherwise); refs[i].Pack is nil for a key
+// whose delete-all marker hides the immutable layer.  Packs are staged as in IntersectCompressedWithRows; the mutable
+// layers cross as one C allocation (offsets, uids, flags, modes).  The size threshold applies to the batch total.
+// Returns false when the caller must keep pl.Uids.
+func ListUidsRows(refs []PackRef, modes []uint8, muts []MutRow, afterUID uint64, v *pb.List) ([]*pb.List, bool) {
+	n, m := len(refs), len(v.Uids)
+	if n == 0 {
+		return []*pb.List{}, true
+	}
+	if m == 0 || uint64(m) >= 1<<31 || len(modes) != n || len(muts) != n {
+		return nil, false
+	}
+	total, capOut, img, nmut := m, 0, 0, 0
+	for i, r := range refs {
+		nm, e := len(muts[i].Uids), 0
+		nmut += nm
+		if r.Pack != nil && len(r.Pack.Blocks) > 0 {
+			total += ApproxLen(r.Pack)
+			e = ExactLen(r.Pack)
+			if r.Key == 0 {
+				img += int(C.dgx_pack_image_size(C.size_t(len(r.Pack.Blocks)), C.size_t(deltaBytes(r.Pack))))
+			}
+		}
+		if e+nm < m {
+			capOut += e + nm
+		} else {
+			capOut += m
+		}
+	}
+	if total+nmut < dgxMinDecode {
+		return nil, false
+	}
+	// [mut_off (n + 1) | mut_uids (nmut, plus one spare word so &words[n+1] exists) | mut_flags (nmut bytes) | modes]
+	csr := C.malloc(C.size_t((n+2+nmut)*8 + nmut + n + 16))
+	crefs := (*[1 << 28]C.dgx_pack_ref)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(C.dgx_pack_ref{}))))
+	views := (*[1 << 28]C.dgx_pack_view)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(C.dgx_pack_view{}))))
+	stage := C.malloc(C.size_t(img + 64))
+	frees := []func(){}
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+		C.free(csr)
+		C.free(unsafe.Pointer(crefs))
+		C.free(unsafe.Pointer(views))
+		C.free(stage)
+	}()
+	words := unsafe.Slice((*uint64)(csr), n+2+nmut)
+	small := unsafe.Slice((*uint8)(unsafe.Add(csr, (n+2+nmut)*8)), nmut+n)
+	w := 0
+	for i, mr := range muts {
+		if len(mr.Flags) != len(mr.Uids) {
+			return nil, false
+		}
+		words[i] = uint64(w)
+		copy(words[n+1+w:], mr.Uids)
+		copy(small[w:], mr.Flags)
+		w += len(mr.Uids)
+	}
+	words[n] = uint64(w)
+	copy(small[nmut:], modes)
+	o := 0
+	for i, r := range refs {
+		crefs[i] = C.dgx_pack_ref{key: C.uint64_t(r.Key), version: C.uint64_t(r.Version)}
+		if r.Pack == nil || len(r.Pack.Blocks) == 0 {
+			continue // delete-all marker or empty immutable layer
+		}
+		if r.Key != 0 {
+			view, free := flatten(r.Pack)
+			frees = append(frees, free)
+			views[i] = view
+		} else {
+			nb, db := len(r.Pack.Blocks), deltaBytes(r.Pack)
+			if C.dgx_pack_image_view(unsafe.Add(stage, o), C.uint32_t(r.Pack.BlockSize), C.size_t(nb), C.size_t(db), &views[i]) != C.DGX_OK {
+				return nil, false
+			}
+			fillImage(&views[i], r.Pack)
+			o += int(C.dgx_pack_image_size(C.size_t(nb), C.size_t(db)))
+		}
+		crefs[i].pack = &views[i]
+	}
+	out := make([]uint64, capOut+1)
+	off := make([]uint64, n+1)
+	if C.dgx_list_uids_rows(&crefs[0], (*C.uint8_t)(unsafe.Pointer(&small[nmut])), C.size_t(n),
+		(*C.uint64_t)(unsafe.Pointer(&words[n+1])), (*C.uint8_t)(unsafe.Pointer(&small[0])), (*C.uint64_t)(unsafe.Pointer(&words[0])),
+		C.uint64_t(afterUID), (*C.uint64_t)(unsafe.Pointer(&v.Uids[0])), C.size_t(m),
+		(*C.uint64_t)(unsafe.Pointer(&out[0])), (*C.uint64_t)(unsafe.Pointer(&off[0])), C.size_t(capOut)) != C.DGX_OK {
+		return nil, false
+	}
+	rows := make([]*pb.List, n)
+	for i := range refs {
+		rows[i] = &pb.List{}
+		if off[i+1] > off[i] {
+			rows[i].Uids = out[off[i]:off[i+1]:off[i+1]]
+		}
+	}
+	return rows, true
+}

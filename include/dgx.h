@@ -223,6 +223,35 @@ int dgx_intersect_compressed_rows(const dgx_pack_ref* refs, size_t nrows, uint64
 int dgx_intersect_compressed_matrix(const dgx_pack_ref* ref, const uint64_t* v, const uint64_t* v_off, size_t nrows,
                                     uint64_t* out, uint64_t* out_off, size_t out_cap);
 
+/* posting.List.Uids(opts) for every key of a task, mutable layers included, one call: the handleUidPostings loop
+ * (worker/task.go:783-987 -> posting/list.go:1758-1870) of a filtered read of unsplit lists.  v = opts.Intersect.Uids
+ * (ascending, duplicate-free, 0 < m < 2^31), after_uid = opts.AfterUid.  Row i takes the branch mode[i] of List.Uids:
+ *   DGX_UIDS_COMPRESSED  no mutable layer (:1795-1800): {x in v : x in pack, x >= after}, exactly
+ *                        dgx_intersect_compressed_rows; such a row has no mutable entries
+ *   DGX_UIDS_PROBE       len(v) < ApproxLen (:1805-1820), findPostingWithItr per x of v, after ignored:
+ *                        {x in v : mut(x) exists ? mut(x) is not DGX_MUT_DEL : x in pack}
+ *   DGX_UIDS_ITERATE     otherwise (:1822-1862), iterate with the REF filter then IntersectWith; the pack side is
+ *                        Seek(after, SeekCurrent): {x in v : x > after, mut(x) exists ? mut(x) has no flag : x in pack}
+ * mut(x) is row i's resolved mutable entry of uid x -- the posting List.Uids would see (first of pickPostings per uid
+ * for iterate rows, MutableLayer.findPosting for probe rows): the caller does the MVCC work.  Row i's entries are
+ * mut_uids / mut_flags[mut_off[i] .. mut_off[i+1]) (host offsets, mut_off[0] == 0), strictly ascending, nonzero, with
+ * flags DGX_MUT_DEL (Op == Del) and DGX_MUT_VALUE (PostingType != REF).  A row with a delete-all marker is passed with a
+ * NULL pack.  refs[i] as in dgx_intersect_compressed_rows.  Row i of the CSR result is out[out_off[i] .. out_off[i+1]);
+ * out_cap >= sum_i min(m, ExactLen(pack_i) + |mut_i|) always suffices; a longer result than out_cap is DGX_ERR_CAP and
+ * nothing is written past out_cap.  nrows == 0 gives out_off[0] = 0 and needs no device.
+ * DGX_ERR_ARG before anything is copied: a mode not listed, a compressed row with mutable entries, mut_off[0] != 0 or
+ * decreasing offsets, m == 0 or m >= 2^31, 2^31 or more mutable entries in all, an iterate row with
+ * ExactLen + |mut| >= 2^31 (the MaxInt32 cut of :1864-1870 must not bite), a null array that is needed.
+ * DGX_ERR_ARG after the kernels, with out untouched: a mutable entry that does not ascend strictly, is 0 or has other
+ * flag bits, or a probe / iterate row whose pack starts at uid 0.  The call runs a fixed number of kernel launches
+ * whatever nrows, the number of mutable entries and the pack sizes are. */
+enum { DGX_UIDS_COMPRESSED = 0, DGX_UIDS_PROBE = 1, DGX_UIDS_ITERATE = 2 };
+enum { DGX_MUT_DEL = 1, DGX_MUT_VALUE = 2 };
+int dgx_list_uids_rows(const dgx_pack_ref* refs, const uint8_t* mode, size_t nrows,
+                       const uint64_t* mut_uids, const uint8_t* mut_flags, const uint64_t* mut_off,
+                       uint64_t after_uid, const uint64_t* v, size_t m,
+                       uint64_t* out, uint64_t* out_off, size_t out_cap);
+
 /* algo.MergeSorted(rows) over the rows of a uid matrix, one call: sg.DestUIDs = algo.MergeSorted(result.UidMatrix)
  * (query/query.go:2290, 2505; query/recurse.go:134; worker/task.go:1629, 1706; worker/match.go:100).
  * Row i is v[v_off[i] .. v_off[i+1]) (host offsets, nrows + 1 values, v_off[0] == 0).  Rows ascend; duplicates
@@ -385,6 +414,15 @@ int dgx_dev_intersect_compressed_rows(dgx_lane* lane, const dgx_dev_pack* const*
 int dgx_dev_intersect_compressed_matrix(dgx_lane* lane, const dgx_dev_pack* pk, const uint64_t* d_v,
                                         const uint64_t* v_off, size_t nrows,
                                         uint64_t* d_out, size_t out_cap, uint64_t* d_out_off);
+/* Device form of dgx_list_uids_rows: packs resident (dgx_dev_pack_upload; NULL = empty pack or delete-all marker),
+ * d_mut_uids / d_mut_flags / d_v / d_out / d_out_off (nrows + 1 values) device pointers; mode and mut_off in HOST
+ * memory, checked as in the host form before anything is queued.  Asynchronous on the lane: past out_cap nothing is
+ * written and the next dgx_lane_sync returns DGX_ERR_CAP; a malformed mutable entry or a probe / iterate pack that
+ * starts at uid 0 leaves d_out untouched, zeroes d_out_off and makes the next dgx_lane_sync return DGX_ERR_ARG. */
+int dgx_dev_list_uids_rows(dgx_lane* lane, const dgx_dev_pack* const* packs, const uint8_t* mode, size_t nrows,
+                           const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
+                           uint64_t after_uid, const uint64_t* d_v, size_t m,
+                           uint64_t* d_out, size_t out_cap, uint64_t* d_out_off);
 /* Device form of dgx_merge_sorted_matrix: d_v and d_v_off (nrows + 1 values) are DEVICE pointers, so the
  * (d_out, d_out_off) of dgx_dev_intersect_compressed_rows / dgx_dev_filter_batch feed it directly.  v_cap >=
  * d_v_off[nrows] sizes the workspace (v_cap >= 2^32 is DGX_ERR_ARG).  d_out_len: one device uint64, the result length.

@@ -134,6 +134,7 @@ def main():
     ap.add_argument("--c6-only", action="store_true", help="only the C6 handleUidPostings rows")
     ap.add_argument("--c7-only", action="store_true", help="only the C7 sort-bucket rows")
     ap.add_argument("--c8-only", action="store_true", help="only the C8 DestUIDs (MergeSorted of a uid matrix) rows")
+    ap.add_argument("--c9-only", action="store_true", help="only the C9 List.Uids rows with mutable layers")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -141,9 +142,11 @@ def main():
         rows = c7_rows(Lane())
     elif args.c8_only:
         rows = c8_rows(Lane())
+    elif args.c9_only:
+        rows = c9_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -394,6 +397,7 @@ def run(L, S, quick):
     rows += c6_rows(L)
     rows += c7_rows(L)
     rows += c8_rows(L)
+    rows += c9_rows(L)
     return rows
 
 
@@ -743,6 +747,151 @@ def c8_rows(L, reps: int = 10):
             out_rows.append(row(op, cfg, ms, m, abytes, ok, dict(extra, note=note, launches_per_call=launches,
                                                                  overflow_chunks=overflows)))
         del d_v, d_off, d_out
+    return out_rows
+
+
+def c9_rows(L, threads: int = 16):
+    """C9 "handleUidPostings with writes": the C6 task (10 000 UidPacks, one v of about 1e6 uids) where 30 % of the
+    keys carry a mutable layer of about 1 % of their length (deletes, new uids from the master, value postings;
+    tests/gen_mut.py), each key read with the List.Uids branch the ApproxLen rule picks.  Legs on the same inputs, each
+    checked row by row against the oracle's List.Uids: (1) dgx_dev_list_uids_rows on resident packs (CUDA events),
+    (2) dgx_list_uids_rows with named packs in steady state, (3) today's path: dgx_intersect_compressed_rows for the
+    clean keys, then the oracle's List.Uids for every key with a layer on `threads` host threads, (4) the oracle row
+    loop on one thread and on `threads` threads."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    import gen_mut
+    import gen_rows
+    import list_uids_oracle as luo
+    from oracle import pyoracle as orc
+
+    lib = L.lib
+    master, rows_u, v = gen_rows.c6_inputs()
+    nrows, m = len(rows_u), v.size
+    ops = [orc.encode(r, 256) for r in rows_u]
+    rng = np.random.default_rng(909)
+    muts, modes = [], []
+    for r, op in zip(rows_u, ops):
+        layer = rng.random() < 0.3
+        mu, mf = gen_mut.layer(rng, r, master, max(1, r.size // 100)) if layer else (np.zeros(0, np.uint64),
+                                                                                      np.zeros(0, np.uint8))
+        muts.append((mu, mf))
+        modes.append(gen_mut.mode_of(orc.approx_len(op), m, layer))
+    exact = sum(r.size for r in rows_u)
+    del rows_u
+    mode = np.array(modes, np.uint8)
+    mut_off = np.zeros(nrows + 1, np.uint64)
+    np.cumsum([t[0].size for t in muts], out=mut_off[1:])
+    mu_all = np.concatenate([t[0] for t in muts])
+    mf_all = np.concatenate([t[1] for t in muts])
+    nmut = int(mut_off[-1])
+    dirty = [i for i in range(nrows) if modes[i] != gen_mut.COMPRESSED]
+    clean = [i for i in range(nrows) if modes[i] == gen_mut.COMPRESSED]
+    views = []
+    for op in ops:
+        arrs = (op.base, op.num_uids, op.delta_off, op.deltas)  # copies: they stay alive with the view
+        views.append((_lib.PackView(256, op.nblocks, *[a.ctypes.data for a in arrs]),) + arrs)
+    refs = (_lib.PackRef * nrows)()
+    for i in range(nrows):
+        refs[i].pack, refs[i].key, refs[i].version = C.pointer(views[i][0]), 950_000 + i, 1
+    crefs = (_lib.PackRef * len(clean))(*[refs[i] for i in clean])
+    hv = np.ascontiguousarray(v)
+    cap = sum(min(m, int(op.num_uids.sum(dtype=np.uint64)) + t[0].size) for op, t in zip(ops, muts))
+    hout = np.empty(max(cap, 1), np.uint64)
+    hoff = np.zeros(nrows + 1, np.uint64)
+    ccap = sum(min(m, int(ops[i].num_uids.sum(dtype=np.uint64))) for i in clean)
+    cout = np.empty(max(ccap, 1), np.uint64)
+    coff = np.zeros(len(clean) + 1, np.uint64)
+
+    def p(a):
+        return a.ctypes.data_as(C.c_void_p)
+
+    def oracle_row(i, after):
+        return luo.list_uids(ops[i], modes[i], muts[i][0], muts[i][1], after, v)
+
+    def wall(fn, reps):
+        fn()
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            fn()
+        return (time.perf_counter() - t0) / reps * 1e3
+
+    handles = []
+    for pv in views:
+        h = C.c_void_p()
+        _lib.check(lib.dgx_dev_pack_upload(L.h, C.byref(pv[0]), C.byref(h)))
+        handles.append(h)
+    tab = (C.c_void_p * nrows)(*[h.value for h in handles])
+    d_v = torch.from_numpy(hv.view(np.int64)).to(DEV)
+    d_mu = torch.from_numpy(mu_all.view(np.int64)).to(DEV)
+    d_mf = torch.from_numpy(mf_all).to(DEV)
+    d_out = torch.empty(cap + 8, dtype=torch.int64, device=DEV)
+    d_off = torch.zeros(nrows + 1, dtype=torch.int64, device=DEV)
+    lib.dgx_cache_clear()
+    _lib.check(lib.dgx_cache_configure(16 << 30))
+    out_rows = []
+    try:
+        for after in (0, int(v[v.size // 2])):
+            t0 = time.perf_counter()
+            want = [oracle_row(i, after) for i in range(nrows)]
+            t_orc1 = time.perf_counter() - t0
+            t0 = time.perf_counter()
+            with ThreadPoolExecutor(max_workers=threads) as ex:   # ctypes releases the GIL
+                list(ex.map(lambda i: oracle_row(i, after), range(nrows)))
+            t_orcn = time.perf_counter() - t0
+            want_off = np.concatenate([[0], np.cumsum([w.size for w in want])]).astype(np.uint64)
+            want_all = np.concatenate(want) if want_off[-1] else np.zeros(0, np.uint64)
+            nout = int(want_off[-1])
+
+            def same(out, off):
+                return bool(np.array_equal(off, want_off) and np.array_equal(out[:nout], want_all))
+
+            def dev():
+                _lib.check(lib.dgx_dev_list_uids_rows(L.h, tab, p(mode), nrows, C.c_void_p(d_mu.data_ptr()),
+                                                      C.c_void_p(d_mf.data_ptr()), p(mut_off), after,
+                                                      C.c_void_p(d_v.data_ptr()), m, C.c_void_p(d_out.data_ptr()), cap,
+                                                      C.c_void_p(d_off.data_ptr())))
+            ms1, _ = timeit(dev, warm=3, reps=10)
+            L.sync()
+            ok1 = same(d_out[:nout].cpu().numpy().view(np.uint64), d_off.cpu().numpy().view(np.uint64))
+
+            def host():
+                _lib.check(lib.dgx_list_uids_rows(refs, p(mode), nrows, p(mu_all), p(mf_all), p(mut_off), after, p(hv), m,
+                                                  p(hout), p(hoff), cap))
+            ms2 = wall(host, 5)
+            ok2 = same(hout, hoff)
+            got3 = [None] * nrows
+
+            def today():
+                _lib.check(lib.dgx_intersect_compressed_rows(crefs, len(clean), after, p(hv), m, p(cout), p(coff), ccap))
+                for j, i in enumerate(clean):
+                    got3[i] = cout[int(coff[j]): int(coff[j + 1])]
+                with ThreadPoolExecutor(max_workers=threads) as ex:
+                    for i, r in zip(dirty, ex.map(lambda i: oracle_row(i, after), dirty)):
+                        got3[i] = r
+            ms3 = wall(today, 3)
+            ok3 = all(np.array_equal(got3[i], want[i]) for i in range(nrows))
+            cfg = (f"C9 handleUidPostings with mutable layers: the C6 task ({nrows} UidPacks, BlockSize 256, {exact} UIDs; "
+                   f"v of {m} UIDs); {len(dirty)} keys with a resolved layer of ~1 % of their length ({nmut} entries: "
+                   f"deletes, new uids, value postings), modes by the ApproxLen rule "
+                   f"({int((mode == 1).sum())} probe, {int((mode == 2).sum())} iterate); afterUID={after}")
+            extra = {"rows": nrows, "out": nout, "after": after, "mutable_entries": nmut, "rows_with_layer": len(dirty),
+                     "bytes_note": "algorithmic bytes here are 8 per pack uid, v uid, mutable entry and result uid: a "
+                                   "size of the work, not an HBM rate (packs are read compressed and probed sparsely)"}
+            for name, ms, ok, note in (
+                ("ListUidsRows (device, resident packs)", ms1, ok1, "dgx_dev_list_uids_rows, CUDA events"),
+                ("ListUidsRows (host, named packs, cache hits)", ms2, ok2, "dgx_list_uids_rows, wall clock incl. D2H"),
+                (f"clean rows batched + oracle List.Uids per layered row ({threads} threads)", ms3, ok3,
+                 "dgx_intersect_compressed_rows for keys without a layer, then the CPU for the rest, wall clock"),
+                ("oracle row loop (1 thread)", t_orc1 * 1e3, True, "List.Uids restated in C, one row after another"),
+                (f"oracle row loop ({threads} threads)", t_orcn * 1e3, True, "same, rows spread over host threads"),
+            ):
+                out_rows.append(row(name, cfg, ms, exact + m + nmut, 8 * (exact + m + nmut + nout), ok,
+                                    dict(extra, rows_per_s=nrows / (ms * 1e-3), note=note)))
+    finally:
+        for h in handles:
+            lib.dgx_dev_pack_free(h)
+        lib.dgx_cache_clear()
     return out_rows
 
 
