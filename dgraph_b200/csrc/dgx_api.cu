@@ -2009,7 +2009,7 @@ extern "C" void dgx_encode_bound(size_t n, uint32_t block_size, size_t* nblocks_
 
 struct EncOut {           // device arrays of one encoded pack (workspace memory)
     u64* base; u32* num; u64* delta_off; unsigned char* deltas; u64* counts;
-    size_t nblocks_cap, delta_cap;
+    size_t n, nblocks_cap, delta_cap;  // n: most uids encoded (the list's length when it is read from the device)
 };
 // Encodes d_u[0..n) (n from *d_n when d_n != nullptr, at most n) into workspace arrays.
 static int encode_impl(dgx_lane* l, const uint64_t* d_u, size_t n, const uint64_t* d_n, uint32_t block_size,
@@ -2068,7 +2068,7 @@ static int encode_impl(dgx_lane* l, const uint64_t* d_u, size_t n, const uint64_
     l->launches += 5;
     g_stats.launches += 5;
     out->base = P.base; out->num = P.num; out->delta_off = P.delta_off; out->deltas = P.deltas; out->counts = P.counts;
-    out->nblocks_cap = nblocks_cap; out->delta_cap = delta_cap;
+    out->n = n; out->nblocks_cap = nblocks_cap; out->delta_cap = delta_cap;
     return DGX_OK;
 }
 
@@ -2078,7 +2078,10 @@ static int encode_to_host(dgx_lane* l, const EncOut& E, uint32_t block_size, uin
     CK(cudaMemcpyAsync(l->h_word, E.counts, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
     int rc = dgx_lane_sync(l);
     if (rc) return rc;
-    const uint64_t nb = l->h_word[1], db = l->h_word[2];
+    const uint64_t nb = l->h_word[1];
+    // the deltas are sized only when the blocks fit; otherwise the call again needs room for the most that nb blocks
+    // of n uids can take (every group is at most 17 bytes), so that it does not fail a second time on the deltas
+    const uint64_t db = nb > E.nblocks_cap ? 17 * (E.n / 4 + nb + 1) : l->h_word[2];
     const size_t cap_nb = *nblocks, cap_db = *delta_bytes;
     *nblocks = (size_t)nb;
     *delta_bytes = (size_t)db;
@@ -2179,6 +2182,7 @@ static int packed_op_host(int kind /*0 intersect, 1 difference, 2 merge*/, const
     size_t nb_cap, db_cap;
     dgx_encode_bound(cap, block_size, &nb_cap, &db_cap);
     nb_cap = std::max(nb_cap, std::min(*nblocks, cap));  // a larger capacity from the caller is honoured
+    db_cap = std::max(db_cap, 17 * (cap / 4 + nb_cap + 1));  // and room for the deltas of that many blocks
     EncOut E;
     rc = encode_impl(l, (const uint64_t*)d_out, cap, (const uint64_t*)d_len, block_size, nb_cap, db_cap, &E);
     if (rc) return rc;

@@ -15,6 +15,8 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(__file__))
 import gen  # noqa: E402
+import merge_geometry  # noqa: E402
+from merge_geometry import tree_launches as _tree_launches  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -428,31 +430,10 @@ def test_properties_at_scale(dgx):
 
 # ---- MergeSorted: the multiway merge and its grouping --------------------------------------
 
-MERGE_MULTI_MIN = 1 << 18  # merge_runs_impl (dgx_api.cu): smallest total that leaves the pairwise tree
-MM_K = 64                  # largest fan-in of one multiway merge
-
-
-def _tree_launches(k):
-    """merge_tree_impl: one merge_kernel launch per level; a single run still takes one (in-run de-duplication)."""
-    levels = 0
-    while k > 1:
-        k, levels = (k + 1) // 2, levels + 1
-    return max(levels, 1)
-
-
 def _merge_plan(lens):
-    """(path, kernel launches) of merge_runs_impl for non-empty runs of these lengths."""
-    k, total = len(lens), sum(lens)
-    if 3 <= k <= MM_K and total >= MERGE_MULTI_MIN:
-        # merge_multi_impl: msample, the tree over the non-empty sample runs, mplan2, mmerge3, mscan, mcompact
-        ntarget = min(max(total // 512, 1), 1 << 24)
-        return "multiway", 5 + _tree_launches(sum(1 for n in lens if n * ntarget // total))
-    ngroups = -(-k // MM_K)
-    if k <= MM_K or total // ngroups < 4 * MERGE_MULTI_MIN:
-        return "tree", _tree_launches(k)
-    gsz = -(-k // ngroups)
-    groups = [lens[b:b + gsz] for b in range(0, k, gsz)]
-    return "grouped", sum(_merge_plan(g)[1] for g in groups) + _merge_plan([sum(g) for g in groups])[1]
+    """(path, kernel launches) of merge_runs_impl for non-empty runs of these lengths (tests/merge_geometry.py)."""
+    plan = merge_geometry.merge_plan(lens)
+    return plan.path, plan.launches
 
 
 def _random_k(k, lo, hi):
