@@ -233,6 +233,56 @@ def ListUidsRows(packs, modes, muts, afterUID: int, v, keys=None):
     return out[: int(out_off[-1])], out_off
 
 
+def _mut_csr(muts):
+    """The resolved mutable layers of a task's rows as one CSR: (uids, flags, off), never empty arrays."""
+    mu = [np.zeros(0, np.uint64) if t is None else _u64(t[0]) for t in muts]
+    mf = [np.zeros(0, np.uint8) if t is None else np.ascontiguousarray(np.asarray(t[1], np.uint8)) for t in muts]
+    off = np.zeros(len(muts) + 1, dtype=np.uint64)
+    np.cumsum([a.size for a in mu], out=off[1:])
+    n = int(off[-1])
+    return (np.concatenate(mu) if n else np.zeros(1, np.uint64)), (np.concatenate(mf) if n else np.zeros(1, np.uint8)), off
+
+
+def ListUidsUnfilteredRows(packs, muts, afterUID: int, first: int = 0, keys=None):
+    """posting.List.Uids(opts) with opts.Intersect == nil for every key of a task in ONE call
+    (dgx_list_uids_unfiltered_rows): the handleUidPostings loop (worker/task.go:783-987) of a plain edge traversal over
+    unsplit lists, mutable layers included.
+
+    packs[i]: the immutable layer (None for an empty one, or for a delete-all marker).  muts[i]: None or (uids, flags),
+    the resolved mutable entries of row i, strictly ascending, flags MUT_DEL / MUT_VALUE.  first: opts.First as an
+    int32 (0 is MaxInt32; a negative value keeps at most one uid).  keys: optional [(key, version)] naming each pack for
+    the HBM-resident cache.  Returns (out, out_off): row i is out[out_off[i]:out_off[i+1]]."""
+    nrows = len(packs)
+    if nrows == 0:
+        return np.zeros(0, np.uint64), np.zeros(1, np.uint64)
+    mut_uids, mut_flags, mut_off = _mut_csr(muts)
+    lib = _lib.load()
+    refs, keep = _refs_of(packs, keys)
+    most = 0x7FFFFFFF if first == 0 else (1 if first < 0 else first)
+    cap = sum(min(most, (_exact(p) if p is not None else 0) + int(mut_off[i + 1] - mut_off[i]))
+              for i, p in enumerate(packs))
+    out = np.empty(max(cap, 1), dtype=np.uint64)
+    out_off = np.zeros(nrows + 1, dtype=np.uint64)
+    _lib.check(lib.dgx_list_uids_unfiltered_rows(refs, nrows, _p(mut_uids), _p(mut_flags), _p(mut_off), afterUID, first,
+                                                 _p(out), _p(out_off), cap))
+    return out[: int(out_off[-1])], out_off
+
+
+def ListCountRows(packs, muts, afterUID: int, keys=None):
+    """countForUidPostings with a nil facets tree (worker/task.go:743-755, 866-876) for every key of a task in ONE call
+    (dgx_list_count_rows): the REF postings List.Postings yields above afterUID, mutable layers included.  Arguments as
+    in ListUidsUnfilteredRows.  Returns a uint32 array of counts."""
+    nrows = len(packs)
+    counts = np.zeros(nrows, dtype=np.uint32)
+    if nrows == 0:
+        return counts
+    mut_uids, mut_flags, mut_off = _mut_csr(muts)
+    refs, keep = _refs_of(packs, keys)
+    _lib.check(_lib.load().dgx_list_count_rows(refs, nrows, _p(mut_uids), _p(mut_flags), _p(mut_off), afterUID,
+                                               _p(counts)))
+    return counts
+
+
 def IntersectCompressedWithMatrix(pack, rows, key=None):
     """algo.IntersectCompressedWith(pack, 0, rows[i], o_i) for every row i in ONE call
     (dgx_intersect_compressed_matrix): the intersectBucket loop (worker/sort.go:605-700) of one index bucket over a

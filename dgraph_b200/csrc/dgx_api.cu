@@ -35,6 +35,7 @@
 #include "probe_kernel.cuh"
 #include "compressed_kernel.cuh"
 #include "list_uids_kernel.cuh"
+#include "list_uids_unfiltered_kernel.cuh"
 #include "encode_kernel.cuh"
 #include "wire.hpp"
 
@@ -451,7 +452,7 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
         if (flag & kLaneErrOrder) return fail(DGX_ERR_ARG, "a row of the uid matrix is not strictly ascending");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
-                                     "flags) or a probe / iterate row's pack starts at uid 0");
+                                     "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
         return fail(DGX_ERR_CAP, "result does not fit out_cap");
     }
     return DGX_OK;
@@ -2756,6 +2757,249 @@ extern "C" int dgx_list_uids_rows(const dgx_pack_ref* refs, const uint8_t* mode,
                         (uint64_t*)d_out, cap, (uint64_t*)d_off);
     if (rc) return rc;
     return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
+}
+
+// ---------------------------------------------------------------------------
+// List.Uids without a filter, and the count of the same postings, over a task's keys (handleUidPostings)
+// ---------------------------------------------------------------------------
+// The host-side checks of the four entry points, before anything is copied: offsets, and the bounds that keep |S_i|
+// and the class fields below 2^31.  exact(i) is ExactLen of row i's pack.
+template <class ExactLen>
+static int list_unfiltered_check(size_t nrows, const uint64_t* mut_off, ExactLen exact) {
+    const uint64_t k31 = uint64_t(1) << 31;
+    if (mut_off[0] != 0) return fail(DGX_ERR_ARG, "mut_off[0] is %llu, not 0", (unsigned long long)mut_off[0]);
+    for (size_t r = 0; r < nrows; ++r) {
+        if (mut_off[r + 1] < mut_off[r]) return fail(DGX_ERR_ARG, "mut_off decreases at row %zu", r);
+        const uint64_t nm = mut_off[r + 1] - mut_off[r];
+        if (exact(r) + nm >= k31)
+            return fail(DGX_ERR_ARG, "row %zu has %llu postings: at most 2^31 - 1", r, (unsigned long long)(exact(r) + nm));
+    }
+    if (mut_off[nrows] >= k31)
+        return fail(DGX_ERR_ARG, "the mutable layers have %llu entries: at most 2^31 - 1", (unsigned long long)mut_off[nrows]);
+    return DGX_OK;
+}
+
+// The most values a row keeps for opts.First (posting/list.go:1759-1761, 1841-1843, 1864-1872): 0 is MaxInt32; a
+// negative First stops the callback after the first value and the cut keeps it.
+static uint64_t first_keep(int32_t first) { return first == 0 ? 0x7fffffffull : first < 0 ? 1 : (uint64_t)first; }
+
+// Rows (d_counts == nullptr) or counts of the unfiltered read (list_uids_unfiltered_kernel.cuh): classify, entry scan,
+// rows, and for rows a row scan and the write, so 5 or 3 launches whatever the row count, entry count and pack sizes
+// are.  mut_off is host memory, already checked.
+static int list_unfiltered_impl(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows, const uint64_t* d_mut,
+                                const uint8_t* d_flags, const uint64_t* mut_off, uint64_t after, uint64_t first,
+                                uint64_t* d_out, size_t out_cap, uint64_t* d_out_off, uint32_t* d_counts) {
+    const uint64_t nmut = mut_off[nrows];
+    size_t nj = 0;
+    for (size_t i = 0; i < nrows; ++i)
+        if (packs[i] && packs[i]->pk.nblocks) ++nj;
+    if (nj >= kLuuNoJob) return fail(DGX_ERR_ARG, "batch too large for one launch (%zu rows)", nrows);
+    // table (copied): [jobs | row_job | mut_off | nmut | nrows];  zeroed: [scan status + tickets | bad];  then cls,
+    // cls_ex, rank, skip, sblk, len
+    const size_t b_jobs = (nj * sizeof(LuuJob) + 15) & ~size_t(15), b_rj = (nrows * sizeof(u32) + 15) & ~size_t(15);
+    const size_t b_tab = b_jobs + b_rj + (nrows + 3) * sizeof(uint64_t);
+    void* h_raw;
+    int rc = l->host.alloc(b_tab, &h_raw);
+    if (rc) return rc;
+    LuuJob* hj = (LuuJob*)h_raw;
+    u32* h_rj = (u32*)((char*)h_raw + b_jobs);
+    uint64_t* h_off = (uint64_t*)((char*)h_raw + b_jobs + b_rj);
+    uint64_t warps = 0, exact = 0;
+    for (size_t i = 0, j = 0; i < nrows; ++i) {
+        const dgx_dev_pack* p = packs[i];
+        if (!p || p->pk.nblocks == 0) { h_rj[i] = kLuuNoJob; continue; }
+        h_rj[i] = (u32)j;
+        LuuJob& J = hj[j++];
+        J.pk = p->pk;
+        J.row = i;
+        J.warp_base = warps;
+        warps += (p->pk.nblocks + D_BPW - 1) / D_BPW;
+        exact += p->exact_len;
+    }
+    memcpy(h_off, mut_off, (nrows + 1) * sizeof(uint64_t));
+    h_off[nrows + 1] = nmut;
+    h_off[nrows + 2] = nrows;
+    const uint64_t kMaxGrid = 0x7fffffffull;
+    const uint64_t g_cls = (nmut + nrows + 255) / 256, g_rows = (nrows + 255) / 256;
+    const uint64_t g_write = (warps + D_WARPS - 1) / D_WARPS + (nmut + D_NT - 1) / D_NT;
+    const uint64_t t_mut = std::max<uint64_t>((nmut + EN_TILE - 1) / EN_TILE, 1), t_rows = (nrows + EN_TILE - 1) / EN_TILE;
+    if (std::max({g_cls, g_write}) > kMaxGrid)
+        return fail(DGX_ERR_ARG, "batch too large for one launch (%llu entries, %zu rows)", (unsigned long long)nmut, nrows);
+    const size_t b_zero = (t_mut + t_rows) * sizeof(u64) + 16;
+    const size_t b_rest = (3 * nmut + 1 + 3 * nrows) * sizeof(u64);
+    void* d_raw;
+    rc = l->ws.alloc(b_tab + b_zero + b_rest, &d_raw);
+    if (rc) return rc;
+    char* d = (char*)d_raw;
+    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
+    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
+    g_stats.h2d += b_tab;
+    LuuParams P;
+    P.jobs = (const LuuJob*)d;
+    P.njobs = (u32)nj;
+    P.nwarps = warps;
+    P.row_job = (const u32*)(d + b_jobs);
+    P.mut_off = (const u64*)(d + b_jobs + b_rj);
+    const u64* d_nmut = P.mut_off + nrows + 1;  // scan lengths as device words
+    const u64* d_nrows = d_nmut + 1;
+    P.nrows = nrows;
+    P.mut = (const u64*)d_mut;
+    P.flags = d_flags;
+    P.nmut = nmut;
+    P.after = after;
+    P.first = first;
+    u64* status = (u64*)(d + b_tab);
+    u32* tickets = (u32*)(status + t_mut + t_rows);
+    P.bad = (int*)(tickets + 2);
+    P.cls = (u64*)(d + b_tab + b_zero);
+    P.cls_ex = P.cls + nmut;
+    P.rank = P.cls_ex + nmut + 1;
+    P.skip = P.rank + nmut;
+    P.sblk = P.skip + nrows;
+    P.len = P.sblk + nrows;
+    P.counts = d_counts;
+    P.out = (u64*)d_out;
+    P.out_cap = out_cap;
+    P.out_off = (u64*)d_out_off;
+    P.err = l->d_err;
+    luu_classify_kernel<<<(unsigned)g_cls, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    scan_u64_kernel<<<(unsigned)t_mut, EN_NT, 0, l->stream>>>(P.cls, P.cls_ex, d_nmut, nmut, status, tickets, nullptr);
+    CK(cudaGetLastError());
+    luu_rows_kernel<<<(unsigned)g_rows, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    int launches = 3;
+    if (!d_counts) {
+        scan_u64_kernel<<<(unsigned)t_rows, EN_NT, 0, l->stream>>>(P.len, P.out_off, d_nrows, nrows, status + t_mut,
+                                                                    tickets + 1, nullptr);
+        CK(cudaGetLastError());
+        luu_write_kernel<<<(unsigned)std::max<uint64_t>(g_write, 1), D_NT, sizeof(DWarpSmem) * D_WARPS, l->stream>>>(P);
+        CK(cudaGetLastError());
+        launches = 5;
+    }
+    l->launches += launches;
+    g_stats.launches += launches;
+    g_stats.uids_in += exact + nmut;
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_list_uids_unfiltered_rows(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows,
+                                                 const uint64_t* d_mut_uids, const uint8_t* d_mut_flags,
+                                                 const uint64_t* mut_off, uint64_t after_uid, int32_t first,
+                                                 uint64_t* d_out, size_t out_cap, uint64_t* d_out_off) {
+    if (!l || !d_out_off) return fail(DGX_ERR_ARG, "null argument");
+    if (nrows == 0) {
+        if (int rc = lane_begin_op(l)) return rc;
+        CK(cudaMemsetAsync(d_out_off, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (!packs || !mut_off) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = list_unfiltered_check(nrows, mut_off, [&](size_t r) -> uint64_t {
+            return packs[r] ? packs[r]->exact_len : 0;
+        }))
+        return rc;
+    if (mut_off[nrows] && (!d_mut_uids || !d_mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    const int rc = list_unfiltered_impl(l, packs, nrows, d_mut_uids, d_mut_flags, mut_off, after_uid, first_keep(first),
+                                        d_out, out_cap, d_out_off, nullptr);
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    return rc;
+}
+
+extern "C" int dgx_dev_list_count_rows(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows,
+                                       const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
+                                       uint64_t after_uid, uint32_t* d_counts) {
+    if (!l) return fail(DGX_ERR_ARG, "null lane");
+    if (nrows == 0) return DGX_OK;
+    if (!packs || !mut_off || !d_counts) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = list_unfiltered_check(nrows, mut_off, [&](size_t r) -> uint64_t {
+            return packs[r] ? packs[r]->exact_len : 0;
+        }))
+        return rc;
+    if (mut_off[nrows] && (!d_mut_uids || !d_mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    const int rc = list_unfiltered_impl(l, packs, nrows, d_mut_uids, d_mut_flags, mut_off, after_uid, first_keep(0),
+                                        nullptr, 0, nullptr, d_counts);
+    l->note_output(d_counts, nrows * sizeof(uint32_t));
+    return rc;
+}
+
+// The host forms: packs staged as in dgx_list_uids_rows, the layers as one copy of uids and one of flags; returns
+// the rows (counts == nullptr) or the counts to the host.
+static int list_unfiltered_host(const dgx_pack_ref* refs, size_t nrows, const uint64_t* mut_uids,
+                                const uint8_t* mut_flags, const uint64_t* mut_off, uint64_t after_uid, int32_t first,
+                                uint64_t* out, uint64_t* out_off, size_t out_cap, uint32_t* counts) {
+    if (!refs || !mut_off) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = list_unfiltered_check(nrows, mut_off, [&](size_t r) -> uint64_t {
+            const dgx_pack_view* p = refs[r].pack;
+            uint64_t n = 0;
+            for (size_t b = 0; p && b < p->nblocks; ++b) n += p->num_uids[b];
+            return n;
+        }))
+        return rc;
+    const uint64_t nmut = mut_off[nrows];
+    if (nmut && (!mut_uids || !mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    PackSet ps(l, refs, nrows);  // nil / empty packs are packs of no blocks
+    if (ps.rc) return ps.rc;
+    const uint64_t keep = first_keep(first);
+    std::vector<const dgx_dev_pack*> rows(nrows);
+    size_t cap = 0;
+    for (size_t i = 0; i < nrows; ++i) {
+        rows[i] = &ps.pk[i];
+        cap += std::min<uint64_t>(keep, ps.pk[i].exact_len + (mut_off[i + 1] - mut_off[i]));
+    }
+    uint64_t* d_mut;
+    int rc = upload_list(l, mut_uids, nmut, &d_mut);
+    if (rc) return rc;
+    void* d_flags;
+    rc = l->ws.alloc(nmut + 16, &d_flags);
+    if (rc) return rc;
+    if (nmut) CK(cudaMemcpyAsync(d_flags, mut_flags, nmut, cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += nmut;
+    if (counts) {
+        void* d_counts;
+        rc = l->ws.alloc(nrows * sizeof(uint32_t), &d_counts);
+        if (rc) return rc;
+        rc = list_unfiltered_impl(l, rows.data(), nrows, d_mut, (const uint8_t*)d_flags, mut_off, after_uid, keep,
+                                  nullptr, 0, nullptr, (uint32_t*)d_counts);
+        if (rc) return rc;
+        CK(cudaMemcpyAsync(counts, d_counts, nrows * sizeof(uint32_t), cudaMemcpyDeviceToHost, l->stream));
+        g_stats.d2h += nrows * sizeof(uint32_t);
+        return ps.synced(dgx_lane_sync(l));
+    }
+    void *d_out, *d_off;
+    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
+    if (rc) return rc;
+    rc = list_unfiltered_impl(l, rows.data(), nrows, d_mut, (const uint8_t*)d_flags, mut_off, after_uid, keep,
+                              (uint64_t*)d_out, cap, (uint64_t*)d_off, nullptr);
+    if (rc) return rc;
+    return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
+}
+
+extern "C" int dgx_list_uids_unfiltered_rows(const dgx_pack_ref* refs, size_t nrows, const uint64_t* mut_uids,
+                                             const uint8_t* mut_flags, const uint64_t* mut_off, uint64_t after_uid,
+                                             int32_t first, uint64_t* out, uint64_t* out_off, size_t out_cap) {
+    if (!out_off) return fail(DGX_ERR_ARG, "null out_off");
+    if (nrows == 0) { out_off[0] = 0; return DGX_OK; }
+    return list_unfiltered_host(refs, nrows, mut_uids, mut_flags, mut_off, after_uid, first, out, out_off, out_cap,
+                                nullptr);
+}
+
+extern "C" int dgx_list_count_rows(const dgx_pack_ref* refs, size_t nrows, const uint64_t* mut_uids,
+                                   const uint8_t* mut_flags, const uint64_t* mut_off, uint64_t after_uid,
+                                   uint32_t* counts) {
+    if (nrows == 0) return DGX_OK;
+    if (!counts) return fail(DGX_ERR_ARG, "null counts");
+    return list_unfiltered_host(refs, nrows, mut_uids, mut_flags, mut_off, after_uid, 0, nullptr, nullptr, 0, counts);
 }
 
 // ---------------------------------------------------------------------------

@@ -16,6 +16,7 @@ package codec
 import "C"
 
 import (
+	"math"
 	"unsafe"
 
 	"github.com/dgraph-io/dgraph/v25/protos/pb"
@@ -517,4 +518,159 @@ func ListUidsRows(refs []PackRef, modes []uint8, muts []MutRow, afterUID uint64,
 		}
 	}
 	return rows, true
+}
+
+// unfilteredStage holds what the unfiltered and count calls pass: the packs staged as in ListUidsRows and the mutable
+// layers as one C allocation [mut_off (n + 1) | mut_uids (nmut, plus one spare word) | mut_flags (nmut bytes)].
+type unfilteredStage struct {
+	crefs *C.dgx_pack_ref
+	off   *C.uint64_t
+	uids  *C.uint64_t
+	flags *C.uint8_t
+	exact []int // ExactLen + |mut| per key
+	free  func()
+}
+
+// stageUnfiltered stages a task's keys for dgx_list_uids_unfiltered_rows / dgx_list_count_rows.  It returns false
+// when the batch is too small to pay for a call or the input is malformed.
+func stageUnfiltered(refs []PackRef, muts []MutRow) (*unfilteredStage, bool) {
+	n := len(refs)
+	if len(muts) != n {
+		return nil, false
+	}
+	total, img, nmut := 0, 0, 0
+	exact := make([]int, n)
+	for i, r := range refs {
+		if len(muts[i].Flags) != len(muts[i].Uids) {
+			return nil, false
+		}
+		nmut += len(muts[i].Uids)
+		exact[i] = len(muts[i].Uids)
+		if r.Pack != nil && len(r.Pack.Blocks) > 0 {
+			total += ApproxLen(r.Pack)
+			exact[i] += ExactLen(r.Pack)
+			if r.Key == 0 {
+				img += int(C.dgx_pack_image_size(C.size_t(len(r.Pack.Blocks)), C.size_t(deltaBytes(r.Pack))))
+			}
+		}
+	}
+	if total+nmut < dgxMinDecode || nmut >= 1<<31 {
+		return nil, false
+	}
+	csr := C.malloc(C.size_t((n+2+nmut)*8 + nmut + 16))
+	crefs := (*[1 << 28]C.dgx_pack_ref)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(C.dgx_pack_ref{}))))
+	views := (*[1 << 28]C.dgx_pack_view)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(C.dgx_pack_view{}))))
+	stage := C.malloc(C.size_t(img + 64))
+	frees := []func(){}
+	s := &unfilteredStage{exact: exact, free: func() {
+		for _, f := range frees {
+			f()
+		}
+		C.free(csr)
+		C.free(unsafe.Pointer(crefs))
+		C.free(unsafe.Pointer(views))
+		C.free(stage)
+	}}
+	words := unsafe.Slice((*uint64)(csr), n+2+nmut)
+	flags := unsafe.Slice((*uint8)(unsafe.Add(csr, (n+2+nmut)*8)), nmut+1)
+	w := 0
+	for i, mr := range muts {
+		words[i] = uint64(w)
+		copy(words[n+1+w:], mr.Uids)
+		copy(flags[w:], mr.Flags)
+		w += len(mr.Uids)
+	}
+	words[n] = uint64(w)
+	o := 0
+	for i, r := range refs {
+		crefs[i] = C.dgx_pack_ref{key: C.uint64_t(r.Key), version: C.uint64_t(r.Version)}
+		if r.Pack == nil || len(r.Pack.Blocks) == 0 {
+			continue // delete-all marker or empty immutable layer
+		}
+		if r.Key != 0 {
+			view, free := flatten(r.Pack)
+			frees = append(frees, free)
+			views[i] = view
+		} else {
+			nb, db := len(r.Pack.Blocks), deltaBytes(r.Pack)
+			if C.dgx_pack_image_view(unsafe.Add(stage, o), C.uint32_t(r.Pack.BlockSize), C.size_t(nb), C.size_t(db), &views[i]) != C.DGX_OK {
+				s.free()
+				return nil, false
+			}
+			fillImage(&views[i], r.Pack)
+			o += int(C.dgx_pack_image_size(C.size_t(nb), C.size_t(db)))
+		}
+		crefs[i].pack = &views[i]
+	}
+	s.crefs = &crefs[0]
+	s.off = (*C.uint64_t)(unsafe.Pointer(&words[0]))
+	s.uids = (*C.uint64_t)(unsafe.Pointer(&words[n+1]))
+	s.flags = (*C.uint8_t)(unsafe.Pointer(&flags[0]))
+	return s, true
+}
+
+// ListUidsUnfilteredRows is posting.List.Uids(opts) with opts.Intersect == nil (posting/list.go:1758-1874) for every
+// key of a task in ONE library call: the default branch of handleUidPostings without facets (worker/task.go:960-967)
+// over unsplit lists, mutable layers included (INTEGRATION §2 lists the keys that qualify).  refs[i].Pack is nil for a
+// key whose delete-all marker hides the immutable layer; first is opts.First.  Returns false when the caller must keep
+// pl.Uids.
+func ListUidsUnfilteredRows(refs []PackRef, muts []MutRow, afterUID uint64, first int32) ([]*pb.List, bool) {
+	n := len(refs)
+	if n == 0 {
+		return []*pb.List{}, true
+	}
+	s, ok := stageUnfiltered(refs, muts)
+	if !ok {
+		return nil, false
+	}
+	defer s.free()
+	keep := int(first)
+	if first == 0 {
+		keep = math.MaxInt32
+	} else if first < 0 {
+		keep = 1
+	}
+	capOut := 0
+	for _, e := range s.exact {
+		if e < keep {
+			capOut += e
+		} else {
+			capOut += keep
+		}
+	}
+	out := make([]uint64, capOut+1)
+	off := make([]uint64, n+1)
+	if C.dgx_list_uids_unfiltered_rows(s.crefs, C.size_t(n), s.uids, s.flags, s.off, C.uint64_t(afterUID), C.int32_t(first),
+		(*C.uint64_t)(unsafe.Pointer(&out[0])), (*C.uint64_t)(unsafe.Pointer(&off[0])), C.size_t(capOut)) != C.DGX_OK {
+		return nil, false
+	}
+	rows := make([]*pb.List, n)
+	for i := range refs {
+		rows[i] = &pb.List{}
+		if off[i+1] > off[i] {
+			rows[i].Uids = out[off[i]:off[i+1]:off[i+1]]
+		}
+	}
+	return rows, true
+}
+
+// ListCountRows is countForUidPostings with a nil facets tree (worker/task.go:743-755) for every key of a task in ONE
+// library call: the DoCount branch of handleUidPostings (:866-876), the REF postings List.Postings yields above
+// afterUID.  Arguments as in ListUidsUnfilteredRows.  Returns false when the caller must keep the count loop.
+func ListCountRows(refs []PackRef, muts []MutRow, afterUID uint64) ([]uint32, bool) {
+	n := len(refs)
+	if n == 0 {
+		return []uint32{}, true
+	}
+	s, ok := stageUnfiltered(refs, muts)
+	if !ok {
+		return nil, false
+	}
+	defer s.free()
+	counts := make([]uint32, n)
+	if C.dgx_list_count_rows(s.crefs, C.size_t(n), s.uids, s.flags, s.off, C.uint64_t(afterUID),
+		(*C.uint32_t)(unsafe.Pointer(&counts[0]))) != C.DGX_OK {
+		return nil, false
+	}
+	return counts, true
 }

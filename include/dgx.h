@@ -252,6 +252,37 @@ int dgx_list_uids_rows(const dgx_pack_ref* refs, const uint8_t* mode, size_t nro
                        uint64_t after_uid, const uint64_t* v, size_t m,
                        uint64_t* out, uint64_t* out_off, size_t out_cap);
 
+/* posting.List.Uids(opts) with opts.Intersect == nil for every key of a task, mutable layers included, one call: the
+ * handleUidPostings loop (worker/task.go:783-987, the default branch without facets) of a plain edge traversal over
+ * unsplit lists.  Every row runs iterate(readTs, after_uid) with the REF filter (posting/list.go:1116-1232, 1830-1845)
+ * and the First cut (:1864-1872).  With refs / mut_* / mut_off as in dgx_list_uids_rows (NULL pack: delete-all marker
+ * or empty immutable layer; mut(x) the first posting of pickPostings for uid x):
+ *   S_i = {x > after_uid : mut_i(x) exists ? mut_i(x) has no flag : x in pack_i}
+ * The pack side is Decoder.Seek(after_uid, SeekCurrent), the mutable side starts at the first entry above after_uid.
+ * first = opts.First as the worker passes it (q.First + q.Offset): 0 means MaxInt32; first > 0 keeps the first
+ * smallest values of S_i; first < 0 keeps min(|S_i|, 1) values, as the callback stops after one value and the
+ * negative cut keeps it.  Row i of the CSR result is out[out_off[i] .. out_off[i+1]); out_cap >=
+ * sum_i min(first_eff, ExactLen(pack_i) + |mut_i|) always suffices (first_eff: the values a row keeps); a longer
+ * result than out_cap is DGX_ERR_CAP and nothing is written past out_cap.  nrows == 0 gives out_off[0] = 0 and needs
+ * no device.
+ * DGX_ERR_ARG before anything is copied: mut_off[0] != 0 or decreasing offsets, 2^31 or more mutable entries in all, a
+ * row with ExactLen + |mut| >= 2^31, a null array that is needed.
+ * DGX_ERR_ARG after the kernels, with out untouched and out_off zeroed: a mutable entry that does not ascend strictly,
+ * is 0 or has other flag bits, or a non-NULL pack that starts at uid 0.  The call runs a fixed number of kernel
+ * launches whatever nrows, the number of mutable entries and the pack sizes are; a block of a pack is read only when
+ * it holds a value of the row above after_uid and within the first cut. */
+int dgx_list_uids_unfiltered_rows(const dgx_pack_ref* refs, size_t nrows,
+                                  const uint64_t* mut_uids, const uint8_t* mut_flags, const uint64_t* mut_off,
+                                  uint64_t after_uid, int32_t first,
+                                  uint64_t* out, uint64_t* out_off, size_t out_cap);
+/* countForUidPostings with a nil facets tree (worker/task.go:743-755, 866-876) for every key of a task:
+ * counts[i] = |S_i| as above, which List.Postings (posting/list.go:1878-1890) yields; First plays no part.  Arguments
+ * and errors as in dgx_list_uids_unfiltered_rows; a device-detected error zeroes counts.  Only the block each row's
+ * seek lands in and the block each entry lands in are read. */
+int dgx_list_count_rows(const dgx_pack_ref* refs, size_t nrows,
+                        const uint64_t* mut_uids, const uint8_t* mut_flags, const uint64_t* mut_off,
+                        uint64_t after_uid, uint32_t* counts);
+
 /* algo.MergeSorted(rows) over the rows of a uid matrix, one call: sg.DestUIDs = algo.MergeSorted(result.UidMatrix)
  * (query/query.go:2290, 2505; query/recurse.go:134; worker/task.go:1629, 1706; worker/match.go:100).
  * Row i is v[v_off[i] .. v_off[i+1]) (host offsets, nrows + 1 values, v_off[0] == 0).  Rows ascend; duplicates
@@ -423,6 +454,19 @@ int dgx_dev_list_uids_rows(dgx_lane* lane, const dgx_dev_pack* const* packs, con
                            const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
                            uint64_t after_uid, const uint64_t* d_v, size_t m,
                            uint64_t* d_out, size_t out_cap, uint64_t* d_out_off);
+/* Device forms of dgx_list_uids_unfiltered_rows and dgx_list_count_rows: packs resident (dgx_dev_pack_upload; NULL =
+ * empty pack or delete-all marker), d_mut_uids / d_mut_flags / d_out / d_out_off (nrows + 1 values) / d_counts (nrows
+ * values) device pointers; mut_off in HOST memory, checked as in the host forms before anything is queued.
+ * Asynchronous on the lane: past out_cap nothing is written and the next dgx_lane_sync returns DGX_ERR_CAP; a malformed
+ * mutable entry or a pack that starts at uid 0 leaves d_out untouched, zeroes d_out_off / d_counts and makes the next
+ * dgx_lane_sync return DGX_ERR_ARG. */
+int dgx_dev_list_uids_unfiltered_rows(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t nrows,
+                                      const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
+                                      uint64_t after_uid, int32_t first,
+                                      uint64_t* d_out, size_t out_cap, uint64_t* d_out_off);
+int dgx_dev_list_count_rows(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t nrows,
+                            const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
+                            uint64_t after_uid, uint32_t* d_counts);
 /* Device form of dgx_merge_sorted_matrix: d_v and d_v_off (nrows + 1 values) are DEVICE pointers, so the
  * (d_out, d_out_off) of dgx_dev_intersect_compressed_rows / dgx_dev_filter_batch feed it directly.  v_cap >=
  * d_v_off[nrows] sizes the workspace (v_cap >= 2^32 is DGX_ERR_ARG).  d_out_len: one device uint64, the result length.

@@ -135,6 +135,7 @@ def main():
     ap.add_argument("--c7-only", action="store_true", help="only the C7 sort-bucket rows")
     ap.add_argument("--c8-only", action="store_true", help="only the C8 DestUIDs (MergeSorted of a uid matrix) rows")
     ap.add_argument("--c9-only", action="store_true", help="only the C9 List.Uids rows with mutable layers")
+    ap.add_argument("--c10-only", action="store_true", help="only the C10 unfiltered List.Uids and count rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -144,9 +145,11 @@ def main():
         rows = c8_rows(Lane())
     elif args.c9_only:
         rows = c9_rows(Lane())
+    elif args.c10_only:
+        rows = c10_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -888,6 +891,159 @@ def c9_rows(L, threads: int = 16):
             ):
                 out_rows.append(row(name, cfg, ms, exact + m + nmut, 8 * (exact + m + nmut + nout), ok,
                                     dict(extra, rows_per_s=nrows / (ms * 1e-3), note=note)))
+    finally:
+        for h in handles:
+            lib.dgx_dev_pack_free(h)
+        lib.dgx_cache_clear()
+    return out_rows
+
+
+def c10_rows(L, threads: int = 16):
+    """C10 "handleUidPostings without a filter": the C9 task (the C6 packs, mutable layers on 30 % of the keys) read as
+    a plain edge traversal (List.Uids with Intersect == nil) and as count(pred), at after = 0 and after = the master's
+    median, with first = MaxInt32 (opts.First 0), first = 10 and as counts.  Legs on the same inputs, each checked row
+    by row against the oracle's unfiltered List.Uids / count: (1) the device form on resident packs (CUDA events),
+    (2) the host form with named packs in steady state, (3) today's path: the oracle per key on 1 and on `threads`
+    host threads."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    import gen_mut
+    import gen_mut_unfiltered
+    import gen_rows
+    import list_uids_unfiltered_oracle as luo
+    from oracle import pyoracle as orc
+
+    lib = L.lib
+    master, rows_u, _ = gen_rows.c6_inputs()
+    nrows = len(rows_u)
+    ops = [orc.encode(r, 256) for r in rows_u]
+    rng = np.random.default_rng(909)
+    muts = []
+    for r, op in zip(rows_u, ops):  # the C9 layers (the same draws)
+        layer = rng.random() < 0.3
+        muts.append(gen_mut.layer(rng, r, master, max(1, r.size // 100)) if layer else (np.zeros(0, np.uint64),
+                                                                                        np.zeros(0, np.uint8)))
+    exact = sum(r.size for r in rows_u)
+    del rows_u
+    mut_off = np.zeros(nrows + 1, np.uint64)
+    np.cumsum([t[0].size for t in muts], out=mut_off[1:])
+    mu_all = np.concatenate([t[0] for t in muts])
+    mf_all = np.concatenate([t[1] for t in muts])
+    nmut = int(mut_off[-1])
+    views = []
+    for op in ops:
+        arrs = (op.base, op.num_uids, op.delta_off, op.deltas)  # copies: they stay alive with the view
+        views.append((_lib.PackView(256, op.nblocks, *[a.ctypes.data for a in arrs]),) + arrs)
+    refs = (_lib.PackRef * nrows)()
+    for i in range(nrows):
+        refs[i].pack, refs[i].key, refs[i].version = C.pointer(views[i][0]), 960_000 + i, 1
+    pack_bytes = sum(int(op.deltas.size) + 12 * int(op.nblocks) for op in ops)
+    lens = [int(op.num_uids.sum(dtype=np.uint64)) + t[0].size for op, t in zip(ops, muts)]
+
+    def p(a):
+        return a.ctypes.data_as(C.c_void_p)
+
+    def wall(fn, reps):
+        fn()
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            fn()
+        return (time.perf_counter() - t0) / reps * 1e3
+
+    handles = []
+    for pv in views:
+        h = C.c_void_p()
+        _lib.check(lib.dgx_dev_pack_upload(L.h, C.byref(pv[0]), C.byref(h)))
+        handles.append(h)
+    tab = (C.c_void_p * nrows)(*[h.value for h in handles])
+    d_mu = torch.from_numpy(mu_all.view(np.int64)).to(DEV)
+    d_mf = torch.from_numpy(mf_all).to(DEV)
+    cap_full = sum(lens)
+    d_out = torch.empty(cap_full + 8, dtype=torch.int64, device=DEV)
+    d_off = torch.zeros(nrows + 1, dtype=torch.int64, device=DEV)
+    d_cnt = torch.zeros(nrows, dtype=torch.int32, device=DEV)
+    hout = np.empty(max(cap_full, 1), np.uint64)
+    hoff = np.zeros(nrows + 1, np.uint64)
+    hcnt = np.zeros(nrows, np.uint32)
+    lib.dgx_cache_clear()
+    _lib.check(lib.dgx_cache_configure(16 << 30))
+    out_rows = []
+    try:
+        for after in (0, int(master[master.size // 2])):
+            for first in (0, 10, None):  # None: the count
+                if first is None:
+                    def oracle_row(i):
+                        return luo.list_count(ops[i], muts[i][0], muts[i][1], after)
+                else:
+                    def oracle_row(i):
+                        return luo.list_uids_unfiltered(ops[i], muts[i][0], muts[i][1], after, first)
+                t0 = time.perf_counter()
+                want = [oracle_row(i) for i in range(nrows)]
+                t_orc1 = time.perf_counter() - t0
+                t0 = time.perf_counter()
+                with ThreadPoolExecutor(max_workers=threads) as ex:   # ctypes releases the GIL
+                    got_n = list(ex.map(oracle_row, range(nrows)))
+                t_orcn = time.perf_counter() - t0
+                if first is None:
+                    want_cnt = np.array(want, np.uint32)
+                    nout = 0
+                    ok_n = bool(np.array_equal(np.array(got_n, np.uint32), want_cnt))
+
+                    def dev():
+                        _lib.check(lib.dgx_dev_list_count_rows(L.h, tab, nrows, C.c_void_p(d_mu.data_ptr()),
+                                                               C.c_void_p(d_mf.data_ptr()), p(mut_off), after,
+                                                               C.c_void_p(d_cnt.data_ptr())))
+
+                    def host():
+                        _lib.check(lib.dgx_list_count_rows(refs, nrows, p(mu_all), p(mf_all), p(mut_off), after,
+                                                           p(hcnt)))
+                    ms1, _ = timeit(dev, warm=3, reps=10)
+                    L.sync()
+                    ok1 = bool(np.array_equal(d_cnt.cpu().numpy().view(np.uint32), want_cnt))
+                    ms2 = wall(host, 5)
+                    ok2 = bool(np.array_equal(hcnt, want_cnt))
+                    what = "count"
+                else:
+                    want_off = np.concatenate([[0], np.cumsum([w.size for w in want])]).astype(np.uint64)
+                    want_all = np.concatenate(want) if want_off[-1] else np.zeros(0, np.uint64)
+                    nout = int(want_off[-1])
+                    ok_n = all(np.array_equal(a, b) for a, b in zip(got_n, want))
+                    cap = sum(min(gen_mut_unfiltered.most_kept(first), n) for n in lens)
+
+                    def same(out, off):
+                        return bool(np.array_equal(off, want_off) and np.array_equal(out[:nout], want_all))
+
+                    def dev():
+                        _lib.check(lib.dgx_dev_list_uids_unfiltered_rows(
+                            L.h, tab, nrows, C.c_void_p(d_mu.data_ptr()), C.c_void_p(d_mf.data_ptr()), p(mut_off),
+                            after, first, C.c_void_p(d_out.data_ptr()), cap, C.c_void_p(d_off.data_ptr())))
+
+                    def host():
+                        _lib.check(lib.dgx_list_uids_unfiltered_rows(refs, nrows, p(mu_all), p(mf_all), p(mut_off),
+                                                                     after, first, p(hout), p(hoff), cap))
+                    ms1, _ = timeit(dev, warm=3, reps=10)
+                    L.sync()
+                    ok1 = same(d_out[:nout].cpu().numpy().view(np.uint64), d_off.cpu().numpy().view(np.uint64))
+                    ms2 = wall(host, 5)
+                    ok2 = same(hout, hoff)
+                    what = "first = MaxInt32 (opts.First 0)" if first == 0 else f"first = {first}"
+                cfg = (f"C10 handleUidPostings without a filter: the C9 task ({nrows} UidPacks, BlockSize 256, {exact} "
+                       f"UIDs, {pack_bytes} pack bytes; {nmut} resolved entries on "
+                       f"{int((np.diff(mut_off) > 0).sum())} keys); {what}; afterUID={after}")
+                extra = {"rows": nrows, "out": nout, "after": after, "first": first, "mutable_entries": nmut,
+                         "pack_bytes": pack_bytes,
+                         "bytes_note": "algorithmic bytes: the pack bytes, 9 per mutable entry and 8 per result uid (4 "
+                                       "per count); a size of the work, not an HBM rate"}
+                algo_bytes = pack_bytes + 9 * nmut + (4 * nrows if first is None else 8 * nout)
+                fn = "count_rows" if first is None else "unfiltered_rows"
+                for name, ms, ok, note in (
+                    (f"List {fn} (device, resident packs)", ms1, ok1, f"dgx_dev_list_{fn}, CUDA events"),
+                    (f"List {fn} (host, named packs, cache hits)", ms2, ok2, f"dgx_list_{fn}, wall clock incl. D2H"),
+                    ("today: oracle per key (1 thread)", t_orc1 * 1e3, True, "restated in C, one key after another"),
+                    (f"today: oracle per key ({threads} threads)", t_orcn * 1e3, ok_n, "same, keys spread over threads"),
+                ):
+                    out_rows.append(row(name, cfg, ms, exact + nmut, algo_bytes, ok,
+                                        dict(extra, rows_per_s=nrows / (ms * 1e-3), note=note)))
     finally:
         for h in handles:
             lib.dgx_dev_pack_free(h)
