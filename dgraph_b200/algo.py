@@ -201,6 +201,16 @@ UIDS_COMPRESSED, UIDS_PROBE, UIDS_ITERATE = 0, 1, 2  # List.Uids branch of a row
 MUT_DEL, MUT_VALUE = 1, 2                             # flags of a resolved mutable entry (DGX_MUT_*)
 
 
+def _mut_csr(muts):
+    """The resolved mutable layers of a task's rows as one CSR: (uids, flags, off), never empty arrays."""
+    mu = [np.zeros(0, np.uint64) if t is None else _u64(t[0]) for t in muts]
+    mf = [np.zeros(0, np.uint8) if t is None else np.ascontiguousarray(np.asarray(t[1], np.uint8)) for t in muts]
+    off = np.zeros(len(muts) + 1, dtype=np.uint64)
+    np.cumsum([a.size for a in mu], out=off[1:])
+    n = int(off[-1])
+    return (np.concatenate(mu) if n else np.zeros(1, np.uint64)), (np.concatenate(mf) if n else np.zeros(1, np.uint8)), off
+
+
 def ListUidsRows(packs, modes, muts, afterUID: int, v, keys=None):
     """posting.List.Uids(opts) for every key of a task in ONE call (dgx_list_uids_rows), mutable layers included: the
     handleUidPostings loop (worker/task.go:783-987) of a filtered read of unsplit lists.
@@ -216,31 +226,16 @@ def ListUidsRows(packs, modes, muts, afterUID: int, v, keys=None):
     if nrows == 0:
         return np.zeros(0, np.uint64), np.zeros(1, np.uint64)
     mode = np.ascontiguousarray(np.asarray(modes, dtype=np.uint8))
-    mu = [np.zeros(0, np.uint64) if t is None else _u64(t[0]) for t in muts]
-    mf = [np.zeros(0, np.uint8) if t is None else np.ascontiguousarray(np.asarray(t[1], np.uint8)) for t in muts]
-    mut_off = np.zeros(nrows + 1, dtype=np.uint64)
-    np.cumsum([a.size for a in mu], out=mut_off[1:])
-    nmut = int(mut_off[-1])
-    mut_uids = np.concatenate(mu) if nmut else np.zeros(1, np.uint64)
-    mut_flags = np.concatenate(mf) if nmut else np.zeros(1, np.uint8)
+    mut_uids, mut_flags, mut_off = _mut_csr(muts)
     lib = _lib.load()
     refs, keep = _refs_of(packs, keys)
-    cap = sum(min(vv.size, (_exact(p) if p is not None else 0) + a.size) for p, a in zip(packs, mu))
+    cap = sum(min(vv.size, (_exact(p) if p is not None else 0) + int(mut_off[i + 1] - mut_off[i]))
+              for i, p in enumerate(packs))
     out = np.empty(max(cap, 1), dtype=np.uint64)
     out_off = np.zeros(nrows + 1, dtype=np.uint64)
     _lib.check(lib.dgx_list_uids_rows(refs, _p(mode), nrows, _p(mut_uids), _p(mut_flags), _p(mut_off), afterUID,
                                       _p(vv), vv.size, _p(out), _p(out_off), cap))
     return out[: int(out_off[-1])], out_off
-
-
-def _mut_csr(muts):
-    """The resolved mutable layers of a task's rows as one CSR: (uids, flags, off), never empty arrays."""
-    mu = [np.zeros(0, np.uint64) if t is None else _u64(t[0]) for t in muts]
-    mf = [np.zeros(0, np.uint8) if t is None else np.ascontiguousarray(np.asarray(t[1], np.uint8)) for t in muts]
-    off = np.zeros(len(muts) + 1, dtype=np.uint64)
-    np.cumsum([a.size for a in mu], out=off[1:])
-    n = int(off[-1])
-    return (np.concatenate(mu) if n else np.zeros(1, np.uint64)), (np.concatenate(mf) if n else np.zeros(1, np.uint8)), off
 
 
 def ListUidsUnfilteredRows(packs, muts, afterUID: int, first: int = 0, keys=None):

@@ -1278,7 +1278,15 @@ extern "C" void dgx_dev_pack_free(dgx_dev_pack* pk) {
     if (pk->d_mem) cudaFree(pk->d_mem);
     delete pk;
 }
-extern "C" size_t dgx_dev_pack_exact_len(const dgx_dev_pack* pk) { return pk ? pk->exact_len : 0; }
+// ExactLen of a pack, 0 when it is nil: read from a staged pack, or summed from the block counts of a ref's host view.
+static uint64_t exact_len(const dgx_dev_pack* pk) { return pk ? pk->exact_len : 0; }
+static uint64_t exact_len(const dgx_pack_ref& ref) {
+    const dgx_pack_view* p = ref.pack;
+    uint64_t n = 0;
+    for (size_t b = 0; p && b < p->nblocks; ++b) n += p->num_uids[b];
+    return n;
+}
+extern "C" size_t dgx_dev_pack_exact_len(const dgx_dev_pack* pk) { return exact_len(pk); }
 extern "C" size_t dgx_dev_pack_bytes(const dgx_dev_pack* pk) { return pk ? pk->bytes : 0; }
 
 static int decode_impl(dgx_lane* l, const DPack& pk, uint64_t seek, uint64_t* d_out, size_t out_cap,
@@ -1413,6 +1421,20 @@ static int batch_to_host(dgx_lane* l, const void* d_out, const void* d_off, size
     return DGX_OK;
 }
 
+// The CSR epilogue of a host-pointer batch call: room for `cap` values (and the two a kernel may pad with) and nrows + 1
+// offsets in the lane's workspace, filled by run(d_out, d_off), then copied back by batch_to_host.
+template <class Run>
+static int csr_to_host(dgx_lane* l, size_t cap, size_t nrows, uint64_t* out, uint64_t* out_off, size_t out_cap, Run run) {
+    void *d_out, *d_off;
+    int rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
+    if (rc) return rc;
+    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
+    if (rc) return rc;
+    rc = run((uint64_t*)d_out, (uint64_t*)d_off);
+    if (rc) return rc;
+    return batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap);
+}
+
 static int filter_host(int op, const uint64_t* const* lists, const size_t* lens, size_t k, uint64_t* out,
                        size_t out_cap, size_t* out_len) {
     LaneLease lease;
@@ -1514,14 +1536,9 @@ extern "C" int dgx_intersect_batch(const uint64_t* a, const uint64_t* a_off, con
         cap += std::min(la, lb);
     }
     k_off[npairs] = 2 * npairs;
-    void *d_out, *d_off;
-    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-    if (rc) return rc;
-    rc = l->ws.alloc((npairs + 1) * sizeof(uint64_t), &d_off);
-    if (rc) return rc;
-    rc = filter_batch_impl(l, DGX_OP_INTERSECT, ld.data(), k_off.data(), npairs, (uint64_t*)d_out, cap, (uint64_t*)d_off);
-    if (rc) return rc;
-    return batch_to_host(l, d_out, d_off, npairs, out, out_off, out_cap);
+    return csr_to_host(l, cap, npairs, out, out_off, out_cap, [&](uint64_t* d_out, uint64_t* d_off) {
+        return filter_batch_impl(l, DGX_OP_INTERSECT, ld.data(), k_off.data(), npairs, d_out, cap, d_off);
+    });
 }
 
 extern "C" int dgx_decode(const dgx_pack_view* p, uint64_t seek, uint64_t* out, size_t out_cap, size_t* out_len) {
@@ -1765,6 +1782,12 @@ struct PackSet {
         bool mapped = false;
         if (zero_copy) rc = packs_map_ws(l, oneshot.data(), k, pk.data(), &mapped);
         if (rc == DGX_OK && !mapped) rc = packs_upload_ws(l, oneshot.data(), k, pk.data());
+    }
+    // &pk[i] for every i: the row table of the *_rows impls
+    std::vector<const dgx_dev_pack*> rows() const {
+        std::vector<const dgx_dev_pack*> r(pk.size());
+        for (size_t i = 0; i < pk.size(); ++i) r[i] = &pk[i];
+        return r;
     }
     // rc of the call's final step, which ends in a host sync when it succeeds
     int synced(int call_rc) {
@@ -2269,14 +2292,9 @@ extern "C" int dgx_intersect_batch_shared(const uint64_t* a, const uint64_t* a_o
         cap += std::min(la, m);
     }
     k_off[npairs] = 2 * npairs;
-    void *d_out, *d_off;
-    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-    if (rc) return rc;
-    rc = l->ws.alloc((npairs + 1) * sizeof(uint64_t), &d_off);
-    if (rc) return rc;
-    rc = filter_batch_impl(l, DGX_OP_INTERSECT, ld.data(), k_off.data(), npairs, (uint64_t*)d_out, cap, (uint64_t*)d_off);
-    if (rc) return rc;
-    return batch_to_host(l, d_out, d_off, npairs, out, out_off, out_cap);
+    return csr_to_host(l, cap, npairs, out, out_off, out_cap, [&](uint64_t* d_out, uint64_t* d_off) {
+        return filter_batch_impl(l, DGX_OP_INTERSECT, ld.data(), k_off.data(), npairs, d_out, cap, d_off);
+    });
 }
 
 // ---------------------------------------------------------------------------
@@ -2407,35 +2425,29 @@ extern "C" int dgx_intersect_compressed_rows(const dgx_pack_ref* refs, size_t nr
     g_stats.calls += 1;
     PackSet ps(l, refs, nrows);  // nil / empty packs are packs of no blocks: empty rows
     if (ps.rc) return ps.rc;
-    std::vector<const dgx_dev_pack*> rows(nrows);
+    const std::vector<const dgx_dev_pack*> rows = ps.rows();
     size_t cap = 0;
-    for (size_t i = 0; i < nrows; ++i) {
-        rows[i] = &ps.pk[i];
-        cap += std::min<size_t>(m, ps.pk[i].exact_len);
-    }
+    for (const dgx_dev_pack& p : ps.pk) cap += std::min<size_t>(m, p.exact_len);
     uint64_t* d_v;
     int rc = upload_list(l, v, m, &d_v);
     if (rc) return rc;
-    void *d_out, *d_off;
-    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-    if (rc) return rc;
-    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
-    if (rc) return rc;
-    rc = icw_rows_impl(l, rows.data(), nrows, after_uid, d_v, m, (uint64_t*)d_out, cap, (uint64_t*)d_off);
-    if (rc) return rc;
-    return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
+    return ps.synced(csr_to_host(l, cap, nrows, out, out_off, out_cap, [&](uint64_t* d_out, uint64_t* d_off) {
+        return icw_rows_impl(l, rows.data(), nrows, after_uid, d_v, m, d_out, cap, d_off);
+    }));
 }
 
 // ---------------------------------------------------------------------------
 // IntersectCompressedWith of one pack against every row of a uid matrix (intersectBucket)
 // ---------------------------------------------------------------------------
-// v_off (host) must start at 0, never decrease and end below 2^32: checked before anything of v is read.
-static int check_v_off(const uint64_t* v_off, size_t nrows) {
-    if (v_off[0] != 0) return fail(DGX_ERR_ARG, "v_off[0] is %llu, not 0", (unsigned long long)v_off[0]);
+// The offsets off[0 .. nrows] (host memory) of the CSR array `name` must start at 0, never decrease and total less than
+// `limit`, the width the kernels count its elements in: checked before anything the offsets index is read.
+static int check_offsets(const char* name, const uint64_t* off, size_t nrows, uint64_t limit) {
+    if (off[0] != 0) return fail(DGX_ERR_ARG, "%s[0] is %llu, not 0", name, (unsigned long long)off[0]);
     for (size_t r = 0; r < nrows; ++r)
-        if (v_off[r + 1] < v_off[r]) return fail(DGX_ERR_ARG, "v_off decreases at row %zu", r);
-    if (v_off[nrows] >= (uint64_t(1) << 32))
-        return fail(DGX_ERR_ARG, "the matrix has %llu uids: unit ranges are 32-bit", (unsigned long long)v_off[nrows]);
+        if (off[r + 1] < off[r]) return fail(DGX_ERR_ARG, "%s decreases at row %zu", name, r);
+    if (off[nrows] >= limit)
+        return fail(DGX_ERR_ARG, "%s totals %llu: at most %llu", name, (unsigned long long)off[nrows],
+                    (unsigned long long)(limit - 1));
     return DGX_OK;
 }
 
@@ -2525,7 +2537,7 @@ extern "C" int dgx_dev_intersect_compressed_matrix(dgx_lane* l, const dgx_dev_pa
     if (!l || !d_out_off || (nrows && !v_off)) return fail(DGX_ERR_ARG, "null argument");
     static const uint64_t zero_off = 0;
     if (nrows == 0) v_off = &zero_off;
-    if (int rc = check_v_off(v_off, nrows)) return rc;
+    if (int rc = check_offsets("v_off", v_off, nrows, uint64_t(1) << 32)) return rc;
     if (v_off[nrows] && !d_v) return fail(DGX_ERR_ARG, "null d_v");
     if (int rc = lane_begin_op(l)) return rc;
     g_stats.calls += 1;
@@ -2541,7 +2553,7 @@ extern "C" int dgx_intersect_compressed_matrix(const dgx_pack_ref* ref, const ui
     if (!out_off) return fail(DGX_ERR_ARG, "null out_off");
     if (nrows == 0) { out_off[0] = 0; return DGX_OK; }
     if (!ref || !v_off) return fail(DGX_ERR_ARG, "null argument");
-    if (int rc = check_v_off(v_off, nrows)) return rc;
+    if (int rc = check_offsets("v_off", v_off, nrows, uint64_t(1) << 32)) return rc;
     const size_t m = v_off[nrows];
     if (m && !v) return fail(DGX_ERR_ARG, "null v");
     if (!ref->pack || ref->pack->nblocks == 0) {  // nil / empty pack: every row is empty, nothing runs
@@ -2559,41 +2571,57 @@ extern "C" int dgx_intersect_compressed_matrix(const dgx_pack_ref* ref, const ui
     uint64_t* d_v;
     int rc = upload_list(l, v, m, &d_v);
     if (rc) return rc;
-    void *d_out, *d_off;
-    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-    if (rc) return rc;
-    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
-    if (rc) return rc;
-    rc = icw_matrix_impl(l, ps.pk[0], d_v, v_off, nrows, (uint64_t*)d_out, cap, (uint64_t*)d_off);
-    if (rc) return rc;
-    return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
+    return ps.synced(csr_to_host(l, cap, nrows, out, out_off, out_cap, [&](uint64_t* d_out, uint64_t* d_off) {
+        return icw_matrix_impl(l, ps.pk[0], d_v, v_off, nrows, d_out, cap, d_off);
+    }));
 }
 
 // ---------------------------------------------------------------------------
 // List.Uids over a task's keys, mutable layers included (handleUidPostings)
 // ---------------------------------------------------------------------------
-// The host-side checks of both forms, before anything is copied: modes, offsets, m, and the bounds that keep the
-// MaxInt32 cut of List.Uids (posting/list.go:1840, 1864-1870) from biting.  exact(i) is ExactLen of row i's pack.
+// The resolved mutable layers of a task's rows, as every List.Uids entry point takes them: mut_off (host memory) with
+// fewer than 2^31 entries in all, so that no sum of class words carries (list_uids_kernel.cuh), and the uids and flags
+// present when there are entries.
+static int check_mut_layers(const uint64_t* mut_off, size_t nrows, const void* mut_uids, const void* mut_flags) {
+    if (int rc = check_offsets("mut_off", mut_off, nrows, uint64_t(1) << 31)) return rc;
+    if (mut_off[nrows] && (!mut_uids || !mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    return DGX_OK;
+}
+
+// The host forms stage the layers' nmut uids and flags in the lane's workspace, one copy each.
+static int upload_mut_layers(dgx_lane* l, const uint64_t* mut_uids, const uint8_t* mut_flags, size_t nmut,
+                             uint64_t** d_uids, const uint8_t** d_flags) {
+    int rc = upload_list(l, mut_uids, nmut, d_uids);
+    if (rc) return rc;
+    void* p;
+    rc = l->ws.alloc(nmut + 16, &p);
+    if (rc) return rc;
+    if (nmut) CK(cudaMemcpyAsync(p, mut_flags, nmut, cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += nmut;
+    *d_flags = (const uint8_t*)p;
+    return DGX_OK;
+}
+
+// The host-side checks of both forms, before anything is copied: m, the mutable layers, modes, and the bound that keeps
+// the MaxInt32 cut of List.Uids (posting/list.go:1840, 1864-1870) from biting.  rows[i] is row i's pack.
 static_assert(LU_COMPRESSED == DGX_UIDS_COMPRESSED && LU_PROBE == DGX_UIDS_PROBE && LU_ITERATE == DGX_UIDS_ITERATE &&
                   LU_DEL == DGX_MUT_DEL && LU_VALUE == DGX_MUT_VALUE,
               "list_uids_kernel.cuh reads the modes and flags of include/dgx.h");
-template <class ExactLen>
-static int list_uids_check(const uint8_t* mode, size_t nrows, const uint64_t* mut_off, size_t m, ExactLen exact) {
+template <class Row>
+static int list_uids_check(const uint8_t* mode, size_t nrows, const uint64_t* mut_off, const void* mut_uids,
+                           const void* mut_flags, size_t m, const Row* rows) {
     const uint64_t k31 = uint64_t(1) << 31;
     if (m == 0) return fail(DGX_ERR_ARG, "v is empty: an unfiltered read is not a List.Uids row call");
     if (m >= k31) return fail(DGX_ERR_ARG, "v has %zu uids: at most 2^31 - 1", m);
-    if (mut_off[0] != 0) return fail(DGX_ERR_ARG, "mut_off[0] is %llu, not 0", (unsigned long long)mut_off[0]);
+    if (int rc = check_mut_layers(mut_off, nrows, mut_uids, mut_flags)) return rc;
     for (size_t r = 0; r < nrows; ++r) {
         if (mode[r] > LU_ITERATE) return fail(DGX_ERR_ARG, "row %zu has mode %u", r, (unsigned)mode[r]);
-        if (mut_off[r + 1] < mut_off[r]) return fail(DGX_ERR_ARG, "mut_off decreases at row %zu", r);
         const uint64_t nm = mut_off[r + 1] - mut_off[r];
         if (mode[r] == LU_COMPRESSED && nm) return fail(DGX_ERR_ARG, "row %zu is compressed but has mutable entries", r);
-        if (mode[r] == LU_ITERATE && exact(r) + nm >= k31)
+        if (mode[r] == LU_ITERATE && exact_len(rows[r]) + nm >= k31)
             return fail(DGX_ERR_ARG, "iterate row %zu has %llu postings: at most 2^31 - 1", r,
-                        (unsigned long long)(exact(r) + nm));
+                        (unsigned long long)(exact_len(rows[r]) + nm));
     }
-    if (mut_off[nrows] >= k31)
-        return fail(DGX_ERR_ARG, "the mutable layers have %llu entries: at most 2^31 - 1", (unsigned long long)mut_off[nrows]);
     return DGX_OK;
 }
 
@@ -2605,8 +2633,7 @@ static int list_uids_impl(dgx_lane* l, const dgx_dev_pack* const* packs, const u
                           const uint64_t* d_v, size_t m, uint64_t* d_out, size_t out_cap, uint64_t* d_out_off) {
     const uint64_t nmut = mut_off[nrows];
     uint64_t a_cap = 0;
-    for (size_t i = 0; i < nrows; ++i)
-        if (packs[i]) a_cap += std::min<uint64_t>(m, packs[i]->exact_len);
+    for (size_t i = 0; i < nrows; ++i) a_cap += std::min<uint64_t>(m, exact_len(packs[i]));
     const uint64_t kMaxGrid = 0x7fffffffull;
     const uint64_t g_mut = std::max<uint64_t>((nmut + 255) / 256, 1), g_rows = (nrows + 255) / 256;
     const uint64_t g_write = (std::max<uint64_t>(a_cap + nmut, nrows + 1) + 255) / 256;
@@ -2697,11 +2724,7 @@ extern "C" int dgx_dev_list_uids_rows(dgx_lane* l, const dgx_dev_pack* const* pa
         return DGX_OK;
     }
     if (!packs || !mode || !mut_off || !d_v) return fail(DGX_ERR_ARG, "null argument");
-    if (int rc = list_uids_check(mode, nrows, mut_off, m, [&](size_t r) -> uint64_t {
-            return packs[r] ? packs[r]->exact_len : 0;
-        }))
-        return rc;
-    if (mut_off[nrows] && (!d_mut_uids || !d_mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    if (int rc = list_uids_check(mode, nrows, mut_off, d_mut_uids, d_mut_flags, m, packs)) return rc;
     if (int rc = lane_begin_op(l)) return rc;
     g_stats.calls += 1;
     const int rc = list_uids_impl(l, packs, mode, nrows, d_mut_uids, d_mut_flags, mut_off, after_uid, d_v, m, d_out,
@@ -2717,65 +2740,41 @@ extern "C" int dgx_list_uids_rows(const dgx_pack_ref* refs, const uint8_t* mode,
     if (!out_off) return fail(DGX_ERR_ARG, "null out_off");
     if (nrows == 0) { out_off[0] = 0; return DGX_OK; }
     if (!refs || !mode || !mut_off || !v) return fail(DGX_ERR_ARG, "null argument");
-    if (int rc = list_uids_check(mode, nrows, mut_off, m, [&](size_t r) -> uint64_t {
-            const dgx_pack_view* p = refs[r].pack;
-            uint64_t n = 0;
-            for (size_t b = 0; p && b < p->nblocks; ++b) n += p->num_uids[b];
-            return n;
-        }))
-        return rc;
-    const uint64_t nmut = mut_off[nrows];
-    if (nmut && (!mut_uids || !mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    if (int rc = list_uids_check(mode, nrows, mut_off, mut_uids, mut_flags, m, refs)) return rc;
     LaneLease lease;
     if (lease.rc) return lease.rc;
     dgx_lane* l = lease.l;
     g_stats.calls += 1;
     PackSet ps(l, refs, nrows);  // nil / empty packs are packs of no blocks
     if (ps.rc) return ps.rc;
-    std::vector<const dgx_dev_pack*> rows(nrows);
+    const std::vector<const dgx_dev_pack*> rows = ps.rows();
     size_t cap = 0;
-    for (size_t i = 0; i < nrows; ++i) {
-        rows[i] = &ps.pk[i];
-        cap += std::min<size_t>(m, ps.pk[i].exact_len + (mut_off[i + 1] - mut_off[i]));
-    }
+    for (size_t i = 0; i < nrows; ++i) cap += std::min<size_t>(m, ps.pk[i].exact_len + (mut_off[i + 1] - mut_off[i]));
     uint64_t *d_v, *d_mut;
+    const uint8_t* d_flags;
     int rc = upload_list(l, v, m, &d_v);
     if (rc) return rc;
-    rc = upload_list(l, mut_uids, nmut, &d_mut);
+    rc = upload_mut_layers(l, mut_uids, mut_flags, mut_off[nrows], &d_mut, &d_flags);
     if (rc) return rc;
-    void* d_flags;
-    rc = l->ws.alloc(nmut + 16, &d_flags);
-    if (rc) return rc;
-    if (nmut) CK(cudaMemcpyAsync(d_flags, mut_flags, nmut, cudaMemcpyHostToDevice, l->stream));
-    g_stats.h2d += nmut;
-    void *d_out, *d_off;
-    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-    if (rc) return rc;
-    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
-    if (rc) return rc;
-    rc = list_uids_impl(l, rows.data(), mode, nrows, d_mut, (const uint8_t*)d_flags, mut_off, after_uid, d_v, m,
-                        (uint64_t*)d_out, cap, (uint64_t*)d_off);
-    if (rc) return rc;
-    return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
+    return ps.synced(csr_to_host(l, cap, nrows, out, out_off, out_cap, [&](uint64_t* d_out, uint64_t* d_off) {
+        return list_uids_impl(l, rows.data(), mode, nrows, d_mut, d_flags, mut_off, after_uid, d_v, m, d_out, cap, d_off);
+    }));
 }
 
 // ---------------------------------------------------------------------------
 // List.Uids without a filter, and the count of the same postings, over a task's keys (handleUidPostings)
 // ---------------------------------------------------------------------------
-// The host-side checks of the four entry points, before anything is copied: offsets, and the bounds that keep |S_i|
-// and the class fields below 2^31.  exact(i) is ExactLen of row i's pack.
-template <class ExactLen>
-static int list_unfiltered_check(size_t nrows, const uint64_t* mut_off, ExactLen exact) {
-    const uint64_t k31 = uint64_t(1) << 31;
-    if (mut_off[0] != 0) return fail(DGX_ERR_ARG, "mut_off[0] is %llu, not 0", (unsigned long long)mut_off[0]);
+// The host-side checks of the four entry points, before anything is copied: the mutable layers, and the bound that
+// keeps |S_i| below 2^31.  rows[i] is row i's pack.
+template <class Row>
+static int list_unfiltered_check(size_t nrows, const uint64_t* mut_off, const void* mut_uids, const void* mut_flags,
+                                 const Row* rows) {
+    if (int rc = check_mut_layers(mut_off, nrows, mut_uids, mut_flags)) return rc;
     for (size_t r = 0; r < nrows; ++r) {
-        if (mut_off[r + 1] < mut_off[r]) return fail(DGX_ERR_ARG, "mut_off decreases at row %zu", r);
-        const uint64_t nm = mut_off[r + 1] - mut_off[r];
-        if (exact(r) + nm >= k31)
-            return fail(DGX_ERR_ARG, "row %zu has %llu postings: at most 2^31 - 1", r, (unsigned long long)(exact(r) + nm));
+        const uint64_t n = exact_len(rows[r]) + (mut_off[r + 1] - mut_off[r]);
+        if (n >= (uint64_t(1) << 31))
+            return fail(DGX_ERR_ARG, "row %zu has %llu postings: at most 2^31 - 1", r, (unsigned long long)n);
     }
-    if (mut_off[nrows] >= k31)
-        return fail(DGX_ERR_ARG, "the mutable layers have %llu entries: at most 2^31 - 1", (unsigned long long)mut_off[nrows]);
     return DGX_OK;
 }
 
@@ -2894,11 +2893,7 @@ extern "C" int dgx_dev_list_uids_unfiltered_rows(dgx_lane* l, const dgx_dev_pack
         return DGX_OK;
     }
     if (!packs || !mut_off) return fail(DGX_ERR_ARG, "null argument");
-    if (int rc = list_unfiltered_check(nrows, mut_off, [&](size_t r) -> uint64_t {
-            return packs[r] ? packs[r]->exact_len : 0;
-        }))
-        return rc;
-    if (mut_off[nrows] && (!d_mut_uids || !d_mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    if (int rc = list_unfiltered_check(nrows, mut_off, d_mut_uids, d_mut_flags, packs)) return rc;
     if (int rc = lane_begin_op(l)) return rc;
     g_stats.calls += 1;
     const int rc = list_unfiltered_impl(l, packs, nrows, d_mut_uids, d_mut_flags, mut_off, after_uid, first_keep(first),
@@ -2914,11 +2909,7 @@ extern "C" int dgx_dev_list_count_rows(dgx_lane* l, const dgx_dev_pack* const* p
     if (!l) return fail(DGX_ERR_ARG, "null lane");
     if (nrows == 0) return DGX_OK;
     if (!packs || !mut_off || !d_counts) return fail(DGX_ERR_ARG, "null argument");
-    if (int rc = list_unfiltered_check(nrows, mut_off, [&](size_t r) -> uint64_t {
-            return packs[r] ? packs[r]->exact_len : 0;
-        }))
-        return rc;
-    if (mut_off[nrows] && (!d_mut_uids || !d_mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    if (int rc = list_unfiltered_check(nrows, mut_off, d_mut_uids, d_mut_flags, packs)) return rc;
     if (int rc = lane_begin_op(l)) return rc;
     g_stats.calls += 1;
     const int rc = list_unfiltered_impl(l, packs, nrows, d_mut_uids, d_mut_flags, mut_off, after_uid, first_keep(0),
@@ -2933,15 +2924,7 @@ static int list_unfiltered_host(const dgx_pack_ref* refs, size_t nrows, const ui
                                 const uint8_t* mut_flags, const uint64_t* mut_off, uint64_t after_uid, int32_t first,
                                 uint64_t* out, uint64_t* out_off, size_t out_cap, uint32_t* counts) {
     if (!refs || !mut_off) return fail(DGX_ERR_ARG, "null argument");
-    if (int rc = list_unfiltered_check(nrows, mut_off, [&](size_t r) -> uint64_t {
-            const dgx_pack_view* p = refs[r].pack;
-            uint64_t n = 0;
-            for (size_t b = 0; p && b < p->nblocks; ++b) n += p->num_uids[b];
-            return n;
-        }))
-        return rc;
-    const uint64_t nmut = mut_off[nrows];
-    if (nmut && (!mut_uids || !mut_flags)) return fail(DGX_ERR_ARG, "null mutable layer");
+    if (int rc = list_unfiltered_check(nrows, mut_off, mut_uids, mut_flags, refs)) return rc;
     LaneLease lease;
     if (lease.rc) return lease.rc;
     dgx_lane* l = lease.l;
@@ -2949,40 +2932,28 @@ static int list_unfiltered_host(const dgx_pack_ref* refs, size_t nrows, const ui
     PackSet ps(l, refs, nrows);  // nil / empty packs are packs of no blocks
     if (ps.rc) return ps.rc;
     const uint64_t keep = first_keep(first);
-    std::vector<const dgx_dev_pack*> rows(nrows);
+    const std::vector<const dgx_dev_pack*> rows = ps.rows();
     size_t cap = 0;
-    for (size_t i = 0; i < nrows; ++i) {
-        rows[i] = &ps.pk[i];
-        cap += std::min<uint64_t>(keep, ps.pk[i].exact_len + (mut_off[i + 1] - mut_off[i]));
-    }
+    for (size_t i = 0; i < nrows; ++i) cap += std::min<uint64_t>(keep, ps.pk[i].exact_len + (mut_off[i + 1] - mut_off[i]));
     uint64_t* d_mut;
-    int rc = upload_list(l, mut_uids, nmut, &d_mut);
+    const uint8_t* d_flags;
+    int rc = upload_mut_layers(l, mut_uids, mut_flags, mut_off[nrows], &d_mut, &d_flags);
     if (rc) return rc;
-    void* d_flags;
-    rc = l->ws.alloc(nmut + 16, &d_flags);
-    if (rc) return rc;
-    if (nmut) CK(cudaMemcpyAsync(d_flags, mut_flags, nmut, cudaMemcpyHostToDevice, l->stream));
-    g_stats.h2d += nmut;
     if (counts) {
         void* d_counts;
         rc = l->ws.alloc(nrows * sizeof(uint32_t), &d_counts);
         if (rc) return rc;
-        rc = list_unfiltered_impl(l, rows.data(), nrows, d_mut, (const uint8_t*)d_flags, mut_off, after_uid, keep,
-                                  nullptr, 0, nullptr, (uint32_t*)d_counts);
+        rc = list_unfiltered_impl(l, rows.data(), nrows, d_mut, d_flags, mut_off, after_uid, keep, nullptr, 0, nullptr,
+                                  (uint32_t*)d_counts);
         if (rc) return rc;
         CK(cudaMemcpyAsync(counts, d_counts, nrows * sizeof(uint32_t), cudaMemcpyDeviceToHost, l->stream));
         g_stats.d2h += nrows * sizeof(uint32_t);
         return ps.synced(dgx_lane_sync(l));
     }
-    void *d_out, *d_off;
-    rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-    if (rc) return rc;
-    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
-    if (rc) return rc;
-    rc = list_unfiltered_impl(l, rows.data(), nrows, d_mut, (const uint8_t*)d_flags, mut_off, after_uid, keep,
-                              (uint64_t*)d_out, cap, (uint64_t*)d_off, nullptr);
-    if (rc) return rc;
-    return ps.synced(batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap));
+    return ps.synced(csr_to_host(l, cap, nrows, out, out_off, out_cap, [&](uint64_t* d_out, uint64_t* d_off) {
+        return list_unfiltered_impl(l, rows.data(), nrows, d_mut, d_flags, mut_off, after_uid, keep, d_out, cap, d_off,
+                                    nullptr);
+    }));
 }
 
 extern "C" int dgx_list_uids_unfiltered_rows(const dgx_pack_ref* refs, size_t nrows, const uint64_t* mut_uids,
@@ -3103,11 +3074,8 @@ extern "C" int dgx_merge_sorted_matrix(const uint64_t* v, const uint64_t* v_off,
                                        size_t out_cap, size_t* out_len) {
     if (nrows == 0) { if (out_len) *out_len = 0; return DGX_OK; }
     if (!v_off) return fail(DGX_ERR_ARG, "null v_off");
-    if (v_off[0] != 0) return fail(DGX_ERR_ARG, "v_off[0] is %llu, not 0", (unsigned long long)v_off[0]);
-    for (size_t r = 0; r < nrows; ++r)
-        if (v_off[r + 1] < v_off[r]) return fail(DGX_ERR_ARG, "v_off decreases at row %zu", r);
+    if (int rc = check_offsets("v_off", v_off, nrows, kMergeMatrixMax + 1)) return rc;
     const uint64_t m = v_off[nrows];
-    if (m > kMergeMatrixMax) return fail(DGX_ERR_ARG, "the matrix has %llu uids: positions are 32-bit", (unsigned long long)m);
     if (m == 0) { if (out_len) *out_len = 0; return DGX_OK; }  // every row empty: nothing runs
     if (!v || (out_cap && !out)) return fail(DGX_ERR_ARG, "null argument");
     LaneLease lease;

@@ -27,9 +27,18 @@
 namespace dgx {
 
 constexpr int kLaneErrMut = 4;  // lane error flag bit: a mutable entry (or a mode-1/2 pack) is malformed (DGX_ERR_ARG)
-constexpr u64 kLuMask = (1ull << 31) - 1;  // an entry's class word: drop in bits 0..30, insert in bits 31..61
 constexpr unsigned LU_COMPRESSED = 0, LU_PROBE = 1, LU_ITERATE = 2;  // a row's mode (DGX_UIDS_*)
 constexpr unsigned LU_DEL = 1, LU_VALUE = 2;                          // an entry's flags (DGX_MUT_*)
+
+// An entry's class word: drops in bits 0..30, inserts in bits 31..61.  scan_u64_kernel sums the words; the host keeps
+// a call's entries below 2^31, so no sum carries from one field into the other.
+constexpr u64 kLuDrop = 1, kLuInsert = 1ull << 31;
+constexpr u64 kLuMask = kLuInsert - 1;
+
+// n with the drops of the summed class word d taken out and its inserts added.
+__device__ __forceinline__ u64 lu_apply(u64 n, u64 d) { return n - (d & kLuMask) + (d >> 31); }
+__device__ __forceinline__ bool lu_drops(u64 c) { return c & kLuMask; }
+__device__ __forceinline__ bool lu_inserts(u64 c) { return c >> 31; }
 
 struct LuParams {
     const unsigned char* mode;  // nrows
@@ -81,16 +90,23 @@ __device__ __forceinline__ bool lu_passes(unsigned mode, u64 x, u64 after) {
     return mode == LU_PROBE || (mode == LU_ITERATE ? x > after : x >= after);
 }
 
+// Entry k of row r (uid x, flags f) of LuParams or LuuParams P: uid 0, an unknown flag, or a uid not above the row's
+// previous entry marks the call malformed.
+template <class Params>
+__device__ __forceinline__ void lu_check_entry(const Params& P, u64 r, u64 k, u64 x, unsigned f) {
+    if (x == 0 || (f & ~(LU_DEL | LU_VALUE)) || (k > ld_probe(P.mut_off + r) && P.mut[k - 1] >= x)) {
+        *P.bad = 1;
+        atomicOr(P.err, kLaneErrMut);
+    }
+}
+
 __global__ void __launch_bounds__(256) lu_classify_kernel(const LuParams P) {
     const u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= P.nmut) return;
     const u64 r = lu_row_of(P.mut_off, P.nrows, k);
     const u64 x = P.mut[k];
     const unsigned f = P.flags[k];
-    if (x == 0 || (f & ~(LU_DEL | LU_VALUE)) || (k > ld_probe(P.mut_off + r) && P.mut[k - 1] >= x)) {
-        *P.bad = 1;
-        atomicOr(P.err, kLaneErrMut);
-    }
+    lu_check_entry(P, r, k, x, f);
     const unsigned mode = P.mode[r];
     u64 c = 0;
     if (lu_passes(mode, x, P.after)) {
@@ -99,10 +115,10 @@ __global__ void __launch_bounds__(256) lu_classify_kernel(const LuParams P) {
         const u64 s = ld_probe(P.a_off + r), e = ld_probe(P.a_off + r + 1);
         const u64 p = s + lower_bound_g(P.a + s, e - s, x);
         const bool in_a = p < e && ld_probe(P.a + p) == x;
-        if (in_a && !emits) c = 1;  // drop
+        if (in_a && !emits) c = kLuDrop;
         if (!in_a && emits) {
             const u64 j = lower_bound_g(P.v, P.m, x);
-            if (j < P.m && ld_probe(P.v + j) == x) c = 1ull << 31;  // insert
+            if (j < P.m && ld_probe(P.v + j) == x) c = kLuInsert;
         }
     }
     P.cls[k] = c;
@@ -116,9 +132,9 @@ __global__ void __launch_bounds__(256) lu_rows_kernel(const LuParams P) {
     u64 lo = s;
     if (mode == LU_COMPRESSED) lo = s + lower_bound_g(P.a + s, e - s, P.after);
     else if (mode == LU_ITERATE) lo = s + upper_bound_g(P.a + s, e - s, P.after);
-    const u64 d = P.cls_ex[P.mut_off[r + 1]] - P.cls_ex[P.mut_off[r]];  // field sums stay below 2^31: no carry
+    const u64 d = P.cls_ex[P.mut_off[r + 1]] - P.cls_ex[P.mut_off[r]];
     P.lo[r] = lo;
-    P.cnt[r] = (e - lo) - (d & kLuMask) + (d >> 31);
+    P.cnt[r] = lu_apply(e - lo, d);
     const u64* first = P.first[r];
     if (first && *first == 0) {  // iterate reads uid 0 as the end of the list (:1178-1196)
         *P.bad = 1;
@@ -148,19 +164,19 @@ __global__ void __launch_bounds__(256) lu_write_kernel(const LuParams P) {
         x = P.a[t];
         const u64 ms = ld_probe(P.mut_off + r), me = ld_probe(P.mut_off + r + 1);
         const u64 j = ms + lower_bound_g(P.mut + ms, me - ms, x);
-        if (j < me && ld_probe(P.mut + j) == x && (P.cls[j] & kLuMask)) return;  // dropped
+        if (j < me && ld_probe(P.mut + j) == x && lu_drops(P.cls[j])) return;
         rank = t - lo;
         below = P.cls_ex[j] - P.cls_ex[ms];
     } else {
         const u64 k = t - P.a_cap;
-        if (k >= P.nmut || !(P.cls[k] >> 31)) return;
+        if (k >= P.nmut || !lu_inserts(P.cls[k])) return;
         r = lu_row_of(P.mut_off, P.nrows, k);
         x = P.mut[k];
         const u64 lo = P.lo[r], e = P.a_off[r + 1];
         rank = lower_bound_g(P.a + lo, e - lo, x);
         below = P.cls_ex[k] - P.cls_ex[ld_probe(P.mut_off + r)];
     }
-    P.out[P.out_off[r] + rank - (below & kLuMask) + (below >> 31)] = x;
+    P.out[lu_apply(P.out_off[r] + rank, below)] = x;
 }
 
 }  // namespace dgx

@@ -107,10 +107,7 @@ __global__ void __launch_bounds__(256) luu_classify_kernel(const LuuParams P) {
     const u64 r = lu_row_of(P.mut_off, P.nrows, k);
     const u64 x = P.mut[k];
     const unsigned f = P.flags[k];
-    if (x == 0 || (f & ~(LU_DEL | LU_VALUE)) || (k > ld_probe(P.mut_off + r) && P.mut[k - 1] >= x)) {
-        *P.bad = 1;
-        atomicOr(P.err, kLaneErrMut);
-    }
+    lu_check_entry(P, r, k, x, f);
     u64 c = 0, rank = 0;
     if (x > P.after) {  // iterate starts the mutable side at the first entry above after (:1126-1131)
         bool in_pack = false;
@@ -121,8 +118,8 @@ __global__ void __launch_bounds__(256) luu_classify_kernel(const LuuParams P) {
             rank = s.le - (s.hit ? 1 : 0);
         }
         const bool emits = f == 0;  // a SET of a REF posting
-        if (in_pack && !emits) c = 1;                // drop
-        if (!in_pack && emits) c = 1ull << 31;       // insert
+        if (in_pack && !emits) c = kLuDrop;
+        if (!in_pack && emits) c = kLuInsert;
     }
     P.cls[k] = c;
     P.rank[k] = rank;
@@ -147,8 +144,8 @@ __global__ void __launch_bounds__(256) luu_rows_kernel(const LuuParams P) {
         if (s.b >= 0) sb = s.le - pk.uid_off[s.b] < pk.num[s.b] ? (u64)s.b : (u64)s.b + 1;
         above = pk.uid_off[pk.nblocks] - skip;
     }
-    const u64 d = P.cls_ex[P.mut_off[r + 1]] - P.cls_ex[P.mut_off[r]];  // field sums stay below 2^31: no carry
-    const u64 n = above - (d & kLuMask) + (d >> 31);
+    const u64 d = P.cls_ex[P.mut_off[r + 1]] - P.cls_ex[P.mut_off[r]];
+    const u64 n = lu_apply(above, d);
     P.skip[r] = skip;
     P.sblk[r] = sb;
     P.len[r] = n < P.first ? n : P.first;
@@ -159,9 +156,9 @@ __global__ void __launch_bounds__(256) luu_rows_kernel(const LuuParams P) {
 // mut[js, je), and ms is the row's first entry.  kU64Max when an entry drops y.
 __device__ __forceinline__ u64 luu_pos_of(const LuuParams& P, u64 y, u64 q, u64 skip, u64 ms, u64 js, u64 je) {
     const u64 j = js + lower_bound_g(P.mut + js, je - js, y);
-    if (j < je && ld_probe(P.mut + j) == y && (P.cls[j] & kLuMask)) return kU64Max;
+    if (j < je && ld_probe(P.mut + j) == y && lu_drops(P.cls[j])) return kU64Max;
     const u64 below = P.cls_ex[j] - P.cls_ex[ms];
-    return (q - skip) - (below & kLuMask) + (below >> 31);
+    return lu_apply(q - skip, below);
 }
 
 // One warp writes the kept uids of blocks [b, b + D_BPW) of row r's pack.  Per batch of 32 blocks: every lane finds
@@ -189,7 +186,7 @@ __device__ __forceinline__ void luu_write_blocks(const LuuParams& P, const DPack
             je = bi + 1 < pk.nblocks ? ms + lower_bound_g(P.mut + ms, me - ms, pk.base[bi + 1]) : me;
             if (bi > sb) {  // values of S below base: pack uids in (after, base) - drops + inserts below base
                 const u64 d = P.cls_ex[js] - P.cls_ex[ms];
-                lower = (uoff - skip) - (d & kLuMask) + (d >> 31);
+                lower = lu_apply(uoff - skip, d);
             }
         }
         // lower ascends with the block: the live blocks are lanes [0, last]
@@ -263,10 +260,10 @@ __global__ void __launch_bounds__(D_NT, 4) luu_write_kernel(const LuuParams P) {
         return;
     }
     const u64 k = (u64)(blockIdx.x - g_blk) * blockDim.x + threadIdx.x;
-    if (k >= P.nmut || !(P.cls[k] >> 31)) return;
+    if (k >= P.nmut || !lu_inserts(P.cls[k])) return;
     const u64 r = lu_row_of(P.mut_off, P.nrows, k);
     const u64 below = P.cls_ex[k] - P.cls_ex[ld_probe(P.mut_off + r)];
-    const u64 pos = (P.rank[k] - P.skip[r]) - (below & kLuMask) + (below >> 31);
+    const u64 pos = lu_apply(P.rank[k] - P.skip[r], below);
     if (pos < P.len[r]) P.out[P.out_off[r] + pos] = P.mut[k];
 }
 

@@ -64,6 +64,8 @@ def test_host_checks_fire_without_a_device():
         "compressed row with entries": dict(ok, mode=[0, 2]),
         "mut_off[0] != 0": dict(ok, mut_off=[1, 1, 2]),
         "decreasing offsets": dict(ok, mut_off=[0, 2, 1]),
+        # each row passes its own bounds; the total alone is refused, before any entry is read
+        "2^31 entries in all": dict(ok, mut_off=[0, 2**30, 2**31]),
         "empty v": dict(ok, v=[]),
     }
     for what, kw in cases.items():

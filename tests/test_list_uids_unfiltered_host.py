@@ -66,6 +66,8 @@ def test_host_checks_fire_without_a_device(count):
     cases = {
         "mut_off[0] != 0": dict(ok, mut_off=[1, 1, 2]),
         "decreasing offsets": dict(ok, mut_off=[0, 2, 1]),
+        # each row passes its own bound; the total alone is refused, before any entry is read
+        "2^31 entries in all": dict(ok, mut_off=[0, 2**30, 2**31]),
     }
     for what, kw in cases.items():
         assert _call(count, **kw) == ERR_ARG, what
