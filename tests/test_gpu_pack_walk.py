@@ -4,7 +4,6 @@ The Encoder starts a new block whenever the upper 32 bits change, so its packs n
 inside a block; the reference still sums `last + uint64(delta)` (codec.go:191-196), and a hand-built pack can rely on
 it.  One block of 9 uids is expanded in shared memory by the warp; one of 300 uids (more than 256) is walked by one
 thread from global memory.  Runs on an H100 only (`pytest -m gpu`)."""
-import ctypes as C
 import os
 import sys
 
@@ -12,9 +11,8 @@ import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.dirname(__file__))
+from pack_geometry import ArrayPack  # noqa: E402
 from test_gpu_parity import L, eq  # noqa: E402
-
-from oracle import pyoracle  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -30,21 +28,6 @@ def dgx():
     lib = _lib.load()
     _lib.check(lib.dgx_init(-1))
     return dgraph_b200
-
-
-class ArrayPack(pyoracle.Pack):
-    """An oracle pack over arrays held here: the oracle's encoder cannot make one whose deltas pass 2^32."""
-
-    def __init__(self, block_size, base, num, delta_off, deltas):
-        self.arrays = (base, num, delta_off, deltas)
-        self.s = pyoracle._Pack(block_size, base.size, base.ctypes.data_as(C.POINTER(C.c_uint64)),
-                                num.ctypes.data_as(C.POINTER(C.c_uint32)),
-                                delta_off.ctypes.data_as(C.POINTER(C.c_uint64)),
-                                deltas.ctypes.data_as(C.POINTER(C.c_uint8)))
-        super().__init__(C.pointer(self.s))
-
-    def __del__(self):
-        pass  # the arrays are numpy's
 
 
 def one_block(dgx, n):
