@@ -142,9 +142,10 @@ def _pack_out_arrays(n_uids: int, block_size: int):
 
 
 def _call_pack_out(fn, n_uids: int, block_size: int) -> Optional[UidPack]:
-    """Run `fn(base, num, doff, deltas, &nblocks, &delta_bytes, &view)`, growing the arrays once on DGX_ERR_CAP."""
+    """Run `fn(base, num, doff, deltas, &nblocks, &delta_bytes, &view)`, growing the arrays once on DGX_ERR_CAP (the
+    sizes it returns suffice, so a second DGX_ERR_CAP is an error)."""
     nb_cap, db_cap = _pack_out_arrays(n_uids, block_size)
-    for _ in range(3):
+    for _ in range(2):
         base = np.empty(max(nb_cap, 1), np.uint64)
         num = np.empty(max(nb_cap, 1), np.uint32)
         doff = np.zeros(max(nb_cap, 1) + 1, np.uint64)

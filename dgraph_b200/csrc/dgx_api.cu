@@ -2024,8 +2024,8 @@ extern "C" int dgx_pack_image_view(void* image, uint32_t block_size, size_t nblo
 
 extern "C" void dgx_encode_bound(size_t n, uint32_t block_size, size_t* nblocks_cap, size_t* delta_cap) {
     const size_t B = block_size ? block_size : 1;
-    // a sorted list crosses a multiple of 2^32 rarely: room for 64 extra (short) blocks; dgx_encode reports the
-    // exact need with DGX_ERR_CAP when a list has more upper-word changes than that
+    // a sorted list crosses a multiple of 2^32 rarely: room for 64 extra (short) blocks; dgx_encode reports sizes
+    // that suffice with DGX_ERR_CAP when a list has more upper-word changes than that, so one retry succeeds
     const size_t nb = n ? (n + B - 1) / B + 64 : 0;
     if (nblocks_cap) *nblocks_cap = nb;
     if (delta_cap) *delta_cap = 17 * (n / 4 + nb + 1);  // every group is at most 17 bytes

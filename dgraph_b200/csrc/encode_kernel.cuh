@@ -15,6 +15,8 @@
 //   scan_u64_kernel       exclusive scan of the byte lengths -> delta_off (single-pass look-back)
 //   enc_write_kernel      warp per block: lane g encodes group g at its offset inside the block
 // Bound: HBM (8 B/uid in, ~1.3-2.6 B/uid out).
+// Limit: a list of 2^32 uids or more, or a block of 2^32 - 2 uids or more, wraps the u32 num, ngroups and per-round
+// totals; that is 32 GB of uids in one call, far past any posting list, and is not supported.
 #pragma once
 
 #include "common.cuh"
@@ -95,8 +97,15 @@ __global__ void __launch_bounds__(1024) enc_segscan_kernel(const EncParams P) {
     __shared__ u32 s_warp[1024 / 32 + 1];
     __shared__ u64 s_carry;
     const u64 nseg = P.counts[0];
-    if (nseg + 1 > P.seg_cap) {  // more segments than the arrays hold: at least that many blocks are needed
-        if (threadIdx.x == 0) { P.counts[1] = nseg > P.nblocks_cap ? nseg : P.nblocks_cap + 1; atomicExch(P.err, 2); }
+    if (nseg + 1 > P.seg_cap) {  // more segments than the arrays hold: report a block count that suffices
+        if (threadIdx.x == 0) {
+            // a segment of len uids takes ceil(len / bsz) <= floor(len / bsz) + 1 blocks, and every block holds a uid:
+            // with this capacity the next call's segment array holds nseg + 1 entries and the exact count fits.  It
+            // exceeds nblocks_cap, as nseg does (min(n, nblocks_cap) + 2 < nseg + 1 <= n + 1)
+            const u64 n = enc_n(P), nb = n / P.bsz + nseg;
+            P.counts[1] = nb < n ? nb : n;
+            atomicExch(P.err, 2);
+        }
         return;
     }
     if (threadIdx.x == 0) s_carry = 0;

@@ -170,7 +170,8 @@ int dgx_intersect_sorted_packed(const dgx_pack_ref* refs, size_t k,
  * upper 32 bits or after BlockSize uids, group-varint deltas.  The caller allocates base[*nblocks],
  * num_uids[*nblocks], delta_off[*nblocks + 1], deltas[*delta_bytes] (dgx_encode_bound gives sizes that hold any
  * list with at most 64 upper-word changes); on return *nblocks / *delta_bytes are the pack's sizes and `view`
- * points at the arrays.  DGX_ERR_CAP: the arrays are too small, the sizes needed were returned, call again.
+ * points at the arrays.  DGX_ERR_CAP: the arrays are too small, sizes that suffice were returned (the exact ones
+ * when the list's segments fit the arrays given), and one call again with them succeeds.
  * n == 0 is the nil pack (nblocks 0). */
 void dgx_encode_bound(size_t n, uint32_t block_size, size_t* nblocks_cap, size_t* delta_cap);
 int dgx_encode(const uint64_t* uids, size_t n, uint32_t block_size,

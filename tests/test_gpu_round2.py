@@ -530,7 +530,8 @@ def test_encode_matches_oracle_bytes(dgx, orc):
         g = rng.integers(1, 1 << shift, 4000, dtype=np.uint64) + np.uint64(1 << shift)
         u = np.cumsum(g, dtype=np.uint64)
         same_pack(dgx.codec.Encode(u, 256), orc.encode(u, 256), f"shift {shift}")
-    wide = np.cumsum(rng.integers(1, 1 << 31, 200_000, dtype=np.uint64), dtype=np.uint64)   # ~45 upper-word changes
+    # ~50,000 upper-word changes: with BlockSize 10 the segments overflow the bound's arrays (one retry)
+    wide = np.cumsum(rng.integers(1, 1 << 31, 200_000, dtype=np.uint64), dtype=np.uint64)
     same_pack(dgx.codec.Encode(wide, 256), orc.encode(wide, 256), "msb splits")
     same_pack(dgx.codec.Encode(wide, 10), orc.encode(wide, 10), "msb splits bs 10")
     scattered = np.sort(rng.integers(0, 2**64 - 1, 5000, dtype=np.uint64))                  # a new block per uid: > 64 splits
