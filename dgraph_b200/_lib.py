@@ -75,6 +75,8 @@ SYMBOLS = {
     "dgx_list_uids_rows": (_int, [C.POINTER(PackRef), _vp, _sz, _vp, _vp, _vp, _u64, _vp, _sz, _vp, _vp, _sz]),
     "dgx_list_uids_unfiltered_rows": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _vp, _u64, C.c_int32, _vp, _vp, _sz]),
     "dgx_list_count_rows": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _vp, _u64, _vp]),
+    "dgx_decode_to_buffer_rows": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _sz]),
+    "dgx_encode_from_buffer_rows": (_int, [_vp, _vp, _sz, C.c_uint32, _vp, _sz, _vp, _vp, _vp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
     "dgx_encode_bound": (None, [_sz, C.c_uint32, _szp, _szp]),
     "dgx_encode": (_int, [_vp, _sz, C.c_uint32, _vp, _vp, _vp, _vp, _szp, _szp, C.POINTER(PackView)]),
@@ -108,6 +110,8 @@ SYMBOLS = {
     "dgx_dev_decode": (_int, [_vp, _vp, _u64, _vp, _sz, _vp]),
     "dgx_dev_intersect_compressed_rows": (_int, [_vp, _vp, _sz, _u64, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_intersect_compressed_matrix": (_int, [_vp, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "dgx_dev_decode_to_buffer_rows": (_int, [_vp, _vp, _sz, _vp, _sz, _vp]),
+    "dgx_dev_encode_from_buffer_rows": (_int, [_vp, _vp, _vp, _sz, C.c_uint32, _vp, _sz, _vp, _vp, _vp]),
     "dgx_dev_merge_sorted_matrix": (_int, [_vp, _vp, _vp, _sz, _sz, _vp, _sz, _vp]),
     "dgx_dev_list_uids_rows": (_int, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _u64, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_list_uids_unfiltered_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, C.c_int32, _vp, _sz, _vp]),

@@ -173,3 +173,81 @@ def Encode(uids, blockSize: int) -> Optional[UidPack]:
         return None
     return _call_pack_out(lambda b, n, d, dl, pnb, pdb, pv: lib.dgx_encode(
         u.ctypes.data_as(C.c_void_p), u.size, blockSize, b, n, d, dl, pnb, pdb, pv), u.size, blockSize)
+
+
+def _aligned_bytes(n: int) -> np.ndarray:
+    """A zeroed uint8 array of n bytes at a 16-byte aligned address (the flat pack image layout needs it)."""
+    raw = np.zeros(n + 16, dtype=np.uint8)
+    skip = (-raw.ctypes.data) % 16
+    return raw[skip: skip + n]
+
+
+def DecodeToBufferRows(packs: Sequence[Optional[UidPack]], keys=None):
+    """codec.DecodeToBuffer (codec/codec.go:456-467) for every pack in ONE call (dgx_decode_to_buffer_rows): the
+    BackupPostingList.uid_bytes of a batch of keys.  keys: optional [(key, version)] naming each pack for the
+    HBM-resident cache.  Returns (out, out_off): row i's bytes are out[out_off[i]:out_off[i+1]]."""
+    from .algo import _refs_of
+
+    nrows = len(packs)
+    out_off = np.zeros(nrows + 1, dtype=np.uint64)
+    if nrows == 0:
+        return np.zeros(0, np.uint8), out_off
+    lib = _lib.load()
+    refs, keep = _refs_of(packs, keys)
+    cap = 10 * sum(ExactLen(p) for p in packs)  # a uvarint takes at most 10 bytes: one call always fits
+    out = np.empty(max(cap, 1), dtype=np.uint8)
+    _lib.check(lib.dgx_decode_to_buffer_rows(refs, nrows, out.ctypes.data_as(C.c_void_p),
+                                             out_off.ctypes.data_as(C.c_void_p), cap))
+    return out[: int(out_off[-1])], out_off
+
+
+def DecodeToBuffer(pack: Optional[UidPack]) -> bytes:
+    """codec.DecodeToBuffer(pack): the uvarint deltas of Decode(pack, 0); a nil or empty pack gives no bytes."""
+    out, _ = DecodeToBufferRows([pack])
+    return out.tobytes()
+
+
+def EncodeFromBufferRows(bufs, blockSize: int):
+    """codec.EncodeFromBuffer (codec/codec.go:402-414) for every buffer in ONE call (dgx_encode_from_buffer_rows): the
+    packs FromBackupPostingList rebuilds from a batch of keys' uid_bytes.  Returns one UidPack per buffer, None for an
+    empty one (the nil pack).  A buffer that is not a sequence of valid uvarints raises DgxError (DGX_ERR_ARG)."""
+    nrows = len(bufs)
+    if nrows == 0:
+        return []
+    arrs = [np.frombuffer(bytes(b), dtype=np.uint8) for b in bufs]
+    buf_off = np.zeros(nrows + 1, dtype=np.uint64)
+    buf_off[1:] = np.cumsum([a.size for a in arrs], dtype=np.uint64)
+    buf = np.ascontiguousarray(np.concatenate(arrs)) if int(buf_off[-1]) else np.zeros(1, np.uint8)
+    img_off = np.zeros(nrows + 1, dtype=np.uint64)
+    nblocks = np.zeros(nrows, dtype=np.uint64)
+    dbytes = np.zeros(nrows, dtype=np.uint64)
+    lib = _lib.load()
+    ptr = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+    args = (ptr(buf), ptr(buf_off), nrows, blockSize)
+    # A guess that holds the images of ordinary streams (at most a block's header and a 5-byte group per 4 uids of at
+    # least one byte each, plus the padding); DGX_ERR_CAP leaves the exact sizes behind for the one call that follows.
+    cap = 2 * int(buf_off[-1]) + 48 * nrows + 64
+    for _ in range(2):
+        img = _aligned_bytes(max(cap, 16))
+        rc = lib.dgx_encode_from_buffer_rows(*args, ptr(img), cap, ptr(img_off), ptr(nblocks), ptr(dbytes))
+        if rc != -4 or int(img_off[-1]) <= cap:
+            break
+        cap = int(img_off[-1])
+    _lib.check(rc)
+    lib_meta = lib.dgx_pack_image_size
+    packs = []
+    for i in range(nrows):
+        nb, db, o = int(nblocks[i]), int(dbytes[i]), int(img_off[i])
+        if nb == 0:
+            packs.append(None)
+            continue
+        meta = o + int(lib_meta(nb, 0))
+        packs.append(UidPack(blockSize, img[o: o + 8 * nb].view(np.uint64).copy(),
+                             img[o + 16 * nb + 8: o + 20 * nb + 8].view(np.uint32).copy(),
+                             img[o + 8 * nb: o + 16 * nb + 8].view(np.uint64).copy(), img[meta: meta + db].copy()))
+    return packs
+
+
+def EncodeFromBuffer(buf, blockSize: int) -> Optional[UidPack]:
+    """codec.EncodeFromBuffer(buf, blockSize): the pack of the uvarint-delta stream buf; an empty buf is the nil pack."""
+    return EncodeFromBufferRows([buf], blockSize)[0]

@@ -41,6 +41,10 @@ __device__ __forceinline__ void st_relaxed(u64* p, u64 v) {
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
+// Bytes of the metadata of a flat pack image (dgx_pack_image_view): [base u64 x nb | delta_off u64 x (nb+1) |
+// num_uids u32 x nb | pad to 16]; the delta bytes follow, padded to 16.
+__host__ __device__ __forceinline__ u64 pack_image_meta_bytes(u64 nb) { return (nb * 8 + (nb + 1) * 8 + nb * 4 + 15) & ~15ull; }
+
 // ---- searches --------------------------------------------------------------
 
 // First index in [0, n) with a[i] >= x (n if none).  Per-thread, global memory.

@@ -37,6 +37,7 @@
 #include "list_uids_kernel.cuh"
 #include "list_uids_unfiltered_kernel.cuh"
 #include "encode_kernel.cuh"
+#include "backup_codec_kernel.cuh"
 #include "wire.hpp"
 
 using namespace dgx;
@@ -450,6 +451,7 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
         *l->h_err = 0;
         CK(cudaMemsetAsync(l->d_err, 0, sizeof(int), l->stream));
         if (flag & kLaneErrOrder) return fail(DGX_ERR_ARG, "a row of the uid matrix is not strictly ascending");
+        if (flag & kLaneErrVarint) return fail(DGX_ERR_ARG, "a uid_bytes row is not a sequence of valid uvarints");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -1163,7 +1165,7 @@ static int packs_map_ws(dgx_lane* l, const dgx_pack_view* const* views, size_t k
 // Flat image of a pack (dgx_pack_image_size / dgx_pack_image_view): [base u64 x nb | delta_off u64 x (nb+1) |
 // num_uids u32 x nb | pad to 16 | deltas | pad to 16].  A shim that flattens pb.UidPack.Blocks into pinned staging
 // memory writes this directly; images written back to back travel as ONE DMA transfer.
-static size_t image_meta_bytes(size_t nb) { return (nb * 8 + (nb + 1) * 8 + nb * 4 + 15) & ~size_t(15); }
+static size_t image_meta_bytes(size_t nb) { return (size_t)pack_image_meta_bytes(nb); }
 static bool view_is_image(const dgx_pack_view* v) {
     const size_t nb = v->nblocks;
     const char* b = (const char*)v->base;
@@ -2971,6 +2973,388 @@ extern "C" int dgx_list_count_rows(const dgx_pack_ref* refs, size_t nrows, const
     if (nrows == 0) return DGX_OK;
     if (!counts) return fail(DGX_ERR_ARG, "null counts");
     return list_unfiltered_host(refs, nrows, mut_uids, mut_flags, mut_off, after_uid, 0, nullptr, nullptr, 0, counts);
+}
+
+// ---------------------------------------------------------------------------
+// Backup and restore: codec.DecodeToBuffer / codec.EncodeFromBuffer over a task's keys (backup_codec_kernel.cuh)
+// ---------------------------------------------------------------------------
+static void count_launches(dgx_lane* l, int n) {
+    l->launches += n;
+    g_stats.launches += n;
+}
+// Grid of the grid-stride passes whose length only the device knows (segments, blocks).
+static unsigned stride_grid() { return (unsigned)(g_num_sms * 8); }
+
+// Sum of ExactLen over the rows must stay below 2^32: checked before anything is copied.
+template <class Row>
+static int check_exact_total(const Row* rows, size_t nrows) {
+    uint64_t total = 0;
+    for (size_t r = 0; r < nrows; ++r) {
+        total += exact_len(rows[r]);
+        if (total >= (uint64_t(1) << 32))
+            return fail(DGX_ERR_ARG, "the packs hold %llu uids or more: at most 2^32 - 1", (unsigned long long)total);
+    }
+    return DGX_OK;
+}
+
+// Packs -> uid_bytes, planned: the job table, the per-block arrays and the look-back words in the lane's workspace.
+struct TbRun {
+    TbParams P;
+    u64* status;
+    u32* ticket;
+    const u64* d_nblk;
+};
+static int tb_plan(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows, TbRun* R) {
+    size_t nj = 0;
+    uint64_t nblk = 0, exact = 0;
+    for (size_t i = 0; i < nrows; ++i)
+        if (packs[i] && packs[i]->pk.nblocks) ++nj;
+    // table (copied): [jobs | row_blk (nrows + 1) | nblk];  zeroed: [status | ticket];  stop (all ones);  last, bytes, boff
+    const size_t b_jobs = (nj * sizeof(TbJob) + 15) & ~size_t(15), b_tab = b_jobs + (nrows + 2) * sizeof(uint64_t);
+    void* h_raw;
+    int rc = l->host.alloc(b_tab, &h_raw);
+    if (rc) return rc;
+    TbJob* hj = (TbJob*)h_raw;
+    uint64_t* h_rb = (uint64_t*)((char*)h_raw + b_jobs);
+    for (size_t i = 0, j = 0; i < nrows; ++i) {
+        h_rb[i] = nblk;
+        const dgx_dev_pack* p = packs[i];
+        if (!p || p->pk.nblocks == 0) continue;
+        TbJob& J = hj[j++];
+        J.pk = p->pk;
+        J.blk0 = nblk;
+        J.row = i;
+        nblk += p->pk.nblocks;
+        exact += p->exact_len;
+    }
+    h_rb[nrows] = nblk;
+    h_rb[nrows + 1] = nblk;
+    const size_t tiles = std::max<size_t>(1, (nblk + EN_TILE - 1) / EN_TILE);
+    const size_t b_zero = tiles * sizeof(u64) + 16, b_stop = nrows * sizeof(u64);
+    void* d_raw;
+    rc = l->ws.alloc(b_tab + b_zero + b_stop + (3 * nblk + 1) * sizeof(u64), &d_raw);
+    if (rc) return rc;
+    char* d = (char*)d_raw;
+    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
+    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
+    CK(cudaMemsetAsync(d + b_tab + b_zero, 0xff, b_stop, l->stream));
+    g_stats.h2d += b_tab;
+    g_stats.uids_in += exact;
+    TbParams& P = R->P;
+    P.jobs = (const TbJob*)d;
+    P.njobs = (u32)nj;
+    P.nblk = nblk;
+    P.row_blk = (const u64*)(d + b_jobs);
+    P.nrows = nrows;
+    R->d_nblk = P.row_blk + nrows + 1;
+    R->status = (u64*)(d + b_tab);
+    R->ticket = (u32*)(R->status + tiles);
+    P.stop = (u64*)(d + b_tab + b_zero);
+    P.last = P.stop + nrows;
+    P.bytes = P.last + nblk;
+    P.boff = P.bytes + nblk;
+    P.out = nullptr;
+    P.out_cap = 0;
+    P.out_off = nullptr;
+    P.err = nullptr;
+    return DGX_OK;
+}
+// The four launches (blocks, sizes, scan, write); write_only: the write pass again, once the host has sized the output.
+static int tb_launch(dgx_lane* l, const TbRun& R, bool write_only) {
+    const TbParams& P = R.P;
+    const unsigned g_blk = (unsigned)std::max<uint64_t>(1, (P.nblk + 255) / 256);
+    int launches = 1;
+    if (!write_only) {
+        tb_blocks_kernel<<<g_blk, 256, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        tb_sizes_kernel<<<g_blk, 256, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        const unsigned tiles = (unsigned)std::max<uint64_t>(1, (P.nblk + EN_TILE - 1) / EN_TILE);
+        scan_u64_kernel<<<tiles, EN_NT, 0, l->stream>>>(P.bytes, P.boff, R.d_nblk, P.nblk, R.status, R.ticket, nullptr);
+        CK(cudaGetLastError());
+        launches = 4;
+    }
+    const uint64_t nthreads = std::max<uint64_t>(P.nblk, P.nrows + 1);
+    tb_write_kernel<<<(unsigned)((nthreads + 255) / 256), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, launches);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_decode_to_buffer_rows(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows, uint8_t* d_out,
+                                             size_t out_cap, uint64_t* d_out_off) {
+    if (!l || !d_out_off) return fail(DGX_ERR_ARG, "null argument");
+    if (nrows == 0) {
+        if (int rc = lane_begin_op(l)) return rc;
+        CK(cudaMemsetAsync(d_out_off, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (!packs) return fail(DGX_ERR_ARG, "null packs");
+    if (int rc = check_exact_total(packs, nrows)) return rc;
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    TbRun R;
+    int rc = tb_plan(l, packs, nrows, &R);
+    if (rc) return rc;
+    R.P.out = d_out;
+    R.P.out_cap = out_cap;
+    R.P.out_off = (u64*)d_out_off;
+    R.P.err = l->d_err;
+    rc = tb_launch(l, R, false);
+    l->note_output(d_out, out_cap);
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    return rc;
+}
+
+extern "C" int dgx_decode_to_buffer_rows(const dgx_pack_ref* refs, size_t nrows, uint8_t* out, uint64_t* out_off,
+                                         size_t out_cap) {
+    if (!out_off) return fail(DGX_ERR_ARG, "null out_off");
+    if (nrows == 0) { out_off[0] = 0; return DGX_OK; }
+    if (!refs) return fail(DGX_ERR_ARG, "null refs");
+    if (int rc = check_exact_total(refs, nrows)) return rc;
+    {  // malformed packs are refused without a device (the staging below walks the same tables again)
+        std::vector<uint64_t> uoff;
+        for (size_t r = 0; r < nrows; ++r) {
+            const dgx_pack_view* v = refs[r].pack;
+            if (!v || v->nblocks == 0) continue;
+            uoff.resize(v->nblocks + 1);
+            uint64_t exact;
+            uint32_t max_num;
+            if (int rc = walk_block_table(v, uoff.data(), &exact, &max_num)) return rc;
+        }
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    PackSet ps(l, refs, nrows);
+    if (ps.rc) return ps.rc;
+    const std::vector<const dgx_dev_pack*> rows = ps.rows();
+    TbRun R;
+    int rc = tb_plan(l, rows.data(), nrows, &R);
+    if (rc) return rc;
+    void* d_off;
+    if ((rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off))) return rc;
+    R.P.out_off = (u64*)d_off;
+    if ((rc = tb_launch(l, R, false))) return rc;  // sizes only: the exact byte count is known after this pass
+    CK(cudaMemcpyAsync(out_off, d_off, (nrows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) return ps.synced(rc);
+    g_stats.d2h += (nrows + 1) * sizeof(uint64_t);
+    const uint64_t total = out_off[nrows];
+    if (!out || total == 0) return ps.synced(DGX_OK);
+    if (total > out_cap)
+        return ps.synced(fail(DGX_ERR_CAP, "uid_bytes (%llu bytes) do not fit out_cap (%zu)", (unsigned long long)total, out_cap));
+    void* d_out;
+    if ((rc = l->ws.alloc(total + 16, &d_out))) return rc;
+    R.P.out = (unsigned char*)d_out;
+    R.P.out_cap = total;
+    if ((rc = tb_launch(l, R, true))) return rc;
+    CK(cudaMemcpyAsync(out, d_out, total, cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += total;
+    return ps.synced(DGX_OK);
+}
+
+// uid_bytes -> packs, planned: the row offsets copied, the look-back words zeroed, the per-value, per-segment and
+// per-block arrays in the lane's workspace.  The counts are only known on the device, so the arrays are sized for the
+// bound every one of them obeys (values, segments and blocks are at most one per input byte): about 52 bytes per byte.
+struct BfRun {
+    BfParams P;
+    size_t tiles, row_tiles;
+    u64 *st_segscan, *st_bytescan, *st_imgscan;
+    const u64* d_nrows;
+};
+static int bf_plan(dgx_lane* l, const uint8_t* d_buf, const uint64_t* buf_off, size_t nrows, uint32_t block_size,
+                   BfRun* R) {
+    const uint64_t n = buf_off[nrows];
+    const size_t T = n / EN_TILE + 1, Tr = nrows / EN_TILE + 1;  // look-back words per scan region
+    const size_t b_tab = (nrows + 2) * sizeof(uint64_t);
+    const size_t b_zero = 64 + 32 + 16 + (4 * T + Tr) * sizeof(u64) + ((T * sizeof(u32) + 15) & ~size_t(15)) + 2 * T * sizeof(u64);
+    const size_t b_rest = (8 * n) + ((4 * n + 15) & ~size_t(15)) + 8 * nrows + ((4 * (n + 1) + 15) & ~size_t(15)) +
+                          8 * n + 8 * (n + 1) + 8 * n + 8 * (n + 1) + ((4 * n + 15) & ~size_t(15)) + 8 * (nrows + 1) +
+                          8 * nrows + 64;
+    void *h_raw, *d_raw;
+    int rc = l->host.alloc(b_tab, &h_raw);
+    if (rc) return rc;
+    memcpy(h_raw, buf_off, (nrows + 1) * sizeof(uint64_t));
+    ((uint64_t*)h_raw)[nrows + 1] = nrows;
+    rc = l->ws.alloc(b_tab + b_zero + b_rest, &d_raw);
+    if (rc) return rc;
+    char* d = (char*)d_raw;
+    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
+    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
+    g_stats.h2d += b_tab;
+    BfParams& P = R->P;
+    P.buf = d_buf;
+    P.n = n;
+    P.row_off = (const u64*)d;
+    R->d_nrows = P.row_off + nrows + 1;
+    P.nrows = nrows;
+    P.bsz = block_size ? block_size : 1;
+    char* z = d + b_tab;
+    P.counts = (u64*)z;
+    P.ticket = (u32*)(z + 64);
+    P.bad = (int*)(z + 96);
+    P.status = (u64*)(z + 112);
+    R->st_segscan = P.status + 2 * T;
+    R->st_bytescan = P.status + 3 * T;
+    R->st_imgscan = P.status + 4 * T;
+    P.sum_flag = (u32*)(P.status + 4 * T + Tr);
+    P.sum_val = (u64*)((char*)P.sum_flag + ((T * sizeof(u32) + 15) & ~size_t(15)));
+    char* q = d + b_tab + b_zero;
+    auto take = [&](size_t bytes) { char* r = q; q += (bytes + 15) & ~size_t(15); return r; };
+    P.pre = (u64*)take(8 * n);
+    P.vrow = (u32*)take(4 * n);
+    P.rowbase = (u64*)take(8 * nrows);
+    P.seg_start = (u32*)take(4 * (n + 1));
+    P.seg_cnt = (u64*)take(8 * n);
+    P.seg_blk = (u64*)take(8 * (n + 1));
+    P.blk_bytes = (u64*)take(8 * n);
+    P.blk_doff = (u64*)take(8 * (n + 1));
+    P.brow = (u32*)take(4 * n);
+    P.row_blk = (u64*)take(8 * (nrows + 1));
+    P.img_bytes = (u64*)take(8 * nrows);
+    R->tiles = (n + EN_TILE - 1) / EN_TILE;
+    R->row_tiles = (nrows + EN_TILE - 1) / EN_TILE;
+    P.img = nullptr;
+    P.img_cap = 0;
+    P.img_off = P.nblocks = P.delta_bytes = nullptr;
+    P.err = nullptr;
+    g_stats.uids_in += n;
+    return DGX_OK;
+}
+// The nine launches; write_only: the write pass again, once the host has sized the images.
+static int bf_launch(dgx_lane* l, const BfRun& R, bool write_only) {
+    const BfParams& P = R.P;
+    const unsigned G = stride_grid(), tiles = (unsigned)R.tiles;
+    int launches = 1;
+    if (!write_only) {
+        bf_values_kernel<<<tiles, EN_NT, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        bf_segments_kernel<<<tiles, EN_NT, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        bf_segcount_kernel<<<G, 256, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        scan_u64_kernel<<<tiles, EN_NT, 0, l->stream>>>(P.seg_cnt, P.seg_blk, P.counts + 1, P.n, R.st_segscan, P.ticket + 2,
+                                                         P.counts + 2);
+        CK(cudaGetLastError());
+        bf_sizes_kernel<<<G, 256, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        scan_u64_kernel<<<tiles, EN_NT, 0, l->stream>>>(P.blk_bytes, P.blk_doff, P.counts + 2, P.n, R.st_bytescan,
+                                                         P.ticket + 3, P.counts + 3);
+        CK(cudaGetLastError());
+        bf_rows_kernel<<<G, 256, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        scan_u64_kernel<<<(unsigned)R.row_tiles, EN_NT, 0, l->stream>>>(P.img_bytes, P.img_off, R.d_nrows, P.nrows,
+                                                                         R.st_imgscan, P.ticket + 4, P.counts + 4);
+        CK(cudaGetLastError());
+        launches = 9;
+    }
+    bf_write_kernel<<<G, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, launches);
+    return DGX_OK;
+}
+// The checks of both forms before anything is copied; *n gets the byte count.
+static int bf_check(const void* buf, const uint64_t* buf_off, size_t nrows, const void* img, const void* nblocks,
+                    const void* delta_bytes, uint64_t* n) {
+    if (!buf_off || !nblocks || !delta_bytes) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = check_offsets("buf_off", buf_off, nrows, uint64_t(1) << 32)) return rc;
+    *n = buf_off[nrows];
+    if (*n && !buf) return fail(DGX_ERR_ARG, "null buf");
+    if (reinterpret_cast<uintptr_t>(img) & 15u) return fail(DGX_ERR_ARG, "img must be 16-byte aligned");
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_encode_from_buffer_rows(dgx_lane* l, const uint8_t* d_buf, const uint64_t* buf_off, size_t nrows,
+                                               uint32_t block_size, void* d_img, size_t img_cap, uint64_t* d_img_off,
+                                               uint64_t* d_nblocks, uint64_t* d_delta_bytes) {
+    if (!l || !d_img_off) return fail(DGX_ERR_ARG, "null argument");
+    if (nrows == 0) {
+        if (int rc = lane_begin_op(l)) return rc;
+        CK(cudaMemsetAsync(d_img_off, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    uint64_t n;
+    if (int rc = bf_check(d_buf, buf_off, nrows, d_img, d_nblocks, d_delta_bytes, &n)) return rc;
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_img, img_cap);
+    l->note_output(d_img_off, (nrows + 1) * sizeof(uint64_t));
+    l->note_output(d_nblocks, nrows * sizeof(uint64_t));
+    l->note_output(d_delta_bytes, nrows * sizeof(uint64_t));
+    if (n == 0) {  // every row empty: nil packs
+        CK(cudaMemsetAsync(d_img_off, 0, (nrows + 1) * sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_nblocks, 0, nrows * sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_delta_bytes, 0, nrows * sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    BfRun R;
+    int rc = bf_plan(l, d_buf, buf_off, nrows, block_size, &R);
+    if (rc) return rc;
+    R.P.img = (unsigned char*)d_img;
+    R.P.img_cap = img_cap;
+    R.P.img_off = (u64*)d_img_off;
+    R.P.nblocks = (u64*)d_nblocks;
+    R.P.delta_bytes = (u64*)d_delta_bytes;
+    R.P.err = l->d_err;
+    return bf_launch(l, R, false);
+}
+
+extern "C" int dgx_encode_from_buffer_rows(const uint8_t* buf, const uint64_t* buf_off, size_t nrows, uint32_t block_size,
+                                           void* img, size_t img_cap, uint64_t* img_off, uint64_t* nblocks,
+                                           uint64_t* delta_bytes) {
+    if (!img_off) return fail(DGX_ERR_ARG, "null img_off");
+    if (nrows == 0) { img_off[0] = 0; return DGX_OK; }
+    uint64_t n;
+    if (int rc = bf_check(buf, buf_off, nrows, img, nblocks, delta_bytes, &n)) return rc;
+    if (n == 0) {  // every row empty: nil packs
+        memset(img_off, 0, (nrows + 1) * sizeof(uint64_t));
+        memset(nblocks, 0, nrows * sizeof(uint64_t));
+        memset(delta_bytes, 0, nrows * sizeof(uint64_t));
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    void *d_buf, *d_arr;
+    int rc = l->ws.alloc(n + 16, &d_buf);
+    if (rc) return rc;
+    if ((rc = l->ws.alloc((3 * nrows + 1) * sizeof(uint64_t), &d_arr))) return rc;
+    CK(cudaMemcpyAsync(d_buf, buf, n, cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += n;
+    BfRun R;
+    if ((rc = bf_plan(l, (const uint8_t*)d_buf, buf_off, nrows, block_size, &R))) return rc;
+    R.P.img_off = (u64*)d_arr;
+    R.P.nblocks = R.P.img_off + nrows + 1;
+    R.P.delta_bytes = R.P.nblocks + nrows;
+    if ((rc = bf_launch(l, R, false))) return rc;  // sizes only: the exact image bytes are known after this pass
+    CK(cudaMemcpyAsync(l->h_word, R.P.bad, sizeof(int), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(img_off, R.P.img_off, (nrows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(nblocks, R.P.nblocks, nrows * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(delta_bytes, R.P.delta_bytes, nrows * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) return rc;
+    g_stats.d2h += (3 * nrows + 1) * sizeof(uint64_t);
+    if (*(const int*)l->h_word) {
+        memset(img_off, 0, (nrows + 1) * sizeof(uint64_t));
+        memset(nblocks, 0, nrows * sizeof(uint64_t));
+        memset(delta_bytes, 0, nrows * sizeof(uint64_t));
+        return fail(DGX_ERR_ARG, "a uid_bytes row is not a sequence of valid uvarints");
+    }
+    const uint64_t total = img_off[nrows];
+    if (!img || total == 0) return DGX_OK;
+    if (total > img_cap)
+        return fail(DGX_ERR_CAP, "pack images (%llu bytes) do not fit img_cap (%zu)", (unsigned long long)total, img_cap);
+    void* d_img;
+    if ((rc = l->ws.alloc(total, &d_img))) return rc;
+    R.P.img = (unsigned char*)d_img;
+    R.P.img_cap = total;
+    if ((rc = bf_launch(l, R, true))) return rc;
+    CK(cudaMemcpyAsync(img, d_img, total, cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += total;
+    return DGX_OK;
 }
 
 // ---------------------------------------------------------------------------

@@ -138,14 +138,73 @@ __device__ __forceinline__ u64 enc_n(const EncParams& P) {
 
 __device__ __forceinline__ u32 gv_len(u32 v) { return v < (1u << 8) ? 1u : (v < (1u << 16) ? 2u : (v < (1u << 24) ? 3u : 4u)); }
 
-// The four deltas of group g of the block starting at uid index `start` with `num` uids (zero-padded).
-__device__ __forceinline__ void enc_group(const u64* __restrict__ u, u64 start, u32 num, u32 g, u32 (&d)[4]) {
+// The four deltas of group g of the block starting at uid index `start` with `num` uids (zero-padded); uid(i) reads
+// uid i of the list being encoded.
+template <class Uid>
+__device__ __forceinline__ void enc_group(const Uid& uid, u64 start, u32 num, u32 g, u32 (&d)[4]) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const u32 pos = 1u + 4u * g + (u32)j;  // uid position inside the block
-        d[j] = pos < num ? (u32)(u[start + pos] - u[start + pos - 1]) : 0u;
+        d[j] = pos < num ? (u32)(uid(start + pos) - uid(start + pos - 1)) : 0u;
     }
 }
+
+// Groups of an encoded block of num uids: max(1, ceil((num-1)/4)) -- a 1-uid block still emits one all-zero group.
+__device__ __forceinline__ u32 enc_groups(u32 num) { return num > 1 ? (num + 2) / 4 : 1; }
+
+// Byte length of the block's groups, summed over the warp (every lane returns it).  Called by the whole warp.
+template <class Uid>
+__device__ __forceinline__ u32 enc_block_bytes(const Uid& uid, u64 start, u32 num, int lane) {
+    const u32 ngroups = enc_groups(num);
+    u32 bytes = 0;
+    for (u32 g = lane; g < ngroups; g += 32) {
+        u32 d[4];
+        enc_group(uid, start, num, g, d);
+        bytes += 1u + gv_len(d[0]) + gv_len(d[1]) + gv_len(d[2]) + gv_len(d[3]);
+    }
+#pragma unroll
+    for (int dl = 16; dl > 0; dl >>= 1) bytes += __shfl_xor_sync(0xffffffffu, bytes, dl);
+    return bytes;
+}
+
+// The block's groups written at dst: lane g writes group g of every round of 32.  Called by the whole warp.
+template <class Uid>
+__device__ __forceinline__ void enc_block_write(const Uid& uid, u64 start, u32 num, unsigned char* dst, int lane) {
+    const u32 ngroups = enc_groups(num);
+    u32 carry = 0;
+    for (u32 g0 = 0; g0 < ngroups; g0 += 32) {
+        const u32 g = g0 + lane;
+        u32 d[4] = {0, 0, 0, 0};
+        u32 l[4] = {0, 0, 0, 0};
+        u32 bytes = 0;
+        if (g < ngroups) {
+            enc_group(uid, start, num, g, d);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) l[j] = gv_len(d[j]);
+            bytes = 1u + l[0] + l[1] + l[2] + l[3];
+        }
+        u32 inc = bytes;
+#pragma unroll
+        for (int dl = 1; dl < 32; dl <<= 1) {
+            const u32 t = __shfl_up_sync(0xffffffffu, inc, dl);
+            if (lane >= dl) inc += t;
+        }
+        if (g < ngroups) {
+            unsigned char* p = dst + carry + inc - bytes;
+            *p++ = (unsigned char)((l[0] - 1u) | ((l[1] - 1u) << 2) | ((l[2] - 1u) << 4) | ((l[3] - 1u) << 6));
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                for (u32 t = 0; t < l[j]; ++t) *p++ = (unsigned char)(d[j] >> (8u * t));
+        }
+        carry += __shfl_sync(0xffffffffu, inc, 31);
+    }
+}
+
+// uid(i) of a list held as an array
+struct EncUidArray {
+    const u64* u;
+    __device__ __forceinline__ u64 operator()(u64 i) const { return u[i]; }
+};
 
 // Warp per block: Base, NumUids, bytes.
 __global__ void __launch_bounds__(256) enc_sizes_kernel(const EncParams P) {
@@ -163,15 +222,7 @@ __global__ void __launch_bounds__(256) enc_sizes_kernel(const EncParams P) {
     const u64 start = P.seg_start[lo] + (b - P.seg_blk[lo]) * (u64)P.bsz;
     const u64 seg_end = P.seg_start[lo + 1];
     const u32 num = (u32)((seg_end - start) < (u64)P.bsz ? (seg_end - start) : (u64)P.bsz);
-    const u32 ngroups = num > 1 ? (num + 2) / 4 : 1;  // max(1, ceil((num-1)/4))
-    u32 bytes = 0;
-    for (u32 g = lane; g < ngroups; g += 32) {
-        u32 d[4];
-        enc_group(P.u, start, num, g, d);
-        bytes += 1u + gv_len(d[0]) + gv_len(d[1]) + gv_len(d[2]) + gv_len(d[3]);
-    }
-#pragma unroll
-    for (int dl = 16; dl > 0; dl >>= 1) bytes += __shfl_xor_sync(0xffffffffu, bytes, dl);
+    const u32 bytes = enc_block_bytes(EncUidArray{P.u}, start, num, lane);
     if (lane == 0) {
         P.base[b] = P.u[start];
         P.num[b] = num;
@@ -233,37 +284,7 @@ __global__ void __launch_bounds__(256) enc_write_kernel(const EncParams P) {
     const int lane = threadIdx.x & 31;
     const u64 b = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (b >= nblocks) return;
-    const u64 start = P.blk_start[b];
-    const u32 num = P.num[b];
-    const u32 ngroups = num > 1 ? (num + 2) / 4 : 1;
-    unsigned char* dst = P.deltas + P.delta_off[b];
-    u32 carry = 0;
-    for (u32 g0 = 0; g0 < ngroups; g0 += 32) {
-        const u32 g = g0 + lane;
-        u32 d[4] = {0, 0, 0, 0};
-        u32 l[4] = {0, 0, 0, 0};
-        u32 bytes = 0;
-        if (g < ngroups) {
-            enc_group(P.u, start, num, g, d);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) l[j] = gv_len(d[j]);
-            bytes = 1u + l[0] + l[1] + l[2] + l[3];
-        }
-        u32 inc = bytes;
-#pragma unroll
-        for (int dl = 1; dl < 32; dl <<= 1) {
-            const u32 t = __shfl_up_sync(0xffffffffu, inc, dl);
-            if (lane >= dl) inc += t;
-        }
-        if (g < ngroups) {
-            unsigned char* p = dst + carry + inc - bytes;
-            *p++ = (unsigned char)((l[0] - 1u) | ((l[1] - 1u) << 2) | ((l[2] - 1u) << 4) | ((l[3] - 1u) << 6));
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-                for (u32 t = 0; t < l[j]; ++t) *p++ = (unsigned char)(d[j] >> (8u * t));
-        }
-        carry += __shfl_sync(0xffffffffu, inc, 31);
-    }
+    enc_block_write(EncUidArray{P.u}, P.blk_start[b], P.num[b], P.deltas + P.delta_off[b], lane);
 }
 
 }  // namespace dgx

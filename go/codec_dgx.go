@@ -674,3 +674,135 @@ func ListCountRows(refs []PackRef, muts []MutRow, afterUID uint64) ([]uint32, bo
 	}
 	return counts, true
 }
+
+// DecodeToBufferRows is codec.DecodeToBuffer (codec/codec.go:456-467) for every key of a backup batch in ONE library
+// call: the uid_bytes List.ToBackupPostingList (posting/list.go:1461-1482) writes for each key that worker/backup.go:712
+// visits.  Row i is the uvarint-delta stream of refs[i].Pack (nil / empty pack: no bytes); the rows are slices of one
+// buffer.  Named packs use the HBM cache, anonymous ones are staged as one run of flat images.  Returns false when the
+// caller must keep the Go path: on any error (a malformed pack, 2^32 uids or more in the batch).
+func DecodeToBufferRows(refs []PackRef) ([][]byte, bool) {
+	n := len(refs)
+	if n == 0 {
+		return [][]byte{}, true
+	}
+	img := 0
+	for _, r := range refs {
+		if r.Pack != nil && len(r.Pack.Blocks) > 0 && r.Key == 0 {
+			img += int(C.dgx_pack_image_size(C.size_t(len(r.Pack.Blocks)), C.size_t(deltaBytes(r.Pack))))
+		}
+	}
+	crefs := (*[1 << 28]C.dgx_pack_ref)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(C.dgx_pack_ref{}))))
+	views := (*[1 << 28]C.dgx_pack_view)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(C.dgx_pack_view{}))))
+	stage := C.malloc(C.size_t(img + 64))
+	frees := []func(){}
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+		C.free(unsafe.Pointer(crefs))
+		C.free(unsafe.Pointer(views))
+		C.free(stage)
+	}()
+	o := 0
+	for i, r := range refs {
+		crefs[i] = C.dgx_pack_ref{key: C.uint64_t(r.Key), version: C.uint64_t(r.Version)}
+		if r.Pack == nil || len(r.Pack.Blocks) == 0 {
+			continue // no bytes
+		}
+		if r.Key != 0 {
+			view, free := flatten(r.Pack)
+			frees = append(frees, free)
+			views[i] = view
+		} else {
+			nb, db := len(r.Pack.Blocks), deltaBytes(r.Pack)
+			if C.dgx_pack_image_view(unsafe.Add(stage, o), C.uint32_t(r.Pack.BlockSize), C.size_t(nb), C.size_t(db), &views[i]) != C.DGX_OK {
+				return nil, false
+			}
+			fillImage(&views[i], r.Pack)
+			o += int(C.dgx_pack_image_size(C.size_t(nb), C.size_t(db)))
+		}
+		crefs[i].pack = &views[i]
+	}
+	// at most 10 bytes per uid: one call sizes nothing and writes everything
+	capOut := 0
+	for _, r := range refs {
+		capOut += 10 * ExactLen(r.Pack)
+	}
+	out := make([]byte, capOut+1)
+	off := make([]uint64, n+1)
+	if C.dgx_decode_to_buffer_rows(&crefs[0], C.size_t(n), (*C.uint8_t)(unsafe.Pointer(&out[0])),
+		(*C.uint64_t)(unsafe.Pointer(&off[0])), C.size_t(capOut)) != C.DGX_OK {
+		return nil, false
+	}
+	rows := make([][]byte, n)
+	for i := range refs {
+		rows[i] = out[off[i]:off[i+1]:off[i+1]]
+	}
+	return rows, true
+}
+
+// EncodeFromBufferRows is codec.EncodeFromBuffer(bufs[i], blockSize) (codec/codec.go:402-414) for every key of a
+// restore batch in ONE library call: the packs FromBackupPostingList (posting/list.go:2427-2441) rebuilds from each
+// backed-up key's uid_bytes (worker/restore_map.go:372-377).  An empty buffer gives the nil pack.  The bytes cross as
+// one C allocation; the packs come back as flat images and are copied into pb.UidPack values.  Returns false when the
+// caller must keep the Go path: on any error, including a buffer that is not a sequence of valid uvarints (where
+// EncodeFromBuffer would panic or never return) and 2^32 input bytes or more.
+func EncodeFromBufferRows(bufs [][]byte, blockSize int) ([]*pb.UidPack, bool) {
+	n := len(bufs)
+	if n == 0 {
+		return []*pb.UidPack{}, true
+	}
+	total := 0
+	for _, b := range bufs {
+		total += len(b)
+	}
+	if uint64(total) >= 1<<32 {
+		return nil, false
+	}
+	cbuf := C.malloc(C.size_t(total + 1))
+	defer C.free(cbuf)
+	off := make([]uint64, n+1)
+	for i, b := range bufs {
+		if len(b) > 0 {
+			C.memcpy(unsafe.Add(cbuf, off[i]), unsafe.Pointer(&b[0]), C.size_t(len(b)))
+		}
+		off[i+1] = off[i] + uint64(len(b))
+	}
+	imgOff := make([]uint64, n+1)
+	nblocks := make([]uint64, n)
+	dbytes := make([]uint64, n)
+	call := func(img unsafe.Pointer, imgCap int) C.int {
+		return C.dgx_encode_from_buffer_rows((*C.uint8_t)(cbuf), (*C.uint64_t)(unsafe.Pointer(&off[0])), C.size_t(n),
+			C.uint32_t(blockSize), img, C.size_t(imgCap), (*C.uint64_t)(unsafe.Pointer(&imgOff[0])),
+			(*C.uint64_t)(unsafe.Pointer(&nblocks[0])), (*C.uint64_t)(unsafe.Pointer(&dbytes[0])))
+	}
+	if call(nil, 0) != C.DGX_OK { // sizes
+		return nil, false
+	}
+	img := C.aligned_alloc(16, C.size_t(imgOff[n]+16))
+	defer C.free(img)
+	if call(img, int(imgOff[n])) != C.DGX_OK {
+		return nil, false
+	}
+	packs := make([]*pb.UidPack, n)
+	for i := 0; i < n; i++ {
+		nb := int(nblocks[i])
+		if nb == 0 {
+			continue // the nil pack
+		}
+		var v C.dgx_pack_view
+		if C.dgx_pack_image_view(unsafe.Add(img, imgOff[i]), C.uint32_t(blockSize), C.size_t(nb), C.size_t(dbytes[i]), &v) != C.DGX_OK {
+			return nil, false
+		}
+		base := unsafe.Slice((*uint64)(unsafe.Pointer(v.base)), nb)
+		num := unsafe.Slice((*uint32)(unsafe.Pointer(v.num_uids)), nb)
+		doff := unsafe.Slice((*uint64)(unsafe.Pointer(v.delta_off)), nb+1)
+		deltas := C.GoBytes(unsafe.Pointer(v.deltas), C.int(dbytes[i]))
+		p := &pb.UidPack{BlockSize: uint32(blockSize), Blocks: make([]*pb.UidBlock, nb)}
+		for b := 0; b < nb; b++ {
+			p.Blocks[b] = &pb.UidBlock{Base: base[b], NumUids: num[b], Deltas: deltas[doff[b]:doff[b+1]:doff[b+1]]}
+		}
+		packs[i] = p
+	}
+	return packs, true
+}

@@ -284,6 +284,41 @@ int dgx_list_count_rows(const dgx_pack_ref* refs, size_t nrows,
                         const uint64_t* mut_uids, const uint8_t* mut_flags, const uint64_t* mut_off,
                         uint64_t after_uid, uint32_t* counts);
 
+/* The uid path of backup and restore over a task's keys, one call each: List.ToBackupPostingList writes
+ * BackupPostingList.uid_bytes with codec.DecodeToBuffer (posting/list.go:1461-1482, codec/codec.go:456-467) and
+ * FromBackupPostingList rebuilds the pack with codec.EncodeFromBuffer(uid_bytes, 256) (posting/list.go:2427-2441,
+ * codec/codec.go:402-414).  uid_bytes is binary.PutUvarint(u - last) for every uid u of Decode(pack, 0), the subtraction
+ * on uint64 (it wraps: a pack need not ascend), last starting at 0.  Decoding stops at the first block with NumUids 0, as
+ * the reference's `for len(uids) > 0` loop does; dgx_decode is not changed by this.
+ *
+ * codec.DecodeToBuffer(pack_i) for every row: row i's bytes are out[out_off[i] .. out_off[i+1]).  refs[i] as in
+ * dgx_intersect_compressed_rows (named packs use the HBM cache, anonymous ones cross PCIe together); a NULL / empty pack
+ * gives no bytes.  out == NULL only sizes (out_off is filled; a device is still needed).  A result longer than out_cap
+ * is DGX_ERR_CAP: nothing is written to out and out_off holds the exact offsets, so out_off[nrows] is the capacity that
+ * makes one more call succeed.  DGX_ERR_ARG before anything is copied: a null array that is needed, a sum of ExactLen of
+ * 2^32 or more, a malformed pack.  nrows == 0 gives out_off[0] = 0 and needs no device.  The call runs a fixed number of
+ * kernel launches whatever nrows, the number of uids and the pack sizes are. */
+int dgx_decode_to_buffer_rows(const dgx_pack_ref* refs, size_t nrows,
+                              uint8_t* out, uint64_t* out_off, size_t out_cap);
+/* codec.EncodeFromBuffer(buf_i, block_size) for every row: row i's input is buf[buf_off[i] .. buf_off[i+1]) (host
+ * offsets, nrows + 1 values, buf_off[0] == 0), a value never continues into the next row.  Row i's pack is a flat image
+ * (dgx_pack_image_view layout) at img + img_off[i] with nblocks[i] blocks and delta_bytes[i] delta bytes; an empty row
+ * is the nil pack (nblocks 0, empty image).  The images are 16-byte aligned and back to back, so the result passed to
+ * any pack entry point crosses PCIe as one transfer.  binary.Uvarint rules: a byte < 0x80 ends a value, non-minimal
+ * encodings are accepted, a value has at most 10 bytes and its 10th is <= 1.  img == NULL only sizes (img_off, nblocks
+ * and delta_bytes are filled; a device is still needed).  Images longer than img_cap are DGX_ERR_CAP: nothing is written
+ * to img and the offset and size arrays hold the exact values.  DGX_ERR_ARG before anything is copied: buf_off[0] != 0,
+ * decreasing offsets, buf_off[nrows] >= 2^32, a null array that is needed, img not 16-byte aligned.  DGX_ERR_ARG after
+ * the kernels, with img untouched and img_off / nblocks / delta_bytes zeroed: a row that is not a sequence of valid
+ * uvarints (a value of more than 10 bytes, a 10th byte > 1, a row that ends inside a value -- where the reference
+ * panics or loops).  nrows == 0 gives img_off[0] = 0 and needs no device.  The call runs a fixed number of kernel
+ * launches whatever nrows, the number of bytes and block_size are.  Workspace: the value, segment and block counts are
+ * only known on the device, so the call reserves room for one of each per input byte, about 52 bytes of HBM per input
+ * byte (5.2 GB for 100 MB of uid_bytes); a batch larger than the free HBM allows is DGX_ERR_OOM, and the caller splits
+ * it by keys.  A lane of the host form whose workspace grew past 4 GiB gives it back when the call returns. */
+int dgx_encode_from_buffer_rows(const uint8_t* buf, const uint64_t* buf_off, size_t nrows, uint32_t block_size,
+                                void* img, size_t img_cap, uint64_t* img_off, uint64_t* nblocks, uint64_t* delta_bytes);
+
 /* algo.MergeSorted(rows) over the rows of a uid matrix, one call: sg.DestUIDs = algo.MergeSorted(result.UidMatrix)
  * (query/query.go:2290, 2505; query/recurse.go:134; worker/task.go:1629, 1706; worker/match.go:100).
  * Row i is v[v_off[i] .. v_off[i+1]) (host offsets, nrows + 1 values, v_off[0] == 0).  Rows ascend; duplicates
@@ -468,6 +503,18 @@ int dgx_dev_list_uids_unfiltered_rows(dgx_lane* lane, const dgx_dev_pack* const*
 int dgx_dev_list_count_rows(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t nrows,
                             const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
                             uint64_t after_uid, uint32_t* d_counts);
+/* Device forms of dgx_decode_to_buffer_rows and dgx_encode_from_buffer_rows: packs resident (dgx_dev_pack_upload; NULL
+ * = nil pack), d_out / d_out_off (nrows + 1 values) and d_buf / d_img / d_img_off (nrows + 1 values) / d_nblocks /
+ * d_delta_bytes (nrows values) device pointers, buf_off in HOST memory, checked as in the host forms before anything is
+ * queued.  d_out == NULL / d_img == NULL only size.  Asynchronous on the lane: past out_cap / img_cap nothing is written
+ * to d_out / d_img, the offsets are exact and the next dgx_lane_sync returns DGX_ERR_CAP; a malformed uid_bytes row
+ * leaves d_img untouched, zeroes d_img_off / d_nblocks / d_delta_bytes and makes the next dgx_lane_sync return
+ * DGX_ERR_ARG. */
+int dgx_dev_decode_to_buffer_rows(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t nrows,
+                                  uint8_t* d_out, size_t out_cap, uint64_t* d_out_off);
+int dgx_dev_encode_from_buffer_rows(dgx_lane* lane, const uint8_t* d_buf, const uint64_t* buf_off, size_t nrows,
+                                    uint32_t block_size, void* d_img, size_t img_cap, uint64_t* d_img_off,
+                                    uint64_t* d_nblocks, uint64_t* d_delta_bytes);
 /* Device form of dgx_merge_sorted_matrix: d_v and d_v_off (nrows + 1 values) are DEVICE pointers, so the
  * (d_out, d_out_off) of dgx_dev_intersect_compressed_rows / dgx_dev_filter_batch feed it directly.  v_cap >=
  * d_v_off[nrows] sizes the workspace (v_cap >= 2^32 is DGX_ERR_ARG).  d_out_len: one device uint64, the result length.

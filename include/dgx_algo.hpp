@@ -6,7 +6,8 @@
 // meaning, aliasing rules and nil/empty result shapes as
 //   /root/reference/algo/uidlist.go   (IntersectWith :142, IntersectSorted :297,
 //                                      MergeSorted :448, Difference :332)
-//   /root/reference/codec/codec.go    (Decode :444, ApproxLen :418, ExactLen :427)
+//   /root/reference/codec/codec.go    (Decode :444, ApproxLen :418, ExactLen :427, DecodeToBuffer :456,
+//                                      EncodeFromBuffer :402)
 // Every body is one libdgx call -- exactly what the cgo shim (go/algo_dgx.go) does.
 // Errors: the Go functions cannot fail; here a non-zero dgx status throws
 // dgx::Error so callers (the shim: fall back to the Go code) can react.
@@ -144,6 +145,44 @@ inline std::vector<uint64_t> Decode(const pb::UidPack* p, uint64_t seek) {
     check(dgx_decode(&v, seek, out.data(), cap, &n));
     out.resize(n);
     return out;
+}
+
+// DecodeToBuffer(pack) (codec.go:456-467): binary.PutUvarint(u - last) for every uid of Decode(pack, 0), the
+// subtraction on uint64; nil pack -> no bytes.  One dgx_decode_to_buffer_rows call (a uvarint is at most 10 bytes).
+inline std::vector<uint8_t> DecodeToBuffer(const pb::UidPack* p) {
+    std::vector<uint8_t> out;
+    if (p == nullptr || p->base.empty()) return out;
+    const size_t cap = 10 * ExactLen(p);
+    out.resize(std::max<size_t>(cap, 1));
+    const dgx_pack_view v = p->view();
+    const dgx_pack_ref ref{&v, 0, 0};
+    uint64_t off[2] = {0, 0};
+    check(dgx_decode_to_buffer_rows(&ref, 1, out.data(), off, cap));
+    out.resize(off[1]);
+    return out;
+}
+
+// EncodeFromBuffer(buf, blockSize) (codec.go:402-414): the pack of the uvarint-delta stream; an empty buf is the nil
+// pack (no blocks).  A buf that is not a sequence of valid uvarints (where the Go function panics or never returns)
+// throws dgx::Error with DGX_ERR_ARG.  One dgx_encode_from_buffer_rows call to size, one to write.
+inline pb::UidPack EncodeFromBuffer(const std::vector<uint8_t>& buf, uint32_t block_size) {
+    pb::UidPack p;
+    p.block_size = block_size;
+    if (buf.empty()) return p;
+    const uint64_t buf_off[2] = {0, buf.size()};
+    uint64_t img_off[2] = {0, 0}, nb = 0, db = 0;
+    check(dgx_encode_from_buffer_rows(buf.data(), buf_off, 1, block_size, nullptr, 0, img_off, &nb, &db));
+    std::vector<uint64_t> img((img_off[1] + 7) / 8 + 2);  // 8-byte aligned storage; the image needs 16
+    char* a = reinterpret_cast<char*>(img.data());
+    a += (16 - reinterpret_cast<uintptr_t>(a) % 16) % 16;
+    check(dgx_encode_from_buffer_rows(buf.data(), buf_off, 1, block_size, a, img_off[1], img_off, &nb, &db));
+    dgx_pack_view v;
+    check(dgx_pack_image_view(a, block_size, nb, db, &v));
+    p.base.assign(v.base, v.base + nb);
+    p.num_uids.assign(v.num_uids, v.num_uids + nb);
+    p.delta_off.assign(v.delta_off, v.delta_off + nb + 1);
+    p.deltas.assign(v.deltas, v.deltas + db);
+    return p;
 }
 
 }  // namespace codec

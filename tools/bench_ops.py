@@ -136,6 +136,7 @@ def main():
     ap.add_argument("--c8-only", action="store_true", help="only the C8 DestUIDs (MergeSorted of a uid matrix) rows")
     ap.add_argument("--c9-only", action="store_true", help="only the C9 List.Uids rows with mutable layers")
     ap.add_argument("--c10-only", action="store_true", help="only the C10 unfiltered List.Uids and count rows")
+    ap.add_argument("--c11-only", action="store_true", help="only the C11 backup / restore codec rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -147,9 +148,11 @@ def main():
         rows = c9_rows(Lane())
     elif args.c10_only:
         rows = c10_rows(Lane())
+    elif args.c11_only:
+        rows = c11_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1045,6 +1048,174 @@ def c10_rows(L, threads: int = 16):
                 ):
                     out_rows.append(row(name, cfg, ms, exact + nmut, algo_bytes, ok,
                                         dict(extra, rows_per_s=nrows / (ms * 1e-3), note=note)))
+    finally:
+        for h in handles:
+            lib.dgx_dev_pack_free(h)
+        lib.dgx_cache_clear()
+    return out_rows
+
+
+def c11_rows(L, threads: int = 16):
+    """C11 "backup and restore": the C6 task's 10 000 packs (BlockSize 256) converted to BackupPostingList.uid_bytes
+    (codec.DecodeToBuffer per key) and those bytes back to packs (codec.EncodeFromBuffer(uid_bytes, 256) per key).
+    Legs on the same inputs, each checked row by row against the oracle's restatement (tests/backup_codec_oracle.c):
+    (1) the device form on resident inputs (CUDA events), (2) the host form with named packs (backup) / pinned bytes
+    (restore), (3) the host form with anonymous packs over PCIe (one run of images) / pageable bytes, (4) today's path:
+    the oracle per key on 1 and on `threads` host threads."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    import backup_codec_oracle as bco
+    import gen_rows
+    from backup_codec_cases import pack_images
+    from oracle import pyoracle as orc
+
+    lib = L.lib
+    _, rows_u, _ = gen_rows.c6_inputs()
+    nrows = len(rows_u)
+    ops = [orc.encode(r, 256) for r in rows_u]
+    exact = sum(r.size for r in rows_u)
+    del rows_u
+    pack_bytes = sum(int(op.deltas.size) + 12 * int(op.nblocks) for op in ops)
+
+    def p(a):
+        return a.ctypes.data_as(C.c_void_p)
+
+    def wall(fn, reps):
+        fn()
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            fn()
+        return (time.perf_counter() - t0) / reps * 1e3
+
+    def per_key(fn):
+        t0 = time.perf_counter()
+        got = [fn(i) for i in range(nrows)]
+        t1 = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        with ThreadPoolExecutor(max_workers=threads) as ex:  # ctypes releases the GIL
+            got_n = list(ex.map(fn, range(nrows)))
+        return got, t1 * 1e3, got_n, (time.perf_counter() - t0) * 1e3
+
+    # ---- backup: packs -> uid_bytes ----------------------------------------------------------------------------
+    want, t_b1, got_n, t_bn = per_key(lambda i: bco.decode_to_buffer(ops[i]))
+    ok_bn = got_n == want
+    want_off = np.zeros(nrows + 1, np.uint64)
+    np.cumsum([len(w) for w in want], out=want_off[1:])
+    want_all = np.frombuffer(b"".join(want), np.uint8)
+    nbytes = int(want_off[-1])
+
+    def same_bytes(out, off):
+        return bool(np.array_equal(off, want_off) and np.array_equal(out[:nbytes], want_all))
+
+    views = []
+    for op in ops:
+        arrs = (op.base, op.num_uids, op.delta_off, op.deltas)  # copies: they stay alive with the view
+        views.append((_lib.PackView(256, op.nblocks, *[a.ctypes.data for a in arrs]),) + arrs)
+    named = (_lib.PackRef * nrows)()
+    for i in range(nrows):
+        named[i].pack, named[i].key, named[i].version = C.pointer(views[i][0]), 1_100_000 + i, 1
+    img_in, img_in_off, img_in_nb, img_in_db = pack_images(ops)
+    anon_views = [_lib.PackView() for _ in range(nrows)]
+    anon = (_lib.PackRef * nrows)()
+    for i in range(nrows):
+        _lib.check(lib.dgx_pack_image_view(C.c_void_p(img_in.ctypes.data + int(img_in_off[i])), 256, int(img_in_nb[i]),
+                                           int(img_in_db[i]), C.byref(anon_views[i])))
+        anon[i].pack = C.pointer(anon_views[i])
+    handles = []
+    for pv in views:
+        h = C.c_void_p()
+        _lib.check(lib.dgx_dev_pack_upload(L.h, C.byref(pv[0]), C.byref(h)))
+        handles.append(h)
+    tab = (C.c_void_p * nrows)(*[h.value for h in handles])
+    d_out = torch.empty(nbytes + 16, dtype=torch.uint8, device=DEV)
+    d_off = torch.zeros(nrows + 1, dtype=torch.int64, device=DEV)
+    hout = np.empty(nbytes + 16, np.uint8)
+    hoff = np.zeros(nrows + 1, np.uint64)
+    lib.dgx_cache_clear()
+    _lib.check(lib.dgx_cache_configure(16 << 30))
+    out_rows = []
+    try:
+        def b_dev():
+            _lib.check(lib.dgx_dev_decode_to_buffer_rows(L.h, tab, nrows, C.c_void_p(d_out.data_ptr()), nbytes,
+                                                         C.c_void_p(d_off.data_ptr())))
+        ms_b_dev, _ = timeit(b_dev, warm=3, reps=10)
+        L.sync()
+        ok_b_dev = same_bytes(d_out.cpu().numpy(), d_off.cpu().numpy().view(np.uint64))
+        legs = [("Backup DecodeToBuffer rows (device, resident packs)", ms_b_dev, ok_b_dev,
+                 "dgx_dev_decode_to_buffer_rows, CUDA events")]
+        for name, refs, note in (("host, named packs, cache hits", named, "dgx_decode_to_buffer_rows, wall clock"),
+                                 ("host, anonymous packs over PCIe", anon,
+                                  "dgx_decode_to_buffer_rows, one run of pack images, wall clock")):
+            hout[:] = 0
+            ms = wall(lambda: _lib.check(lib.dgx_decode_to_buffer_rows(refs, nrows, p(hout), p(hoff), nbytes)), 5)
+            legs.append((f"Backup DecodeToBuffer rows ({name})", ms, same_bytes(hout, hoff), note))
+        legs += [("Backup today: oracle per key (1 thread)", t_b1, True, "restated in C, one key after another"),
+                 (f"Backup today: oracle per key ({threads} threads)", t_bn, ok_bn, "same, keys spread over threads")]
+        cfg = (f"C11 backup: the C6 task ({nrows} UidPacks, BlockSize 256, {exact} UIDs, {pack_bytes} pack bytes) "
+               f"to {nbytes} bytes of uvarint uid_bytes")
+        for name, ms, ok, note in legs:
+            out_rows.append(row(name, cfg, ms, exact, pack_bytes + nbytes,
+                                ok, {"rows": nrows, "rows_per_s": nrows / (ms * 1e-3), "out_bytes": nbytes,
+                                     "note": note, "bytes_note": "algorithmic bytes: pack bytes in + uid_bytes out"}))
+
+        # ---- restore: uid_bytes -> packs ---------------------------------------------------------------------
+        back, t_r1, back_n, t_rn = per_key(lambda i: bco.encode_from_buffer(want[i], 256))
+
+        def same_pack(rp, op):
+            rc, q = rp
+            return rc == 0 and all(np.array_equal(getattr(q, f), getattr(op, f))
+                                   for f in ("base", "num_uids", "delta_off", "deltas"))
+        ok_r1 = all(same_pack(b, op) for b, op in zip(back, ops))
+        ok_rn = all(same_pack(b, op) for b, op in zip(back_n, ops))
+        img_want, io_want, nb_want, db_want = pack_images([q for _, q in back])
+        itotal = int(io_want[-1])
+
+        def same_img(img, io, nb, db):
+            return bool(np.array_equal(io, io_want) and np.array_equal(nb, nb_want) and np.array_equal(db, db_want)
+                        and np.array_equal(img[:itotal], img_want[:itotal]))
+
+        buf_off = want_off.copy()
+        d_buf = torch.from_numpy(want_all.copy()).to(DEV)
+        d_img = torch.zeros(itotal + 16, dtype=torch.uint8, device=DEV)
+        d_io = torch.zeros(nrows + 1, dtype=torch.int64, device=DEV)
+        d_nb = torch.zeros(nrows, dtype=torch.int64, device=DEV)
+        d_db = torch.zeros(nrows, dtype=torch.int64, device=DEV)
+
+        def dp(t):
+            return C.c_void_p(t.data_ptr())
+
+        def r_dev():
+            _lib.check(lib.dgx_dev_encode_from_buffer_rows(L.h, dp(d_buf), p(buf_off), nrows, 256, dp(d_img), itotal,
+                                                           dp(d_io), dp(d_nb), dp(d_db)))
+        ms_r_dev, _ = timeit(r_dev, warm=3, reps=10)
+        L.sync()
+        ok_r_dev = same_img(d_img.cpu().numpy(), d_io.cpu().numpy().view(np.uint64), d_nb.cpu().numpy().view(np.uint64),
+                            d_db.cpu().numpy().view(np.uint64))
+        legs = [("Restore EncodeFromBuffer rows (device, resident bytes)", ms_r_dev, ok_r_dev,
+                 "dgx_dev_encode_from_buffer_rows, CUDA events")]
+        pin = lib.dgx_host_alloc(max(nbytes, 1))
+        try:
+            pinned = np.ctypeslib.as_array(C.cast(pin, C.POINTER(C.c_uint8)), shape=(max(nbytes, 1),))
+            pinned[:nbytes] = want_all
+            raw = np.zeros(itotal + 32, np.uint8)
+            himg = raw[(-raw.ctypes.data) % 16:][: itotal + 16]
+            hio, hnb, hdb = np.zeros(nrows + 1, np.uint64), np.zeros(nrows, np.uint64), np.zeros(nrows, np.uint64)
+            for name, src, note in (("host, pinned bytes", pinned, "dgx_encode_from_buffer_rows, wall clock"),
+                                    ("host, pageable bytes over PCIe", want_all,
+                                     "dgx_encode_from_buffer_rows, wall clock")):
+                himg[:] = 0
+                ms = wall(lambda: _lib.check(lib.dgx_encode_from_buffer_rows(p(src), p(buf_off), nrows, 256, p(himg),
+                                                                             itotal, p(hio), p(hnb), p(hdb))), 5)
+                legs.append((f"Restore EncodeFromBuffer rows ({name})", ms, same_img(himg, hio, hnb, hdb), note))
+        finally:
+            lib.dgx_host_free(pin)
+        legs += [("Restore today: oracle per key (1 thread)", t_r1, ok_r1, "restated in C, one key after another"),
+                 (f"Restore today: oracle per key ({threads} threads)", t_rn, ok_rn, "same, keys spread over threads")]
+        cfg = f"C11 restore: the {nbytes} uid_bytes of the C6 task's {nrows} keys back to {itotal} bytes of pack images"
+        for name, ms, ok, note in legs:
+            out_rows.append(row(name, cfg, ms, exact, nbytes + itotal,
+                                ok, {"rows": nrows, "rows_per_s": nrows / (ms * 1e-3), "image_bytes": itotal,
+                                     "note": note, "bytes_note": "algorithmic bytes: uid_bytes in + images out"}))
     finally:
         for h in handles:
             lib.dgx_dev_pack_free(h)
