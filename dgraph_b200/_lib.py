@@ -40,6 +40,12 @@ class PackRef(C.Structure):
     _fields_ = [("pack", C.POINTER(PackView)), ("key", C.c_uint64), ("version", C.c_uint64)]
 
 
+class QueryTree(C.Structure):
+    """dgx_query_tree (include/dgx.h): a cindex.Query tree as CSR arrays, node 0 the root."""
+    _fields_ = [("nnodes", C.c_size_t), ("op", C.c_void_p), ("leaf_off", C.c_void_p), ("leaf_idx", C.c_void_p),
+                ("sub_off", C.c_void_p), ("sub_idx", C.c_void_p)]
+
+
 class CacheStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("hits", "misses", "evictions", "bytes", "entries", "max_bytes")]
 
@@ -77,6 +83,7 @@ SYMBOLS = {
     "dgx_list_count_rows": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _vp, _u64, _vp]),
     "dgx_decode_to_buffer_rows": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _sz]),
     "dgx_encode_from_buffer_rows": (_int, [_vp, _vp, _sz, C.c_uint32, _vp, _sz, _vp, _vp, _vp]),
+    "dgx_trigram_query": (_int, [C.POINTER(QueryTree), C.POINTER(PackRef), _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _szp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
     "dgx_encode_bound": (None, [_sz, C.c_uint32, _szp, _szp]),
     "dgx_encode": (_int, [_vp, _sz, C.c_uint32, _vp, _vp, _vp, _vp, _szp, _szp, C.POINTER(PackView)]),
@@ -116,6 +123,7 @@ SYMBOLS = {
     "dgx_dev_list_uids_rows": (_int, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _u64, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_list_uids_unfiltered_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, C.c_int32, _vp, _sz, _vp]),
     "dgx_dev_list_count_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, _vp]),
+    "dgx_dev_trigram_query": (_int, [_vp, C.POINTER(QueryTree), _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),
     "dgx_filter_tail_queries": (_u64, [_vp]),
     "dgx_wire_posting_list_pack": (_int, [_vp, _sz, C.POINTER(_vp), _szp]),

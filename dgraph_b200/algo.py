@@ -278,6 +278,67 @@ def ListCountRows(packs, muts, afterUID: int, keys=None):
     return counts
 
 
+QAND, QOR = 2, 3  # cindex.Query ops of a trigram query node (include/dgx.h DGX_QAND / DGX_QOR)
+
+
+def query_tree(tree):
+    """A cindex.Query tree as the CSR arrays of dgx_query_tree: (tree struct, the arrays it points at).  tree[i] is
+    (op, leaf indices, sub-node indices); node 0 is the root."""
+    n = len(tree)
+    op = np.array([t[0] for t in tree] or [0], dtype=np.uint8)
+    leaf_off, sub_off = np.zeros(n + 1, np.uint32), np.zeros(n + 1, np.uint32)
+    np.cumsum([len(t[1]) for t in tree], out=leaf_off[1:])
+    np.cumsum([len(t[2]) for t in tree], out=sub_off[1:])
+    leaf_idx = np.array([i for t in tree for i in t[1]] or [0], dtype=np.uint32)
+    sub_idx = np.array([i for t in tree for i in t[2]] or [0], dtype=np.uint32)
+    arrays = (op, leaf_off, leaf_idx, sub_off, sub_idx)
+    return _lib.QueryTree(n, *[a.ctypes.data for a in arrays]), arrays
+
+
+def query_bound(tree, leaf_bounds) -> int:
+    """The root's bound of a trigram query (the out_cap dgx_trigram_query needs): a leaf's is ExactLen + |mut| or its
+    length, an AND's the minimum of its children's, an OR's their sum."""
+    b = [0] * len(tree)
+    for i in reversed(range(len(tree))):
+        op, leaves, subs = tree[i]
+        ch = [leaf_bounds[j] for j in leaves] + [b[s] for s in subs]
+        b[i] = min(ch) if op == QAND and ch else sum(ch)
+    return b[0] if tree else 0
+
+
+def UidsForRegex(tree, leaves, afterUID: int, keys=None) -> List:
+    """uidsForRegex(attr, arg, query, &pb.List{}) (worker/trigram.go:24-102) over a regexp()'s trigram query tree in ONE
+    call (dgx_trigram_query): every trigram's List.Uids read, the ANDs and ORs, on the device.
+
+    tree[i]: (op, leaf indices, sub-node indices) with op QAND / QOR; node 0 is the root, every other node has one
+    parent and a larger index.  leaves[j]: a pack leaf (pack, mut) -- pack None for an empty list or a delete-all
+    marker, mut None or (uids, flags), the resolved layer of REF postings as in ListUidsUnfilteredRows -- or a list leaf,
+    an ascending duplicate-free array (or pb.List) the caller decoded itself.  keys: optional [(key, version)] per leaf
+    naming the pack leaves for the HBM-resident cache.  Returns the root's uids."""
+    pack_ids = [j for j, lf in enumerate(leaves) if isinstance(lf, tuple)]
+    list_ids = [j for j, lf in enumerate(leaves) if not isinstance(lf, tuple)]
+    order = {j: k for k, j in enumerate(pack_ids + list_ids)}  # the ABI numbers pack leaves first
+    tr = [(op, [order[j] for j in ls], list(subs)) for op, ls, subs in tree]
+    packs = [leaves[j][0] for j in pack_ids]
+    mut_uids, mut_flags, mut_off = _mut_csr([leaves[j][1] for j in pack_ids])
+    arrs = []
+    for j in list_ids:
+        u = leaves[j].Uids if isinstance(leaves[j], List) else leaves[j]
+        arrs.append(np.zeros(0, np.uint64) if u is None else _u64(u))
+    list_off = np.zeros(len(arrs) + 1, dtype=np.uint64)
+    np.cumsum([a.size for a in arrs], out=list_off[1:])
+    lists = np.concatenate(arrs) if int(list_off[-1]) else np.zeros(1, np.uint64)
+    bounds = [(_exact(p) if p is not None else 0) + int(mut_off[k + 1] - mut_off[k]) for k, p in enumerate(packs)]
+    cap = query_bound(tr, bounds + [a.size for a in arrs])
+    refs, keep = _refs_of(packs, [keys[j] for j in pack_ids] if keys is not None else None)
+    qt, qa = query_tree(tr)
+    out = np.empty(max(cap, 1), dtype=np.uint64)
+    n = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_trigram_query(C.byref(qt), refs, len(packs), _p(mut_uids), _p(mut_flags), _p(mut_off),
+                                             _p(lists), _p(list_off), len(arrs), afterUID, _p(out), cap, C.byref(n)))
+    return List(out[: n.value])
+
+
 def IntersectCompressedWithMatrix(pack, rows, key=None):
     """algo.IntersectCompressedWith(pack, 0, rows[i], o_i) for every row i in ONE call
     (dgx_intersect_compressed_matrix): the intersectBucket loop (worker/sort.go:605-700) of one index bucket over a

@@ -38,6 +38,7 @@
 #include "list_uids_unfiltered_kernel.cuh"
 #include "encode_kernel.cuh"
 #include "backup_codec_kernel.cuh"
+#include "trigram_kernel.cuh"
 #include "wire.hpp"
 
 using namespace dgx;
@@ -3480,6 +3481,293 @@ extern "C" int dgx_merge_sorted_matrix(const uint64_t* v, const uint64_t* v_off,
     rc = merge_matrix_impl(l, d_v, d_off, nrows, m, (uint64_t*)d_out, m, (uint64_t*)d_len);
     if (rc) return rc;
     return finish_to_host(l, (uint64_t*)d_len, (uint64_t*)d_out, m, out, out_cap, out_len);
+}
+
+// ---------------------------------------------------------------------------
+// uidsForRegex: a regexp()'s trigram query tree in one call (trigram_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr size_t kTgMaxNodes = size_t(1) << 16, kTgMaxLeaves = size_t(1) << 16, kTgMaxRefs = size_t(1) << 20;
+constexpr uint32_t kTgMaxDepth = 32;
+
+// The host plan, from bounds only: the pre-order program, the root's distinct driving leaves and the sum of their
+// bounds (dcap, the room of every per-candidate buffer), and whether every node is an OR.
+struct TgPlan {
+    std::vector<TgOp> prog;
+    std::vector<uint32_t> drive;
+    uint64_t root_bound = 0, dcap = 0;
+    bool all_or = true;
+};
+
+struct TgBuild {
+    const dgx_query_tree* t;
+    const uint64_t* lb;  // leaf bounds
+    std::vector<uint64_t> bound;
+    std::vector<char> seen;
+    TgPlan* P;
+
+    // A node's children as (bound, leaf index or kTgNode | node): its leaves, then its subs, in the given order; an
+    // AND's sorted by bound (stably), so that its first child is the smallest, the one that drives it.
+    std::vector<std::pair<uint64_t, uint32_t>> children(uint32_t i) const {
+        std::vector<std::pair<uint64_t, uint32_t>> ch;
+        for (uint32_t k = t->leaf_off[i]; k < t->leaf_off[i + 1]; ++k) ch.push_back({lb[t->leaf_idx[k]], t->leaf_idx[k]});
+        for (uint32_t k = t->sub_off[i]; k < t->sub_off[i + 1]; ++k) ch.push_back({bound[t->sub_idx[k]], kTgNode | t->sub_idx[k]});
+        if (t->op[i] == DGX_QAND)
+            std::stable_sort(ch.begin(), ch.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+        return ch;
+    }
+    void emit(uint32_t i, uint32_t parent) {
+        const uint32_t at = (uint32_t)P->prog.size();
+        P->prog.push_back(TgOp{0, parent});
+        for (const auto& c : children(i)) {
+            if (c.second & kTgNode) emit(c.second & ~kTgNode, at);
+            else P->prog.push_back(TgOp{c.second, 0});
+        }
+        P->prog[at].w0 = kTgNode | (t->op[i] == DGX_QAND ? kTgAnd : 0u) | (uint32_t)P->prog.size();
+    }
+    void drive(uint32_t i) {
+        const auto ch = children(i);
+        const size_t n = t->op[i] == DGX_QAND ? 1 : ch.size();
+        for (size_t k = 0; k < n; ++k) {
+            const uint32_t c = ch[k].second;
+            if (c & kTgNode) drive(c & ~kTgNode);
+            else if (!seen[c]) {
+                seen[c] = 1;
+                P->drive.push_back(c);
+                P->dcap += lb[c];
+            }
+        }
+    }
+};
+
+// The tree's checks and the plan, before anything is copied.  lb[i]: leaf i's bound.
+static int tg_plan(const dgx_query_tree* t, const uint64_t* lb, size_t nleaves, TgPlan* P) {
+    if (!t) return fail(DGX_ERR_ARG, "null tree");
+    const size_t nn = t->nnodes;
+    if (nn == 0 || nn >= kTgMaxNodes) return fail(DGX_ERR_ARG, "%zu nodes: between 1 and 2^16 - 1", nn);
+    if (!t->op || !t->leaf_off || !t->sub_off) return fail(DGX_ERR_ARG, "null tree array");
+    if (t->leaf_off[0] != 0 || t->sub_off[0] != 0) return fail(DGX_ERR_ARG, "leaf_off[0] and sub_off[0] must be 0");
+    for (size_t i = 0; i < nn; ++i)
+        if (t->leaf_off[i + 1] < t->leaf_off[i] || t->sub_off[i + 1] < t->sub_off[i])
+            return fail(DGX_ERR_ARG, "the offsets of node %zu decrease", i);
+    if (t->leaf_off[nn] >= kTgMaxRefs) return fail(DGX_ERR_ARG, "%u leaf references: at most 2^20 - 1", t->leaf_off[nn]);
+    if ((t->leaf_off[nn] && !t->leaf_idx) || (t->sub_off[nn] && !t->sub_idx)) return fail(DGX_ERR_ARG, "null tree array");
+    std::vector<uint32_t> parent(nn, kTgNoParent), depth(nn, 1);
+    for (size_t i = 0; i < nn; ++i) {
+        const unsigned op = t->op[i];
+        if (op != DGX_QAND && op != DGX_QOR) return fail(DGX_ERR_ARG, "node %zu has op %u: not QAnd or QOr", i, op);
+        if (op == DGX_QAND && t->leaf_off[i + 1] == t->leaf_off[i] && t->sub_off[i + 1] == t->sub_off[i])
+            return fail(DGX_ERR_ARG, "AND node %zu has no trigram and no sub", i);
+        if (i > 0 && parent[i] == kTgNoParent) return fail(DGX_ERR_ARG, "node %zu has no parent", i);
+        for (uint32_t k = t->leaf_off[i]; k < t->leaf_off[i + 1]; ++k)
+            if (t->leaf_idx[k] >= nleaves) return fail(DGX_ERR_ARG, "node %zu names leaf %u of %zu", i, t->leaf_idx[k], nleaves);
+        for (uint32_t k = t->sub_off[i]; k < t->sub_off[i + 1]; ++k) {
+            const uint32_t s = t->sub_idx[k];
+            if (s <= i || s >= nn) return fail(DGX_ERR_ARG, "node %zu names sub %u: subs follow their parent", i, s);
+            if (parent[s] != kTgNoParent) return fail(DGX_ERR_ARG, "node %u has two parents", s);
+            parent[s] = (uint32_t)i;
+            depth[s] = depth[i] + 1;
+            if (depth[s] > kTgMaxDepth) return fail(DGX_ERR_ARG, "node %u is deeper than %u", s, kTgMaxDepth);
+        }
+    }
+    TgBuild B{t, lb, std::vector<uint64_t>(nn), std::vector<char>(nleaves, 0), P};
+    for (size_t i = nn; i-- > 0;) {  // children have larger indices
+        const bool is_and = t->op[i] == DGX_QAND;
+        uint64_t b = is_and ? ~uint64_t(0) : 0;
+        for (const auto& c : B.children((uint32_t)i)) b = is_and ? std::min(b, c.first) : b + c.first;
+        B.bound[i] = b;
+        if (is_and) P->all_or = false;
+    }
+    P->root_bound = B.bound[0];
+    if (P->root_bound == 0) return DGX_OK;
+    B.emit(0, kTgNoParent);
+    B.drive(0);
+    return DGX_OK;
+}
+
+// The leaves' checks (the layers as for dgx_list_uids_unfiltered_rows, the list offsets, the sum of bounds), then the
+// tree's.  rows[i] is pack leaf i.
+template <class Row>
+static int tg_check(const dgx_query_tree* tree, const Row* rows, size_t npacks, const uint64_t* mut_off,
+                    const void* mut_uids, const void* mut_flags, const uint64_t* list_off, size_t nlists, TgPlan* P) {
+    const size_t nleaves = npacks + nlists;
+    if (nleaves >= kTgMaxLeaves) return fail(DGX_ERR_ARG, "%zu leaves: at most 2^16 - 1", nleaves);
+    if ((npacks && (!rows || !mut_off)) || (nlists && !list_off)) return fail(DGX_ERR_ARG, "null argument");
+    if (npacks)
+        if (int rc = list_unfiltered_check(npacks, mut_off, mut_uids, mut_flags, rows)) return rc;
+    if (nlists)
+        if (int rc = check_offsets("list_off", list_off, nlists, uint64_t(1) << 32)) return rc;
+    std::vector<uint64_t> lb(nleaves);
+    uint64_t sum = 0;
+    for (size_t i = 0; i < npacks; ++i) sum += lb[i] = exact_len(rows[i]) + (mut_off[i + 1] - mut_off[i]);
+    for (size_t j = 0; j < nlists; ++j) sum += lb[npacks + j] = list_off[j + 1] - list_off[j];
+    if (sum >> 32) return fail(DGX_ERR_ARG, "the leaves' bounds total %llu: at most 2^32 - 1", (unsigned long long)sum);
+    return tg_plan(tree, lb.data(), nleaves, P);
+}
+
+// The pipeline of trigram_kernel.cuh for a plan of root bound > 0.  Launches: the unfiltered rows call's 5 when there
+// are pack leaves; tg_leaves and tg_gather; merge_matrix_impl's when two or more leaves drive; tg_eval and
+// compact_kernel unless every node is an OR.  Workspace: the pack leaves' rows (8 bytes per bound uid plus the rows
+// call's 24 per mutable entry and 24 per leaf), the driving rows gathered (8 per dcap), the merge's about 22 per dcap,
+// the candidates (8 per dcap) and keep (1 per dcap).  mut_off and list_off are host memory, already checked.
+static int trigram_impl(dgx_lane* l, const TgPlan& T, const dgx_dev_pack* const* packs, size_t npacks,
+                        const uint64_t* d_mut, const uint8_t* d_flags, const uint64_t* mut_off, const uint64_t* d_lists,
+                        const uint64_t* list_off, size_t nlists, uint64_t after, uint64_t* d_out, size_t out_cap,
+                        uint64_t* d_out_len) {
+    const size_t nleaves = npacks + nlists, nd = T.drive.size();
+    const uint64_t dcap = T.dcap;
+    uint64_t rows_cap = 0;
+    for (size_t i = 0; i < npacks; ++i) rows_cap += exact_len(packs[i]) + (mut_off[i + 1] - mut_off[i]);
+    // table (copied): [prog | drive | list_off];  then leaf, drive_off, row_off, rows
+    const size_t b_prog = (T.prog.size() * sizeof(TgOp) + 15) & ~size_t(15);
+    const size_t b_drive = (nd * sizeof(uint32_t) + 15) & ~size_t(15);
+    const size_t b_tab = b_prog + b_drive + (nlists + 1) * sizeof(uint64_t);
+    void *h_raw, *d_raw;
+    int rc = l->host.alloc(b_tab, &h_raw);
+    if (rc) return rc;
+    memcpy(h_raw, T.prog.data(), T.prog.size() * sizeof(TgOp));
+    memcpy((char*)h_raw + b_prog, T.drive.data(), nd * sizeof(uint32_t));
+    uint64_t* h_loff = (uint64_t*)((char*)h_raw + b_prog + b_drive);
+    if (nlists) memcpy(h_loff, list_off, (nlists + 1) * sizeof(uint64_t));
+    else h_loff[0] = 0;
+    const size_t b_rest = nleaves * sizeof(TgLeaf) + (nd + 1 + npacks + 1 + rows_cap + 2) * sizeof(uint64_t);
+    if ((rc = l->ws.alloc(b_tab + b_rest, &d_raw))) return rc;
+    char* d = (char*)d_raw;
+    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += b_tab;
+    TgParams P;
+    P.prog = (const TgOp*)d;
+    P.drive = (const u32*)(d + b_prog);
+    P.list_off = (const u64*)(d + b_prog + b_drive);
+    P.leaf = (TgLeaf*)(d + b_tab);
+    P.drive_off = (u64*)(P.leaf + nleaves);
+    u64* row_off = P.drive_off + nd + 1;
+    u64* rows = row_off + npacks + 1;
+    P.npacks = (u32)npacks;
+    P.nleaves = (u32)nleaves;
+    P.rows = rows;
+    P.row_off = row_off;
+    P.lists = (const u64*)d_lists;
+    P.flags = d_flags;
+    P.nmut = npacks ? mut_off[npacks] : 0;
+    P.ndrive = (u32)nd;
+    P.dcap = dcap;
+    P.err = l->d_err;
+    if (npacks && (rc = list_unfiltered_impl(l, packs, npacks, d_mut, d_flags, mut_off, after, first_keep(0),
+                                             (uint64_t*)rows, rows_cap, (uint64_t*)row_off, nullptr)))
+        return rc;
+    const bool merge = nd >= 2;
+    const bool gather_is_result = T.all_or && !merge;
+    void* p;
+    if (gather_is_result) P.gathered = (u64*)d_out;
+    else if ((rc = l->ws.alloc((dcap + 2) * sizeof(uint64_t), &p))) return rc;
+    else P.gathered = (u64*)p;
+    P.len_word = gather_is_result ? (u64*)d_out_len : nullptr;
+    const unsigned g_val = (unsigned)((dcap + 255) / 256);
+    tg_leaves_kernel<<<1, TG_NT, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    tg_gather_kernel<<<g_val, 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 2);
+    P.cand = P.gathered;
+    P.ncand = P.drive_off + nd;
+    if (merge) {
+        uint64_t *m_out = d_out, *m_len = d_out_len;
+        if (!T.all_or) {
+            if ((rc = l->ws.alloc((dcap + 2 + 8) * sizeof(uint64_t), &p))) return rc;
+            m_len = (uint64_t*)p;
+            m_out = m_len + 8;
+        }
+        rc = merge_matrix_impl(l, (const uint64_t*)P.gathered, (const uint64_t*)P.drive_off, nd, dcap, m_out,
+                               T.all_or ? out_cap : dcap, m_len);
+        if (rc) return rc;
+        P.cand = (const u64*)m_out;
+        P.ncand = (const u64*)m_len;
+    }
+    if (!T.all_or) {
+        const uint64_t tiles = (dcap + CP_TILE - 1) / CP_TILE;
+        const size_t b_keep = (dcap + 15) & ~size_t(15), b_stat = tiles * sizeof(u64) + 64;
+        if ((rc = l->ws.alloc(b_keep + b_stat, &p))) return rc;
+        CK(cudaMemsetAsync((char*)p + b_keep, 0, b_stat, l->stream));
+        P.keep = (unsigned char*)p;
+        tg_eval_kernel<<<g_val, 256, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        CompactParams C;
+        C.v = P.cand;
+        C.keep = P.keep;
+        C.m = dcap;
+        C.out = (u64*)d_out;
+        C.out_cap = out_cap;
+        C.out_len = (u64*)d_out_len;
+        C.status = (u64*)((char*)p + b_keep);
+        C.ticket = (u32*)(C.status + tiles);
+        C.err = l->d_err;
+        compact_kernel<<<(unsigned)tiles, CP_NT, 0, l->stream>>>(C);
+        CK(cudaGetLastError());
+        count_launches(l, 2);
+    }
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_trigram_query(dgx_lane* l, const dgx_query_tree* tree, const dgx_dev_pack* const* packs,
+                                     size_t npacks, const uint64_t* d_mut_uids, const uint8_t* d_mut_flags,
+                                     const uint64_t* mut_off, const uint64_t* d_lists, const uint64_t* list_off,
+                                     size_t nlists, uint64_t after_uid, uint64_t* d_out, size_t out_cap,
+                                     uint64_t* d_out_len) {
+    if (!l || !d_out_len) return fail(DGX_ERR_ARG, "null argument");
+    TgPlan T;
+    if (int rc = tg_check(tree, packs, npacks, mut_off, d_mut_uids, d_mut_flags, list_off, nlists, &T)) return rc;
+    if (T.root_bound && (!d_out || (nlists && list_off[nlists] && !d_lists))) return fail(DGX_ERR_ARG, "null argument");
+    if (out_cap < T.root_bound)
+        return fail(DGX_ERR_CAP, "out_cap (%zu) is below the root's bound (%llu)", out_cap,
+                    (unsigned long long)T.root_bound);
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    if (T.root_bound == 0) {
+        CK(cudaMemsetAsync(d_out_len, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    const int rc = trigram_impl(l, T, packs, npacks, d_mut_uids, d_mut_flags, mut_off, d_lists, list_off, nlists,
+                                after_uid, d_out, out_cap, d_out_len);
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_len, sizeof(uint64_t));
+    return rc;
+}
+
+extern "C" int dgx_trigram_query(const dgx_query_tree* tree, const dgx_pack_ref* refs, size_t npacks,
+                                 const uint64_t* mut_uids, const uint8_t* mut_flags, const uint64_t* mut_off,
+                                 const uint64_t* lists, const uint64_t* list_off, size_t nlists, uint64_t after_uid,
+                                 uint64_t* out, size_t out_cap, size_t* out_len) {
+    if (!out_len) return fail(DGX_ERR_ARG, "null out_len");
+    TgPlan T;
+    if (int rc = tg_check(tree, refs, npacks, mut_off, mut_uids, mut_flags, list_off, nlists, &T)) return rc;
+    const uint64_t nmut = npacks ? mut_off[npacks] : 0, nlist = nlists ? list_off[nlists] : 0;
+    for (uint64_t k = 0; k < nmut; ++k)
+        if (mut_flags[k] & DGX_MUT_VALUE)
+            return fail(DGX_ERR_ARG, "mutable entry %llu is not a REF posting", (unsigned long long)k);
+    if (T.root_bound && (!out || (nlist && !lists))) return fail(DGX_ERR_ARG, "null argument");
+    if (out_cap < T.root_bound)
+        return fail(DGX_ERR_CAP, "out_cap (%zu) is below the root's bound (%llu)", out_cap,
+                    (unsigned long long)T.root_bound);
+    if (T.root_bound == 0) { *out_len = 0; return DGX_OK; }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    PackSet ps(l, refs, npacks);  // nil / empty packs are packs of no blocks
+    if (ps.rc) return ps.rc;
+    const std::vector<const dgx_dev_pack*> rows = ps.rows();
+    uint64_t *d_mut = nullptr, *d_lists;
+    const uint8_t* d_flags = nullptr;
+    int rc;
+    if (npacks && (rc = upload_mut_layers(l, mut_uids, mut_flags, nmut, &d_mut, &d_flags))) return rc;
+    if ((rc = upload_list(l, lists, nlist, &d_lists))) return rc;  // the list leaves: one copy
+    void* p;
+    if ((rc = l->ws.alloc((T.dcap + 10) * sizeof(uint64_t), &p))) return rc;  // the length word, then the values
+    uint64_t* d_out = (uint64_t*)p;
+    rc = trigram_impl(l, T, rows.data(), npacks, d_mut, d_flags, mut_off, d_lists, list_off, nlists, after_uid,
+                      d_out + 8, T.dcap, d_out);
+    if (rc) return rc;
+    return ps.synced(finish_to_host(l, d_out, d_out + 8, T.dcap, out, out_cap, out_len));
 }
 
 extern "C" uint64_t dgx_merge_matrix_overflows(const dgx_lane* l) { return l ? l->xm_overflows : g_xm_overflows.load(); }

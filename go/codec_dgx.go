@@ -19,6 +19,8 @@ import (
 	"math"
 	"unsafe"
 
+	cindex "github.com/google/codesearch/index"
+
 	"github.com/dgraph-io/dgraph/v25/protos/pb"
 )
 
@@ -531,9 +533,10 @@ type unfilteredStage struct {
 	free  func()
 }
 
-// stageUnfiltered stages a task's keys for dgx_list_uids_unfiltered_rows / dgx_list_count_rows.  It returns false
-// when the batch is too small to pay for a call or the input is malformed.
-func stageUnfiltered(refs []PackRef, muts []MutRow) (*unfilteredStage, bool) {
+// stageUnfiltered stages a task's keys for dgx_list_uids_unfiltered_rows / dgx_list_count_rows / dgx_trigram_query.
+// It returns false when the packs' ApproxLen plus the pending entries stay below minUids (too small to pay for a call)
+// or the input is malformed.
+func stageUnfiltered(refs []PackRef, muts []MutRow, minUids int) (*unfilteredStage, bool) {
 	n := len(refs)
 	if len(muts) != n {
 		return nil, false
@@ -554,7 +557,7 @@ func stageUnfiltered(refs []PackRef, muts []MutRow) (*unfilteredStage, bool) {
 			}
 		}
 	}
-	if total+nmut < dgxMinDecode || nmut >= 1<<31 {
+	if total+nmut < minUids || nmut >= 1<<31 {
 		return nil, false
 	}
 	csr := C.malloc(C.size_t((n+2+nmut)*8 + nmut + 16))
@@ -619,7 +622,7 @@ func ListUidsUnfilteredRows(refs []PackRef, muts []MutRow, afterUID uint64, firs
 	if n == 0 {
 		return []*pb.List{}, true
 	}
-	s, ok := stageUnfiltered(refs, muts)
+	s, ok := stageUnfiltered(refs, muts, dgxMinDecode)
 	if !ok {
 		return nil, false
 	}
@@ -662,7 +665,7 @@ func ListCountRows(refs []PackRef, muts []MutRow, afterUID uint64) ([]uint32, bo
 	if n == 0 {
 		return []uint32{}, true
 	}
-	s, ok := stageUnfiltered(refs, muts)
+	s, ok := stageUnfiltered(refs, muts, dgxMinDecode)
 	if !ok {
 		return nil, false
 	}
@@ -805,4 +808,206 @@ func EncodeFromBufferRows(bufs [][]byte, blockSize int) ([]*pb.UidPack, bool) {
 		packs[i] = p
 	}
 	return packs, true
+}
+
+// TrigramLeaf is one trigram's index posting list as UidsForRegex needs it, read by the caller (INTEGRATION §2): an
+// unsplit list as a pack leaf (Ref named (hash(index key), minTs), Mut its resolved layer of REF postings), or, for a
+// split list or one where canUseCalculatedUids holds, a list leaf (IsList, List = pl.Uids without Intersect or
+// calculatedUids).  OK false: the caller must keep uidsForRegex for the query (a read error, ReadTs < minTs, non-REF
+// postings, findPosting and pickPostings resolutions that disagree).
+type TrigramLeaf struct {
+	Ref    PackRef
+	Mut    MutRow
+	IsList bool
+	List   []uint64
+	OK     bool
+}
+
+// dgxMinTrigram: below this many leaf uids (packs' ExactLen + pending entries + list lengths, the whole tree)
+// UidsForRegex stays on the Go path.  Set from the C12 record (profiles/h100_c12_trigram_query.json, H100 80GB HBM3,
+// 700 W): the host form with named packs took 0.24-0.46 ms per tree with a small result, and the oracle's restatement
+// 8-16 ns per leaf uid, so about 16 000 to 30 000 leaf uids cost the Go walk what one library call costs.
+const dgxMinTrigram = 1 << 14
+
+// UidsForRegex is uidsForRegex(attr, arg, query, &pb.List{}) (worker/trigram.go:24-102) in ONE library call: every
+// trigram's posting list read, the ANDs and ORs, on the device.  read(t) is called once per distinct trigram of the
+// tree, as the query holds it before tok.EncodeRegexTokens (the caller encodes it to build the index key, as
+// uidsForTrigram does).  first is arg.q.First.  Returns false when the caller must keep uidsForRegex: a QAll / QNone
+// node or an AND with nothing under it, First other than 0 or MaxInt32, any leaf the caller could not read as the
+// library needs it (the Go path reads only what its early exits reach, so an error must not surface where it would
+// not), a batch below dgxMinTrigram, and any library error.
+func UidsForRegex(query *cindex.Query, read func(trigram string) TrigramLeaf, afterUID uint64, first int) (*pb.List, bool) {
+	if first != 0 && first != math.MaxInt32 {
+		return nil, false
+	}
+	var ops []uint8
+	var perNode []nodeLists
+	index := map[string]uint32{}
+	var tris []string
+	// pre-order numbering: every sub gets an index above its parent's
+	var walk func(q *cindex.Query) (uint32, bool)
+	walk = func(q *cindex.Query) (uint32, bool) {
+		if q.Op != cindex.QAnd && q.Op != cindex.QOr || (q.Op == cindex.QAnd && len(q.Trigram) == 0 && len(q.Sub) == 0) {
+			return 0, false
+		}
+		i := uint32(len(ops))
+		ops = append(ops, uint8(q.Op))
+		perNode = append(perNode, nodeLists{})
+		for _, t := range q.Trigram {
+			j, seen := index[t]
+			if !seen {
+				j = uint32(len(tris))
+				index[t] = j
+				tris = append(tris, t)
+			}
+			perNode[i].leaves = append(perNode[i].leaves, j)
+		}
+		for _, sq := range q.Sub {
+			c, ok := walk(sq)
+			if !ok {
+				return 0, false
+			}
+			perNode[i].subs = append(perNode[i].subs, c)
+		}
+		return i, true
+	}
+	if _, ok := walk(query); !ok {
+		return nil, false
+	}
+	n := len(ops)
+	leafOff, subOff := make([]uint32, 1, n+1), make([]uint32, 1, n+1)
+	var leafIdx, subIdx []uint32
+	for i := 0; i < n; i++ {
+		leafIdx = append(leafIdx, perNode[i].leaves...)
+		subIdx = append(subIdx, perNode[i].subs...)
+		leafOff = append(leafOff, uint32(len(leafIdx)))
+		subOff = append(subOff, uint32(len(subIdx)))
+	}
+	// read every leaf up front: pack leaves first, as the library numbers them
+	leaves := make([]TrigramLeaf, len(tris))
+	var refs []PackRef
+	var muts []MutRow
+	var lists []uint64
+	listOff := []uint64{0}
+	order := make([]uint32, len(tris))
+	total := 0
+	for j, t := range tris {
+		if leaves[j] = read(t); !leaves[j].OK {
+			return nil, false
+		}
+		if !leaves[j].IsList {
+			order[j] = uint32(len(refs))
+			refs = append(refs, leaves[j].Ref)
+			muts = append(muts, leaves[j].Mut)
+		}
+	}
+	for j := range tris {
+		if leaves[j].IsList {
+			order[j] = uint32(len(refs) + len(listOff) - 1)
+			lists = append(lists, leaves[j].List...)
+			listOff = append(listOff, uint64(len(lists)))
+			total += len(leaves[j].List)
+		}
+	}
+	for k := range leafIdx {
+		leafIdx[k] = order[leafIdx[k]]
+	}
+	for _, m := range muts {
+		for _, f := range m.Flags {
+			if f&C.DGX_MUT_VALUE != 0 {
+				return nil, false
+			}
+		}
+	}
+	// the whole tree is held to dgxMinTrigram below, not the pack leaves alone to dgxMinDecode
+	var s *unfilteredStage
+	if len(refs) > 0 {
+		var ok bool
+		if s, ok = stageUnfiltered(refs, muts, 0); !ok {
+			return nil, false
+		}
+		defer s.free()
+		for _, e := range s.exact {
+			total += e
+		}
+	}
+	if total < dgxMinTrigram || uint64(total) >= 1<<32 {
+		return nil, false
+	}
+	// the root's bound: an AND's is the minimum of its children's, an OR's their sum
+	bound := make([]int, len(tris))
+	for j := range tris {
+		if leaves[j].IsList {
+			bound[j] = len(leaves[j].List)
+		} else {
+			bound[j] = s.exact[order[j]]
+		}
+	}
+	nb := make([]int, n)
+	for i := n - 1; i >= 0; i-- {
+		b, and := 0, ops[i] == uint8(cindex.QAnd)
+		if and {
+			b = math.MaxInt
+		}
+		for _, j := range perNode[i].leaves {
+			if and {
+				b = min(b, bound[j])
+			} else {
+				b += bound[j]
+			}
+		}
+		for _, c := range perNode[i].subs {
+			if and {
+				b = min(b, nb[c])
+			} else {
+				b += nb[c]
+			}
+		}
+		nb[i] = b
+	}
+	// every array the call reads gets its own C allocation, sized from the slice it holds
+	frees := []func(){}
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+	}()
+	carr := func(p unsafe.Pointer, free func()) unsafe.Pointer {
+		frees = append(frees, free)
+		return p
+	}
+	ctree := (*C.dgx_query_tree)(carr(cArray([]C.dgx_query_tree{{nnodes: C.size_t(n)}})))
+	ctree.op = (*C.uint8_t)(carr(cArray(ops)))
+	ctree.leaf_off = (*C.uint32_t)(carr(cArray(leafOff)))
+	ctree.leaf_idx = (*C.uint32_t)(carr(cArray(leafIdx)))
+	ctree.sub_off = (*C.uint32_t)(carr(cArray(subOff)))
+	ctree.sub_idx = (*C.uint32_t)(carr(cArray(subIdx)))
+	cLists := (*C.uint64_t)(carr(cArray(lists)))
+	cListOff := (*C.uint64_t)(carr(cArray(listOff)))
+	out := make([]uint64, nb[0]+1)
+	var outLen C.size_t
+	var crefs *C.dgx_pack_ref
+	var mutUids, mutOff *C.uint64_t
+	var mutFlags *C.uint8_t
+	if s != nil {
+		crefs, mutUids, mutFlags, mutOff = s.crefs, s.uids, s.flags, s.off
+	}
+	if C.dgx_trigram_query(ctree, crefs, C.size_t(len(refs)), mutUids, mutFlags, mutOff, cLists, cListOff,
+		C.size_t(len(listOff)-1), C.uint64_t(afterUID), (*C.uint64_t)(unsafe.Pointer(&out[0])), C.size_t(nb[0]),
+		&outLen) != C.DGX_OK {
+		return nil, false
+	}
+	return &pb.List{Uids: out[:outLen:outLen]}, true
+}
+
+// nodeLists: a query node's leaf indices and sub-node indices while UidsForRegex flattens the tree.
+type nodeLists struct{ leaves, subs []uint32 }
+
+// cArray copies v into a C allocation of max(len(v), 1) elements (an empty array still has an address) and returns it
+// with the function that frees it.
+func cArray[T any](v []T) (unsafe.Pointer, func()) {
+	var zero T
+	p := C.malloc(C.size_t(int(unsafe.Sizeof(zero)) * max(len(v), 1)))
+	copy(unsafe.Slice((*T)(p), len(v)), v)
+	return p, func() { C.free(p) }
 }

@@ -330,6 +330,41 @@ int dgx_encode_from_buffer_rows(const uint8_t* buf, const uint64_t* buf_off, siz
 int dgx_merge_sorted_matrix(const uint64_t* v, const uint64_t* v_off, size_t nrows,
                             uint64_t* out, size_t out_cap, size_t* out_len);
 
+/* uidsForRegex(attr, arg, query, &pb.List{}) (worker/trigram.go:24-102): the cindex.Query tree of a regexp() over a
+ * trigram index, every trigram's posting list read with List.Uids, evaluated in one call.  Node 0 is the root; node i
+ * has op[i] (DGX_QAND or DGX_QOR, cindex's values), the leaves leaf_idx[leaf_off[i] .. leaf_off[i+1]) (its trigrams) and
+ * the sub-nodes sub_idx[sub_off[i] .. sub_off[i+1]).  Every node but the root has exactly one parent and a larger index
+ * than it; two nodes may name the same leaf. */
+enum { DGX_QAND = 2, DGX_QOR = 3 };
+typedef struct dgx_query_tree {
+    size_t nnodes;
+    const uint8_t* op;         /* nnodes */
+    const uint32_t* leaf_off;  /* nnodes + 1, leaf_off[0] == 0 */
+    const uint32_t* leaf_idx;  /* leaf_off[nnodes] */
+    const uint32_t* sub_off;   /* nnodes + 1, sub_off[0] == 0 */
+    const uint32_t* sub_idx;   /* sub_off[nnodes] */
+} dgx_query_tree;
+/* Leaves 0 .. npacks-1 are PACK leaves: refs[i] (NULL pack: empty list or delete-all marker) with its resolved layer
+ * mut_uids / mut_flags[mut_off[i] .. mut_off[i+1]), exactly as row i of dgx_list_uids_unfiltered_rows; the layers hold
+ * REF postings only (no DGX_MUT_VALUE).  Leaves npacks .. npacks+nlists-1 are LIST leaves: list j is
+ * lists[list_off[j] .. list_off[j+1]) (host offsets, list_off[0] == 0), ascending and duplicate-free, a list the caller
+ * decoded itself (a split list's pl.Uids, calculatedUids), which is above after_uid as such a read is.  With S_i the
+ * unfiltered List.Uids row of pack leaf i from after_uid (First = MaxInt32) and the list itself for a list leaf, the
+ * result is f(root) with f(leaf) = S_leaf, f(AND) = the intersection of its leaves and subs, f(OR) = their union: what
+ * uidsForRegex returns whichever List.Uids branch each filtered read takes (DESIGN section 5).  *out_len values are
+ * written, ascending.
+ * Bounds: a pack leaf's is ExactLen + |mut|, a list leaf's its length; an AND's the minimum of its children's, an OR's
+ * their sum.  out_cap < the root's bound is DGX_ERR_CAP before anything is copied; a root bound of 0 gives *out_len = 0
+ * and needs no device.  DGX_ERR_ARG before anything is copied: nnodes == 0 or >= 2^16, npacks + nlists >= 2^16,
+ * leaf_off[nnodes] >= 2^20, an op that is not DGX_QAND / DGX_QOR, an AND with no leaf and no sub (codesearch makes that
+ * QAll), a node with a second parent, a sub index not above its parent's or past nnodes, a node deeper than 32 (the root
+ * is depth 1), a leaf index past the leaves, a sum of leaf bounds of 2^32 or more, list_off not starting at 0 or
+ * decreasing, a DGX_MUT_VALUE flag, the layer errors of dgx_list_uids_unfiltered_rows, a null array that is needed.
+ * The kernel launches depend only on the plan's case: see DESIGN section 3.8. */
+int dgx_trigram_query(const dgx_query_tree* tree, const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids,
+                      const uint8_t* mut_flags, const uint64_t* mut_off, const uint64_t* lists, const uint64_t* list_off,
+                      size_t nlists, uint64_t after_uid, uint64_t* out, size_t out_cap, size_t* out_len);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -522,6 +557,15 @@ int dgx_dev_encode_from_buffer_rows(dgx_lane* lane, const uint8_t* d_buf, const 
  * when d_v_off[nrows] > v_cap; a row that descends makes the next dgx_lane_sync return DGX_ERR_ARG. */
 int dgx_dev_merge_sorted_matrix(dgx_lane* lane, const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows,
                                 size_t v_cap, uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
+/* Device form of dgx_trigram_query: packs resident (dgx_dev_pack_upload; NULL = empty pack or delete-all marker),
+ * d_mut_uids / d_mut_flags / d_lists / d_out device pointers, d_out_len one device uint64; tree, mut_off and list_off in
+ * HOST memory, checked as in the host form before anything is queued (the DGX_MUT_VALUE check runs on the device: such
+ * a flag leaves d_out untouched, writes d_out_len = 0 and makes the next dgx_lane_sync return DGX_ERR_ARG, as a malformed
+ * layer does).  Asynchronous on the lane; nothing waits on the host between the stages. */
+int dgx_dev_trigram_query(dgx_lane* lane, const dgx_query_tree* tree, const dgx_dev_pack* const* packs, size_t npacks,
+                          const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
+                          const uint64_t* d_lists, const uint64_t* list_off, size_t nlists, uint64_t after_uid,
+                          uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

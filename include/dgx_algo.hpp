@@ -187,6 +187,73 @@ inline pb::UidPack EncodeFromBuffer(const std::vector<uint8_t>& buf, uint32_t bl
 
 }  // namespace codec
 
+namespace algo {
+
+// A node of a regexp()'s trigram query tree (cindex.Query): op DGX_QAND / DGX_QOR, its trigrams as leaf indices and its
+// sub-nodes (indices above its own).  A leaf is an unsplit list's pack (nullptr: empty; no pending postings) or a list
+// the caller decoded.
+struct QueryNode {
+    uint8_t op;
+    std::vector<uint32_t> leaves, subs;
+};
+struct TrigramLeaf {
+    const pb::UidPack* pack = nullptr;
+    const pb::List* list = nullptr;  // set: a list leaf
+};
+
+// uidsForRegex(attr, arg, query, &pb.List{}) (worker/trigram.go:24-102) with AfterUid = afterUID: one
+// dgx_trigram_query call, pack leaves passed first as the ABI numbers them.
+inline pb::List UidsForRegex(const std::vector<QueryNode>& tree, const std::vector<TrigramLeaf>& leaves,
+                             uint64_t afterUID) {
+    std::vector<uint32_t> order(leaves.size());
+    std::vector<dgx_pack_view> views;
+    std::vector<uint64_t> lists, list_off{0}, bound(leaves.size());
+    uint32_t k = 0;
+    for (size_t j = 0; j < leaves.size(); ++j)
+        if (!leaves[j].list) {
+            order[j] = k++;
+            bound[j] = codec::ExactLen(leaves[j].pack);
+            views.push_back(leaves[j].pack ? leaves[j].pack->view() : dgx_pack_view{});
+        }
+    std::vector<dgx_pack_ref> refs(views.size());
+    for (size_t i = 0; i < views.size(); ++i) refs[i] = {views[i].nblocks ? &views[i] : nullptr, 0, 0};
+    for (size_t j = 0; j < leaves.size(); ++j)
+        if (leaves[j].list) {
+            order[j] = k++;
+            lists.insert(lists.end(), leaves[j].list->Uids.begin(), leaves[j].list->Uids.end());
+            list_off.push_back(lists.size());
+            bound[j] = leaves[j].list->Uids.size();
+        }
+    std::vector<uint8_t> op;
+    std::vector<uint32_t> leaf_off{0}, leaf_idx, sub_off{0}, sub_idx;
+    std::vector<uint64_t> nb(tree.size());  // the root's bound is the out_cap the call needs
+    for (size_t i = tree.size(); i-- > 0;) {
+        uint64_t b = tree[i].op == DGX_QAND ? ~0ull : 0;
+        for (uint32_t j : tree[i].leaves) b = tree[i].op == DGX_QAND ? std::min(b, bound[j]) : b + bound[j];
+        for (uint32_t s : tree[i].subs) b = tree[i].op == DGX_QAND ? std::min(b, nb[s]) : b + nb[s];
+        nb[i] = b == ~0ull ? 0 : b;
+    }
+    for (const QueryNode& q : tree) {
+        op.push_back(q.op);
+        for (uint32_t j : q.leaves) leaf_idx.push_back(order[j]);
+        leaf_off.push_back(leaf_idx.size());
+        sub_idx.insert(sub_idx.end(), q.subs.begin(), q.subs.end());
+        sub_off.push_back(sub_idx.size());
+    }
+    const dgx_query_tree t{tree.size(), op.data(), leaf_off.data(), leaf_idx.data(), sub_off.data(), sub_idx.data()};
+    const std::vector<uint64_t> mut_off(refs.size() + 1, 0);
+    const uint64_t cap = tree.empty() ? 0 : nb[0];
+    pb::List out;
+    out.Uids.resize(std::max<uint64_t>(cap, 1));
+    size_t n = 0;
+    check(dgx_trigram_query(&t, refs.data(), refs.size(), nullptr, nullptr, mut_off.data(), lists.data(),
+                            list_off.data(), list_off.size() - 1, afterUID, out.Uids.data(), cap, &n));
+    out.Uids.resize(n);
+    return out;
+}
+
+}  // namespace algo
+
 // Wire-format adjacency (dgx_wire_*, host only): the bytes proto.Unmarshal sees at posting/list.go:1045 and
 // the pb.List messages of pb.Result.uid_matrix (protos/pb.proto:22-24, 76-78).
 namespace wire {

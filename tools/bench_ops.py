@@ -137,6 +137,7 @@ def main():
     ap.add_argument("--c9-only", action="store_true", help="only the C9 List.Uids rows with mutable layers")
     ap.add_argument("--c10-only", action="store_true", help="only the C10 unfiltered List.Uids and count rows")
     ap.add_argument("--c11-only", action="store_true", help="only the C11 backup / restore codec rows")
+    ap.add_argument("--c12-only", action="store_true", help="only the C12 regexp() trigram query rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -150,9 +151,11 @@ def main():
         rows = c10_rows(Lane())
     elif args.c11_only:
         rows = c11_rows(Lane())
+    elif args.c12_only:
+        rows = c12_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1221,6 +1224,183 @@ def c11_rows(L, threads: int = 16):
             lib.dgx_dev_pack_free(h)
         lib.dgx_cache_clear()
     return out_rows
+
+
+C12_PATTERNS = ("abcd", "abc|def", "abc.*def", "(abc|xyz)def", "abc(de|fg)h", "qu[aeiou]ck")
+
+
+def c12_trees(gt, idx):
+    """(label, tree, trigrams) of C12: the six patterns' trees, then two trees over the index's largest trigram lists,
+    the regime where a selective pattern still reads big lists: an AND of the three largest lists of different words and
+    a rare trigram (one small driving leaf, three large non-driving ones), and an AND of the two largest (a large
+    driving leaf)."""
+    trees = [(f"/{pat}/", *gt.tree_of_pattern(gt.PATTERNS[pat])) for pat in C12_PATTERNS]
+    words = np.diff(idx.word_off)  # values per word: a trigram's list is at most the sum over its words
+    est = sorted(((int(words[ws].sum()), t) for t, ws in idx.tri_words.items()), reverse=True)
+    big, used = [], set()
+    for _, t in est:  # from different words, so that the lists are not near copies of each other
+        if len(big) < 3 and not used & set(idx.tri_words[t]):
+            big.append(t)
+            used |= set(idx.tri_words[t])
+    rare = min(est, key=lambda e: abs(e[0] - 20_000))[1]
+    trees.append((f"large AND selective ({'&'.join(big)}&{rare})", [(gt.QAND, [0, 1, 2, 3], [])], big + [rare]))
+    trees.append((f"large AND ({'&'.join(big[:2])})", [(gt.QAND, [0, 1], [])], big[:2]))
+    return trees
+
+
+def c12_rows(L, threads: int = 16, n_nodes: int = 10_000_000):
+    """C12 "regexp() over a trigram index": a synthetic index of n_nodes string values (tests/gen_trigram.py), the query
+    trees codesearch would build for six patterns and two trees over the index's largest lists (c12_trees), every
+    trigram a posting list held as a UidPack (BlockSize 256, no mutable layer).  Legs per tree, each checked in full against the oracle's restatement of
+    uidsForRegex (tests/trigram_oracle.c): (1) the device form on resident packs (CUDA events), (2) the host form with
+    named packs, (3) with anonymous packs over PCIe, (4) the same tree composed from existing device calls -- the
+    unfiltered rows, then dgx_dev_filter_batch per AND and dgx_dev_merge_sorted per OR, bottom up, reading each length
+    back -- (5) the oracle on 1 thread (warmed up, then the mean of several calls), and 16 copies of the query on `threads`
+    threads (time per query)."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    import gen_trigram as gt
+    import trigram_oracle as tgo
+    import trigram_plan as tp
+    from dgraph_b200 import algo, codec, pb
+    from oracle import pyoracle as orc
+
+    lib = L.lib
+    idx = gt.TrigramIndex(seed=12, n_nodes=n_nodes, n_words=20_000)
+    out_rows = []
+    lib.dgx_cache_clear()
+    _lib.check(lib.dgx_cache_configure(16 << 30))
+
+    def dp(t):
+        return C.c_void_p(t.data_ptr())
+
+    def wall(fn, reps):
+        fn()
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            fn()
+        return (time.perf_counter() - t0) / reps * 1e3
+
+    for pi, (label, tree, tris) in enumerate(c12_trees(gt, idx)):
+        uids = [idx.posting(t) for t in tris]
+        ops = [orc.encode(u, 256) if u.size else None for u in uids]
+        packs = [pb.UidPack(o.block_size, o.base, o.num_uids, o.delta_off, o.deltas) if o is not None else None
+                 for o in ops]
+        nl = len(tris)
+        leaf_uids = int(sum(u.size for u in uids))
+        plan = tp.plan(tree, [u.size for u in uids])
+        cand = int(np.unique(np.concatenate([uids[j] for j in plan.drive] + [np.zeros(0, np.uint64)])).size)
+        q = tgo.Query(tree, [(o, None) for o in ops])
+        want = q.run(0)
+        t_o1 = wall(lambda: q.run(0), 5)
+        t0 = time.perf_counter()
+        with ThreadPoolExecutor(max_workers=threads) as ex:  # ctypes releases the GIL
+            got_n = list(ex.map(lambda _: q.run(0), range(16)))
+        t_on = (time.perf_counter() - t0) * 1e3 / 16
+        ok_on = all(np.array_equal(g, want) for g in got_n)
+        cap = plan.root_bound
+        qt, qa = algo.query_tree(tree)
+        zero_off = np.zeros(nl + 1, np.uint64)
+        dummy = np.zeros(1, np.uint64)
+        named = [(1_200_000 + 100 * pi + j, 1) for j in range(nl)]
+        refs_n, keep_n = algo._refs_of(packs, named)
+        refs_a, keep_a = algo._refs_of(packs)
+        hout = np.empty(max(cap, 1), np.uint64)
+        n = C.c_size_t(0)
+
+        def host(refs):
+            _lib.check(lib.dgx_trigram_query(C.byref(qt), refs, nl, _p_(dummy), _p_(dummy), _p_(zero_off), _p_(dummy),
+                                             _p_(zero_off), 0, 0, _p_(hout), cap, C.byref(n)))
+        handles, tab = [], (C.c_void_p * nl)()
+        for j, pk in enumerate(packs):
+            if pk is None:
+                continue
+            view = codec.view_of(pk.normalized())
+            h = C.c_void_p()
+            _lib.check(lib.dgx_dev_pack_upload(L.h, C.byref(view), C.byref(h)))
+            handles.append(h)
+            tab[j] = h.value
+        try:
+            d_out = torch.empty(max(cap, 1) + 4, dtype=torch.int64, device=DEV)
+            d_len = torch.zeros(1, dtype=torch.int64, device=DEV)
+            d_mu = torch.zeros(1, dtype=torch.int64, device=DEV)
+            d_mf = torch.zeros(16, dtype=torch.uint8, device=DEV)
+
+            def dev():
+                _lib.check(lib.dgx_dev_trigram_query(L.h, C.byref(qt), tab, nl, dp(d_mu), dp(d_mf), _p_(zero_off),
+                                                     dp(d_mu), _p_(zero_off), 0, 0, dp(d_out), cap, dp(d_len)))
+            ms_dev, _ = timeit(dev, warm=3, reps=10)
+            L.sync()
+            nd = int(d_len.cpu()[0])
+            ok_dev = np.array_equal(d_out[:nd].cpu().numpy().view(np.uint64), want)
+            legs = [("device form, resident packs", ms_dev, ok_dev, "dgx_dev_trigram_query, CUDA events")]
+            for name, refs in (("host form, named packs", refs_n), ("host form, anonymous packs", refs_a)):
+                ms = wall(lambda: host(refs), 5)
+                legs.append((name, ms, bool(np.array_equal(hout[:n.value], want)), "dgx_trigram_query, wall clock"))
+
+            # composed from existing device calls: rows, then each node bottom up with its length read back
+            rows_cap = sum(u.size for u in uids)
+            d_rows = torch.empty(rows_cap + 4, dtype=torch.int64, device=DEV)
+            d_roff = torch.zeros(nl + 1, dtype=torch.int64, device=DEV)
+            bufs = []
+
+            def composed():
+                bufs.clear()
+                _lib.check(lib.dgx_dev_list_uids_unfiltered_rows(L.h, tab, nl, dp(d_mu), dp(d_mf), _p_(zero_off), 0, 0,
+                                                                 dp(d_rows), rows_cap, dp(d_roff)))
+                L.sync()
+                off = d_roff.cpu().numpy()
+                leaf = [(d_rows.data_ptr() + 8 * int(off[j]), int(off[j + 1] - off[j])) for j in range(nl)]
+                val = [None] * len(tree)
+                for i in reversed(range(len(tree))):
+                    op, ls, subs = tree[i]
+                    ch = [leaf[j] for j in ls] + [val[s] for s in subs]
+                    if len(ch) == 1:
+                        val[i] = ch[0]
+                        continue
+                    tot = sum(c[1] for c in ch) if op == gt.QOR else min(c[1] for c in ch)
+                    o = torch.empty(tot + 4, dtype=torch.int64, device=DEV)
+                    ln = torch.zeros(2, dtype=torch.int64, device=DEV)
+                    bufs.extend([o, ln])
+                    ptrs = (C.c_void_p * len(ch))(*[c[0] for c in ch])
+                    lens = (C.c_size_t * len(ch))(*[c[1] for c in ch])
+                    if op == gt.QOR:
+                        _lib.check(lib.dgx_dev_merge_sorted(L.h, ptrs, lens, len(ch), dp(o), tot, dp(ln)))
+                        L.sync()
+                        val[i] = (o.data_ptr(), int(ln[0].cpu()))
+                    else:
+                        koff = (C.c_size_t * 2)(0, len(ch))
+                        _lib.check(lib.dgx_dev_filter_batch(L.h, 0, ptrs, lens, koff, 1, dp(o), tot, dp(ln)))
+                        L.sync()
+                        val[i] = (o.data_ptr(), int(ln[1].cpu()))
+                return val[0]
+            res = composed()
+            ms_c = wall(composed, 5)
+            res = composed()
+            got_c = np.empty(res[1], np.uint64)
+            if res[1]:
+                _lib.check(lib.dgx_memcpy_d2h(L.h, _p_(got_c), C.c_void_p(res[0]), 8 * res[1]))
+            L.sync()
+            legs.append(("composed from existing device calls", ms_c, bool(np.array_equal(got_c, want)),
+                         "unfiltered rows, then dgx_dev_filter_batch / dgx_dev_merge_sorted per node, a sync per node"))
+            legs += [("oracle uidsForRegex (1 thread)", t_o1, True, "restated in C"),
+                     (f"oracle uidsForRegex, 16 queries on {threads} threads", t_on, ok_on, "time per query")]
+            cfg = (f"C12 regexp {label}: {len(tree)} nodes, {nl} trigram packs of {leaf_uids} uids over {n_nodes} values, "
+                   f"{cand} candidates, {want.size} uids out")
+            for name, ms, ok, note in legs:
+                out_rows.append(row(f"UidsForRegex {label} ({name})", cfg, ms, leaf_uids, 8 * (leaf_uids + want.size), ok,
+                                    {"leaf_uids": leaf_uids, "candidates": cand, "driving_bound": plan.dcap,
+                                     "result": int(want.size), "nodes": len(tree), "leaves": nl, "note": note,
+                                     "bytes_note": "algorithmic bytes: 8 per leaf uid in and per uid out"}))
+        finally:
+            for h in handles:
+                lib.dgx_dev_pack_free(h)
+    lib.dgx_cache_clear()
+    return out_rows
+
+
+def _p_(a):
+    return a.ctypes.data_as(C.c_void_p)
 
 
 if __name__ == "__main__":
