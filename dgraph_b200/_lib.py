@@ -13,6 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.environ.get("DGX_LIB") or os.path.join(_HERE, "libdgx.so")  # DGX_LIB: try an experimental build
 
 DGX_OK = 0
+DGX_ERR_ARG, DGX_ERR_CAP = -3, -4
 STATUS_NAMES = {0: "DGX_OK", -1: "DGX_ERR_CUDA", -2: "DGX_ERR_OOM", -3: "DGX_ERR_ARG", -4: "DGX_ERR_CAP", -5: "DGX_ERR_NODEV"}
 OP_INTERSECT, OP_DIFFERENCE = 0, 1
 
@@ -84,6 +85,7 @@ SYMBOLS = {
     "dgx_decode_to_buffer_rows": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _sz]),
     "dgx_encode_from_buffer_rows": (_int, [_vp, _vp, _sz, C.c_uint32, _vp, _sz, _vp, _vp, _vp]),
     "dgx_trigram_query": (_int, [C.POINTER(QueryTree), C.POINTER(PackRef), _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _szp]),
+    "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
     "dgx_encode_bound": (None, [_sz, C.c_uint32, _szp, _szp]),
     "dgx_encode": (_int, [_vp, _sz, C.c_uint32, _vp, _vp, _vp, _vp, _szp, _szp, C.POINTER(PackView)]),
@@ -124,6 +126,7 @@ SYMBOLS = {
     "dgx_dev_list_uids_unfiltered_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, C.c_int32, _vp, _sz, _vp]),
     "dgx_dev_list_count_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, _vp]),
     "dgx_dev_trigram_query": (_int, [_vp, C.POINTER(QueryTree), _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _vp]),
+    "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),
     "dgx_filter_tail_queries": (_u64, [_vp]),
     "dgx_wire_posting_list_pack": (_int, [_vp, _sz, C.POINTER(_vp), _szp]),

@@ -389,6 +389,58 @@ def MergeSortedMatrix(rows) -> List:
     return List(out[: n.value])
 
 
+def _csr_u64(rows):
+    arrs = []
+    for r in rows:
+        u = r.Uids if isinstance(r, List) else r
+        arrs.append(np.zeros(0, np.uint64) if u is None else _u64(u))
+    off = np.zeros(len(arrs) + 1, dtype=np.uint64)
+    np.cumsum([a.size for a in arrs], out=off[1:])
+    flat = np.concatenate(arrs) if int(off[-1]) else np.zeros(1, np.uint64)
+    return flat, off
+
+
+def GroupByUid(parents, src, rows, dest, members: bool = True):
+    """@groupby over one uid predicate (query/groupby.go formResult / formGroups / groupLess) for every parent row in
+    ONE call (dgx_groupby_uid).
+
+    parents: sg.uidMatrix, strictly ascending rows; src: child.SrcUIDs, strictly ascending; rows: child.uidMatrix,
+    row i the values of src[i], strictly ascending; dest: child.DestUIDs, holding every value of every row.  A parent
+    with one row equal to src gives fillGroupedVars' grouping.  Returns per parent (keys, counts, members): its groups
+    ordered by (count, key), each group's key and count(uid), and members = (values, offsets) with each group's
+    ascending source uids, or None when members is False (counts only: the members stay on the device)."""
+    par, par_off = _csr_u64(parents)
+    v, v_off = _csr_u64(rows)
+    src_a = _u64(src.Uids if isinstance(src, List) else src)
+    dest_a = _u64(dest.Uids if isinstance(dest, List) else dest)
+    if src_a.size != len(rows):
+        raise ValueError(f"{src_a.size} sources for {len(rows)} rows")
+    lib = _lib.load()
+    npar = len(parents)
+    grp_off = np.zeros(npar + 1, dtype=np.uint64)
+    ng, nm = C.c_size_t(0), C.c_size_t(0)
+    gcap = mcap = int(v_off[-1])  # a single parent never has more; a larger call is sized again from the exact counts
+    for _ in range(2):
+        keys = np.empty(max(gcap, 1), dtype=np.uint64)
+        mem_off = np.empty(gcap + 1, dtype=np.uint64)
+        mem = np.empty(max(mcap, 1), dtype=np.uint64) if members else None
+        rc = lib.dgx_groupby_uid(_p(src_a), src_a.size, _p(v), _p(v_off), _p(dest_a), dest_a.size, _p(par),
+                                 _p(par_off), npar, _p(keys), _p(grp_off), _p(mem_off), gcap,
+                                 _p(mem) if members else None, mcap, C.byref(ng), C.byref(nm))
+        if rc != _lib.DGX_ERR_CAP:
+            break
+        gcap, mcap = ng.value, nm.value
+    _lib.check(rc)
+    out = []
+    for p in range(npar):
+        g0, g1 = int(grp_off[p]), int(grp_off[p + 1])
+        off = mem_off[g0:g1 + 1] if g1 > g0 else np.zeros(1, np.uint64)
+        counts = np.diff(off)
+        m = (mem[int(off[0]):int(off[-1])].copy(), off - off[0]) if members else None
+        out.append((keys[g0:g1].copy(), counts, m))
+    return out
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

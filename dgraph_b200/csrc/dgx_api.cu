@@ -39,6 +39,7 @@
 #include "encode_kernel.cuh"
 #include "backup_codec_kernel.cuh"
 #include "trigram_kernel.cuh"
+#include "groupby_kernel.cuh"
 #include "wire.hpp"
 
 using namespace dgx;
@@ -453,6 +454,10 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
         CK(cudaMemsetAsync(l->d_err, 0, sizeof(int), l->stream));
         if (flag & kLaneErrOrder) return fail(DGX_ERR_ARG, "a row of the uid matrix is not strictly ascending");
         if (flag & kLaneErrVarint) return fail(DGX_ERR_ARG, "a uid_bytes row is not a sequence of valid uvarints");
+        if (flag & kLaneErrGroupBy)
+            return fail(DGX_ERR_ARG, "a groupby input is malformed (src, a row, a parent row or dest not strictly "
+                                     "ascending, offsets not starting at 0, decreasing or past their arrays, a row "
+                                     "value missing from dest, or 2^32 restricted edges or more)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -3481,6 +3486,262 @@ extern "C" int dgx_merge_sorted_matrix(const uint64_t* v, const uint64_t* v_off,
     rc = merge_matrix_impl(l, d_v, d_off, nrows, m, (uint64_t*)d_out, m, (uint64_t*)d_len);
     if (rc) return rc;
     return finish_to_host(l, (uint64_t*)d_len, (uint64_t*)d_out, m, out, out_cap, out_len);
+}
+
+// ---------------------------------------------------------------------------
+// @groupby over a uid predicate: a uid matrix inverted into ordered groups per parent row (groupby_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr uint64_t kGbMax = uint64_t(1) << 32;  // rows, parents, dest values, row values and edges are 32-bit counts
+
+static uint32_t gb_bits(uint64_t x) { return x ? 64u - (uint32_t)__builtin_clzll(x) : 0u; }
+static unsigned gb_grid(uint64_t n) { return (unsigned)std::max<uint64_t>(1, (n + 255) / 256); }
+
+// The key widths and radix passes of a call, from its sizes alone: parents need b_p = bits(npar - 1), dest ranks
+// b_d = bits(ndest - 1), group sizes (at most nrows) b_s = bits(nrows).
+struct GbPlan {
+    uint32_t b_p, b_d, b_s, p1, p2;
+};
+static GbPlan gb_plan(uint64_t nrows, uint64_t ndest, uint64_t npar) {
+    GbPlan g;
+    g.b_p = gb_bits(npar - 1);
+    g.b_d = gb_bits(ndest ? ndest - 1 : 0);
+    g.b_s = gb_bits(nrows);
+    g.p1 = (g.b_p + g.b_d + GB_DIGIT_BITS - 1) / GB_DIGIT_BITS;
+    g.p2 = (g.b_p + g.b_s + GB_DIGIT_BITS - 1) / GB_DIGIT_BITS;
+    return g;
+}
+
+// One stable LSD pass per 8 key bits, ping-ponging between k[0] / p[0] and k[1] / p[1]: the result is in buffer
+// passes & 1.  Three launches per pass.
+static int gb_sort(dgx_lane* l, const GbParams& P, u64* const k[2], u32* const p[2], const u64* n_word,
+                   uint32_t passes, u64* hist, u64* hoff, u64*& status, u32*& ticket) {
+    const uint64_t hn = (uint64_t)GB_RADIX * P.tiles, ht = (hn + EN_TILE - 1) / EN_TILE;
+    for (uint32_t q = 0; q < passes; ++q) {
+        const int a = q & 1;
+        const u32 shift = q * GB_DIGIT_BITS;
+        gb_hist_kernel<<<(unsigned)P.tiles, GB_NT, 0, l->stream>>>(k[a], n_word, P.bad, shift, P.tiles, hist);
+        scan_u64_kernel<<<(unsigned)ht, EN_NT, 0, l->stream>>>(hist, hoff, P.words + GB_W_H, hn, status, ticket, nullptr);
+        gb_scatter_kernel<<<(unsigned)P.tiles, GB_NT, 0, l->stream>>>(k[a], p[a], n_word, P.bad, shift, P.tiles, hoff,
+                                                                       k[a ^ 1], p[a ^ 1]);
+        CK(cudaGetLastError());
+        status += ht;
+        ticket += 1;
+    }
+    count_launches(l, 3 * (int)passes);
+    return DGX_OK;
+}
+
+// The checks, the pairs and the edge scan: three launches.  Workspace: 24 bytes per parent value of par_cap.
+static int gb_front(dgx_lane* l, GbParams& P, u32** tickets) {
+    const uint64_t pc = std::max<uint64_t>(P.par_cap, 1), st = (pc + EN_TILE - 1) / EN_TILE;
+    // zeroed: [bad | words | tickets | scan status], so a refused input leaves every count at 0
+    const size_t b_head = 64 + GB_WORDS * sizeof(u64) + 32 * sizeof(u32), b_zero = b_head + st * sizeof(u64);
+    void *z, *w;
+    int rc = l->ws.alloc(b_zero, &z);
+    if (rc) return rc;
+    if ((rc = l->ws.alloc((2 * pc + 1) * sizeof(u64) + 2 * pc * sizeof(u32), &w))) return rc;
+    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
+    P.bad = (int*)z;
+    P.words = (u64*)((char*)z + 64);
+    *tickets = (u32*)(P.words + GB_WORDS);
+    u64* status = (u64*)((char*)z + b_head);
+    P.plen = (u64*)w;
+    P.eoff = P.plen + pc;
+    P.prow = (u32*)(P.eoff + pc + 1);
+    P.ppar = P.prow + pc;
+    P.err = l->d_err;
+    const uint64_t nt = std::max(std::max(P.nrows + 1, P.npar + 1), std::max(P.ndest, P.v_cap));
+    gb_check_kernel<<<gb_grid(nt), 256, 0, l->stream>>>(P);
+    gb_pairs_kernel<<<gb_grid(pc), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)st, EN_NT, 0, l->stream>>>(P.plen, P.eoff, P.words + GB_W_PV, P.par_cap, status,
+                                                           *tickets, P.words + GB_W_E);
+    CK(cudaGetLastError());
+    count_launches(l, 3);
+    *tickets += 1;
+    return DGX_OK;
+}
+
+// Expand, both sorts, the groups and the write: 8 + 3 (P1 + P2) launches.  Workspace: 94 bytes per edge of e_cap
+// (edge keys and rows twice 24, heads and group indices 16, group starts, order keys twice and group of each position
+// 36, sizes and offsets 16, positions 4, hist and its scan 2).
+static int gb_back(dgx_lane* l, GbParams& P, const GbPlan& g, u32* ticket) {
+    const uint64_t ec = std::max<uint64_t>(P.e_cap, 1);
+    P.tiles = (ec + GB_TILE - 1) / GB_TILE;
+    const uint64_t hn = (uint64_t)GB_RADIX * P.tiles, ht = (hn + EN_TILE - 1) / EN_TILE, et = (ec + EN_TILE - 1) / EN_TILE;
+    const size_t b_zero = ((g.p1 + g.p2) * ht + 2 * et) * sizeof(u64);
+    void *z, *w;
+    int rc = l->ws.alloc(b_zero, &z);
+    if (rc) return rc;
+    const size_t n64 = 2 * ec + ec + (ec + 1) + (ec + 1) + 2 * ec + ec + (ec + 1) + hn + (hn + 1);
+    if ((rc = l->ws.alloc(n64 * sizeof(u64) + 5 * ec * sizeof(u32), &w))) return rc;
+    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
+    u64* status = (u64*)z;
+    u64* q = (u64*)w;
+    u64* ek[2] = {q, q + ec};
+    q += 2 * ec;
+    P.head = q;
+    P.gidx = P.head + ec;
+    P.gstart = P.gidx + ec + 1;
+    u64* gk[2] = {P.gstart + ec + 1, P.gstart + 2 * ec + 1};
+    P.gsz = gk[1] + ec;
+    P.moff = P.gsz + ec;
+    u64* hist = P.moff + ec + 1;
+    u64* hoff = hist + hn;
+    u32* r = (u32*)(hoff + hn + 1);
+    u32* ep[2] = {r, r + ec};
+    u32* gp[2] = {r + 2 * ec, r + 3 * ec};
+    P.inv = r + 4 * ec;
+    P.ek = ek[0];
+    P.ep = ep[0];
+    gb_expand_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    if ((rc = gb_sort(l, P, ek, ep, P.words + GB_W_E, g.p1, hist, hoff, status, ticket))) return rc;
+    P.ek = ek[g.p1 & 1];
+    P.ep = ep[g.p1 & 1];
+    gb_heads_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)et, EN_NT, 0, l->stream>>>(P.head, P.gidx, P.words + GB_W_E, P.e_cap, status, ticket,
+                                                           P.words + GB_W_G);
+    status += et;
+    ticket += 1;
+    gb_groups_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
+    gb_gkeys_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P, gk[0], gp[0]);
+    CK(cudaGetLastError());
+    if ((rc = gb_sort(l, P, gk, gp, P.words + GB_W_G, g.p2, hist, hoff, status, ticket))) return rc;
+    P.gk = gk[g.p2 & 1];
+    P.gp = gp[g.p2 & 1];
+    gb_sizes_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)et, EN_NT, 0, l->stream>>>(P.gsz, P.moff, P.words + GB_W_G, P.e_cap, status, ticket,
+                                                           nullptr);
+    gb_write_kernel<<<gb_grid(std::max<uint64_t>(ec + 1, P.npar + 1)), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 8);
+    return DGX_OK;
+}
+
+static GbParams gb_params(const uint64_t* src, size_t nrows, const uint64_t* v, const uint64_t* v_off, uint64_t v_cap,
+                          const uint64_t* dest, size_t ndest, const uint64_t* par, const uint64_t* par_off, size_t npar,
+                          uint64_t par_cap, const GbPlan& g) {
+    GbParams P{};
+    P.src = (const u64*)src;
+    P.nrows = nrows;
+    P.v = (const u64*)v;
+    P.v_off = (const u64*)v_off;
+    P.v_cap = v_cap;
+    P.dest = (const u64*)dest;
+    P.ndest = ndest;
+    P.par = (const u64*)par;
+    P.par_off = (const u64*)par_off;
+    P.npar = npar;
+    P.par_cap = par_cap;
+    P.b_d = g.b_d;
+    P.b_s = g.b_s;
+    return P;
+}
+
+extern "C" int dgx_dev_groupby_uid(dgx_lane* l, const uint64_t* d_src, size_t nrows, const uint64_t* d_v,
+                                   const uint64_t* d_v_off, size_t v_cap, const uint64_t* d_dest, size_t ndest,
+                                   const uint64_t* d_par, const uint64_t* d_par_off, size_t npar, size_t par_cap,
+                                   size_t e_cap, uint64_t* d_keys, uint64_t* d_grp_off, uint64_t* d_mem_off,
+                                   size_t grp_cap, uint64_t* d_members, size_t mem_cap, uint64_t* d_sizes) {
+    if (!l || !d_sizes || !d_grp_off || !d_mem_off) return fail(DGX_ERR_ARG, "null argument");
+    if (nrows >= kGbMax || npar >= kGbMax || ndest >= kGbMax || v_cap >= kGbMax || par_cap >= kGbMax || e_cap >= kGbMax)
+        return fail(DGX_ERR_ARG, "groupby sizes are 32-bit: nrows, npar, ndest, v_cap, par_cap and e_cap below 2^32");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_grp_off, (npar + 1) * sizeof(uint64_t));
+    l->note_output(d_mem_off, (grp_cap + 1) * sizeof(uint64_t));
+    l->note_output(d_sizes, 2 * sizeof(uint64_t));
+    if (npar == 0 || nrows == 0 || v_cap == 0 || par_cap == 0) {  // no edge can exist: zero groups
+        CK(cudaMemsetAsync(d_grp_off, 0, (npar + 1) * sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_mem_off, 0, sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_sizes, 0, 2 * sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (!d_src || !d_v || !d_v_off || !d_par || !d_par_off || (ndest && !d_dest) || (grp_cap && !d_keys))
+        return fail(DGX_ERR_ARG, "null argument");
+    const GbPlan g = gb_plan(nrows, ndest, npar);
+    GbParams P = gb_params(d_src, nrows, d_v, d_v_off, v_cap, d_dest, ndest, d_par, d_par_off, npar, par_cap, g);
+    P.e_cap = e_cap;
+    P.keys = (u64*)d_keys;
+    P.grp_off = (u64*)d_grp_off;
+    P.mem_off = (u64*)d_mem_off;
+    P.members = (u64*)d_members;
+    P.grp_cap = grp_cap;
+    P.mem_cap = mem_cap;
+    P.sizes = (u64*)d_sizes;
+    u32* tickets;
+    if (int rc = gb_front(l, P, &tickets)) return rc;
+    if (int rc = gb_back(l, P, g, tickets)) return rc;
+    l->note_output(d_keys, grp_cap * sizeof(uint64_t));
+    l->note_output(d_members, mem_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_groupby_uid(const uint64_t* src, size_t nrows, const uint64_t* v, const uint64_t* v_off,
+                               const uint64_t* dest, size_t ndest, const uint64_t* par, const uint64_t* par_off,
+                               size_t npar, uint64_t* keys, uint64_t* grp_off, uint64_t* mem_off, size_t grp_cap,
+                               uint64_t* members, size_t mem_cap, size_t* ngroups, size_t* nmembers) {
+    if (!ngroups || !nmembers || !grp_off || !mem_off || (npar && !par_off) || (nrows && !v_off))
+        return fail(DGX_ERR_ARG, "null argument");
+    if (nrows >= kGbMax || npar >= kGbMax || ndest >= kGbMax)
+        return fail(DGX_ERR_ARG, "groupby sizes are 32-bit: nrows, npar and ndest below 2^32");
+    if (nrows) if (int rc = check_offsets("v_off", v_off, nrows, kGbMax)) return rc;
+    if (npar) if (int rc = check_offsets("par_off", par_off, npar, kGbMax)) return rc;
+    const uint64_t m = nrows ? v_off[nrows] : 0, pv = npar ? par_off[npar] : 0;
+    auto none = [&]() {  // zero groups: every parent owns none
+        memset(grp_off, 0, (npar + 1) * sizeof(uint64_t));
+        mem_off[0] = 0;
+        *ngroups = *nmembers = 0;
+        return DGX_OK;
+    };
+    if (m == 0 || pv == 0) return none();
+    if (!src || !v || !par || (ndest && !dest) || (grp_cap && !keys)) return fail(DGX_ERR_ARG, "null argument");
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += nrows + m + ndest + pv;
+    uint64_t *d_src, *d_v, *d_v_off, *d_dest, *d_par, *d_par_off;  // one copy each
+    int rc;
+    if ((rc = upload_list(l, src, nrows, &d_src)) || (rc = upload_list(l, v, m, &d_v)) ||
+        (rc = upload_list(l, v_off, nrows + 1, &d_v_off)) || (rc = upload_list(l, dest, ndest, &d_dest)) ||
+        (rc = upload_list(l, par, pv, &d_par)) || (rc = upload_list(l, par_off, npar + 1, &d_par_off)))
+        return rc;
+    const GbPlan g = gb_plan(nrows, ndest, npar);
+    GbParams P = gb_params(d_src, nrows, d_v, d_v_off, m, d_dest, ndest, d_par, d_par_off, npar, pv, g);
+    u32* tickets;
+    if ((rc = gb_front(l, P, &tickets))) return rc;
+    // the edge count sizes the rest: one round trip, which also surfaces a refused input
+    CK(cudaMemcpyAsync(l->h_word, P.words + GB_W_E, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) return rc;
+    const uint64_t E = l->h_word[0];
+    if (E == 0) return none();
+    if (E >= kGbMax) return fail(DGX_ERR_ARG, "%llu restricted edges: at most 2^32 - 1", (unsigned long long)E);
+    void* d_o;
+    if ((rc = l->ws.alloc((3 * E + npar + 4) * sizeof(uint64_t), &d_o))) return rc;
+    P.keys = (u64*)d_o;
+    P.members = members ? P.keys + E : nullptr;
+    P.mem_off = P.keys + 2 * E;
+    P.grp_off = P.mem_off + E + 1;
+    P.sizes = P.grp_off + npar + 1;
+    P.e_cap = P.grp_cap = P.mem_cap = E;
+    if ((rc = gb_back(l, P, g, tickets))) return rc;
+    CK(cudaMemcpyAsync(l->h_word, P.sizes, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) return rc;
+    const uint64_t G = l->h_word[0];
+    *ngroups = G;
+    *nmembers = E;
+    if (G > grp_cap || (members && E > mem_cap))
+        return fail(DGX_ERR_CAP, "%llu groups of %llu members do not fit grp_cap %zu / mem_cap %zu",
+                    (unsigned long long)G, (unsigned long long)E, grp_cap, mem_cap);
+    if (G) CK(cudaMemcpyAsync(keys, P.keys, G * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(mem_off, P.mem_off, (G + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(grp_off, P.grp_off, (npar + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (members) CK(cudaMemcpyAsync(members, P.members, E * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += (2 * G + npar + 2 + (members ? E : 0)) * sizeof(uint64_t);
+    g_stats.uids_out += members ? E : G;
+    return DGX_OK;
 }
 
 // ---------------------------------------------------------------------------

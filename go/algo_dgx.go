@@ -250,3 +250,88 @@ func IntersectRowsWith(matrix []*pb.List, dest *pb.List) {
 		l.Uids = append(l.Uids[:0], out[outOff[i]:outOff[i+1]]...)
 	}
 }
+
+// dgxMinGroupBy: below this many row values GroupByUid stays on the Go path (formResult's per-edge map).  The C13
+// record (profiles/h100_c13_groupby.json) times the library against a C restatement of that path, not against Go, so
+// this is the same bound as dgxMinMergeMatrix until a Go comparison sets it.
+const dgxMinGroupBy = 1 << 14
+
+// UidGroup is one group of a parent row of a @groupby over a uid predicate: its key (a uid of child.DestUIDs), its
+// count(uid), and its ascending source uids when GroupByUid was asked for members.
+type UidGroup struct {
+	Key   uint64
+	Count int
+	Uids  []uint64
+}
+
+// GroupByUid is formResult's UID-node branch (query/groupby.go:208-221) for every parent row at once, and
+// fillGroupedVars with parents = [{SrcUIDs}]: row i of matrix belongs to srcUIDs[i]; for each parent, the rows whose
+// source is in it are grouped by destination, and the groups come back ordered by (count, key).  That is
+// sort.Slice(groupLess)'s order when every aggregate child is count(uid); with value aggregates the caller sorts
+// again.  dest is child.DestUIDs.  It returns false, and the caller keeps the Go path, below dgxMinGroupBy row values,
+// when a parent row does not strictly ascend (orderasc / orderdesc on sg), and on any library error.
+func GroupByUid(parents []*pb.List, srcUIDs []uint64, matrix []*pb.List, dest []uint64,
+	withMembers bool) ([][]UidGroup, bool) {
+	n, m, np := len(matrix), totalUids(matrix), len(parents)
+	if n != len(srcUIDs) || m < dgxMinGroupBy || uint64(m) >= 1<<32 || np == 0 || uint64(np) >= 1<<32 {
+		return nil, false
+	}
+	// every slice handed to C is its own Go allocation holding no Go pointers
+	vOff, v := make([]uint64, n+1), make([]uint64, 0, m)
+	for i, r := range matrix {
+		vOff[i] = uint64(len(v))
+		if r != nil {
+			v = append(v, r.Uids...)
+		}
+	}
+	vOff[n] = uint64(len(v))
+	parOff, par := make([]uint64, np+1), make([]uint64, 0, totalUids(parents))
+	for i, p := range parents {
+		parOff[i] = uint64(len(par))
+		if p != nil {
+			for k, u := range p.Uids {
+				if k > 0 && p.Uids[k-1] >= u {
+					return nil, false // ordered parents: IndexOf bisects an unsorted list, keep Go's answer
+				}
+			}
+			par = append(par, p.Uids...)
+		}
+	}
+	parOff[np] = uint64(len(par))
+	src := append([]uint64(nil), srcUIDs...)
+	dst := append([]uint64(nil), dest...)
+	grpOff := make([]uint64, np+1)
+	gcap, mcap := m, m // one parent never has more; a larger call is sized again from the exact counts
+	var keys, memOff, mem []uint64
+	var ng, nm C.size_t
+	rc := C.int(C.DGX_ERR_CAP)
+	for attempt := 0; attempt < 2 && rc == C.DGX_ERR_CAP; attempt++ {
+		keys, memOff = make([]uint64, gcap+1), make([]uint64, gcap+1)
+		var memPtr *C.uint64_t
+		if withMembers {
+			mem = make([]uint64, mcap+1)
+			memPtr = u64ptr(mem)
+		}
+		rc = C.dgx_groupby_uid(u64ptr(src), C.size_t(n), u64ptr(v), u64ptr(vOff), u64ptr(dst), C.size_t(len(dst)),
+			u64ptr(par), u64ptr(parOff), C.size_t(np), u64ptr(keys), u64ptr(grpOff), u64ptr(memOff), C.size_t(gcap),
+			memPtr, C.size_t(mcap), &ng, &nm)
+		gcap, mcap = int(ng), int(nm)
+	}
+	if rc != C.DGX_OK {
+		return nil, false
+	}
+	out := make([][]UidGroup, np)
+	for p := 0; p < np; p++ {
+		g0, g1 := int(grpOff[p]), int(grpOff[p+1])
+		gs := make([]UidGroup, g1-g0)
+		for g := g0; g < g1; g++ {
+			lo, hi := memOff[g], memOff[g+1]
+			gs[g-g0] = UidGroup{Key: keys[g], Count: int(hi - lo)}
+			if withMembers {
+				gs[g-g0].Uids = mem[lo:hi:hi]
+			}
+		}
+		out[p] = gs
+	}
+	return out, true
+}

@@ -365,6 +365,28 @@ int dgx_trigram_query(const dgx_query_tree* tree, const dgx_pack_ref* refs, size
                       const uint8_t* mut_flags, const uint64_t* mut_off, const uint64_t* lists, const uint64_t* list_off,
                       size_t nlists, uint64_t after_uid, uint64_t* out, size_t out_cap, size_t* out_len);
 
+/* @groupby over one uid predicate (query/groupby.go formResult :208-221, formGroups, groupLess, fillGroupedVars): the
+ * child's uid matrix inverted into groups `dest uid -> ascending source uids`, restricted to every parent row, in one
+ * call.  Row i (v[v_off[i] .. v_off[i+1]), strictly ascending) belongs to source src[i] (src strictly ascending); parent
+ * p is par[par_off[p] .. par_off[p+1]) (strictly ascending).  Row i takes part in parent p iff src[i] is in parent p, and
+ * each of its values d then adds src[i] to parent p's group d.  dest (strictly ascending, child.DestUIDs) holds every
+ * value of every row.
+ * Output: parent p owns the groups grp_off[p] .. grp_off[p+1] (npar + 1 values), ordered by (size, key) ascending, which
+ * is groupLess's order when every group has the same number of aggregates; group g has key keys[g] and its members
+ * members[mem_off[g] .. mem_off[g+1]), ascending (mem_off has room for grp_cap + 1 values).  members == NULL: counts
+ * only, nothing is written to members and mem_cap is not read.  *ngroups / *nmembers get the exact sizes (nmembers is
+ * the number of restricted edges).  npar == 0, or no row value or parent value at all: zero groups, no device.
+ * DGX_ERR_CAP, with the exact sizes and nothing else written: *ngroups > grp_cap, or *nmembers > mem_cap with members.
+ * DGX_ERR_ARG with nothing written: nrows, npar or ndest of 2^32 or more, offsets not starting at 0, decreasing or
+ * totalling 2^32 or more, a null array that is needed (checked on the host); src, a row, a parent row or dest not
+ * strictly ascending, a row value not in dest, 2^32 restricted edges or more (checked on the device).
+ * Launches: 11 + 3 (P1 + P2) with P1 = ceil((b_p + b_d) / 8), P2 = ceil((b_p + b_s) / 8), b_p, b_d and b_s the bit
+ * widths of npar - 1, ndest - 1 and nrows (DESIGN section 3.9). */
+int dgx_groupby_uid(const uint64_t* src, size_t nrows, const uint64_t* v, const uint64_t* v_off, const uint64_t* dest,
+                    size_t ndest, const uint64_t* par, const uint64_t* par_off, size_t npar, uint64_t* keys,
+                    uint64_t* grp_off, uint64_t* mem_off, size_t grp_cap, uint64_t* members, size_t mem_cap,
+                    size_t* ngroups, size_t* nmembers);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -566,6 +588,20 @@ int dgx_dev_trigram_query(dgx_lane* lane, const dgx_query_tree* tree, const dgx_
                           const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
                           const uint64_t* d_lists, const uint64_t* list_off, size_t nlists, uint64_t after_uid,
                           uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
+/* Device form of dgx_groupby_uid: every array in device memory, offsets included, so the rows of
+ * dgx_dev_list_uids_unfiltered_rows (and their dgx_dev_merge_sorted_matrix as d_dest) feed it directly.  v_cap and
+ * par_cap are the room of d_v and d_par (d_v_off[nrows] and d_par_off[npar] must not pass them); e_cap is the room for
+ * restricted edges the workspace holds (94 bytes each).  d_sizes is two device uint64: [ngroups, nmembers].  Sizes of
+ * 2^32 or more and missing pointers are DGX_ERR_ARG at the call; npar, nrows, v_cap or par_cap of 0 writes zero groups
+ * without a launch.  Every other check runs on the device and surfaces at the next dgx_lane_sync: a refused input
+ * writes d_sizes = {0, 0} and nothing else (DGX_ERR_ARG); an output that does not fit writes the exact d_sizes and
+ * nothing else (DGX_ERR_CAP); more than e_cap edges writes d_sizes = {0, edges} and nothing else (DGX_ERR_CAP).
+ * Asynchronous on the lane. */
+int dgx_dev_groupby_uid(dgx_lane* lane, const uint64_t* d_src, size_t nrows, const uint64_t* d_v,
+                        const uint64_t* d_v_off, size_t v_cap, const uint64_t* d_dest, size_t ndest,
+                        const uint64_t* d_par, const uint64_t* d_par_off, size_t npar, size_t par_cap, size_t e_cap,
+                        uint64_t* d_keys, uint64_t* d_grp_off, uint64_t* d_mem_off, size_t grp_cap,
+                        uint64_t* d_members, size_t mem_cap, uint64_t* d_sizes);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

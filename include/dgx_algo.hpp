@@ -252,6 +252,49 @@ inline pb::List UidsForRegex(const std::vector<QueryNode>& tree, const std::vect
     return out;
 }
 
+// One parent row's groups of a @groupby over a uid predicate, ordered by (count, key): group g has key keys[g],
+// count(uid) counts[g] and, unless counts only, the ascending source uids members[mem_off[g] .. mem_off[g+1]).
+struct ParentGroups {
+    std::vector<uint64_t> keys, counts, members, mem_off{0};
+};
+
+// formResult (query/groupby.go:208-221) for every parent row at once: one dgx_groupby_uid call, sized again from the
+// exact counts when the first guess (the number of row values) is short.
+inline std::vector<ParentGroups> GroupByUid(const std::vector<pb::List>& parents, const std::vector<uint64_t>& src,
+                                            const std::vector<pb::List>& rows, const std::vector<uint64_t>& dest,
+                                            bool withMembers = true) {
+    if (src.size() != rows.size()) throw Error(DGX_ERR_ARG, "one source per row");
+    std::vector<uint64_t> v, v_off{0}, par, par_off{0};
+    for (const pb::List& r : rows) { v.insert(v.end(), r.Uids.begin(), r.Uids.end()); v_off.push_back(v.size()); }
+    for (const pb::List& p : parents) { par.insert(par.end(), p.Uids.begin(), p.Uids.end()); par_off.push_back(par.size()); }
+    size_t gcap = v.size(), mcap = v.size(), ng = 0, nm = 0;
+    std::vector<uint64_t> keys, grp_off(parents.size() + 1), mem_off, mem;
+    int rc = DGX_OK;
+    for (int attempt = 0; attempt < 2; ++attempt) {
+        keys.assign(std::max<size_t>(gcap, 1), 0);
+        mem_off.assign(gcap + 1, 0);
+        mem.assign(withMembers ? std::max<size_t>(mcap, 1) : 0, 0);
+        rc = dgx_groupby_uid(src.data(), src.size(), v.data(), v_off.data(), dest.data(), dest.size(), par.data(),
+                             par_off.data(), parents.size(), keys.data(), grp_off.data(), mem_off.data(), gcap,
+                             withMembers ? mem.data() : nullptr, mcap, &ng, &nm);
+        if (rc != DGX_ERR_CAP) break;
+        gcap = ng;
+        mcap = nm;
+    }
+    check(rc);
+    std::vector<ParentGroups> out(parents.size());
+    for (size_t p = 0; p < parents.size(); ++p) {
+        ParentGroups& g = out[p];
+        for (uint64_t i = grp_off[p]; i < grp_off[p + 1]; ++i) {
+            g.keys.push_back(keys[i]);
+            g.counts.push_back(mem_off[i + 1] - mem_off[i]);
+            if (withMembers) g.members.insert(g.members.end(), mem.begin() + mem_off[i], mem.begin() + mem_off[i + 1]);
+            g.mem_off.push_back(g.mem_off.back() + g.counts.back());
+        }
+    }
+    return out;
+}
+
 }  // namespace algo
 
 // Wire-format adjacency (dgx_wire_*, host only): the bytes proto.Unmarshal sees at posting/list.go:1045 and

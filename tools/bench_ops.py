@@ -138,6 +138,7 @@ def main():
     ap.add_argument("--c10-only", action="store_true", help="only the C10 unfiltered List.Uids and count rows")
     ap.add_argument("--c11-only", action="store_true", help="only the C11 backup / restore codec rows")
     ap.add_argument("--c12-only", action="store_true", help="only the C12 regexp() trigram query rows")
+    ap.add_argument("--c13-only", action="store_true", help="only the C13 @groupby over a uid predicate rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -153,9 +154,11 @@ def main():
         rows = c11_rows(Lane())
     elif args.c12_only:
         rows = c12_rows(Lane())
+    elif args.c13_only:
+        rows = c13_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1396,6 +1399,115 @@ def c12_rows(L, threads: int = 16, n_nodes: int = 10_000_000):
             for h in handles:
                 lib.dgx_dev_pack_free(h)
     lib.dgx_cache_clear()
+    return out_rows
+
+
+
+def c13_rows(L, n_sample: int = 20):
+    """C13 "@groupby over a uid predicate": 1e6 source rows of about 20 values each after repeats are dropped (about 2e7
+    edges), destinations drawn Zipf-popular over 1e6 uids (tests/gen_groupby.py c13_rows).  C13a: one parent holding
+    every source (fillGroupedVars, or a @groupby at the root).  C13b: 10 000 parents of about 100 sources each.  Legs:
+    (1) the device form on resident inputs with members and (2) counts only (CUDA events), (3) the host form (wall
+    clock), (4) the line-by-line restatement (tests/groupby_oracle.c) on 1 thread as a stand-in for today's Go path --
+    it is C, not Go.  C13a is checked in full against the restatement.  The restatement loops over every source row for
+    every parent (formResult's IndexOf per child row), about 1e10 searches for C13b: there it runs on the first
+    n_sample parents only, its time is per parent, and those parents' groups are checked against it; the device and
+    host forms must agree in full."""
+    import gen_groupby as gg
+    import groupby_oracle as gbo
+
+    lib = L.lib
+    rng = np.random.default_rng(13)
+    src, v, v_off, dest = gg.c13_rows(rng)
+    nrows, m = src.size, int(v_off[-1])
+    parents_b = [src[np.unique(rng.integers(0, nrows, int(rng.integers(50, 151))))] for _ in range(10_000)]
+    work = {"C13a": [src], "C13b": parents_b}
+    out_rows = []
+
+    def dp(t):
+        return C.c_void_p(t.data_ptr())
+
+    def up(x):
+        return torch.from_numpy(np.ascontiguousarray(x).view(np.int64)).to(DEV)
+
+    d_src, d_v, d_voff, d_dest = up(src), up(v), up(v_off), up(dest)
+    for name, parents in work.items():
+        par, par_off = gbo.csr(parents)
+        npar, pv = len(parents), int(par_off[-1])
+        # the restatement (all parents for C13a, a sample for C13b)
+        samp = parents if name == "C13a" else parents[:n_sample]
+        lens = np.diff(v_off.astype(np.int64))
+        scap = max(sum(int(lens[np.isin(src, pr)].sum()) for pr in samp), 1)  # the sample's edges
+        skeys, sagg, smem = (np.empty(scap, np.uint64) for _ in range(3))
+        sgrp, smoff = np.empty(len(samp) + 1, np.uint64), np.empty(scap + 1, np.uint64)
+        spar, spar_off = gbo.csr(samp)
+
+        def oracle():
+            return gbo.lib().orc_groupby_uid(src.ctypes.data, nrows, v.ctypes.data, v_off.ctypes.data, spar.ctypes.data,
+                                             spar_off.ctypes.data, len(samp), skeys.ctypes.data, sagg.ctypes.data,
+                                             sgrp.ctypes.data, smoff.ctypes.data, smem.ctypes.data)
+        t0 = time.perf_counter()
+        ng_o = oracle()
+        t_or = (time.perf_counter() - t0) * 1e3
+        # the host form, sized from a first counts-only call
+        grp_off = np.empty(npar + 1, np.uint64)
+        ng, nm = C.c_size_t(), C.c_size_t()
+        probe = np.empty(1, np.uint64)
+        rc = lib.dgx_groupby_uid(_p_(src), nrows, _p_(v), _p_(v_off), _p_(dest), dest.size, _p_(par), _p_(par_off), npar,
+                                 _p_(probe), _p_(grp_off), _p_(probe), 0, None, 0, C.byref(ng), C.byref(nm))
+        assert rc in (0, -4), rc
+        G, E = ng.value, nm.value
+        keys, mem_off, mem = np.empty(G, np.uint64), np.empty(G + 1, np.uint64), np.empty(E, np.uint64)
+
+        def host():
+            _lib.check(lib.dgx_groupby_uid(_p_(src), nrows, _p_(v), _p_(v_off), _p_(dest), dest.size, _p_(par),
+                                           _p_(par_off), npar, _p_(keys), _p_(grp_off), _p_(mem_off), G, _p_(mem), E,
+                                           C.byref(ng), C.byref(nm)))
+        host()
+        t0 = time.perf_counter()
+        for _ in range(3):
+            host()
+        t_host = (time.perf_counter() - t0) * 1e3 / 3
+        # the device form, resident inputs
+        d_par, d_poff = up(par), up(par_off)
+        d_keys, d_grp = torch.empty(G + 1, dtype=torch.int64, device=DEV), torch.empty(npar + 1, dtype=torch.int64, device=DEV)
+        d_moff, d_mem = torch.empty(G + 1, dtype=torch.int64, device=DEV), torch.empty(E + 1, dtype=torch.int64, device=DEV)
+        d_sizes = torch.zeros(2, dtype=torch.int64, device=DEV)
+
+        def dev(with_members):
+            _lib.check(lib.dgx_dev_groupby_uid(L.h, dp(d_src), nrows, dp(d_v), dp(d_voff), m, dp(d_dest), dest.size,
+                                               dp(d_par), dp(d_poff), npar, pv, E, dp(d_keys), dp(d_grp), dp(d_moff), G,
+                                               dp(d_mem) if with_members else None, E, dp(d_sizes)))
+        ms_cnt, _ = timeit(lambda: dev(False), warm=2, reps=10)
+        L.sync()
+        ok_cnt = (np.array_equal(d_keys[:G].cpu().numpy().view(np.uint64), keys)
+                  and np.array_equal(d_moff[:G + 1].cpu().numpy().view(np.uint64), mem_off))
+        ms_mem, _ = timeit(lambda: dev(True), warm=2, reps=10)
+        L.sync()
+        ok_dev = (np.array_equal(d_keys[:G].cpu().numpy().view(np.uint64), keys)
+                  and np.array_equal(d_grp.cpu().numpy().view(np.uint64), grp_off)
+                  and np.array_equal(d_moff[:G + 1].cpu().numpy().view(np.uint64), mem_off)
+                  and np.array_equal(d_mem[:E].cpu().numpy().view(np.uint64), mem)
+                  and tuple(d_sizes.cpu().numpy()) == (G, E))
+        # the restatement's groups against the library's, parent by parent
+        k = len(samp)
+        g_end = int(grp_off[k])
+        ok_or = (ng_o == g_end and np.array_equal(skeys[:ng_o], keys[:g_end])
+                 and np.array_equal(sgrp[:k + 1], grp_off[:k + 1])
+                 and np.array_equal(smoff[:ng_o + 1], mem_off[:g_end + 1])
+                 and np.array_equal(smem[:int(smoff[ng_o])], mem[:int(mem_off[g_end])]))
+        cfg = (f"{name}: {npar} parent(s) ({pv} parent values), {nrows} source rows, {m} row values over {dest.size} "
+               f"destinations; {E} restricted edges in {G} groups")
+        legs = [("device form, resident, members", ms_mem, ok_dev and ok_or, "dgx_dev_groupby_uid, CUDA events"),
+                ("device form, resident, counts only", ms_cnt, ok_cnt and ok_or, "dgx_dev_groupby_uid, CUDA events"),
+                ("host form, members", t_host, ok_or, "dgx_groupby_uid, wall clock, mean of 3 after one warm call"),
+                (f"restatement, 1 thread (C, not Go){'' if name == 'C13a' else f', {k} parents'}", t_or, ok_or,
+                 "tests/groupby_oracle.c, wall clock, one call" + ("" if name == "C13a" else
+                                                                   f"; per parent {t_or / k:.1f} ms"))]
+        for leg, ms, ok, how in legs:
+            out_rows.append({"op": "GroupByUid", "workload": name, "leg": leg, "config": cfg, "ms": round(ms, 4),
+                             "edges": E, "groups": G, "check": bool(ok), "timing": how})
+            print(json.dumps(out_rows[-1]), flush=True)
     return out_rows
 
 
