@@ -85,6 +85,11 @@ SYMBOLS = {
     "dgx_decode_to_buffer_rows": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _sz]),
     "dgx_encode_from_buffer_rows": (_int, [_vp, _vp, _sz, C.c_uint32, _vp, _sz, _vp, _vp, _vp]),
     "dgx_trigram_query": (_int, [C.POINTER(QueryTree), C.POINTER(PackRef), _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _szp]),
+    "dgx_reach_create": (_int, [_vp, _vp, _sz, C.POINTER(_vp)]),
+    "dgx_reach_destroy": (None, [_vp]),
+    "dgx_reach_size": (_int, [_vp, _szp]),
+    "dgx_reach_export": (_int, [_vp, _vp, _vp, _sz, _szp]),
+    "dgx_recurse_filter": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _szp]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
     "dgx_encode_bound": (None, [_sz, C.c_uint32, _szp, _szp]),
@@ -126,6 +131,7 @@ SYMBOLS = {
     "dgx_dev_list_uids_unfiltered_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, C.c_int32, _vp, _sz, _vp]),
     "dgx_dev_list_count_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, _vp]),
     "dgx_dev_trigram_query": (_int, [_vp, C.POINTER(QueryTree), _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _vp]),
+    "dgx_dev_recurse_filter": (_int, [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),
     "dgx_filter_tail_queries": (_u64, [_vp]),

@@ -441,6 +441,93 @@ def GroupByUid(parents, src, rows, dest, members: bool = True):
     return out
 
 
+class ReachSet:
+    """The edges one sg.Attr has taken during one @recurse (query/recurse.go expandRecurse's reachMap, loop: false),
+    kept in device memory (dgx_reach_set).  One set per distinct Attr, for the life of one recursion."""
+
+    def __init__(self):
+        self._set = None
+        self._open(np.zeros(1, np.uint64), np.zeros(1, np.uint64), 0)
+
+    def _open(self, f, t, n):
+        h = C.c_void_p()
+        _lib.check(_lib.load().dgx_reach_create(_p(f), _p(t), n, C.byref(h)))
+        self._set = h
+
+    @classmethod
+    def from_edges(cls, frm, to) -> "ReachSet":
+        """A set holding the edges (frm[k], to[k]), strictly ascending by (from, to): how a recursion started on the
+        host continues on the device."""
+        f, t = _u64(frm), _u64(to)
+        if f.size != t.size:
+            raise ValueError(f"{f.size} from values for {t.size} to values")
+        s = cls.__new__(cls)
+        s._set = None
+        s._open(f if f.size else np.zeros(1, np.uint64), t if t.size else np.zeros(1, np.uint64), f.size)
+        return s
+
+    @property
+    def handle(self):
+        """The dgx_reach_set pointer, for dgx_dev_recurse_filter."""
+        if self._set is None:
+            raise ValueError("ReachSet is closed")
+        return self._set
+
+    def filter(self, src, rows, dest=None):
+        """One sg of one level (:105-134): rows[i] (strictly ascending) belongs to src[i] (strictly ascending).  dest
+        (sg.DestUIDs after its filters) or None when the sg has no filters.  Returns (kept rows, DestUIDs, kept), and
+        the kept edges join the set."""
+        v, v_off = _csr_u64(rows)
+        src_a = _u64(src.Uids if isinstance(src, List) else src)
+        if src_a.size != len(rows):
+            raise ValueError(f"{src_a.size} sources for {len(rows)} rows")
+        d = None if dest is None else _u64(dest.Uids if isinstance(dest, List) else dest)
+        m = int(v_off[-1])
+        out, dest_out = np.empty(max(m, 1), np.uint64), np.empty(max(m, 1), np.uint64)
+        out_off = np.zeros(len(rows) + 1, np.uint64)
+        n = C.c_size_t(0)
+        if src_a.size == 0:
+            src_a = np.zeros(1, np.uint64)
+        if d is not None and d.size == 0:
+            d = np.zeros(1, np.uint64)
+        nd = 0 if dest is None else int(np.size(dest.Uids if isinstance(dest, List) else dest))
+        _lib.check(_lib.load().dgx_recurse_filter(self.handle, _p(src_a), len(rows), _p(v), _p(v_off),
+                                                  None if d is None else _p(d), nd, _p(out), _p(out_off), m,
+                                                  _p(dest_out), m, C.byref(n)))
+        kept = [out[int(out_off[i]):int(out_off[i + 1])].copy() for i in range(len(rows))]
+        return kept, List(dest_out[: n.value].copy()), int(out_off[-1])
+
+    def size(self) -> int:
+        n = C.c_size_t(0)
+        _lib.check(_lib.load().dgx_reach_size(self.handle, C.byref(n)))
+        return n.value
+
+    def export(self):
+        """(from, to) of every edge, ascending: how a recursion hands back to the host."""
+        n = self.size()
+        f, t = np.empty(max(n, 1), np.uint64), np.empty(max(n, 1), np.uint64)
+        got = C.c_size_t(0)
+        _lib.check(_lib.load().dgx_reach_export(self.handle, _p(f), _p(t), n, C.byref(got)))
+        return f[: got.value].copy(), t[: got.value].copy()
+
+    def close(self) -> None:
+        if self._set is not None:
+            _lib.load().dgx_reach_destroy(self._set)
+            self._set = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -40,6 +40,7 @@
 #include "backup_codec_kernel.cuh"
 #include "trigram_kernel.cuh"
 #include "groupby_kernel.cuh"
+#include "recurse_kernel.cuh"
 #include "wire.hpp"
 
 using namespace dgx;
@@ -458,6 +459,9 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
             return fail(DGX_ERR_ARG, "a groupby input is malformed (src, a row, a parent row or dest not strictly "
                                      "ascending, offsets not starting at 0, decreasing or past their arrays, a row "
                                      "value missing from dest, or 2^32 restricted edges or more)");
+        if (flag & kLaneErrRecurse)
+            return fail(DGX_ERR_ARG, "a recurse step's input is malformed (src, a row or dest not strictly ascending, "
+                                     "or offsets not starting at 0, decreasing or past v_cap)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -3741,6 +3745,300 @@ extern "C" int dgx_groupby_uid(const uint64_t* src, size_t nrows, const uint64_t
     CK(cudaStreamSynchronize(l->stream));
     g_stats.d2h += (2 * G + npar + 2 + (members ? E : 0)) * sizeof(uint64_t);
     g_stats.uids_out += members ? E : G;
+    return DGX_OK;
+}
+
+// ---------------------------------------------------------------------------
+// @recurse: each sg's uid matrix filtered against the edges already taken, in HBM (recurse_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr uint64_t kRcMax = uint64_t(1) << 32;  // rows, values and set sizes are 32-bit counts
+
+// Buffer b holds from[] at buf[b] and to[] at buf[b] + cap.  Which buffer is current, and the size, are device words
+// (d_state) that queued steps update; size / cur mirror them as of the last wait, and bound is the size then plus the
+// v_cap of every step queued since, which sizes the capacity without a round trip.
+struct dgx_reach_set {
+    std::mutex mu;
+    int device = 0;
+    uint64_t* buf[2] = {nullptr, nullptr};
+    uint64_t cap = 0;
+    uint64_t* d_state = nullptr;  // [current buffer, size]
+    uint64_t size = 0, cur = 0, bound = 0;
+    dgx_lane* lane = nullptr;     // the lane of the device-form steps queued since the last wait
+    std::vector<void*> retired;   // buffers replaced by growth, still read by queued steps until the next wait
+};
+
+static void rc_free_retired(dgx_reach_set* s) {
+    for (void* p : s->retired) cudaFree(p);
+    s->retired.clear();
+}
+
+// Waits for the set's queued steps and reads its words back.  Caller holds s->mu.
+static int rc_wait(dgx_reach_set* s) {
+    CK(cudaSetDevice(s->device));
+    if (!s->lane) return DGX_OK;
+    uint64_t st[2];
+    CK(cudaMemcpyAsync(st, s->d_state, sizeof(st), cudaMemcpyDeviceToHost, s->lane->stream));
+    CK(cudaStreamSynchronize(s->lane->stream));
+    s->cur = st[0];
+    s->size = s->bound = st[1];
+    s->lane = nullptr;
+    rc_free_retired(s);
+    return DGX_OK;
+}
+
+// Capacity for `need` edges: both buffers grow geometrically, their first `bound` records copied on the stream (the
+// current buffer is only known on the device).  The new buffers replace the old ones only once every copy is queued,
+// so an allocation or a copy that fails leaves the set as it was.
+static int rc_reserve(dgx_reach_set* s, cudaStream_t stream, uint64_t need) {
+    if (need <= s->cap) return DGX_OK;
+    const uint64_t ncap = std::max(need, 2 * s->cap);
+    uint64_t* nb[2] = {nullptr, nullptr};
+    auto drop = [&](int code, const char* what) {
+        cudaGetLastError();
+        for (uint64_t* p : nb) if (p) cudaFree(p);
+        return fail(code, "reach set growth to %llu edges: %s failed", (unsigned long long)ncap, what);
+    };
+    for (int b = 0; b < 2; ++b)
+        if (cudaMalloc(&nb[b], 2 * ncap * sizeof(uint64_t)) != cudaSuccess) return drop(DGX_ERR_OOM, "cudaMalloc");
+    for (int b = 0; b < 2; ++b)
+        if (s->bound && (s->lane || (uint64_t)b == s->cur)) {  // an idle set's other buffer holds nothing live
+            const size_t bytes = s->bound * sizeof(uint64_t);
+            if (cudaMemcpyAsync(nb[b], s->buf[b], bytes, cudaMemcpyDeviceToDevice, stream) != cudaSuccess ||
+                cudaMemcpyAsync(nb[b] + ncap, s->buf[b] + s->cap, bytes, cudaMemcpyDeviceToDevice, stream) != cudaSuccess) {
+                if (stream) cudaStreamSynchronize(stream);  // copies already queued read and write nb
+                return drop(DGX_ERR_CUDA, "cudaMemcpyAsync");
+            }
+        }
+    for (int b = 0; b < 2; ++b) {
+        if (s->buf[b]) s->retired.push_back(s->buf[b]);
+        s->buf[b] = nb[b];
+    }
+    s->cap = ncap;
+    return DGX_OK;
+}
+
+extern "C" int dgx_reach_create(const uint64_t* from, const uint64_t* to, size_t n, dgx_reach_set** set) {
+    if (!set || (n && (!from || !to))) return fail(DGX_ERR_ARG, "null argument");
+    if (n >= kRcMax) return fail(DGX_ERR_ARG, "%zu edges: a reach set holds at most 2^32 - 1", n);
+    for (size_t k = 1; k < n; ++k)
+        if (from[k - 1] > from[k] || (from[k - 1] == from[k] && to[k - 1] >= to[k]))
+            return fail(DGX_ERR_ARG, "edge %zu does not strictly ascend by (from, to)", k);
+    if (int rc = dgx_init(-1)) return rc;
+    CK(cudaSetDevice(g_device));
+    dgx_reach_set* s = new dgx_reach_set();
+    s->device = g_device;
+    int rc = DGX_OK;
+    if (cudaMalloc(&s->d_state, 2 * sizeof(uint64_t)) != cudaSuccess) rc = fail(DGX_ERR_OOM, "reach set allocation failed");
+    if (!rc) rc = rc_reserve(s, nullptr, std::max<uint64_t>(n, 1024));
+    const uint64_t st[2] = {0, n};
+    if (!rc && n &&
+        (cudaMemcpy(s->buf[0], from, n * sizeof(uint64_t), cudaMemcpyHostToDevice) != cudaSuccess ||
+         cudaMemcpy(s->buf[0] + s->cap, to, n * sizeof(uint64_t), cudaMemcpyHostToDevice) != cudaSuccess))
+        rc = fail(DGX_ERR_CUDA, "reach set upload failed");
+    if (!rc && cudaMemcpy(s->d_state, st, sizeof(st), cudaMemcpyHostToDevice) != cudaSuccess)
+        rc = fail(DGX_ERR_CUDA, "reach set upload failed");
+    rc_free_retired(s);
+    s->size = s->bound = n;
+    if (rc) {
+        dgx_reach_destroy(s);
+        return rc;
+    }
+    g_stats.h2d += 2 * n * sizeof(uint64_t);
+    *set = s;
+    return DGX_OK;
+}
+
+extern "C" void dgx_reach_destroy(dgx_reach_set* s) {
+    if (!s) return;
+    {
+        std::lock_guard<std::mutex> lk(s->mu);
+        rc_wait(s);
+        rc_free_retired(s);
+        for (uint64_t* b : s->buf) if (b) cudaFree(b);
+        if (s->d_state) cudaFree(s->d_state);
+    }
+    delete s;
+}
+
+extern "C" int dgx_reach_size(dgx_reach_set* s, size_t* n) {
+    if (!s || !n) return fail(DGX_ERR_ARG, "null argument");
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (int rc = rc_wait(s)) return rc;
+    *n = s->size;
+    return DGX_OK;
+}
+
+extern "C" int dgx_reach_export(dgx_reach_set* s, uint64_t* from, uint64_t* to, size_t cap, size_t* n) {
+    if (!s || !n) return fail(DGX_ERR_ARG, "null argument");
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (int rc = rc_wait(s)) return rc;
+    *n = s->size;
+    if (s->size > cap) return fail(DGX_ERR_CAP, "%llu edges do not fit cap %zu", (unsigned long long)s->size, cap);
+    if (s->size && (!from || !to)) return fail(DGX_ERR_ARG, "null argument");
+    if (s->size) {
+        CK(cudaMemcpy(from, s->buf[s->cur], s->size * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(to, s->buf[s->cur] + s->cap, s->size * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    }
+    g_stats.d2h += 2 * s->size * sizeof(uint64_t);
+    return DGX_OK;
+}
+
+// One step on the lane, for a set with room for bound + v_cap edges: 5 launches, the matrix merge's, 2 launches.
+// Workspace: 28 bytes per value of v_cap (row 4, keep flag 8, its scan 8, kept from 8), 24 per row (slice bounds 16,
+// the merge's offsets 8), the merge's about 22 per value, and the scan's look-back words.  d_out_off and d_sizes are
+// written by the kernels.
+static int rc_step(dgx_lane* l, dgx_reach_set* s, const uint64_t* d_src, size_t nrows, const uint64_t* d_v,
+                   const uint64_t* d_v_off, uint64_t v_cap, const uint64_t* d_dest, size_t ndest, uint64_t* d_out,
+                   uint64_t* d_out_off, uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_sizes) {
+    const uint64_t tiles = (v_cap + EN_TILE - 1) / EN_TILE;
+    // zeroed: [bad | words | ticket | scan status];  then lo, hi, w_off, keep, kex, kfrom, row
+    const size_t b_zero = 64 + tiles * sizeof(u64);
+    const size_t n64 = 2 * nrows + (nrows + 1) + v_cap + (v_cap + 1) + v_cap;
+    void* d_raw;
+    int rc = l->ws.alloc(b_zero + n64 * sizeof(u64) + v_cap * sizeof(u32), &d_raw);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(d_raw, 0, b_zero, l->stream));
+    RcParams P;
+    P.src = (const u64*)d_src;
+    P.nrows = nrows;
+    P.v = (const u64*)d_v;
+    P.v_off = (const u64*)d_v_off;
+    P.v_cap = v_cap;
+    P.dest = (const u64*)d_dest;
+    P.ndest = d_dest ? ndest : 0;
+    for (int b = 0; b < 2; ++b) {
+        P.sfrom[b] = (u64*)s->buf[b];
+        P.sto[b] = (u64*)s->buf[b] + s->cap;
+    }
+    P.state = (u64*)s->d_state;
+    P.bad = (int*)d_raw;
+    P.words = (u64*)((char*)d_raw + 16);
+    u32* ticket = (u32*)(P.words + RC_WORDS);
+    u64* status = (u64*)((char*)d_raw + 64);
+    P.lo = (u64*)((char*)d_raw + b_zero);
+    P.hi = P.lo + nrows;
+    P.w_off = P.hi + nrows;
+    P.keep = P.w_off + nrows + 1;
+    P.kex = P.keep + v_cap;
+    P.kfrom = P.kex + v_cap + 1;
+    P.row = (u32*)(P.kfrom + v_cap);
+    P.out = (u64*)d_out;
+    P.out_off = (u64*)d_out_off;
+    P.sizes = (u64*)d_sizes;
+    P.err = l->d_err;
+    const uint64_t nt = std::max<uint64_t>(std::max<uint64_t>(nrows + 1, v_cap), P.ndest);
+    rc_check_kernel<<<gb_grid(nt), 256, 0, l->stream>>>(P);
+    rc_locate_kernel<<<gb_grid(nrows), 256, 0, l->stream>>>(P);
+    rc_flags_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)tiles, EN_NT, 0, l->stream>>>(P.keep, P.kex, P.words + RC_W_M, v_cap, status, ticket,
+                                                                P.words + RC_W_K);
+    rc_gather_kernel<<<gb_grid(std::max<uint64_t>(v_cap, nrows + 1)), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 5);
+    if ((rc = merge_matrix_impl(l, d_out, (const uint64_t*)P.w_off, nrows, v_cap, d_dest_out, dest_cap,
+                                (uint64_t*)(P.words + RC_W_D))))
+        return rc;
+    rc_insert_kernel<<<stride_grid(), 256, 0, l->stream>>>(P);
+    rc_commit_kernel<<<1, 1, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 2);
+    return DGX_OK;
+}
+
+// The checks both forms make before anything is copied.  Caller holds s->mu.
+static int rc_check_step(dgx_reach_set* s, const dgx_lane* l, size_t nrows, uint64_t m, size_t out_cap,
+                         size_t dest_cap) {
+    if (s->lane && s->lane != l)
+        return fail(DGX_ERR_ARG, "the reach set has steps queued on another lane: wait for them with dgx_reach_size");
+    if (nrows >= kRcMax || m >= kRcMax) return fail(DGX_ERR_ARG, "recurse sizes are 32-bit: nrows and values below 2^32");
+    if (s->bound + m >= kRcMax)
+        return fail(DGX_ERR_ARG, "the reach set could reach %llu edges: at most 2^32 - 1",
+                    (unsigned long long)(s->bound + m));
+    if (out_cap < m || dest_cap < m)
+        return fail(DGX_ERR_CAP, "out_cap %zu / dest_cap %zu below the %llu values", out_cap, dest_cap,
+                    (unsigned long long)m);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_recurse_filter(dgx_lane* l, dgx_reach_set* s, const uint64_t* d_src, size_t nrows,
+                                      const uint64_t* d_v, const uint64_t* d_v_off, size_t v_cap,
+                                      const uint64_t* d_dest, size_t ndest, uint64_t* d_out, uint64_t* d_out_off,
+                                      size_t out_cap, uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_sizes) {
+    if (!l || !s || !d_sizes || !d_out_off) return fail(DGX_ERR_ARG, "null argument");
+    if (nrows && v_cap && (!d_src || !d_v || !d_v_off || !d_out || !d_dest_out))
+        return fail(DGX_ERR_ARG, "null argument");
+    if (d_dest && ndest >= kRcMax) return fail(DGX_ERR_ARG, "ndest of %zu: at most 2^32 - 1", ndest);
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (int rc = rc_check_step(s, l, nrows, v_cap, out_cap, dest_cap)) return rc;
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    l->note_output(d_sizes, 2 * sizeof(uint64_t));
+    if (nrows == 0 || v_cap == 0) {  // no edge: nothing is kept
+        CK(cudaMemsetAsync(d_out_off, 0, (nrows + 1) * sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_sizes, 0, 2 * sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = rc_reserve(s, l->stream, s->bound + v_cap)) return rc;
+    s->lane = l;  // queued copies or steps now read the set
+    s->bound += v_cap;
+    if (int rc = rc_step(l, s, d_src, nrows, d_v, d_v_off, v_cap, d_dest, ndest, d_out, d_out_off, d_dest_out,
+                         dest_cap, d_sizes))
+        return rc;
+    g_stats.uids_in += v_cap;
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_dest_out, dest_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_recurse_filter(dgx_reach_set* s, const uint64_t* src, size_t nrows, const uint64_t* v,
+                                  const uint64_t* v_off, const uint64_t* dest, size_t ndest, uint64_t* out,
+                                  uint64_t* out_off, size_t out_cap, uint64_t* dest_out, size_t dest_cap,
+                                  size_t* dest_len) {
+    if (!s || !out_off || !dest_len || (nrows && !v_off)) return fail(DGX_ERR_ARG, "null argument");
+    if (nrows >= kRcMax) return fail(DGX_ERR_ARG, "recurse sizes are 32-bit: nrows below 2^32");
+    if (nrows) if (int rc = check_offsets("v_off", v_off, nrows, kRcMax)) return rc;
+    const uint64_t m = nrows ? v_off[nrows] : 0;
+    if (m && (!src || !v || !out || !dest_out)) return fail(DGX_ERR_ARG, "null argument");
+    if (dest && ndest >= kRcMax) return fail(DGX_ERR_ARG, "ndest of %zu: at most 2^32 - 1", ndest);
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (int rc = rc_check_step(s, nullptr, nrows, m, out_cap, dest_cap)) return rc;
+    if (m == 0) {
+        memset(out_off, 0, (nrows + 1) * sizeof(uint64_t));
+        *dest_len = 0;
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += nrows + m + (dest ? ndest : 0);
+    uint64_t *d_src, *d_v, *d_v_off, *d_dest = nullptr;
+    int rc;
+    if ((rc = upload_list(l, src, nrows, &d_src)) || (rc = upload_list(l, v, m, &d_v)) ||
+        (rc = upload_list(l, v_off, nrows + 1, &d_v_off)) || (dest && (rc = upload_list(l, dest, ndest, &d_dest))))
+        return rc;
+    void* d_o;
+    if ((rc = l->ws.alloc((2 * m + nrows + 3) * sizeof(uint64_t), &d_o))) return rc;
+    uint64_t* d_sizes = (uint64_t*)d_o;
+    uint64_t* d_out = d_sizes + 2;
+    uint64_t* d_dest_out = d_out + m;
+    uint64_t* d_off = d_dest_out + m;
+    if ((rc = rc_reserve(s, l->stream, s->bound + m))) return rc;
+    s->lane = l;  // waited for below, whatever happens
+    s->bound += m;
+    rc = rc_step(l, s, d_src, nrows, d_v, d_v_off, m, d_dest, ndest, d_out, d_off, d_dest_out, m, d_sizes);
+    if (!rc) CK(cudaMemcpyAsync(l->h_word, d_sizes, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (int wrc = rc_wait(s)) return wrc;
+    if (rc || (rc = dgx_lane_sync(l))) return rc;
+    const uint64_t K = l->h_word[0], D = l->h_word[1];
+    CK(cudaMemcpyAsync(out_off, d_off, (nrows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (K) CK(cudaMemcpyAsync(out, d_out, K * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (D) CK(cudaMemcpyAsync(dest_out, d_dest_out, D * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    *dest_len = D;
+    g_stats.d2h += (K + D + nrows + 3) * sizeof(uint64_t);
+    g_stats.uids_out += K + D;
     return DGX_OK;
 }
 

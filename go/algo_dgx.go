@@ -21,6 +21,7 @@ import "C"
 
 import (
 	"runtime"
+	"sort"
 	"unsafe"
 
 	"github.com/dgraph-io/dgraph/v25/protos/pb"
@@ -334,4 +335,106 @@ func GroupByUid(parents []*pb.List, srcUIDs []uint64, matrix []*pb.List, dest []
 		out[p] = gs
 	}
 	return out, true
+}
+
+// dgxMinRecurse: an expandRecurse attr moves its taken edges to the device once one sg's matrix of that attr reaches
+// this many values; below it the Go map stays.  From the C14 record (profiles/h100_c14_recurse.json, H100 80GB HBM3,
+// 700 W): a device-form step costs about 0.46 ms at C14b's sizes, and the C restatement of the Go loop spends 0.09-0.11
+// us per value, so the two meet near 5 000 values.  The restatement is C with a hash set, not Go with Sprintf keys,
+// which is slower, so the bound errs towards the Go path.
+const dgxMinRecurse = 1 << 13
+
+// Edge is one key of expandRecurse's reachMap for one attr: (fromUID, toUID).
+type Edge struct{ From, To uint64 }
+
+// ReachSet holds the edges one sg.Attr has taken during one @recurse (query/recurse.go expandRecurse, loop: false) in
+// device memory.  Keep one per distinct Attr for the life of one expandRecurse; Close it when the recursion ends.
+type ReachSet struct{ s *C.dgx_reach_set }
+
+// NewReachSet creates a set from the edges Go has taken so far (any order; they are sorted here).  It returns false
+// when the library refuses them (2^32 edges or more, no device); the caller keeps its map.
+func NewReachSet(edges []Edge) (*ReachSet, bool) {
+	sorted := append([]Edge(nil), edges...)
+	sortEdges(sorted)
+	from, to := make([]uint64, len(sorted)), make([]uint64, len(sorted))
+	for i, e := range sorted {
+		from[i], to[i] = e.From, e.To
+	}
+	var s *C.dgx_reach_set
+	if C.dgx_reach_create(u64ptr(from), u64ptr(to), C.size_t(len(from)), &s) != C.DGX_OK {
+		return nil, false
+	}
+	return &ReachSet{s: s}, true
+}
+
+func sortEdges(e []Edge) {
+	sort.Slice(e, func(i, j int) bool { return e[i].From < e[j].From || (e[i].From == e[j].From && e[i].To < e[j].To) })
+}
+
+// Filter is :106-134 for one sg: with dest != nil (the sg has filters) every row is first intersected with dest
+// (updateUidMatrix), then every edge already in the set is dropped and the rest are added.  It returns the kept rows
+// (the new sg.uidMatrix), sg.DestUIDs and the step's contribution to numEdges.  ok == false, on any library error,
+// means nothing was written and the set is unchanged: the caller exports it and finishes the attr in Go.
+func (r *ReachSet) Filter(src *pb.List, matrix []*pb.List, dest *pb.List) (rows []*pb.List, destUIDs *pb.List,
+	kept uint64, ok bool) {
+	n, m := len(matrix), totalUids(matrix)
+	if n != len(src.Uids) {
+		return nil, nil, 0, false
+	}
+	// every slice handed to C is its own Go allocation holding no Go pointers
+	vOff, v := make([]uint64, n+1), make([]uint64, 0, m)
+	for i, l := range matrix {
+		vOff[i] = uint64(len(v))
+		if l != nil {
+			v = append(v, l.Uids...)
+		}
+	}
+	vOff[n] = uint64(len(v))
+	srcs := append([]uint64(nil), src.Uids...)
+	var dst []uint64
+	var dstPtr *C.uint64_t
+	var nd int
+	if dest != nil {
+		dst = append(make([]uint64, 0, len(dest.Uids)+1), dest.Uids...)
+		dstPtr, nd = (*C.uint64_t)(unsafe.Pointer(&dst[:1][0])), len(dest.Uids)
+	}
+	out, outOff, dOut := make([]uint64, m+1), make([]uint64, n+1), make([]uint64, m+1)
+	var dLen C.size_t
+	rc := C.dgx_recurse_filter(r.s, u64ptr(srcs), C.size_t(n), u64ptr(v), u64ptr(vOff), dstPtr, C.size_t(nd),
+		u64ptr(out), u64ptr(outOff), C.size_t(m), u64ptr(dOut), C.size_t(m), &dLen)
+	if rc != C.DGX_OK {
+		return nil, nil, 0, false
+	}
+	rows = make([]*pb.List, n)
+	for i := range rows {
+		lo, hi := outOff[i], outOff[i+1]
+		rows[i] = &pb.List{Uids: out[lo:hi:hi]}
+	}
+	return rows, &pb.List{Uids: dOut[:dLen:dLen]}, outOff[n], true
+}
+
+// Export returns the set's edges, ascending by (From, To): how a recursion hands back to the Go map.
+func (r *ReachSet) Export() ([]Edge, bool) {
+	var n C.size_t
+	if C.dgx_reach_size(r.s, &n) != C.DGX_OK {
+		return nil, false
+	}
+	from, to := make([]uint64, int(n)+1), make([]uint64, int(n)+1)
+	var got C.size_t
+	if C.dgx_reach_export(r.s, u64ptr(from), u64ptr(to), n, &got) != C.DGX_OK {
+		return nil, false
+	}
+	e := make([]Edge, int(got))
+	for i := range e {
+		e[i] = Edge{From: from[i], To: to[i]}
+	}
+	return e, true
+}
+
+// Close frees the set's device memory.
+func (r *ReachSet) Close() {
+	if r.s != nil {
+		C.dgx_reach_destroy(r.s)
+		r.s = nil
+	}
 }

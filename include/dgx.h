@@ -387,6 +387,36 @@ int dgx_groupby_uid(const uint64_t* src, size_t nrows, const uint64_t* v, const 
                     uint64_t* grp_off, uint64_t* mem_off, size_t grp_cap, uint64_t* members, size_t mem_cap,
                     size_t* ngroups, size_t* nmembers);
 
+/* @recurse with loop: false (query/recurse.go expandRecurse :96-135): the edges one sg.Attr has taken so far, kept in
+ * device memory for the life of one recursion.  An edge is (from, to) with from = sg.SrcUIDs[i] and to a value of row
+ * i.  Calls on one set are serialised by the library; different sets may be used concurrently.  A set that a
+ * device-form step bound to a lane must be waited for (dgx_reach_size / dgx_reach_export) or destroyed before that
+ * lane is destroyed: the set refers to the lane's stream until then. */
+typedef struct dgx_reach_set dgx_reach_set;
+/* A set holding the n edges (from[k], to[k]), which strictly ascend by (from, to); n == 0 makes an empty set.
+ * DGX_ERR_ARG: n of 2^32 or more, a null array with n > 0, edges that do not strictly ascend. */
+int dgx_reach_create(const uint64_t* from, const uint64_t* to, size_t n, dgx_reach_set** set);
+void dgx_reach_destroy(dgx_reach_set* set);
+/* The exact edge count; waits for the device-form steps queued on the set. */
+int dgx_reach_size(dgx_reach_set* set, size_t* n);
+/* The edges, ascending by (from, to), into from / to (room for cap each); *n gets the count.  Waits like
+ * dgx_reach_size.  DGX_ERR_CAP with *n set and nothing written when the count exceeds cap. */
+int dgx_reach_export(dgx_reach_set* set, uint64_t* from, uint64_t* to, size_t cap, size_t* n);
+/* One sg of one level: row i (v[v_off[i] .. v_off[i+1]), strictly ascending) belongs to src[i] (strictly ascending).
+ * dest == NULL: the sg has no filters; otherwise (strictly ascending, ndest values) updateUidMatrix first drops every
+ * value not in dest.  Then every edge already in the set is dropped and the rest are added to it.  out / out_off get
+ * the kept rows (out_off has nrows + 1 values; the kept count is out_off[nrows]) and dest_out / *dest_len their sorted
+ * union (sg.DestUIDs).  nrows == 0 or no value at all keeps nothing and launches nothing.
+ * DGX_ERR_ARG before anything is copied: a null array that is needed, v_off not starting at 0 or decreasing, nrows or
+ * v_off[nrows] of 2^32 or more, or a set that could reach 2^32 edges; the set is bound to a lane with queued
+ * device-form steps.  DGX_ERR_CAP before anything is copied: out_cap or dest_cap below v_off[nrows].  DGX_ERR_ARG
+ * after the kernels: src, a row or dest not strictly ascending.  A refused step writes nothing to the outputs and
+ * leaves the set unchanged.  Launches: 7 plus the matrix merge's 7 + max(1, ceil(log2 ceil(v_off[nrows] / 2048)))
+ * (DESIGN section 3.10). */
+int dgx_recurse_filter(dgx_reach_set* set, const uint64_t* src, size_t nrows, const uint64_t* v, const uint64_t* v_off,
+                       const uint64_t* dest, size_t ndest, uint64_t* out, uint64_t* out_off, size_t out_cap,
+                       uint64_t* dest_out, size_t dest_cap, size_t* dest_len);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -602,6 +632,19 @@ int dgx_dev_groupby_uid(dgx_lane* lane, const uint64_t* d_src, size_t nrows, con
                         const uint64_t* d_par, const uint64_t* d_par_off, size_t npar, size_t par_cap, size_t e_cap,
                         uint64_t* d_keys, uint64_t* d_grp_off, uint64_t* d_mem_off, size_t grp_cap,
                         uint64_t* d_members, size_t mem_cap, uint64_t* d_sizes);
+/* Device form of dgx_recurse_filter: every array in device memory, offsets included, so the rows of
+ * dgx_dev_list_uids_unfiltered_rows feed it directly.  v_cap is the room of d_v (d_v_off[nrows] must not pass it) and
+ * stands for v_off[nrows] in the host form's limits: out_cap and dest_cap below v_cap are DGX_ERR_CAP.  d_sizes is two
+ * device uint64: {kept, dest_len}.  Sizes, missing pointers and a set bound to another lane (one whose queued steps no
+ * dgx_reach_size or dgx_reach_export has waited for yet) are DGX_ERR_ARG at the call; nrows or v_cap of 0 writes
+ * zero offsets and sizes without a launch.  Every other check (offsets, ascending src, rows and dest) runs on the
+ * device: a refused step writes d_sizes = {0, 0}, nothing else, leaves the set unchanged and surfaces as DGX_ERR_ARG at
+ * the next dgx_lane_sync.  Asynchronous on the lane: the set is bound to it until waited for.  Growing the set past its
+ * capacity allocates device memory; DGX_ERR_OOM leaves the set unchanged. */
+int dgx_dev_recurse_filter(dgx_lane* lane, dgx_reach_set* set, const uint64_t* d_src, size_t nrows, const uint64_t* d_v,
+                           const uint64_t* d_v_off, size_t v_cap, const uint64_t* d_dest, size_t ndest,
+                           uint64_t* d_out, uint64_t* d_out_off, size_t out_cap, uint64_t* d_dest_out,
+                           size_t dest_cap, uint64_t* d_sizes);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

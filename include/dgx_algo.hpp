@@ -18,6 +18,7 @@
 #include <numeric>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "dgx.h"
@@ -294,6 +295,70 @@ inline std::vector<ParentGroups> GroupByUid(const std::vector<pb::List>& parents
     }
     return out;
 }
+
+// The edges one sg.Attr has taken during one @recurse (query/recurse.go expandRecurse's reachMap, loop: false), held
+// in device memory (dgx_reach_set).  One per distinct Attr for the life of one recursion; move-only.
+class ReachSet {
+public:
+    ReachSet() { check(dgx_reach_create(nullptr, nullptr, 0, &s_)); }
+    // A set holding the edges (from[k], to[k]), strictly ascending by (from, to): a recursion continued from the host.
+    ReachSet(const std::vector<uint64_t>& from, const std::vector<uint64_t>& to) {
+        if (from.size() != to.size()) throw Error(DGX_ERR_ARG, "one to per from");
+        check(dgx_reach_create(from.data(), to.data(), from.size(), &s_));
+    }
+    ReachSet(ReachSet&& o) noexcept : s_(o.s_) { o.s_ = nullptr; }
+    ReachSet& operator=(ReachSet&& o) noexcept {
+        std::swap(s_, o.s_);
+        return *this;
+    }
+    ReachSet(const ReachSet&) = delete;
+    ReachSet& operator=(const ReachSet&) = delete;
+    ~ReachSet() { dgx_reach_destroy(s_); }
+
+    struct Step {
+        std::vector<pb::List> rows;  // the kept rows
+        pb::List dest;               // sg.DestUIDs: their sorted union
+        uint64_t kept = 0;           // the step's numEdges
+    };
+    // One sg (:105-134): rows[i] belongs to src[i]; dest is sg.DestUIDs after its filters, or nullptr without filters.
+    Step Filter(const std::vector<uint64_t>& src, const std::vector<pb::List>& rows, const pb::List* dest = nullptr) {
+        if (src.size() != rows.size()) throw Error(DGX_ERR_ARG, "one source per row");
+        std::vector<uint64_t> v, v_off{0};
+        for (const pb::List& r : rows) { v.insert(v.end(), r.Uids.begin(), r.Uids.end()); v_off.push_back(v.size()); }
+        const size_t m = v.size();
+        std::vector<uint64_t> out(std::max<size_t>(m, 1)), out_off(rows.size() + 1), dout(std::max<size_t>(m, 1));
+        static const uint64_t none = 0;
+        size_t dlen = 0;
+        check(dgx_recurse_filter(s_, src.data(), src.size(), v.data(), v_off.data(),
+                                 dest ? (dest->Uids.empty() ? &none : dest->Uids.data()) : nullptr,
+                                 dest ? dest->Uids.size() : 0, out.data(), out_off.data(), m, dout.data(), m, &dlen));
+        Step st;
+        for (size_t i = 0; i < rows.size(); ++i)
+            st.rows.emplace_back(std::vector<uint64_t>(out.begin() + out_off[i], out.begin() + out_off[i + 1]));
+        st.dest = pb::List(std::vector<uint64_t>(dout.begin(), dout.begin() + dlen));
+        st.kept = out_off[rows.size()];
+        return st;
+    }
+    size_t Size() {
+        size_t n = 0;
+        check(dgx_reach_size(s_, &n));
+        return n;
+    }
+    // (from, to) of every edge, ascending: how a recursion hands back to the host.
+    std::pair<std::vector<uint64_t>, std::vector<uint64_t>> Export() {
+        const size_t n = Size();
+        std::vector<uint64_t> f(std::max<size_t>(n, 1)), t(std::max<size_t>(n, 1));
+        size_t got = 0;
+        check(dgx_reach_export(s_, f.data(), t.data(), n, &got));
+        f.resize(got);
+        t.resize(got);
+        return {f, t};
+    }
+    dgx_reach_set* handle() const { return s_; }
+
+private:
+    dgx_reach_set* s_ = nullptr;
+};
 
 }  // namespace algo
 

@@ -139,6 +139,7 @@ def main():
     ap.add_argument("--c11-only", action="store_true", help="only the C11 backup / restore codec rows")
     ap.add_argument("--c12-only", action="store_true", help="only the C12 regexp() trigram query rows")
     ap.add_argument("--c13-only", action="store_true", help="only the C13 @groupby over a uid predicate rows")
+    ap.add_argument("--c14-only", action="store_true", help="only the C14 @recurse filter rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -156,9 +157,11 @@ def main():
         rows = c12_rows(Lane())
     elif args.c13_only:
         rows = c13_rows(Lane())
+    elif args.c14_only:
+        rows = c14_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1513,6 +1516,114 @@ def c13_rows(L, n_sample: int = 20):
 
 def _p_(a):
     return a.ctypes.data_as(C.c_void_p)
+
+
+def c14_rows(L):
+    """C14 "@recurse, loop: false": Zipf graphs of tests/gen_recurse.py (friend out-degree mean 8, follow mean 2, the
+    popular targets the hubs), the per-level uid matrices precomputed on the host (gen_recurse.plan_levels) so the legs
+    time the filter steps, not the row reads.  C14a: { friend }, depth 6 from 100 roots over 2e6 nodes.  C14b:
+    { friend follow }, depth 5 from 100 roots over 2e5 nodes: many small sgs, the per-call cost.  C14c: { friend } over
+    2e6 nodes until the default 1e6-edge limit stops it.  Legs, each a whole recursion with fresh sets: (1) the device
+    form on resident inputs (CUDA events, one wait at the end), (2) the host form (wall clock), (3) the line-by-line
+    restatement (tests/recurse_oracle.c) on 1 thread -- C with a hash set, not Go.  Every leg's rows and DestUIDs are
+    checked against the plan."""
+    import gen_recurse as gr
+    import recurse_oracle as ro
+    from dgraph_b200 import algo
+
+    lib = L.lib
+    big = gr.c14_graph(np.random.default_rng(14))
+    small = gr.c14_graph(np.random.default_rng(15), 200_000)
+    roots = np.random.default_rng(2).integers(1, 2_000_001, 100)
+    cases = [("C14a", {"friend": big["friend"]}, ["friend"], 6, None, roots),
+             ("C14b", small, ["friend", "follow"], 5, None, roots % 200_000 + 1),
+             ("C14c", {"friend": big["friend"]}, ["friend"], 64, 10 ** 6, roots)]
+    out_rows = []
+
+    def dp(t):
+        return C.c_void_p(t.data_ptr())
+
+    def up(x):
+        return torch.from_numpy(np.ascontiguousarray(x).view(np.int64)).to(DEV)
+
+    for name, graph, preds, depth, limit, rts in cases:
+        steps, total, err = gr.plan_levels(graph, rts, preds, depth, limit)
+        vals = sum(s[2].size for s in steps)
+        # (1) device form: inputs and outputs resident, one output buffer per step
+        dev_in = [(up(s[1]), up(s[2]) if s[2].size else up(np.zeros(1, np.uint64)), up(s[3])) for s in steps]
+        dev_out = [tuple(torch.empty(max(s[2].size, 1), dtype=torch.int64, device=DEV) for _ in range(2)) +
+                   (torch.empty(s[1].size + 1, dtype=torch.int64, device=DEV),
+                    torch.empty(2, dtype=torch.int64, device=DEV)) for s in steps]
+        holder = {}
+
+        def dev():
+            sets = {p: algo.ReachSet() for p in preds}
+            for s, (ds, dv, doff), (do, dd, doo, dz) in zip(steps, dev_in, dev_out):
+                _lib.check(lib.dgx_dev_recurse_filter(L.h, sets[s[0]].handle, dp(ds), s[1].size, dp(dv), dp(doff),
+                                                      s[2].size, None, 0, dp(do), dp(doo), s[2].size, dp(dd),
+                                                      s[2].size, dp(dz)))
+            for st in sets.values():
+                st.size()  # waits for the queued steps
+            holder["sets"] = sets
+        ms_dev, _ = timeit(dev, warm=1, reps=3)
+        L.sync()
+        ok_dev = True
+        for s, (do, dd, doo, dz) in zip(steps, dev_out):
+            k, d = (int(x) for x in dz.cpu().numpy())
+            ok_dev &= (k == s[7] and d == s[6].size and np.array_equal(doo.cpu().numpy().view(np.uint64), s[5])
+                       and np.array_equal(do[:k].cpu().numpy().view(np.uint64), s[4])
+                       and np.array_equal(dd[:d].cpu().numpy().view(np.uint64), s[6]))
+        ok_dev &= sum(st.size() for st in holder["sets"].values()) == total
+        for st in holder["sets"].values():
+            st.close()
+        # (2) host form
+        bufs = [(np.empty(max(s[2].size, 1), np.uint64), np.empty(s[1].size + 1, np.uint64),
+                 np.empty(max(s[2].size, 1), np.uint64)) for s in steps]
+        lens = [C.c_size_t() for _ in steps]
+
+        def host():
+            sets = {p: algo.ReachSet() for p in preds}
+            for s, (o, oo, dd), n in zip(steps, bufs, lens):
+                v = s[2] if s[2].size else np.zeros(1, np.uint64)
+                _lib.check(lib.dgx_recurse_filter(sets[s[0]].handle, _p_(s[1]), s[1].size, _p_(v), _p_(s[3]), None, 0,
+                                                  _p_(o), _p_(oo), s[2].size, _p_(dd), s[2].size, C.byref(n)))
+            for st in sets.values():
+                st.close()
+        host()
+        t0 = time.perf_counter()
+        host()
+        t_host = (time.perf_counter() - t0) * 1e3
+        ok_host = all(np.array_equal(oo, s[5]) and np.array_equal(o[:s[7]], s[4]) and n.value == s[6].size
+                      and np.array_equal(dd[:n.value], s[6]) for s, (o, oo, dd), n in zip(steps, bufs, lens))
+        # (3) the restatement, 1 thread
+        attr_id = {p: i + 1 for i, p in enumerate(preds)}
+        obufs = [(np.empty(max(s[2].size, 1), np.uint64), np.empty(s[1].size + 1, np.uint64),
+                  np.empty(max(s[2].size, 1), np.uint64)) for s in steps]
+        reach = ro.Reach()
+        olens = [C.c_size_t() for _ in steps]
+        t0 = time.perf_counter()
+        kept_or = []
+        for s, (o, oo, dd), n in zip(steps, obufs, olens):
+            v = s[2] if s[2].size else np.zeros(1, np.uint64)
+            kept_or.append(ro.lib().orc_recurse_sg(reach._h, attr_id[s[0]], s[1].ctypes.data, s[1].size, v.ctypes.data,
+                                                   s[3].ctypes.data, 0, None, 0, 0, o.ctypes.data, oo.ctypes.data,
+                                                   dd.ctypes.data, C.byref(n)))
+        t_or = (time.perf_counter() - t0) * 1e3
+        reach.close()
+        ok_or = all(k == s[7] and np.array_equal(oo, s[5]) and np.array_equal(dd[:n.value], s[6])
+                    for s, (o, oo, dd), n, k in zip(steps, obufs, olens, kept_or))
+        cfg = (f"{name}: {'{ ' + ' '.join(preds) + ' }'}, {len(steps)} sg steps, {vals} row values, {total} kept edges"
+               f"{', stopped by the edge limit' if err else ''}")
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev, "dgx_dev_recurse_filter, CUDA events, "
+                                     "median of 3 after one warm recursion"),
+                                    ("host form", t_host, ok_host, "dgx_recurse_filter, wall clock, one recursion after "
+                                     "one warm recursion"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, ok_or, "orc_recurse_sg, wall clock")):
+            out_rows.append({"op": "RecurseFilter", "workload": name, "leg": leg, "config": cfg, "ms": round(ms, 4),
+                             "steps": len(steps), "values": vals, "kept": total, "check": bool(ok), "timing": timing})
+            print(json.dumps(out_rows[-1]), flush=True)
+        del dev_in, dev_out
+    return out_rows
 
 
 if __name__ == "__main__":
