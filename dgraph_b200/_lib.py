@@ -47,6 +47,18 @@ class QueryTree(C.Structure):
                 ("sub_off", C.c_void_p), ("sub_idx", C.c_void_p)]
 
 
+class CascadeTree(C.Structure):
+    """dgx_cascade_tree (include/dgx.h): a forest of subgraph nodes in pre-order."""
+    _fields_ = [("nnodes", C.c_size_t), ("parent", C.c_void_p), ("flags", C.c_void_p), ("first", C.c_void_p),
+                ("offset", C.c_void_p), ("counts_len", C.c_void_p)]
+
+
+class CascadeNode(C.Structure):
+    """dgx_cascade_node (include/dgx.h): one node's device arrays for dgx_dev_cascade."""
+    _fields_ = [("v", C.c_void_p), ("v_off", C.c_void_p), ("nrows", C.c_size_t), ("v_cap", C.c_size_t),
+                ("dest", C.c_void_p), ("ndest", C.c_size_t), ("has_val", C.c_void_p), ("nhas", C.c_size_t)]
+
+
 class CacheStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("hits", "misses", "evictions", "bytes", "entries", "max_bytes")]
 
@@ -90,6 +102,7 @@ SYMBOLS = {
     "dgx_reach_size": (_int, [_vp, _szp]),
     "dgx_reach_export": (_int, [_vp, _vp, _vp, _sz, _szp]),
     "dgx_recurse_filter": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _szp]),
+    "dgx_cascade": (_int, [C.POINTER(CascadeTree), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _sz]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
     "dgx_encode_bound": (None, [_sz, C.c_uint32, _szp, _szp]),
@@ -132,6 +145,7 @@ SYMBOLS = {
     "dgx_dev_list_count_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, _vp]),
     "dgx_dev_trigram_query": (_int, [_vp, C.POINTER(QueryTree), _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _vp]),
     "dgx_dev_recurse_filter": (_int, [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "dgx_dev_cascade": (_int, [_vp, C.POINTER(CascadeTree), C.POINTER(CascadeNode), _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),
     "dgx_filter_tail_queries": (_u64, [_vp]),

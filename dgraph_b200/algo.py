@@ -441,6 +441,81 @@ def GroupByUid(parents, src, rows, dest, members: bool = True):
     return out
 
 
+CC_CASCADE, CC_CHECKED, CC_FILTERED, CC_ORDERED, CC_SKIP = 1, 2, 4, 8, 16  # DGX_CASCADE_* (include/dgx.h)
+
+
+class CascadeNode:
+    """One subgraph node of a @cascade forest, in pre-order (dgx_cascade): parent index (-1 for a query root), CC_* flags
+    resolved from the SubGraph, Params.Cascade.First / Offset, len(counts), DestUIDs (strictly ascending), uidMatrix
+    rows (row i belongs to parent.DestUIDs[i]) and has_val (one byte per row: valueMatrix[i] has values)."""
+
+    __slots__ = ("parent", "flags", "first", "offset", "counts_len", "dest", "rows", "has_val")
+
+    def __init__(self, parent=-1, flags=0, first=0, offset=0, counts_len=0, dest=(), rows=(), has_val=()):
+        self.parent, self.flags, self.first, self.offset, self.counts_len = parent, flags, first, offset, counts_len
+        self.dest = _u64(dest.Uids if isinstance(dest, List) else dest)
+        self.rows = [_u64(r.Uids if isinstance(r, List) else r) for r in rows]
+        self.has_val = np.ascontiguousarray(np.asarray(has_val, np.uint8))
+
+
+def cascade_arrays(nodes) -> dict:
+    """The flat CSR form of dgx_cascade: tree arrays, values with per-row offsets and per-node row offsets, dest and
+    has_val with per-node offsets.  Every array has at least one element."""
+    n = len(nodes)
+
+    def off(sizes):
+        o = np.zeros(len(sizes) + 1, np.uint64)
+        np.cumsum(sizes, out=o[1:])
+        return o
+
+    def cat(arrs, dt):
+        arrs = [a for a in arrs if a.size]
+        return np.ascontiguousarray(np.concatenate(arrs).astype(dt)) if arrs else np.zeros(1, dt)
+
+    rows = [r for nd in nodes for r in nd.rows]
+    a = {"parent": np.array([0xFFFFFFFF if nd.parent < 0 else nd.parent for nd in nodes] or [0], np.uint32),
+         "flags": np.array([nd.flags for nd in nodes] or [0], np.uint8),
+         "first": np.array([nd.first for nd in nodes] or [0], np.int32),
+         "offset": np.array([nd.offset for nd in nodes] or [0], np.int32),
+         "counts_len": np.array([nd.counts_len for nd in nodes] or [0], np.uint64),
+         "v": cat(rows, np.uint64), "v_off": off([r.size for r in rows]),
+         "row_off": off([len(nd.rows) for nd in nodes]),
+         "dest": cat([nd.dest for nd in nodes], np.uint64), "dest_off": off([nd.dest.size for nd in nodes]),
+         "has_val": cat([nd.has_val for nd in nodes], np.uint8), "hv_off": off([nd.has_val.size for nd in nodes])}
+    a["nnodes"] = n
+    return a
+
+
+def cascade_split(a, out, out_off, dest_out, dest_out_off):
+    """Per-node results of a flat call: ([rows of each node], [dest of each node])."""
+    ro = a["row_off"]
+    rows = [[out[int(out_off[r]):int(out_off[r + 1])].copy() for r in range(int(ro[k]), int(ro[k + 1]))]
+            for k in range(a["nnodes"])]
+    dests = [dest_out[int(dest_out_off[k]):int(dest_out_off[k + 1])].copy() for k in range(a["nnodes"])]
+    return rows, dests
+
+
+def cascade_tree(a) -> _lib.CascadeTree:
+    """The dgx_cascade_tree over the tree arrays of cascade_arrays (which must outlive it)."""
+    return _lib.CascadeTree(a["nnodes"], *[a[k].ctypes.data for k in ("parent", "flags", "first", "offset",
+                                                                        "counts_len")])
+
+
+def Cascade(nodes):
+    """@cascade over a forest (query/query.go populateVarMap :1445-1527 and ProcessQuery's root pagination :3004-3011)
+    in one call (dgx_cascade).  Returns ([rows of each node], [DestUIDs of each node as List]) after the cascade."""
+    a = cascade_arrays(nodes)
+    m, nd = int(a["v_off"][-1]), int(a["dest_off"][-1])
+    out, dest_out = np.empty(max(m, 1), np.uint64), np.empty(max(nd, 1), np.uint64)
+    out_off, dest_off = np.zeros(int(a["row_off"][-1]) + 1, np.uint64), np.zeros(len(nodes) + 1, np.uint64)
+    tree = cascade_tree(a)
+    _lib.check(_lib.load().dgx_cascade(C.byref(tree), _p(a["v"]), _p(a["v_off"]), _p(a["row_off"]), _p(a["dest"]),
+                                       _p(a["dest_off"]), _p(a["has_val"]), _p(a["hv_off"]), _p(out), _p(out_off), m,
+                                       _p(dest_out), _p(dest_off), nd))
+    rows, dests = cascade_split(a, out, out_off, dest_out, dest_off)
+    return rows, [List(d) for d in dests]
+
+
 class ReachSet:
     """The edges one sg.Attr has taken during one @recurse (query/recurse.go expandRecurse's reachMap, loop: false),
     kept in device memory (dgx_reach_set).  One set per distinct Attr, for the life of one recursion."""

@@ -41,6 +41,7 @@
 #include "trigram_kernel.cuh"
 #include "groupby_kernel.cuh"
 #include "recurse_kernel.cuh"
+#include "cascade_kernel.cuh"
 #include "wire.hpp"
 
 using namespace dgx;
@@ -462,6 +463,9 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
         if (flag & kLaneErrRecurse)
             return fail(DGX_ERR_ARG, "a recurse step's input is malformed (src, a row or dest not strictly ascending, "
                                      "or offsets not starting at 0, decreasing or past v_cap)");
+        if (flag & kLaneErrCascade)
+            return fail(DGX_ERR_ARG, "a cascade input is malformed (a dest or an unordered row not strictly ascending, "
+                                     "or row offsets not starting at 0, decreasing or past v_cap)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -4039,6 +4043,351 @@ extern "C" int dgx_recurse_filter(dgx_reach_set* s, const uint64_t* src, size_t 
     *dest_len = D;
     g_stats.d2h += (K + D + nrows + 3) * sizeof(uint64_t);
     g_stats.uids_out += K + D;
+    return DGX_OK;
+}
+
+// ---------------------------------------------------------------------------
+// @cascade: a forest's uid matrices pruned bottom-up, with cascade pagination, in one call (cascade_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr size_t kCcMaxNodes = size_t(1) << 16;
+constexpr uint32_t kCcMaxDepth = 64;            // levels: a node's depth is at most kCcMaxDepth - 1
+constexpr uint64_t kCcMax = uint64_t(1) << 32;  // rows, values and dest values in all are 32-bit counts
+
+// One node's arrays, node order: host pointers (host form) or device pointers, which only the kernels read.
+struct CcSrc {
+    const uint64_t* v;
+    const uint64_t* v_off;
+    uint64_t v_base, nrows, vcap;
+    const uint64_t* dest;
+    uint64_t ndest;
+    const uint8_t* hv;
+    uint64_t nhv;
+};
+
+struct CcPlan {
+    std::vector<CcNode> node;    // level order
+    std::vector<uint32_t> ck;    // checked children, level-order indices
+    std::vector<CcLevel> level;  // the levels with work, deepest first
+    uint64_t nv = 0, no = 0, nd = 0, nh = 0, rows = 0, max_nv = 0, max_nd = 0;
+};
+
+static int cc_check_tree(const dgx_cascade_tree* t) {
+    if (!t) return fail(DGX_ERR_ARG, "null tree");
+    const size_t n = t->nnodes;
+    if (n >= kCcMaxNodes) return fail(DGX_ERR_ARG, "%zu nodes: at most 2^16 - 1", n);
+    if (n && (!t->parent || !t->flags || !t->first || !t->offset || !t->counts_len))
+        return fail(DGX_ERR_ARG, "null tree array");
+    std::vector<uint32_t> depth(n);
+    for (size_t k = 0; k < n; ++k) {
+        const uint32_t p = t->parent[k];
+        if (t->flags[k] & ~uint8_t(DGX_CASCADE_CASCADE | DGX_CASCADE_CHECKED | DGX_CASCADE_FILTERED |
+                                   DGX_CASCADE_ORDERED | DGX_CASCADE_SKIP))
+            return fail(DGX_ERR_ARG, "node %zu: unknown flag bits 0x%x", k, (unsigned)t->flags[k]);
+        if (p == UINT32_MAX) { depth[k] = 0; continue; }
+        if (p >= k) return fail(DGX_ERR_ARG, "node %zu: parent %u is not below it", k, p);
+        if (t->flags[p] & DGX_CASCADE_SKIP) return fail(DGX_ERR_ARG, "node %zu: its parent %u is SKIP", k, p);
+        depth[k] = depth[p] + 1;
+        if (depth[k] >= kCcMaxDepth) return fail(DGX_ERR_ARG, "node %zu is deeper than %u", k, kCcMaxDepth - 1);
+    }
+    return DGX_OK;
+}
+
+// The level-order plan of a checked tree: modes, slots, checked children and the levels with work.
+static void cc_plan(const dgx_cascade_tree* t, const CcSrc* src, CcPlan* P) {
+    const size_t n = t->nnodes;
+    std::vector<uint32_t> depth(n), pos(n);
+    uint32_t maxd = 0;
+    for (size_t k = 0; k < n; ++k) {
+        depth[k] = t->parent[k] == UINT32_MAX ? 0 : depth[t->parent[k]] + 1;
+        maxd = std::max(maxd, depth[k]);
+    }
+    std::vector<uint32_t> order;  // deepest level first, node order inside a level
+    std::vector<uint32_t> lb;     // level boundaries in `order`
+    for (int64_t d = maxd; d >= 0 && n; --d) {
+        lb.push_back((uint32_t)order.size());
+        for (size_t k = 0; k < n; ++k)
+            if (depth[k] == (uint32_t)d) { pos[k] = (uint32_t)order.size(); order.push_back((uint32_t)k); }
+    }
+    lb.push_back((uint32_t)order.size());
+    std::vector<uint64_t> out_row(n + 1, 0);
+    for (size_t k = 0; k < n; ++k) out_row[k + 1] = out_row[k] + src[k].nrows;
+    P->rows = out_row[n];
+    std::vector<std::vector<uint32_t>> checked(n);
+    for (size_t k = 0; k < n; ++k)
+        if (t->parent[k] != UINT32_MAX && (t->flags[k] & DGX_CASCADE_CHECKED)) checked[t->parent[k]].push_back(pos[k]);
+    P->node.resize(n);
+    for (size_t q = 0; q < n; ++q) {
+        const uint32_t k = order[q];
+        const CcSrc& s = src[k];
+        const uint8_t f = t->flags[k];
+        const bool root = t->parent[k] == UINT32_MAX, cascade = f & DGX_CASCADE_CASCADE, skip = f & DGX_CASCADE_SKIP;
+        CcNode& c = P->node[q];
+        c.v = (const u64*)s.v;
+        c.v_off = (const u64*)s.v_off;
+        c.dest = (const u64*)s.dest;
+        c.hv = s.hv;
+        c.v_base = s.v_base;
+        c.vb = P->nv;
+        c.vcap = s.vcap;
+        c.ob = P->no;
+        c.nrows = s.nrows;
+        c.db = P->nd;
+        c.ndest = s.ndest;
+        c.hb = P->nh;
+        c.nhv = s.nhv;
+        c.counts_len = t->counts_len[k];
+        c.out_row = out_row[k];
+        c.id = k;
+        const bool paged = cascade && (!root || t->first[k] != 0 || t->offset[k] != 0);
+        c.mode = paged ? CC_ROWS_NEW : (f & DGX_CASCADE_FILTERED) && !skip ? CC_ROWS_OLD : CC_ROWS_KEEP;
+        c.prune = cascade && !skip;
+        c.ordered = (f & DGX_CASCADE_ORDERED) != 0;
+        c.first = paged ? t->first[k] : 0;
+        c.offset = paged ? t->offset[k] : 0;
+        c.ck_b = (uint32_t)P->ck.size();
+        if (c.prune) P->ck.insert(P->ck.end(), checked[k].begin(), checked[k].end());
+        c.ck_e = (uint32_t)P->ck.size();
+        P->nv += s.vcap;
+        P->no += s.nrows + 1;
+        P->nd += s.ndest;
+        P->nh += s.nhv;
+    }
+    for (size_t i = 0; i + 1 < lb.size(); ++i) {
+        const CcNode &a = P->node[lb[i]], &z = P->node[lb[i + 1] - 1];
+        CcLevel L{};
+        L.a = lb[i];
+        L.b = lb[i + 1];
+        L.va = a.vb;
+        L.nv = z.vb + z.vcap - a.vb;
+        L.da = a.db;
+        L.nd = z.db + z.ndest - a.db;
+        L.oa = a.ob;
+        L.no = z.ob + z.nrows + 1 - a.ob;
+        if (L.nv == 0 && L.nd == 0) continue;  // its rows and dest are empty already
+        P->max_nv = std::max<uint64_t>(P->max_nv, L.nv);
+        P->max_nd = std::max<uint64_t>(P->max_nd, L.nd);
+        P->level.push_back(L);
+    }
+}
+
+static uint64_t cc_tiles(uint64_t n) { return std::max<uint64_t>(1, (n + EN_TILE - 1) / EN_TILE); }
+
+// The whole call on the lane: one metadata copy, 4 + 7 * D launches.  Workspace: 44 bytes per value slot (gathered
+// and kept values 16, and a level's flags, their three scans and rows 28), 16 per offset slot, 16 per dest slot plus
+// 16 per dest slot of the largest level, 1 per has_val byte, about 140 per node, and the scans' look-back words.
+static int cc_run(dgx_lane* l, const CcPlan& T, uint64_t* d_out, uint64_t* d_out_off, uint64_t* d_dest_out,
+                  uint64_t* d_dest_off, uint64_t* d_sizes) {
+    const uint64_t NN = T.node.size(), D = T.level.size();
+    uint64_t nstatus = cc_tiles(2 * NN);
+    for (const CcLevel& L : T.level) nstatus += cc_tiles(L.nd) + 2 * cc_tiles(L.nv);
+    const uint64_t nscan = 3 * D + 1;
+    // host metadata, one copy: nodes, checked children, the scans' size words
+    const size_t b_node = NN * sizeof(CcNode), b_ck = (T.ck.size() + 1) * sizeof(uint32_t);
+    const size_t b_meta = ((b_node + b_ck + 15) & ~size_t(15)) + (2 * D + 1) * sizeof(uint64_t);
+    void* h_meta;
+    int rc = l->host.alloc(b_meta, &h_meta);
+    if (rc) return rc;
+    memcpy(h_meta, T.node.data(), b_node);
+    if (!T.ck.empty()) memcpy((char*)h_meta + b_node, T.ck.data(), T.ck.size() * sizeof(uint32_t));
+    uint64_t* h_words = (uint64_t*)((char*)h_meta + ((b_node + b_ck + 15) & ~size_t(15)));
+    for (uint64_t i = 0; i < D; ++i) {
+        h_words[2 * i] = T.level[i].nd;
+        h_words[2 * i + 1] = T.level[i].nv;
+    }
+    h_words[2 * D] = 2 * NN;
+    // zeroed: [bad | tickets | look-back status], then the arrays
+    const size_t b_zero = ((16 + nscan * sizeof(u32) + 15) & ~size_t(15)) + nstatus * sizeof(u64);
+    const size_t n64 = 2 * T.nv + 2 * T.no + 2 * T.nd + NN + (2 * T.max_nd + 1) + (3 * T.max_nv + 2) + (4 * NN + 1);
+    const size_t b_meta16 = (b_meta + 15) & ~size_t(15);  // the zeroed region starts 16-byte aligned
+    const size_t bytes = b_meta16 + b_zero + n64 * sizeof(u64) + T.max_nv * sizeof(u32) + T.nh;
+    void* d_raw;
+    if ((rc = l->ws.alloc(bytes, &d_raw))) return rc;
+    char* z = (char*)d_raw + b_meta16;
+    CK(cudaMemcpyAsync(d_raw, h_meta, b_meta, cudaMemcpyHostToDevice, l->stream));
+    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
+    g_stats.h2d += b_meta;
+    CcParams P;
+    P.node = (const CcNode*)d_raw;
+    P.ck = (const u32*)((char*)d_raw + b_node);
+    const u64* d_words = (const u64*)((char*)d_raw + ((b_node + b_ck + 15) & ~size_t(15)));
+    P.nnodes = (u32)NN;
+    P.nv = T.nv;
+    P.no = T.no;
+    P.nd = T.nd;
+    P.nh = T.nh;
+    P.out_rows = T.rows;
+    P.bad = (int*)z;
+    u32* ticket = (u32*)(z + 16);
+    u64* status = (u64*)(z + ((16 + nscan * sizeof(u32) + 15) & ~size_t(15)));
+    u64* a = (u64*)(z + b_zero);
+    auto take = [&](uint64_t n) { u64* p = a; a += n; return p; };
+    P.V = take(T.nv);
+    P.OV = take(T.nv);
+    P.VO = take(T.no);
+    P.OO = take(T.no);
+    P.D = take(T.nd);
+    P.ND = take(T.nd);
+    P.NDE = take(NN);
+    P.keep = take(T.max_nd);
+    P.kx = take(T.max_nd + 1);
+    P.fv = take(T.max_nv);
+    P.fx = take(T.max_nv + 1);
+    P.fy = take(T.max_nv + 1);
+    P.cnt = take(2 * NN);
+    P.cx = take(2 * NN + 1);
+    P.rw = (u32*)a;
+    P.H = (unsigned char*)(P.rw + T.max_nv);
+    if (P.H + T.nh != (unsigned char*)d_raw + bytes)
+        return fail(DGX_ERR_CUDA, "cascade workspace layout (%zu bytes) does not match its size (%zu bytes)",
+                    (size_t)(P.H + T.nh - (unsigned char*)d_raw), bytes);
+    P.err = l->d_err;
+    P.out = (u64*)d_out;
+    P.out_off = (u64*)d_out_off;
+    P.dest_out = (u64*)d_dest_out;
+    P.dest_off = (u64*)d_dest_off;
+    P.sizes = (u64*)d_sizes;
+    auto scan = [&](const u64* in, u64* out, const u64* n_word, uint64_t n) {
+        const uint64_t tiles = cc_tiles(n);
+        scan_u64_kernel<<<(unsigned)tiles, EN_NT, 0, l->stream>>>(in, out, n_word, n, status, ticket, nullptr);
+        status += tiles;
+        ticket += 1;
+    };
+    cc_gather_kernel<<<gb_grid(std::max<uint64_t>({T.nv, T.no, T.nd, T.nh, NN})), 256, 0, l->stream>>>(P);
+    for (uint64_t i = 0; i < D; ++i) {
+        CcLevel L = T.level[i];
+        L.n_dest = d_words + 2 * i;
+        L.n_val = d_words + 2 * i + 1;
+        cc_keep_kernel<<<gb_grid(L.nd), 256, 0, l->stream>>>(P, L);
+        scan(P.keep, P.kx, L.n_dest, L.nd);
+        cc_filter_kernel<<<gb_grid(std::max<uint64_t>({L.nd, L.nv, L.b - L.a})), 256, 0, l->stream>>>(P, L);
+        scan(P.fv, P.fx, L.n_val, L.nv);
+        cc_page_kernel<<<gb_grid(L.nv), 256, 0, l->stream>>>(P, L);
+        scan(P.fv, P.fy, L.n_val, L.nv);
+        cc_compact_kernel<<<gb_grid(std::max<uint64_t>(L.nv, L.no)), 256, 0, l->stream>>>(P, L);
+    }
+    cc_count_kernel<<<gb_grid(NN), 256, 0, l->stream>>>(P);
+    scan(P.cnt, P.cx, d_words + 2 * D, 2 * NN);
+    cc_place_kernel<<<gb_grid(std::max<uint64_t>({T.nv, T.no, T.nd, NN + 1})), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 4 + 7 * (int)D);
+    return DGX_OK;
+}
+
+// Sizes and pointers of a planned call, before anything is copied.
+static int cc_check_plan(const CcPlan& T, size_t out_cap, size_t dest_cap) {
+    if (T.rows >= kCcMax || T.nv >= kCcMax || T.nd >= kCcMax)
+        return fail(DGX_ERR_ARG, "cascade sizes are 32-bit: %llu rows, %llu values, %llu dest values in all",
+                    (unsigned long long)T.rows, (unsigned long long)T.nv, (unsigned long long)T.nd);
+    if (out_cap < T.nv || dest_cap < T.nd)
+        return fail(DGX_ERR_CAP, "out_cap %zu / dest_cap %zu below the bounds %llu / %llu", out_cap, dest_cap,
+                    (unsigned long long)T.nv, (unsigned long long)T.nd);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_cascade(dgx_lane* l, const dgx_cascade_tree* tree, const dgx_cascade_node* nodes,
+                               uint64_t* d_out, uint64_t* d_out_off, size_t out_cap, uint64_t* d_dest_out,
+                               uint64_t* d_dest_out_off, size_t dest_cap, uint64_t* d_sizes) {
+    if (!l || !d_out_off || !d_dest_out_off || !d_sizes) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = cc_check_tree(tree)) return rc;
+    const size_t n = tree->nnodes;
+    if (n && !nodes) return fail(DGX_ERR_ARG, "null nodes");
+    std::vector<CcSrc> src(n);
+    for (size_t k = 0; k < n; ++k) {
+        const dgx_cascade_node& c = nodes[k];
+        if (!c.v_off || (c.v_cap && !c.v) || (c.ndest && !c.dest) || (c.nhas && !c.has_val))
+            return fail(DGX_ERR_ARG, "node %zu: null array", k);
+        src[k] = {c.v, c.v_off, 0, c.nrows, c.v_cap, c.dest, c.ndest, c.has_val, c.nhas};
+    }
+    CcPlan T;
+    cc_plan(tree, src.data(), &T);
+    if (int rc = cc_check_plan(T, out_cap, dest_cap)) return rc;
+    if ((T.nv && !d_out) || (T.nd && !d_dest_out)) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_out_off, (T.rows + 1) * sizeof(uint64_t));
+    l->note_output(d_dest_out_off, (n + 1) * sizeof(uint64_t));
+    l->note_output(d_sizes, 2 * sizeof(uint64_t));
+    if (T.level.empty()) {  // no dest value and no value slot: every row and dest is empty
+        CK(cudaMemsetAsync(d_out_off, 0, (T.rows + 1) * sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_dest_out_off, 0, (n + 1) * sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_sizes, 0, 2 * sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = cc_run(l, T, d_out, d_out_off, d_dest_out, d_dest_out_off, d_sizes)) return rc;
+    g_stats.uids_in += T.nv + T.nd;
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_dest_out, dest_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_cascade(const dgx_cascade_tree* tree, const uint64_t* v, const uint64_t* v_off,
+                           const uint64_t* row_off, const uint64_t* dest, const uint64_t* dest_off,
+                           const uint8_t* has_val, const uint64_t* hv_off, uint64_t* out, uint64_t* out_off,
+                           size_t out_cap, uint64_t* dest_out, uint64_t* dest_out_off, size_t dest_cap) {
+    if (!out_off || !dest_out_off) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = cc_check_tree(tree)) return rc;
+    const size_t n = tree->nnodes;
+    if (n == 0) {
+        out_off[0] = dest_out_off[0] = 0;
+        return DGX_OK;
+    }
+    if (!row_off || !v_off || !dest_off || !hv_off) return fail(DGX_ERR_ARG, "null argument");
+    int rc;
+    if ((rc = check_offsets("row_off", row_off, n, kCcMax)) || (rc = check_offsets("v_off", v_off, row_off[n], kCcMax)) ||
+        (rc = check_offsets("dest_off", dest_off, n, kCcMax)) || (rc = check_offsets("hv_off", hv_off, n, UINT64_MAX)))
+        return rc;
+    const uint64_t rows = row_off[n], m = v_off[rows], nd = dest_off[n], nh = hv_off[n];
+    if ((m && !v) || (nd && !dest) || (nh && !has_val)) return fail(DGX_ERR_ARG, "null argument");
+    if ((m && !out) || (nd && !dest_out)) return fail(DGX_ERR_ARG, "null argument");
+    if (out_cap < m || dest_cap < nd)
+        return fail(DGX_ERR_CAP, "out_cap %zu / dest_cap %zu below the bounds %llu / %llu", out_cap, dest_cap,
+                    (unsigned long long)m, (unsigned long long)nd);
+    if (m == 0 && nd == 0) {
+        memset(out_off, 0, (rows + 1) * sizeof(uint64_t));
+        memset(dest_out_off, 0, (n + 1) * sizeof(uint64_t));
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += m + nd;
+    uint64_t *d_v, *d_v_off, *d_dest;
+    uint8_t* d_hv;
+    void* p;
+    if ((rc = upload_list(l, v, m, &d_v)) || (rc = upload_list(l, v_off, rows + 1, &d_v_off)) ||
+        (rc = upload_list(l, dest, nd, &d_dest)) || (rc = l->ws.alloc(nh + 16, &p)))
+        return rc;
+    d_hv = (uint8_t*)p;
+    if (nh) CK(cudaMemcpyAsync(d_hv, has_val, nh, cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += nh;
+    std::vector<CcSrc> src(n);
+    for (size_t k = 0; k < n; ++k) {
+        const uint64_t r0 = row_off[k], r1 = row_off[k + 1];
+        src[k] = {d_v + v_off[r0], d_v_off + r0, v_off[r0], r1 - r0, v_off[r1] - v_off[r0], d_dest + dest_off[k],
+                  dest_off[k + 1] - dest_off[k], d_hv + hv_off[k], hv_off[k + 1] - hv_off[k]};
+    }
+    CcPlan T;
+    cc_plan(tree, src.data(), &T);
+    if ((rc = cc_check_plan(T, m, nd))) return rc;
+    void* d_o;
+    if ((rc = l->ws.alloc((m + nd + rows + n + 4) * sizeof(uint64_t), &d_o))) return rc;
+    uint64_t* d_sizes = (uint64_t*)d_o;
+    uint64_t* d_out = d_sizes + 2;
+    uint64_t* d_dout = d_out + m;
+    uint64_t* d_ooff = d_dout + nd;
+    uint64_t* d_doff = d_ooff + rows + 1;
+    if ((rc = cc_run(l, T, d_out, d_ooff, d_dout, d_doff, d_sizes))) return rc;
+    CK(cudaMemcpyAsync(l->h_word, d_sizes, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) return rc;
+    const uint64_t K = l->h_word[0], DN = l->h_word[1];
+    CK(cudaMemcpyAsync(out_off, d_ooff, (rows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(dest_out_off, d_doff, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (K) CK(cudaMemcpyAsync(out, d_out, K * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (DN) CK(cudaMemcpyAsync(dest_out, d_dout, DN * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += (K + DN + rows + n + 4) * sizeof(uint64_t);
+    g_stats.uids_out += K + DN;
     return DGX_OK;
 }
 

@@ -438,3 +438,123 @@ func (r *ReachSet) Close() {
 		r.s = nil
 	}
 }
+
+// dgxMinCascade: below this many row values in a forest Cascade stays on the Go path (populateVarMap's per-row loops).
+// The C15 record (profiles/h100_c15_cascade.json) times the library against a C restatement of that path, not against
+// Go, so this is the same bound as dgxMinMergeMatrix until a Go comparison sets it.
+const dgxMinCascade = 1 << 14
+
+// Cascade flags, resolved by the caller from each SubGraph (INTEGRATION.md, @cascade).
+const (
+	CascadeOn       = uint8(C.DGX_CASCADE_CASCADE)  // len(Params.Cascade.Fields) > 0
+	CascadeChecked  = uint8(C.DGX_CASCADE_CHECKED)  // the parent's cascade consults it: listed or __all__, not uid, not internal
+	CascadeFiltered = uint8(C.DGX_CASCADE_FILTERED) // len(Filters) > 0
+	CascadeOrdered  = uint8(C.DGX_CASCADE_ORDERED)  // Order or FacetsOrder
+	CascadeSkip     = uint8(C.DGX_CASCADE_SKIP)     // IsGroupBy() or the shortest alias; such a node has no children here
+)
+
+// CascadeNode is one SubGraph of a @cascade forest, in pre-order: Parent is -1 for a query root and a smaller index
+// otherwise; Rows is sg.uidMatrix, HasVal[i] is len(sg.valueMatrix[i].Values) > 0, CountsLen is len(sg.counts).
+type CascadeNode struct {
+	Parent        int
+	Flags         uint8
+	First, Offset int
+	CountsLen     int
+	Dest          []uint64
+	Rows          []*pb.List
+	HasVal        []byte
+}
+
+// Cascade runs populateVarMap's cascade path (query/query.go:1445-1527, updateUidMatrix without facets) for the whole
+// forest and ProcessQuery's root pagination (:3004-3011) in one call.  It returns every node's rows and DestUIDs after
+// the cascade, in node order.  It returns false, and the caller keeps the Go path, below dgxMinCascade row values,
+// when a First / Offset does not fit int32, and on any library error (a malformed forest, rows that do not ascend).
+func Cascade(nodes []CascadeNode) ([][][]uint64, [][]uint64, bool) {
+	n := len(nodes)
+	parent, flags := make([]uint32, n+1), make([]uint8, n+1)
+	first, offset := make([]int32, n+1), make([]int32, n+1)
+	counts := make([]uint64, n+1)
+	rowOff, destOff, hvOff := make([]uint64, n+1), make([]uint64, n+1), make([]uint64, n+1)
+	m, nd, nh, nr := 0, 0, 0, 0
+	for _, c := range nodes {
+		m += totalUids(c.Rows)
+		nd += len(c.Dest)
+		nh += len(c.HasVal)
+		nr += len(c.Rows)
+	}
+	if m < dgxMinCascade || n == 0 {
+		return nil, nil, false
+	}
+	// every slice handed to C directly is its own Go allocation holding no Go pointers
+	v, vOff := make([]uint64, 0, m), make([]uint64, 1, nr+1)
+	dest, hv := make([]uint64, 0, nd+1), make([]uint8, 0, nh+1)
+	for k, c := range nodes {
+		if c.First != int(int32(c.First)) || c.Offset != int(int32(c.Offset)) {
+			return nil, nil, false
+		}
+		parent[k] = ^uint32(0)
+		if c.Parent >= 0 {
+			parent[k] = uint32(c.Parent)
+		}
+		flags[k], first[k], offset[k], counts[k] = c.Flags, int32(c.First), int32(c.Offset), uint64(c.CountsLen)
+		for _, r := range c.Rows {
+			if r != nil {
+				v = append(v, r.Uids...)
+			}
+			vOff = append(vOff, uint64(len(v)))
+		}
+		rowOff[k+1] = uint64(len(vOff) - 1)
+		dest = append(dest, c.Dest...)
+		destOff[k+1] = uint64(len(dest))
+		hv = append(hv, c.HasVal...)
+		hvOff[k+1] = uint64(len(hv))
+	}
+	out, outOff := make([]uint64, m+1), make([]uint64, nr+1)
+	dout, doutOff := make([]uint64, nd+1), make([]uint64, n+1)
+	// the tree struct points at its arrays, so it and they live in C memory: Go memory handed to C must not hold Go
+	// pointers
+	frees := []func(){}
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+	}()
+	carr := func(p unsafe.Pointer, free func()) unsafe.Pointer {
+		frees = append(frees, free)
+		return p
+	}
+	tree := (*C.dgx_cascade_tree)(carr(cArray([]C.dgx_cascade_tree{{nnodes: C.size_t(n)}})))
+	tree.parent = (*C.uint32_t)(carr(cArray(parent)))
+	tree.flags = (*C.uint8_t)(carr(cArray(flags)))
+	tree.first = (*C.int32_t)(carr(cArray(first)))
+	tree.offset = (*C.int32_t)(carr(cArray(offset)))
+	tree.counts_len = (*C.uint64_t)(carr(cArray(counts)))
+	var hvPtr *C.uint8_t
+	if len(hv) > 0 {
+		hvPtr = (*C.uint8_t)(unsafe.Pointer(&hv[0]))
+	}
+	rc := C.dgx_cascade(tree, u64ptr(v), u64ptr(vOff), u64ptr(rowOff), u64ptr(dest), u64ptr(destOff), hvPtr,
+		u64ptr(hvOff), u64ptr(out), u64ptr(outOff), C.size_t(m), u64ptr(dout), u64ptr(doutOff), C.size_t(nd))
+	if rc != C.DGX_OK {
+		return nil, nil, false
+	}
+	rows, dests := make([][][]uint64, n), make([][]uint64, n)
+	for k := range nodes {
+		rows[k] = make([][]uint64, rowOff[k+1]-rowOff[k])
+		for i := range rows[k] {
+			r := rowOff[k] + uint64(i)
+			rows[k][i] = out[outOff[r]:outOff[r+1]:outOff[r+1]]
+		}
+		dests[k] = dout[doutOff[k]:doutOff[k+1]:doutOff[k+1]]
+	}
+	return rows, dests, true
+}
+
+// cArray copies v into a C allocation of max(len(v), 1) elements (an empty array still has an address) and returns it
+// with the function that frees it.
+func cArray[T any](v []T) (unsafe.Pointer, func()) {
+	var zero T
+	p := C.malloc(C.size_t(int(unsafe.Sizeof(zero)) * max(len(v), 1)))
+	copy(unsafe.Slice((*T)(p), len(v)), v)
+	return p, func() { C.free(p) }
+}

@@ -417,6 +417,47 @@ int dgx_recurse_filter(dgx_reach_set* set, const uint64_t* src, size_t nrows, co
                        const uint64_t* dest, size_t ndest, uint64_t* out, uint64_t* out_off, size_t out_cap,
                        uint64_t* dest_out, size_t dest_cap, size_t* dest_len);
 
+/* @cascade over a forest of subgraph nodes (query/query.go populateVarMap :1445-1527, updateUidMatrix :1425-1439
+ * without facets, and ProcessQuery's root pagination :3004-3011), in pre-order: parent[n] is UINT32_MAX for a query root
+ * and below n otherwise.  flags[n] is a set of DGX_CASCADE_* bits resolved on the host; first[n] / offset[n] are
+ * Params.Cascade.First / Offset; counts_len[n] is len(n.counts). */
+#define DGX_CASCADE_CASCADE 1u  /* len(Params.Cascade.Fields) > 0 */
+#define DGX_CASCADE_CHECKED 2u  /* the parent's cascade consults it: listed or __all__, Attr != "uid", not internal */
+#define DGX_CASCADE_FILTERED 4u /* len(Filters) > 0 */
+#define DGX_CASCADE_ORDERED 8u  /* Order or FacetsOrder: rows not uid-sorted */
+#define DGX_CASCADE_SKIP 16u    /* IsGroupBy() or the shortest alias: populateVarMap does nothing; it has no children */
+typedef struct dgx_cascade_tree {
+    size_t nnodes;
+    const uint32_t* parent;       /* nnodes */
+    const uint8_t* flags;         /* nnodes */
+    const int32_t* first;         /* nnodes */
+    const int32_t* offset;        /* nnodes */
+    const uint64_t* counts_len;   /* nnodes */
+} dgx_cascade_tree;
+/* Node n has dest[dest_off[n] .. dest_off[n+1]) (n.DestUIDs, strictly ascending), the rows row_off[n] .. row_off[n+1]
+ * of the forest's uid matrix (row r is v[v_off[r] .. v_off[r+1]); its i-th row belongs to parent.dest[i], and rows past
+ * the last count as empty) and has_val[hv_off[n] .. hv_off[n+1]) (nonzero iff valueMatrix[i] has values; missing bytes
+ * count as zero).  Rows of a node without DGX_CASCADE_ORDERED strictly ascend.  Post-order, every node:
+ *   FILTERED and not SKIP: its rows are filtered by its dest;
+ *   every CASCADE child: its rows are filtered by its dest as it stands after its own step, then cut by
+ *     x.PageRange(first, offset, len);
+ *   CASCADE and not SKIP: dest keeps dest[i] unless a CHECKED child has an empty or missing row i, a zero or missing
+ *     has_val byte i and i >= counts_len;
+ * and a CASCADE root with first or offset has its rows filtered by its new dest and paged.  The filters keep row order.
+ * out / out_off get every node's new rows (out_off has row_off[nnodes] + 1 values, node n's rows are rows row_off[n]
+ * .. row_off[n+1]), dest_out / dest_out_off (nnodes + 1 values) every node's new dest.  out_cap >= v_off[row_off[nnodes]]
+ * and dest_cap >= dest_off[nnodes] (the bounds) are required: DGX_ERR_CAP before anything is copied otherwise.
+ * DGX_ERR_ARG before anything is copied: nnodes >= 2^16, a parent not below its child, an unknown flag bit, a SKIP node
+ * with a child, a node deeper than 63 (64 levels), offsets not starting at 0 or decreasing, 2^32 or more rows, values or
+ * dest values in all, a null array that is needed.  DGX_ERR_ARG after the kernels, with nothing written to the outputs:
+ * a dest, or a row of a node without ORDERED, that does not strictly ascend.  nnodes == 0, or a forest without a dest
+ * value and a row value, writes zero offsets and needs no device.  Launches: 4 + 7 * D, D the levels holding a dest or
+ * a row value (DESIGN section 3.11). */
+int dgx_cascade(const dgx_cascade_tree* tree, const uint64_t* v, const uint64_t* v_off, const uint64_t* row_off,
+                const uint64_t* dest, const uint64_t* dest_off, const uint8_t* has_val, const uint64_t* hv_off,
+                uint64_t* out, uint64_t* out_off, size_t out_cap, uint64_t* dest_out, uint64_t* dest_out_off,
+                size_t dest_cap);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -645,6 +686,30 @@ int dgx_dev_recurse_filter(dgx_lane* lane, dgx_reach_set* set, const uint64_t* d
                            const uint64_t* d_v_off, size_t v_cap, const uint64_t* d_dest, size_t ndest,
                            uint64_t* d_out, uint64_t* d_out_off, size_t out_cap, uint64_t* d_dest_out,
                            size_t dest_cap, uint64_t* d_sizes);
+/* One node of dgx_dev_cascade, every pointer in device memory: its rows v[v_off[i] .. v_off[i+1]) (v_off has nrows + 1
+ * values, v_off[0] == 0, v_off[nrows] <= v_cap, the room of v), its dest (ndest values) and its has_val (nhas bytes). */
+typedef struct dgx_cascade_node {
+    const uint64_t* v;
+    const uint64_t* v_off;
+    size_t nrows;
+    size_t v_cap;
+    const uint64_t* dest;
+    size_t ndest;
+    const uint8_t* has_val;
+    size_t nhas;
+} dgx_cascade_node;
+/* Device form of dgx_cascade: tree and nodes in host memory, the arrays they point at in device memory, so the rows of
+ * dgx_dev_list_uids_unfiltered_rows and the dest of dgx_dev_merge_sorted_matrix feed it directly.  d_out_off gets
+ * sum(nrows) + 1 offsets, d_dest_out_off nnodes + 1, d_sizes two device uint64 {values, dest values}.  The bounds are
+ * sum(v_cap) and sum(ndest): out_cap or dest_cap below them is DGX_ERR_CAP at the call, as every argument error of the
+ * host form is DGX_ERR_ARG there (a null pointer with a nonzero size).  Offsets, and dest and rows that do not strictly
+ * ascend, are checked on the device: a refused call writes d_sizes = {0, 0} and nothing else, and surfaces as
+ * DGX_ERR_ARG at the next dgx_lane_sync.  A forest with no dest value and every v_cap 0 writes the zero offsets and
+ * sizes without a launch and without reading the nodes' v_off, which then go unchecked (every row is empty whatever
+ * they hold).  Asynchronous on the lane. */
+int dgx_dev_cascade(dgx_lane* lane, const dgx_cascade_tree* tree, const dgx_cascade_node* nodes, uint64_t* d_out,
+                    uint64_t* d_out_off, size_t out_cap, uint64_t* d_dest_out, uint64_t* d_dest_out_off,
+                    size_t dest_cap, uint64_t* d_sizes);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

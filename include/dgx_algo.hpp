@@ -360,6 +360,56 @@ private:
     dgx_reach_set* s_ = nullptr;
 };
 
+// One subgraph node of a @cascade forest, in pre-order (dgx_cascade): parent index (-1 for a query root), DGX_CASCADE_*
+// flags, Params.Cascade.First / Offset, len(counts), DestUIDs, uidMatrix rows and has_val (one byte per row).
+struct CascadeNode {
+    int64_t parent = -1;
+    uint8_t flags = 0;
+    int32_t first = 0, offset = 0;
+    uint64_t counts_len = 0;
+    pb::List dest;
+    std::vector<pb::List> rows;
+    std::vector<uint8_t> has_val;
+};
+
+// @cascade over a forest (query/query.go populateVarMap :1445-1527 and ProcessQuery's root pagination :3004-3011) in
+// one call: every node's rows and DestUIDs after the cascade, in node order.
+inline std::pair<std::vector<std::vector<pb::List>>, std::vector<pb::List>> Cascade(const std::vector<CascadeNode>& nodes) {
+    const size_t n = nodes.size();
+    std::vector<uint32_t> parent(n);
+    std::vector<uint8_t> flags(n), hv;
+    std::vector<int32_t> first(n), offset(n);
+    std::vector<uint64_t> counts(n), v, v_off{0}, row_off{0}, dest, dest_off{0}, hv_off{0};
+    for (size_t k = 0; k < n; ++k) {
+        const CascadeNode& c = nodes[k];
+        parent[k] = c.parent < 0 ? UINT32_MAX : (uint32_t)c.parent;
+        flags[k] = c.flags;
+        first[k] = c.first;
+        offset[k] = c.offset;
+        counts[k] = c.counts_len;
+        for (const pb::List& r : c.rows) { v.insert(v.end(), r.Uids.begin(), r.Uids.end()); v_off.push_back(v.size()); }
+        row_off.push_back(v_off.size() - 1);
+        dest.insert(dest.end(), c.dest.Uids.begin(), c.dest.Uids.end());
+        dest_off.push_back(dest.size());
+        hv.insert(hv.end(), c.has_val.begin(), c.has_val.end());
+        hv_off.push_back(hv.size());
+    }
+    const dgx_cascade_tree tree{n, parent.data(), flags.data(), first.data(), offset.data(), counts.data()};
+    std::vector<uint64_t> out(std::max<size_t>(v.size(), 1)), out_off(row_off.back() + 1),
+        dout(std::max<size_t>(dest.size(), 1)), dout_off(n + 1);
+    check(dgx_cascade(&tree, v.data(), v_off.data(), row_off.data(), dest.data(), dest_off.data(), hv.data(),
+                      hv_off.data(), out.data(), out_off.data(), v.size(), dout.data(), dout_off.data(), dest.size()));
+    std::pair<std::vector<std::vector<pb::List>>, std::vector<pb::List>> res;
+    for (size_t k = 0; k < n; ++k) {
+        std::vector<pb::List> rows;
+        for (uint64_t r = row_off[k]; r < row_off[k + 1]; ++r)
+            rows.emplace_back(std::vector<uint64_t>(out.begin() + out_off[r], out.begin() + out_off[r + 1]));
+        res.first.push_back(std::move(rows));
+        res.second.emplace_back(std::vector<uint64_t>(dout.begin() + dout_off[k], dout.begin() + dout_off[k + 1]));
+    }
+    return res;
+}
+
 }  // namespace algo
 
 // Wire-format adjacency (dgx_wire_*, host only): the bytes proto.Unmarshal sees at posting/list.go:1045 and

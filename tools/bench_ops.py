@@ -140,6 +140,7 @@ def main():
     ap.add_argument("--c12-only", action="store_true", help="only the C12 regexp() trigram query rows")
     ap.add_argument("--c13-only", action="store_true", help="only the C13 @groupby over a uid predicate rows")
     ap.add_argument("--c14-only", action="store_true", help="only the C14 @recurse filter rows")
+    ap.add_argument("--c15-only", action="store_true", help="only the C15 @cascade rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -159,9 +160,11 @@ def main():
         rows = c13_rows(Lane())
     elif args.c14_only:
         rows = c14_rows(Lane())
+    elif args.c15_only:
+        rows = c15_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1623,6 +1626,138 @@ def c14_rows(L):
                              "steps": len(steps), "values": vals, "kept": total, "check": bool(ok), "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del dev_in, dev_out
+    return out_rows
+
+
+def c15_chain(rng, levels=8, width=64, deg=4):
+    """C15b: a narrow chain of `levels` cascaded nodes, each with first: 2, offset: 1, `width` uids a level and about
+    `deg` values a row: launch-bound."""
+    from dgraph_b200.algo import CC_CASCADE, CC_CHECKED, CascadeNode
+
+    dest = np.arange(1, width + 1, dtype=np.uint64)
+    nodes = [CascadeNode(-1, CC_CASCADE, 2, 1, 0, dest, [dest])]
+    for k in range(1, levels):
+        rows = [np.unique(rng.integers(1, 2 * width, int(rng.integers(0, 2 * deg)))).astype(np.uint64)
+                for _ in range(nodes[-1].dest.size)]
+        d = np.unique(np.concatenate(rows)).astype(np.uint64)
+        nodes.append(CascadeNode(k - 1, CC_CASCADE | CC_CHECKED, 2, 1, 0, d, rows))
+    return nodes
+
+
+def c15_directive():
+    """C15c: TestCascadeDirective's tree (query/query0_test.go) on the friend fixture's uids: me(func: uid(0x01))
+    @cascade { name gender friend { name friend { name dob age } } } -- a handful of values."""
+    from dgraph_b200.algo import CC_CASCADE, CC_CHECKED, CascadeNode
+
+    C2 = CC_CASCADE | CC_CHECKED
+    f1 = np.array([23, 24, 25, 31, 101], np.uint64)
+    return [CascadeNode(-1, CC_CASCADE, 0, 0, 0, [1], [[1]]),
+            CascadeNode(0, C2, 0, 0, 0, [], [], [1]), CascadeNode(0, C2, 0, 0, 0, [], [], [1]),
+            CascadeNode(0, C2, 0, 0, 0, f1, [f1]),
+            CascadeNode(3, C2, 0, 0, 0, [], [], [1, 1, 1, 1, 0]),
+            CascadeNode(3, C2, 0, 0, 0, [1, 24], [[1], [], [], [24], []]),
+            CascadeNode(5, C2, 0, 0, 0, [], [], [1, 1]), CascadeNode(5, C2, 0, 0, 0, [], [], [1, 1]),
+            CascadeNode(5, C2, 0, 0, 0, [], [], [1, 1])]
+
+
+def c15_rows(L):
+    """C15 "@cascade": C15a, TestCascadeWithPaginationDeep scaled up (tests/gen_cascade.c15a_arrays: 1e6 Person roots,
+    friend rows Zipf over 2e6 uids, has_val densities 0.8 and 0.5, first: 2, offset: 1 at the leaf); C15b, a chain 8
+    levels deep with pagination at every level (launch-bound); C15c, TestCascadeDirective's tree.  Legs: (1) the device
+    form on resident inputs (CUDA events), (2) the host form (wall clock), (3) the line-by-line restatement
+    (tests/cascade_oracle.c) on 1 thread -- C, not Go.  Every leg is checked against the restatement."""
+    import cascade_oracle as co
+    import cascade_plan as cp
+    import gen_cascade as gc
+    from dgraph_b200.algo import cascade_arrays, cascade_tree
+
+    lib = L.lib
+
+    def up(x, dt=np.uint64):
+        x = np.ascontiguousarray(np.asarray(x, dt))
+        if x.size == 0:
+            x = np.zeros(1, dt)
+        return torch.from_numpy(x.view(np.int64) if dt == np.uint64 else x).to(DEV)
+
+    cases = [("C15a", gc.c15a_arrays(np.random.default_rng(15)), 3),
+             ("C15b", cascade_arrays(c15_chain(np.random.default_rng(16))), 50),
+             ("C15c", cascade_arrays(c15_directive()), 200)]
+    out_rows = []
+    for name, a, reps in cases:
+        n = a["nnodes"]
+        m, nd, nr = int(a["v_off"][-1]), int(a["dest_off"][-1]), int(a["row_off"][-1])
+        t0 = time.perf_counter()
+        want = co.cascade_flat(a)
+        t_or = (time.perf_counter() - t0) * 1e3
+        ok_or = True  # the restatement is the reference of the other legs
+        tree = cascade_tree(a)
+        # (1) device form: every node's arrays resident, the outputs resident
+        keep, descs = [], []
+        for k in range(n):
+            r0, r1 = int(a["row_off"][k]), int(a["row_off"][k + 1])
+            b0, b1 = int(a["v_off"][r0]), int(a["v_off"][r1])
+            dv, doff = up(a["v"][b0:b1]), up(a["v_off"][r0:r1 + 1] - np.uint64(b0))
+            dd = up(a["dest"][int(a["dest_off"][k]):int(a["dest_off"][k + 1])])
+            dh = up(a["has_val"][int(a["hv_off"][k]):int(a["hv_off"][k + 1])], np.uint8)
+            keep += [dv, doff, dd, dh]
+            descs.append(_lib.CascadeNode(dv.data_ptr(), doff.data_ptr(), r1 - r0, b1 - b0, dd.data_ptr(),
+                                          int(a["dest_off"][k + 1] - a["dest_off"][k]), dh.data_ptr(),
+                                          int(a["hv_off"][k + 1] - a["hv_off"][k])))
+        tab = (_lib.CascadeNode * n)(*descs)
+        d_out, d_oo, d_dout, d_do, d_sz = (torch.empty(x, dtype=torch.int64, device=DEV)
+                                           for x in (max(m, 1), nr + 1, max(nd, 1), n + 1, 2))
+
+        def dev():
+            _lib.check(lib.dgx_dev_cascade(L.h, C.byref(tree), tab, C.c_void_p(d_out.data_ptr()),
+                                           C.c_void_p(d_oo.data_ptr()), m, C.c_void_p(d_dout.data_ptr()),
+                                           C.c_void_p(d_do.data_ptr()), nd, C.c_void_p(d_sz.data_ptr())))
+        l0 = lib.dgx_lane_launches(L.h)
+        dev()
+        L.sync()
+        launches = lib.dgx_lane_launches(L.h) - l0
+        ms_dev, _ = timeit(dev, warm=2, reps=reps)
+        L.sync()
+        K, D = (int(x) for x in d_sz.cpu().numpy())
+        ok_dev = (np.array_equal(d_oo.cpu().numpy().view(np.uint64), want[1]) and
+                  np.array_equal(d_do.cpu().numpy().view(np.uint64), want[3]) and
+                  np.array_equal(d_out[:K].cpu().numpy().view(np.uint64), want[0][:K]) and
+                  np.array_equal(d_dout[:D].cpu().numpy().view(np.uint64), want[2][:D]))
+        # (2) host form
+        out, oo = np.empty(max(m, 1), np.uint64), np.empty(nr + 1, np.uint64)
+        dout, do = np.empty(max(nd, 1), np.uint64), np.empty(n + 1, np.uint64)
+        p = {k: a[k].ctypes.data for k in ("v", "v_off", "row_off", "dest", "dest_off", "has_val", "hv_off")}
+
+        def host():
+            _lib.check(lib.dgx_cascade(C.byref(tree), p["v"], p["v_off"], p["row_off"], p["dest"], p["dest_off"],
+                                       p["has_val"], p["hv_off"], out.ctypes.data, oo.ctypes.data, m,
+                                       dout.ctypes.data, do.ctypes.data, nd))
+        host()
+        hreps = max(1, min(reps, 20))
+        t0 = time.perf_counter()
+        for _ in range(hreps):
+            host()
+        t_host = (time.perf_counter() - t0) * 1e3 / hreps
+        ok_host = (np.array_equal(oo, want[1]) and np.array_equal(do, want[3]) and
+                   np.array_equal(out[:K], want[0][:K]) and np.array_equal(dout[:D], want[2][:D]))
+        depth, work = [0] * n, set()
+        for k in range(n):
+            pk = int(a["parent"][k])
+            depth[k] = 0 if pk == 0xFFFFFFFF else depth[pk] + 1
+            r0, r1 = int(a["row_off"][k]), int(a["row_off"][k + 1])
+            if a["dest_off"][k + 1] > a["dest_off"][k] or a["v_off"][r1] > a["v_off"][r0]:
+                work.add(depth[k])
+        levels = max(depth) + 1
+        ok_launch = launches == cp.launches(len(work))
+        cfg = f"{name}: {n} nodes, {levels} levels, {nr} rows, {m} row values, {nd} dest values -> {K} values, {D} dest"
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev and ok_launch,
+                                     f"dgx_dev_cascade, CUDA events, median of {reps} after 2 warm calls"),
+                                    ("host form", t_host, ok_host, f"dgx_cascade, wall clock, mean of {hreps} after "
+                                     "one warm call"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, ok_or, "orc_cascade, wall clock")):
+            out_rows.append({"op": "Cascade", "workload": name, "leg": leg, "config": cfg, "ms": round(ms, 4),
+                             "values": m, "launches": launches, "check": bool(ok), "timing": timing})
+            print(json.dumps(out_rows[-1]), flush=True)
+        del keep
     return out_rows
 
 
