@@ -59,6 +59,16 @@ class CascadeNode(C.Structure):
                 ("dest", C.c_void_p), ("ndest", C.c_size_t), ("has_val", C.c_void_p), ("nhas", C.c_size_t)]
 
 
+class PathLevel(C.Structure):
+    """dgx_path_level (include/dgx.h): one shortest-path expansion level, nsg sgs in exec order as CSR arrays."""
+    _fields_ = [("nsg", C.c_size_t), ("attr", C.c_void_p), ("src_off", C.c_void_p), ("src", C.c_void_p),
+                ("v_off", C.c_void_p), ("v", C.c_void_p), ("dest_off", C.c_void_p), ("dest", C.c_void_p)]
+
+
+class PathStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("edges", "discovered", "to_level")]
+
+
 class CacheStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("hits", "misses", "evictions", "bytes", "entries", "max_bytes")]
 
@@ -102,6 +112,10 @@ SYMBOLS = {
     "dgx_reach_size": (_int, [_vp, _szp]),
     "dgx_reach_export": (_int, [_vp, _vp, _vp, _sz, _szp]),
     "dgx_recurse_filter": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _szp]),
+    "dgx_path_create": (_int, [_u64, _u64, C.POINTER(_vp)]),
+    "dgx_path_destroy": (None, [_vp]),
+    "dgx_path_expand": (_int, [_vp, C.POINTER(PathLevel), _vp, _vp, _sz, C.POINTER(PathStats)]),
+    "dgx_path_result": (_int, [_vp, _vp, _vp, _sz, _szp]),
     "dgx_cascade": (_int, [C.POINTER(CascadeTree), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _sz]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
@@ -145,6 +159,7 @@ SYMBOLS = {
     "dgx_dev_list_count_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, _vp]),
     "dgx_dev_trigram_query": (_int, [_vp, C.POINTER(QueryTree), _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _vp]),
     "dgx_dev_recurse_filter": (_int, [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "dgx_dev_path_expand": (_int, [_vp, _vp, C.POINTER(PathLevel), _sz, _sz, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_cascade": (_int, [_vp, C.POINTER(CascadeTree), C.POINTER(CascadeNode), _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),

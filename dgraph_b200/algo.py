@@ -603,6 +603,88 @@ class ReachSet:
             pass
 
 
+def path_level_arrays(sgs):
+    """One shortest-path level as the CSR arrays of dgx_path_level: sgs is a list of (attr, src, rows, dest) in exec
+    order, rows[i] the values of src[i].  Returns (attr u32, src_off, src, v_off, v, dest_off, dest); empty arrays hold
+    one element so that every pointer is valid."""
+    attr = np.asarray([int(a) for a, _, _, _ in sgs], np.uint32)
+    srcs = [_u64(s.Uids if isinstance(s, List) else s) for _, s, _, _ in sgs]
+    rows = [r for _, _, rs, _ in sgs for r in rs]
+    for (_, _, rs, _), s in zip(sgs, srcs):
+        if len(rs) != s.size:
+            raise ValueError(f"{s.size} sources for {len(rs)} rows")
+    src, src_off = _csr_u64(srcs)
+    v, v_off = _csr_u64(rows)
+    dest, dest_off = _csr_u64([d.Uids if isinstance(d, List) else d for _, _, _, d in sgs])
+    return (attr if attr.size else np.zeros(1, np.uint32)), src_off, src, v_off, v, dest_off, dest
+
+
+def path_level(arrays, nsg: int) -> "_lib.PathLevel":
+    """The dgx_path_level over path_level_arrays' arrays (host) or over device tensors of the same layout."""
+    ptr = [a.ctypes.data if isinstance(a, np.ndarray) else a.data_ptr() for a in arrays]
+    return _lib.PathLevel(nsg, *ptr)
+
+
+class PathSearch:
+    """shortest() with numpaths <= 1 and no facets (query/shortest.go expandOut + shortestPath at unit cost): a
+    breadth-first search from `frm` to `to` held in device memory (dgx_path_search), one expand() per level."""
+
+    def __init__(self, frm: int, to: int):
+        self._ps = None
+        h = C.c_void_p()
+        _lib.check(_lib.load().dgx_path_create(int(frm), int(to), C.byref(h)))
+        self._ps = h
+
+    @property
+    def handle(self):
+        """The dgx_path_search pointer, for dgx_dev_path_expand."""
+        if self._ps is None:
+            raise ValueError("PathSearch is closed")
+        return self._ps
+
+    def expand(self, sgs):
+        """One level: sgs is a list of (attr, src, rows, dest) in exec order (attr the child index, rows[i] the values
+        of src[i], dest the sg's DestUIDs).  Returns (next SrcUIDs per sg, (edges, discovered, to_level))."""
+        if not sgs:
+            raise ValueError("a level has at least one sg")
+        arrs = path_level_arrays(sgs)
+        lv = path_level(arrs, len(sgs))
+        d = int(arrs[5][-1])
+        nxt, nxt_off = np.empty(max(d, 1), np.uint64), np.zeros(len(sgs) + 1, np.uint64)
+        st = _lib.PathStats()
+        _lib.check(_lib.load().dgx_path_expand(self.handle, C.byref(lv), _p(nxt), _p(nxt_off), d, C.byref(st)))
+        nexts = [nxt[int(nxt_off[i]):int(nxt_off[i + 1])].copy() for i in range(len(sgs))]
+        return nexts, (st.edges, st.discovered, st.to_level)
+
+    def path(self):
+        """(uids From .. To, attr index of each hop), both empty when To was not reached."""
+        n = C.c_size_t(0)
+        lib = _lib.load()
+        rc = lib.dgx_path_result(self.handle, None, None, 0, C.byref(n))
+        if rc != _lib.DGX_OK and n.value == 0:
+            _lib.check(rc)
+        uids, attrs = np.empty(max(n.value, 1), np.uint64), np.empty(max(n.value, 1), np.uint32)
+        _lib.check(lib.dgx_path_result(self.handle, _p(uids), _p(attrs), n.value, C.byref(n)))
+        return uids[: n.value].copy(), attrs[: max(n.value - 1, 0)].copy()
+
+    def close(self) -> None:
+        if self._ps is not None:
+            _lib.load().dgx_path_destroy(self._ps)
+            self._ps = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -42,6 +42,7 @@
 #include "groupby_kernel.cuh"
 #include "recurse_kernel.cuh"
 #include "cascade_kernel.cuh"
+#include "path_kernel.cuh"
 #include "wire.hpp"
 
 using namespace dgx;
@@ -466,6 +467,10 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
         if (flag & kLaneErrCascade)
             return fail(DGX_ERR_ARG, "a cascade input is malformed (a dest or an unordered row not strictly ascending, "
                                      "or row offsets not starting at 0, decreasing or past v_cap)");
+        if (flag & kLaneErrPath)
+            return fail(DGX_ERR_ARG, "a shortest-path level's input is malformed (src, a row or a dest not strictly "
+                                     "ascending, offsets not starting at 0, decreasing or past their caps, or a source "
+                                     "with a kept edge not discovered at the previous level)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -4388,6 +4393,357 @@ extern "C" int dgx_cascade(const dgx_cascade_tree* tree, const uint64_t* v, cons
     CK(cudaStreamSynchronize(l->stream));
     g_stats.d2h += (K + DN + rows + n + 4) * sizeof(uint64_t);
     g_stats.uids_out += K + DN;
+    return DGX_OK;
+}
+
+// ---------------------------------------------------------------------------
+// shortest() without weights: one expansion level of every exec sg, the search kept in HBM (path_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr uint64_t kPsMax = uint64_t(1) << 32;  // sgs, rows, values, dest values and set sizes are 32-bit counts
+
+// Seen buffer b holds uid[] at sbuf[b], parent[] at + 8 scap, attr[] at + 16 scap and level[] at + 20 scap bytes;
+// expanded buffer b is ebuf[b].  The current buffers, the sizes, the level count and To's level are device words
+// (d_state); st mirrors them as of the last wait.  sbound / ebound are the sizes then plus, for every level queued
+// since, its bound on new nodes (min(v_cap, dest_cap): a new node is a distinct dest value) and its src_cap, which size
+// the capacities without a round trip.
+struct dgx_path_search {
+    std::mutex mu;
+    int device = 0;
+    char* sbuf[2] = {nullptr, nullptr};
+    uint64_t* ebuf[2] = {nullptr, nullptr};
+    uint64_t scap = 0, ecap = 0;
+    uint64_t* d_state = nullptr;
+    uint64_t st[PS_STATE] = {};
+    uint64_t sbound = 0, ebound = 0;
+    dgx_lane* lane = nullptr;    // the lane of the device-form levels queued since the last wait
+    std::vector<void*> retired;  // buffers replaced by growth, still read by queued levels until the next wait
+};
+
+static void ps_free_retired(dgx_path_search* s) {
+    for (void* p : s->retired) cudaFree(p);
+    s->retired.clear();
+}
+
+// Waits for the search's queued levels and reads its words back.  Caller holds s->mu.
+static int ps_wait(dgx_path_search* s) {
+    CK(cudaSetDevice(s->device));
+    if (!s->lane) return DGX_OK;
+    CK(cudaMemcpyAsync(s->lane->h_word, s->d_state, sizeof(s->st), cudaMemcpyDeviceToHost, s->lane->stream));
+    CK(cudaStreamSynchronize(s->lane->stream));
+    memcpy(s->st, s->lane->h_word, sizeof(s->st));
+    s->sbound = s->st[PS_S_N];
+    s->ebound = s->st[PS_E_N];
+    s->lane = nullptr;
+    ps_free_retired(s);
+    return DGX_OK;
+}
+
+// Capacity for `need` records of `rec` bytes (columns of the given widths, each cap records long) in both buffers of a
+// ping-pong pair: they grow geometrically, their first `bound` records copied on the stream (the current buffer is only
+// known on the device while levels are queued).  The new buffers replace the old ones only once every copy is queued,
+// so an allocation or a copy that fails leaves the search as it was.
+static int ps_reserve(dgx_path_search* s, cudaStream_t stream, void** buf, uint64_t* cap, uint64_t need,
+                      std::initializer_list<size_t> cols, uint64_t bound, uint64_t cur, const char* what) {
+    if (need <= *cap) return DGX_OK;
+    const uint64_t ncap = std::max(need, 2 * *cap);
+    size_t rec = 0;
+    for (size_t c : cols) rec += c;
+    void* nb[2] = {nullptr, nullptr};
+    auto drop = [&](int code, const char* op) {
+        cudaGetLastError();
+        for (void* p : nb) if (p) cudaFree(p);
+        return fail(code, "shortest-path %s growth to %llu records: %s failed", what, (unsigned long long)ncap, op);
+    };
+    for (int b = 0; b < 2; ++b)
+        if (cudaMalloc(&nb[b], ncap * rec) != cudaSuccess) return drop(DGX_ERR_OOM, "cudaMalloc");
+    for (int b = 0; b < 2; ++b)
+        if (bound && (s->lane || (uint64_t)b == cur)) {  // an idle search's other buffer holds nothing live
+            size_t off = 0;
+            for (size_t c : cols) {
+                if (cudaMemcpyAsync((char*)nb[b] + off * ncap, (char*)buf[b] + off * *cap, bound * c,
+                                    cudaMemcpyDeviceToDevice, stream) != cudaSuccess) {
+                    if (stream) cudaStreamSynchronize(stream);  // copies already queued read and write nb
+                    return drop(DGX_ERR_CUDA, "cudaMemcpyAsync");
+                }
+                off += c;
+            }
+        }
+    for (int b = 0; b < 2; ++b) {
+        if (buf[b]) s->retired.push_back(buf[b]);
+        buf[b] = nb[b];
+    }
+    *cap = ncap;
+    return DGX_OK;
+}
+
+static int ps_reserve_all(dgx_path_search* s, cudaStream_t stream, uint64_t seen, uint64_t expanded) {
+    if (int rc = ps_reserve(s, stream, (void**)s->sbuf, &s->scap, seen, {8, 8, 4, 4}, s->sbound, s->st[PS_S_CUR], "seen"))
+        return rc;
+    return ps_reserve(s, stream, (void**)s->ebuf, &s->ecap, expanded, {8}, s->ebound, s->st[PS_E_CUR], "expanded");
+}
+
+extern "C" int dgx_path_create(uint64_t from, uint64_t to, dgx_path_search** ps) {
+    if (!ps) return fail(DGX_ERR_ARG, "null argument");
+    if (from == 0 || to == 0 || from == to)
+        return fail(DGX_ERR_ARG, "from %llu / to %llu: both nonzero and distinct", (unsigned long long)from,
+                    (unsigned long long)to);
+    if (int rc = dgx_init(-1)) return rc;
+    CK(cudaSetDevice(g_device));
+    dgx_path_search* s = new dgx_path_search();
+    s->device = g_device;
+    s->st[PS_S_N] = 1;
+    s->st[PS_TO] = to;
+    int rc = DGX_OK;
+    if (cudaMalloc(&s->d_state, sizeof(s->st)) != cudaSuccess) rc = fail(DGX_ERR_OOM, "path search allocation failed");
+    if (!rc) rc = ps_reserve_all(s, nullptr, 1024, 1024);
+    const uint64_t zero[2] = {0, 0};  // From's parent, and its attr and level as two u32
+    if (!rc && (cudaMemcpy(s->sbuf[0], &from, 8, cudaMemcpyHostToDevice) != cudaSuccess ||
+                cudaMemcpy(s->sbuf[0] + 8 * s->scap, zero, 8, cudaMemcpyHostToDevice) != cudaSuccess ||
+                cudaMemcpy(s->sbuf[0] + 16 * s->scap, zero, 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+                cudaMemcpy(s->sbuf[0] + 20 * s->scap, zero, 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+                cudaMemcpy(s->d_state, s->st, sizeof(s->st), cudaMemcpyHostToDevice) != cudaSuccess))
+        rc = fail(DGX_ERR_CUDA, "path search upload failed");
+    ps_free_retired(s);
+    s->sbound = 1;
+    if (rc) {
+        dgx_path_destroy(s);
+        return rc;
+    }
+    *ps = s;
+    return DGX_OK;
+}
+
+extern "C" void dgx_path_destroy(dgx_path_search* s) {
+    if (!s) return;
+    {
+        std::lock_guard<std::mutex> lk(s->mu);
+        ps_wait(s);
+        ps_free_retired(s);
+        for (char* b : s->sbuf) if (b) cudaFree(b);
+        for (uint64_t* b : s->ebuf) if (b) cudaFree(b);
+        if (s->d_state) cudaFree(s->d_state);
+    }
+    delete s;
+}
+
+// One level on the lane, for a search with room for sbound + min(v_cap, d_cap) seen nodes and ebound + r_cap expanded
+// sources: 5 launches, the two matrix merges', 6 launches.  Workspace: 52 bytes per value of v_cap (row and sg 8, new
+// flag and position 16, new value 8, N 8, parent 8, sg index 4), 40 per row, 16 per dest value, 8 per sg, the merges'
+// about 22 per value of their caps, and the scans' look-back words.  d_next, d_next_off and d_stats are written by the kernels.
+static int ps_level(dgx_lane* l, dgx_path_search* s, size_t nsg, const uint32_t* d_attr, const uint64_t* d_src_off,
+                    const uint64_t* d_src, uint64_t r_cap, const uint64_t* d_v_off, const uint64_t* d_v, uint64_t v_cap,
+                    const uint64_t* d_dest_off, const uint64_t* d_dest, uint64_t d_cap, uint64_t* d_next,
+                    uint64_t* d_next_off, uint64_t* d_stats) {
+    const uint64_t vc = std::max<uint64_t>(v_cap, 1), rc1 = std::max<uint64_t>(r_cap, 1), dc = std::max<uint64_t>(d_cap, 1);
+    auto tiles = [](uint64_t n) { return (n + EN_TILE - 1) / EN_TILE; };
+    const uint64_t tv = tiles(vc), tr = tiles(rc1), td = tiles(dc);
+    // zeroed: [bad | words | tickets | scan status | rflag | nsgi];  all ones: npar;  then the u64 and u32 arrays
+    const size_t b_head = 128, b_zero = b_head + (tv + tr + td + r_cap + 1) * sizeof(u64) + ((vc * 4 + 15) & ~15ull);
+    const size_t n64 = vc + (vc + 1) + (r_cap + 2) + vc + (r_cap + 2) + (r_cap + 1) + (nsg + 1) + vc + (r_cap + 1) +
+                       dc + (dc + 1);
+    void* d_raw;
+    int rc = l->ws.alloc(b_zero + (vc + n64) * sizeof(u64) + 2 * vc * sizeof(u32), &d_raw);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(d_raw, 0, b_zero, l->stream));
+    CK(cudaMemsetAsync((char*)d_raw + b_zero, 0xff, vc * sizeof(u64), l->stream));
+    PsParams P;
+    P.nsg = nsg;
+    P.attr = (const u32*)d_attr;
+    P.src_off = (const u64*)d_src_off;
+    P.src = (const u64*)d_src;
+    P.r_cap = r_cap;
+    P.v_off = (const u64*)d_v_off;
+    P.v = (const u64*)d_v;
+    P.v_cap = v_cap;
+    P.dest_off = (const u64*)d_dest_off;
+    P.dest = (const u64*)d_dest;
+    P.d_cap = d_cap;
+    for (int b = 0; b < 2; ++b) {
+        P.su[b] = (u64*)s->sbuf[b];
+        P.sp[b] = (u64*)(s->sbuf[b] + 8 * s->scap);
+        P.sa[b] = (u32*)(s->sbuf[b] + 16 * s->scap);
+        P.sl[b] = (u32*)(s->sbuf[b] + 20 * s->scap);
+        P.ex[b] = (u64*)s->ebuf[b];
+    }
+    P.state = (u64*)s->d_state;
+    char* p = (char*)d_raw;
+    P.bad = (int*)p;
+    P.words = (u64*)(p + 16);
+    u32* tickets = (u32*)(P.words + PS_WORDS);
+    u64* status = (u64*)(p + b_head);
+    P.rflag = status + tv + tr + td;
+    P.nsgi = (u32*)(P.rflag + r_cap + 1);
+    P.npar = (u64*)(p + b_zero);
+    P.vflag = P.npar + vc;
+    P.vpos = P.vflag + vc;
+    P.rpos = P.vpos + vc + 1;
+    P.nv = P.rpos + r_cap + 2;
+    P.nv_off = P.nv + vc;
+    P.es = P.nv_off + r_cap + 2;
+    P.es_off = P.es + r_cap + 1;
+    P.nn = P.es_off + nsg + 1;
+    P.ne = P.nn + vc;
+    P.dflag = P.ne + r_cap + 1;
+    P.dpos = P.dflag + dc;
+    P.vrow = (u32*)(P.dpos + dc + 1);
+    P.vsg = P.vrow + vc;
+    P.next = (u64*)d_next;
+    P.next_off = (u64*)d_next_off;
+    P.stats = (u64*)d_stats;
+    P.err = l->d_err;
+    static_assert(16 + PS_WORDS * sizeof(u64) + 3 * sizeof(u32) <= 128, "the level's head words fit their 128 bytes");
+    if ((char*)(P.vsg + vc) != p + b_zero + (vc + n64) * sizeof(u64) + 2 * vc * sizeof(u32))
+        return fail(DGX_ERR_CUDA, "shortest-path workspace layout mismatch");
+    ps_check_kernel<<<gb_grid(std::max<uint64_t>({nsg + 1, r_cap + 1, v_cap, d_cap})), 256, 0, l->stream>>>(P);
+    ps_flags_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)tv, EN_NT, 0, l->stream>>>(P.vflag, P.vpos, P.words + PS_W_M, v_cap, status, tickets,
+                                                           P.words + PS_W_NV);
+    scan_u64_kernel<<<(unsigned)tr, EN_NT, 0, l->stream>>>(P.rflag, P.rpos, P.words + PS_W_R, r_cap, status + tv,
+                                                           tickets + 1, P.words + PS_W_NR);
+    ps_gather_kernel<<<gb_grid(std::max<uint64_t>({v_cap, r_cap + 2, nsg + 1})), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 5);
+    auto U = [](u64* q) { return (uint64_t*)q; };
+    if ((rc = merge_matrix_impl(l, U(P.nv), U(P.nv_off), rc1, vc, U(P.nn), vc, U(P.words + PS_W_NN))) ||
+        (rc = merge_matrix_impl(l, U(P.es), U(P.es_off), nsg, rc1, U(P.ne), rc1, U(P.words + PS_W_NE))))
+        return rc;
+    ps_parent_kernel<<<gb_grid(std::max<uint64_t>(v_cap, d_cap)), 256, 0, l->stream>>>(P);
+    ps_attr_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)td, EN_NT, 0, l->stream>>>(P.dflag, P.dpos, P.words + PS_W_D, d_cap,
+                                                           status + tv + tr, tickets + 2, P.words + PS_W_NX);
+    ps_insert_kernel<<<stride_grid(), 256, 0, l->stream>>>(P);
+    ps_write_kernel<<<gb_grid(std::max<uint64_t>(d_cap, nsg + 1)), 256, 0, l->stream>>>(P);
+    ps_commit_kernel<<<1, 1, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 6);
+    return DGX_OK;
+}
+
+// The checks both forms make before anything is copied.  Caller holds s->mu.
+static int ps_check_level(dgx_path_search* s, const dgx_lane* l, size_t nsg, uint64_t rows, uint64_t values,
+                          uint64_t dests, size_t next_cap) {
+    const uint64_t fresh = std::min(values, dests);  // new nodes are distinct dest values
+    if (s->lane && s->lane != l)
+        return fail(DGX_ERR_ARG, "the path search has levels queued on another lane: wait for them with dgx_path_result");
+    if (nsg == 0 || nsg >= kPsMax || rows >= kPsMax || values >= kPsMax || dests >= kPsMax)
+        return fail(DGX_ERR_ARG, "shortest-path sizes are 32-bit: 1 to 2^32 - 1 sgs, rows, values and dests below 2^32");
+    if (s->sbound + fresh >= kPsMax || s->ebound + rows >= kPsMax)
+        return fail(DGX_ERR_ARG, "the path search could reach %llu nodes: at most 2^32 - 1",
+                    (unsigned long long)(s->sbound + fresh));
+    if (next_cap < dests)
+        return fail(DGX_ERR_CAP, "next_cap %zu below the %llu dest values", next_cap, (unsigned long long)dests);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_path_expand(dgx_lane* l, dgx_path_search* s, const dgx_path_level* L, size_t src_cap,
+                                   size_t v_cap, size_t dest_cap, uint64_t* d_next, uint64_t* d_next_off,
+                                   size_t next_cap, uint64_t* d_stats) {
+    if (!l || !s || !L || !d_stats || !d_next_off || !L->attr || !L->src_off || !L->v_off || !L->dest_off ||
+        (src_cap && !L->src) || (v_cap && !L->v) || (dest_cap && (!L->dest || !d_next)))
+        return fail(DGX_ERR_ARG, "null argument");
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (int rc = ps_check_level(s, l, L->nsg, src_cap, v_cap, dest_cap, next_cap)) return rc;
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    const uint64_t fresh = std::min<uint64_t>(v_cap, dest_cap);
+    if (int rc = ps_reserve_all(s, l->stream, s->sbound + fresh, s->ebound + src_cap)) return rc;
+    s->lane = l;  // queued copies or levels now read the search
+    s->sbound += fresh;
+    s->ebound += src_cap;
+    if (int rc = ps_level(l, s, L->nsg, L->attr, L->src_off, L->src, src_cap, L->v_off, L->v, v_cap, L->dest_off,
+                          L->dest, dest_cap, d_next, d_next_off, d_stats))
+        return rc;
+    g_stats.uids_in += v_cap;
+    l->note_output(d_next, next_cap * sizeof(uint64_t));
+    l->note_output(d_next_off, (L->nsg + 1) * sizeof(uint64_t));
+    l->note_output(d_stats, 3 * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_path_expand(dgx_path_search* s, const dgx_path_level* L, uint64_t* next, uint64_t* next_off,
+                               size_t next_cap, dgx_path_stats* stats) {
+    if (!L || !next_off || !stats || !L->attr || !L->src_off || !L->dest_off) return fail(DGX_ERR_ARG, "null argument");
+    const size_t S = L->nsg;
+    if (S == 0 || S >= kPsMax) return fail(DGX_ERR_ARG, "nsg of %zu: 1 to 2^32 - 1", S);
+    if (int rc = check_offsets("src_off", L->src_off, S, kPsMax)) return rc;
+    if (int rc = check_offsets("dest_off", L->dest_off, S, kPsMax)) return rc;
+    const uint64_t R = L->src_off[S], D = L->dest_off[S];
+    if (R && (!L->src || !L->v_off)) return fail(DGX_ERR_ARG, "null argument");
+    if (R) if (int rc = check_offsets("v_off", L->v_off, R, kPsMax)) return rc;
+    const uint64_t M = R ? L->v_off[R] : 0;
+    if ((M && !L->v) || (D && (!L->dest || !next))) return fail(DGX_ERR_ARG, "null argument");
+    if (R >= kPsMax || M >= kPsMax || D >= kPsMax) return fail(DGX_ERR_ARG, "shortest-path sizes are 32-bit");
+    if (next_cap < D) return fail(DGX_ERR_CAP, "next_cap %zu below the %llu dest values", next_cap, (unsigned long long)D);
+    if (!s) return fail(DGX_ERR_ARG, "null path search");  // the level's own errors are reported first
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (int rc = ps_check_level(s, nullptr, S, R, M, D, next_cap)) return rc;
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += R + M + D;
+    static const uint64_t zero = 0;
+    uint64_t *d_src_off, *d_src, *d_v_off, *d_v, *d_dest_off, *d_dest;
+    void *d_attr, *d_o;
+    int rc;
+    if ((rc = upload_list(l, L->src_off, S + 1, &d_src_off)) || (rc = upload_list(l, L->src, R, &d_src)) ||
+        (rc = upload_list(l, R ? L->v_off : &zero, R + 1, &d_v_off)) || (rc = upload_list(l, L->v, M, &d_v)) ||
+        (rc = upload_list(l, L->dest_off, S + 1, &d_dest_off)) || (rc = upload_list(l, L->dest, D, &d_dest)) ||
+        (rc = l->ws.alloc(S * sizeof(uint32_t), &d_attr)))
+        return rc;
+    CK(cudaMemcpyAsync(d_attr, L->attr, S * sizeof(uint32_t), cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += S * sizeof(uint32_t);
+    if ((rc = l->ws.alloc((S + 4 + D + 1) * sizeof(uint64_t), &d_o))) return rc;
+    uint64_t* d_stats = (uint64_t*)d_o;  // stats, then next_off: read back in one copy
+    uint64_t* d_next_off = d_stats + 3;
+    uint64_t* d_next = d_next_off + S + 1;
+    if ((rc = ps_reserve_all(s, l->stream, s->sbound + std::min(M, D), s->ebound + R))) return rc;
+    s->lane = l;  // waited for below, whatever happens
+    s->sbound += std::min(M, D);
+    s->ebound += R;
+    rc = ps_level(l, s, S, (const uint32_t*)d_attr, d_src_off, d_src, R, d_v_off, d_v, M, d_dest_off, d_dest, D,
+                  d_next, d_next_off, d_stats);
+    std::vector<uint64_t> head(S + 4);
+    if (!rc) CK(cudaMemcpyAsync(head.data(), d_stats, (S + 4) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (int wrc = ps_wait(s)) return wrc;
+    if (rc || (rc = dgx_lane_sync(l))) return rc;
+    const uint64_t NX = head[3 + S];
+    if (NX) CK(cudaMemcpyAsync(next, d_next, NX * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    memcpy(next_off, head.data() + 3, (S + 1) * sizeof(uint64_t));
+    stats->edges = head[0];
+    stats->discovered = head[1];
+    stats->to_level = head[2];
+    g_stats.d2h += (S + 4 + NX) * sizeof(uint64_t);
+    g_stats.uids_out += NX;
+    return DGX_OK;
+}
+
+extern "C" int dgx_path_result(dgx_path_search* s, uint64_t* uids, uint32_t* attrs, size_t cap, size_t* len) {
+    if (!s || !len) return fail(DGX_ERR_ARG, "null argument");
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (int rc = ps_wait(s)) return rc;
+    const uint64_t L = s->st[PS_TO_LEVEL], n = L ? L + 1 : 0;
+    *len = n;
+    if (n > cap) return fail(DGX_ERR_CAP, "a path of %llu uids does not fit cap %zu", (unsigned long long)n, cap);
+    if (n == 0) return DGX_OK;
+    if (!uids || !attrs) return fail(DGX_ERR_ARG, "null argument");
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    void* d_o;
+    if (int rc = l->ws.alloc(n * sizeof(uint64_t) + L * sizeof(uint32_t), &d_o)) return rc;
+    const uint64_t c = s->st[PS_S_CUR];
+    ps_walk_kernel<<<1, 1, 0, l->stream>>>((const u64*)s->sbuf[c], (const u64*)(s->sbuf[c] + 8 * s->scap),
+                                           (const u32*)(s->sbuf[c] + 16 * s->scap), (const u64*)s->d_state, L,
+                                           (u64*)d_o, (u32*)((uint64_t*)d_o + n));
+    CK(cudaGetLastError());
+    count_launches(l, 1);
+    CK(cudaMemcpyAsync(uids, d_o, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(attrs, (uint64_t*)d_o + n, L * sizeof(uint32_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += n * sizeof(uint64_t) + L * sizeof(uint32_t);
     return DGX_OK;
 }
 

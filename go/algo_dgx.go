@@ -558,3 +558,124 @@ func cArray[T any](v []T) (unsafe.Pointer, func()) {
 	copy(unsafe.Slice((*T)(p), len(v)), v)
 	return p, func() { C.free(p) }
 }
+
+// dgxMinShortest: a shortest() block goes to the device when the rows of its first level (From's edges over every
+// child) hold at least this many values; below it Go's shortestPath runs.  From the C16 record
+// (profiles/h100_c16_shortest.json, H100 80GB HBM3, 700 W): C16c, TestShortestPath4's 3 levels of 20 values, takes
+// 0.70 ms through the host form, about 0.23 ms a level, and the C restatement spends about 2.4 us per row value at
+// C16a's sizes, so the two meet near 100 values a level.  The restatement is C, not Go, and a first level is the
+// smallest of a search, so the bound errs towards the Go path.
+const dgxMinShortest = 1 << 10
+
+// PathSearch is shortest() with numpaths <= 1 and no facets (query/shortest.go expandOut + shortestPath at unit
+// cost) as a breadth-first search held in device memory.  Create one per query with NewPathSearch, call Expand once
+// per level with that level's exec sgs in exec order, read the answer with Path, and Close it.
+type PathSearch struct{ ps *C.dgx_path_search }
+
+// PathSg is one exec sg of a level: the index of its child in sg.Children, SrcUIDs, the uidMatrix after
+// updateUidMatrix (one row per source) and DestUIDs.
+type PathSg struct {
+	Attr   uint32
+	Src    []uint64
+	Matrix []*pb.List
+	Dest   []uint64
+}
+
+// PathStats is one level's result: its numEdges, the nodes it discovered, and To's level (0 while unreached).
+type PathStats struct{ Edges, Discovered, ToLevel uint64 }
+
+// NewPathSearch starts a search from `from` to `to`.  It returns false when the library refuses them (a uid of 0,
+// from == to, no device); the caller runs Go's shortestPath.
+func NewPathSearch(from, to uint64) (*PathSearch, bool) {
+	var ps *C.dgx_path_search
+	if C.dgx_path_create(C.uint64_t(from), C.uint64_t(to), &ps) != C.DGX_OK {
+		return nil, false
+	}
+	return &PathSearch{ps: ps}, true
+}
+
+// Expand runs one level over the exec sgs and returns each sg's next SrcUIDs.  ok == false, on any library error,
+// means nothing was written: the caller closes the search and runs Go's shortestPath from the start.
+func (p *PathSearch) Expand(sgs []PathSg) (next [][]uint64, st PathStats, ok bool) {
+	n := len(sgs)
+	if n == 0 {
+		return nil, st, false
+	}
+	attr := make([]uint32, n)
+	srcOff, destOff := make([]uint64, n+1), make([]uint64, n+1)
+	var src, vOff, v, dest []uint64
+	vOff = append(vOff, 0)
+	for i, sg := range sgs {
+		if len(sg.Matrix) != len(sg.Src) {
+			return nil, st, false
+		}
+		attr[i] = sg.Attr
+		src = append(src, sg.Src...)
+		srcOff[i+1] = uint64(len(src))
+		for _, l := range sg.Matrix {
+			if l != nil {
+				v = append(v, l.Uids...)
+			}
+			vOff = append(vOff, uint64(len(v)))
+		}
+		dest = append(dest, sg.Dest...)
+		destOff[i+1] = uint64(len(dest))
+	}
+	// the level struct points at its arrays, so it and they live in C memory: Go memory handed to C must not hold Go
+	// pointers
+	frees := []func(){}
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+	}()
+	carr := func(q unsafe.Pointer, free func()) unsafe.Pointer {
+		frees = append(frees, free)
+		return q
+	}
+	lv := (*C.dgx_path_level)(carr(cArray([]C.dgx_path_level{{nsg: C.size_t(n)}})))
+	lv.attr = (*C.uint32_t)(carr(cArray(attr)))
+	lv.src_off = (*C.uint64_t)(carr(cArray(srcOff)))
+	lv.src = (*C.uint64_t)(carr(cArray(src)))
+	lv.v_off = (*C.uint64_t)(carr(cArray(vOff)))
+	lv.v = (*C.uint64_t)(carr(cArray(v)))
+	lv.dest_off = (*C.uint64_t)(carr(cArray(destOff)))
+	lv.dest = (*C.uint64_t)(carr(cArray(dest)))
+	out, outOff := make([]uint64, len(dest)+1), make([]uint64, n+1)
+	var cst C.dgx_path_stats
+	if C.dgx_path_expand(p.ps, lv, u64ptr(out), u64ptr(outOff), C.size_t(len(dest)), &cst) != C.DGX_OK {
+		return nil, st, false
+	}
+	next = make([][]uint64, n)
+	for i := range next {
+		lo, hi := outOff[i], outOff[i+1]
+		next[i] = out[lo:hi:hi]
+	}
+	return next, PathStats{Edges: uint64(cst.edges), Discovered: uint64(cst.discovered),
+		ToLevel: uint64(cst.to_level)}, true
+}
+
+// Path returns the path From .. To and the child index of each hop (attrs[i] is the hop into uids[i+1]), both empty
+// when To was not reached.
+func (p *PathSearch) Path() (uids []uint64, attrs []uint32, ok bool) {
+	var n C.size_t
+	if rc := C.dgx_path_result(p.ps, nil, nil, 0, &n); rc != C.DGX_OK && rc != C.DGX_ERR_CAP {
+		return nil, nil, false
+	}
+	if n == 0 {
+		return nil, nil, true
+	}
+	uids, attrs = make([]uint64, int(n)), make([]uint32, int(n))
+	if C.dgx_path_result(p.ps, u64ptr(uids), (*C.uint32_t)(unsafe.Pointer(&attrs[0])), n, &n) != C.DGX_OK {
+		return nil, nil, false
+	}
+	return uids, attrs[:int(n)-1], true
+}
+
+// Close frees the search's device memory.
+func (p *PathSearch) Close() {
+	if p.ps != nil {
+		C.dgx_path_destroy(p.ps)
+		p.ps = nil
+	}
+}

@@ -417,6 +417,57 @@ int dgx_recurse_filter(dgx_reach_set* set, const uint64_t* src, size_t nrows, co
                        const uint64_t* dest, size_t ndest, uint64_t* out, uint64_t* out_off, size_t out_cap,
                        uint64_t* dest_out, size_t dest_cap, size_t* dest_len);
 
+/* shortest() with numpaths <= 1 and no facets, so every edge costs 1 (query/shortest.go expandOut :141-273 and
+ * shortestPath :457-618): a breadth-first search held in device memory for the life of one query.  It keeps
+ *   seen      the discovered nodes, each with its parent, the attr index of the hop into it and its level (From: 0);
+ *   expanded  the sources that have had a kept edge (adjacencyMap's keys).
+ * Level k's rules, which Go's Dijkstra loop reduces to at unit cost (DESIGN section 5):
+ *   - a row value is kept iff it is in its sg's dest (updateUidMatrix); stats.edges counts the kept values of every sg
+ *     (the level's numEdges: an edge held by two sgs counts twice);
+ *   - a kept value not yet in seen is discovered at level k; its parent is the smallest source with a kept edge to it
+ *     at this level, and its attr index is attr[s] of the largest sg index s holding (parent, node);
+ *   - every source with a kept edge joins expanded, and sg s's next SrcUIDs are its dest minus expanded;
+ *   - a source with a kept edge must be a node discovered at the previous level (at level 1: From), as every such
+ *     source of Go's exec lists is; any other is refused, which also refuses a source already expanded.
+ * Calls on one search are serialised by the library; different searches may be used concurrently.  A search that a
+ * device-form level bound to a lane must be waited for (dgx_path_result) or destroyed before that lane is. */
+typedef struct dgx_path_search dgx_path_search;
+/* One level: nsg sgs in exec order.  Sg s has the child index attr[s], the sources src[src_off[s] .. src_off[s+1])
+ * (strictly ascending), one row per source (row r = v[v_off[r] .. v_off[r+1]), strictly ascending) and its DestUIDs
+ * dest[dest_off[s] .. dest_off[s+1]) (strictly ascending).  Host memory for dgx_path_expand, device memory for
+ * dgx_dev_path_expand. */
+typedef struct {
+    size_t nsg;
+    const uint32_t* attr;      /* nsg */
+    const uint64_t* src_off;   /* nsg + 1 */
+    const uint64_t* src;       /* src_off[nsg] */
+    const uint64_t* v_off;     /* src_off[nsg] + 1 */
+    const uint64_t* v;         /* v_off[src_off[nsg]] */
+    const uint64_t* dest_off;  /* nsg + 1 */
+    const uint64_t* dest;      /* dest_off[nsg] */
+} dgx_path_level;
+/* edges: the level's numEdges; discovered: the nodes it reached first; to_level: To's level, 0 while unreached. */
+typedef struct {
+    uint64_t edges, discovered, to_level;
+} dgx_path_stats;
+/* A search from `from` to `to`: seen = {from at level 0}, expanded empty.  DGX_ERR_ARG: a uid of 0, or from == to. */
+int dgx_path_create(uint64_t from, uint64_t to, dgx_path_search** ps);
+void dgx_path_destroy(dgx_path_search* ps);
+/* Expands one level (the rules above) and returns each sg's next SrcUIDs as CSR over the sgs: next_off has nsg + 1
+ * values, next[next_off[s] .. next_off[s+1]).  Each input array is copied to the device once.
+ * DGX_ERR_ARG before anything is copied: a null array that is needed, nsg of 0, offsets not starting at 0 or
+ * decreasing, nsg, rows, values or dests of 2^32 or more, a search that could reach 2^32 nodes.  DGX_ERR_CAP before
+ * anything is copied: next_cap below dest_off[nsg].  DGX_ERR_ARG after the kernels: src, a row or a dest not strictly
+ * ascending, or a source with a kept edge not discovered at the previous level.  A refused level writes nothing to the outputs and
+ * leaves the search unchanged.  Launches: 11 plus two matrix merges of 7 + max(1, ceil(log2 ceil(n / 2048))) each,
+ * with n = max(1, values) and max(1, rows) (DESIGN section 3.12), whatever the sg count and the set sizes. */
+int dgx_path_expand(dgx_path_search* ps, const dgx_path_level* level, uint64_t* next, uint64_t* next_off,
+                    size_t next_cap, dgx_path_stats* stats);
+/* Waits for the search's queued levels and returns the path From .. To: uids[0 .. len) and attrs[0 .. len - 1) (attrs[i]
+ * is the attr index of the hop into uids[i + 1]), both with room for cap.  len is To's level + 1, or 0 when To was not
+ * reached.  DGX_ERR_CAP with *len set and nothing written when len exceeds cap.  One launch. */
+int dgx_path_result(dgx_path_search* ps, uint64_t* uids, uint32_t* attrs, size_t cap, size_t* len);
+
 /* @cascade over a forest of subgraph nodes (query/query.go populateVarMap :1445-1527, updateUidMatrix :1425-1439
  * without facets, and ProcessQuery's root pagination :3004-3011), in pre-order: parent[n] is UINT32_MAX for a query root
  * and below n otherwise.  flags[n] is a set of DGX_CASCADE_* bits resolved on the host; first[n] / offset[n] are
@@ -686,6 +737,19 @@ int dgx_dev_recurse_filter(dgx_lane* lane, dgx_reach_set* set, const uint64_t* d
                            const uint64_t* d_v_off, size_t v_cap, const uint64_t* d_dest, size_t ndest,
                            uint64_t* d_out, uint64_t* d_out_off, size_t out_cap, uint64_t* d_dest_out,
                            size_t dest_cap, uint64_t* d_sizes);
+/* Device form of dgx_path_expand: every array of *level in device memory, offsets and attr included, so the rows of
+ * dgx_dev_list_uids_unfiltered_rows and the dest of dgx_dev_merge_sorted_matrix feed it directly.  src_cap, v_cap and
+ * dest_cap are the room of src, v and dest (the offsets must end inside them) and stand for the host form's counts in
+ * its limits: next_cap below dest_cap is DGX_ERR_CAP.  d_stats is three device uint64 {edges, discovered, to_level}.
+ * Sizes, missing pointers and a search bound to another lane are DGX_ERR_ARG at the call.  Every other check
+ * (offsets, ascending src, rows and dests, the level of sources with an edge) runs on the device: a refused level writes nothing, leaves
+ * the search unchanged and surfaces as DGX_ERR_ARG at the next dgx_lane_sync.  Asynchronous on the lane: the search is
+ * bound to it until waited for.  Growing the search past its capacity allocates device memory (24 bytes per node in
+ * each of two buffers, reserved for min(v_cap, dest_cap) new nodes per queued level; 8 bytes per source in each of
+ * two buffers, for src_cap per level); DGX_ERR_OOM leaves it unchanged.  Launches as the host form's with values = v_cap and rows = src_cap. */
+int dgx_dev_path_expand(dgx_lane* lane, dgx_path_search* ps, const dgx_path_level* level, size_t src_cap,
+                        size_t v_cap, size_t dest_cap, uint64_t* d_next, uint64_t* d_next_off, size_t next_cap,
+                        uint64_t* d_stats);
 /* One node of dgx_dev_cascade, every pointer in device memory: its rows v[v_off[i] .. v_off[i+1]) (v_off has nrows + 1
  * values, v_off[0] == 0, v_off[nrows] <= v_cap, the room of v), its dest (ndest values) and its has_val (nhas bytes). */
 typedef struct dgx_cascade_node {

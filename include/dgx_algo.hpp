@@ -410,6 +410,74 @@ inline std::pair<std::vector<std::vector<pb::List>>, std::vector<pb::List>> Casc
     return res;
 }
 
+// shortest() with numpaths <= 1 and no facets (query/shortest.go expandOut + shortestPath at unit cost): a
+// breadth-first search from `from` to `to` held in device memory (dgx_path_search), one Expand per level; move-only.
+class PathSearch {
+public:
+    PathSearch(uint64_t from, uint64_t to) { check(dgx_path_create(from, to, &ps_)); }
+    PathSearch(PathSearch&& o) noexcept : ps_(o.ps_) { o.ps_ = nullptr; }
+    PathSearch& operator=(PathSearch&& o) noexcept {
+        std::swap(ps_, o.ps_);
+        return *this;
+    }
+    PathSearch(const PathSearch&) = delete;
+    PathSearch& operator=(const PathSearch&) = delete;
+    ~PathSearch() { dgx_path_destroy(ps_); }
+
+    // One exec sg: the child index, SrcUIDs (strictly ascending), one row per source, and DestUIDs.
+    struct Sg {
+        uint32_t attr = 0;
+        std::vector<uint64_t> src;
+        std::vector<pb::List> rows;
+        pb::List dest;
+    };
+    struct Level {
+        std::vector<pb::List> next;  // each sg's next SrcUIDs
+        dgx_path_stats stats{};      // {numEdges of the level, nodes discovered, To's level or 0}
+    };
+    // One level over the exec sgs in exec order.
+    Level Expand(const std::vector<Sg>& sgs) {
+        std::vector<uint32_t> attr;
+        std::vector<uint64_t> src_off{0}, src, v_off{0}, v, dest_off{0}, dest;
+        for (const Sg& sg : sgs) {
+            if (sg.src.size() != sg.rows.size()) throw Error(DGX_ERR_ARG, "one source per row");
+            attr.push_back(sg.attr);
+            src.insert(src.end(), sg.src.begin(), sg.src.end());
+            src_off.push_back(src.size());
+            for (const pb::List& r : sg.rows) {
+                v.insert(v.end(), r.Uids.begin(), r.Uids.end());
+                v_off.push_back(v.size());
+            }
+            dest.insert(dest.end(), sg.dest.Uids.begin(), sg.dest.Uids.end());
+            dest_off.push_back(dest.size());
+        }
+        const dgx_path_level lv{sgs.size(), attr.data(), src_off.data(), src.data(), v_off.data(), v.data(),
+                                dest_off.data(), dest.data()};
+        std::vector<uint64_t> next(std::max<size_t>(dest.size(), 1)), next_off(sgs.size() + 1);
+        Level out;
+        check(dgx_path_expand(ps_, &lv, next.data(), next_off.data(), dest.size(), &out.stats));
+        for (size_t i = 0; i < sgs.size(); ++i)
+            out.next.emplace_back(std::vector<uint64_t>(next.begin() + next_off[i], next.begin() + next_off[i + 1]));
+        return out;
+    }
+    // The path From .. To and the child index of each hop; both empty when To was not reached.
+    std::pair<std::vector<uint64_t>, std::vector<uint32_t>> Path() {
+        size_t n = 0;
+        const int rc = dgx_path_result(ps_, nullptr, nullptr, 0, &n);
+        if (rc != DGX_OK && rc != DGX_ERR_CAP) check(rc);
+        std::vector<uint64_t> uids(std::max<size_t>(n, 1));
+        std::vector<uint32_t> attrs(std::max<size_t>(n, 1));
+        check(dgx_path_result(ps_, uids.data(), attrs.data(), n, &n));
+        uids.resize(n);
+        attrs.resize(n ? n - 1 : 0);
+        return {uids, attrs};
+    }
+    dgx_path_search* handle() const { return ps_; }
+
+private:
+    dgx_path_search* ps_ = nullptr;
+};
+
 }  // namespace algo
 
 // Wire-format adjacency (dgx_wire_*, host only): the bytes proto.Unmarshal sees at posting/list.go:1045 and

@@ -141,6 +141,7 @@ def main():
     ap.add_argument("--c13-only", action="store_true", help="only the C13 @groupby over a uid predicate rows")
     ap.add_argument("--c14-only", action="store_true", help="only the C14 @recurse filter rows")
     ap.add_argument("--c15-only", action="store_true", help="only the C15 @cascade rows")
+    ap.add_argument("--c16-only", action="store_true", help="only the C16 shortest() rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -162,9 +163,11 @@ def main():
         rows = c14_rows(Lane())
     elif args.c15_only:
         rows = c15_rows(Lane())
+    elif args.c16_only:
+        rows = c16_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1624,6 +1627,122 @@ def c14_rows(L):
                                     ("restatement, 1 thread (C, not Go)", t_or, ok_or, "orc_recurse_sg, wall clock")):
             out_rows.append({"op": "RecurseFilter", "workload": name, "leg": leg, "config": cfg, "ms": round(ms, 4),
                              "steps": len(steps), "values": vals, "kept": total, "check": bool(ok), "timing": timing})
+            print(json.dumps(out_rows[-1]), flush=True)
+        del dev_in, dev_out
+    return out_rows
+
+
+def c16_rows(L):
+    """C16 "shortest() without weights": searches with Go's exec structure (tests/gen_shortest.py), each level's arrays
+    precomputed on the host (gen_shortest.plan) so the legs time the search, not the row reads.  C16a: C14's 2e6-node
+    Zipf friend graph, from a random root to a node at the deepest level reached within 6 hops.  C16b: { friend follow }
+    over C14b's 2e5-node graph, depth 5 (up to 2^k sgs at level k), to a node at the deepest level reached.  C16c: the
+    fixture's TestShortestPath4 search (launch-bound).  C16d: C16a's graph and root with an unreachable To.  Legs, each
+    a whole search: (1) the device form on resident inputs (CUDA events, the path read at the end), (2) the host form
+    (wall clock), (3) the line-by-line restatement (tests/shortest_oracle.c) on 1 thread -- C, not Go.  Every leg is
+    checked against the plan's formula: the device and host forms level by level and by path, the restatement by
+    reachability, path length and each level's numEdges."""
+    import gen_recurse as gr
+    import gen_shortest as gs
+    import shortest_oracle as so
+    from dgraph_b200 import algo
+
+    lib = L.lib
+    big = gr.c14_graph(np.random.default_rng(14))
+    small = gr.c14_graph(np.random.default_rng(15), 200_000)
+
+    def graph_of(g, preds):
+        return gs.Graph(g[preds[0]].ptr.size - 1, [(g[p].ptr.astype(np.uint64), g[p].idx) for p in preds],
+                        [(i, None) for i in range(len(preds))])
+
+    ga, gb = graph_of(big, ["friend"]), graph_of(small, ["friend", "follow"])
+    with open(os.path.join(ROOT, "tests", "golden", "shortest_path_follow.json")) as f:
+        gc, fc, tc, _ = gs.fixture_case(json.load(f), "TestShortestPath4")
+    rng = np.random.default_rng(16)
+    root_a, root_b = int(rng.integers(1, 2_000_001)), int(rng.integers(1, 200_001))
+
+    def deepest(g, frm, hops):
+        lv, f = gs.plan(g, frm, g.nnodes + 5, hops)
+        far = np.flatnonzero(f.level_of == f.level_of.max())
+        return int(far[len(far) // 2])
+
+    cases = [("C16a", ga, root_a, deepest(ga, root_a, 6), 6), ("C16b", gb, root_b, deepest(gb, root_b, 5), 5),
+             ("C16c", gc, fc, tc, None), ("C16d", ga, root_a, ga.nnodes + 5, 6)]
+    out_rows = []
+
+    def dp(t):
+        return t.data_ptr()
+
+    def up(x):
+        x = np.concatenate([x, np.zeros(1, x.dtype)])
+        return torch.from_numpy(x.view(np.int32 if x.dtype == np.uint32 else np.int64)).to(DEV)
+
+    for name, g, frm, to, hops in cases:
+        levels, f = gs.plan(g, frm, to, hops)
+        want_u, want_a = f.path()
+        vals = sum(int(a[4].size) for a, _, _, _ in levels)
+        sgs = sum(int(a[0].size) for a, _, _, _ in levels)
+        # (1) device form: inputs and outputs resident
+        dev_in = [[up(x) for x in a] for a, _, _, _ in levels]
+        dev_lv = [_lib.PathLevel(int(a[0].size), *[dp(x) for x in t]) for (a, _, _, _), t in zip(levels, dev_in)]
+        dev_out = [(torch.empty(max(int(a[6].size), 1), dtype=torch.int64, device=DEV),
+                    torch.empty(int(a[0].size) + 1, dtype=torch.int64, device=DEV),
+                    torch.empty(3, dtype=torch.int64, device=DEV)) for a, _, _, _ in levels]
+        holder = {}
+
+        def dev():
+            with algo.PathSearch(frm, to) as ps:
+                for (a, _, _, _), lv, (dn, do, dst) in zip(levels, dev_lv, dev_out):
+                    _lib.check(lib.dgx_dev_path_expand(L.h, ps.handle, C.byref(lv), a[2].size, a[4].size, a[6].size,
+                                                       dp(dn), dp(do), a[6].size, dp(dst)))
+                holder["path"] = ps.path()  # waits for the queued levels
+        ms_dev, _ = timeit(dev, warm=1, reps=3)
+        L.sync()
+        ok_dev = np.array_equal(holder["path"][0], want_u) and np.array_equal(holder["path"][1], want_a)
+        for (a, nxt, noff, st), (dn, do, dst) in zip(levels, dev_out):
+            k = int(noff[-1])
+            ok_dev &= (tuple(int(x) for x in dst.cpu().numpy()) == st and
+                       np.array_equal(do.cpu().numpy().view(np.uint64), noff) and
+                       np.array_equal(dn[:k].cpu().numpy().view(np.uint64), nxt))
+        # (2) host form
+        bufs = [(np.empty(max(int(a[6].size), 1), np.uint64), np.empty(int(a[0].size) + 1, np.uint64),
+                 _lib.PathStats()) for a, _, _, _ in levels]
+        hkeep = [[x if x.size else np.zeros(1, x.dtype) for x in a] for a, _, _, _ in levels]
+        host_lv = [_lib.PathLevel(int(a[0].size), *[x.ctypes.data for x in k]) for (a, _, _, _), k in
+                   zip(levels, hkeep)]
+
+        def host():
+            with algo.PathSearch(frm, to) as ps:
+                for (a, _, _, _), lv, (n, no, st) in zip(levels, host_lv, bufs):
+                    _lib.check(lib.dgx_path_expand(ps.handle, C.byref(lv), n.ctypes.data, no.ctypes.data, a[6].size,
+                                                   C.byref(st)))
+                return ps.path()
+        host()
+        t0 = time.perf_counter()
+        hp = host()
+        t_host = (time.perf_counter() - t0) * 1e3
+        ok_host = np.array_equal(hp[0], want_u) and np.array_equal(hp[1], want_a) and all(
+            (st.edges, st.discovered, st.to_level) == w[3] and np.array_equal(no, w[2]) and
+            np.array_equal(n[:int(w[2][-1])], w[1]) for w, (n, no, st) in zip(levels, bufs))
+        # (3) the restatement, 1 thread
+        t0 = time.perf_counter()
+        r = so.run(g, frm, to, hops, 0x9E3779B97F4A7C15)
+        t_or = (time.perf_counter() - t0) * 1e3
+        L_ = f.to_level
+        k = len(levels)
+        ok_or = ((to in r.dist) == bool(L_) and r.level_edges[:k] == [w[3][0] for w in levels] and
+                 (r.levels in (L_, L_ + 1) if L_ else r.levels == k) and len(r.path) == (L_ + 1 if L_ else 0))
+        cfg = (f"{name}: {len(g.children)} child(ren), {g.nnodes - 1} nodes, {k} levels, {sgs} sgs, {vals} row "
+               f"values, {'To at level ' + str(L_) if L_ else 'To unreachable'}")
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev, "dgx_dev_path_expand per level and "
+                                     "dgx_path_result, CUDA events, median of 3 after one warm search"),
+                                    ("host form", t_host, ok_host, "dgx_path_expand per level and dgx_path_result, "
+                                     "wall clock, one search after one warm search"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, ok_or, "orc_shortest including its "
+                                     "ProcessGraph restatement, wall clock")):
+            out_rows.append({"op": "ShortestPath", "workload": name, "leg": leg, "config": cfg, "ms": round(ms, 4),
+                             "levels": k, "sgs": sgs, "values": vals, "to_level": L_, "check": bool(ok),
+                             "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del dev_in, dev_out
     return out_rows
