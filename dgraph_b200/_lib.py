@@ -69,6 +69,12 @@ class PathStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("edges", "discovered", "to_level")]
 
 
+class VarLevel(C.Structure):
+    """dgx_var_level (include/dgx.h): one node of a value variable's path, its SrcUIDs, uid matrix and DestUIDs."""
+    _fields_ = [("src", C.c_void_p), ("v_off", C.c_void_p), ("v", C.c_void_p), ("dest", C.c_void_p),
+                ("nrows", C.c_size_t), ("v_cap", C.c_size_t), ("ndest", C.c_size_t)]
+
+
 class CacheStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("hits", "misses", "evictions", "bytes", "entries", "max_bytes")]
 
@@ -112,6 +118,8 @@ SYMBOLS = {
     "dgx_reach_size": (_int, [_vp, _szp]),
     "dgx_reach_export": (_int, [_vp, _vp, _vp, _sz, _szp]),
     "dgx_recurse_filter": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _szp]),
+    "dgx_var_propagate": (_int, [_int, _vp, _vp, _sz, C.POINTER(VarLevel), _sz, _vp, _vp, _sz, _szp]),
+    "dgx_var_level_agg": (_int, [_int, _int, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _szp]),
     "dgx_path_create": (_int, [_u64, _u64, C.POINTER(_vp)]),
     "dgx_path_destroy": (None, [_vp]),
     "dgx_path_expand": (_int, [_vp, C.POINTER(PathLevel), _vp, _vp, _sz, C.POINTER(PathStats)]),
@@ -159,6 +167,8 @@ SYMBOLS = {
     "dgx_dev_list_count_rows": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _u64, _vp]),
     "dgx_dev_trigram_query": (_int, [_vp, C.POINTER(QueryTree), _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, _vp]),
     "dgx_dev_recurse_filter": (_int, [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "dgx_dev_var_propagate": (_int, [_vp, _int, _vp, _vp, _sz, C.POINTER(VarLevel), _sz, _vp, _vp, _sz, _vp]),
+    "dgx_dev_var_level_agg": (_int, [_vp, _int, _int, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_path_expand": (_int, [_vp, _vp, C.POINTER(PathLevel), _sz, _sz, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_cascade": (_int, [_vp, C.POINTER(CascadeTree), C.POINTER(CascadeNode), _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),

@@ -685,6 +685,77 @@ class PathSearch:
             pass
 
 
+VAL_INT64, VAL_FLOAT64 = 1, 2  # DGX_VAL_* (include/dgx.h)
+AGG = {"min": 0, "max": 1, "sum": 2, "avg": 3}  # DGX_AGG_*
+
+
+def _val_map(keys, vals):
+    """(type, keys u64, values as u64 words) of a value map: int64 values are DGX_VAL_INT64, float64 DGX_VAL_FLOAT64."""
+    v = np.asarray(vals)
+    if v.dtype == np.int64:
+        typ = VAL_INT64
+    elif v.dtype == np.float64:
+        typ = VAL_FLOAT64
+    else:
+        raise TypeError(f"a value map holds int64 or float64 values, not {v.dtype}")
+    k = _u64(keys.Uids if isinstance(keys, List) else keys)
+    if k.size != v.size:
+        raise ValueError(f"{k.size} keys for {v.size} values")
+    w = np.ascontiguousarray(v).view(np.uint64)
+    return typ, (k if k.size else np.zeros(1, np.uint64)), (w if w.size else np.zeros(1, np.uint64)), k.size
+
+
+def _val_out(typ, key, val, n):
+    return key[:n].copy(), val[:n].view(np.float64 if typ == VAL_FLOAT64 else np.int64).copy()
+
+
+def var_level_arrays(src, rows, dest):
+    """One level of a value variable's path as host arrays (src, v_off, v, dest), each holding at least one value,
+    and its ndest."""
+    s = _u64(src.Uids if isinstance(src, List) else src)
+    if s.size != len(rows):
+        raise ValueError(f"{s.size} sources for {len(rows)} rows")
+    v, v_off = _csr_u64(rows)
+    d = _u64(dest.Uids if isinstance(dest, List) else dest)
+    return (s if s.size else np.zeros(1, np.uint64)), v_off, v, (d if d.size else np.zeros(1, np.uint64)), d.size
+
+
+def PropagateVar(keys, vals, levels):
+    """transformTo (query/query.go :1143-1236) over a whole path in ONE call (dgx_var_propagate).
+
+    keys: the map's uids, strictly ascending; vals: int64 or float64 values (the map's type).  levels: the path's nodes
+    from len(fromNode.path) on, index 0 skipped, each (SrcUIDs, uidMatrix rows, DestUIDs).  Returns the map at the last
+    level as (keys, values of the same dtype)."""
+    if not levels:
+        raise ValueError("a path has at least one level")
+    typ, k, w, n = _val_map(keys, vals)
+    arrs = [var_level_arrays(*lv) for lv in levels]
+    lv = (_lib.VarLevel * len(arrs))()
+    for i, (s, o, v, d, nd) in enumerate(arrs):
+        lv[i] = _lib.VarLevel(s.ctypes.data, o.ctypes.data, v.ctypes.data, d.ctypes.data, o.size - 1, int(o[-1]), nd)
+    cap = arrs[-1][4]
+    ok, ov = np.empty(max(cap, 1), np.uint64), np.empty(max(cap, 1), np.uint64)
+    m = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_var_propagate(typ, _p(k), _p(w), n, lv, len(arrs), _p(ok), _p(ov), cap, C.byref(m)))
+    return _val_out(typ, ok, ov, m.value)
+
+
+def LevelAgg(fn: str, keys, vals, src, rows):
+    """evalLevelAgg's per-row branch (query/query.go :1088-1123) in ONE call (dgx_var_level_agg): fn one of min, max,
+    sum, avg over the map (keys, int64 or float64 vals) for every row of relSG's uid matrix (rows[i] the values of
+    src[i]).  Returns (keys, values): float64 for avg, the map's dtype otherwise."""
+    if fn not in AGG:
+        raise ValueError(f"unknown aggregation {fn!r}")
+    typ, k, w, n = _val_map(keys, vals)
+    s, v_off, v, _, _ = var_level_arrays(src, rows, ())
+    nrows = v_off.size - 1
+    ok, ov = np.empty(max(nrows, 1), np.uint64), np.empty(max(nrows, 1), np.uint64)
+    m = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_var_level_agg(typ, AGG[fn], _p(k), _p(w), n, _p(s), nrows, _p(v_off), _p(v), _p(ok),
+                                             _p(ov), nrows, C.byref(m)))
+    return _val_out(VAL_FLOAT64 if fn == "avg" else typ, ok, ov, m.value)
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

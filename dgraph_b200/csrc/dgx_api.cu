@@ -43,6 +43,7 @@
 #include "recurse_kernel.cuh"
 #include "cascade_kernel.cuh"
 #include "path_kernel.cuh"
+#include "valvar_kernel.cuh"
 #include "wire.hpp"
 
 using namespace dgx;
@@ -471,6 +472,10 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
             return fail(DGX_ERR_ARG, "a shortest-path level's input is malformed (src, a row or a dest not strictly "
                                      "ascending, offsets not starting at 0, decreasing or past their caps, or a source "
                                      "with a kept edge not discovered at the previous level)");
+        if (flag & kLaneErrVar)
+            return fail(DGX_ERR_ARG, "a value-variable input is malformed (map keys, src or dest not strictly ascending, "
+                                     "offsets not starting at 0, decreasing or past v_cap, or a row value missing from "
+                                     "its level's dest)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -3525,17 +3530,18 @@ static GbPlan gb_plan(uint64_t nrows, uint64_t ndest, uint64_t npar) {
 }
 
 // One stable LSD pass per 8 key bits, ping-ponging between k[0] / p[0] and k[1] / p[1]: the result is in buffer
-// passes & 1.  Three launches per pass.
-static int gb_sort(dgx_lane* l, const GbParams& P, u64* const k[2], u32* const p[2], const u64* n_word,
-                   uint32_t passes, u64* hist, u64* hoff, u64*& status, u32*& ticket) {
-    const uint64_t hn = (uint64_t)GB_RADIX * P.tiles, ht = (hn + EN_TILE - 1) / EN_TILE;
+// passes & 1.  Three launches per pass.  `tiles` radix tiles cover the items; *h_word must hold GB_RADIX * tiles (the
+// hist scan's length) and *bad stops every pass.
+static int gb_sort(dgx_lane* l, uint64_t tiles, const int* bad, const u64* h_word, u64* const k[2], u32* const p[2],
+                   const u64* n_word, uint32_t passes, u64* hist, u64* hoff, u64*& status, u32*& ticket) {
+    const uint64_t hn = (uint64_t)GB_RADIX * tiles, ht = (hn + EN_TILE - 1) / EN_TILE;
     for (uint32_t q = 0; q < passes; ++q) {
         const int a = q & 1;
         const u32 shift = q * GB_DIGIT_BITS;
-        gb_hist_kernel<<<(unsigned)P.tiles, GB_NT, 0, l->stream>>>(k[a], n_word, P.bad, shift, P.tiles, hist);
-        scan_u64_kernel<<<(unsigned)ht, EN_NT, 0, l->stream>>>(hist, hoff, P.words + GB_W_H, hn, status, ticket, nullptr);
-        gb_scatter_kernel<<<(unsigned)P.tiles, GB_NT, 0, l->stream>>>(k[a], p[a], n_word, P.bad, shift, P.tiles, hoff,
-                                                                       k[a ^ 1], p[a ^ 1]);
+        gb_hist_kernel<<<(unsigned)tiles, GB_NT, 0, l->stream>>>(k[a], n_word, bad, shift, tiles, hist);
+        scan_u64_kernel<<<(unsigned)ht, EN_NT, 0, l->stream>>>(hist, hoff, h_word, hn, status, ticket, nullptr);
+        gb_scatter_kernel<<<(unsigned)tiles, GB_NT, 0, l->stream>>>(k[a], p[a], n_word, bad, shift, tiles, hoff,
+                                                                     k[a ^ 1], p[a ^ 1]);
         CK(cudaGetLastError());
         status += ht;
         ticket += 1;
@@ -3608,7 +3614,9 @@ static int gb_back(dgx_lane* l, GbParams& P, const GbPlan& g, u32* ticket) {
     P.ep = ep[0];
     gb_expand_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
     CK(cudaGetLastError());
-    if ((rc = gb_sort(l, P, ek, ep, P.words + GB_W_E, g.p1, hist, hoff, status, ticket))) return rc;
+    if ((rc = gb_sort(l, P.tiles, P.bad, P.words + GB_W_H, ek, ep, P.words + GB_W_E, g.p1, hist, hoff, status,
+                      ticket)))
+        return rc;
     P.ek = ek[g.p1 & 1];
     P.ep = ep[g.p1 & 1];
     gb_heads_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
@@ -3619,7 +3627,9 @@ static int gb_back(dgx_lane* l, GbParams& P, const GbPlan& g, u32* ticket) {
     gb_groups_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
     gb_gkeys_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P, gk[0], gp[0]);
     CK(cudaGetLastError());
-    if ((rc = gb_sort(l, P, gk, gp, P.words + GB_W_G, g.p2, hist, hoff, status, ticket))) return rc;
+    if ((rc = gb_sort(l, P.tiles, P.bad, P.words + GB_W_H, gk, gp, P.words + GB_W_G, g.p2, hist, hoff, status,
+                      ticket)))
+        return rc;
     P.gk = gk[g.p2 & 1];
     P.gp = gp[g.p2 & 1];
     gb_sizes_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
@@ -4745,6 +4755,359 @@ extern "C" int dgx_path_result(dgx_path_search* s, uint64_t* uids, uint32_t* att
     CK(cudaStreamSynchronize(l->stream));
     g_stats.d2h += n * sizeof(uint64_t) + L * sizeof(uint32_t);
     return DGX_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Value variables: transformTo over a path and evalLevelAgg's per-row fold (valvar_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr uint64_t kVvMax = uint64_t(1) << 32;  // map sizes, levels, rows, values and dest sizes are 32-bit counts
+
+static uint64_t vv_tiles(uint64_t n) { return std::max<uint64_t>(1, (n + EN_TILE - 1) / EN_TILE); }
+static uint64_t vv_rtiles(uint64_t n) { return std::max<uint64_t>(1, (n + GB_TILE - 1) / GB_TILE); }
+
+// Radix passes of a level: a dest rank needs bits(ndest - 1), the range two more.
+static uint32_t vv_passes(uint64_t ndest) {
+    return (gb_bits(ndest ? ndest - 1 : 0) + VV_RANGE_BITS + GB_DIGIT_BITS - 1) / GB_DIGIT_BITS;
+}
+
+// One level with device pointers; v_cap bounds v_off[nrows].
+struct VvLevel {
+    const uint64_t *src, *v_off, *v, *dest;
+    uint64_t nrows, v_cap, ndest;
+};
+
+// Every level on the lane, 9 + 3 P launches each (P = vv_passes(ndest)).  Workspace: 128 bytes of words and tickets per
+// level and the scans' look-back words, zeroed; 72 bytes per value of the largest v_cap (flag and position 16, keys
+// before and after the compaction 16, payloads 8, heads, head indices, segment starts and parts 32) and the largest
+// radix hist; both intermediate maps, 16 bytes per entry of the largest intermediate ndest.  The last level
+// writes out_key / out_val / *out_len, or only *out_len when the result passes out_cap.
+static int vv_run(dgx_lane* l, bool is_float, const uint64_t* d_key, const uint64_t* d_val, uint64_t n,
+                  const VvLevel* L, size_t nl, uint64_t* out_key, uint64_t* out_val, uint64_t out_cap,
+                  uint64_t* out_len) {
+    uint64_t vc = 1, hn = GB_RADIX, mcap = 1, zst = 0;
+    for (size_t k = 0; k < nl; ++k) {
+        const uint64_t c = std::max<uint64_t>(L[k].v_cap, 1), h = (uint64_t)GB_RADIX * vv_rtiles(c);
+        vc = std::max(vc, c);
+        hn = std::max(hn, h);
+        zst += 2 * vv_tiles(c) + vv_passes(L[k].ndest) * vv_tiles(h);
+        if (k + 1 < nl) mcap = std::max<uint64_t>(mcap, L[k].ndest);
+    }
+    const size_t b_head = 64 + 128 * nl, b_zero = b_head + zst * sizeof(u64);
+    const size_t n64 = 8 * vc + 3 + hn + (hn + 1) + 4 * mcap, n32 = 2 * vc;
+    void *z, *w;
+    int rc = l->ws.alloc(b_zero, &z);
+    if (rc) return rc;
+    if ((rc = l->ws.alloc(n64 * sizeof(u64) + n32 * sizeof(u32), &w))) return rc;
+    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
+    int* bad = (int*)z;
+    u64* status = (u64*)((char*)z + b_head);
+    u64* q = (u64*)w;
+    u64* flag = q;
+    u64* pos = flag + vc;
+    u64* ek[2] = {pos + vc + 1, pos + 2 * vc + 1};  // compacted keys, and the raw keys (then the sort's spare)
+    u64* head = ek[1] + vc;
+    u64* hidx = head + vc;
+    u64* sstart = hidx + vc + 1;
+    u64* part = sstart + vc + 1;
+    u64* hist = part + vc;
+    u64* hoff = hist + hn;
+    u64* mk[2] = {hoff + hn + 1, hoff + hn + 1 + mcap};
+    u64* mv[2] = {mk[1] + mcap, mk[1] + 2 * mcap};
+    u32* ep[2] = {(u32*)(mv[1] + mcap), (u32*)(mv[1] + mcap) + vc};
+    static_assert(64 + VV_WORDS * sizeof(u64) + 8 * sizeof(u32) <= 64 + 128, "a level's words and tickets fit");
+    if ((char*)(ep[1] + vc) != (char*)w + n64 * sizeof(u64) + n32 * sizeof(u32))
+        return fail(DGX_ERR_CUDA, "value-variable workspace layout mismatch");
+    const u64* prev_n = nullptr;
+    for (size_t k = 0; k < nl; ++k) {
+        const VvLevel& V = L[k];
+        const uint64_t c = std::max<uint64_t>(V.v_cap, 1), tv = vv_tiles(c);
+        const uint32_t passes = vv_passes(V.ndest);
+        u64* words = (u64*)((char*)z + 64 + 128 * k);
+        u32* ticket = (u32*)(words + VV_WORDS);
+        VvParams P{};
+        P.first = k == 0;
+        P.n0 = n;
+        P.mk = k ? mk[(k - 1) & 1] : (const u64*)d_key;
+        P.mv = k ? mv[(k - 1) & 1] : (const u64*)d_val;
+        P.mn = k ? prev_n : words + VV_W_N0;
+        P.src = (const u64*)V.src;
+        P.nrows = V.nrows;
+        P.v_off = (const u64*)V.v_off;
+        P.v = (const u64*)V.v;
+        P.v_cap = V.v_cap;
+        P.dest = (const u64*)V.dest;
+        P.ndest = V.ndest;
+        P.is_float = is_float;
+        P.tiles = vv_rtiles(c);
+        P.words = words;
+        P.bad = bad;
+        P.err = l->d_err;
+        P.flag = flag;
+        P.pos = pos;
+        P.ek_in = ek[0];
+        P.ek_raw = ek[1];
+        P.ep_in = ep[0];
+        P.ep_raw = ep[1];
+        P.head = head;
+        P.hidx = hidx;
+        P.sstart = sstart;
+        P.part = part;
+        const bool last = k + 1 == nl;
+        P.ok = last ? (u64*)out_key : mk[k & 1];
+        P.ov = last ? (u64*)out_val : mv[k & 1];
+        P.on = last ? (u64*)out_len : words + VV_W_NX;
+        P.o_cap = last ? out_cap : V.ndest;
+        prev_n = words + VV_W_NX;
+        vv_check_kernel<<<gb_grid(std::max<uint64_t>({V.nrows + 1, V.v_cap, V.ndest, k ? 0 : n})), 256, 0,
+                          l->stream>>>(P);
+        vv_flags_kernel<<<gb_grid(V.v_cap), 256, 0, l->stream>>>(P);
+        scan_u64_kernel<<<(unsigned)tv, EN_NT, 0, l->stream>>>(flag, pos, words + VV_W_M, V.v_cap, status, ticket,
+                                                               words + VV_W_E);
+        status += tv;
+        ticket += 1;
+        vv_compact_kernel<<<gb_grid(V.v_cap), 256, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        if ((rc = gb_sort(l, P.tiles, bad, words + VV_W_H, ek, ep, words + VV_W_E, passes, hist, hoff, status,
+                          ticket)))
+            return rc;
+        P.ek = ek[passes & 1];
+        P.ep = ep[passes & 1];
+        vv_heads_kernel<<<gb_grid(V.v_cap), 256, 0, l->stream>>>(P);
+        scan_u64_kernel<<<(unsigned)tv, EN_NT, 0, l->stream>>>(head, hidx, words + VV_W_E, V.v_cap, status, ticket,
+                                                               words + VV_W_SG);
+        status += tv;
+        vv_starts_kernel<<<gb_grid(V.v_cap), 256, 0, l->stream>>>(P);
+        vv_fold_kernel<<<gb_grid(V.v_cap), 256, 0, l->stream>>>(P);
+        vv_combine_kernel<<<gb_grid(V.v_cap), 256, 0, l->stream>>>(P);
+        CK(cudaGetLastError());
+        count_launches(l, 9);
+    }
+    return DGX_OK;
+}
+
+// The argument checks both forms make before anything is copied.  The host form's v_cap is v_off[nrows].
+static int vv_check_type(int type) {
+    if (type != DGX_VAL_INT64 && type != DGX_VAL_FLOAT64) return fail(DGX_ERR_ARG, "unknown value type %d", type);
+    return DGX_OK;
+}
+
+static int vv_check_levels(const VvLevel* L, size_t nl) {
+    for (size_t k = 0; k < nl; ++k) {
+        const VvLevel& V = L[k];
+        if (V.nrows >= kVvMax || V.v_cap >= kVvMax || V.ndest >= kVvMax)
+            return fail(DGX_ERR_ARG, "level %zu: rows, values and dest values are 32-bit counts", k);
+        if (!V.v_off || (V.nrows && !V.src) || (V.v_cap && !V.v) || (V.ndest && !V.dest))
+            return fail(DGX_ERR_ARG, "level %zu: null argument", k);
+    }
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_var_propagate(dgx_lane* l, int type, const uint64_t* d_key, const uint64_t* d_val, size_t n,
+                                     const dgx_var_level* levels, size_t nlevels, uint64_t* d_out_key,
+                                     uint64_t* d_out_val, size_t out_cap, uint64_t* d_out_len) {
+    if (!l || !levels || !d_out_len || (n && (!d_key || !d_val)) || (out_cap && (!d_out_key || !d_out_val)))
+        return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = vv_check_type(type)) return rc;
+    if (nlevels == 0 || nlevels >= kVvMax || n >= kVvMax)
+        return fail(DGX_ERR_ARG, "nlevels of 1 to 2^32 - 1 and a map below 2^32 entries");
+    std::vector<VvLevel> L(nlevels);
+    for (size_t k = 0; k < nlevels; ++k)
+        L[k] = {levels[k].src, levels[k].v_off, levels[k].v, levels[k].dest, levels[k].nrows, levels[k].v_cap,
+                levels[k].ndest};
+    if (int rc = vv_check_levels(L.data(), nlevels)) return rc;
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_out_len, sizeof(uint64_t));
+    if (n == 0) {  // transformTo returns an empty map as it is
+        CK(cudaMemsetAsync(d_out_len, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = vv_run(l, type == DGX_VAL_FLOAT64, d_key, d_val, n, L.data(), nlevels, d_out_key, d_out_val, out_cap,
+                        d_out_len))
+        return rc;
+    g_stats.uids_in += n;
+    l->note_output(d_out_key, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_val, out_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+// Copies *d_len entries of the two device arrays to the host when they fit cap: DGX_ERR_CAP with *len set otherwise.
+static int vv_finish(dgx_lane* l, const uint64_t* d_len, const uint64_t* d_key, const uint64_t* d_val, uint64_t* key,
+                     uint64_t* val, size_t cap, size_t* len) {
+    CK(cudaMemcpyAsync(l->h_word, d_len, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (int rc = dgx_lane_sync(l)) return rc;
+    const uint64_t G = l->h_word[0];
+    *len = G;
+    if (G > cap) return fail(DGX_ERR_CAP, "%llu entries do not fit out_cap %zu", (unsigned long long)G, cap);
+    if (G) {
+        CK(cudaMemcpyAsync(key, d_key, G * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+        CK(cudaMemcpyAsync(val, d_val, G * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    }
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += 2 * G * sizeof(uint64_t);
+    g_stats.uids_out += G;
+    return DGX_OK;
+}
+
+extern "C" int dgx_var_propagate(int type, const uint64_t* key, const uint64_t* val, size_t n,
+                                 const dgx_var_level* levels, size_t nlevels, uint64_t* out_key, uint64_t* out_val,
+                                 size_t out_cap, size_t* out_len) {
+    if (!levels || !out_len || (n && (!key || !val)) || (out_cap && (!out_key || !out_val)))
+        return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = vv_check_type(type)) return rc;
+    if (nlevels == 0 || nlevels >= kVvMax || n >= kVvMax)
+        return fail(DGX_ERR_ARG, "nlevels of 1 to 2^32 - 1 and a map below 2^32 entries");
+    std::vector<VvLevel> L(nlevels);
+    for (size_t k = 0; k < nlevels; ++k) {
+        const dgx_var_level& V = levels[k];
+        if (V.nrows >= kVvMax) return fail(DGX_ERR_ARG, "level %zu: nrows of 2^32 or more", k);
+        if (!V.v_off) return fail(DGX_ERR_ARG, "level %zu: null argument", k);
+        if (int rc = check_offsets("v_off", V.v_off, V.nrows, kVvMax)) return rc;
+        L[k] = {V.src, V.v_off, V.v, V.dest, V.nrows, V.v_off[V.nrows], V.ndest};
+    }
+    if (int rc = vv_check_levels(L.data(), nlevels)) return rc;
+    if (n == 0) {  // transformTo returns an empty map as it is
+        *out_len = 0;
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += n;
+    uint64_t *d_key, *d_val;  // one copy of each array
+    int rc;
+    if ((rc = upload_list(l, key, n, &d_key)) || (rc = upload_list(l, val, n, &d_val))) return rc;
+    for (size_t k = 0; k < nlevels; ++k) {
+        VvLevel& V = L[k];
+        uint64_t *s, *o, *v, *d;
+        if ((rc = upload_list(l, V.src, V.nrows, &s)) || (rc = upload_list(l, V.v_off, V.nrows + 1, &o)) ||
+            (rc = upload_list(l, V.v, V.v_cap, &v)) || (rc = upload_list(l, V.dest, V.ndest, &d)))
+            return rc;
+        V.src = s;
+        V.v_off = o;
+        V.v = v;
+        V.dest = d;
+        g_stats.uids_in += V.nrows + V.v_cap + V.ndest;
+    }
+    const uint64_t D = L[nlevels - 1].ndest;  // the last map has at most one entry per dest value
+    void* d_o;
+    if ((rc = l->ws.alloc((2 * D + 1) * sizeof(uint64_t), &d_o))) return rc;
+    uint64_t* o_len = (uint64_t*)d_o;
+    if ((rc = vv_run(l, type == DGX_VAL_FLOAT64, d_key, d_val, n, L.data(), nlevels, o_len + 1, o_len + 1 + D, D,
+                     o_len)))
+        return rc;
+    return vv_finish(l, o_len, o_len + 1, o_len + 1 + D, out_key, out_val, out_cap, out_len);
+}
+
+// 4 launches.  Workspace: 24 bytes per row and the scan's look-back words.
+static int la_run(dgx_lane* l, int fn, bool is_float, const uint64_t* d_key, const uint64_t* d_val, uint64_t n,
+                  const uint64_t* d_src, uint64_t nrows, const uint64_t* d_v_off, const uint64_t* d_v, uint64_t v_cap,
+                  uint64_t* out_key, uint64_t* out_val, uint64_t out_cap, uint64_t* out_len) {
+    const uint64_t tr = vv_tiles(nrows);
+    const size_t b_zero = 64 + tr * sizeof(u64);
+    void *z, *w;
+    int rc = l->ws.alloc(b_zero, &z);
+    if (rc) return rc;
+    if ((rc = l->ws.alloc((3 * nrows + 1) * sizeof(u64), &w))) return rc;
+    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
+    VaParams P{};
+    P.mk = (const u64*)d_key;
+    P.mv = (const u64*)d_val;
+    P.n = n;
+    P.src = (const u64*)d_src;
+    P.nrows = nrows;
+    P.v_off = (const u64*)d_v_off;
+    P.v = (const u64*)d_v;
+    P.v_cap = v_cap;
+    P.fn = fn;
+    P.is_float = is_float;
+    P.bad = (int*)z;
+    P.words = (u64*)((char*)z + 16);
+    u32* ticket = (u32*)(P.words + VA_WORDS);
+    u64* status = (u64*)((char*)z + 64);
+    P.err = l->d_err;
+    P.rval = (u64*)w;
+    P.rflag = P.rval + nrows;
+    P.rpos = P.rflag + nrows;
+    P.out_key = (u64*)out_key;
+    P.out_val = (u64*)out_val;
+    P.out_cap = out_cap;
+    P.out_len = (u64*)out_len;
+    static_assert(16 + VA_WORDS * sizeof(u64) + sizeof(u32) <= 64, "the aggregation's words fit their 64 bytes");
+    la_check_kernel<<<gb_grid(std::max<uint64_t>(nrows + 1, n)), 256, 0, l->stream>>>(P);
+    la_fold_kernel<<<gb_grid(32 * nrows), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)tr, EN_NT, 0, l->stream>>>(P.rflag, P.rpos, P.words + VA_W_R, nrows, status, ticket,
+                                                           P.words + VA_W_G);
+    la_write_kernel<<<gb_grid(nrows), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 4);
+    return DGX_OK;
+}
+
+static int la_check_args(int type, int fn, size_t n, size_t nrows, uint64_t values) {
+    if (int rc = vv_check_type(type)) return rc;
+    if (fn < DGX_AGG_MIN || fn > DGX_AGG_AVG) return fail(DGX_ERR_ARG, "unknown aggregation %d", fn);
+    if (n >= kVvMax || nrows >= kVvMax || values >= kVvMax)
+        return fail(DGX_ERR_ARG, "level aggregation sizes are 32-bit: n, nrows and values below 2^32");
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_var_level_agg(dgx_lane* l, int type, int fn, const uint64_t* d_key, const uint64_t* d_val,
+                                     size_t n, const uint64_t* d_src, size_t nrows, const uint64_t* d_v_off,
+                                     const uint64_t* d_v, size_t v_cap, uint64_t* d_out_key, uint64_t* d_out_val,
+                                     size_t out_cap, uint64_t* d_out_len) {
+    if (!l || !d_out_len || !d_v_off || (n && (!d_key || !d_val)) || (nrows && !d_src) || (v_cap && !d_v) ||
+        (out_cap && (!d_out_key || !d_out_val)))
+        return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = la_check_args(type, fn, n, nrows, v_cap)) return rc;
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_out_len, sizeof(uint64_t));
+    if (n == 0 || nrows == 0 || v_cap == 0) {  // no row can hold a value of the map
+        CK(cudaMemsetAsync(d_out_len, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = la_run(l, fn, type == DGX_VAL_FLOAT64, d_key, d_val, n, d_src, nrows, d_v_off, d_v, v_cap, d_out_key,
+                        d_out_val, out_cap, d_out_len))
+        return rc;
+    g_stats.uids_in += n + v_cap;
+    l->note_output(d_out_key, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_val, out_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_var_level_agg(int type, int fn, const uint64_t* key, const uint64_t* val, size_t n,
+                                 const uint64_t* src, size_t nrows, const uint64_t* v_off, const uint64_t* v,
+                                 uint64_t* out_key, uint64_t* out_val, size_t out_cap, size_t* out_len) {
+    if (!out_len || !v_off || (n && (!key || !val)) || (nrows && !src) || (out_cap && (!out_key || !out_val)))
+        return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = la_check_args(type, fn, n, nrows, 0)) return rc;
+    if (int rc = check_offsets("v_off", v_off, nrows, kVvMax)) return rc;
+    const uint64_t M = v_off[nrows];
+    if (M && !v) return fail(DGX_ERR_ARG, "null argument");
+    if (n == 0 || nrows == 0 || M == 0) {  // no row can hold a value of the map
+        *out_len = 0;
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += n + nrows + M;
+    uint64_t *d_key, *d_val, *d_src, *d_v_off, *d_v;  // one copy of each array
+    int rc;
+    if ((rc = upload_list(l, key, n, &d_key)) || (rc = upload_list(l, val, n, &d_val)) ||
+        (rc = upload_list(l, src, nrows, &d_src)) || (rc = upload_list(l, v_off, nrows + 1, &d_v_off)) ||
+        (rc = upload_list(l, v, M, &d_v)))
+        return rc;
+    void* d_o;
+    if ((rc = l->ws.alloc((2 * nrows + 1) * sizeof(uint64_t), &d_o))) return rc;
+    uint64_t* o_len = (uint64_t*)d_o;
+    if ((rc = la_run(l, fn, type == DGX_VAL_FLOAT64, d_key, d_val, n, d_src, nrows, d_v_off, d_v, M, o_len + 1,
+                     o_len + 1 + nrows, nrows, o_len)))
+        return rc;
+    return vv_finish(l, o_len, o_len + 1, o_len + 1 + nrows, out_key, out_val, out_cap, out_len);
 }
 
 // ---------------------------------------------------------------------------

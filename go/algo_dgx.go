@@ -679,3 +679,121 @@ func (p *PathSearch) Close() {
 		p.ps = nil
 	}
 }
+
+// dgxMinVarProp / dgxMinLevelAgg: below this many row values (summed over a path's levels, or in relSG's matrix) a
+// value variable stays on the Go path (transformTo, evalLevelAgg).  The C17 record (profiles/h100_c17_value_vars.json)
+// times the library against a C restatement, not against Go, and every call also pays the ShardedMap <-> sorted-array
+// conversion on the host, so both are the dgxMinMergeMatrix bound until a Go comparison sets them.
+const (
+	dgxMinVarProp  = dgxMinMergeMatrix
+	dgxMinLevelAgg = dgxMinMergeMatrix
+)
+
+// VarLevel is one node of a value variable's path: SrcUIDs, uidMatrix (one row per source) and DestUIDs.
+type VarLevel struct {
+	Src    []uint64
+	Matrix []*pb.List
+	Dest   []uint64
+}
+
+// Value-map types (DGX_VAL_*) and level aggregations (DGX_AGG_*).
+const (
+	ValInt64   = C.DGX_VAL_INT64
+	ValFloat64 = C.DGX_VAL_FLOAT64
+	AggMin     = C.DGX_AGG_MIN
+	AggMax     = C.DGX_AGG_MAX
+	AggSum     = C.DGX_AGG_SUM
+	AggAvg     = C.DGX_AGG_AVG
+)
+
+// varValues counts a uid matrix's values, for the gates, before anything is copied.
+func varValues(rows []*pb.List) int {
+	m := 0
+	for _, l := range rows {
+		if l != nil {
+			m += len(l.Uids)
+		}
+	}
+	return m
+}
+
+// varFlat flattens a uid matrix into C memory: (values, offsets, count, free).
+func varFlat(rows []*pb.List) (unsafe.Pointer, unsafe.Pointer, int, func()) {
+	off := make([]uint64, 1, len(rows)+1)
+	var v []uint64
+	for _, l := range rows {
+		if l != nil {
+			v = append(v, l.Uids...)
+		}
+		off = append(off, uint64(len(v)))
+	}
+	pv, fv := cArray(v)
+	po, fo := cArray(off)
+	return pv, po, len(v), func() { fv(); fo() }
+}
+
+// PropagateVar runs transformTo (query/query.go:1143-1236) over levels, the path from len(fromNode.path) on with
+// index 0 skipped, for a map given as strictly ascending keys and 64-bit words of type typ (ValInt64 or
+// ValFloat64).  It returns the map at the last level, ascending.  ok == false, below dgxMinVarProp values or on any
+// library error, means the caller keeps transformTo.
+func PropagateVar(typ int, keys, words []uint64, levels []VarLevel) (outKeys, outWords []uint64, ok bool) {
+	if len(levels) == 0 || len(keys) != len(words) {
+		return nil, nil, false
+	}
+	total := 0
+	for _, l := range levels {
+		if len(l.Matrix) != len(l.Src) {
+			return nil, nil, false
+		}
+		total += varValues(l.Matrix)
+	}
+	if total < dgxMinVarProp {
+		return nil, nil, false
+	}
+	frees := []func(){}
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+	}()
+	lv := make([]C.dgx_var_level, len(levels))
+	for i, l := range levels {
+		pv, po, _, free := varFlat(l.Matrix)
+		ps, fs := cArray(l.Src)
+		pd, fd := cArray(l.Dest)
+		frees = append(frees, free, fs, fd)
+		lv[i] = C.dgx_var_level{src: (*C.uint64_t)(ps), v_off: (*C.uint64_t)(po), v: (*C.uint64_t)(pv),
+			dest: (*C.uint64_t)(pd), nrows: C.size_t(len(l.Src)), ndest: C.size_t(len(l.Dest))}
+	}
+	plv, flv := cArray(lv)
+	frees = append(frees, flv)
+	d := len(levels[len(levels)-1].Dest)
+	outKeys, outWords = make([]uint64, d+1), make([]uint64, d+1)
+	var n C.size_t
+	if C.dgx_var_propagate(C.int(typ), u64ptr(keys), u64ptr(words), C.size_t(len(keys)),
+		(*C.dgx_var_level)(plv), C.size_t(len(levels)), u64ptr(outKeys), u64ptr(outWords), C.size_t(d),
+		&n) != C.DGX_OK {
+		return nil, nil, false
+	}
+	return outKeys[:int(n)], outWords[:int(n)], true
+}
+
+// LevelAgg runs evalLevelAgg's per-row branch (query/query.go:1088-1123): fn (AggMin .. AggAvg) of the map's values
+// over each row of relSG's uidMatrix.  It returns the keys (src[i] of every row with a present value) and the words,
+// of type ValFloat64 for AggAvg and typ otherwise.  ok == false, below dgxMinLevelAgg values or on any library error,
+// means the caller keeps evalLevelAgg.
+func LevelAgg(typ, fn int, keys, words, src []uint64, matrix []*pb.List) (outKeys, outWords []uint64, ok bool) {
+	if len(matrix) != len(src) || len(keys) != len(words) || varValues(matrix) < dgxMinLevelAgg {
+		return nil, nil, false
+	}
+	pv, po, _, free := varFlat(matrix)
+	defer free()
+	outKeys, outWords = make([]uint64, len(src)+1), make([]uint64, len(src)+1)
+	var n C.size_t
+	if C.dgx_var_level_agg(C.int(typ), C.int(fn), u64ptr(keys), u64ptr(words), C.size_t(len(keys)), u64ptr(src),
+		C.size_t(len(src)), (*C.uint64_t)(po), (*C.uint64_t)(pv), u64ptr(outKeys), u64ptr(outWords),
+		C.size_t(len(src)), &n) != C.DGX_OK {
+		return nil, nil, false
+	}
+	return outKeys[:int(n)], outWords[:int(n)], true
+}

@@ -468,6 +468,54 @@ int dgx_path_expand(dgx_path_search* ps, const dgx_path_level* level, uint64_t* 
  * reached.  DGX_ERR_CAP with *len set and nothing written when len exceeds cap.  One launch. */
 int dgx_path_result(dgx_path_search* ps, uint64_t* uids, uint32_t* attrs, size_t cap, size_t* len);
 
+/* Value variables (query/query.go): a value map is key[n] (strictly ascending uids) with val[n], 64-bit words that are
+ * int64 two's-complement patterns (DGX_VAL_INT64) or IEEE binary64 patterns (DGX_VAL_FLOAT64); one type per map.
+ * clamp is aggregator.Value's: +Inf -> MaxFloat64, -Inf -> -MaxFloat64, NaN -> +0.0. */
+#define DGX_VAL_INT64 1
+#define DGX_VAL_FLOAT64 2
+#define DGX_AGG_MIN 0
+#define DGX_AGG_MAX 1
+#define DGX_AGG_SUM 2
+#define DGX_AGG_AVG 3
+/* One level of a path, a node curNode: row i (v[v_off[i] .. v_off[i+1]), in stored order, not necessarily ascending)
+ * belongs to src[i] (curNode.SrcUIDs, strictly ascending); dest (curNode.DestUIDs, strictly ascending) holds every row
+ * value.  Host memory for dgx_var_propagate, device memory for dgx_dev_var_propagate.  v_cap is the room of v, read by
+ * the device form only (the host form reads v_off[nrows]). */
+typedef struct {
+    const uint64_t* src;    /* nrows */
+    const uint64_t* v_off;  /* nrows + 1 */
+    const uint64_t* v;
+    const uint64_t* dest;   /* ndest */
+    size_t nrows, v_cap, ndest;
+} dgx_var_level;
+/* transformTo (query/query.go :1143-1236) over the levels in path order (len(fromNode.path) to the end, index 0
+ * skipped): the map at the last level into out_key / out_val (ascending keys, the input's type) and *out_len.  Each
+ * level: row i contributes iff src[i] is a key of the current map, and then each of its values dst receives
+ * curVal = map[src[i]].  int64: a wrapping sum.  float64: the rows split into Go's 4 ranges (width = nrows / 4, the
+ * last to nrows); within a range dst's contributions in row-major order fold as v = clamp(curVal), then
+ * v = clamp(curVal + v); the ranges then combine in ascending order, acc = clamp(acc + part) (the chunks finishing in
+ * index order).  Intermediate maps stay on the device.  n == 0 gives *out_len = 0 and needs no device.
+ * out_cap >= the last level's ndest always suffices; a longer result is DGX_ERR_CAP with *out_len set and nothing
+ * written.  DGX_ERR_ARG before anything is copied: an unknown type, nlevels of 0, n, nlevels, nrows, v_off[nrows] or
+ * ndest of 2^32 or more, v_off not starting at 0 or decreasing, a null array that is needed.  DGX_ERR_ARG after the
+ * kernels, with nothing written: map keys, src or dest not strictly ascending, a row value not in its level's dest.
+ * Launches: 9 + 3 ceil((b_d + 2) / 8) per level, b_d the bit width of the level's ndest - 1 (DESIGN section 3.13). */
+int dgx_var_propagate(int type, const uint64_t* key, const uint64_t* val, size_t n, const dgx_var_level* levels,
+                      size_t nlevels, uint64_t* out_key, uint64_t* out_val, size_t out_cap, size_t* out_len);
+/* evalLevelAgg's per-row branch (query/query.go :1088-1123): for every row i with at least one value present in the
+ * map, key src[i] and the fold of its present values in row order, as aggregator.Apply does: MIN acc = acc < x ? acc : x
+ * and MAX acc = acc < x ? x : acc (the later of equal values wins), SUM a wrapping int64 add or sequential IEEE adds,
+ * AVG the sum over the count in float64 (an int64 sum through float64(int64)); clamp once on float results.  Output
+ * type: DGX_VAL_FLOAT64 for AVG, the input type otherwise.  Row i is v[v_off[i] .. v_off[i+1]); src strictly ascends,
+ * so the keys come out ascending.  out_cap >= nrows always suffices; a longer result is DGX_ERR_CAP with *out_len set
+ * and nothing written.  n == 0 or no row value gives *out_len = 0 and needs no device.  DGX_ERR_ARG before anything is
+ * copied: an unknown type or fn, n, nrows or v_off[nrows] of 2^32 or more, v_off not starting at 0 or decreasing, a
+ * null array that is needed.  DGX_ERR_ARG after the kernels, with nothing written: map keys or src not strictly
+ * ascending.  4 launches. */
+int dgx_var_level_agg(int type, int fn, const uint64_t* key, const uint64_t* val, size_t n, const uint64_t* src,
+                      size_t nrows, const uint64_t* v_off, const uint64_t* v, uint64_t* out_key, uint64_t* out_val,
+                      size_t out_cap, size_t* out_len);
+
 /* @cascade over a forest of subgraph nodes (query/query.go populateVarMap :1445-1527, updateUidMatrix :1425-1439
  * without facets, and ProcessQuery's root pagination :3004-3011), in pre-order: parent[n] is UINT32_MAX for a query root
  * and below n otherwise.  flags[n] is a set of DGX_CASCADE_* bits resolved on the host; first[n] / offset[n] are
@@ -750,6 +798,27 @@ int dgx_dev_recurse_filter(dgx_lane* lane, dgx_reach_set* set, const uint64_t* d
 int dgx_dev_path_expand(dgx_lane* lane, dgx_path_search* ps, const dgx_path_level* level, size_t src_cap,
                         size_t v_cap, size_t dest_cap, uint64_t* d_next, uint64_t* d_next_off, size_t next_cap,
                         uint64_t* d_stats);
+/* Device form of dgx_var_propagate: the map, the outputs and every array of *levels (host array, nlevels entries) in
+ * device memory, so the rows of dgx_dev_list_uids_unfiltered_rows and the dest of dgx_dev_merge_sorted_matrix feed it
+ * directly.  v_cap is the room of a level's v (its v_off[nrows] must not pass it).  nrows and ndest are exact sizes
+ * the host must know: a dest made by dgx_dev_merge_sorted_matrix has its length in a device word, which the caller
+ * reads (one sync) before this call, since a dest padded to a cap does not strictly ascend and is refused.  d_out_len
+ * is one device uint64.
+ * Argument errors are DGX_ERR_ARG at the call, as in the host form (sizes, type, null pointers with a nonzero size);
+ * n == 0 writes *d_out_len = 0 without a launch.  Offsets and the order and membership checks run on the device: a
+ * refused call writes nothing and surfaces as DGX_ERR_ARG at the next dgx_lane_sync; a result longer than out_cap
+ * writes only *d_out_len and surfaces as DGX_ERR_CAP.  Asynchronous on the lane; launches as the host form's. */
+int dgx_dev_var_propagate(dgx_lane* lane, int type, const uint64_t* d_key, const uint64_t* d_val, size_t n,
+                          const dgx_var_level* levels, size_t nlevels, uint64_t* d_out_key, uint64_t* d_out_val,
+                          size_t out_cap, uint64_t* d_out_len);
+/* Device form of dgx_var_level_agg: every array in device memory, offsets included; v_cap is the room of d_v.
+ * Argument errors at the call as in the host form; n, nrows or v_cap of 0 writes *d_out_len = 0 without a launch.
+ * Offsets, map keys and src are checked on the device: a refused call writes nothing (DGX_ERR_ARG at the next
+ * dgx_lane_sync); a result longer than out_cap writes only *d_out_len (DGX_ERR_CAP).  Asynchronous on the lane. */
+int dgx_dev_var_level_agg(dgx_lane* lane, int type, int fn, const uint64_t* d_key, const uint64_t* d_val, size_t n,
+                          const uint64_t* d_src, size_t nrows, const uint64_t* d_v_off, const uint64_t* d_v,
+                          size_t v_cap, uint64_t* d_out_key, uint64_t* d_out_val, size_t out_cap,
+                          uint64_t* d_out_len);
 /* One node of dgx_dev_cascade, every pointer in device memory: its rows v[v_off[i] .. v_off[i+1]) (v_off has nrows + 1
  * values, v_off[0] == 0, v_off[nrows] <= v_cap, the room of v), its dest (ndest values) and its has_val (nhas bytes). */
 typedef struct dgx_cascade_node {

@@ -478,6 +478,70 @@ private:
     dgx_path_search* ps_ = nullptr;
 };
 
+// A value variable's map (query/query.go varValue.Vals for IntID or FloatID values): strictly ascending keys and one
+// 64-bit word per key, the int64 or binary64 bit pattern of type DGX_VAL_INT64 or DGX_VAL_FLOAT64.
+struct ValueMap {
+    int type = DGX_VAL_INT64;
+    std::vector<uint64_t> keys, words;
+};
+
+// One node of a value variable's path: SrcUIDs, uidMatrix (one row per source, in stored order) and DestUIDs.
+struct VarLevel {
+    std::vector<uint64_t> src;
+    std::vector<pb::List> rows;
+    std::vector<uint64_t> dest;
+};
+
+// transformTo (query/query.go:1143-1236) over `levels` (the path from len(fromNode.path) on, index 0 skipped) in one
+// dgx_var_propagate call: the map at the last level.
+inline ValueMap PropagateVar(const ValueMap& m, const std::vector<VarLevel>& levels) {
+    if (m.keys.size() != m.words.size()) throw Error(DGX_ERR_ARG, "one word per key");
+    std::vector<std::vector<uint64_t>> v(levels.size()), v_off(levels.size());
+    std::vector<dgx_var_level> lv(levels.size());
+    for (size_t k = 0; k < levels.size(); ++k) {
+        const VarLevel& L = levels[k];
+        if (L.src.size() != L.rows.size()) throw Error(DGX_ERR_ARG, "one source per row");
+        v_off[k].push_back(0);
+        for (const pb::List& r : L.rows) {
+            v[k].insert(v[k].end(), r.Uids.begin(), r.Uids.end());
+            v_off[k].push_back(v[k].size());
+        }
+        lv[k] = dgx_var_level{L.src.data(), v_off[k].data(), v[k].data(), L.dest.data(), L.src.size(), 0,
+                              L.dest.size()};
+    }
+    const size_t cap = levels.empty() ? 0 : levels.back().dest.size();
+    ValueMap out;
+    out.type = m.type;
+    out.keys.assign(std::max<size_t>(cap, 1), 0);
+    out.words.assign(std::max<size_t>(cap, 1), 0);
+    size_t n = 0;
+    check(dgx_var_propagate(m.type, m.keys.data(), m.words.data(), m.keys.size(), lv.data(), lv.size(),
+                            out.keys.data(), out.words.data(), cap, &n));
+    out.keys.resize(n);
+    out.words.resize(n);
+    return out;
+}
+
+// evalLevelAgg's per-row branch (query/query.go:1088-1123) in one dgx_var_level_agg call: fn (DGX_AGG_*) of the map
+// over every row of relSG's uidMatrix, keyed by src; DGX_VAL_FLOAT64 for DGX_AGG_AVG, the map's type otherwise.
+inline ValueMap LevelAgg(int fn, const ValueMap& m, const std::vector<uint64_t>& src,
+                         const std::vector<pb::List>& rows) {
+    if (m.keys.size() != m.words.size()) throw Error(DGX_ERR_ARG, "one word per key");
+    if (src.size() != rows.size()) throw Error(DGX_ERR_ARG, "one source per row");
+    std::vector<uint64_t> v, v_off{0};
+    for (const pb::List& r : rows) { v.insert(v.end(), r.Uids.begin(), r.Uids.end()); v_off.push_back(v.size()); }
+    ValueMap out;
+    out.type = fn == DGX_AGG_AVG ? DGX_VAL_FLOAT64 : m.type;
+    out.keys.assign(std::max<size_t>(rows.size(), 1), 0);
+    out.words.assign(std::max<size_t>(rows.size(), 1), 0);
+    size_t n = 0;
+    check(dgx_var_level_agg(m.type, fn, m.keys.data(), m.words.data(), m.keys.size(), src.data(), src.size(),
+                            v_off.data(), v.data(), out.keys.data(), out.words.data(), rows.size(), &n));
+    out.keys.resize(n);
+    out.words.resize(n);
+    return out;
+}
+
 }  // namespace algo
 
 // Wire-format adjacency (dgx_wire_*, host only): the bytes proto.Unmarshal sees at posting/list.go:1045 and

@@ -142,6 +142,7 @@ def main():
     ap.add_argument("--c14-only", action="store_true", help="only the C14 @recurse filter rows")
     ap.add_argument("--c15-only", action="store_true", help="only the C15 @cascade rows")
     ap.add_argument("--c16-only", action="store_true", help="only the C16 shortest() rows")
+    ap.add_argument("--c17-only", action="store_true", help="only the C17 value-variable rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -165,9 +166,11 @@ def main():
         rows = c15_rows(Lane())
     elif args.c16_only:
         rows = c16_rows(Lane())
+    elif args.c17_only:
+        rows = c17_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1629,6 +1632,143 @@ def c14_rows(L):
                              "steps": len(steps), "values": vals, "kept": total, "check": bool(ok), "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del dev_in, dev_out
+    return out_rows
+
+
+def c17_rows(L):
+    """C17 "value variables": transformTo over a path and evalLevelAgg per row.  C17a: query-039's shape, math(1.0) and
+    math(1) carried 3 levels from 1e4 roots over C14's 2e6-node Zipf friend graph (tests/gen_recurse.py c14_graph).
+    C17b: min / max / sum / avg over C13's matrix (tests/gen_groupby.py c13_rows, 1e6 rows) with int and float maps
+    over 90% of the destinations, and the same matrix as one propagation level, whose most popular destination is a
+    hub.  C17c: a path of TestLevelBasedFacetVarSum2's size (2 levels, a handful of uids): latency-bound.  Legs: (1) the
+    device form on resident inputs (CUDA events), (2) the host form (wall clock), (3) the line-by-line restatement
+    (tests/valvar_oracle.c) on 1 thread -- C with hash maps, not Go.  Every leg is checked bit for bit against the
+    restatement."""
+    import gen_groupby as gg
+    import gen_recurse as gr
+    import valvar_oracle as vo
+
+    lib = L.lib
+    U64 = np.uint64
+
+    def dp(t):
+        return t.data_ptr()
+
+    def up(x):
+        x = np.concatenate([np.ascontiguousarray(x, U64), np.zeros(1, U64)])
+        return torch.from_numpy(x.view(np.int64)).to(DEV)
+
+    friend = gr.c14_graph(np.random.default_rng(14))["friend"]
+    roots = np.unique(np.random.default_rng(17).integers(1, 2_000_001, 10_000).astype(U64))
+    path_a, src = [], roots
+    for _ in range(3):
+        v, off = friend.csr(src)
+        dest = np.unique(v)
+        path_a.append((src, v, off, dest))
+        src = dest
+    csrc, cv, coff, cdest = gg.c13_rows(np.random.default_rng(13))
+    indeg = int(np.bincount(np.searchsorted(cdest, cv)).max())
+    path_c = [(np.array([1, 2, 3], U64), np.array([4, 5, 5, 6], U64), np.array([0, 2, 3, 4], U64),
+               np.array([4, 5, 6], U64)),
+              (np.array([4, 5, 6], U64), np.array([7, 7, 8], U64), np.array([0, 1, 2, 3], U64), np.array([7, 8], U64))]
+    rng = np.random.default_rng(18)
+    cases = []
+    for typ, vals in (("float", np.ones(roots.size)), ("int", np.ones(roots.size, np.int64))):
+        cases.append(("C17a", f"math(1{'.0' if typ == 'float' else ''}) over 3 friend levels from {roots.size} roots",
+                      "propagate", roots, vals, path_a))
+    for typ in ("int", "float"):
+        mk = np.sort(rng.choice(cdest, int(cdest.size * 0.9), replace=False))
+        mv = rng.integers(-1000, 1000, mk.size) if typ == "int" else rng.normal(0, 1e3, mk.size)
+        for fn in ("min", "max", "sum", "avg"):
+            cases.append(("C17b", f"{fn}(val(x)) over C13's matrix, {typ} map over 90% of dest", fn, mk, mv,
+                          [(csrc, cv, coff, cdest)]))
+        pk = np.sort(rng.choice(csrc, int(csrc.size * 0.9), replace=False))
+        pv = rng.integers(-1000, 1000, pk.size) if typ == "int" else rng.normal(0, 1e3, pk.size)
+        cases.append(("C17b", f"C13's matrix as one propagation level (hub of {indeg} in-edges), {typ} map over 90% "
+                      "of src", "propagate", pk, pv, [(csrc, cv, coff, cdest)]))
+    for typ, vals in (("float", np.array([0.1, 0.2, 0.3])), ("int", np.array([1, 2, 3], np.int64))):
+        cases.append(("C17c", f"TestLevelBasedFacetVarSum2's size: 2 levels, {typ} map", "propagate",
+                      np.array([1, 2, 3], U64), vals, path_c))
+    out_rows = []
+    for name, cfg, op, keys, vals, levels in cases:
+        keys = np.ascontiguousarray(keys, U64)
+        vals = np.ascontiguousarray(vals)
+        typ = 2 if vals.dtype == np.float64 else 1
+        w = vals.view(U64)
+        values = sum(int(lv[2][-1]) for lv in levels)
+        t0 = time.perf_counter()
+        if op == "propagate":
+            want = vo.propagate_csr(keys, vals, [lv[:3] for lv in levels])
+        else:
+            s_, v_, o_, _ = levels[0]
+            want = vo.level_agg_csr(op, keys, vals, s_, v_, o_)
+        t_or = (time.perf_counter() - t0) * 1e3
+        cap = levels[-1][3].size if op == "propagate" else levels[0][0].size
+        want_w = np.asarray(want[1]).view(U64)
+        # (1) device form, inputs and outputs resident
+        dk, dv = up(keys), up(w)
+        dlv = [[up(x) for x in lv] for lv in levels]
+        ok_t, ov_t = (torch.empty(cap + 1, dtype=torch.int64, device=DEV) for _ in range(2))
+        dn = torch.empty(1, dtype=torch.int64, device=DEV)
+        if op == "propagate":
+            arr = (_lib.VarLevel * len(levels))()
+            for i, (lv, t) in enumerate(zip(levels, dlv)):
+                arr[i] = _lib.VarLevel(dp(t[0]), dp(t[2]), dp(t[1]), dp(t[3]), lv[2].size - 1, int(lv[2][-1]),
+                                       lv[3].size)
+
+            def dev():
+                _lib.check(lib.dgx_dev_var_propagate(L.h, typ, dp(dk), dp(dv), keys.size, arr, len(levels), dp(ok_t),
+                                                     dp(ov_t), cap, dp(dn)))
+        else:
+            t = dlv[0]
+
+            def dev():
+                _lib.check(lib.dgx_dev_var_level_agg(L.h, typ, vo.AGG[op], dp(dk), dp(dv), keys.size, dp(t[0]),
+                                                     levels[0][0].size, dp(t[2]), dp(t[1]), int(levels[0][2][-1]),
+                                                     dp(ok_t), dp(ov_t), cap, dp(dn)))
+        ms_dev, _ = timeit(dev, warm=2, reps=10)
+        L.sync()
+        n = int(dn.cpu().numpy()[0])
+        ok_dev = (n == want[0].size and np.array_equal(ok_t[:n].cpu().numpy().view(U64), want[0]) and
+                  np.array_equal(ov_t[:n].cpu().numpy().view(U64), want_w))
+        # (2) host form
+        hk, hv, hn = np.empty(max(cap, 1), U64), np.empty(max(cap, 1), U64), C.c_size_t(0)
+        if op == "propagate":
+            harr = (_lib.VarLevel * len(levels))()
+            hkeep = [[np.concatenate([np.ascontiguousarray(x, U64), np.zeros(1, U64)]) for x in lv] for lv in levels]
+            for i, (lv, h) in enumerate(zip(levels, hkeep)):
+                harr[i] = _lib.VarLevel(h[0].ctypes.data, h[2].ctypes.data, h[1].ctypes.data, h[3].ctypes.data,
+                                        lv[2].size - 1, 0, lv[3].size)
+
+            def host():
+                _lib.check(lib.dgx_var_propagate(typ, keys.ctypes.data, w.ctypes.data, keys.size, harr, len(levels),
+                                                 hk.ctypes.data, hv.ctypes.data, cap, C.byref(hn)))
+        else:
+            s_, v_, o_, _ = (np.ascontiguousarray(x, U64) for x in levels[0])
+
+            def host():
+                _lib.check(lib.dgx_var_level_agg(typ, vo.AGG[op], keys.ctypes.data, w.ctypes.data, keys.size,
+                                                 s_.ctypes.data, s_.size, o_.ctypes.data, v_.ctypes.data,
+                                                 hk.ctypes.data, hv.ctypes.data, cap, C.byref(hn)))
+        host()
+        ts = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            host()
+            ts.append((time.perf_counter() - t0) * 1e3)
+        t_host = float(np.median(ts))
+        m = hn.value
+        ok_host = m == want[0].size and np.array_equal(hk[:m], want[0]) and np.array_equal(hv[:m], want_w)
+        full = f"{name}: {cfg}; {len(levels)} level(s), {values} row values, map {keys.size}, result {want[0].size}"
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev, "CUDA events, median of 10 after 2 warm"),
+                                    ("host form", t_host, ok_host, "wall clock, median of 3 after 1 warm"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, True, "orc_propagate / orc_level_agg, "
+                                     "wall clock, one run; the reference the other legs are checked against")):
+            out_rows.append({"op": "PropagateVar" if op == "propagate" else f"LevelAgg({op})", "workload": name,
+                             "leg": leg, "config": full, "ms": round(ms, 4), "values": values,
+                             "max_in_degree": indeg if name == "C17b" else None, "check": bool(ok), "timing": timing})
+            print(json.dumps(out_rows[-1]), flush=True)
+        del dk, dv, dlv, ok_t, ov_t
     return out_rows
 
 
