@@ -45,6 +45,7 @@
 #include "path_kernel.cuh"
 #include "valvar_kernel.cuh"
 #include "wire.hpp"
+#include "ws_layout.hpp"
 
 using namespace dgx;
 
@@ -239,6 +240,67 @@ static int lane_begin_op(dgx_lane* l) {
     l->ws.reset();
     return DGX_OK;
 }
+
+// One call's scratch arrays carved from the lane's workspace by a WsLayout (ws_layout.hpp).  Declare the regions in
+// section order; stage() places the copied section in the lane's pinned staging, where the caller fills the tables
+// through the host pointers; commit() takes one arena allocation, uploads the copied section in one copy, sets the
+// zeroed and ones sections with one memset each and writes every declared device pointer.
+class WsCarve {
+  public:
+    explicit WsCarve(dgx_lane* l) : l_(l) {}
+    template <class D, class H>
+    void copied(D** d, H** h, size_t n) {
+        static_assert(sizeof(D) == sizeof(H) && alignof(D) == alignof(H), "device and host views of one table");
+        if (h_) L_.ok = false;  // the staged section cannot grow
+        const size_t off = L_.add<H>(WsLayout::kCopied, n);
+        put(d, off, false);
+        put(h, off, true);
+    }
+    template <class T> void zeroed(T** d, size_t n) { put(d, L_.add<T>(WsLayout::kZeroed, n), false); }
+    template <class T> void ones(T** d, size_t n) { put(d, L_.add<T>(WsLayout::kOnes, n), false); }
+    template <class T> void plain(T** d, size_t n) { put(d, L_.add<T>(WsLayout::kPlain, n), false); }
+
+    int stage() {
+        const size_t nc = L_.end(WsLayout::kCopied);
+        if (int rc = l_->host.alloc(nc, (void**)&h_)) return rc;
+        bind(h_, true);
+        return DGX_OK;
+    }
+    int commit() {
+        const size_t nc = L_.end(WsLayout::kCopied);
+        if (!L_.ok || nslots_ > kMaxSlots || (nc && !h_))
+            return fail(DGX_ERR_CUDA, "workspace layout: a region out of section order, or its table not staged");
+        char* d;
+        if (int rc = l_->ws.alloc(L_.bytes, (void**)&d)) return rc;
+        if (nc) {
+            CK(cudaMemcpyAsync(d, h_, nc, cudaMemcpyHostToDevice, l_->stream));
+            g_stats.h2d += nc;
+        }
+        for (int s : {int(WsLayout::kZeroed), int(WsLayout::kOnes)})
+            if (L_.end(s) > L_.begin(s))
+                CK(cudaMemsetAsync(d + L_.begin(s), s == WsLayout::kOnes ? 0xff : 0, L_.end(s) - L_.begin(s), l_->stream));
+        bind(d, false);
+        return DGX_OK;
+    }
+
+  private:
+    static constexpr int kMaxSlots = 48;
+    struct Slot { void* p; void (*set)(void*, char*); size_t off; bool host; };
+    template <class T>
+    void put(T** p, size_t off, bool host) {
+        if (nslots_ < kMaxSlots) slots_[nslots_] = {p, [](void* s, char* b) { *(T**)s = (T*)b; }, off, host};
+        ++nslots_;
+    }
+    void bind(char* base, bool host) {
+        for (int i = 0; i < std::min(nslots_, kMaxSlots); ++i)
+            if (slots_[i].host == host) slots_[i].set(slots_[i].p, base + slots_[i].off);
+    }
+    dgx_lane* l_;
+    WsLayout L_;
+    char* h_ = nullptr;
+    Slot slots_[kMaxSlots];
+    int nslots_ = 0;
+};
 
 // ---------------------------------------------------------------------------
 // lifecycle
@@ -1451,13 +1513,12 @@ static int batch_to_host(dgx_lane* l, const void* d_out, const void* d_off, size
 // offsets in the lane's workspace, filled by run(d_out, d_off), then copied back by batch_to_host.
 template <class Run>
 static int csr_to_host(dgx_lane* l, size_t cap, size_t nrows, uint64_t* out, uint64_t* out_off, size_t out_cap, Run run) {
-    void *d_out, *d_off;
-    int rc = l->ws.alloc((cap + 2) * sizeof(uint64_t), &d_out);
-    if (rc) return rc;
-    rc = l->ws.alloc((nrows + 1) * sizeof(uint64_t), &d_off);
-    if (rc) return rc;
-    rc = run((uint64_t*)d_out, (uint64_t*)d_off);
-    if (rc) return rc;
+    uint64_t *d_out, *d_off;
+    WsCarve ws(l);
+    ws.plain(&d_out, cap + 2);
+    ws.plain(&d_off, nrows + 1);
+    if (int rc = ws.commit()) return rc;
+    if (int rc = run(d_out, d_off)) return rc;
     return batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap);
 }
 
@@ -1649,21 +1710,19 @@ static int icw_impl(dgx_lane* l, const dgx_dev_pack& pk, uint64_t after, const u
         return DGX_OK;
     }
     const size_t tiles = (m + CP_TILE - 1) / CP_TILE;
-    const size_t b_rng = ((2 * nb * sizeof(u32)) + 15) & ~size_t(15);
-    const size_t b_keep = (m + 15) & ~size_t(15);
-    const size_t b_stat = tiles * sizeof(u64) + 64;
-    void* d_raw;
-    int rc = l->ws.alloc(b_rng + b_keep + b_stat, &d_raw);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(d_raw, 0, b_rng + b_keep + b_stat, l->stream));
     IcwParams P;
+    CompactParams C;
+    WsCarve ws(l);
+    ws.zeroed(&P.vlo, nb);
+    ws.zeroed(&P.vhi, nb);
+    ws.zeroed(&P.keep, m);
+    ws.zeroed(&C.status, tiles);
+    ws.zeroed(&C.ticket, 16);
+    if (int rc = ws.commit()) return rc;
     P.pk = pk.pk;
     P.v = (const u64*)d_v;
     P.m = m;
     P.after = after;
-    P.vlo = (u32*)d_raw;
-    P.vhi = P.vlo + nb;
-    P.keep = (unsigned char*)d_raw + b_rng;
     // search the shorter side's elements in the longer side (the reference's linVsBinRatio idea, :49-59)
     if (m < nb) icw_ranges_by_v_kernel<<<(unsigned)((m + 255) / 256), 256, 0, l->stream>>>(P);
     else icw_ranges_by_block_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, l->stream>>>(P);
@@ -1671,15 +1730,12 @@ static int icw_impl(dgx_lane* l, const dgx_dev_pack& pk, uint64_t after, const u
     const uint64_t warps = (nb + D_BPW - 1) / D_BPW;
     icw_probe_kernel<<<(unsigned)((warps + D_WARPS - 1) / D_WARPS), D_NT, sizeof(DWarpSmem) * D_WARPS, l->stream>>>(P);
     CK(cudaGetLastError());
-    CompactParams C;
     C.v = (const u64*)d_v;
     C.keep = P.keep;
     C.m = m;
     C.out = (u64*)d_out;
     C.out_cap = out_cap;
     C.out_len = (u64*)d_len;
-    C.status = (u64*)((char*)d_raw + b_rng + b_keep);
-    C.ticket = (u32*)((char*)d_raw + b_rng + b_keep + tiles * sizeof(u64));
     C.err = l->d_err;
     compact_kernel<<<(unsigned)tiles, CP_NT, 0, l->stream>>>(C);
     CK(cudaGetLastError());
@@ -2066,40 +2122,29 @@ static int encode_impl(dgx_lane* l, const uint64_t* d_u, size_t n, const uint64_
                        size_t nblocks_cap, size_t delta_cap, EncOut* out) {
     const size_t tiles_a = std::max<size_t>(1, (n + EN_TILE - 1) / EN_TILE);
     const size_t tiles_b = std::max<size_t>(1, (nblocks_cap + EN_TILE - 1) / EN_TILE);
-    // workspace: [counts 8w | tickets | err][status_a][status_b] zeroed; seg arrays, block arrays
-    const size_t z_bytes = 128 + (tiles_a + tiles_b) * sizeof(u64);
-    void *d_z, *d_seg, *d_blk, *d_del;
-    int rc = l->ws.alloc(z_bytes, &d_z);
-    if (rc) return rc;
     const size_t seg_cap = std::min<size_t>(n, nblocks_cap) + 2;  // more segments than blocks cannot fit anyway
-    rc = l->ws.alloc(2 * seg_cap * sizeof(u64), &d_seg);
-    if (rc) return rc;
-    rc = l->ws.alloc((nblocks_cap + 1) * (4 * sizeof(u64) + sizeof(u32)) + 64, &d_blk);
-    if (rc) return rc;
-    rc = l->ws.alloc(delta_cap + 64, &d_del);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(d_z, 0, z_bytes, l->stream));
     EncParams P;
+    WsCarve ws(l);
+    ws.zeroed(&P.counts, 8);
+    ws.zeroed(&P.ticket, 8);
+    ws.zeroed(&P.err, 8);
+    ws.zeroed(&P.status, tiles_a + tiles_b);
+    ws.plain(&P.seg_start, seg_cap);
+    ws.plain(&P.seg_blk, seg_cap);
+    ws.plain(&P.base, nblocks_cap + 1);
+    ws.plain(&P.blk_start, nblocks_cap + 1);
+    ws.plain(&P.blk_bytes, nblocks_cap + 1);
+    ws.plain(&P.delta_off, nblocks_cap + 1);
+    ws.plain(&P.num, nblocks_cap + 1 + 16);
+    ws.plain(&P.deltas, delta_cap + 64);
+    if (int rc = ws.commit()) return rc;
     P.u = (const u64*)d_u;
     P.n = n;
     P.n_dyn = (const u64*)d_n;
     P.bsz = block_size ? block_size : 1;
-    P.counts = (u64*)d_z;
-    P.ticket = (u32*)((char*)d_z + 64);
-    P.err = (int*)((char*)d_z + 96);
-    P.status = (u64*)((char*)d_z + 128);
     u64* status_b = P.status + tiles_a;
-    P.seg_start = (u64*)d_seg;
     P.seg_cap = seg_cap;
-    P.seg_blk = P.seg_start + seg_cap;
     P.nblocks_cap = nblocks_cap;
-    char* bp = (char*)d_blk;
-    P.base = (u64*)bp; bp += (nblocks_cap + 1) * sizeof(u64);
-    P.blk_start = (u64*)bp; bp += (nblocks_cap + 1) * sizeof(u64);
-    P.blk_bytes = (u64*)bp; bp += (nblocks_cap + 1) * sizeof(u64);
-    P.delta_off = (u64*)bp; bp += (nblocks_cap + 1) * sizeof(u64);
-    P.num = (u32*)bp;
-    P.deltas = (unsigned char*)d_del;
     P.delta_cap = delta_cap;
     // a list with more segments than seg_cap cannot be encoded into nblocks_cap blocks: the segment pass would
     // overrun its array, so it is bounded by the same capacity check (segments <= blocks)
@@ -2336,12 +2381,13 @@ static int icw_rows_impl(dgx_lane* l, const dgx_dev_pack* const* packs, size_t n
     uint64_t nb = 0, thr = 0, warps = 0, exact = 0, slots_cap = 0;
     for (size_t i = 0; i < nrows; ++i)
         if (packs[i] && packs[i]->pk.nblocks) ++nj;
-    const size_t b_jobs = (nj * sizeof(IcwJob) + 15) & ~size_t(15), b_rows = (nrows + 1) * sizeof(uint64_t);
-    void* h_raw;
-    int rc = l->host.alloc(b_jobs + b_rows, &h_raw);
-    if (rc) return rc;
-    IcwJob* hj = (IcwJob*)h_raw;
-    uint64_t* h_rows = (uint64_t*)((char*)h_raw + b_jobs);
+    IcwRowsParams P;
+    IcwJob* hj;
+    uint64_t* h_rows;
+    WsCarve ws(l);
+    ws.copied(&P.jobs, &hj, nj);
+    ws.copied(&P.row_blk, &h_rows, nrows + 1);
+    if (int rc = ws.stage()) return rc;
     size_t j = 0;
     for (size_t i = 0; i < nrows; ++i) {
         h_rows[i] = nb;
@@ -2371,20 +2417,18 @@ static int icw_rows_impl(dgx_lane* l, const dgx_dev_pack* const* packs, size_t n
     const uint64_t g_probe = (warps + D_WARPS - 1) / D_WARPS, g_gather = (std::max<uint64_t>(nb * 32, nrows + 1) + 255) / 256;
     if (std::max({g_rng, g_blk, tiles, g_probe, g_gather}) > kMaxGrid || nj > 0xffffffffull)
         return fail(DGX_ERR_ARG, "batch too large for one launch (%llu blocks, %zu rows)", (unsigned long long)nb, nrows);
-    // workspace: [table | zeroed: vlo vhi, scan status + tickets | slot | slot_off | cnt | cnt_off | slots]
-    const size_t b_tab = b_jobs + b_rows;
-    const size_t b_rng = (2 * nb * sizeof(u32) + 15) & ~size_t(15), b_stat = 2 * tiles * sizeof(u64) + 16;
-    const size_t b_zero = b_rng + b_stat;
-    const size_t b_words = (4 * nb + 2) * sizeof(u64);
-    void* d_raw;
-    rc = l->ws.alloc(b_tab + b_zero + b_words + slots_cap * sizeof(u64), &d_raw);
-    if (rc) return rc;
-    char* d = (char*)d_raw;
-    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
-    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
-    g_stats.h2d += b_tab;
-    IcwRowsParams P;
-    P.jobs = (const IcwJob*)d;
+    u64* status;
+    u32* tickets;
+    ws.zeroed(&P.vlo, nb);
+    ws.zeroed(&P.vhi, nb);
+    ws.zeroed(&status, 2 * tiles);
+    ws.zeroed(&tickets, 4);
+    ws.plain(&P.slot, nb);
+    ws.plain(&P.slot_off, nb + 1);
+    ws.plain(&P.cnt, nb);
+    ws.plain(&P.cnt_off, nb + 1);
+    ws.plain(&P.slots, slots_cap);
+    if (int rc = ws.commit()) return rc;
     P.njobs = (u32)nj;
     P.v = (const u64*)d_v;
     P.m = m;
@@ -2392,16 +2436,6 @@ static int icw_rows_impl(dgx_lane* l, const dgx_dev_pack* const* packs, size_t n
     P.nblocks = nb;
     P.nthreads = thr;
     P.nwarps = warps;
-    P.row_blk = (const u64*)(d + b_jobs);
-    P.vlo = (u32*)(d + b_tab);
-    P.vhi = P.vlo + nb;
-    u64* status = (u64*)(d + b_tab + b_rng);
-    u32* tickets = (u32*)(status + 2 * tiles);
-    P.slot = (u64*)(d + b_tab + b_zero);
-    P.slot_off = P.slot + nb;
-    P.cnt = P.slot_off + nb + 1;
-    P.cnt_off = P.cnt + nb;
-    P.slots = P.cnt_off + nb + 1;
     P.slots_cap = slots_cap;
     P.nrows = nrows;
     P.out = (u64*)d_out;
@@ -2497,44 +2531,35 @@ static int icw_matrix_impl(dgx_lane* l, const dgx_dev_pack& pk, const uint64_t* 
     const uint64_t g_probe = ((units + 31) / 32 + D_WARPS - 1) / D_WARPS;
     if (std::max({g_elem, g_gather, g_probe}) > kMaxGrid)
         return fail(DGX_ERR_ARG, "matrix too large for one launch (%llu uids, %zu rows)", (unsigned long long)m, nrows);
-    // table (copied): [v_off | nb | m];  zeroed: [bcount | bfill | scan status + tickets | bad];  then head, boff,
-    // unit, ublk, keep, kex
-    const size_t b_tab = (nrows + 3) * sizeof(uint64_t);
-    const size_t b_zero = nb * sizeof(u64) + ((nb * sizeof(u32) + 15) & ~size_t(15)) + (t_blk + t_elem) * sizeof(u64) + 16;
-    const size_t b_rest = (m + (nb + 1) + units + m + (m + 1)) * sizeof(u64) + ((units * sizeof(u32) + 15) & ~size_t(15));
-    void *h_raw, *d_raw;
-    int rc = l->host.alloc(b_tab, &h_raw);
-    if (rc) return rc;
-    rc = l->ws.alloc(b_tab + b_zero + b_rest, &d_raw);
-    if (rc) return rc;
-    uint64_t* h_tab = (uint64_t*)h_raw;
+    // the copied table is [v_off | nb | m]
+    IcwMatrixParams P;
+    uint64_t* h_tab;
+    u64* status;
+    u32* tickets;
+    WsCarve ws(l);
+    ws.copied(&P.v_off, &h_tab, nrows + 3);
+    if (int rc = ws.stage()) return rc;
     memcpy(h_tab, v_off, (nrows + 1) * sizeof(uint64_t));
     h_tab[nrows + 1] = nb;
     h_tab[nrows + 2] = m;
-    char* d = (char*)d_raw;
-    CK(cudaMemcpyAsync(d, h_tab, b_tab, cudaMemcpyHostToDevice, l->stream));
-    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
-    g_stats.h2d += b_tab;
-    IcwMatrixParams P;
+    ws.zeroed(&P.bcount, nb);
+    ws.zeroed(&P.bfill, nb);
+    ws.zeroed(&status, t_blk + t_elem);
+    ws.zeroed(&tickets, 2);
+    ws.zeroed(&P.bad, 1);
+    ws.plain(&P.head, m);
+    ws.plain(&P.boff, nb + 1);
+    ws.plain(&P.unit, units);
+    ws.plain(&P.keep, m);
+    ws.plain(&P.kex, m + 1);
+    ws.plain(&P.ublk, units);
+    if (int rc = ws.commit()) return rc;
     P.pk = pk.pk;
     P.v = (const u64*)d_v;
     P.m = m;
-    P.v_off = (const u64*)d;
     P.nrows = nrows;
     const u64* d_nb = P.v_off + nrows + 1;  // scan lengths as device words
     const u64* d_m = P.v_off + nrows + 2;
-    char* z = d + b_tab;
-    P.bcount = (u64*)z;
-    P.bfill = (u32*)(P.bcount + nb);
-    u64* status = (u64*)((char*)P.bfill + ((nb * sizeof(u32) + 15) & ~size_t(15)));
-    u32* tickets = (u32*)(status + t_blk + t_elem);
-    P.bad = (int*)(tickets + 2);
-    P.head = (u64*)(z + b_zero);
-    P.boff = P.head + m;
-    P.unit = P.boff + nb + 1;
-    P.keep = P.unit + units;
-    P.kex = P.keep + m;
-    P.ublk = (u32*)(P.kex + m + 1);
     P.unit_cap = units;
     P.out = (u64*)d_out;
     P.out_cap = out_cap;
@@ -2667,35 +2692,37 @@ static int list_uids_impl(dgx_lane* l, const dgx_dev_pack* const* packs, const u
     if (std::max({g_mut, g_rows, g_write}) > kMaxGrid)
         return fail(DGX_ERR_ARG, "batch too large for one launch (%llu uids, %zu rows)", (unsigned long long)(a_cap + nmut),
                     nrows);
-    // table (copied): [mut_off | first | nmut | nrows | mode];  zeroed: [scan status + tickets | bad];  then a, a_off,
-    // cls, cls_ex, lo, cnt
-    const size_t b_tab = ((2 * nrows + 3) * sizeof(uint64_t) + nrows + 15) & ~size_t(15);
-    const size_t b_zero = (t_mut + t_rows) * sizeof(u64) + 16;
-    const size_t b_rest = (a_cap + 2 + (nrows + 1) + nmut + (nmut + 1) + 2 * nrows) * sizeof(u64);
-    void *h_raw, *d_raw;
-    int rc = l->host.alloc(b_tab, &h_raw);
-    if (rc) return rc;
-    rc = l->ws.alloc(b_tab + b_zero + b_rest, &d_raw);
-    if (rc) return rc;
-    uint64_t* h_tab = (uint64_t*)h_raw;
-    memcpy(h_tab, mut_off, (nrows + 1) * sizeof(uint64_t));
+    LuParams P;
+    uint64_t *h_off, *h_first, *h_len;
+    const u64* d_nmut;  // scan lengths as device words: nmut, nrows
+    unsigned char* h_mode;
+    u64 *status, *a, *a_off;
+    u32* tickets;
+    WsCarve ws(l);
+    ws.copied(&P.mut_off, &h_off, nrows + 1);
+    ws.copied(&P.first, &h_first, nrows);
+    ws.copied(&d_nmut, &h_len, 2);
+    ws.copied(&P.mode, &h_mode, nrows);
+    if (int rc = ws.stage()) return rc;
+    memcpy(h_off, mut_off, (nrows + 1) * sizeof(uint64_t));
     for (size_t i = 0; i < nrows; ++i) {
         const bool reads_pack = mode[i] != LU_COMPRESSED && packs[i] && packs[i]->pk.nblocks;
-        h_tab[nrows + 1 + i] = reads_pack ? (uint64_t)(uintptr_t)packs[i]->pk.base : 0;
+        h_first[i] = reads_pack ? (uint64_t)(uintptr_t)packs[i]->pk.base : 0;
     }
-    h_tab[2 * nrows + 1] = nmut;
-    h_tab[2 * nrows + 2] = nrows;
-    memcpy(h_tab + 2 * nrows + 3, mode, nrows);
-    char* d = (char*)d_raw;
-    CK(cudaMemcpyAsync(d, h_tab, b_tab, cudaMemcpyHostToDevice, l->stream));
-    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
-    g_stats.h2d += b_tab;
-    LuParams P;
-    P.mut_off = (const u64*)d;
-    P.first = (const u64* const*)(P.mut_off + nrows + 1);
-    const u64* d_nmut = P.mut_off + 2 * nrows + 1;  // scan lengths as device words
+    h_len[0] = nmut;
+    h_len[1] = nrows;
+    memcpy(h_mode, mode, nrows);
+    ws.zeroed(&status, t_mut + t_rows);
+    ws.zeroed(&tickets, 2);
+    ws.zeroed(&P.bad, 1);
+    ws.plain(&a, a_cap + 2);
+    ws.plain(&a_off, nrows + 1);
+    ws.plain(&P.cls, nmut);
+    ws.plain(&P.cls_ex, nmut + 1);
+    ws.plain(&P.lo, nrows);
+    ws.plain(&P.cnt, nrows);
+    if (int rc = ws.commit()) return rc;
     const u64* d_nrows = d_nmut + 1;
-    P.mode = (const unsigned char*)(d_nrows + 1);
     P.nrows = nrows;
     P.mut = (const u64*)d_mut;
     P.flags = d_flags;
@@ -2703,25 +2730,15 @@ static int list_uids_impl(dgx_lane* l, const dgx_dev_pack* const* packs, const u
     P.after = after;
     P.v = (const u64*)d_v;
     P.m = m;
-    u64* status = (u64*)(d + b_tab);
-    u32* tickets = (u32*)(status + t_mut + t_rows);
-    P.bad = (int*)(tickets + 2);
-    u64* a = (u64*)(d + b_tab + b_zero);
-    u64* a_off = a + a_cap + 2;
     P.a = a;
     P.a_off = a_off;
     P.a_cap = a_cap;
-    P.cls = a_off + nrows + 1;
-    P.cls_ex = P.cls + nmut;
-    P.lo = P.cls_ex + nmut + 1;
-    P.cnt = P.lo + nrows;
     P.out = (u64*)d_out;
     P.out_cap = out_cap;
     P.out_off = (u64*)d_out_off;
     P.err = l->d_err;
     // pack ∩ v of every row from uid 0: each mode applies its own bound afterwards
-    rc = icw_rows_impl(l, packs, nrows, 0, d_v, m, (uint64_t*)a, a_cap, (uint64_t*)a_off);
-    if (rc) return rc;
+    if (int rc = icw_rows_impl(l, packs, nrows, 0, d_v, m, (uint64_t*)a, a_cap, (uint64_t*)a_off)) return rc;
     lu_classify_kernel<<<(unsigned)g_mut, 256, 0, l->stream>>>(P);
     CK(cudaGetLastError());
     scan_u64_kernel<<<(unsigned)t_mut, EN_NT, 0, l->stream>>>(P.cls, P.cls_ex, d_nmut, nmut, status, tickets, nullptr);
@@ -2819,16 +2836,16 @@ static int list_unfiltered_impl(dgx_lane* l, const dgx_dev_pack* const* packs, s
     for (size_t i = 0; i < nrows; ++i)
         if (packs[i] && packs[i]->pk.nblocks) ++nj;
     if (nj >= kLuuNoJob) return fail(DGX_ERR_ARG, "batch too large for one launch (%zu rows)", nrows);
-    // table (copied): [jobs | row_job | mut_off | nmut | nrows];  zeroed: [scan status + tickets | bad];  then cls,
-    // cls_ex, rank, skip, sblk, len
-    const size_t b_jobs = (nj * sizeof(LuuJob) + 15) & ~size_t(15), b_rj = (nrows * sizeof(u32) + 15) & ~size_t(15);
-    const size_t b_tab = b_jobs + b_rj + (nrows + 3) * sizeof(uint64_t);
-    void* h_raw;
-    int rc = l->host.alloc(b_tab, &h_raw);
-    if (rc) return rc;
-    LuuJob* hj = (LuuJob*)h_raw;
-    u32* h_rj = (u32*)((char*)h_raw + b_jobs);
-    uint64_t* h_off = (uint64_t*)((char*)h_raw + b_jobs + b_rj);
+    // the copied table ends [mut_off | nmut | nrows]
+    LuuParams P;
+    LuuJob* hj;
+    u32* h_rj;
+    uint64_t* h_off;
+    WsCarve ws(l);
+    ws.copied(&P.jobs, &hj, nj);
+    ws.copied(&P.row_job, &h_rj, nrows);
+    ws.copied(&P.mut_off, &h_off, nrows + 3);
+    if (int rc = ws.stage()) return rc;
     uint64_t warps = 0, exact = 0;
     for (size_t i = 0, j = 0; i < nrows; ++i) {
         const dgx_dev_pack* p = packs[i];
@@ -2850,21 +2867,20 @@ static int list_unfiltered_impl(dgx_lane* l, const dgx_dev_pack* const* packs, s
     const uint64_t t_mut = std::max<uint64_t>((nmut + EN_TILE - 1) / EN_TILE, 1), t_rows = (nrows + EN_TILE - 1) / EN_TILE;
     if (std::max({g_cls, g_write}) > kMaxGrid)
         return fail(DGX_ERR_ARG, "batch too large for one launch (%llu entries, %zu rows)", (unsigned long long)nmut, nrows);
-    const size_t b_zero = (t_mut + t_rows) * sizeof(u64) + 16;
-    const size_t b_rest = (3 * nmut + 1 + 3 * nrows) * sizeof(u64);
-    void* d_raw;
-    rc = l->ws.alloc(b_tab + b_zero + b_rest, &d_raw);
-    if (rc) return rc;
-    char* d = (char*)d_raw;
-    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
-    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
-    g_stats.h2d += b_tab;
-    LuuParams P;
-    P.jobs = (const LuuJob*)d;
+    u64* status;
+    u32* tickets;
+    ws.zeroed(&status, t_mut + t_rows);
+    ws.zeroed(&tickets, 2);
+    ws.zeroed(&P.bad, 1);
+    ws.plain(&P.cls, nmut);
+    ws.plain(&P.cls_ex, nmut + 1);
+    ws.plain(&P.rank, nmut);
+    ws.plain(&P.skip, nrows);
+    ws.plain(&P.sblk, nrows);
+    ws.plain(&P.len, nrows);
+    if (int rc = ws.commit()) return rc;
     P.njobs = (u32)nj;
     P.nwarps = warps;
-    P.row_job = (const u32*)(d + b_jobs);
-    P.mut_off = (const u64*)(d + b_jobs + b_rj);
     const u64* d_nmut = P.mut_off + nrows + 1;  // scan lengths as device words
     const u64* d_nrows = d_nmut + 1;
     P.nrows = nrows;
@@ -2873,15 +2889,6 @@ static int list_unfiltered_impl(dgx_lane* l, const dgx_dev_pack* const* packs, s
     P.nmut = nmut;
     P.after = after;
     P.first = first;
-    u64* status = (u64*)(d + b_tab);
-    u32* tickets = (u32*)(status + t_mut + t_rows);
-    P.bad = (int*)(tickets + 2);
-    P.cls = (u64*)(d + b_tab + b_zero);
-    P.cls_ex = P.cls + nmut;
-    P.rank = P.cls_ex + nmut + 1;
-    P.skip = P.rank + nmut;
-    P.sblk = P.skip + nrows;
-    P.len = P.sblk + nrows;
     P.counts = d_counts;
     P.out = (u64*)d_out;
     P.out_cap = out_cap;
@@ -3008,6 +3015,8 @@ static void count_launches(dgx_lane* l, int n) {
 }
 // Grid of the grid-stride passes whose length only the device knows (segments, blocks).
 static unsigned stride_grid() { return (unsigned)(g_num_sms * 8); }
+// Tiles of a scan_u64_kernel over n values, at least one (its grid).
+static uint64_t scan_tiles(uint64_t n) { return std::max<uint64_t>(1, (n + EN_TILE - 1) / EN_TILE); }
 
 // Sum of ExactLen over the rows must stay below 2^32: checked before anything is copied.
 template <class Row>
@@ -3033,13 +3042,14 @@ static int tb_plan(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows, 
     uint64_t nblk = 0, exact = 0;
     for (size_t i = 0; i < nrows; ++i)
         if (packs[i] && packs[i]->pk.nblocks) ++nj;
-    // table (copied): [jobs | row_blk (nrows + 1) | nblk];  zeroed: [status | ticket];  stop (all ones);  last, bytes, boff
-    const size_t b_jobs = (nj * sizeof(TbJob) + 15) & ~size_t(15), b_tab = b_jobs + (nrows + 2) * sizeof(uint64_t);
-    void* h_raw;
-    int rc = l->host.alloc(b_tab, &h_raw);
-    if (rc) return rc;
-    TbJob* hj = (TbJob*)h_raw;
-    uint64_t* h_rb = (uint64_t*)((char*)h_raw + b_jobs);
+    // the copied row_blk table ends with nblk again: the scan length as a device word
+    TbParams& P = R->P;
+    TbJob* hj;
+    uint64_t* h_rb;
+    WsCarve ws(l);
+    ws.copied(&P.jobs, &hj, nj);
+    ws.copied(&P.row_blk, &h_rb, nrows + 2);
+    if (int rc = ws.stage()) return rc;
     for (size_t i = 0, j = 0; i < nrows; ++i) {
         h_rb[i] = nblk;
         const dgx_dev_pack* p = packs[i];
@@ -3054,29 +3064,18 @@ static int tb_plan(dgx_lane* l, const dgx_dev_pack* const* packs, size_t nrows, 
     h_rb[nrows] = nblk;
     h_rb[nrows + 1] = nblk;
     const size_t tiles = std::max<size_t>(1, (nblk + EN_TILE - 1) / EN_TILE);
-    const size_t b_zero = tiles * sizeof(u64) + 16, b_stop = nrows * sizeof(u64);
-    void* d_raw;
-    rc = l->ws.alloc(b_tab + b_zero + b_stop + (3 * nblk + 1) * sizeof(u64), &d_raw);
-    if (rc) return rc;
-    char* d = (char*)d_raw;
-    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
-    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
-    CK(cudaMemsetAsync(d + b_tab + b_zero, 0xff, b_stop, l->stream));
-    g_stats.h2d += b_tab;
+    ws.zeroed(&R->status, tiles);
+    ws.zeroed(&R->ticket, 4);
+    ws.ones(&P.stop, nrows);
+    ws.plain(&P.last, nblk);
+    ws.plain(&P.bytes, nblk);
+    ws.plain(&P.boff, nblk + 1);
+    if (int rc = ws.commit()) return rc;
     g_stats.uids_in += exact;
-    TbParams& P = R->P;
-    P.jobs = (const TbJob*)d;
     P.njobs = (u32)nj;
     P.nblk = nblk;
-    P.row_blk = (const u64*)(d + b_jobs);
     P.nrows = nrows;
     R->d_nblk = P.row_blk + nrows + 1;
-    R->status = (u64*)(d + b_tab);
-    R->ticket = (u32*)(R->status + tiles);
-    P.stop = (u64*)(d + b_tab + b_zero);
-    P.last = P.stop + nrows;
-    P.bytes = P.last + nblk;
-    P.boff = P.bytes + nblk;
     P.out = nullptr;
     P.out_cap = 0;
     P.out_off = nullptr;
@@ -3192,52 +3191,40 @@ static int bf_plan(dgx_lane* l, const uint8_t* d_buf, const uint64_t* buf_off, s
                    BfRun* R) {
     const uint64_t n = buf_off[nrows];
     const size_t T = n / EN_TILE + 1, Tr = nrows / EN_TILE + 1;  // look-back words per scan region
-    const size_t b_tab = (nrows + 2) * sizeof(uint64_t);
-    const size_t b_zero = 64 + 32 + 16 + (4 * T + Tr) * sizeof(u64) + ((T * sizeof(u32) + 15) & ~size_t(15)) + 2 * T * sizeof(u64);
-    const size_t b_rest = (8 * n) + ((4 * n + 15) & ~size_t(15)) + 8 * nrows + ((4 * (n + 1) + 15) & ~size_t(15)) +
-                          8 * n + 8 * (n + 1) + 8 * n + 8 * (n + 1) + ((4 * n + 15) & ~size_t(15)) + 8 * (nrows + 1) +
-                          8 * nrows + 64;
-    void *h_raw, *d_raw;
-    int rc = l->host.alloc(b_tab, &h_raw);
-    if (rc) return rc;
-    memcpy(h_raw, buf_off, (nrows + 1) * sizeof(uint64_t));
-    ((uint64_t*)h_raw)[nrows + 1] = nrows;
-    rc = l->ws.alloc(b_tab + b_zero + b_rest, &d_raw);
-    if (rc) return rc;
-    char* d = (char*)d_raw;
-    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
-    CK(cudaMemsetAsync(d + b_tab, 0, b_zero, l->stream));
-    g_stats.h2d += b_tab;
+    // the copied row_off table ends with nrows: the scan length as a device word
     BfParams& P = R->P;
+    uint64_t* h_off;
+    WsCarve ws(l);
+    ws.copied(&P.row_off, &h_off, nrows + 2);
+    if (int rc = ws.stage()) return rc;
+    memcpy(h_off, buf_off, (nrows + 1) * sizeof(uint64_t));
+    h_off[nrows + 1] = nrows;
+    ws.zeroed(&P.counts, 8);
+    ws.zeroed(&P.ticket, 8);
+    ws.zeroed(&P.bad, 4);
+    ws.zeroed(&P.status, 4 * T + Tr);
+    ws.zeroed(&P.sum_flag, T);
+    ws.zeroed(&P.sum_val, 2 * T);
+    ws.plain(&P.pre, n);
+    ws.plain(&P.vrow, n);
+    ws.plain(&P.rowbase, nrows);
+    ws.plain(&P.seg_start, n + 1);
+    ws.plain(&P.seg_cnt, n);
+    ws.plain(&P.seg_blk, n + 1);
+    ws.plain(&P.blk_bytes, n);
+    ws.plain(&P.blk_doff, n + 1);
+    ws.plain(&P.brow, n);
+    ws.plain(&P.row_blk, nrows + 1);
+    ws.plain(&P.img_bytes, nrows);
+    if (int rc = ws.commit()) return rc;
     P.buf = d_buf;
     P.n = n;
-    P.row_off = (const u64*)d;
     R->d_nrows = P.row_off + nrows + 1;
     P.nrows = nrows;
     P.bsz = block_size ? block_size : 1;
-    char* z = d + b_tab;
-    P.counts = (u64*)z;
-    P.ticket = (u32*)(z + 64);
-    P.bad = (int*)(z + 96);
-    P.status = (u64*)(z + 112);
     R->st_segscan = P.status + 2 * T;
     R->st_bytescan = P.status + 3 * T;
     R->st_imgscan = P.status + 4 * T;
-    P.sum_flag = (u32*)(P.status + 4 * T + Tr);
-    P.sum_val = (u64*)((char*)P.sum_flag + ((T * sizeof(u32) + 15) & ~size_t(15)));
-    char* q = d + b_tab + b_zero;
-    auto take = [&](size_t bytes) { char* r = q; q += (bytes + 15) & ~size_t(15); return r; };
-    P.pre = (u64*)take(8 * n);
-    P.vrow = (u32*)take(4 * n);
-    P.rowbase = (u64*)take(8 * nrows);
-    P.seg_start = (u32*)take(4 * (n + 1));
-    P.seg_cnt = (u64*)take(8 * n);
-    P.seg_blk = (u64*)take(8 * (n + 1));
-    P.blk_bytes = (u64*)take(8 * n);
-    P.blk_doff = (u64*)take(8 * (n + 1));
-    P.brow = (u32*)take(4 * n);
-    P.row_blk = (u64*)take(8 * (nrows + 1));
-    P.img_bytes = (u64*)take(8 * nrows);
     R->tiles = (n + EN_TILE - 1) / EN_TILE;
     R->row_tiles = (nrows + EN_TILE - 1) / EN_TILE;
     P.img = nullptr;
@@ -3396,40 +3383,35 @@ static int merge_matrix_impl(dgx_lane* l, const uint64_t* d_v, const uint64_t* d
     const uint64_t ntiles = (v_cap + XM_T - 1) / XM_T, ns_cap = ntiles * XM_SPR, nk_cap = 2 * ns_cap + 1;
     const uint64_t nchunks = (v_cap + XM_H - 1) / XM_H;
     const uint64_t t_keys = (nk_cap + EN_TILE - 1) / EN_TILE, t_chunks = (nchunks + EN_TILE - 1) / EN_TILE;
-    // zeroed: [kcnt | kfill | scan status | tickets];  then runs, samples, soff, split, words, koff, bucketed, cstart,
-    // ccount, cpos, rlen (u32), key (u32)
-    const size_t b_zero = (2 * nk_cap + t_keys + t_chunks + 2) * sizeof(u64);
-    const size_t w_rest = ntiles * XM_T + ns_cap + 2 * ntiles + ns_cap + 4 + (nk_cap + 1) + v_cap + 3 * nchunks + 1;
-    const size_t b_u32 = ((ntiles + ntiles * XM_T) * sizeof(u32) + 15) & ~size_t(15);
-    void* d_raw;
-    int rc = l->ws.alloc(b_zero + w_rest * sizeof(u64) + b_u32, &d_raw);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(d_raw, 0, b_zero, l->stream));
     XmParams P;
+    u64 *status, *split, *words;  // words: nsplit, nkeys, nchunks
+    u32* tickets;
+    WsCarve ws(l);
+    ws.zeroed(&P.kcnt, nk_cap);
+    ws.zeroed(&P.kfill, nk_cap);
+    ws.zeroed(&status, t_keys + t_chunks);
+    ws.zeroed(&tickets, 4);
+    ws.plain(&P.runs, ntiles * XM_T);
+    ws.plain(&P.samples, ns_cap);
+    ws.plain(&P.soff, 2 * ntiles);
+    ws.plain(&split, ns_cap);
+    ws.plain(&words, 4);
+    ws.plain(&P.koff, nk_cap + 1);
+    ws.plain(&P.bucketed, v_cap);
+    ws.plain(&P.cstart, nchunks);
+    ws.plain(&P.ccount, nchunks);
+    ws.plain(&P.cpos, nchunks + 1);
+    ws.plain(&P.rlen, ntiles);
+    ws.plain(&P.key, ntiles * XM_T);
+    if (int rc = ws.commit()) return rc;
     P.v = (const u64*)d_v;
     P.v_off = (const u64*)d_v_off;
     P.nrows = nrows;
     P.v_cap = v_cap;
-    P.kcnt = (u64*)d_raw;
-    P.kfill = P.kcnt + nk_cap;
-    u64* status = P.kfill + nk_cap;
-    u32* tickets = (u32*)(status + t_keys + t_chunks);
-    P.runs = (u64*)((char*)d_raw + b_zero);
-    P.samples = P.runs + ntiles * XM_T;
-    P.soff = P.samples + ns_cap;
-    u64* split = P.soff + 2 * ntiles;
-    u64* words = split + ns_cap;  // nsplit, nkeys, nchunks
     P.split = split;
     P.nsplit = words;
     P.nkeys = words + 1;
     P.nch = words + 2;
-    P.koff = words + 4;
-    P.bucketed = P.koff + nk_cap + 1;
-    P.cstart = P.bucketed + v_cap;
-    P.ccount = P.cstart + nchunks;
-    P.cpos = P.ccount + nchunks;
-    P.rlen = (u32*)(P.cpos + nchunks + 1);
-    P.key = P.rlen + ntiles;
     P.ntiles = (u32)ntiles;
     P.nchunks = (u32)nchunks;
     P.out = (u64*)d_out;
@@ -3443,8 +3425,8 @@ static int merge_matrix_impl(dgx_lane* l, const uint64_t* d_v, const uint64_t* d
     std::vector<MRef> sruns(ntiles);
     std::vector<uint64_t> sub(ntiles, XM_SPR);
     for (uint64_t t = 0; t < ntiles; ++t) sruns[t] = MRef{P.samples, P.soff + 2 * t, (u64)XM_SPR};
-    rc = merge_tree_impl(l, std::move(sruns), std::move(sub), ns_cap, (uint64_t*)split, ns_cap, (uint64_t*)words);
-    if (rc) return rc;
+    if (int rc = merge_tree_impl(l, std::move(sruns), std::move(sub), ns_cap, (uint64_t*)split, ns_cap, (uint64_t*)words))
+        return rc;
     xm_count_kernel<<<(unsigned)ntiles, XM_NT, 0, l->stream>>>(P);
     CK(cudaGetLastError());
     scan_u64_kernel<<<(unsigned)t_keys, EN_NT, 0, l->stream>>>(P.kcnt, P.koff, P.nkeys, nk_cap, status, tickets, nullptr);
@@ -3553,21 +3535,18 @@ static int gb_sort(dgx_lane* l, uint64_t tiles, const int* bad, const u64* h_wor
 // The checks, the pairs and the edge scan: three launches.  Workspace: 24 bytes per parent value of par_cap.
 static int gb_front(dgx_lane* l, GbParams& P, u32** tickets) {
     const uint64_t pc = std::max<uint64_t>(P.par_cap, 1), st = (pc + EN_TILE - 1) / EN_TILE;
-    // zeroed: [bad | words | tickets | scan status], so a refused input leaves every count at 0
-    const size_t b_head = 64 + GB_WORDS * sizeof(u64) + 32 * sizeof(u32), b_zero = b_head + st * sizeof(u64);
-    void *z, *w;
-    int rc = l->ws.alloc(b_zero, &z);
-    if (rc) return rc;
-    if ((rc = l->ws.alloc((2 * pc + 1) * sizeof(u64) + 2 * pc * sizeof(u32), &w))) return rc;
-    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
-    P.bad = (int*)z;
-    P.words = (u64*)((char*)z + 64);
-    *tickets = (u32*)(P.words + GB_WORDS);
-    u64* status = (u64*)((char*)z + b_head);
-    P.plen = (u64*)w;
-    P.eoff = P.plen + pc;
-    P.prow = (u32*)(P.eoff + pc + 1);
-    P.ppar = P.prow + pc;
+    // the words are zeroed, so a refused input leaves every count at 0
+    u64* status;
+    WsCarve ws(l);
+    ws.zeroed(&P.bad, 16);
+    ws.zeroed(&P.words, GB_WORDS);
+    ws.zeroed(tickets, 32);
+    ws.zeroed(&status, st);
+    ws.plain(&P.plen, pc);
+    ws.plain(&P.eoff, pc + 1);
+    ws.plain(&P.prow, pc);
+    ws.plain(&P.ppar, pc);
+    if (int rc = ws.commit()) return rc;
     P.err = l->d_err;
     const uint64_t nt = std::max(std::max(P.nrows + 1, P.npar + 1), std::max(P.ndest, P.v_cap));
     gb_check_kernel<<<gb_grid(nt), 256, 0, l->stream>>>(P);
@@ -3587,35 +3566,33 @@ static int gb_back(dgx_lane* l, GbParams& P, const GbPlan& g, u32* ticket) {
     const uint64_t ec = std::max<uint64_t>(P.e_cap, 1);
     P.tiles = (ec + GB_TILE - 1) / GB_TILE;
     const uint64_t hn = (uint64_t)GB_RADIX * P.tiles, ht = (hn + EN_TILE - 1) / EN_TILE, et = (ec + EN_TILE - 1) / EN_TILE;
-    const size_t b_zero = ((g.p1 + g.p2) * ht + 2 * et) * sizeof(u64);
-    void *z, *w;
-    int rc = l->ws.alloc(b_zero, &z);
-    if (rc) return rc;
-    const size_t n64 = 2 * ec + ec + (ec + 1) + (ec + 1) + 2 * ec + ec + (ec + 1) + hn + (hn + 1);
-    if ((rc = l->ws.alloc(n64 * sizeof(u64) + 5 * ec * sizeof(u32), &w))) return rc;
-    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
-    u64* status = (u64*)z;
-    u64* q = (u64*)w;
-    u64* ek[2] = {q, q + ec};
-    q += 2 * ec;
-    P.head = q;
-    P.gidx = P.head + ec;
-    P.gstart = P.gidx + ec + 1;
-    u64* gk[2] = {P.gstart + ec + 1, P.gstart + 2 * ec + 1};
-    P.gsz = gk[1] + ec;
-    P.moff = P.gsz + ec;
-    u64* hist = P.moff + ec + 1;
-    u64* hoff = hist + hn;
-    u32* r = (u32*)(hoff + hn + 1);
-    u32* ep[2] = {r, r + ec};
-    u32* gp[2] = {r + 2 * ec, r + 3 * ec};
-    P.inv = r + 4 * ec;
+    u64 *status, *ek[2], *gk[2], *hist, *hoff;
+    u32 *ep[2], *gp[2];
+    WsCarve ws(l);
+    ws.zeroed(&status, (g.p1 + g.p2) * ht + 2 * et);
+    ws.plain(&ek[0], ec);
+    ws.plain(&ek[1], ec);
+    ws.plain(&P.head, ec);
+    ws.plain(&P.gidx, ec + 1);
+    ws.plain(&P.gstart, ec + 1);
+    ws.plain(&gk[0], ec);
+    ws.plain(&gk[1], ec);
+    ws.plain(&P.gsz, ec);
+    ws.plain(&P.moff, ec + 1);
+    ws.plain(&hist, hn);
+    ws.plain(&hoff, hn + 1);
+    ws.plain(&ep[0], ec);
+    ws.plain(&ep[1], ec);
+    ws.plain(&gp[0], ec);
+    ws.plain(&gp[1], ec);
+    ws.plain(&P.inv, ec);
+    if (int rc = ws.commit()) return rc;
     P.ek = ek[0];
     P.ep = ep[0];
     gb_expand_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
     CK(cudaGetLastError());
-    if ((rc = gb_sort(l, P.tiles, P.bad, P.words + GB_W_H, ek, ep, P.words + GB_W_E, g.p1, hist, hoff, status,
-                      ticket)))
+    if (int rc = gb_sort(l, P.tiles, P.bad, P.words + GB_W_H, ek, ep, P.words + GB_W_E, g.p1, hist, hoff, status,
+                         ticket))
         return rc;
     P.ek = ek[g.p1 & 1];
     P.ep = ep[g.p1 & 1];
@@ -3627,8 +3604,8 @@ static int gb_back(dgx_lane* l, GbParams& P, const GbPlan& g, u32* ticket) {
     gb_groups_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P);
     gb_gkeys_kernel<<<gb_grid(ec), 256, 0, l->stream>>>(P, gk[0], gp[0]);
     CK(cudaGetLastError());
-    if ((rc = gb_sort(l, P.tiles, P.bad, P.words + GB_W_H, gk, gp, P.words + GB_W_G, g.p2, hist, hoff, status,
-                      ticket)))
+    if (int rc = gb_sort(l, P.tiles, P.bad, P.words + GB_W_H, gk, gp, P.words + GB_W_G, g.p2, hist, hoff, status,
+                         ticket))
         return rc;
     P.gk = gk[g.p2 & 1];
     P.gp = gp[g.p2 & 1];
@@ -3740,13 +3717,15 @@ extern "C" int dgx_groupby_uid(const uint64_t* src, size_t nrows, const uint64_t
     const uint64_t E = l->h_word[0];
     if (E == 0) return none();
     if (E >= kGbMax) return fail(DGX_ERR_ARG, "%llu restricted edges: at most 2^32 - 1", (unsigned long long)E);
-    void* d_o;
-    if ((rc = l->ws.alloc((3 * E + npar + 4) * sizeof(uint64_t), &d_o))) return rc;
-    P.keys = (u64*)d_o;
-    P.members = members ? P.keys + E : nullptr;
-    P.mem_off = P.keys + 2 * E;
-    P.grp_off = P.mem_off + E + 1;
-    P.sizes = P.grp_off + npar + 1;
+    u64* d_members;
+    WsCarve o(l);
+    o.plain(&P.keys, E);
+    o.plain(&d_members, E);
+    o.plain(&P.mem_off, E + 1);
+    o.plain(&P.grp_off, npar + 1);
+    o.plain(&P.sizes, 2);
+    if ((rc = o.commit())) return rc;
+    P.members = members ? d_members : nullptr;
     P.e_cap = P.grp_cap = P.mem_cap = E;
     if ((rc = gb_back(l, P, g, tickets))) return rc;
     CK(cudaMemcpyAsync(l->h_word, P.sizes, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
@@ -3910,14 +3889,22 @@ static int rc_step(dgx_lane* l, dgx_reach_set* s, const uint64_t* d_src, size_t 
                    const uint64_t* d_v_off, uint64_t v_cap, const uint64_t* d_dest, size_t ndest, uint64_t* d_out,
                    uint64_t* d_out_off, uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_sizes) {
     const uint64_t tiles = (v_cap + EN_TILE - 1) / EN_TILE;
-    // zeroed: [bad | words | ticket | scan status];  then lo, hi, w_off, keep, kex, kfrom, row
-    const size_t b_zero = 64 + tiles * sizeof(u64);
-    const size_t n64 = 2 * nrows + (nrows + 1) + v_cap + (v_cap + 1) + v_cap;
-    void* d_raw;
-    int rc = l->ws.alloc(b_zero + n64 * sizeof(u64) + v_cap * sizeof(u32), &d_raw);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(d_raw, 0, b_zero, l->stream));
     RcParams P;
+    u64* status;
+    u32* ticket;
+    WsCarve ws(l);
+    ws.zeroed(&P.bad, 4);
+    ws.zeroed(&P.words, RC_WORDS);
+    ws.zeroed(&ticket, 6);
+    ws.zeroed(&status, tiles);
+    ws.plain(&P.lo, nrows);
+    ws.plain(&P.hi, nrows);
+    ws.plain(&P.w_off, nrows + 1);
+    ws.plain(&P.keep, v_cap);
+    ws.plain(&P.kex, v_cap + 1);
+    ws.plain(&P.kfrom, v_cap);
+    ws.plain(&P.row, v_cap);
+    if (int rc = ws.commit()) return rc;
     P.src = (const u64*)d_src;
     P.nrows = nrows;
     P.v = (const u64*)d_v;
@@ -3930,17 +3917,6 @@ static int rc_step(dgx_lane* l, dgx_reach_set* s, const uint64_t* d_src, size_t 
         P.sto[b] = (u64*)s->buf[b] + s->cap;
     }
     P.state = (u64*)s->d_state;
-    P.bad = (int*)d_raw;
-    P.words = (u64*)((char*)d_raw + 16);
-    u32* ticket = (u32*)(P.words + RC_WORDS);
-    u64* status = (u64*)((char*)d_raw + 64);
-    P.lo = (u64*)((char*)d_raw + b_zero);
-    P.hi = P.lo + nrows;
-    P.w_off = P.hi + nrows;
-    P.keep = P.w_off + nrows + 1;
-    P.kex = P.keep + v_cap;
-    P.kfrom = P.kex + v_cap + 1;
-    P.row = (u32*)(P.kfrom + v_cap);
     P.out = (u64*)d_out;
     P.out_off = (u64*)d_out_off;
     P.sizes = (u64*)d_sizes;
@@ -3954,8 +3930,8 @@ static int rc_step(dgx_lane* l, dgx_reach_set* s, const uint64_t* d_src, size_t 
     rc_gather_kernel<<<gb_grid(std::max<uint64_t>(v_cap, nrows + 1)), 256, 0, l->stream>>>(P);
     CK(cudaGetLastError());
     count_launches(l, 5);
-    if ((rc = merge_matrix_impl(l, d_out, (const uint64_t*)P.w_off, nrows, v_cap, d_dest_out, dest_cap,
-                                (uint64_t*)(P.words + RC_W_D))))
+    if (int rc = merge_matrix_impl(l, d_out, (const uint64_t*)P.w_off, nrows, v_cap, d_dest_out, dest_cap,
+                                   (uint64_t*)(P.words + RC_W_D)))
         return rc;
     rc_insert_kernel<<<stride_grid(), 256, 0, l->stream>>>(P);
     rc_commit_kernel<<<1, 1, 0, l->stream>>>(P);
@@ -4037,12 +4013,13 @@ extern "C" int dgx_recurse_filter(dgx_reach_set* s, const uint64_t* src, size_t 
     if ((rc = upload_list(l, src, nrows, &d_src)) || (rc = upload_list(l, v, m, &d_v)) ||
         (rc = upload_list(l, v_off, nrows + 1, &d_v_off)) || (dest && (rc = upload_list(l, dest, ndest, &d_dest))))
         return rc;
-    void* d_o;
-    if ((rc = l->ws.alloc((2 * m + nrows + 3) * sizeof(uint64_t), &d_o))) return rc;
-    uint64_t* d_sizes = (uint64_t*)d_o;
-    uint64_t* d_out = d_sizes + 2;
-    uint64_t* d_dest_out = d_out + m;
-    uint64_t* d_off = d_dest_out + m;
+    uint64_t *d_sizes, *d_out, *d_dest_out, *d_off;
+    WsCarve o(l);
+    o.plain(&d_sizes, 2);
+    o.plain(&d_out, m);
+    o.plain(&d_dest_out, m);
+    o.plain(&d_off, nrows + 1);
+    if ((rc = o.commit())) return rc;
     if ((rc = rc_reserve(s, l->stream, s->bound + m))) return rc;
     s->lane = l;  // waited for below, whatever happens
     s->bound += m;
@@ -4185,76 +4162,61 @@ static void cc_plan(const dgx_cascade_tree* t, const CcSrc* src, CcPlan* P) {
     }
 }
 
-static uint64_t cc_tiles(uint64_t n) { return std::max<uint64_t>(1, (n + EN_TILE - 1) / EN_TILE); }
-
 // The whole call on the lane: one metadata copy, 4 + 7 * D launches.  Workspace: 44 bytes per value slot (gathered
 // and kept values 16, and a level's flags, their three scans and rows 28), 16 per offset slot, 16 per dest slot plus
 // 16 per dest slot of the largest level, 1 per has_val byte, about 140 per node, and the scans' look-back words.
 static int cc_run(dgx_lane* l, const CcPlan& T, uint64_t* d_out, uint64_t* d_out_off, uint64_t* d_dest_out,
                   uint64_t* d_dest_off, uint64_t* d_sizes) {
     const uint64_t NN = T.node.size(), D = T.level.size();
-    uint64_t nstatus = cc_tiles(2 * NN);
-    for (const CcLevel& L : T.level) nstatus += cc_tiles(L.nd) + 2 * cc_tiles(L.nv);
+    uint64_t nstatus = scan_tiles(2 * NN);
+    for (const CcLevel& L : T.level) nstatus += scan_tiles(L.nd) + 2 * scan_tiles(L.nv);
     const uint64_t nscan = 3 * D + 1;
-    // host metadata, one copy: nodes, checked children, the scans' size words
-    const size_t b_node = NN * sizeof(CcNode), b_ck = (T.ck.size() + 1) * sizeof(uint32_t);
-    const size_t b_meta = ((b_node + b_ck + 15) & ~size_t(15)) + (2 * D + 1) * sizeof(uint64_t);
-    void* h_meta;
-    int rc = l->host.alloc(b_meta, &h_meta);
-    if (rc) return rc;
-    memcpy(h_meta, T.node.data(), b_node);
-    if (!T.ck.empty()) memcpy((char*)h_meta + b_node, T.ck.data(), T.ck.size() * sizeof(uint32_t));
-    uint64_t* h_words = (uint64_t*)((char*)h_meta + ((b_node + b_ck + 15) & ~size_t(15)));
+    // copied: the nodes, the checked children and the scans' size words
+    CcParams P;
+    CcNode* h_node;
+    uint32_t* h_ck;
+    uint64_t* h_words;
+    const u64* d_words;
+    u64* status;
+    u32* ticket;
+    WsCarve ws(l);
+    ws.copied(&P.node, &h_node, NN);
+    ws.copied(&P.ck, &h_ck, T.ck.size() + 1);
+    ws.copied(&d_words, &h_words, 2 * D + 1);
+    if (int rc = ws.stage()) return rc;
+    memcpy(h_node, T.node.data(), NN * sizeof(CcNode));
+    if (!T.ck.empty()) memcpy(h_ck, T.ck.data(), T.ck.size() * sizeof(uint32_t));
     for (uint64_t i = 0; i < D; ++i) {
         h_words[2 * i] = T.level[i].nd;
         h_words[2 * i + 1] = T.level[i].nv;
     }
     h_words[2 * D] = 2 * NN;
-    // zeroed: [bad | tickets | look-back status], then the arrays
-    const size_t b_zero = ((16 + nscan * sizeof(u32) + 15) & ~size_t(15)) + nstatus * sizeof(u64);
-    const size_t n64 = 2 * T.nv + 2 * T.no + 2 * T.nd + NN + (2 * T.max_nd + 1) + (3 * T.max_nv + 2) + (4 * NN + 1);
-    const size_t b_meta16 = (b_meta + 15) & ~size_t(15);  // the zeroed region starts 16-byte aligned
-    const size_t bytes = b_meta16 + b_zero + n64 * sizeof(u64) + T.max_nv * sizeof(u32) + T.nh;
-    void* d_raw;
-    if ((rc = l->ws.alloc(bytes, &d_raw))) return rc;
-    char* z = (char*)d_raw + b_meta16;
-    CK(cudaMemcpyAsync(d_raw, h_meta, b_meta, cudaMemcpyHostToDevice, l->stream));
-    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
-    g_stats.h2d += b_meta;
-    CcParams P;
-    P.node = (const CcNode*)d_raw;
-    P.ck = (const u32*)((char*)d_raw + b_node);
-    const u64* d_words = (const u64*)((char*)d_raw + ((b_node + b_ck + 15) & ~size_t(15)));
+    ws.zeroed(&P.bad, 4);
+    ws.zeroed(&ticket, nscan);
+    ws.zeroed(&status, nstatus);
+    ws.plain(&P.V, T.nv);
+    ws.plain(&P.OV, T.nv);
+    ws.plain(&P.VO, T.no);
+    ws.plain(&P.OO, T.no);
+    ws.plain(&P.D, T.nd);
+    ws.plain(&P.ND, T.nd);
+    ws.plain(&P.NDE, NN);
+    ws.plain(&P.keep, T.max_nd);
+    ws.plain(&P.kx, T.max_nd + 1);
+    ws.plain(&P.fv, T.max_nv);
+    ws.plain(&P.fx, T.max_nv + 1);
+    ws.plain(&P.fy, T.max_nv + 1);
+    ws.plain(&P.cnt, 2 * NN);
+    ws.plain(&P.cx, 2 * NN + 1);
+    ws.plain(&P.rw, T.max_nv);
+    ws.plain(&P.H, T.nh);
+    if (int rc = ws.commit()) return rc;
     P.nnodes = (u32)NN;
     P.nv = T.nv;
     P.no = T.no;
     P.nd = T.nd;
     P.nh = T.nh;
     P.out_rows = T.rows;
-    P.bad = (int*)z;
-    u32* ticket = (u32*)(z + 16);
-    u64* status = (u64*)(z + ((16 + nscan * sizeof(u32) + 15) & ~size_t(15)));
-    u64* a = (u64*)(z + b_zero);
-    auto take = [&](uint64_t n) { u64* p = a; a += n; return p; };
-    P.V = take(T.nv);
-    P.OV = take(T.nv);
-    P.VO = take(T.no);
-    P.OO = take(T.no);
-    P.D = take(T.nd);
-    P.ND = take(T.nd);
-    P.NDE = take(NN);
-    P.keep = take(T.max_nd);
-    P.kx = take(T.max_nd + 1);
-    P.fv = take(T.max_nv);
-    P.fx = take(T.max_nv + 1);
-    P.fy = take(T.max_nv + 1);
-    P.cnt = take(2 * NN);
-    P.cx = take(2 * NN + 1);
-    P.rw = (u32*)a;
-    P.H = (unsigned char*)(P.rw + T.max_nv);
-    if (P.H + T.nh != (unsigned char*)d_raw + bytes)
-        return fail(DGX_ERR_CUDA, "cascade workspace layout (%zu bytes) does not match its size (%zu bytes)",
-                    (size_t)(P.H + T.nh - (unsigned char*)d_raw), bytes);
     P.err = l->d_err;
     P.out = (u64*)d_out;
     P.out_off = (u64*)d_out_off;
@@ -4262,7 +4224,7 @@ static int cc_run(dgx_lane* l, const CcPlan& T, uint64_t* d_out, uint64_t* d_out
     P.dest_off = (u64*)d_dest_off;
     P.sizes = (u64*)d_sizes;
     auto scan = [&](const u64* in, u64* out, const u64* n_word, uint64_t n) {
-        const uint64_t tiles = cc_tiles(n);
+        const uint64_t tiles = scan_tiles(n);
         scan_u64_kernel<<<(unsigned)tiles, EN_NT, 0, l->stream>>>(in, out, n_word, n, status, ticket, nullptr);
         status += tiles;
         ticket += 1;
@@ -4369,11 +4331,11 @@ extern "C" int dgx_cascade(const dgx_cascade_tree* tree, const uint64_t* v, cons
     g_stats.uids_in += m + nd;
     uint64_t *d_v, *d_v_off, *d_dest;
     uint8_t* d_hv;
-    void* p;
+    WsCarve in(l);
+    in.plain(&d_hv, nh + 16);
     if ((rc = upload_list(l, v, m, &d_v)) || (rc = upload_list(l, v_off, rows + 1, &d_v_off)) ||
-        (rc = upload_list(l, dest, nd, &d_dest)) || (rc = l->ws.alloc(nh + 16, &p)))
+        (rc = upload_list(l, dest, nd, &d_dest)) || (rc = in.commit()))
         return rc;
-    d_hv = (uint8_t*)p;
     if (nh) CK(cudaMemcpyAsync(d_hv, has_val, nh, cudaMemcpyHostToDevice, l->stream));
     g_stats.h2d += nh;
     std::vector<CcSrc> src(n);
@@ -4385,13 +4347,14 @@ extern "C" int dgx_cascade(const dgx_cascade_tree* tree, const uint64_t* v, cons
     CcPlan T;
     cc_plan(tree, src.data(), &T);
     if ((rc = cc_check_plan(T, m, nd))) return rc;
-    void* d_o;
-    if ((rc = l->ws.alloc((m + nd + rows + n + 4) * sizeof(uint64_t), &d_o))) return rc;
-    uint64_t* d_sizes = (uint64_t*)d_o;
-    uint64_t* d_out = d_sizes + 2;
-    uint64_t* d_dout = d_out + m;
-    uint64_t* d_ooff = d_dout + nd;
-    uint64_t* d_doff = d_ooff + rows + 1;
+    uint64_t *d_sizes, *d_out, *d_dout, *d_ooff, *d_doff;
+    WsCarve o(l);
+    o.plain(&d_sizes, 2);
+    o.plain(&d_out, m);
+    o.plain(&d_dout, nd);
+    o.plain(&d_ooff, rows + 1);
+    o.plain(&d_doff, n + 1);
+    if ((rc = o.commit())) return rc;
     if ((rc = cc_run(l, T, d_out, d_ooff, d_dout, d_doff, d_sizes))) return rc;
     CK(cudaMemcpyAsync(l->h_word, d_sizes, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
     if ((rc = dgx_lane_sync(l))) return rc;
@@ -4547,16 +4510,31 @@ static int ps_level(dgx_lane* l, dgx_path_search* s, size_t nsg, const uint32_t*
     const uint64_t vc = std::max<uint64_t>(v_cap, 1), rc1 = std::max<uint64_t>(r_cap, 1), dc = std::max<uint64_t>(d_cap, 1);
     auto tiles = [](uint64_t n) { return (n + EN_TILE - 1) / EN_TILE; };
     const uint64_t tv = tiles(vc), tr = tiles(rc1), td = tiles(dc);
-    // zeroed: [bad | words | tickets | scan status | rflag | nsgi];  all ones: npar;  then the u64 and u32 arrays
-    const size_t b_head = 128, b_zero = b_head + (tv + tr + td + r_cap + 1) * sizeof(u64) + ((vc * 4 + 15) & ~15ull);
-    const size_t n64 = vc + (vc + 1) + (r_cap + 2) + vc + (r_cap + 2) + (r_cap + 1) + (nsg + 1) + vc + (r_cap + 1) +
-                       dc + (dc + 1);
-    void* d_raw;
-    int rc = l->ws.alloc(b_zero + (vc + n64) * sizeof(u64) + 2 * vc * sizeof(u32), &d_raw);
-    if (rc) return rc;
-    CK(cudaMemsetAsync(d_raw, 0, b_zero, l->stream));
-    CK(cudaMemsetAsync((char*)d_raw + b_zero, 0xff, vc * sizeof(u64), l->stream));
     PsParams P;
+    u64* status;
+    u32* tickets;
+    WsCarve ws(l);
+    ws.zeroed(&P.bad, 4);
+    ws.zeroed(&P.words, PS_WORDS);
+    ws.zeroed(&tickets, 10);
+    ws.zeroed(&status, tv + tr + td);
+    ws.zeroed(&P.rflag, r_cap + 1);
+    ws.zeroed(&P.nsgi, vc);
+    ws.ones(&P.npar, vc);
+    ws.plain(&P.vflag, vc);
+    ws.plain(&P.vpos, vc + 1);
+    ws.plain(&P.rpos, r_cap + 2);
+    ws.plain(&P.nv, vc);
+    ws.plain(&P.nv_off, r_cap + 2);
+    ws.plain(&P.es, r_cap + 1);
+    ws.plain(&P.es_off, nsg + 1);
+    ws.plain(&P.nn, vc);
+    ws.plain(&P.ne, r_cap + 1);
+    ws.plain(&P.dflag, dc);
+    ws.plain(&P.dpos, dc + 1);
+    ws.plain(&P.vrow, vc);
+    ws.plain(&P.vsg, vc);
+    if (int rc = ws.commit()) return rc;
     P.nsg = nsg;
     P.attr = (const u32*)d_attr;
     P.src_off = (const u64*)d_src_off;
@@ -4576,34 +4554,10 @@ static int ps_level(dgx_lane* l, dgx_path_search* s, size_t nsg, const uint32_t*
         P.ex[b] = (u64*)s->ebuf[b];
     }
     P.state = (u64*)s->d_state;
-    char* p = (char*)d_raw;
-    P.bad = (int*)p;
-    P.words = (u64*)(p + 16);
-    u32* tickets = (u32*)(P.words + PS_WORDS);
-    u64* status = (u64*)(p + b_head);
-    P.rflag = status + tv + tr + td;
-    P.nsgi = (u32*)(P.rflag + r_cap + 1);
-    P.npar = (u64*)(p + b_zero);
-    P.vflag = P.npar + vc;
-    P.vpos = P.vflag + vc;
-    P.rpos = P.vpos + vc + 1;
-    P.nv = P.rpos + r_cap + 2;
-    P.nv_off = P.nv + vc;
-    P.es = P.nv_off + r_cap + 2;
-    P.es_off = P.es + r_cap + 1;
-    P.nn = P.es_off + nsg + 1;
-    P.ne = P.nn + vc;
-    P.dflag = P.ne + r_cap + 1;
-    P.dpos = P.dflag + dc;
-    P.vrow = (u32*)(P.dpos + dc + 1);
-    P.vsg = P.vrow + vc;
     P.next = (u64*)d_next;
     P.next_off = (u64*)d_next_off;
     P.stats = (u64*)d_stats;
     P.err = l->d_err;
-    static_assert(16 + PS_WORDS * sizeof(u64) + 3 * sizeof(u32) <= 128, "the level's head words fit their 128 bytes");
-    if ((char*)(P.vsg + vc) != p + b_zero + (vc + n64) * sizeof(u64) + 2 * vc * sizeof(u32))
-        return fail(DGX_ERR_CUDA, "shortest-path workspace layout mismatch");
     ps_check_kernel<<<gb_grid(std::max<uint64_t>({nsg + 1, r_cap + 1, v_cap, d_cap})), 256, 0, l->stream>>>(P);
     ps_flags_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P);
     scan_u64_kernel<<<(unsigned)tv, EN_NT, 0, l->stream>>>(P.vflag, P.vpos, P.words + PS_W_M, v_cap, status, tickets,
@@ -4614,6 +4568,7 @@ static int ps_level(dgx_lane* l, dgx_path_search* s, size_t nsg, const uint32_t*
     CK(cudaGetLastError());
     count_launches(l, 5);
     auto U = [](u64* q) { return (uint64_t*)q; };
+    int rc;
     if ((rc = merge_matrix_impl(l, U(P.nv), U(P.nv_off), rc1, vc, U(P.nn), vc, U(P.words + PS_W_NN))) ||
         (rc = merge_matrix_impl(l, U(P.es), U(P.es_off), nsg, rc1, U(P.ne), rc1, U(P.words + PS_W_NE))))
         return rc;
@@ -4693,25 +4648,26 @@ extern "C" int dgx_path_expand(dgx_path_search* s, const dgx_path_level* L, uint
     g_stats.calls += 1;
     g_stats.uids_in += R + M + D;
     static const uint64_t zero = 0;
-    uint64_t *d_src_off, *d_src, *d_v_off, *d_v, *d_dest_off, *d_dest;
-    void *d_attr, *d_o;
+    uint64_t *d_src_off, *d_src, *d_v_off, *d_v, *d_dest_off, *d_dest, *d_stats, *d_next;
+    uint32_t* d_attr;
+    WsCarve o(l);
+    o.plain(&d_attr, S);
+    o.plain(&d_stats, 3 + S + 1);  // stats, then next_off: read back in one copy
+    o.plain(&d_next, D + 1);
     int rc;
     if ((rc = upload_list(l, L->src_off, S + 1, &d_src_off)) || (rc = upload_list(l, L->src, R, &d_src)) ||
         (rc = upload_list(l, R ? L->v_off : &zero, R + 1, &d_v_off)) || (rc = upload_list(l, L->v, M, &d_v)) ||
         (rc = upload_list(l, L->dest_off, S + 1, &d_dest_off)) || (rc = upload_list(l, L->dest, D, &d_dest)) ||
-        (rc = l->ws.alloc(S * sizeof(uint32_t), &d_attr)))
+        (rc = o.commit()))
         return rc;
     CK(cudaMemcpyAsync(d_attr, L->attr, S * sizeof(uint32_t), cudaMemcpyHostToDevice, l->stream));
     g_stats.h2d += S * sizeof(uint32_t);
-    if ((rc = l->ws.alloc((S + 4 + D + 1) * sizeof(uint64_t), &d_o))) return rc;
-    uint64_t* d_stats = (uint64_t*)d_o;  // stats, then next_off: read back in one copy
     uint64_t* d_next_off = d_stats + 3;
-    uint64_t* d_next = d_next_off + S + 1;
     if ((rc = ps_reserve_all(s, l->stream, s->sbound + std::min(M, D), s->ebound + R))) return rc;
     s->lane = l;  // waited for below, whatever happens
     s->sbound += std::min(M, D);
     s->ebound += R;
-    rc = ps_level(l, s, S, (const uint32_t*)d_attr, d_src_off, d_src, R, d_v_off, d_v, M, d_dest_off, d_dest, D,
+    rc = ps_level(l, s, S, d_attr, d_src_off, d_src, R, d_v_off, d_v, M, d_dest_off, d_dest, D,
                   d_next, d_next_off, d_stats);
     std::vector<uint64_t> head(S + 4);
     if (!rc) CK(cudaMemcpyAsync(head.data(), d_stats, (S + 4) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
@@ -4742,16 +4698,20 @@ extern "C" int dgx_path_result(dgx_path_search* s, uint64_t* uids, uint32_t* att
     if (lease.rc) return lease.rc;
     dgx_lane* l = lease.l;
     g_stats.calls += 1;
-    void* d_o;
-    if (int rc = l->ws.alloc(n * sizeof(uint64_t) + L * sizeof(uint32_t), &d_o)) return rc;
+    u64* d_uids;
+    u32* d_attrs;
+    WsCarve o(l);
+    o.plain(&d_uids, n);
+    o.plain(&d_attrs, L);
+    if (int rc = o.commit()) return rc;
     const uint64_t c = s->st[PS_S_CUR];
     ps_walk_kernel<<<1, 1, 0, l->stream>>>((const u64*)s->sbuf[c], (const u64*)(s->sbuf[c] + 8 * s->scap),
                                            (const u32*)(s->sbuf[c] + 16 * s->scap), (const u64*)s->d_state, L,
-                                           (u64*)d_o, (u32*)((uint64_t*)d_o + n));
+                                           d_uids, d_attrs);
     CK(cudaGetLastError());
     count_launches(l, 1);
-    CK(cudaMemcpyAsync(uids, d_o, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
-    CK(cudaMemcpyAsync(attrs, (uint64_t*)d_o + n, L * sizeof(uint32_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(uids, d_uids, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(attrs, d_attrs, L * sizeof(uint32_t), cudaMemcpyDeviceToHost, l->stream));
     CK(cudaStreamSynchronize(l->stream));
     g_stats.d2h += n * sizeof(uint64_t) + L * sizeof(uint32_t);
     return DGX_OK;
@@ -4762,7 +4722,6 @@ extern "C" int dgx_path_result(dgx_path_search* s, uint64_t* uids, uint32_t* att
 // ---------------------------------------------------------------------------
 constexpr uint64_t kVvMax = uint64_t(1) << 32;  // map sizes, levels, rows, values and dest sizes are 32-bit counts
 
-static uint64_t vv_tiles(uint64_t n) { return std::max<uint64_t>(1, (n + EN_TILE - 1) / EN_TILE); }
 static uint64_t vv_rtiles(uint64_t n) { return std::max<uint64_t>(1, (n + GB_TILE - 1) / GB_TILE); }
 
 // Radix passes of a level: a dest rank needs bits(ndest - 1), the range two more.
@@ -4776,7 +4735,10 @@ struct VvLevel {
     uint64_t nrows, v_cap, ndest;
 };
 
-// Every level on the lane, 9 + 3 P launches each (P = vv_passes(ndest)).  Workspace: 128 bytes of words and tickets per
+// Tickets of a level's scans: two of its own and one per radix pass (at most five passes).
+constexpr size_t kVvTickets = 8;
+
+// Every level on the lane, 9 + 3 P launches each (P = vv_passes(ndest)).  Workspace: 80 bytes of words and tickets per
 // level and the scans' look-back words, zeroed; 72 bytes per value of the largest v_cap (flag and position 16, keys
 // before and after the compaction 16, payloads 8, heads, head indices, segment starts and parts 32) and the largest
 // radix hist; both intermediate maps, 16 bytes per entry of the largest intermediate ndest.  The last level
@@ -4789,41 +4751,41 @@ static int vv_run(dgx_lane* l, bool is_float, const uint64_t* d_key, const uint6
         const uint64_t c = std::max<uint64_t>(L[k].v_cap, 1), h = (uint64_t)GB_RADIX * vv_rtiles(c);
         vc = std::max(vc, c);
         hn = std::max(hn, h);
-        zst += 2 * vv_tiles(c) + vv_passes(L[k].ndest) * vv_tiles(h);
+        zst += 2 * scan_tiles(c) + vv_passes(L[k].ndest) * scan_tiles(h);
         if (k + 1 < nl) mcap = std::max<uint64_t>(mcap, L[k].ndest);
     }
-    const size_t b_head = 64 + 128 * nl, b_zero = b_head + zst * sizeof(u64);
-    const size_t n64 = 8 * vc + 3 + hn + (hn + 1) + 4 * mcap, n32 = 2 * vc;
-    void *z, *w;
-    int rc = l->ws.alloc(b_zero, &z);
-    if (rc) return rc;
-    if ((rc = l->ws.alloc(n64 * sizeof(u64) + n32 * sizeof(u32), &w))) return rc;
-    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
-    int* bad = (int*)z;
-    u64* status = (u64*)((char*)z + b_head);
-    u64* q = (u64*)w;
-    u64* flag = q;
-    u64* pos = flag + vc;
-    u64* ek[2] = {pos + vc + 1, pos + 2 * vc + 1};  // compacted keys, and the raw keys (then the sort's spare)
-    u64* head = ek[1] + vc;
-    u64* hidx = head + vc;
-    u64* sstart = hidx + vc + 1;
-    u64* part = sstart + vc + 1;
-    u64* hist = part + vc;
-    u64* hoff = hist + hn;
-    u64* mk[2] = {hoff + hn + 1, hoff + hn + 1 + mcap};
-    u64* mv[2] = {mk[1] + mcap, mk[1] + 2 * mcap};
-    u32* ep[2] = {(u32*)(mv[1] + mcap), (u32*)(mv[1] + mcap) + vc};
-    static_assert(64 + VV_WORDS * sizeof(u64) + 8 * sizeof(u32) <= 64 + 128, "a level's words and tickets fit");
-    if ((char*)(ep[1] + vc) != (char*)w + n64 * sizeof(u64) + n32 * sizeof(u32))
-        return fail(DGX_ERR_CUDA, "value-variable workspace layout mismatch");
+    int* bad;
+    u64 *level_words, *status, *flag, *pos, *ek[2], *head, *hidx, *sstart, *part, *hist, *hoff, *mk[2], *mv[2];
+    u32 *tickets, *ep[2];
+    WsCarve ws(l);
+    ws.zeroed(&bad, 16);
+    ws.zeroed(&level_words, VV_WORDS * nl);
+    ws.zeroed(&tickets, kVvTickets * nl);
+    ws.zeroed(&status, zst);
+    ws.plain(&flag, vc);
+    ws.plain(&pos, vc + 1);
+    ws.plain(&ek[0], vc);  // compacted keys, and the raw keys (then the sort's spare)
+    ws.plain(&ek[1], vc);
+    ws.plain(&head, vc);
+    ws.plain(&hidx, vc + 1);
+    ws.plain(&sstart, vc + 1);
+    ws.plain(&part, vc);
+    ws.plain(&hist, hn);
+    ws.plain(&hoff, hn + 1);
+    ws.plain(&mk[0], mcap);
+    ws.plain(&mk[1], mcap);
+    ws.plain(&mv[0], mcap);
+    ws.plain(&mv[1], mcap);
+    ws.plain(&ep[0], vc);
+    ws.plain(&ep[1], vc);
+    if (int rc = ws.commit()) return rc;
     const u64* prev_n = nullptr;
     for (size_t k = 0; k < nl; ++k) {
         const VvLevel& V = L[k];
-        const uint64_t c = std::max<uint64_t>(V.v_cap, 1), tv = vv_tiles(c);
+        const uint64_t c = std::max<uint64_t>(V.v_cap, 1), tv = scan_tiles(c);
         const uint32_t passes = vv_passes(V.ndest);
-        u64* words = (u64*)((char*)z + 64 + 128 * k);
-        u32* ticket = (u32*)(words + VV_WORDS);
+        u64* words = level_words + VV_WORDS * k;
+        u32* ticket = tickets + kVvTickets * k;
         VvParams P{};
         P.first = k == 0;
         P.n0 = n;
@@ -4867,8 +4829,8 @@ static int vv_run(dgx_lane* l, bool is_float, const uint64_t* d_key, const uint6
         ticket += 1;
         vv_compact_kernel<<<gb_grid(V.v_cap), 256, 0, l->stream>>>(P);
         CK(cudaGetLastError());
-        if ((rc = gb_sort(l, P.tiles, bad, words + VV_W_H, ek, ep, words + VV_W_E, passes, hist, hoff, status,
-                          ticket)))
+        if (int rc = gb_sort(l, P.tiles, bad, words + VV_W_H, ek, ep, words + VV_W_E, passes, hist, hoff, status,
+                             ticket))
             return rc;
         P.ek = ek[passes & 1];
         P.ep = ep[passes & 1];
@@ -4991,27 +4953,34 @@ extern "C" int dgx_var_propagate(int type, const uint64_t* key, const uint64_t* 
         g_stats.uids_in += V.nrows + V.v_cap + V.ndest;
     }
     const uint64_t D = L[nlevels - 1].ndest;  // the last map has at most one entry per dest value
-    void* d_o;
-    if ((rc = l->ws.alloc((2 * D + 1) * sizeof(uint64_t), &d_o))) return rc;
-    uint64_t* o_len = (uint64_t*)d_o;
-    if ((rc = vv_run(l, type == DGX_VAL_FLOAT64, d_key, d_val, n, L.data(), nlevels, o_len + 1, o_len + 1 + D, D,
-                     o_len)))
+    uint64_t *o_len, *o_key, *o_val;
+    WsCarve o(l);
+    o.plain(&o_len, 1);
+    o.plain(&o_key, D);
+    o.plain(&o_val, D);
+    if ((rc = o.commit())) return rc;
+    if ((rc = vv_run(l, type == DGX_VAL_FLOAT64, d_key, d_val, n, L.data(), nlevels, o_key, o_val, D, o_len)))
         return rc;
-    return vv_finish(l, o_len, o_len + 1, o_len + 1 + D, out_key, out_val, out_cap, out_len);
+    return vv_finish(l, o_len, o_key, o_val, out_key, out_val, out_cap, out_len);
 }
 
 // 4 launches.  Workspace: 24 bytes per row and the scan's look-back words.
 static int la_run(dgx_lane* l, int fn, bool is_float, const uint64_t* d_key, const uint64_t* d_val, uint64_t n,
                   const uint64_t* d_src, uint64_t nrows, const uint64_t* d_v_off, const uint64_t* d_v, uint64_t v_cap,
                   uint64_t* out_key, uint64_t* out_val, uint64_t out_cap, uint64_t* out_len) {
-    const uint64_t tr = vv_tiles(nrows);
-    const size_t b_zero = 64 + tr * sizeof(u64);
-    void *z, *w;
-    int rc = l->ws.alloc(b_zero, &z);
-    if (rc) return rc;
-    if ((rc = l->ws.alloc((3 * nrows + 1) * sizeof(u64), &w))) return rc;
-    CK(cudaMemsetAsync(z, 0, b_zero, l->stream));
+    const uint64_t tr = scan_tiles(nrows);
     VaParams P{};
+    u64* status;
+    u32* ticket;
+    WsCarve ws(l);
+    ws.zeroed(&P.bad, 4);
+    ws.zeroed(&P.words, VA_WORDS);
+    ws.zeroed(&ticket, 8);
+    ws.zeroed(&status, tr);
+    ws.plain(&P.rval, nrows);
+    ws.plain(&P.rflag, nrows);
+    ws.plain(&P.rpos, nrows + 1);
+    if (int rc = ws.commit()) return rc;
     P.mk = (const u64*)d_key;
     P.mv = (const u64*)d_val;
     P.n = n;
@@ -5022,19 +4991,11 @@ static int la_run(dgx_lane* l, int fn, bool is_float, const uint64_t* d_key, con
     P.v_cap = v_cap;
     P.fn = fn;
     P.is_float = is_float;
-    P.bad = (int*)z;
-    P.words = (u64*)((char*)z + 16);
-    u32* ticket = (u32*)(P.words + VA_WORDS);
-    u64* status = (u64*)((char*)z + 64);
     P.err = l->d_err;
-    P.rval = (u64*)w;
-    P.rflag = P.rval + nrows;
-    P.rpos = P.rflag + nrows;
     P.out_key = (u64*)out_key;
     P.out_val = (u64*)out_val;
     P.out_cap = out_cap;
     P.out_len = (u64*)out_len;
-    static_assert(16 + VA_WORDS * sizeof(u64) + sizeof(u32) <= 64, "the aggregation's words fit their 64 bytes");
     la_check_kernel<<<gb_grid(std::max<uint64_t>(nrows + 1, n)), 256, 0, l->stream>>>(P);
     la_fold_kernel<<<gb_grid(32 * nrows), 256, 0, l->stream>>>(P);
     scan_u64_kernel<<<(unsigned)tr, EN_NT, 0, l->stream>>>(P.rflag, P.rpos, P.words + VA_W_R, nrows, status, ticket,
@@ -5101,13 +5062,16 @@ extern "C" int dgx_var_level_agg(int type, int fn, const uint64_t* key, const ui
         (rc = upload_list(l, src, nrows, &d_src)) || (rc = upload_list(l, v_off, nrows + 1, &d_v_off)) ||
         (rc = upload_list(l, v, M, &d_v)))
         return rc;
-    void* d_o;
-    if ((rc = l->ws.alloc((2 * nrows + 1) * sizeof(uint64_t), &d_o))) return rc;
-    uint64_t* o_len = (uint64_t*)d_o;
-    if ((rc = la_run(l, fn, type == DGX_VAL_FLOAT64, d_key, d_val, n, d_src, nrows, d_v_off, d_v, M, o_len + 1,
-                     o_len + 1 + nrows, nrows, o_len)))
+    uint64_t *o_len, *o_key, *o_val;
+    WsCarve o(l);
+    o.plain(&o_len, 1);
+    o.plain(&o_key, nrows);
+    o.plain(&o_val, nrows);
+    if ((rc = o.commit())) return rc;
+    if ((rc = la_run(l, fn, type == DGX_VAL_FLOAT64, d_key, d_val, n, d_src, nrows, d_v_off, d_v, M, o_key, o_val, nrows,
+                     o_len)))
         return rc;
-    return vv_finish(l, o_len, o_len + 1, o_len + 1 + nrows, out_key, out_val, out_cap, out_len);
+    return vv_finish(l, o_len, o_key, o_val, out_key, out_val, out_cap, out_len);
 }
 
 // ---------------------------------------------------------------------------
@@ -5244,31 +5208,25 @@ static int trigram_impl(dgx_lane* l, const TgPlan& T, const dgx_dev_pack* const*
     const uint64_t dcap = T.dcap;
     uint64_t rows_cap = 0;
     for (size_t i = 0; i < npacks; ++i) rows_cap += exact_len(packs[i]) + (mut_off[i + 1] - mut_off[i]);
-    // table (copied): [prog | drive | list_off];  then leaf, drive_off, row_off, rows
-    const size_t b_prog = (T.prog.size() * sizeof(TgOp) + 15) & ~size_t(15);
-    const size_t b_drive = (nd * sizeof(uint32_t) + 15) & ~size_t(15);
-    const size_t b_tab = b_prog + b_drive + (nlists + 1) * sizeof(uint64_t);
-    void *h_raw, *d_raw;
-    int rc = l->host.alloc(b_tab, &h_raw);
-    if (rc) return rc;
-    memcpy(h_raw, T.prog.data(), T.prog.size() * sizeof(TgOp));
-    memcpy((char*)h_raw + b_prog, T.drive.data(), nd * sizeof(uint32_t));
-    uint64_t* h_loff = (uint64_t*)((char*)h_raw + b_prog + b_drive);
+    TgParams P;
+    TgOp* h_prog;
+    uint32_t* h_drive;
+    uint64_t* h_loff;
+    u64 *row_off, *rows;
+    WsCarve ws(l);
+    ws.copied(&P.prog, &h_prog, T.prog.size());
+    ws.copied(&P.drive, &h_drive, nd);
+    ws.copied(&P.list_off, &h_loff, nlists + 1);
+    if (int rc = ws.stage()) return rc;
+    memcpy(h_prog, T.prog.data(), T.prog.size() * sizeof(TgOp));
+    memcpy(h_drive, T.drive.data(), nd * sizeof(uint32_t));
     if (nlists) memcpy(h_loff, list_off, (nlists + 1) * sizeof(uint64_t));
     else h_loff[0] = 0;
-    const size_t b_rest = nleaves * sizeof(TgLeaf) + (nd + 1 + npacks + 1 + rows_cap + 2) * sizeof(uint64_t);
-    if ((rc = l->ws.alloc(b_tab + b_rest, &d_raw))) return rc;
-    char* d = (char*)d_raw;
-    CK(cudaMemcpyAsync(d, h_raw, b_tab, cudaMemcpyHostToDevice, l->stream));
-    g_stats.h2d += b_tab;
-    TgParams P;
-    P.prog = (const TgOp*)d;
-    P.drive = (const u32*)(d + b_prog);
-    P.list_off = (const u64*)(d + b_prog + b_drive);
-    P.leaf = (TgLeaf*)(d + b_tab);
-    P.drive_off = (u64*)(P.leaf + nleaves);
-    u64* row_off = P.drive_off + nd + 1;
-    u64* rows = row_off + npacks + 1;
+    ws.plain(&P.leaf, nleaves);
+    ws.plain(&P.drive_off, nd + 1);
+    ws.plain(&row_off, npacks + 1);
+    ws.plain(&rows, rows_cap + 2);
+    if (int rc = ws.commit()) return rc;
     P.npacks = (u32)npacks;
     P.nleaves = (u32)nleaves;
     P.rows = rows;
@@ -5279,15 +5237,19 @@ static int trigram_impl(dgx_lane* l, const TgPlan& T, const dgx_dev_pack* const*
     P.ndrive = (u32)nd;
     P.dcap = dcap;
     P.err = l->d_err;
+    int rc;
     if (npacks && (rc = list_unfiltered_impl(l, packs, npacks, d_mut, d_flags, mut_off, after, first_keep(0),
                                              (uint64_t*)rows, rows_cap, (uint64_t*)row_off, nullptr)))
         return rc;
     const bool merge = nd >= 2;
     const bool gather_is_result = T.all_or && !merge;
-    void* p;
-    if (gather_is_result) P.gathered = (u64*)d_out;
-    else if ((rc = l->ws.alloc((dcap + 2) * sizeof(uint64_t), &p))) return rc;
-    else P.gathered = (u64*)p;
+    if (gather_is_result) {
+        P.gathered = (u64*)d_out;
+    } else {
+        WsCarve g(l);
+        g.plain(&P.gathered, dcap + 2);
+        if ((rc = g.commit())) return rc;
+    }
     P.len_word = gather_is_result ? (u64*)d_out_len : nullptr;
     const unsigned g_val = (unsigned)((dcap + 255) / 256);
     tg_leaves_kernel<<<1, TG_NT, 0, l->stream>>>(P);
@@ -5300,9 +5262,10 @@ static int trigram_impl(dgx_lane* l, const TgPlan& T, const dgx_dev_pack* const*
     if (merge) {
         uint64_t *m_out = d_out, *m_len = d_out_len;
         if (!T.all_or) {
-            if ((rc = l->ws.alloc((dcap + 2 + 8) * sizeof(uint64_t), &p))) return rc;
-            m_len = (uint64_t*)p;
-            m_out = m_len + 8;
+            WsCarve m(l);
+            m.plain(&m_len, 8);
+            m.plain(&m_out, dcap + 2);
+            if ((rc = m.commit())) return rc;
         }
         rc = merge_matrix_impl(l, (const uint64_t*)P.gathered, (const uint64_t*)P.drive_off, nd, dcap, m_out,
                                T.all_or ? out_cap : dcap, m_len);
@@ -5312,21 +5275,20 @@ static int trigram_impl(dgx_lane* l, const TgPlan& T, const dgx_dev_pack* const*
     }
     if (!T.all_or) {
         const uint64_t tiles = (dcap + CP_TILE - 1) / CP_TILE;
-        const size_t b_keep = (dcap + 15) & ~size_t(15), b_stat = tiles * sizeof(u64) + 64;
-        if ((rc = l->ws.alloc(b_keep + b_stat, &p))) return rc;
-        CK(cudaMemsetAsync((char*)p + b_keep, 0, b_stat, l->stream));
-        P.keep = (unsigned char*)p;
+        CompactParams C;
+        WsCarve k(l);
+        k.zeroed(&C.status, tiles);
+        k.zeroed(&C.ticket, 16);
+        k.plain(&P.keep, dcap);
+        if ((rc = k.commit())) return rc;
         tg_eval_kernel<<<g_val, 256, 0, l->stream>>>(P);
         CK(cudaGetLastError());
-        CompactParams C;
         C.v = P.cand;
         C.keep = P.keep;
         C.m = dcap;
         C.out = (u64*)d_out;
         C.out_cap = out_cap;
         C.out_len = (u64*)d_out_len;
-        C.status = (u64*)((char*)p + b_keep);
-        C.ticket = (u32*)(C.status + tiles);
         C.err = l->d_err;
         compact_kernel<<<(unsigned)tiles, CP_NT, 0, l->stream>>>(C);
         CK(cudaGetLastError());
