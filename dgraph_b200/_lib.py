@@ -75,6 +75,18 @@ class VarLevel(C.Structure):
                 ("nrows", C.c_size_t), ("v_cap", C.c_size_t), ("ndest", C.c_size_t)]
 
 
+class MathNode(C.Structure):
+    """dgx_math_node (include/dgx.h): one node of a math() program in post-order."""
+    _fields_ = [("op", C.c_uint8), ("const_tag", C.c_uint8), ("child", C.c_uint16 * 3), ("leaf", C.c_uint32),
+                ("const_word", C.c_uint64)]
+
+
+class MathLeaf(C.Structure):
+    """dgx_math_leaf (include/dgx.h): one variable's map, per-entry tags or one type, and the nil bit."""
+    _fields_ = [("key", C.c_void_p), ("word", C.c_void_p), ("tag", C.c_void_p), ("d_len", C.c_void_p),
+                ("n", C.c_size_t), ("type", C.c_int), ("nil", C.c_int)]
+
+
 class CacheStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("hits", "misses", "evictions", "bytes", "entries", "max_bytes")]
 
@@ -120,6 +132,7 @@ SYMBOLS = {
     "dgx_recurse_filter": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _szp]),
     "dgx_var_propagate": (_int, [_int, _vp, _vp, _sz, C.POINTER(VarLevel), _sz, _vp, _vp, _sz, _szp]),
     "dgx_var_level_agg": (_int, [_int, _int, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _szp]),
+    "dgx_math_eval": (_int, [C.POINTER(MathNode), _sz, C.POINTER(MathLeaf), _sz, _vp, _sz, _vp, _vp, _vp, _sz, _vp]),
     "dgx_path_create": (_int, [_u64, _u64, C.POINTER(_vp)]),
     "dgx_path_destroy": (None, [_vp]),
     "dgx_path_expand": (_int, [_vp, C.POINTER(PathLevel), _vp, _vp, _sz, C.POINTER(PathStats)]),
@@ -169,6 +182,8 @@ SYMBOLS = {
     "dgx_dev_recurse_filter": (_int, [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_var_propagate": (_int, [_vp, _int, _vp, _vp, _sz, C.POINTER(VarLevel), _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_var_level_agg": (_int, [_vp, _int, _int, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
+    "dgx_dev_math_eval": (_int, [_vp, C.POINTER(MathNode), _sz, C.POINTER(MathLeaf), _sz, _vp, _sz, _vp, _vp, _vp, _sz,
+                                 _vp]),
     "dgx_dev_path_expand": (_int, [_vp, _vp, C.POINTER(PathLevel), _sz, _sz, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_cascade": (_int, [_vp, C.POINTER(CascadeTree), C.POINTER(CascadeNode), _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),

@@ -756,6 +756,87 @@ def LevelAgg(fn: str, keys, vals, src, rows):
     return _val_out(VAL_FLOAT64 if fn == "avg" else typ, ok, ov, m.value)
 
 
+VAL_BOOL, VAL_NIL = 3, 4  # DGX_VAL_* of math() entries
+MATH_OPS = {"const": 0, "var": 1, "+": 2, "-": 3, "*": 4, "/": 5, "%": 6, "min": 7, "max": 8, "u-": 9, "sqrt": 10,
+            "floor": 11, "ceil": 12, "<": 13, ">": 14, "<=": 15, ">=": 16, "==": 17, "!=": 18, "cond": 19}
+MATH_KIND = {0: "none", 1: "map", 2: "const"}  # DGX_MATH_KIND_*
+
+
+def math_program(tree, names):
+    """A math() tree as a post-order list of _lib.MathNode.  tree: ("var", name), ("const", int or float) or
+    (op, child, ...) with op a key of MATH_OPS; names: leaf index of each variable name, filled in first-use order."""
+    nodes = []
+
+    def walk(t):
+        op = t[0]
+        if op not in MATH_OPS:
+            raise ValueError(f"unknown math op {op!r}")
+        kids = [walk(c) for c in t[1:]] if op not in ("var", "const") else []
+        n = _lib.MathNode()
+        n.op = MATH_OPS[op]
+        for i, c in enumerate(kids):
+            n.child[i] = c
+        if op == "var":
+            n.leaf = names.setdefault(t[1], len(names))
+        elif op == "const":
+            v = t[1]
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)):
+                raise TypeError(f"a math constant is an int or a float, not {v!r}")
+            is_f = isinstance(v, (float, np.floating))
+            n.const_tag = VAL_FLOAT64 if is_f else VAL_INT64
+            n.const_word = int(np.array([v], np.float64 if is_f else np.int64).view(np.uint64)[0])
+        nodes.append(n)
+        return len(nodes) - 1
+
+    walk(tree)
+    return nodes
+
+
+def math_leaf_arrays(m):
+    """(keys u64, words u64, tags u8 or None, type, nil) of one variable's map: None (no map), (keys, int64 or
+    float64 values) or (keys, u64 words, u8 tags)."""
+    if m is None:
+        return np.zeros(1, np.uint64), np.zeros(1, np.uint64), None, VAL_INT64, 1
+    if len(m) == 3:
+        k, w, t = _u64(m[0]), np.ascontiguousarray(m[1], np.uint64), np.ascontiguousarray(m[2], np.uint8)
+        if not (k.size == w.size == t.size):
+            raise ValueError("keys, words and tags of one size")
+        return k, w, t, VAL_INT64, 0
+    typ, k, w, _ = _val_map(m[0], m[1])
+    return k, w, None, typ, 0
+
+
+def EvalMath(tree, maps, range_uids=None):
+    """evalMathTree (query/math.go) and valueVarAggregation's math branch (query/query.go :1290-1361) in ONE call
+    (dgx_math_eval).  tree: see math_program; maps: variable name -> its map after transformTo (see
+    math_leaf_arrays); range_uids: SrcUIDs (DestUIDs at the root), or None.  Returns (kind, keys, words, tags): kind
+    "map", "const" or "none", words the 64-bit patterns of the values and tags their DGX_VAL_* types."""
+    names = {}
+    nodes = math_program(tree, names)
+    arrs = [None] * len(names)
+    for name, j in names.items():
+        arrs[j] = math_leaf_arrays(maps.get(name))
+    lv = (_lib.MathLeaf * max(len(arrs), 1))()
+    cap = 1
+    for j, (k, w, t, typ, nil) in enumerate(arrs):
+        n = 0 if nil else k.size
+        lv[j] = _lib.MathLeaf(k.ctypes.data, w.ctypes.data, t.ctypes.data if t is not None else None, None, n, typ,
+                              nil)
+        cap += n
+    r = None if range_uids is None else _u64(range_uids.Uids if isinstance(range_uids, List) else range_uids)
+    nr = 0 if r is None else r.size
+    cap = max(cap, nr, 1)
+    ok, ow, ot = np.empty(cap, np.uint64), np.empty(cap, np.uint64), np.empty(cap, np.uint8)
+    info = C.c_uint64(0)
+    rbuf = None if r is None else (r if r.size else np.zeros(1, np.uint64))
+    rp = None if rbuf is None else rbuf.ctypes.data
+    prog = (_lib.MathNode * len(nodes))(*nodes)
+    _lib.check(_lib.load().dgx_math_eval(prog, len(nodes), lv, len(arrs), rp, nr, _p(ok), _p(ow), _p(ot), cap,
+                                         C.byref(info)))
+    n = info.value & 0xFFFFFFFF
+    return MATH_KIND[(info.value >> 32) & 0xFF], ok[:n].copy(), ow[:n].copy(), ot[:n].copy()
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -44,6 +44,7 @@
 #include "cascade_kernel.cuh"
 #include "path_kernel.cuh"
 #include "valvar_kernel.cuh"
+#include "math_kernel.cuh"
 #include "wire.hpp"
 #include "ws_layout.hpp"
 
@@ -538,6 +539,10 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
             return fail(DGX_ERR_ARG, "a value-variable input is malformed (map keys, src or dest not strictly ascending, "
                                      "offsets not starting at 0, decreasing or past v_cap, or a row value missing from "
                                      "its level's dest)");
+        if (flag & kLaneErrMath)
+            return fail(DGX_ERR_ARG, "a math() input is refused (leaf keys or range not strictly ascending, an unknown "
+                                     "tag, a count word past its room, key 0 among other keys, or a result Go "
+                                     "returns as an error or computes in map-iteration order)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -5072,6 +5077,197 @@ extern "C" int dgx_var_level_agg(int type, int fn, const uint64_t* key, const ui
                      o_len)))
         return rc;
     return vv_finish(l, o_len, o_key, o_val, out_key, out_val, out_cap, out_len);
+}
+
+// ---------------------------------------------------------------------------
+// math() over value variables: evalMathTree and valueVarAggregation's math branch (math_kernel.cuh)
+// ---------------------------------------------------------------------------
+static_assert(sizeof(MtProg) == sizeof(dgx_math_node) && offsetof(dgx_math_node, const_word) == offsetof(MtProg, cword),
+              "the program is uploaded as it is");
+
+// The program's shape, checked on the host before anything is copied: known ops and constant tags, children earlier in
+// post-order and each node but the root the child of exactly one node (Go's tree), leaf indices in range.
+static int mt_check_args(const dgx_math_node* prog, size_t nn, const dgx_math_leaf* leaves, size_t nl, size_t nrange,
+                         bool device) {
+    if (!prog || (nl && !leaves)) return fail(DGX_ERR_ARG, "null argument");
+    if (nn == 0 || nn > DGX_MATH_MAX_NODES || nl > DGX_MATH_MAX_LEAVES)
+        return fail(DGX_ERR_ARG, "a math program has 1 to %d nodes and at most %d leaves", DGX_MATH_MAX_NODES,
+                    DGX_MATH_MAX_LEAVES);
+    if (nrange >= kVvMax) return fail(DGX_ERR_ARG, "range of 2^32 uids or more");
+    int used[DGX_MATH_MAX_NODES] = {0};
+    for (size_t i = 0; i < nn; ++i) {
+        const dgx_math_node& g = prog[i];
+        if (g.op > DGX_MATH_COND) return fail(DGX_ERR_ARG, "node %zu: unknown op %d", i, g.op);
+        if (g.op == DGX_MATH_CONST && g.const_tag != DGX_VAL_INT64 && g.const_tag != DGX_VAL_FLOAT64)
+            return fail(DGX_ERR_ARG, "node %zu: a constant is an int64 or a float64", i);
+        if (g.op == DGX_MATH_VAR && g.leaf >= nl) return fail(DGX_ERR_ARG, "node %zu: leaf %u of %zu", i, g.leaf, nl);
+        for (int c = 0; c < mt_arity(g.op); ++c) {
+            if (g.child[c] >= i) return fail(DGX_ERR_ARG, "node %zu: child %u is not earlier in post-order", i, g.child[c]);
+            used[g.child[c]] += 1;
+        }
+    }
+    for (size_t i = 0; i + 1 < nn; ++i)
+        if (used[i] != 1) return fail(DGX_ERR_ARG, "node %zu is the child of %d nodes: a program is a tree", i, used[i]);
+    uint64_t total = 0;
+    for (size_t j = 0; j < nl; ++j) {
+        const dgx_math_leaf& L = leaves[j];
+        if (!L.tag && L.type != DGX_VAL_INT64 && L.type != DGX_VAL_FLOAT64)
+            return fail(DGX_ERR_ARG, "leaf %zu: a leaf without tags has type DGX_VAL_INT64 or DGX_VAL_FLOAT64", j);
+        if (L.nil && (L.n || L.d_len)) return fail(DGX_ERR_ARG, "leaf %zu: a nil leaf has no entries", j);
+        if (!device && L.d_len) return fail(DGX_ERR_ARG, "leaf %zu: d_len belongs to the device form", j);
+        if (L.n >= kVvMax) return fail(DGX_ERR_ARG, "leaf %zu: 2^32 entries or more", j);
+        if (L.n && (!L.key || !L.word)) return fail(DGX_ERR_ARG, "leaf %zu: null argument", j);
+        total += L.n;
+    }
+    if (total > kMergeMatrixMax) return fail(DGX_ERR_ARG, "the leaves hold 2^32 entries or more");
+    return DGX_OK;
+}
+
+// 7 launches plus merge_matrix_impl's.  Workspace: the program, leaf table and room offsets copied; counts and words
+// zeroed; 42 bytes per unit of the leaves' total room (gathered keys, the union, root tag and word, flag, position)
+// plus the merge's own.  Leaves' arrays are device pointers; outputs get *info, and the entries unless refused or past
+// out_cap.
+static int mt_run(dgx_lane* l, const dgx_math_node* prog, size_t nn, const dgx_math_leaf* leaves, size_t nl,
+                  const uint64_t* d_range, size_t nrange, uint64_t* out_key, uint64_t* out_word, uint8_t* out_tag,
+                  uint64_t out_cap, uint64_t* info) {
+    uint64_t cap = 0;
+    for (size_t j = 0; j < nl; ++j) cap += leaves[j].n;
+    const uint64_t c1 = std::max<uint64_t>(cap, 1), tiles = scan_tiles(c1);
+    MtParams P{};
+    MtProg* h_prog;
+    MtLeaf* h_leaf;
+    u64 *h_cap_off, *status, *ulen;
+    u32* ticket;
+    WsCarve ws(l);
+    ws.copied((MtProg**)&P.prog, &h_prog, nn);
+    ws.copied((MtLeaf**)&P.leaf, &h_leaf, std::max<size_t>(nl, 1));
+    ws.copied((u64**)&P.cap_off, &h_cap_off, nl + 1);
+    ws.zeroed(&P.bad, 4);
+    ws.zeroed(&P.words, MT_WORDS);
+    ws.zeroed(&P.cnt, nn);
+    ws.zeroed(&P.nerr, nn);
+    ws.zeroed(&ticket, 4);
+    ws.zeroed(&status, tiles);
+    ws.plain(&P.plan, nn);
+    ws.plain(&P.llen, std::max<size_t>(nl, 1));
+    ws.plain(&P.row_off, nl + 1);
+    ws.plain(&ulen, 1);
+    ws.plain(&P.cat, c1);
+    ws.plain((u64**)&P.U, c1);
+    ws.plain(&P.rword, c1);
+    ws.plain(&P.flag, c1);
+    ws.plain(&P.pos, c1 + 1);
+    ws.plain(&P.rtag, c1);
+    if (int rc = ws.stage()) return rc;
+    std::memcpy(h_prog, prog, nn * sizeof(MtProg));
+    h_cap_off[0] = 0;
+    for (size_t j = 0; j < nl; ++j) {
+        const dgx_math_leaf& L = leaves[j];
+        h_leaf[j] = MtLeaf{(const u64*)L.key, (const u64*)L.word, L.tag, (const u64*)L.d_len, L.n, L.type, L.nil};
+        h_cap_off[j + 1] = h_cap_off[j] + L.n;
+    }
+    if (int rc = ws.commit()) return rc;
+    P.nn = (u32)nn;
+    P.nl = (u32)nl;
+    P.cap_total = cap;
+    P.range = (const u64*)d_range;
+    P.nrange = nrange;
+    P.ulen = ulen;
+    P.err = l->d_err;
+    P.out_key = (u64*)out_key;
+    P.out_word = (u64*)out_word;
+    P.out_tag = out_tag;
+    P.out_cap = out_cap;
+    P.info = (u64*)info;
+    mt_check_kernel<<<gb_grid(cap + (d_range ? nrange : 0)), 256, 0, l->stream>>>(P);
+    mt_plan_kernel<<<1, 32, 0, l->stream>>>(P);
+    mt_gather_kernel<<<gb_grid(cap), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 3);
+    if (int rc = merge_matrix_impl(l, (const uint64_t*)P.cat, (const uint64_t*)P.row_off, nl, cap, (uint64_t*)P.U, c1, (uint64_t*)ulen)) return rc;
+    mt_eval_kernel<<<gb_grid(cap), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)tiles, EN_NT, 0, l->stream>>>(P.flag, P.pos, ulen, c1, status, ticket, nullptr);
+    mt_finish_kernel<<<1, 32, 0, l->stream>>>(P);
+    mt_write_kernel<<<gb_grid(std::max<uint64_t>(cap, d_range ? nrange : 1)), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 4);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_math_eval(dgx_lane* l, const dgx_math_node* prog, size_t nnodes, const dgx_math_leaf* leaves,
+                                 size_t nleaves, const uint64_t* d_range, size_t nrange, uint64_t* d_out_key,
+                                 uint64_t* d_out_word, uint8_t* d_out_tag, size_t out_cap, uint64_t* d_info) {
+    if (!l || !d_info || (out_cap && (!d_out_key || !d_out_word || !d_out_tag)) || (d_range == nullptr && nrange))
+        return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = mt_check_args(prog, nnodes, leaves, nleaves, nrange, true)) return rc;
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    if (int rc = mt_run(l, prog, nnodes, leaves, nleaves, d_range, nrange, d_out_key, d_out_word, d_out_tag, out_cap,
+                        d_info))
+        return rc;
+    for (size_t j = 0; j < nleaves; ++j) g_stats.uids_in += leaves[j].n;
+    l->note_output(d_info, sizeof(uint64_t));
+    l->note_output(d_out_key, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_word, out_cap * sizeof(uint64_t));
+    l->note_output(d_out_tag, out_cap);
+    return DGX_OK;
+}
+
+extern "C" int dgx_math_eval(const dgx_math_node* prog, size_t nnodes, const dgx_math_leaf* leaves, size_t nleaves,
+                             const uint64_t* range, size_t nrange, uint64_t* out_key, uint64_t* out_word,
+                             uint8_t* out_tag, size_t out_cap, uint64_t* info) {
+    if (!info || (out_cap && (!out_key || !out_word || !out_tag)) || (range == nullptr && nrange))
+        return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = mt_check_args(prog, nnodes, leaves, nleaves, nrange, false)) return rc;
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    std::vector<dgx_math_leaf> D(leaves, leaves + nleaves);  // one copy of each array
+    int rc;
+    uint64_t cap = 0;
+    for (size_t j = 0; j < nleaves; ++j) {
+        dgx_math_leaf& L = D[j];
+        uint64_t *k, *w;
+        if ((rc = upload_list(l, L.key, L.n, &k)) || (rc = upload_list(l, L.word, L.n, &w))) return rc;
+        L.key = k;
+        L.word = w;
+        if (L.tag) {
+            void* t;
+            if ((rc = l->ws.alloc(L.n + 1, &t))) return rc;
+            if (L.n) CK(cudaMemcpyAsync(t, L.tag, L.n, cudaMemcpyHostToDevice, l->stream));
+            g_stats.h2d += L.n;
+            L.tag = (const uint8_t*)t;
+        }
+        g_stats.uids_in += L.n;
+        cap += L.n;
+    }
+    uint64_t* d_range = nullptr;
+    if (range && (rc = upload_list(l, range, nrange, &d_range))) return rc;
+    const uint64_t R = std::max<uint64_t>(cap + 1, range ? nrange : 1);  // room for any result
+    uint64_t *o_info, *o_key, *o_word;
+    uint8_t* o_tag;
+    WsCarve o(l);
+    o.plain(&o_info, 1);
+    o.plain(&o_key, R);
+    o.plain(&o_word, R);
+    o.plain(&o_tag, R);
+    if ((rc = o.commit())) return rc;
+    if ((rc = mt_run(l, prog, nnodes, D.data(), nleaves, d_range, nrange, o_key, o_word, o_tag, R, o_info))) return rc;
+    CK(cudaMemcpyAsync(l->h_word, o_info, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) return rc;
+    const uint64_t w = l->h_word[0], G = DGX_MATH_INFO_LEN(w);
+    *info = w;
+    if (G > out_cap) return fail(DGX_ERR_CAP, "%llu entries do not fit out_cap %zu", (unsigned long long)G, out_cap);
+    if (G) {
+        CK(cudaMemcpyAsync(out_key, o_key, G * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+        CK(cudaMemcpyAsync(out_word, o_word, G * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+        CK(cudaMemcpyAsync(out_tag, o_tag, G, cudaMemcpyDeviceToHost, l->stream));
+    }
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += G * 17;
+    g_stats.uids_out += G;
+    return DGX_OK;
 }
 
 // ---------------------------------------------------------------------------

@@ -797,3 +797,103 @@ func LevelAgg(typ, fn int, keys, words, src []uint64, matrix []*pb.List) (outKey
 	}
 	return outKeys[:int(n)], outWords[:int(n)], true
 }
+
+// dgxMinMath: below this many leaf entries (summed over a math() tree's variables) evalMathTree stays in Go.  No Go
+// comparison exists yet (the C18 record, profiles/h100_c18_math.json, times the library against a C restatement), and
+// every call pays the ShardedMap <-> sorted-array conversion on the host, so it is the dgxMinMergeMatrix bound.
+const dgxMinMath = dgxMinMergeMatrix
+
+// Math ops (DGX_MATH_*) and the extra entry tags of a math() map (DGX_VAL_*).
+const (
+	ValBool       = C.DGX_VAL_BOOL
+	ValNil        = C.DGX_VAL_NIL
+	MathKindNone  = C.DGX_MATH_KIND_NONE
+	MathKindMap   = C.DGX_MATH_KIND_MAP
+	MathKindConst = C.DGX_MATH_KIND_CONST
+)
+
+// MathNode is one node of a math() program in post-order (dgx_math_node): Op a DGX_MATH_* op, Child the indices of
+// its children (earlier nodes), Leaf the Leaves index of a DGX_MATH_VAR node, ConstTag / ConstWord a constant's
+// ValInt64 / ValFloat64 tag and bits.
+type MathNode struct {
+	Op, ConstTag uint8
+	Child        [3]uint16
+	Leaf         uint32
+	ConstWord    uint64
+}
+
+// MathLeaf is one variable's map after transformTo: ascending keys, one word and one DGX_VAL_* tag per key; Nil for
+// a variable with no map (a nil ShardedMap).
+type MathLeaf struct {
+	Keys, Words []uint64
+	Tags        []uint8
+	Nil         bool
+}
+
+// EvalMath runs evalMathTree (query/math.go) and valueVarAggregation's math branch (query/query.go:1290-1361) in one
+// call.  rangeOver is SrcUIDs (DestUIDs at the root), nil when Go's rangeOver is nil.  It returns the kind
+// (MathKindMap, MathKindConst, MathKindNone) and the entries, ascending.  ok == false, for a program outside the
+// library's bounds, below dgxMinMath entries, or on any library error (including a refusal where Go's answer is an
+// error or depends on map iteration order), means the caller keeps evalMathTree.
+func EvalMath(prog []MathNode, leaves []MathLeaf, rangeOver []uint64, hasRange bool) (kind int, keys, words []uint64,
+	tags []uint8, ok bool) {
+	if len(prog) == 0 || len(prog) > C.DGX_MATH_MAX_NODES || len(leaves) > C.DGX_MATH_MAX_LEAVES {
+		return 0, nil, nil, nil, false
+	}
+	total := 0
+	for _, l := range leaves {
+		if len(l.Keys) != len(l.Words) || len(l.Keys) != len(l.Tags) {
+			return 0, nil, nil, nil, false
+		}
+		total += len(l.Keys)
+	}
+	if total < dgxMinMath {
+		return 0, nil, nil, nil, false
+	}
+	cl := make([]C.dgx_math_leaf, max(len(leaves), 1))
+	var frees []func()
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+	}()
+	for j, l := range leaves {
+		pk, fk := cArray(l.Keys)
+		pw, fw := cArray(l.Words)
+		pt, ft := cArray(l.Tags)
+		frees = append(frees, fk, fw, ft)
+		n, isNil := len(l.Keys), C.int(0)
+		if l.Nil {
+			n, isNil = 0, 1
+		}
+		cl[j] = C.dgx_math_leaf{key: (*C.uint64_t)(pk), word: (*C.uint64_t)(pw), tag: (*C.uint8_t)(pt),
+			n: C.size_t(n), _type: C.DGX_VAL_INT64, nil: isNil}
+	}
+	cp := make([]C.dgx_math_node, len(prog))
+	for i, p := range prog {
+		cp[i] = C.dgx_math_node{op: C.uint8_t(p.Op), const_tag: C.uint8_t(p.ConstTag), leaf: C.uint32_t(p.Leaf),
+			const_word: C.uint64_t(p.ConstWord)}
+		for c := 0; c < 3; c++ {
+			cp[i].child[c] = C.uint16_t(p.Child[c])
+		}
+	}
+	pl, fl := cArray(cl)
+	pp, fp := cArray(cp)
+	frees = append(frees, fl, fp)
+	var pr *C.uint64_t
+	if hasRange {
+		r, fr := cArray(rangeOver)
+		frees = append(frees, fr)
+		pr = (*C.uint64_t)(r)
+	}
+	cap := max(total+1, len(rangeOver))
+	keys, words, tags = make([]uint64, cap), make([]uint64, cap), make([]uint8, cap)
+	var info C.uint64_t
+	if C.dgx_math_eval((*C.dgx_math_node)(pp), C.size_t(len(prog)), (*C.dgx_math_leaf)(pl), C.size_t(len(leaves)), pr,
+		C.size_t(len(rangeOver)), u64ptr(keys), u64ptr(words), (*C.uint8_t)(unsafe.Pointer(&tags[0])),
+		C.size_t(cap), &info) != C.DGX_OK {
+		return 0, nil, nil, nil, false
+	}
+	n := int(uint64(info) & 0xffffffff)
+	return int((uint64(info) >> 32) & 0xff), keys[:n], words[:n], tags[:n], true
+}

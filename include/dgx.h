@@ -516,6 +516,100 @@ int dgx_var_level_agg(int type, int fn, const uint64_t* key, const uint64_t* val
                       size_t nrows, const uint64_t* v_off, const uint64_t* v, uint64_t* out_key, uint64_t* out_val,
                       size_t out_cap, size_t* out_len);
 
+/* math() over value variables (query/math.go evalMathTree, with transformVars' leaf rule and valueVarAggregation's
+ * math branch, query/query.go :1239-1361).  Entries of a math() map carry a tag each: DGX_VAL_INT64, DGX_VAL_FLOAT64,
+ * DGX_VAL_BOOL (word 0 or 1, from comparisons) or DGX_VAL_NIL (Go's Val{}, from cond; word 0). */
+#define DGX_VAL_BOOL 3
+#define DGX_VAL_NIL 4
+/* Ops of a dgx_math_node: a leaf (CONST, VAR), binary (ADD .. MAX), unary (NEG .. CEIL), comparison (LT .. NE) and
+ * the ternary COND.  ln, exp, pow, logbase, since and dot are not offered: their Go results are not fixed by IEEE 754
+ * or depend on the clock or on vector types. */
+#define DGX_MATH_CONST 0
+#define DGX_MATH_VAR 1
+#define DGX_MATH_ADD 2
+#define DGX_MATH_SUB 3
+#define DGX_MATH_MUL 4
+#define DGX_MATH_DIV 5
+#define DGX_MATH_MOD 6
+#define DGX_MATH_MIN 7
+#define DGX_MATH_MAX 8
+#define DGX_MATH_NEG 9
+#define DGX_MATH_SQRT 10
+#define DGX_MATH_FLOOR 11
+#define DGX_MATH_CEIL 12
+#define DGX_MATH_LT 13
+#define DGX_MATH_GT 14
+#define DGX_MATH_LE 15
+#define DGX_MATH_GE 16
+#define DGX_MATH_EQ 17
+#define DGX_MATH_NE 18
+#define DGX_MATH_COND 19
+/* A program holds at most DGX_MATH_MAX_NODES nodes and DGX_MATH_MAX_LEAVES leaves: the evaluation keeps one tag and
+ * one word per node for every key in thread-local storage and the node table in shared memory, and the leaves are the
+ * rows of one key-union merge.  math() expressions in queries have a handful of nodes; a larger one stays in Go. */
+#define DGX_MATH_MAX_NODES 64
+#define DGX_MATH_MAX_LEAVES 16
+/* One node; nodes are in post-order (children before parents, the root last).  child[0 .. arity) index earlier nodes
+ * (arity 2 for binary and comparison ops, 1 for unary, 3 for COND, 0 for leaves).  VAR reads leaves[leaf]; several VAR
+ * nodes may share a leaf.  CONST is the literal (const_tag DGX_VAL_INT64 or DGX_VAL_FLOAT64, const_word its word). */
+typedef struct {
+    uint8_t op;
+    uint8_t const_tag;
+    uint16_t child[3];
+    uint32_t leaf;
+    uint64_t const_word;
+} dgx_math_node;
+/* One variable's map after transformTo: key[0 .. n) strictly ascending, word[n], and either tag[n] (one DGX_VAL_* per
+ * entry, a previous math() output) or tag NULL and every entry of type `type` (DGX_VAL_INT64 or DGX_VAL_FLOAT64, a
+ * dgx_var_propagate output).  nil = 1 is a variable with no map at all (Go's nil ShardedMap), which cond tells apart
+ * from an empty one; a nil leaf has no entries.  Host form: n is the entry count.  Device form: n is the room of the
+ * arrays and d_len, when not NULL, one device uint64 whose low 32 bits hold the entry count (at most n), so the
+ * d_out_len of dgx_dev_var_propagate or dgx_dev_var_level_agg, or the info word of a previous dgx_dev_math_eval, feeds
+ * a leaf without a host read. */
+typedef struct {
+    const uint64_t* key;
+    const uint64_t* word;
+    const uint8_t* tag;
+    const uint64_t* d_len;
+    size_t n;
+    int type;
+    int nil;
+} dgx_math_leaf;
+/* The info word of a result: its length (low 32 bits), its kind (bits 32-39) and the set of tags in it (bits 40-47,
+ * bit 1 << t for DGX_VAL_ t).  MAP: a non-empty map, Go's UidToVal.  CONST: a constant set for every uid of the range
+ * (or on uid 0 when there is no range).  NONE: no map and no constant; Go assigns nothing. */
+#define DGX_MATH_KIND_NONE 0
+#define DGX_MATH_KIND_MAP 1
+#define DGX_MATH_KIND_CONST 2
+#define DGX_MATH_INFO_LEN(w) ((uint64_t)(w) & 0xffffffffull)
+#define DGX_MATH_INFO_KIND(w) ((int)(((uint64_t)(w) >> 32) & 0xff))
+#define DGX_MATH_INFO_TAGS(w) ((unsigned)(((uint64_t)(w) >> 40) & 0xff))
+/* evalMathTree over prog[0 .. nnodes) and valueVarAggregation's math branch: the result map into out_key / out_word /
+ * out_tag (ascending keys) and *info.  Go's rules, bit for bit: a leaf {MaxUint64: v} is the constant v; at a binary
+ * node a child {0: v} becomes a constant (the left child first, the right only when the left did not); a binary node
+ * over maps ranges over the union of their keys, a missing entry or a nil value being int64 0, and drops a key whose
+ * operation fails; int op float converts the int; int + - * / overflow and division by zero fail; / and % by zero
+ * fail; MinInt64 / -1 is MinInt64 and MinInt64 % -1 is 0; float % is math.Mod; min / max take the left operand unless
+ * it is less (a NaN makes min take the right, max the left); u- MinInt64, sqrt of a negative value fail; sqrt of an int
+ * is a float, floor / ceil of an int the int; Value()'s clamp (+Inf -> MaxFloat64, -Inf -> -MaxFloat64, NaN -> +0.0)
+ * follows every binary and unary result.  A comparison ranges over its left child's keys, a missing right entry being
+ * nil; ints meet floats as floats, nil compared with nil is neither ordered nor equal.  cond ranges over its first
+ * child's keys, and a missing branch entry is stored as a nil value.  At the top a map holding both ints and floats
+ * has its ints converted to float; a constant is set on every uid of range (range NULL: on uid 0, nrange ignored).
+ * out_cap >= the sum of the leaves' n plus 1, and >= nrange, always suffices; a longer result is DGX_ERR_CAP with
+ * *info set and nothing written.
+ * DGX_ERR_ARG before anything is copied: a malformed program (an unknown op or constant tag, a child not earlier in
+ * post-order, a leaf index out of range, more than DGX_MATH_MAX_NODES nodes or DGX_MATH_MAX_LEAVES leaves), a leaf's
+ * unknown type, a nil leaf with entries, sizes of 2^32 or more, a null array that is needed.
+ * DGX_ERR_ARG after the kernels, with nothing written, where Go's answer is an error or depends on map iteration order:
+ * evalMathTree failing (an operation on two constants or a unary one on a constant failing, cond over a constant or a
+ * nil map), a unary, comparison or cond node failing on some but not all of more than one key, a leaf holding key 0
+ * with other keys, leaf keys or range not strictly ascending, an unknown entry tag.
+ * Launches: 7 plus the key-union merge's (DESIGN section 3.14), whatever the tree and map sizes. */
+int dgx_math_eval(const dgx_math_node* prog, size_t nnodes, const dgx_math_leaf* leaves, size_t nleaves,
+                  const uint64_t* range, size_t nrange, uint64_t* out_key, uint64_t* out_word, uint8_t* out_tag,
+                  size_t out_cap, uint64_t* info);
+
 /* @cascade over a forest of subgraph nodes (query/query.go populateVarMap :1445-1527, updateUidMatrix :1425-1439
  * without facets, and ProcessQuery's root pagination :3004-3011), in pre-order: parent[n] is UINT32_MAX for a query root
  * and below n otherwise.  flags[n] is a set of DGX_CASCADE_* bits resolved on the host; first[n] / offset[n] are
@@ -819,6 +913,14 @@ int dgx_dev_var_level_agg(dgx_lane* lane, int type, int fn, const uint64_t* d_ke
                           const uint64_t* d_src, size_t nrows, const uint64_t* d_v_off, const uint64_t* d_v,
                           size_t v_cap, uint64_t* d_out_key, uint64_t* d_out_val, size_t out_cap,
                           uint64_t* d_out_len);
+/* Device form of dgx_math_eval: prog and leaves are host arrays, every array a leaf points to, d_range and the outputs
+ * are device memory.  A leaf's entry count is *d_len when d_len is set (n its room), n otherwise; nrange is an exact
+ * host size.  d_info is one device uint64.  Argument errors are DGX_ERR_ARG at the call, as in the host form; order,
+ * tags, the count words and Go's errors are checked on the device: a refused call writes nothing (DGX_ERR_ARG at the
+ * next dgx_lane_sync), a result longer than out_cap writes only *d_info (DGX_ERR_CAP).  Asynchronous on the lane. */
+int dgx_dev_math_eval(dgx_lane* lane, const dgx_math_node* prog, size_t nnodes, const dgx_math_leaf* leaves,
+                      size_t nleaves, const uint64_t* d_range, size_t nrange, uint64_t* d_out_key,
+                      uint64_t* d_out_word, uint8_t* d_out_tag, size_t out_cap, uint64_t* d_info);
 /* One node of dgx_dev_cascade, every pointer in device memory: its rows v[v_off[i] .. v_off[i+1]) (v_off has nrows + 1
  * values, v_off[0] == 0, v_off[nrows] <= v_cap, the room of v), its dest (ndest values) and its has_val (nhas bytes). */
 typedef struct dgx_cascade_node {

@@ -542,6 +542,54 @@ inline ValueMap LevelAgg(int fn, const ValueMap& m, const std::vector<uint64_t>&
     return out;
 }
 
+// A math() leaf or result: strictly ascending keys, one 64-bit word and one DGX_VAL_* tag per key.  nil is a variable
+// with no map at all (Go's nil ShardedMap), which cond tells apart from an empty one.
+struct MathMap {
+    std::vector<uint64_t> keys, words;
+    std::vector<uint8_t> tags;
+    bool nil = false;
+};
+
+// The result of EvalMath: kind DGX_MATH_KIND_MAP (the map), DGX_MATH_KIND_CONST (the constant set on every uid of the
+// range, or on uid 0 without one) or DGX_MATH_KIND_NONE (Go assigns nothing).
+struct MathResult {
+    int kind = DGX_MATH_KIND_NONE;
+    MathMap map;
+};
+
+// evalMathTree (query/math.go) and valueVarAggregation's math branch (query/query.go:1290-1361) in one dgx_math_eval
+// call: prog in post-order, leaves indexed by its VAR nodes, range SrcUIDs (DestUIDs at the root) or null.
+inline MathResult EvalMath(const std::vector<dgx_math_node>& prog, const std::vector<MathMap>& leaves,
+                           const std::vector<uint64_t>* range) {
+    std::vector<dgx_math_leaf> lv(leaves.size());
+    size_t cap = 1;
+    for (size_t j = 0; j < leaves.size(); ++j) {
+        const MathMap& m = leaves[j];
+        if (m.keys.size() != m.words.size() || m.keys.size() != m.tags.size())
+            throw Error(DGX_ERR_ARG, "one word and one tag per key");
+        const size_t n = m.nil ? 0 : m.keys.size();
+        lv[j] = dgx_math_leaf{m.keys.data(), m.words.data(), m.tags.data(), nullptr, n, DGX_VAL_INT64, m.nil ? 1 : 0};
+        cap += n;
+    }
+    const size_t nr = range ? range->size() : 0;
+    cap = std::max(cap, nr);
+    MathResult out;
+    out.map.keys.assign(cap, 0);
+    out.map.words.assign(cap, 0);
+    out.map.tags.assign(cap, 0);
+    uint64_t info = 0;
+    static const uint64_t kNoUid = 0;
+    check(dgx_math_eval(prog.data(), prog.size(), lv.data(), lv.size(),
+                        range ? (nr ? range->data() : &kNoUid) : nullptr, nr, out.map.keys.data(),
+                        out.map.words.data(), out.map.tags.data(), cap, &info));
+    const size_t n = DGX_MATH_INFO_LEN(info);
+    out.kind = DGX_MATH_INFO_KIND(info);
+    out.map.keys.resize(n);
+    out.map.words.resize(n);
+    out.map.tags.resize(n);
+    return out;
+}
+
 }  // namespace algo
 
 // Wire-format adjacency (dgx_wire_*, host only): the bytes proto.Unmarshal sees at posting/list.go:1045 and

@@ -143,6 +143,7 @@ def main():
     ap.add_argument("--c15-only", action="store_true", help="only the C15 @cascade rows")
     ap.add_argument("--c16-only", action="store_true", help="only the C16 shortest() rows")
     ap.add_argument("--c17-only", action="store_true", help="only the C17 value-variable rows")
+    ap.add_argument("--c18-only", action="store_true", help="only the C18 math() rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -168,9 +169,11 @@ def main():
         rows = c16_rows(Lane())
     elif args.c17_only:
         rows = c17_rows(Lane())
+    elif args.c18_only:
+        rows = c18_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1769,6 +1772,98 @@ def c17_rows(L):
                              "max_in_degree": indeg if name == "C17b" else None, "check": bool(ok), "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del dk, dv, dlv, ok_t, ov_t
+    return out_rows
+
+
+def c18_rows(L):
+    """C18 "math() over value variables".  C18a: math(p * 2 + a / s) over a float map p of 1.78e7 keys (C17a's row
+    values as a map size), an int age map a over half as many keys and s a {0: v} aggregate.  C18b: a 25-node tree of
+    arithmetic, comparisons and cond over three maps sharing 1e7 keys (shared keys: no comparison meets a missing
+    entry, so nothing is refused).  C18c: TestMathCeil2's size, a handful of keys (launch-bound).  Legs: (1) the device
+    form on resident inputs (CUDA events), (2) the host form (wall clock), (3) the line-by-line restatement
+    (tests/math_oracle.c) on 1 thread -- C, not Go.  Every leg is checked against the restatement in keys, words and
+    tags."""
+    import math_oracle as mo
+    from dgraph_b200 import algo
+
+    lib = L.lib
+    rng = np.random.default_rng(18)
+    U64 = np.uint64
+
+    def dp(t):
+        return t.data_ptr()
+
+    def up(x):
+        x = np.concatenate([np.ascontiguousarray(x, U64), np.zeros(1, U64)])
+        return torch.from_numpy(x.view(np.int64)).to(DEV)
+
+    def keys(n, span):
+        return np.sort(rng.choice(np.arange(1, span, dtype=U64), n, replace=False))
+
+    na = 17_800_000
+    pk, ak = keys(na, 3 * na), keys(na // 2, 3 * na)
+    c18a = ({"p": (pk, rng.random(na) * 100), "a": (ak, rng.integers(1, 90, ak.size)),
+             "s": (np.zeros(1, U64), np.array([3.0]))},
+            ("+", ("*", ("var", "p"), ("const", 2)), ("/", ("var", "a"), ("var", "s"))))
+    nb = 10_000_000
+    kb = keys(nb, 2 * nb)
+    x, y, z = ("var", "x"), ("var", "y"), ("var", "z")
+    tb = ("cond", ("<", ("+", x, ("*", y, ("const", 0.5))), ("-", z, ("const", 3))),
+          ("max", ("floor", ("/", x, ("const", 7))), ("sqrt", ("+", y, ("const", 1)))),
+          ("cond", (">=", z, x), ("min", ("%", x, ("const", 13)), y), ("u-", z)))
+    c18b = ({"x": (kb, rng.integers(0, 1000, nb)), "y": (kb, rng.random(nb) * 500), "z": (kb, rng.integers(0, 1000, nb))},
+            tb)
+    kc = np.array([1, 23, 24, 25, 31], U64)
+    c18c = ({"a": (kc, np.array([38, 15, 15, 17, 19], np.int64))}, ("ceil", ("/", ("var", "a"), ("const", 2.5))))
+    out_rows = []
+    for name, (maps, tree) in (("C18a", c18a), ("C18b", c18b), ("C18c", c18c)):
+        t0 = time.perf_counter()
+        want = mo.evaluate(tree, maps)
+        t_or = (time.perf_counter() - t0) * 1e3
+        assert want[0] == "map" and not want[4]
+        names = {}
+        prog = algo.math_program(tree, names)
+        leaves = [None] * len(names)
+        for nm, j in names.items():
+            leaves[j] = algo.math_leaf_arrays(maps[nm])
+        cap = 1 + sum(k.size for k, *_ in leaves)
+        nodes = (_lib.MathNode * len(prog))(*prog)
+        # (1) device form, inputs and outputs resident
+        dleaf = [(up(k), up(w)) for k, w, *_ in leaves]
+        arr = (_lib.MathLeaf * len(leaves))()
+        for j, ((k, w, t, typ, nil), (dk, dw)) in enumerate(zip(leaves, dleaf)):
+            arr[j] = _lib.MathLeaf(dp(dk), dp(dw), None, None, k.size, typ, nil)
+        ok_t, ow_t = (torch.empty(cap, dtype=torch.int64, device=DEV) for _ in range(2))
+        ot_t = torch.empty(cap, dtype=torch.uint8, device=DEV)
+        di = torch.empty(1, dtype=torch.int64, device=DEV)
+
+        def dev():
+            _lib.check(lib.dgx_dev_math_eval(L.h, nodes, len(prog), arr, len(leaves), None, 0, dp(ok_t), dp(ow_t),
+                                             dp(ot_t), cap, dp(di)))
+        ms_dev, _ = timeit(dev, warm=2, reps=10)
+        L.sync()
+        n = int(di.cpu().numpy()[0]) & 0xFFFFFFFF
+        ok_dev = (n == want[1].size and np.array_equal(ok_t[:n].cpu().numpy().view(U64), want[1]) and
+                  np.array_equal(ow_t[:n].cpu().numpy().view(U64), want[2]) and
+                  np.array_equal(ot_t[:n].cpu().numpy(), want[3]))
+        # (2) host form
+        algo.EvalMath(tree, maps)
+        ts = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            got = algo.EvalMath(tree, maps)
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ok_host = got[0] == want[0] and all(np.array_equal(a, b) for a, b in zip(got[1:], want[1:4]))
+        full = (f"{name}: {len(prog)} nodes over {len(leaves)} maps of {', '.join(str(k.size) for k, *_ in leaves)} "
+                f"keys; result {want[1].size} entries")
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev, "CUDA events, median of 10 after 2 warm"),
+                                    ("host form", float(np.median(ts)), ok_host, "wall clock, median of 3 after 1 warm"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, True, "orc_math, wall clock, one run; "
+                                     "the reference the other legs are checked against")):
+            out_rows.append({"op": "EvalMath", "workload": name, "leg": leg, "config": full, "ms": round(ms, 4),
+                             "keys": int(cap - 1), "check": bool(ok), "timing": timing})
+            print(json.dumps(out_rows[-1]), flush=True)
+        del dleaf, ok_t, ow_t, ot_t
     return out_rows
 
 
