@@ -802,8 +802,8 @@ def math_leaf_arrays(m):
         if not (k.size == w.size == t.size):
             raise ValueError("keys, words and tags of one size")
         return k, w, t, VAL_INT64, 0
-    typ, k, w, _ = _val_map(m[0], m[1])
-    return k, w, None, typ, 0
+    typ, k, w, n = _val_map(m[0], m[1])
+    return k[:n], w[:n], None, typ, 0  # an empty map has no entries (not the one zero key _val_map pads it with)
 
 
 def EvalMath(tree, maps, range_uids=None):
