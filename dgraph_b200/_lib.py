@@ -87,6 +87,17 @@ class MathLeaf(C.Structure):
                 ("n", C.c_size_t), ("type", C.c_int), ("nil", C.c_int)]
 
 
+class SgFilterTree(C.Structure):
+    """dgx_sg_filter_tree (include/dgx.h): a subgraph's @filter tree, node 0 the root, parents below their children."""
+    _fields_ = [("nnodes", C.c_size_t), ("op", C.c_void_p), ("parent", C.c_void_p), ("leaf", C.c_void_p)]
+
+
+class SgFilterLeaf(C.Structure):
+    """dgx_sg_filter_leaf (include/dgx.h): a LIST leaf's uids, or a COUNT leaf's counts / offsets and comparison."""
+    _fields_ = [("kind", C.c_int), ("cmp", C.c_int), ("threshold", C.c_int64), ("uids", C.c_void_p), ("n", C.c_size_t),
+                ("d_len", C.c_void_p), ("counts", C.c_void_p), ("off", C.c_void_p)]
+
+
 class CacheStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("hits", "misses", "evictions", "bytes", "entries", "max_bytes")]
 
@@ -138,6 +149,8 @@ SYMBOLS = {
     "dgx_path_expand": (_int, [_vp, C.POINTER(PathLevel), _vp, _vp, _sz, C.POINTER(PathStats)]),
     "dgx_path_result": (_int, [_vp, _vp, _vp, _sz, _szp]),
     "dgx_cascade": (_int, [C.POINTER(CascadeTree), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _sz]),
+    "dgx_sg_filter": (_int, [C.POINTER(SgFilterTree), C.POINTER(SgFilterLeaf), _sz, _vp, _sz, _vp, _vp, _sz, C.c_int32,
+                             C.c_int32, _vp, _sz, _szp, _vp, _vp, _sz, _vp]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
     "dgx_encode_bound": (None, [_sz, C.c_uint32, _szp, _szp]),
@@ -186,6 +199,8 @@ SYMBOLS = {
                                  _vp]),
     "dgx_dev_path_expand": (_int, [_vp, _vp, C.POINTER(PathLevel), _sz, _sz, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_cascade": (_int, [_vp, C.POINTER(CascadeTree), C.POINTER(CascadeNode), _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
+    "dgx_dev_sg_filter": (_int, [_vp, C.POINTER(SgFilterTree), C.POINTER(SgFilterLeaf), _sz, _vp, _sz, _vp, _vp, _vp,
+                                 _sz, _sz, C.c_int32, C.c_int32, _vp, _sz, _vp, _vp, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),
     "dgx_filter_tail_queries": (_u64, [_vp]),

@@ -516,6 +516,87 @@ def Cascade(nodes):
     return rows, [List(d) for d in dests]
 
 
+SGF_OPS = {"and": 1, "or": 2, "not": 3}   # DGX_SGF_AND / _OR / _NOT; DGX_SGF_LEAF is 0
+SGF_CMP = {"le": 0, "ge": 1, "lt": 2, "gt": 3, "eq": 4}  # DGX_SGF_CMP_*
+
+
+def sg_filter_flat(tree) -> dict:
+    """The flat dgx_sg_filter_tree arrays of a nested filter tree: an int is a leaf index, ("and" | "or", [children])
+    an op and ("not", child) a negation.  Nodes are numbered in pre-order, so node 0 is the root and every parent lies
+    below its children."""
+    op, parent, leaf = [], [], []
+
+    def walk(t, p):
+        k = len(op)
+        parent.append(p)
+        if isinstance(t, (int, np.integer)):
+            op.append(0)
+            leaf.append(int(t))
+            return
+        op.append(SGF_OPS[t[0]])
+        leaf.append(0)
+        for c in ([t[1]] if t[0] == "not" else t[1]):
+            walk(c, k)
+
+    walk(tree, 0xFFFFFFFF)
+    return {"nnodes": len(op), "op": np.array(op, np.uint8), "parent": np.array(parent, np.uint32),
+            "leaf": np.array(leaf, np.uint32)}
+
+
+def sg_filter_tree(f) -> "_lib.SgFilterTree":
+    """The dgx_sg_filter_tree over the arrays of sg_filter_flat (which must outlive it)."""
+    return _lib.SgFilterTree(f["nnodes"], f["op"].ctypes.data, f["parent"].ctypes.data, f["leaf"].ctypes.data)
+
+
+def sg_filter_leaf_arrays(leaves, n0: int):
+    """Host arrays of the leaves: ("list", uids), ("count", cmp, threshold, counts) with one uint32 count per D0 value,
+    or ("len", cmp, threshold, off) with D0's n0 + 1 row offsets.  Returns (kept arrays, dgx_sg_filter_leaf table).
+    Raises ValueError when a COUNT leaf's array does not match n0: the library copies exactly that many entries."""
+    keep, descs = [], []
+    for lf in leaves:
+        if lf[0] == "list":
+            u = _u64(lf[1].Uids if isinstance(lf[1], List) else lf[1])
+            keep.append(u)
+            descs.append(_lib.SgFilterLeaf(0, 0, 0, u.ctypes.data if u.size else None, u.size, None, None, None))
+        else:
+            a = np.ascontiguousarray(np.asarray(lf[3], np.uint32 if lf[0] == "count" else np.uint64))
+            want = n0 if lf[0] == "count" else n0 + 1
+            if a.size != want:
+                raise ValueError(f"a {lf[0]!r} leaf holds {a.size} entries for {n0} D0 values: {want} expected")
+            if a.size == 0:
+                a = np.zeros(1, a.dtype)
+            keep.append(a)
+            descs.append(_lib.SgFilterLeaf(1, SGF_CMP[lf[1]], int(lf[2]), None, 0, None,
+                                           a.ctypes.data if lf[0] == "count" else None,
+                                           a.ctypes.data if lf[0] == "len" else None))
+    return keep, (_lib.SgFilterLeaf * max(len(descs), 1))(*descs)
+
+
+def SubgraphFilter(tree, leaves, d0, rows, count: int = 0, offset: int = 0, counts_only: bool = False):
+    """A subgraph's @filter and first / offset (query/query.go ProcessGraph's filter block, applyPagination and the
+    DoCount block) in ONE call (dgx_sg_filter).
+
+    tree: the filter tree as sg_filter_flat takes it; leaves: as sg_filter_leaf_arrays takes them; d0: DestUIDs from
+    processTask; rows: the uid matrix (strictly ascending rows).  Returns (rows, counts, dest): the filtered and paged
+    rows (None in counts-only mode), counts[i] = len(row i) and the new DestUIDs as a List."""
+    f = sg_filter_flat(tree)
+    d0a = _u64(d0.Uids if isinstance(d0, List) else d0)
+    keep, tab = sg_filter_leaf_arrays(leaves, d0a.size)
+    v, v_off = _csr_u64(rows)
+    nrows, m = len(rows), int(v_off[-1])
+    dest = np.empty(max(d0a.size, 1), np.uint64)
+    out = None if counts_only else np.empty(max(m, 1), np.uint64)
+    out_off = np.zeros(nrows + 1, np.uint64)
+    counts = np.zeros(max(nrows, 1), np.uint32)
+    n = C.c_size_t(0)
+    t = sg_filter_tree(f)
+    _lib.check(_lib.load().dgx_sg_filter(C.byref(t), tab, len(leaves), _p(d0a), d0a.size, _p(v), _p(v_off), nrows,
+                                         count, offset, _p(dest), d0a.size, C.byref(n),
+                                         None if counts_only else _p(out), _p(out_off), m, _p(counts)))
+    res = None if counts_only else [out[int(out_off[i]):int(out_off[i + 1])].copy() for i in range(nrows)]
+    return res, counts[:nrows].copy(), List(dest[: n.value].copy())
+
+
 class ReachSet:
     """The edges one sg.Attr has taken during one @recurse (query/recurse.go expandRecurse's reachMap, loop: false),
     kept in device memory (dgx_reach_set).  One set per distinct Attr, for the life of one recursion."""

@@ -45,6 +45,7 @@
 #include "path_kernel.cuh"
 #include "valvar_kernel.cuh"
 #include "math_kernel.cuh"
+#include "sg_filter_kernel.cuh"
 #include "wire.hpp"
 #include "ws_layout.hpp"
 
@@ -543,6 +544,10 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
             return fail(DGX_ERR_ARG, "a math() input is refused (leaf keys or range not strictly ascending, an unknown "
                                      "tag, a count word past its room, key 0 among other keys, or a result Go "
                                      "returns as an error or computes in map-iteration order)");
+        if (flag & kLaneErrSgFilter)
+            return fail(DGX_ERR_ARG, "an @filter input is malformed (d0, a row or a LIST leaf not strictly ascending, "
+                                     "a COUNT leaf's offsets or the row offsets decreasing, row offsets not starting "
+                                     "at 0 or past v_cap, or a length word past its room)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -4371,6 +4376,323 @@ extern "C" int dgx_cascade(const dgx_cascade_tree* tree, const uint64_t* v, cons
     CK(cudaStreamSynchronize(l->stream));
     g_stats.d2h += (K + DN + rows + n + 4) * sizeof(uint64_t);
     g_stats.uids_out += K + DN;
+    return DGX_OK;
+}
+
+// ---------------------------------------------------------------------------
+// @filter and first / offset: a subgraph's filter tree over its uid matrix in one call (sg_filter_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr uint64_t kSfMax = uint64_t(1) << 32;  // |D0|, rows, values and list lengths are 32-bit counts
+
+// The checks of the tree and the leaves, and the tree's pre-order program.
+static int sf_check_args(const dgx_sg_filter_tree* t, const dgx_sg_filter_leaf* leaves, size_t nleaves, bool dev,
+                         std::vector<SfOp>* prog) {
+    if (!t) return fail(DGX_ERR_ARG, "null tree");
+    const size_t n = t->nnodes;
+    if (n == 0 || n > DGX_SGF_MAX_NODES) return fail(DGX_ERR_ARG, "%zu nodes: 1 to %d", n, DGX_SGF_MAX_NODES);
+    if (!t->op || !t->parent || !t->leaf) return fail(DGX_ERR_ARG, "null tree array");
+    if (nleaves > DGX_SGF_MAX_LEAVES) return fail(DGX_ERR_ARG, "%zu leaves: at most %d", nleaves, DGX_SGF_MAX_LEAVES);
+    if (nleaves && !leaves) return fail(DGX_ERR_ARG, "null leaves");
+    for (size_t j = 0; j < nleaves; ++j) {
+        const dgx_sg_filter_leaf& L = leaves[j];
+        if (L.kind == DGX_SGF_LIST) {
+            if (L.n >= kSfMax) return fail(DGX_ERR_ARG, "leaf %zu: %zu uids, at most 2^32 - 1", j, L.n);
+            if (L.n && !L.uids) return fail(DGX_ERR_ARG, "leaf %zu: null uids", j);
+            if (L.d_len && !dev) return fail(DGX_ERR_ARG, "leaf %zu: a length word in the host form", j);
+        } else if (L.kind == DGX_SGF_COUNT) {
+            if (L.cmp < DGX_SGF_CMP_LE || L.cmp > DGX_SGF_CMP_EQ) return fail(DGX_ERR_ARG, "leaf %zu: cmp %d", j, L.cmp);
+            if (!L.counts == !L.off) return fail(DGX_ERR_ARG, "leaf %zu: not exactly one of counts and off", j);
+        } else {
+            return fail(DGX_ERR_ARG, "leaf %zu: unknown kind %d", j, L.kind);
+        }
+    }
+    std::vector<std::vector<uint32_t>> kids(n);
+    std::vector<uint32_t> depth(n, 0);
+    for (size_t k = 0; k < n; ++k) {
+        const uint8_t op = t->op[k];
+        if (op > DGX_SGF_NOT) return fail(DGX_ERR_ARG, "node %zu: unknown op %u", k, (unsigned)op);
+        if (op == DGX_SGF_LEAF && t->leaf[k] >= nleaves)
+            return fail(DGX_ERR_ARG, "node %zu: leaf %u past %zu leaves", k, t->leaf[k], nleaves);
+        if (k == 0) continue;
+        const uint32_t p = t->parent[k];
+        if (p >= k) return fail(DGX_ERR_ARG, "node %zu: parent %u is not below it", k, p);
+        if (t->op[p] == DGX_SGF_LEAF) return fail(DGX_ERR_ARG, "node %zu: its parent %u is a leaf", k, p);
+        depth[k] = depth[p] + 1;
+        if (depth[k] > DGX_SGF_MAX_DEPTH) return fail(DGX_ERR_ARG, "node %zu is deeper than %d", k, DGX_SGF_MAX_DEPTH);
+        kids[p].push_back((uint32_t)k);
+    }
+    for (size_t k = 0; k < n; ++k) {
+        const uint8_t op = t->op[k];
+        if (op == DGX_SGF_NOT && kids[k].size() != 1)
+            return fail(DGX_ERR_ARG, "node %zu: NOT with %zu children", k, kids[k].size());
+        if ((op == DGX_SGF_AND || op == DGX_SGF_OR) && kids[k].empty())
+            return fail(DGX_ERR_ARG, "node %zu: AND / OR without children", k);
+    }
+    // pre-order: a node's entry is written when it is reached, its end once its subtree is
+    prog->assign(n, SfOp{0, 0});
+    std::vector<std::pair<uint32_t, uint32_t>> stack{{0u, kSfNoParent}};  // (node, parent's entry)
+    std::vector<uint32_t> pos(n);
+    uint32_t pc = 0;
+    while (!stack.empty()) {
+        const auto [k, pe] = stack.back();
+        stack.pop_back();
+        pos[k] = pc;
+        const uint8_t op = t->op[k];
+        (*prog)[pc++] = op == DGX_SGF_LEAF ? SfOp{t->leaf[k], pe} : SfOp{kSfNode | (uint32_t)op << 28, pe};
+        for (size_t c = kids[k].size(); c-- > 0;) stack.push_back({kids[k][c], pos[k]});
+    }
+    // a subtree's end: one past its last pre-order entry, which is the end of its last child (or itself for a leaf)
+    std::vector<uint32_t> end(n);
+    for (size_t k = n; k-- > 0;) end[k] = kids[k].empty() ? pos[k] + 1 : end[kids[k].back()];
+    for (size_t k = 0; k < n; ++k)
+        if (t->op[k] != DGX_SGF_LEAF) (*prog)[pos[k]].w0 |= end[k];
+    return DGX_OK;
+}
+
+// The whole call on the lane: one table copy, 11 launches.  Workspace: 28 bytes per value slot of v_cap (cascade's
+// flags and their two scans, 8 each, and rows, 4), 40 per D0 slot (keep flags and their scan, D1, marks and their
+// scan), and the scans' look-back words.  `out` null: counts-only, no row value written.
+static int sf_run(dgx_lane* l, const std::vector<SfOp>& prog, const dgx_sg_filter_leaf* leaves, size_t nleaves,
+                  const uint64_t* d0, const uint64_t* d0_len, uint64_t d0_cap, const uint64_t* v, const uint64_t* v_off,
+                  uint64_t nrows, uint64_t v_cap, int32_t count, int32_t offset, uint64_t* dest_out,
+                  uint64_t* dest_len, uint64_t* out, uint64_t* out_off, uint32_t* counts) {
+    SfParams S{};
+    CcParams P{};
+    SfLeaf* h_leaf;
+    SfOp* h_prog;
+    CcNode* h_node;
+    u64* status;
+    u32* ticket;
+    const uint64_t td = scan_tiles(d0_cap), tv = scan_tiles(v_cap);
+    WsCarve ws(l);
+    ws.copied(&S.leaf, &h_leaf, std::max<size_t>(nleaves, 1));
+    ws.copied(&S.prog, &h_prog, prog.size());
+    ws.copied(&S.node, &h_node, 1);
+    if (int rc = ws.stage()) return rc;
+    uint64_t slots = 0;
+    for (size_t j = 0; j < nleaves; ++j) {
+        const dgx_sg_filter_leaf& L = leaves[j];
+        SfLeaf& s = h_leaf[j];
+        s = SfLeaf{};
+        s.kind = L.kind == DGX_SGF_LIST ? SF_LIST : SF_COUNT;
+        s.sb = slots;
+        if (L.kind == DGX_SGF_LIST) {
+            s.p = (const u64*)L.uids;
+            s.len = (const u64*)L.d_len;
+            s.room = L.n;
+            slots += L.n + 1;
+        } else {
+            s.cnt = L.counts;
+            s.off = (const u64*)L.off;
+            s.cmp = (u32)L.cmp;
+            s.thr = L.threshold;
+            if (L.off) slots += d0_cap;
+        }
+    }
+    memcpy(h_prog, prog.data(), prog.size() * sizeof(SfOp));
+    CcNode& c = *h_node;
+    c = CcNode{};
+    c.vcap = v_cap;
+    c.nrows = nrows;
+    c.ndest = d0_cap;  // |D0| once sf_check_kernel has run
+    c.mode = CC_ROWS_NEW;
+    c.ordered = 1;     // the rows' order is sf_check_kernel's
+    c.first = count;
+    c.offset = offset;
+    ws.zeroed(&S.bad, 4);
+    ws.zeroed(&ticket, 4);
+    ws.zeroed(&status, 2 * td + 2 * tv);
+    ws.zeroed(&S.mark, d0_cap);
+    ws.plain(&S.words, 2);
+    ws.plain(&P.keep, d0_cap);
+    ws.plain(&P.kx, d0_cap + 1);
+    ws.plain(&P.ND, d0_cap);
+    ws.plain(&P.NDE, 1);
+    ws.plain(&P.fv, v_cap);
+    ws.plain(&P.fx, v_cap + 1);
+    ws.plain(&P.fy, v_cap + 1);
+    ws.plain(&P.rw, v_cap);
+    u64* mx;
+    ws.plain(&mx, d0_cap + 1);
+    if (int rc = ws.commit()) return rc;
+    S.nleaves = (u32)nleaves;
+    S.d0 = (const u64*)d0;
+    S.d0_len = (const u64*)d0_len;
+    S.d0_cap = d0_cap;
+    S.v_off = (const u64*)v_off;
+    S.v = (const u64*)v;
+    S.nrows = nrows;
+    S.v_cap = v_cap;
+    S.slots = slots;
+    S.counts_only = out == nullptr;
+    S.paged = count != 0 || offset != 0;
+    S.keep = P.keep;
+    S.d1 = P.ND;
+    S.n1 = P.NDE;
+    S.fv = P.fv;
+    S.oo = (const u64*)out_off;
+    S.mx = mx;
+    S.err = l->d_err;
+    S.dest_out = (u64*)dest_out;
+    S.dest_len = (u64*)dest_len;
+    S.counts = counts;
+    // cascade's one NEW node reads the inputs in place (the level kernels never write V, VO or D) and writes the
+    // kept values and row offsets straight into the outputs
+    P.node = S.node;
+    P.nnodes = 1;
+    P.nv = v_cap;
+    P.no = nrows + 1;
+    P.nd = d0_cap;
+    P.out_rows = nrows;
+    P.V = const_cast<u64*>(S.v);
+    P.VO = const_cast<u64*>(S.v_off);
+    P.D = const_cast<u64*>(S.d0);
+    P.OV = (u64*)out;
+    P.OO = (u64*)out_off;
+    P.bad = S.bad;
+    P.err = l->d_err;
+    CcLevel L{};
+    L.a = 0;
+    L.b = 1;
+    L.nv = v_cap;
+    L.nd = d0_cap;
+    L.no = nrows + 1;
+    L.n_dest = S.words;
+    L.n_val = S.words + 1;
+    CcLevel Lc = L;
+    if (S.counts_only) Lc.nv = 0;  // the row offsets only
+    auto scan = [&](const u64* in, u64* o, const u64* n_word, uint64_t n) {
+        const uint64_t tiles = scan_tiles(n);
+        scan_u64_kernel<<<(unsigned)tiles, EN_NT, 0, l->stream>>>(in, o, n_word, n, status, ticket, nullptr);
+        status += tiles;
+        ticket += 1;
+    };
+    sf_check_kernel<<<gb_grid(std::max<uint64_t>({d0_cap, slots, nrows + 1, v_cap})), 256, 0, l->stream>>>(S);
+    sf_eval_kernel<<<gb_grid(d0_cap), 256, 0, l->stream>>>(S);
+    scan(P.keep, P.kx, L.n_dest, d0_cap);
+    cc_filter_kernel<<<gb_grid(std::max<uint64_t>({d0_cap, v_cap, 1})), 256, 0, l->stream>>>(P, L);
+    scan(P.fv, P.fx, L.n_val, v_cap);
+    cc_page_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P, L);
+    scan(P.fv, P.fy, L.n_val, v_cap);
+    cc_compact_kernel<<<gb_grid(std::max<uint64_t>(Lc.nv, Lc.no)), 256, 0, l->stream>>>(P, Lc);
+    sf_mark_kernel<<<gb_grid(std::max<uint64_t>(d0_cap, v_cap)), 256, 0, l->stream>>>(S);
+    scan(S.mark, mx, P.NDE, d0_cap);
+    sf_out_kernel<<<gb_grid(std::max<uint64_t>(d0_cap, nrows)), 256, 0, l->stream>>>(S);
+    CK(cudaGetLastError());
+    count_launches(l, 11);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_sg_filter(dgx_lane* l, const dgx_sg_filter_tree* tree, const dgx_sg_filter_leaf* leaves,
+                                 size_t nleaves, const uint64_t* d_d0, size_t d0_cap, const uint64_t* d_d0_len,
+                                 const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows, size_t v_cap,
+                                 int32_t count, int32_t offset, uint64_t* d_dest_out, size_t dest_cap,
+                                 uint64_t* d_dest_len, uint64_t* d_out, uint64_t* d_out_off, size_t out_cap,
+                                 uint32_t* d_counts) {
+    if (!l || !d_dest_len || !d_v_off || !d_out_off || (nrows && !d_counts)) return fail(DGX_ERR_ARG, "null argument");
+    std::vector<SfOp> prog;
+    if (int rc = sf_check_args(tree, leaves, nleaves, true, &prog)) return rc;
+    if (d0_cap >= kSfMax || nrows >= kSfMax || v_cap >= kSfMax)
+        return fail(DGX_ERR_ARG, "sizes are 32-bit: d0_cap %zu, nrows %zu, v_cap %zu", d0_cap, nrows, v_cap);
+    if ((d0_cap && !d_d0) || (v_cap && !d_v)) return fail(DGX_ERR_ARG, "null argument");
+    if (dest_cap < d0_cap || (d_out && out_cap < v_cap))
+        return fail(DGX_ERR_CAP, "dest_cap %zu / out_cap %zu below the bounds %zu / %zu", dest_cap, out_cap, d0_cap,
+                    v_cap);
+    if (d0_cap && !d_dest_out) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_dest_len, sizeof(uint64_t));
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    l->note_output(d_counts, nrows * sizeof(uint32_t));
+    if (d0_cap == 0) {  // D0 is empty: so are D1, the rows and the new dest
+        CK(cudaMemsetAsync(d_dest_len, 0, sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_out_off, 0, (nrows + 1) * sizeof(uint64_t), l->stream));
+        if (nrows) CK(cudaMemsetAsync(d_counts, 0, nrows * sizeof(uint32_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = sf_run(l, prog, leaves, nleaves, d_d0, d_d0_len, d0_cap, d_v, d_v_off, nrows, v_cap, count, offset,
+                        d_dest_out, d_dest_len, d_out, d_out_off, d_counts))
+        return rc;
+    g_stats.uids_in += d0_cap + v_cap;
+    l->note_output(d_dest_out, dest_cap * sizeof(uint64_t));
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_sg_filter(const dgx_sg_filter_tree* tree, const dgx_sg_filter_leaf* leaves, size_t nleaves,
+                             const uint64_t* d0, size_t n0, const uint64_t* v, const uint64_t* v_off, size_t nrows,
+                             int32_t count, int32_t offset, uint64_t* dest_out, size_t dest_cap, size_t* dest_len,
+                             uint64_t* out, uint64_t* out_off, size_t out_cap, uint32_t* counts) {
+    if (!dest_len || !v_off || !out_off || (nrows && !counts)) return fail(DGX_ERR_ARG, "null argument");
+    std::vector<SfOp> prog;
+    int rc;
+    if ((rc = sf_check_args(tree, leaves, nleaves, false, &prog))) return rc;
+    if (n0 >= kSfMax || nrows >= kSfMax)
+        return fail(DGX_ERR_ARG, "sizes are 32-bit: n0 %zu, nrows %zu", n0, nrows);
+    if ((rc = check_offsets("v_off", v_off, nrows, kSfMax))) return rc;
+    const uint64_t m = v_off[nrows];
+    if ((n0 && !d0) || (m && !v)) return fail(DGX_ERR_ARG, "null argument");
+    if (dest_cap < n0 || (out && out_cap < m))
+        return fail(DGX_ERR_CAP, "dest_cap %zu / out_cap %zu below the bounds %zu / %llu", dest_cap, out_cap, n0,
+                    (unsigned long long)m);
+    if (n0 && !dest_out) return fail(DGX_ERR_ARG, "null argument");
+    if (n0 == 0) {  // D0 is empty: so are D1, the rows and the new dest
+        *dest_len = 0;
+        memset(out_off, 0, (nrows + 1) * sizeof(uint64_t));
+        if (nrows) memset(counts, 0, nrows * sizeof(uint32_t));
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += n0 + m;
+    std::vector<dgx_sg_filter_leaf> D(leaves, leaves + nleaves);  // one copy of each array
+    uint64_t *d_d0, *d_v, *d_v_off;
+    if ((rc = upload_list(l, d0, n0, &d_d0)) || (rc = upload_list(l, v, m, &d_v)) ||
+        (rc = upload_list(l, v_off, nrows + 1, &d_v_off)))
+        return rc;
+    for (dgx_sg_filter_leaf& L : D) {
+        uint64_t* p;
+        if (L.kind == DGX_SGF_LIST) {
+            if ((rc = upload_list(l, L.uids, L.n, &p))) return rc;
+            L.uids = p;
+            g_stats.uids_in += L.n;
+        } else if (L.off) {
+            if ((rc = upload_list(l, L.off, n0 + 1, &p))) return rc;
+            L.off = p;
+        } else {
+            void* q;
+            if ((rc = l->ws.alloc(n0 * sizeof(uint32_t) + 16, &q))) return rc;
+            CK(cudaMemcpyAsync(q, L.counts, n0 * sizeof(uint32_t), cudaMemcpyHostToDevice, l->stream));
+            g_stats.h2d += n0 * sizeof(uint32_t);
+            L.counts = (const uint32_t*)q;
+        }
+    }
+    uint64_t *o_len, *o_dest, *o_out = nullptr, *o_off;
+    uint32_t* o_counts;
+    WsCarve o(l);
+    o.plain(&o_len, 2);
+    o.plain(&o_dest, n0);
+    if (out) o.plain(&o_out, m);
+    o.plain(&o_off, nrows + 1);
+    o.plain(&o_counts, nrows + 1);
+    if ((rc = o.commit())) return rc;
+    if ((rc = sf_run(l, prog, D.data(), nleaves, d_d0, nullptr, n0, d_v, d_v_off, nrows, m, count, offset, o_dest,
+                     o_len, o_out, o_off, o_counts)))
+        return rc;
+    CK(cudaMemcpyAsync(l->h_word, o_len, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(l->h_word + 1, o_off + nrows, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) return rc;
+    const uint64_t DN = l->h_word[0], K = l->h_word[1];
+    *dest_len = DN;
+    CK(cudaMemcpyAsync(out_off, o_off, (nrows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (nrows) CK(cudaMemcpyAsync(counts, o_counts, nrows * sizeof(uint32_t), cudaMemcpyDeviceToHost, l->stream));
+    if (DN) CK(cudaMemcpyAsync(dest_out, o_dest, DN * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (out && K) CK(cudaMemcpyAsync(out, o_out, K * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += (DN + (out ? K : 0) + nrows + 3) * sizeof(uint64_t) + nrows * sizeof(uint32_t);
+    g_stats.uids_out += DN + (out ? K : 0);
     return DGX_OK;
 }
 

@@ -897,3 +897,122 @@ func EvalMath(prog []MathNode, leaves []MathLeaf, rangeOver []uint64, hasRange b
 	n := int(uint64(info) & 0xffffffff)
 	return int((uint64(info) >> 32) & 0xff), keys[:n], words[:n], tags[:n], true
 }
+
+// dgxMinSgFilter: below this many D0 values plus row values a node's @filter and pagination stay in Go (ProcessGraph's
+// filter block, applyPagination).  The C19 record (profiles/h100_c19_sg_filter.json) times the library against a C
+// restatement of that path, not against Go, so this is the same bound as dgxMinMergeMatrix until a Go comparison sets
+// it.
+const dgxMinSgFilter = dgxMinMergeMatrix
+
+// SgFilter tree ops and leaf kinds (include/dgx.h).
+const (
+	SgfLeaf = uint8(C.DGX_SGF_LEAF)
+	SgfAnd  = uint8(C.DGX_SGF_AND)
+	SgfOr   = uint8(C.DGX_SGF_OR)
+	SgfNot  = uint8(C.DGX_SGF_NOT)
+)
+
+// SgFilterLeaf is one resolved filter leaf: a LIST (Uids strictly ascending: a function's DestUIDs, uid(var), literal
+// uids, D0 or nil for gt(len(x), n)), or a COUNT (Cmp one of "le" "ge" "lt" "gt" "eq", Threshold, and either Counts,
+// one per D0 value, or Off, D0's row offsets).
+type SgFilterLeaf struct {
+	IsCount   bool
+	Uids      []uint64
+	Cmp       string
+	Threshold int64
+	Counts    []uint32
+	Off       []uint64
+}
+
+// SgFilter runs ProcessGraph's filter block, applyPagination (updateUidMatrix, x.PageRange) and the DoCount block
+// (query/query.go:2310-2413) for one node in one call: op / parent / leaf are filterCopy's tree flattened (node 0 the
+// root, parents below their children), d0 the node's DestUIDs from processTask, rows its uid matrix.  It returns the
+// rows (nil when countsOnly), their lengths and the new DestUIDs.  It returns false, and the caller keeps the Go path,
+// below dgxMinSgFilter values, when the node has facets, an Order or FacetsOrder without DoCount, a count or offset
+// outside int32, a literal uid(...) leaf that does not strictly ascend (the parser keeps duplicates, and Go's answer
+// then depends on which IntersectWith variant runs), a COUNT leaf without exactly one of Counts (len(d0) entries) and
+// Off (len(d0) + 1 entries), and on any library error.
+func SgFilter(op []uint8, parent, leaf []uint32, leaves []SgFilterLeaf, d0 []uint64, rows []*pb.List, count, offset int,
+	ordered, doCount, facets, countsOnly bool) ([][]uint64, []uint32, []uint64, bool) {
+	if facets || (ordered && !doCount) || count != int(int32(count)) || offset != int(int32(offset)) {
+		return nil, nil, nil, false
+	}
+	if ordered { // DoCount with an order skips pagination (:2375-2394)
+		count, offset = 0, 0
+	}
+	m, nrows := totalUids(rows), len(rows)
+	if len(d0)+m < dgxMinSgFilter || len(op) == 0 {
+		return nil, nil, nil, false
+	}
+	cmps := map[string]C.int{"le": C.DGX_SGF_CMP_LE, "ge": C.DGX_SGF_CMP_GE, "lt": C.DGX_SGF_CMP_LT,
+		"gt": C.DGX_SGF_CMP_GT, "eq": C.DGX_SGF_CMP_EQ}
+	frees := []func(){}
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+	}()
+	carr := func(p unsafe.Pointer, free func()) unsafe.Pointer {
+		frees = append(frees, free)
+		return p
+	}
+	cl := make([]C.dgx_sg_filter_leaf, len(leaves)+1)
+	for j, l := range leaves {
+		if !l.IsCount {
+			for i := 1; i < len(l.Uids); i++ {
+				if l.Uids[i-1] >= l.Uids[i] {
+					return nil, nil, nil, false
+				}
+			}
+			cl[j].kind, cl[j].n = C.DGX_SGF_LIST, C.size_t(len(l.Uids))
+			cl[j].uids = (*C.uint64_t)(carr(cArray(l.Uids)))
+			continue
+		}
+		c, ok := cmps[l.Cmp]
+		// the library copies exactly len(d0) counts or len(d0) + 1 offsets: anything else stays in Go
+		if !ok || (l.Counts != nil) == (l.Off != nil) || (l.Counts != nil && len(l.Counts) != len(d0)) ||
+			(l.Off != nil && len(l.Off) != len(d0)+1) {
+			return nil, nil, nil, false
+		}
+		cl[j].kind, cl[j].cmp, cl[j].threshold = C.DGX_SGF_COUNT, c, C.int64_t(l.Threshold)
+		if l.Counts != nil {
+			cl[j].counts = (*C.uint32_t)(carr(cArray(l.Counts)))
+		} else {
+			cl[j].off = (*C.uint64_t)(carr(cArray(l.Off)))
+		}
+	}
+	tree := (*C.dgx_sg_filter_tree)(carr(cArray([]C.dgx_sg_filter_tree{{nnodes: C.size_t(len(op))}})))
+	tree.op = (*C.uint8_t)(carr(cArray(op)))
+	tree.parent = (*C.uint32_t)(carr(cArray(parent)))
+	tree.leaf = (*C.uint32_t)(carr(cArray(leaf)))
+	ctab := (*C.dgx_sg_filter_leaf)(carr(cArray(cl)))
+	v, vOff := make([]uint64, 0, m+1), make([]uint64, 1, nrows+1)
+	for _, r := range rows {
+		if r != nil {
+			v = append(v, r.Uids...)
+		}
+		vOff = append(vOff, uint64(len(v)))
+	}
+	dest, out, outOff := make([]uint64, len(d0)+1), make([]uint64, m+1), make([]uint64, nrows+1)
+	counts := make([]uint32, nrows+1)
+	var n C.size_t
+	outPtr := u64ptr(out)
+	if countsOnly {
+		outPtr = nil
+	}
+	d0c := append(make([]uint64, 0, len(d0)+1), d0...)
+	rc := C.dgx_sg_filter(tree, ctab, C.size_t(len(leaves)), u64ptr(d0c), C.size_t(len(d0)), u64ptr(v), u64ptr(vOff),
+		C.size_t(nrows), C.int32_t(count), C.int32_t(offset), u64ptr(dest), C.size_t(len(d0)), &n, outPtr,
+		u64ptr(outOff), C.size_t(m), (*C.uint32_t)(unsafe.Pointer(&counts[0])))
+	if rc != C.DGX_OK {
+		return nil, nil, nil, false
+	}
+	var res [][]uint64
+	if !countsOnly {
+		res = make([][]uint64, nrows)
+		for i := range res {
+			res[i] = out[outOff[i]:outOff[i+1]:outOff[i+1]]
+		}
+	}
+	return res, counts[:nrows], dest[:n], true
+}

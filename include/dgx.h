@@ -651,6 +651,69 @@ int dgx_cascade(const dgx_cascade_tree* tree, const uint64_t* v, const uint64_t*
                 uint64_t* out, uint64_t* out_off, size_t out_cap, uint64_t* dest_out, uint64_t* dest_out_off,
                 size_t dest_cap);
 
+/* A subgraph's @filter tree and first / offset (query/query.go ProcessGraph :2310-2413: filterCopy's tree, the filter
+ * block, applyPagination :2492-2507 with updateUidMatrix :1425-1439 and x.PageRange, and the DoCount block), without
+ * order or facets.  d0 is the node's DestUIDs from processTask (strictly ascending) and row i of its uid matrix is
+ * v[v_off[i] .. v_off[i+1]) (strictly ascending, v_off[0] == 0).  The tree is flat: node 0 is the root and parent[k] <
+ * k for every other node (parent[0] is ignored); op[k] is DGX_SGF_AND, _OR or _NOT (exactly one child; AND and OR have
+ * at least one) or DGX_SGF_LEAF, which reads leaves[leaf[k]] (several nodes may share a leaf).  Children keep index
+ * order.  At most DGX_SGF_MAX_NODES nodes and DGX_SGF_MAX_LEAVES leaves, and a node at most DGX_SGF_MAX_DEPTH below
+ * the root: filter trees in queries have a handful of nodes, a larger one stays in Go. */
+#define DGX_SGF_LEAF 0
+#define DGX_SGF_AND 1
+#define DGX_SGF_OR 2
+#define DGX_SGF_NOT 3
+#define DGX_SGF_MAX_NODES 1024
+#define DGX_SGF_MAX_LEAVES 1024
+#define DGX_SGF_MAX_DEPTH 64
+typedef struct dgx_sg_filter_tree {
+    size_t nnodes;
+    const uint8_t* op;        /* nnodes */
+    const uint32_t* parent;   /* nnodes */
+    const uint32_t* leaf;     /* nnodes: the leaf of a DGX_SGF_LEAF node */
+} dgx_sg_filter_tree;
+/* A leaf, resolved on the host to one of two kinds:
+ *   DGX_SGF_LIST: uids[0 .. n), strictly ascending (a function leaf's DestUIDs, uid(var), a literal uid(...) list, or
+ *     d0 / nothing for gt(len(x), n)).  Device form: d_len, when set, is a device word whose low 32 bits hold the length
+ *     (at most n, then the room), so the d_out_len of dgx_dev_merge_sorted_matrix or dgx_dev_trigram_query feeds it.
+ *   DGX_SGF_COUNT: d0[i] is in the set iff evalCompare(cmp, c_i, threshold) (worker/compare.go, int64), with c_i =
+ *     counts[i] (a count per d0 value, as dgx_list_count_rows writes) or off[i + 1] - off[i] (row lengths, as the
+ *     d_out_off of dgx_list_uids_rows over d0's keys): exactly one of counts / off is set.  cmp is DGX_SGF_CMP_*. */
+#define DGX_SGF_LIST 0
+#define DGX_SGF_COUNT 1
+#define DGX_SGF_CMP_LE 0
+#define DGX_SGF_CMP_GE 1
+#define DGX_SGF_CMP_LT 2
+#define DGX_SGF_CMP_GT 3
+#define DGX_SGF_CMP_EQ 4
+typedef struct dgx_sg_filter_leaf {
+    int kind;
+    int cmp;
+    int64_t threshold;
+    const uint64_t* uids;
+    size_t n;
+    const uint64_t* d_len;
+    const uint32_t* counts;
+    const uint64_t* off;
+} dgx_sg_filter_leaf;
+/* With f(LIST) its uids, f(COUNT) the d0 values it holds, f(AND) / f(OR) the intersection / union of the children and
+ * f(NOT) = d0 minus its child: D1 = f(root) ∩ d0.  Then each row becomes row ∩ D1 and, when count or offset is not 0,
+ * is cut to x.PageRange(count, offset, len); the new dest is D1 without pagination and MergeSorted(rows) with it.
+ * Writes the new dest to dest_out (*dest_len values), the rows to out / out_off (nrows + 1 offsets) and counts[i] =
+ * len(row i) (the DoCount block; pass count = offset = 0 for DoCount with an order).  out == NULL is counts-only mode:
+ * no row value is written.  dest_cap >= n0 and, unless out is NULL, out_cap >= v_off[nrows] are required:
+ * DGX_ERR_CAP before anything is copied otherwise.  DGX_ERR_ARG before anything is copied: a malformed tree (an
+ * unknown op, a parent not below its child or a leaf node as parent, NOT without exactly one child, AND / OR without
+ * one, a leaf index past nleaves, the limits above), a leaf's unknown kind or cmp, a COUNT leaf without exactly one of
+ * counts / off, n0, nrows, v_off[nrows] or a list length of 2^32 or more, v_off not starting at 0 or decreasing, a null
+ * array that is needed.  DGX_ERR_ARG after the kernels, with nothing written: d0, a row or a LIST leaf that does not
+ * strictly ascend, or a COUNT leaf's off that decreases.  n0 == 0 writes zero lengths and needs no device.
+ * Launches: 11 (DESIGN section 3.15), whatever the rows, values, n0, leaves and tree. */
+int dgx_sg_filter(const dgx_sg_filter_tree* tree, const dgx_sg_filter_leaf* leaves, size_t nleaves, const uint64_t* d0,
+                  size_t n0, const uint64_t* v, const uint64_t* v_off, size_t nrows, int32_t count, int32_t offset,
+                  uint64_t* dest_out, size_t dest_cap, size_t* dest_len, uint64_t* out, uint64_t* out_off,
+                  size_t out_cap, uint32_t* counts);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -945,6 +1008,19 @@ typedef struct dgx_cascade_node {
 int dgx_dev_cascade(dgx_lane* lane, const dgx_cascade_tree* tree, const dgx_cascade_node* nodes, uint64_t* d_out,
                     uint64_t* d_out_off, size_t out_cap, uint64_t* d_dest_out, uint64_t* d_dest_out_off,
                     size_t dest_cap, uint64_t* d_sizes);
+/* Device form of dgx_sg_filter: tree and leaves in host memory, d_d0, the rows, the arrays the leaves point at and the
+ * outputs in device memory, so the rows calls' (d_out, d_out_off), dgx_dev_list_count_rows' d_counts and
+ * dgx_dev_merge_sorted_matrix's dest feed it directly.  |D0| is d0_cap, or the low 32 bits of the device word d_d0_len
+ * when it is set (at most d0_cap); COUNT arrays hold at least |D0| counts or |D0| + 1 offsets.  v_cap is the room of d_v
+ * (d_v_off[nrows] must not pass it).  The bounds are d0_cap and v_cap: dest_cap or out_cap below them is DGX_ERR_CAP at
+ * the call, as every argument error of the host form is DGX_ERR_ARG there.  d_dest_len is one device uint64.  The order
+ * and offset checks, and a length word past its room, run on the device: a refused call writes *d_dest_len = 0 and
+ * nothing else, and surfaces as DGX_ERR_ARG at the next dgx_lane_sync.  Asynchronous on the lane; 11 launches. */
+int dgx_dev_sg_filter(dgx_lane* lane, const dgx_sg_filter_tree* tree, const dgx_sg_filter_leaf* leaves, size_t nleaves,
+                      const uint64_t* d_d0, size_t d0_cap, const uint64_t* d_d0_len, const uint64_t* d_v,
+                      const uint64_t* d_v_off, size_t nrows, size_t v_cap, int32_t count, int32_t offset,
+                      uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_dest_len, uint64_t* d_out,
+                      uint64_t* d_out_off, size_t out_cap, uint32_t* d_counts);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

@@ -360,6 +360,40 @@ private:
     dgx_reach_set* s_ = nullptr;
 };
 
+// The result of SubgraphFilter: the filtered and paged rows (empty in counts-only mode), their lengths and the new
+// DestUIDs.
+struct SgFilterResult {
+    std::vector<pb::List> rows;
+    std::vector<uint32_t> counts;
+    pb::List dest;
+};
+
+// A subgraph's @filter tree and first / offset (query/query.go ProcessGraph's filter block, applyPagination and the
+// DoCount block) in one call (dgx_sg_filter).  op / parent / leaf form the flat tree of dgx_sg_filter_tree; leaves'
+// arrays are host memory with n0 counts or n0 + 1 offsets for a COUNT leaf.
+inline SgFilterResult SubgraphFilter(const std::vector<uint8_t>& op, const std::vector<uint32_t>& parent,
+                                     const std::vector<uint32_t>& leaf, const std::vector<dgx_sg_filter_leaf>& leaves,
+                                     const pb::List& d0, const std::vector<pb::List>& rows, int32_t count = 0,
+                                     int32_t offset = 0, bool counts_only = false) {
+    std::vector<uint64_t> v, v_off{0};
+    for (const pb::List& r : rows) { v.insert(v.end(), r.Uids.begin(), r.Uids.end()); v_off.push_back(v.size()); }
+    const dgx_sg_filter_tree tree{op.size(), op.data(), parent.data(), leaf.data()};
+    const size_t n0 = d0.Uids.size(), nrows = rows.size();
+    std::vector<uint64_t> dest(std::max<size_t>(n0, 1)), out(std::max<size_t>(v.size(), 1)), out_off(nrows + 1);
+    std::vector<uint32_t> counts(std::max<size_t>(nrows, 1));
+    size_t n = 0;
+    check(dgx_sg_filter(&tree, leaves.data(), leaves.size(), d0.Uids.data(), n0, v.data(), v_off.data(), nrows, count,
+                        offset, dest.data(), n0, &n, counts_only ? nullptr : out.data(), out_off.data(), v.size(),
+                        counts.data()));
+    SgFilterResult res;
+    if (!counts_only)
+        for (size_t r = 0; r < nrows; ++r)
+            res.rows.emplace_back(std::vector<uint64_t>(out.begin() + out_off[r], out.begin() + out_off[r + 1]));
+    res.counts.assign(counts.begin(), counts.begin() + nrows);
+    res.dest = pb::List(std::vector<uint64_t>(dest.begin(), dest.begin() + n));
+    return res;
+}
+
 // One subgraph node of a @cascade forest, in pre-order (dgx_cascade): parent index (-1 for a query root), DGX_CASCADE_*
 // flags, Params.Cascade.First / Offset, len(counts), DestUIDs, uidMatrix rows and has_val (one byte per row).
 struct CascadeNode {

@@ -144,6 +144,7 @@ def main():
     ap.add_argument("--c16-only", action="store_true", help="only the C16 shortest() rows")
     ap.add_argument("--c17-only", action="store_true", help="only the C17 value-variable rows")
     ap.add_argument("--c18-only", action="store_true", help="only the C18 math() rows")
+    ap.add_argument("--c19-only", action="store_true", help="only the C19 @filter and first / offset rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -171,9 +172,11 @@ def main():
         rows = c17_rows(Lane())
     elif args.c18_only:
         rows = c18_rows(Lane())
+    elif args.c19_only:
+        rows = c19_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1864,6 +1867,95 @@ def c18_rows(L):
                              "keys": int(cap - 1), "check": bool(ok), "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del dleaf, ok_t, ow_t, ot_t
+    return out_rows
+
+
+def c19_rows(L):
+    """C19 "@filter and first / offset".  C19a: 10 000 parent rows of about 1e7 values over 1.2e7 uids, D0 of about
+    3e6, the 7-node tree AND(COUNT gt 1, OR(LIST 1e5, LIST 1e6), NOT(LIST 5e5)), first: 10.  C19b: C19a in counts-only
+    mode (count(friend @filter(...))).  C19c: TestToFastJSONFilterOrFirst's size (launch-bound).  Legs: (1) the device
+    form on resident inputs (CUDA events), (2) the host form with its copies (wall clock), (3) the line-by-line
+    restatement (tests/sg_filter_oracle.c) on 1 thread -- C, not Go.  Every leg is checked against the restatement."""
+    import gen_sg_filter as gs
+    import sg_filter_oracle as so
+    from dgraph_b200 import algo
+
+    lib = L.lib
+    U64 = np.uint64
+
+    def dp(t):
+        return t.data_ptr()
+
+    def up(x, dt=U64):
+        x = np.concatenate([np.ascontiguousarray(x, dt), np.zeros(1, dt)])
+        return torch.from_numpy(x.view(np.int64 if dt == U64 else np.int32)).to(DEV)
+
+    big = gs.big_case(np.random.default_rng(19), nrows=10_000, nvals=10_000_000, n0=3_000_000)
+    small = (("or", [0, 1, 2]), [("list", [31]), ("list", [24]), ("list", [25])], [23, 24, 25, 31, 101],
+             [np.array([23, 24, 25, 31, 101], U64)], 2, 0)
+    out_rows = []
+    for name, case, co in (("C19a", big, False), ("C19b", big, True), ("C19c", small, False)):
+        tree, leaves, d0, rows, count, offset = case
+        t0 = time.perf_counter()
+        want = so.sg_filter(*case)
+        t_or = (time.perf_counter() - t0) * 1e3
+        d0 = np.asarray(d0, U64)
+        off = np.zeros(len(rows) + 1, U64)
+        np.cumsum([len(r) for r in rows], out=off[1:])
+        v = np.concatenate([np.asarray(r, U64) for r in rows])
+        f = algo.sg_filter_flat(tree)
+        t = algo.sg_filter_tree(f)
+        dleaf, descs = [], []
+        for lf in leaves:
+            if lf[0] == "list":
+                d = up(lf[1])
+                descs.append(_lib.SgFilterLeaf(0, 0, 0, dp(d), len(lf[1]), None, None, None))
+            else:
+                d = up(lf[3], np.uint32)
+                descs.append(_lib.SgFilterLeaf(1, algo.SGF_CMP[lf[1]], int(lf[2]), None, 0, None, dp(d), None))
+            dleaf.append(d)
+        tab = (_lib.SgFilterLeaf * len(descs))(*descs)
+        d_d0, d_v, d_off = up(d0), up(v), up(off)
+        n0, nrows, m = d0.size, len(rows), v.size
+        d_dest, d_len = torch.empty(n0 + 1, dtype=torch.int64, device=DEV), torch.empty(1, dtype=torch.int64,
+                                                                                         device=DEV)
+        d_out = None if co else torch.empty(m + 1, dtype=torch.int64, device=DEV)
+        d_oo, d_c = torch.empty(nrows + 1, dtype=torch.int64, device=DEV), torch.empty(nrows + 1, dtype=torch.int32,
+                                                                                        device=DEV)
+
+        def dev():
+            _lib.check(lib.dgx_dev_sg_filter(L.h, C.byref(t), tab, len(descs), dp(d_d0), n0, None, dp(d_v), dp(d_off),
+                                             nrows, m, count, offset, dp(d_dest), n0, dp(d_len),
+                                             None if co else dp(d_out), dp(d_oo), m, dp(d_c)))
+        ms_dev, _ = timeit(dev, warm=2, reps=10)
+        L.sync()
+        D = int(d_len.cpu().numpy()[0])
+        oo = d_oo.cpu().numpy().view(U64)
+        ok_dev = (np.array_equal(d_dest[:D].cpu().numpy().view(U64), want[2]) and
+                  np.array_equal(d_c[:nrows].cpu().numpy().view(np.uint32), want[1]) and
+                  int(oo[nrows]) == int(want[1].sum()))
+        if not co:
+            ok_dev = ok_dev and np.array_equal(d_out[:int(oo[nrows])].cpu().numpy().view(U64),
+                                               np.concatenate(want[0] + [np.zeros(0, U64)]))
+        algo.SubgraphFilter(*case[:4], count=count, offset=offset, counts_only=co)
+        ts = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            got = algo.SubgraphFilter(*case[:4], count=count, offset=offset, counts_only=co)
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ok_host = (np.array_equal(got[1], want[1]) and np.array_equal(got[2].Uids, want[2]) and
+                   (co or all(np.array_equal(a, b) for a, b in zip(got[0], want[0]))))
+        full = (f"{name}: {nrows} rows of {m} values, |D0| {n0}, {f['nnodes']} tree nodes over {len(leaves)} leaves "
+                f"({', '.join(str(len(lf[1])) if lf[0] == 'list' else 'COUNT' for lf in leaves)}), first {count}"
+                f"{', counts only' if co else ''}; new dest {want[2].size}, kept values {int(want[1].sum())}")
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev, "CUDA events, median of 10 after 2 warm"),
+                                    ("host form", float(np.median(ts)), ok_host, "wall clock, median of 3 after 1 warm"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, True, "orc_sg_filter, wall clock, one "
+                                     "run; the reference the other legs are checked against")):
+            out_rows.append({"op": "SubgraphFilter", "workload": name, "leg": leg, "config": full, "ms": round(ms, 4),
+                             "values": int(m), "check": bool(ok), "timing": timing})
+            print(json.dumps(out_rows[-1]), flush=True)
+        del dleaf, d_d0, d_v, d_off, d_dest, d_out, d_oo, d_c
     return out_rows
 
 
