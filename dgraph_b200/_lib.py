@@ -151,6 +151,8 @@ SYMBOLS = {
     "dgx_cascade": (_int, [C.POINTER(CascadeTree), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _sz]),
     "dgx_sg_filter": (_int, [C.POINTER(SgFilterTree), C.POINTER(SgFilterLeaf), _sz, _vp, _sz, _vp, _vp, _sz, C.c_int32,
                              C.c_int32, _vp, _sz, _szp, _vp, _vp, _sz, _vp]),
+    "dgx_var_order": (_int, [C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _sz, C.c_int32, C.c_int32, _vp, _vp, _sz,
+                             _vp, _sz, _szp]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
     "dgx_encode_bound": (None, [_sz, C.c_uint32, _szp, _szp]),
@@ -201,6 +203,8 @@ SYMBOLS = {
     "dgx_dev_cascade": (_int, [_vp, C.POINTER(CascadeTree), C.POINTER(CascadeNode), _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_sg_filter": (_int, [_vp, C.POINTER(SgFilterTree), C.POINTER(SgFilterLeaf), _sz, _vp, _sz, _vp, _vp, _vp,
                                  _sz, _sz, C.c_int32, C.c_int32, _vp, _sz, _vp, _vp, _vp, _sz, _vp]),
+    "dgx_dev_var_order": (_int, [_vp, C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _vp, _sz, _sz, C.c_int32,
+                                 C.c_int32, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),
     "dgx_filter_tail_queries": (_u64, [_vp]),

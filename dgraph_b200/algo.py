@@ -918,6 +918,43 @@ def EvalMath(tree, maps, range_uids=None):
     return MATH_KIND[(info.value >> 32) & 0xFF], ok[:n].copy(), ow[:n].copy(), ot[:n].copy()
 
 
+def var_order_leaf(m):
+    """(kept arrays, dgx_math_leaf) of the map an order reads: None (Go's nil map, which the call refuses), (keys,
+    int64 or float64 values) as PropagateVar / LevelAgg return it, or (keys, u64 words, u8 tags) as EvalMath returns a
+    "map" result."""
+    k, w, t, typ, nil = math_leaf_arrays(m)
+    n = 0 if nil else k.size
+    keep = [np.ascontiguousarray(a) if a.size else np.zeros(1, a.dtype) for a in (k, w)]
+    if t is not None:
+        keep.append(t if t.size else np.zeros(1, np.uint8))
+    leaf = _lib.MathLeaf(keep[0].ctypes.data, keep[1].ctypes.data, keep[2].ctypes.data if t is not None else None,
+                         None, n, typ, nil)
+    return keep, leaf
+
+
+def OrderByVar(m, desc: bool, dest, rows, count: int = 0, offset: int = 0):
+    """orderasc / orderdesc by a value variable (query/query.go applyOrderAndPagination's value-variable branch:
+    updateUidMatrix, sortAndPaginateUsingVar with types.Sort and x.PageRange, updateDestUids) in ONE call
+    (dgx_var_order), in Go's exact order, ties included.
+
+    m: the variable's map (see var_order_leaf); desc: orderdesc; dest: the node's DestUIDs after its filters; rows:
+    its uid matrix (strictly ascending rows); count / offset: Params.Count / Offset.  Returns (rows, dest): the ordered
+    and paged rows and the new DestUIDs as a List.  A nil map and a row whose first mapped value is a bool raise
+    DgxError (DGX_ERR_ARG), where Go returns an error."""
+    keep, leaf = var_order_leaf(m)
+    d = _u64(dest.Uids if isinstance(dest, List) else dest)
+    v, v_off = _csr_u64(rows)
+    nrows, M = len(rows), int(v_off[-1])
+    out = np.empty(max(M, 1), np.uint64)
+    out_off = np.zeros(nrows + 1, np.uint64)
+    dout = np.empty(max(d.size, 1), np.uint64)
+    n = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_var_order(C.byref(leaf), int(bool(desc)), _p(d), d.size, _p(v), _p(v_off), nrows,
+                                         count, offset, _p(out), _p(out_off), M, _p(dout), d.size, C.byref(n)))
+    del keep
+    return [out[int(out_off[i]):int(out_off[i + 1])].copy() for i in range(nrows)], List(dout[:n.value].copy())
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -46,6 +46,7 @@
 #include "valvar_kernel.cuh"
 #include "math_kernel.cuh"
 #include "sg_filter_kernel.cuh"
+#include "var_order_kernel.cuh"
 #include "wire.hpp"
 #include "ws_layout.hpp"
 
@@ -548,6 +549,11 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
             return fail(DGX_ERR_ARG, "an @filter input is malformed (d0, a row or a LIST leaf not strictly ascending, "
                                      "a COUNT leaf's offsets or the row offsets decreasing, row offsets not starting "
                                      "at 0 or past v_cap, or a length word past its room)");
+        if (flag & kLaneErrVarOrder)
+            return fail(DGX_ERR_ARG, "an order-by-variable input is refused (dest, map keys or a row not strictly "
+                                     "ascending, row offsets not starting at 0, decreasing or past v_cap, a length word "
+                                     "past its room, an unknown entry tag, or a row whose first mapped entry is a bool, "
+                                     "which Go refuses as not sortable)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -4693,6 +4699,234 @@ extern "C" int dgx_sg_filter(const dgx_sg_filter_tree* tree, const dgx_sg_filter
     CK(cudaStreamSynchronize(l->stream));
     g_stats.d2h += (DN + (out ? K : 0) + nrows + 3) * sizeof(uint64_t) + nrows * sizeof(uint32_t);
     g_stats.uids_out += DN + (out ? K : 0);
+    return DGX_OK;
+}
+
+// ---------------------------------------------------------------------------
+// orderasc / orderdesc by a value variable: a uid matrix sorted in Go's exact order and paged (var_order_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr uint64_t kVoMax = uint64_t(1) << 32;  // dest, map, rows and values are 32-bit counts
+
+// The row sort's radix passes, from nrows alone: P_r = ceil(bits(nrows - 1) / 8).
+static uint32_t vo_row_passes(uint64_t nrows) {
+    return (gb_bits(nrows ? nrows - 1 : 0) + GB_DIGIT_BITS - 1) / GB_DIGIT_BITS;
+}
+
+// The checks of the map both forms make before anything is copied.
+static int vo_check_var(const dgx_math_leaf* var, bool dev) {
+    if (!var) return fail(DGX_ERR_ARG, "null map");
+    if (var->nil) return fail(DGX_ERR_ARG, "the variable has no map: used before definition");
+    if (!var->tag && var->type != DGX_VAL_INT64 && var->type != DGX_VAL_FLOAT64)
+        return fail(DGX_ERR_ARG, "a map without tags has type DGX_VAL_INT64 or DGX_VAL_FLOAT64, not %d", var->type);
+    if (!dev && var->d_len) return fail(DGX_ERR_ARG, "d_len belongs to the device form");
+    if (var->n >= kVoMax) return fail(DGX_ERR_ARG, "a map of 2^32 entries or more");
+    if (var->n && (!var->key || !var->word)) return fail(DGX_ERR_ARG, "null map array");
+    return DGX_OK;
+}
+
+// The whole call on the lane: 37 + 3 P_r launches.  Workspace: words, tickets and the look-back words, zeroed; per
+// value slot of v_cap about 120 bytes (U and W flags and their scans 32, map index 4, U 8, W's uids, words, tags and
+// rows 21, order keys 8, radix keys and payloads 24, pair slots 4, the radix hist); per row 44 (offsets of U and W,
+// flags, list, page start, page length and its scan); 16 per dest slot (marks and their scan).
+static int vo_run(dgx_lane* l, const dgx_math_leaf& M, int desc, const uint64_t* dest, const uint64_t* dlen,
+                  uint64_t dcap, const uint64_t* v, const uint64_t* v_off, uint64_t nrows, uint64_t v_cap,
+                  int32_t count, int32_t offset, uint64_t* out, uint64_t* out_off, uint64_t* dest_out,
+                  uint64_t* dest_len) {
+    const uint64_t vc = std::max<uint64_t>(v_cap, 1), tv = scan_tiles(vc), tr = scan_tiles(nrows), td = scan_tiles(dcap);
+    const uint64_t tiles = (vc + GB_TILE - 1) / GB_TILE, hn = (uint64_t)GB_RADIX * tiles, th = scan_tiles(hn);
+    const uint32_t pr = vo_row_passes(nrows);
+    VoParams P{};
+    u64 *status, *ek[2], *hist, *hoff;
+    u32 *tickets, *ep[2];
+    WsCarve ws(l);
+    ws.zeroed(&P.bad, 4);
+    ws.zeroed(&P.words, VO_WORDS);
+    ws.zeroed(&tickets, 32);
+    ws.zeroed(&status, 2 * tv + (VO_KEY_PASSES + pr) * th + tr + td);
+    ws.zeroed(&P.rflag, nrows);
+    ws.zeroed(&P.mark, dcap);
+    ws.plain(&P.uf, vc);
+    ws.plain(&P.ux, vc + 1);
+    ws.plain(&P.wf, vc);
+    ws.plain(&P.wx, vc + 1);
+    ws.plain(&P.U, vc);
+    ws.plain(&P.wuid, vc);
+    ws.plain(&P.wword, vc);
+    ws.plain(&P.okey, vc);
+    ws.plain(&ek[0], vc);
+    ws.plain(&ek[1], vc);
+    ws.plain(&hist, hn);
+    ws.plain(&hoff, hn + 1);
+    ws.plain(&P.uoff, nrows + 1);
+    ws.plain(&P.woff, nrows + 1);
+    ws.plain(&P.plen, nrows);
+    ws.plain(&P.po, nrows + 1);
+    ws.plain(&P.mx, dcap + 1);
+    ws.plain(&P.mj, vc);
+    ws.plain(&P.wrow, vc);
+    ws.plain(&ep[0], vc);
+    ws.plain(&ep[1], vc);
+    ws.plain(&P.pairs, vc);
+    ws.plain(&P.longrows, nrows);
+    ws.plain(&P.pstart, nrows);
+    ws.plain(&P.wtag, vc);
+    if (int rc = ws.commit()) return rc;
+    P.key = (const u64*)M.key;
+    P.word = (const u64*)M.word;
+    P.tag = M.tag;
+    P.mlen = (const u64*)M.d_len;
+    P.mcap = M.n;
+    P.mtype = M.tag ? 0 : (u32)M.type;
+    P.desc = desc != 0;
+    P.dest = (const u64*)dest;
+    P.dlen = (const u64*)dlen;
+    P.dcap = dcap;
+    P.v = (const u64*)v;
+    P.v_off = (const u64*)v_off;
+    P.nrows = nrows;
+    P.v_cap = v_cap;
+    P.count = count;
+    P.offset = offset;
+    P.tiles = tiles;
+    P.err = l->d_err;
+    P.ticket = tickets + 31;
+    P.ek = ek[0];
+    P.ep = ep[0];
+    P.out = (u64*)out;
+    P.out_off = (u64*)out_off;
+    P.dest_out = (u64*)dest_out;
+    P.dest_len = (u64*)dest_len;
+    u32* ticket = tickets;
+    auto scan = [&](const u64* in, u64* o, const u64* n_word, uint64_t n, u64* total) {
+        const uint64_t t = scan_tiles(n);
+        scan_u64_kernel<<<(unsigned)t, EN_NT, 0, l->stream>>>(in, o, n_word, n, status, ticket, total);
+        status += t;
+        ticket += 1;
+    };
+    vo_check_kernel<<<gb_grid(std::max<uint64_t>({dcap, M.n, nrows + 1, v_cap})), 256, 0, l->stream>>>(P);
+    vo_gather_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P);
+    scan(P.uf, P.ux, P.words + VO_W_M, vc, nullptr);
+    scan(P.wf, P.wx, P.words + VO_W_M, vc, P.words + VO_W_W);
+    vo_compact_kernel<<<gb_grid(std::max<uint64_t>(v_cap, nrows + 1)), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 5);
+    // W by order key (64 bits: the result is back in buffer 0), then stably by row
+    if (int rc = gb_sort(l, tiles, P.bad, P.words + VO_W_H, ek, ep, P.words + VO_W_W, VO_KEY_PASSES, hist, hoff, status,
+                         ticket))
+        return rc;
+    vo_rowkey_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P, ep[0], ek[1], ep[1]);
+    u64* const rk[2] = {ek[1], ek[0]};
+    u32* const rp[2] = {ep[1], ep[0]};
+    if (int rc = gb_sort(l, tiles, P.bad, P.words + VO_W_H, rk, rp, P.words + VO_W_W, pr, hist, hoff, status, ticket))
+        return rc;
+    P.S = rp[pr & 1];
+    vo_tier_kernel<<<gb_grid(std::max<uint64_t>(v_cap, nrows)), 256, 0, l->stream>>>(P);
+    vo_rows_kernel<<<gb_grid(nrows), 256, 0, l->stream>>>(P);
+    vo_cta_kernel<<<(unsigned)(2 * g_num_sms), VO_NT, 0, l->stream>>>(P);
+    scan(P.plen, P.po, P.words + VO_W_R, nrows, nullptr);
+    vo_write_kernel<<<gb_grid(std::max<uint64_t>(v_cap, nrows + 1)), 256, 0, l->stream>>>(P);
+    scan(P.mark, P.mx, P.words + VO_W_ND, dcap, nullptr);
+    vo_dest_kernel<<<gb_grid(dcap), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 8);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_var_order(dgx_lane* l, const dgx_math_leaf* var, int desc, const uint64_t* d_dest, size_t ndest,
+                                 const uint64_t* d_ndest, const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows,
+                                 size_t v_cap, int32_t count, int32_t offset, uint64_t* d_out, uint64_t* d_out_off,
+                                 size_t out_cap, uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_dest_len) {
+    if (!l || !d_dest_len || !d_v_off || !d_out_off) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = vo_check_var(var, true)) return rc;
+    if (ndest >= kVoMax || nrows >= kVoMax || v_cap >= kVoMax)
+        return fail(DGX_ERR_ARG, "sizes are 32-bit: ndest %zu, nrows %zu, v_cap %zu", ndest, nrows, v_cap);
+    if ((ndest && !d_dest) || (v_cap && !d_v)) return fail(DGX_ERR_ARG, "null argument");
+    if (out_cap < v_cap || dest_cap < ndest)
+        return fail(DGX_ERR_CAP, "out_cap %zu / dest_cap %zu below the bounds %zu / %zu", out_cap, dest_cap, v_cap,
+                    ndest);
+    if ((v_cap && !d_out) || (ndest && !d_dest_out)) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_dest_len, sizeof(uint64_t));
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    if (ndest == 0 || nrows == 0) {  // no dest value or no row: every row is empty, so is the new dest
+        CK(cudaMemsetAsync(d_dest_len, 0, sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_out_off, 0, (nrows + 1) * sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = vo_run(l, *var, desc, d_dest, d_ndest, ndest, d_v, d_v_off, nrows, v_cap, count, offset, d_out,
+                        d_out_off, d_dest_out, d_dest_len))
+        return rc;
+    g_stats.uids_in += ndest + v_cap + var->n;
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_dest_out, dest_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_var_order(const dgx_math_leaf* var, int desc, const uint64_t* dest, size_t ndest,
+                             const uint64_t* v, const uint64_t* v_off, size_t nrows, int32_t count, int32_t offset,
+                             uint64_t* out, uint64_t* out_off, size_t out_cap, uint64_t* dest_out, size_t dest_cap,
+                             size_t* dest_len) {
+    if (!dest_len || !v_off || !out_off) return fail(DGX_ERR_ARG, "null argument");
+    int rc;
+    if ((rc = vo_check_var(var, false))) return rc;
+    if (ndest >= kVoMax || nrows >= kVoMax) return fail(DGX_ERR_ARG, "sizes are 32-bit: ndest %zu, nrows %zu", ndest, nrows);
+    if ((rc = check_offsets("v_off", v_off, nrows, kVoMax))) return rc;
+    const uint64_t m = v_off[nrows];
+    if ((ndest && !dest) || (m && !v)) return fail(DGX_ERR_ARG, "null argument");
+    if (out_cap < m || dest_cap < ndest)
+        return fail(DGX_ERR_CAP, "out_cap %zu / dest_cap %zu below the bounds %llu / %zu", out_cap, dest_cap,
+                    (unsigned long long)m, ndest);
+    if ((m && !out) || (ndest && !dest_out)) return fail(DGX_ERR_ARG, "null argument");
+    if (ndest == 0 || nrows == 0) {  // no dest value or no row: every row is empty, so is the new dest
+        *dest_len = 0;
+        memset(out_off, 0, (nrows + 1) * sizeof(uint64_t));
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += ndest + m + var->n;
+    dgx_math_leaf D = *var;  // one copy of each array
+    uint64_t *d_dest, *d_v, *d_v_off, *k, *w;
+    if ((rc = upload_list(l, dest, ndest, &d_dest)) || (rc = upload_list(l, v, m, &d_v)) ||
+        (rc = upload_list(l, v_off, nrows + 1, &d_v_off)) || (rc = upload_list(l, var->key, var->n, &k)) ||
+        (rc = upload_list(l, var->word, var->n, &w)))
+        return rc;
+    D.key = k;
+    D.word = w;
+    if (var->tag) {
+        void* t;
+        if ((rc = l->ws.alloc(var->n + 1, &t))) return rc;
+        if (var->n) CK(cudaMemcpyAsync(t, var->tag, var->n, cudaMemcpyHostToDevice, l->stream));
+        g_stats.h2d += var->n;
+        D.tag = (const uint8_t*)t;
+    }
+    uint64_t *o_len, *o_dest, *o_out, *o_off;
+    WsCarve o(l);
+    o.plain(&o_len, 1);
+    o.plain(&o_dest, ndest);
+    o.plain(&o_out, m);
+    o.plain(&o_off, nrows + 1);
+    if ((rc = o.commit())) return rc;
+    if ((rc = vo_run(l, D, desc, d_dest, nullptr, ndest, d_v, d_v_off, nrows, m, count, offset, o_out, o_off, o_dest,
+                     o_len)))
+        return rc;
+    CK(cudaMemcpyAsync(l->h_word, o_len, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(l->h_word + 1, o_off + nrows, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) {
+        *dest_len = 0;
+        return rc;
+    }
+    const uint64_t DN = l->h_word[0], K = l->h_word[1];
+    *dest_len = DN;
+    CK(cudaMemcpyAsync(out_off, o_off, (nrows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (DN) CK(cudaMemcpyAsync(dest_out, o_dest, DN * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (K) CK(cudaMemcpyAsync(out, o_out, K * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += (DN + K + nrows + 3) * sizeof(uint64_t);
+    g_stats.uids_out += DN + K;
     return DGX_OK;
 }
 

@@ -1016,3 +1016,68 @@ func SgFilter(op []uint8, parent, leaf []uint32, leaves []SgFilterLeaf, d0 []uin
 	}
 	return res, counts[:nrows], dest[:n], true
 }
+
+// dgxMinVarOrder: below this many dest values plus row values a node's order by a value variable stays in Go
+// (applyOrderAndPagination's value-variable branch).  The C20 record (profiles/h100_c20_var_order.json) times the
+// library against a C restatement of that path, not against Go, so this is the dgxMinMergeMatrix bound until a Go
+// comparison sets it.
+const dgxMinVarOrder = dgxMinMergeMatrix
+
+// OrderByVar runs applyOrderAndPagination's value-variable branch (query/query.go:2511-2530: updateUidMatrix's order
+// branch, sortAndPaginateUsingVar with types.Sort and x.PageRange, updateDestUids) in one call, in Go's exact order,
+// ties included.  m is Params.UidToVal as a MathLeaf: int64 and float64 values as ValInt64 / ValFloat64 words, a
+// math() map's bools and nils as ValBool / ValNil; a map holding any other type (string, DateTime, ...) is not passed
+// here.  dest is sg.DestUIDs after the filter block, rows the uid matrix, count / offset Params.Count / Offset.  It
+// returns the new rows and DestUIDs.  ok == false -- FacetsOrder set (sortAndPaginateUsingFacet), DoCount, a nil map
+// (Go's "used before definition" error, which Go then returns), sizes outside the library's bounds, below
+// dgxMinVarOrder values, or any library error (including a row whose first mapped value is a bool, Go's "isn't
+// sortable") -- means the caller keeps Go's path.
+func OrderByVar(m MathLeaf, desc bool, dest []uint64, rows []*pb.List, count, offset int, facetsOrder,
+	doCount bool) ([][]uint64, []uint64, bool) {
+	if facetsOrder || doCount || m.Nil || count != int(int32(count)) || offset != int(int32(offset)) ||
+		len(m.Keys) != len(m.Words) || len(m.Keys) != len(m.Tags) {
+		return nil, nil, false
+	}
+	mv, nrows := totalUids(rows), len(rows)
+	if len(dest)+mv < dgxMinVarOrder {
+		return nil, nil, false
+	}
+	var frees []func()
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+	}()
+	pk, fk := cArray(m.Keys)
+	pw, fw := cArray(m.Words)
+	pt, ft := cArray(m.Tags)
+	frees = append(frees, fk, fw, ft)
+	leaf := []C.dgx_math_leaf{{key: (*C.uint64_t)(pk), word: (*C.uint64_t)(pw), tag: (*C.uint8_t)(pt),
+		n: C.size_t(len(m.Keys)), _type: C.DGX_VAL_INT64}}
+	pl, fl := cArray(leaf)
+	frees = append(frees, fl)
+	v, vOff := make([]uint64, 0, mv+1), make([]uint64, 1, nrows+1)
+	for _, r := range rows {
+		if r != nil {
+			v = append(v, r.Uids...)
+		}
+		vOff = append(vOff, uint64(len(v)))
+	}
+	d := append(make([]uint64, 0, len(dest)+1), dest...)
+	destOut, out, outOff := make([]uint64, len(dest)+1), make([]uint64, mv+1), make([]uint64, nrows+1)
+	var n C.size_t
+	isDesc := C.int(0)
+	if desc {
+		isDesc = 1
+	}
+	if C.dgx_var_order((*C.dgx_math_leaf)(pl), isDesc, u64ptr(d), C.size_t(len(dest)), u64ptr(v), u64ptr(vOff),
+		C.size_t(nrows), C.int32_t(count), C.int32_t(offset), u64ptr(out), u64ptr(outOff), C.size_t(mv),
+		u64ptr(destOut), C.size_t(len(dest)), &n) != C.DGX_OK {
+		return nil, nil, false
+	}
+	res := make([][]uint64, nrows)
+	for i := range res {
+		res[i] = out[outOff[i]:outOff[i+1]:outOff[i+1]]
+	}
+	return res, destOut[:n], true
+}

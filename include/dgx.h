@@ -714,6 +714,31 @@ int dgx_sg_filter(const dgx_sg_filter_tree* tree, const dgx_sg_filter_leaf* leav
                   uint64_t* dest_out, size_t dest_cap, size_t* dest_len, uint64_t* out, uint64_t* out_off,
                   size_t out_cap, uint32_t* counts);
 
+/* orderasc / orderdesc by a value variable (query/query.go applyOrderAndPagination :2511-2530, value-variable branch:
+ * updateUidMatrix's order branch :1425-1439, sortAndPaginateUsingVar :2697-2738 and updateDestUids :2594-2609), in
+ * Go's exact order.  dest is the node's DestUIDs after its filters (strictly ascending, e.g. dgx_sg_filter's new dest)
+ * and row i of its uid matrix is v[v_off[i] .. v_off[i+1]) (strictly ascending, v_off[0] == 0).  var is the variable's
+ * map as dgx_math_eval takes a leaf: a dgx_var_propagate / dgx_var_level_agg output (tag NULL, type DGX_VAL_INT64 or
+ * DGX_VAL_FLOAT64) or a dgx_math_eval output (one DGX_VAL_* tag per entry); var->nil is Go's nil map.
+ * Each row keeps, in row order, its uids in dest (U); W is U's uids with a map entry, in row order.  A row with an
+ * empty W stays U.  Otherwise it becomes W sorted by types.Sort(values, &uids, []bool{desc}, ""): sort.Sort(byValue),
+ * Go's pdqsort with its tie order, under byValue.Less (both nil: desc; one nil sorts last; equal values are not less,
+ * -0.0 equals +0.0 and a NaN is neither less nor equal; otherwise types.less, mismatchedLess between int and float or
+ * by Go's type id, negated for desc).  When count or offset is not 0 every row is then cut to x.PageRange(count,
+ * offset, len), a negative count taking items from the back.  The new dest is the dest values some row still holds.
+ * Writes the rows to out / out_off (nrows + 1 offsets) and the new dest to dest_out (*dest_len values).
+ * DGX_ERR_ARG before anything is copied: a nil map (Go's "used before definition"), a tagless map of another type,
+ * d_len set in the host form, var->n, ndest, nrows or v_off[nrows] of 2^32 or more, v_off not starting at 0 or
+ * decreasing, a null array that is needed.  DGX_ERR_CAP before anything is copied: out_cap below v_off[nrows] or
+ * dest_cap below ndest.  DGX_ERR_ARG after the kernels, with nothing written but *dest_len = 0: map keys, dest or a row
+ * not strictly ascending, an unknown entry tag, or a row whose first W entry is a bool (Go's "isn't sortable").
+ * ndest == 0 or nrows == 0 writes zero offsets and *dest_len = 0 and needs no device.
+ * Launches: 37 + 3 ceil(b_r / 8), b_r the bit width of nrows - 1 (DESIGN section 3.16), whatever the values, ties, map
+ * size and the rows' tiers. */
+int dgx_var_order(const dgx_math_leaf* var, int desc, const uint64_t* dest, size_t ndest, const uint64_t* v,
+                  const uint64_t* v_off, size_t nrows, int32_t count, int32_t offset, uint64_t* out, uint64_t* out_off,
+                  size_t out_cap, uint64_t* dest_out, size_t dest_cap, size_t* dest_len);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -1021,6 +1046,19 @@ int dgx_dev_sg_filter(dgx_lane* lane, const dgx_sg_filter_tree* tree, const dgx_
                       const uint64_t* d_v_off, size_t nrows, size_t v_cap, int32_t count, int32_t offset,
                       uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_dest_len, uint64_t* d_out,
                       uint64_t* d_out_off, size_t out_cap, uint32_t* d_counts);
+/* Device form of dgx_var_order: var is a host struct whose arrays are device memory (its d_len, when set, a device word
+ * whose low 32 bits hold the entry count, at most var->n), d_dest, the rows and the outputs are device memory, so
+ * dgx_dev_sg_filter's new dest and rows and a dgx_dev_var_propagate / dgx_dev_math_eval map feed it without a host read.
+ * |dest| is ndest, or the low 32 bits of the device word d_ndest when it is set (at most ndest).  v_cap is the room of
+ * d_v (d_v_off[nrows] must not pass it).  The bounds are v_cap and ndest: out_cap or dest_cap below them is DGX_ERR_CAP
+ * at the call, as every argument error of the host form is DGX_ERR_ARG there.  d_dest_len is one device uint64.  The
+ * order, offset and tag checks, a length word past its room and the bool refusal run on the device: a refused call
+ * writes *d_dest_len = 0 and nothing else, and surfaces as DGX_ERR_ARG at the next dgx_lane_sync.  ndest == 0 or
+ * nrows == 0 writes zero offsets and length without a launch.  Asynchronous on the lane; launches as the host form's. */
+int dgx_dev_var_order(dgx_lane* lane, const dgx_math_leaf* var, int desc, const uint64_t* d_dest, size_t ndest,
+                      const uint64_t* d_ndest, const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows,
+                      size_t v_cap, int32_t count, int32_t offset, uint64_t* d_out, uint64_t* d_out_off,
+                      size_t out_cap, uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_dest_len);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

@@ -624,6 +624,50 @@ inline MathResult EvalMath(const std::vector<dgx_math_node>& prog, const std::ve
     return out;
 }
 
+// The result of OrderByVar: the ordered and paged rows and the new DestUIDs.
+struct OrderResult {
+    std::vector<pb::List> rows;
+    pb::List dest;
+};
+
+namespace detail {
+inline OrderResult order_by_var(const dgx_math_leaf& leaf, bool desc, const pb::List& dest,
+                                const std::vector<pb::List>& rows, int32_t count, int32_t offset) {
+    std::vector<uint64_t> v, v_off{0};
+    for (const pb::List& r : rows) { v.insert(v.end(), r.Uids.begin(), r.Uids.end()); v_off.push_back(v.size()); }
+    const size_t nd = dest.Uids.size(), nrows = rows.size();
+    std::vector<uint64_t> out(std::max<size_t>(v.size(), 1)), out_off(nrows + 1), dout(std::max<size_t>(nd, 1));
+    size_t n = 0;
+    check(dgx_var_order(&leaf, desc ? 1 : 0, dest.Uids.data(), nd, v.data(), v_off.data(), nrows, count, offset,
+                        out.data(), out_off.data(), v.size(), dout.data(), nd, &n));
+    OrderResult res;
+    for (size_t r = 0; r < nrows; ++r)
+        res.rows.emplace_back(std::vector<uint64_t>(out.begin() + out_off[r], out.begin() + out_off[r + 1]));
+    res.dest = pb::List(std::vector<uint64_t>(dout.begin(), dout.begin() + n));
+    return res;
+}
+}  // namespace detail
+
+// orderasc / orderdesc by a value variable (query/query.go applyOrderAndPagination's value-variable branch:
+// updateUidMatrix, sortAndPaginateUsingVar with types.Sort and x.PageRange, updateDestUids) in one dgx_var_order call,
+// in Go's exact order, ties included.  dest: the node's DestUIDs after its filters; rows: its uidMatrix; count /
+// offset: Params.Count / Offset.  A PropagateVar / LevelAgg map, or a math() map (MathMap; nil is Go's nil map, which
+// the call refuses with DGX_ERR_ARG as Go returns an error).
+inline OrderResult OrderByVar(const ValueMap& m, bool desc, const pb::List& dest, const std::vector<pb::List>& rows,
+                              int32_t count = 0, int32_t offset = 0) {
+    if (m.keys.size() != m.words.size()) throw Error(DGX_ERR_ARG, "one word per key");
+    const dgx_math_leaf leaf{m.keys.data(), m.words.data(), nullptr, nullptr, m.keys.size(), m.type, 0};
+    return detail::order_by_var(leaf, desc, dest, rows, count, offset);
+}
+inline OrderResult OrderByVar(const MathMap& m, bool desc, const pb::List& dest, const std::vector<pb::List>& rows,
+                              int32_t count = 0, int32_t offset = 0) {
+    if (m.keys.size() != m.words.size() || m.keys.size() != m.tags.size())
+        throw Error(DGX_ERR_ARG, "one word and one tag per key");
+    const dgx_math_leaf leaf{m.keys.data(), m.words.data(), m.tags.data(), nullptr, m.nil ? 0 : m.keys.size(),
+                             DGX_VAL_INT64, m.nil ? 1 : 0};
+    return detail::order_by_var(leaf, desc, dest, rows, count, offset);
+}
+
 }  // namespace algo
 
 // Wire-format adjacency (dgx_wire_*, host only): the bytes proto.Unmarshal sees at posting/list.go:1045 and

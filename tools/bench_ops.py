@@ -145,6 +145,7 @@ def main():
     ap.add_argument("--c17-only", action="store_true", help="only the C17 value-variable rows")
     ap.add_argument("--c18-only", action="store_true", help="only the C18 math() rows")
     ap.add_argument("--c19-only", action="store_true", help="only the C19 @filter and first / offset rows")
+    ap.add_argument("--c20-only", action="store_true", help="only the C20 orderasc / orderdesc by a value variable rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -174,9 +175,11 @@ def main():
         rows = c18_rows(Lane())
     elif args.c19_only:
         rows = c19_rows(Lane())
+    elif args.c20_only:
+        rows = c20_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only or args.c20_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -1956,6 +1959,99 @@ def c19_rows(L):
                              "values": int(m), "check": bool(ok), "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del dleaf, d_d0, d_v, d_off, d_dest, d_out, d_oo, d_c
+    return out_rows
+
+
+def c20_rows(L):
+    """C20 "orderasc / orderdesc by a value variable".  C20a: C19a's matrix shape (10 000 rows, about 1e7 values over
+    1.2e7 uids), dest every row value but 3 %, an int map over about 90 % of dest with values in 0..99 (nearly every row
+    tier 2), orderdesc, first: 10.  C20b: the same matrix with a distinct-valued float map (every row tier 1).  C20c:
+    the root shape, one row of 3e6 uids: (i) distinct floats, orderdesc, first: 100; (ii) ints in 0..99, so one CTA's
+    pdqsort carries the call.  C20d: TestQueryVarValAggMul's size (launch-bound).  Legs: (1) the device form on
+    resident inputs (CUDA events), (2) the host form with its copies (wall clock), (3) the line-by-line restatement
+    (tests/var_order_oracle.c) on 1 thread -- C, not Go.  Every leg is checked against the restatement."""
+    import var_order_oracle as vo
+    from dgraph_b200 import algo
+
+    lib = L.lib
+    U64 = np.uint64
+    rng = np.random.default_rng(20)
+
+    def dp(t):
+        return t.data_ptr()
+
+    def up(x, dt=U64):
+        x = np.concatenate([np.ascontiguousarray(x, dt), np.zeros(1, dt)])
+        return torch.from_numpy(x.view(np.int64) if dt == U64 else x).to(DEV)
+
+    N = 12_000_000
+    lens = rng.integers(500, 1500, 10_000)
+    big_rows = [np.unique(rng.integers(1, N + 1, int(k)).astype(U64)) for k in lens]
+    allv = np.unique(np.concatenate(big_rows))
+    big_dest = allv[rng.random(allv.size) < 0.97]
+    mk = big_dest[rng.random(big_dest.size) < 0.9]
+    tied = (mk, rng.integers(0, 100, mk.size).astype(np.int64))
+    distinct = (mk, rng.permutation(mk.size).astype(np.float64) * 0.5 - 1e6)
+    root = np.sort(rng.choice(np.arange(1, 4_000_001, dtype=U64), 3_000_000, replace=False))
+    r_distinct = (root, rng.permutation(root.size).astype(np.float64) + 0.25)
+    r_tied = (root, rng.integers(0, 100, root.size).astype(np.int64))
+    fr = np.array([23, 24, 25, 31, 101], U64)
+    small = ((fr, np.array([15, 0, 0, 19, 0], np.int64)), True, fr, [fr], 0, 0)
+    work = (("C20a", (tied, True, big_dest, big_rows, 10, 0)), ("C20b", (distinct, True, big_dest, big_rows, 10, 0)),
+            ("C20c(i)", (r_distinct, True, root, [root], 100, 0)), ("C20c(ii)", (r_tied, False, root, [root], 0, 0)),
+            ("C20d", small))
+    out_rows = []
+    for name, case in work:
+        m, desc, dest, rows, count, offset = case
+        t0 = time.perf_counter()
+        want = vo.var_order(*case)
+        t_or = (time.perf_counter() - t0) * 1e3
+        off = np.zeros(len(rows) + 1, U64)
+        np.cumsum([len(r) for r in rows], out=off[1:])
+        v = np.concatenate([np.asarray(r, U64) for r in rows])
+        keys, vals = m
+        d_k, d_w = up(keys), up(np.ascontiguousarray(vals).view(U64))
+        typ = 1 if vals.dtype == np.int64 else 2
+        leaf = _lib.MathLeaf(dp(d_k), dp(d_w), None, None, keys.size, typ, 0)
+        d_dest, d_v, d_off = up(dest), up(v), up(off)
+        nd, nrows, M = dest.size, len(rows), v.size
+        d_out = torch.empty(M + 1, dtype=torch.int64, device=DEV)
+        d_oo = torch.empty(nrows + 1, dtype=torch.int64, device=DEV)
+        d_do = torch.empty(nd + 1, dtype=torch.int64, device=DEV)
+        d_len = torch.empty(1, dtype=torch.int64, device=DEV)
+
+        def dev():
+            _lib.check(lib.dgx_dev_var_order(L.h, C.byref(leaf), int(desc), dp(d_dest), nd, None, dp(d_v), dp(d_off),
+                                             nrows, M, count, offset, dp(d_out), dp(d_oo), M, dp(d_do), nd,
+                                             dp(d_len)))
+        ms_dev, _ = timeit(dev, warm=2, reps=10)
+        L.sync()
+        D = int(d_len.cpu().numpy()[0])
+        oo = d_oo.cpu().numpy().view(U64)
+        K = int(oo[nrows])
+        wv = np.concatenate(want[0] + [np.zeros(0, U64)])
+        woff = np.zeros(nrows + 1, U64)
+        np.cumsum([len(r) for r in want[0]], out=woff[1:])
+        ok_dev = (np.array_equal(d_do[:D].cpu().numpy().view(U64), want[1]) and np.array_equal(oo, woff) and
+                  np.array_equal(d_out[:K].cpu().numpy().view(U64), wv))
+        algo.OrderByVar(*case)
+        ts = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            got = algo.OrderByVar(*case)
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ok_host = np.array_equal(got[1].Uids, want[1]) and all(np.array_equal(a, b) for a, b in zip(got[0], want[0]))
+        full = (f"{name}: {nrows} rows of {M} values, |dest| {nd}, a {'float' if typ == 2 else 'int'} map of "
+                f"{keys.size} entries ({np.unique(vals).size} distinct values), {'orderdesc' if desc else 'orderasc'}"
+                f"{f', first {count}' if count else ''}; output values {K}, new dest {D}")
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev, "CUDA events, median of 10 after 2 warm"),
+                                    ("host form", float(np.median(ts)), ok_host, "wall clock, median of 3 after 1 warm"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, True, "orc_var_order, wall clock, one "
+                                     "run; the reference the other legs are checked against")):
+            out_rows.append({"op": "OrderByVar", "workload": name, "leg": leg, "config": full, "ms": round(ms, 4),
+                             "values": int(M), "check": bool(ok), "timing": timing})
+            print(json.dumps(out_rows[-1]), flush=True)
+        del d_k, d_w, d_dest, d_v, d_off, d_out, d_oo, d_do, d_len
     return out_rows
 
 
