@@ -87,6 +87,13 @@ class MathLeaf(C.Structure):
                 ("n", C.c_size_t), ("type", C.c_int), ("nil", C.c_int)]
 
 
+class StrColumn(C.Structure):
+    """dgx_str_column (include/dgx.h): a predicate's string values, uid i owning values val_off[i] .. val_off[i+1) and
+    value j the bytes byte_off[j] .. byte_off[j+1)."""
+    _fields_ = [("uid", C.c_void_p), ("val_off", C.c_void_p), ("byte_off", C.c_void_p), ("bytes", C.c_void_p),
+                ("n", C.c_size_t), ("nvals", C.c_size_t), ("nbytes", C.c_size_t)]
+
+
 class SgFilterTree(C.Structure):
     """dgx_sg_filter_tree (include/dgx.h): a subgraph's @filter tree, node 0 the root, parents below their children."""
     _fields_ = [("nnodes", C.c_size_t), ("op", C.c_void_p), ("parent", C.c_void_p), ("leaf", C.c_void_p)]
@@ -151,6 +158,8 @@ SYMBOLS = {
     "dgx_cascade": (_int, [C.POINTER(CascadeTree), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _sz]),
     "dgx_sg_filter": (_int, [C.POINTER(SgFilterTree), C.POINTER(SgFilterLeaf), _sz, _vp, _sz, _vp, _vp, _sz, C.c_int32,
                              C.c_int32, _vp, _sz, _szp, _vp, _vp, _sz, _vp]),
+    "dgx_match": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, C.POINTER(StrColumn), _vp,
+                         _sz, C.c_int64, _vp, _sz, _szp]),
     "dgx_var_order": (_int, [C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _sz, C.c_int32, C.c_int32, _vp, _vp, _sz,
                              _vp, _sz, _szp]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
@@ -203,6 +212,8 @@ SYMBOLS = {
     "dgx_dev_cascade": (_int, [_vp, C.POINTER(CascadeTree), C.POINTER(CascadeNode), _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
     "dgx_dev_sg_filter": (_int, [_vp, C.POINTER(SgFilterTree), C.POINTER(SgFilterLeaf), _sz, _vp, _sz, _vp, _vp, _vp,
                                  _sz, _sz, C.c_int32, C.c_int32, _vp, _sz, _vp, _vp, _vp, _sz, _vp]),
+    "dgx_dev_match": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _int, _vp, _sz, _vp,
+                             C.POINTER(StrColumn), _vp, _sz, C.c_int64, _vp, _sz, _vp]),
     "dgx_dev_var_order": (_int, [_vp, C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _vp, _sz, _sz, C.c_int32,
                                  C.c_int32, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),

@@ -955,6 +955,95 @@ def OrderByVar(m, desc: bool, dest, rows, count: int = 0, offset: int = 0):
     return [out[int(out_off[i]):int(out_off[i + 1])].copy() for i in range(nrows)], List(dout[:n.value].copy())
 
 
+class StrColumn:
+    """A string value column (dgx_str_column): the values Go's match loop reads for one predicate.  uids: strictly
+    ascending, the uids that have a value; values[i]: the values of uids[i], each bytes (any bytes, valid UTF-8 or
+    not) or a str (taken as UTF-8).  One value per uid is a scalar predicate, several a list predicate's."""
+
+    def __init__(self, uids, values):
+        self.uid = np.ascontiguousarray(np.asarray(uids, np.uint64).reshape(-1))
+        if len(values) != self.uid.size:
+            raise ValueError("one list of values per uid")
+        vals = [[v.encode() if isinstance(v, str) else bytes(v) for v in vs] for vs in values]
+        self.val_off = np.zeros(self.uid.size + 1, np.uint64)
+        np.cumsum([len(vs) for vs in vals], out=self.val_off[1:])
+        flat = [v for vs in vals for v in vs]
+        self.byte_off = np.zeros(len(flat) + 1, np.uint64)
+        np.cumsum([len(v) for v in flat], out=self.byte_off[1:])
+        self.bytes = np.frombuffer(b"".join(flat) or b"\0", np.uint8).copy()
+
+    @classmethod
+    def from_csr(cls, uid, val_off, byte_off, data) -> "StrColumn":
+        c = cls.__new__(cls)
+        c.uid, c.val_off, c.byte_off = (np.ascontiguousarray(np.asarray(a, np.uint64)) for a in (uid, val_off, byte_off))
+        d = np.ascontiguousarray(np.asarray(data, np.uint8))
+        c.bytes = d if d.size else np.zeros(1, np.uint8)
+        return c
+
+    def struct(self) -> "_lib.StrColumn":
+        n = self.uid.size
+        nv = self.byte_off.size - 1
+        return _lib.StrColumn(self.uid.ctypes.data if n else None, self.val_off.ctypes.data, self.byte_off.ctypes.data,
+                              self.bytes.ctypes.data, n, nv, int(self.byte_off[-1]))
+
+
+def _query_bytes(query) -> np.ndarray:
+    q = query.encode() if isinstance(query, str) else bytes(query)
+    return np.frombuffer(q + b"\0", np.uint8)[: len(q)].copy() if q else np.zeros(1, np.uint8)
+
+
+def MatchFuzzy(col: StrColumn, query, threshold: int, uids=None, leaves=(), afterUID: int = 0, keys=None) -> List:
+    """match(attr, query, threshold) (worker/task.go handleMatchFunction, worker/match.go uidsForMatch / matchFuzzy) in ONE
+    call (dgx_match): the candidates' values tested on the device with Go's []rune Levenshtein distance.
+
+    col: the predicate's StrColumn, holding the values Go reads (Value, ValueForTag or AllUntaggedValues).  query: str
+    or bytes.  uids: the filter's UidList (ascending); when it is empty or None the candidates are the union of the
+    query's trigram rows, leaves as algo.UidsForRegex takes them (pack leaves (pack, mut) or lists) read from afterUID.
+    keys: optional [(key, version)] per leaf naming the pack leaves for the HBM-resident cache.  Returns the kept
+    candidates."""
+    u = np.zeros(0, np.uint64) if uids is None else _u64(uids.Uids if isinstance(uids, List) else uids)
+    pack_ids = [j for j, lf in enumerate(leaves) if isinstance(lf, tuple)]
+    list_ids = [j for j, lf in enumerate(leaves) if not isinstance(lf, tuple)]
+    packs = [leaves[j][0] for j in pack_ids]
+    mut_uids, mut_flags, mut_off = _mut_csr([leaves[j][1] for j in pack_ids])
+    arrs = [_u64(leaves[j].Uids if isinstance(leaves[j], List) else leaves[j]) for j in list_ids]
+    list_off = np.zeros(len(arrs) + 1, dtype=np.uint64)
+    np.cumsum([a.size for a in arrs], out=list_off[1:])
+    lists = np.concatenate(arrs) if int(list_off[-1]) else np.zeros(1, np.uint64)
+    refs, keep = _refs_of(packs, [keys[j] for j in pack_ids] if keys is not None else None)
+    cap = u.size if u.size else sum((_exact(p) if p is not None else 0) + int(mut_off[k + 1] - mut_off[k])
+                                    for k, p in enumerate(packs)) + int(list_off[-1])
+    q = _query_bytes(query)
+    qlen = len(query.encode() if isinstance(query, str) else bytes(query))
+    cs = col.struct()
+    out = np.empty(max(cap, 1), dtype=np.uint64)
+    n = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_match(refs, len(packs), _p(mut_uids), _p(mut_flags), _p(mut_off), _p(lists),
+                                     _p(list_off), len(arrs), afterUID, _p(u) if u.size else None, u.size,
+                                     C.byref(cs), _p(q), qlen, threshold, _p(out), cap, C.byref(n)))
+    return List(out[: n.value].copy())
+
+
+def dev_match(lane, dcol: "_lib.StrColumn", query, threshold: int, d_out: int, out_cap: int, d_out_len: int,
+              d_uids: int | None = None, nuids: int = 0, d_nuids: int | None = None, packs=(), d_mut_uids=None,
+              d_mut_flags=None, mut_off=None, d_lists=None, list_off=None, afterUID: int = 0) -> None:
+    """The lane form of MatchFuzzy (dgx_dev_match), asynchronous: every pointer argument is a device address.
+
+    dcol: a StrColumn struct whose arrays are device memory (a resident column).  d_uids given: the UidList branch,
+    its count nuids or the low 32 bits of the device word d_nuids (at most nuids); an empty list is an empty result.
+    Otherwise the trigram branch: packs are dgx_dev_pack_upload handles, the layers and lists device arrays with host
+    offsets mut_off / list_off.  Writes the kept uids to d_out and their count to the device word d_out_len; a
+    malformed input surfaces at the next dgx_lane_sync."""
+    tab = (C.c_void_p * max(len(packs), 1))(*packs)
+    mo = np.zeros(1, np.uint64) if mut_off is None else np.ascontiguousarray(np.asarray(mut_off, np.uint64))
+    lo = np.zeros(1, np.uint64) if list_off is None else np.ascontiguousarray(np.asarray(list_off, np.uint64))
+    q = _query_bytes(query)
+    qlen = len(query.encode() if isinstance(query, str) else bytes(query))
+    _lib.check(_lib.load().dgx_dev_match(lane, tab, len(packs), d_mut_uids, d_mut_flags, _p(mo), d_lists, _p(lo),
+                                         lo.size - 1, afterUID, int(d_uids is not None), d_uids, nuids, d_nuids,
+                                         C.byref(dcol), _p(q), qlen, threshold, d_out, out_cap, d_out_len))
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -47,6 +47,7 @@
 #include "math_kernel.cuh"
 #include "sg_filter_kernel.cuh"
 #include "var_order_kernel.cuh"
+#include "match_kernel.cuh"
 #include "wire.hpp"
 #include "ws_layout.hpp"
 
@@ -554,6 +555,10 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
                                      "ascending, row offsets not starting at 0, decreasing or past v_cap, a length word "
                                      "past its room, an unknown entry tag, or a row whose first mapped entry is a bool, "
                                      "which Go refuses as not sortable)");
+        if (flag & kLaneErrMatch)
+            return fail(DGX_ERR_ARG, "a match() input is malformed (candidates or column uids not strictly ascending, "
+                                     "column offsets not starting at 0, decreasing or not ending at nvals / nbytes, or "
+                                     "a length word past its room)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -6109,6 +6114,303 @@ extern "C" int dgx_trigram_query(const dgx_query_tree* tree, const dgx_pack_ref*
                       d_out + 8, T.dcap, d_out);
     if (rc) return rc;
     return ps.synced(finish_to_host(l, d_out, d_out + 8, T.dcap, out, out_cap, out_len));
+}
+
+// ---------------------------------------------------------------------------
+// match(): handleMatchFunction's candidates tested with matchFuzzy against a string value column (match_kernel.cuh)
+// ---------------------------------------------------------------------------
+constexpr uint64_t kFz32 = uint64_t(1) << 32;     // candidates, column uids, values and bytes are 32-bit counts
+constexpr size_t kFzMaxRunes = 64 * FZ_MAX_WORDS;  // the longest query: the long tier holds its words in registers
+static_assert(kFzMaxRunes == DGX_MATCH_MAX_RUNES, "include/dgx.h states the query limit");
+
+// utf8.DecodeRuneInString over p[i .. len), as fz_decode on the device.
+static uint32_t fz_host_decode(const uint8_t* p, size_t len, size_t i, uint32_t* r) {
+    const uint32_t b0 = p[i];
+    if (b0 < 0x80) { *r = b0; return 1; }
+    *r = FZ_FFFD;
+    if (b0 < 0xC2 || b0 > 0xF4) return 1;
+    const uint32_t need = b0 < 0xE0 ? 1 : (b0 < 0xF0 ? 2 : 3);
+    if (i + need >= len) return 1;
+    uint32_t lo = 0x80, hi = 0xBF;
+    if (b0 == 0xE0) lo = 0xA0;
+    else if (b0 == 0xED) hi = 0x9F;
+    else if (b0 == 0xF0) lo = 0x90;
+    else if (b0 == 0xF4) hi = 0x8F;
+    if (p[i + 1] < lo || p[i + 1] > hi) return 1;
+    for (uint32_t k = 2; k <= need; ++k)
+        if (p[i + k] < 0x80 || p[i + k] > 0xBF) return 1;
+    uint32_t v = b0 & (need == 1 ? 0x1F : need == 2 ? 0x0F : 0x07);
+    for (uint32_t k = 1; k <= need; ++k) v = (v << 6) | (p[i + k] & 0x3F);
+    *r = v;
+    return need + 1;
+}
+
+// The query's Peq rows (128 ASCII rows, then one per distinct other rune in ascending order; W words each), from its
+// runes as Go's []rune(query) gives them.
+struct FzQuery {
+    std::vector<uint64_t> peq;
+    std::vector<uint32_t> other;
+    uint32_t m = 0, W = 1, max = 0;
+};
+
+static int fz_query(const uint8_t* q, size_t qlen, int64_t max, FzQuery* Q) {
+    if (max < 0 || max > INT32_MAX) return fail(DGX_ERR_ARG, "max is %lld: a non-negative int32", (long long)max);
+    if (qlen && !q) return fail(DGX_ERR_ARG, "null query");
+    std::vector<uint32_t> runes;
+    for (size_t i = 0; i < qlen;) {
+        if (runes.size() == kFzMaxRunes) return fail(DGX_ERR_ARG, "the query has more than %zu runes", kFzMaxRunes);
+        uint32_t r;
+        i += fz_host_decode(q, qlen, i, &r);
+        runes.push_back(r);
+    }
+    Q->m = (uint32_t)runes.size();
+    Q->W = std::max<uint32_t>(1, (Q->m + 63) / 64);
+    Q->max = (uint32_t)max;
+    for (uint32_t r : runes)
+        if (r >= 128) Q->other.push_back(r);
+    std::sort(Q->other.begin(), Q->other.end());
+    Q->other.erase(std::unique(Q->other.begin(), Q->other.end()), Q->other.end());
+    Q->peq.assign((128 + Q->other.size()) * Q->W, 0);
+    for (uint32_t i = 0; i < Q->m; ++i) {
+        const uint32_t r = runes[i];
+        const size_t row = r < 128 ? r : 128 + (std::lower_bound(Q->other.begin(), Q->other.end(), r) - Q->other.begin());
+        Q->peq[row * Q->W + i / 64] |= uint64_t(1) << (i % 64);
+    }
+    return DGX_OK;
+}
+
+// The column's checks before anything is copied; the host form also checks its offsets (the device form's are checked
+// by fz_lookup_kernel).
+static int fz_check_column(const dgx_str_column* c, bool host) {
+    if (!c) return fail(DGX_ERR_ARG, "null column");
+    if (c->n >= kFz32 || c->nvals >= kFz32 || c->nbytes >= kFz32)
+        return fail(DGX_ERR_ARG, "column sizes are 32-bit: n %zu, nvals %zu, nbytes %zu", c->n, c->nvals, c->nbytes);
+    if (!c->val_off || !c->byte_off || (c->n && !c->uid) || (c->nbytes && !c->bytes))
+        return fail(DGX_ERR_ARG, "null column array");
+    if (!host) return DGX_OK;
+    if (int rc = check_offsets("val_off", c->val_off, c->n, kFz32)) return rc;
+    if (c->val_off[c->n] != c->nvals)
+        return fail(DGX_ERR_ARG, "val_off[n] is %llu, not nvals (%zu)", (unsigned long long)c->val_off[c->n], c->nvals);
+    if (int rc = check_offsets("byte_off", c->byte_off, c->nvals, kFz32)) return rc;
+    if (c->byte_off[c->nvals] != c->nbytes)
+        return fail(DGX_ERR_ARG, "byte_off[nvals] is %llu, not nbytes (%zu)", (unsigned long long)c->byte_off[c->nvals],
+                    c->nbytes);
+    return DGX_OK;
+}
+
+// uidsForMatch's trigram rows: one OR node over every leaf, planned by the trigram query's checks.
+struct FzTree {
+    uint8_t op = DGX_QOR;
+    uint32_t leaf_off[2] = {0, 0}, sub_off[2] = {0, 0};
+    std::vector<uint32_t> leaf_idx;
+    dgx_query_tree t{};
+    explicit FzTree(size_t nleaves) : leaf_idx(std::max<size_t>(nleaves, 1)) {
+        for (size_t i = 0; i < nleaves; ++i) leaf_idx[i] = (uint32_t)i;
+        leaf_off[1] = (uint32_t)std::min<size_t>(nleaves, 0xFFFFFFFFu);
+        t = dgx_query_tree{1, &op, leaf_off, leaf_idx.data(), sub_off, nullptr};
+    }
+};
+
+// The test of ccap candidate slots (cand, with the count in the low 32 bits of *cand_len, or ccap when it is null) on
+// the lane: 5 launches whatever the candidates, the column, the value lengths and max.  Workspace: Peq, 8 per column
+// value (the long-tier queue) and about 33 per candidate slot (value counts, first values, pair offsets, keep flags,
+// the look-back words).  col's arrays are device memory.
+static int fz_run(dgx_lane* l, const FzQuery& Q, const uint64_t* cand, const uint64_t* cand_len, uint64_t ccap,
+                  const dgx_str_column& col, uint64_t* d_out, uint64_t* d_out_len) {
+    FzParams P{};
+    uint64_t* h_peq;
+    uint32_t* h_other;
+    u64* status;
+    u32* tickets;
+    const uint64_t st = scan_tiles(ccap), kt = (ccap + CP_TILE - 1) / CP_TILE;
+    WsCarve ws(l);
+    ws.copied(&P.peq, &h_peq, Q.peq.size());
+    ws.copied(&P.other, &h_other, std::max<size_t>(Q.other.size(), 1));
+    if (int rc = ws.stage()) return rc;
+    memcpy(h_peq, Q.peq.data(), Q.peq.size() * sizeof(uint64_t));
+    h_other[0] = 0;
+    if (!Q.other.empty()) memcpy(h_other, Q.other.data(), Q.other.size() * sizeof(uint32_t));
+    ws.zeroed(&P.words, 4);
+    ws.zeroed(&tickets, 4);
+    ws.zeroed(&status, st + kt);
+    ws.zeroed(&P.keep, ccap);
+    ws.plain(&P.cnt, ccap);
+    ws.plain(&P.vlo, ccap);
+    ws.plain(&P.pair_off, ccap + 1);
+    ws.plain(&P.longq, std::max<size_t>(col.nvals, 1));
+    if (int rc = ws.commit()) return rc;
+    P.cand = (const u64*)cand;
+    P.cand_len = (const u64*)cand_len;
+    P.ccap = ccap;
+    P.uid = (const u64*)col.uid;
+    P.val_off = (const u64*)col.val_off;
+    P.byte_off = (const u64*)col.byte_off;
+    P.bytes = col.bytes;
+    P.n = col.n;
+    P.nvals = col.nvals;
+    P.nbytes = col.nbytes;
+    P.nd = (u32)Q.other.size();
+    P.W = Q.W;
+    P.m = Q.m;
+    P.max = Q.max;
+    P.err = l->d_err;
+    fz_lookup_kernel<<<gb_grid(std::max<uint64_t>({ccap, col.n + 1, col.nvals + 1})), 256, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)st, EN_NT, 0, l->stream>>>(P.cnt, P.pair_off, P.words + FZ_W_N, ccap, status, tickets,
+                                                            P.words + FZ_W_PAIRS);
+    fz_test_kernel<<<gb_grid(col.nvals), 256, 0, l->stream>>>(P);
+    fz_long_kernel<<<(unsigned)(2 * g_num_sms), FZ_LONG_NT, 0, l->stream>>>(P);
+    CompactParams K;
+    K.v = (const u64*)cand;
+    K.keep = P.keep;
+    K.m = ccap;
+    K.out = (u64*)d_out;
+    K.out_cap = ccap;
+    K.out_len = (u64*)d_out_len;
+    K.status = status + st;
+    K.ticket = tickets + 1;
+    K.err = l->d_err;
+    compact_kernel<<<(unsigned)kt, CP_NT, 0, l->stream>>>(K);
+    CK(cudaGetLastError());
+    count_launches(l, 5);
+    return DGX_OK;
+}
+
+// The trigram branch's candidates on the lane: the one-OR plan's pipeline into a carved buffer of T.dcap values.
+static int fz_trigram_candidates(dgx_lane* l, const TgPlan& T, const dgx_dev_pack* const* packs, size_t npacks,
+                                 const uint64_t* d_mut, const uint8_t* d_flags, const uint64_t* mut_off,
+                                 const uint64_t* d_lists, const uint64_t* list_off, size_t nlists, uint64_t after,
+                                 uint64_t** cand, uint64_t** cand_len) {
+    WsCarve c(l);
+    c.plain(cand_len, 1);
+    c.plain(cand, T.dcap + 2);
+    if (int rc = c.commit()) return rc;
+    return trigram_impl(l, T, packs, npacks, d_mut, d_flags, mut_off, d_lists, list_off, nlists, after, *cand, T.dcap,
+                        *cand_len);
+}
+
+extern "C" int dgx_dev_match(dgx_lane* l, const dgx_dev_pack* const* packs, size_t npacks, const uint64_t* d_mut_uids,
+                             const uint8_t* d_mut_flags, const uint64_t* mut_off, const uint64_t* d_lists,
+                             const uint64_t* list_off, size_t nlists, uint64_t after_uid, int use_uids,
+                             const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids, const dgx_str_column* col,
+                             const uint8_t* query, size_t query_len, int64_t max, uint64_t* d_out, size_t out_cap,
+                             uint64_t* d_out_len) {
+    if (!l || !d_out_len) return fail(DGX_ERR_ARG, "null argument");
+    FzQuery Q;
+    if (int rc = fz_query(query, query_len, max, &Q)) return rc;
+    if (int rc = fz_check_column(col, false)) return rc;
+    TgPlan T;
+    FzTree tree(npacks + nlists);
+    uint64_t bound;
+    if (use_uids) {
+        if (nuids >= kFz32) return fail(DGX_ERR_ARG, "nuids %zu: at most 2^32 - 1", nuids);
+        if (nuids && !d_uids) return fail(DGX_ERR_ARG, "null argument");
+        bound = nuids;
+    } else {
+        if (int rc = tg_check(&tree.t, packs, npacks, mut_off, d_mut_uids, d_mut_flags, list_off, nlists, &T)) return rc;
+        if (T.root_bound && nlists && list_off[nlists] && !d_lists) return fail(DGX_ERR_ARG, "null argument");
+        bound = T.root_bound;
+    }
+    if (out_cap < bound)
+        return fail(DGX_ERR_CAP, "out_cap (%zu) is below the candidates' bound (%llu)", out_cap,
+                    (unsigned long long)bound);
+    if (bound && !d_out) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_out_len, sizeof(uint64_t));
+    if (bound == 0) {  // no candidate: an empty UidList room, or no trigram row
+        CK(cudaMemsetAsync(d_out_len, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    const uint64_t* cand = d_uids;
+    const uint64_t* cand_len = d_nuids;
+    if (!use_uids) {
+        uint64_t *c, *cl;
+        if (int rc = fz_trigram_candidates(l, T, packs, npacks, d_mut_uids, d_mut_flags, mut_off, d_lists, list_off,
+                                           nlists, after_uid, &c, &cl))
+            return rc;
+        cand = c;
+        cand_len = cl;
+    }
+    if (int rc = fz_run(l, Q, cand, cand_len, bound, *col, d_out, d_out_len)) return rc;
+    g_stats.uids_in += bound;
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids, const uint8_t* mut_flags,
+                         const uint64_t* mut_off, const uint64_t* lists, const uint64_t* list_off, size_t nlists,
+                         uint64_t after_uid, const uint64_t* uids, size_t nuids, const dgx_str_column* col,
+                         const uint8_t* query, size_t query_len, int64_t max, uint64_t* out, size_t out_cap,
+                         size_t* out_len) {
+    if (!out_len) return fail(DGX_ERR_ARG, "null out_len");
+    FzQuery Q;
+    if (int rc = fz_query(query, query_len, max, &Q)) return rc;
+    if (int rc = fz_check_column(col, true)) return rc;
+    const bool use_uids = nuids > 0;  // handleMatchFunction: a non-empty UidList is the candidates
+    TgPlan T;
+    FzTree tree(npacks + nlists);
+    uint64_t bound, nmut = 0, nlist = 0;
+    if (use_uids) {
+        if (nuids >= kFz32) return fail(DGX_ERR_ARG, "nuids %zu: at most 2^32 - 1", nuids);
+        if (!uids) return fail(DGX_ERR_ARG, "null argument");
+        bound = nuids;
+    } else {
+        if (int rc = tg_check(&tree.t, refs, npacks, mut_off, mut_uids, mut_flags, list_off, nlists, &T)) return rc;
+        nmut = npacks ? mut_off[npacks] : 0;
+        nlist = nlists ? list_off[nlists] : 0;
+        for (uint64_t k = 0; k < nmut; ++k)
+            if (mut_flags[k] & DGX_MUT_VALUE)
+                return fail(DGX_ERR_ARG, "mutable entry %llu is not a REF posting", (unsigned long long)k);
+        if (T.root_bound && nlist && !lists) return fail(DGX_ERR_ARG, "null argument");
+        bound = T.root_bound;
+    }
+    if (out_cap < bound)
+        return fail(DGX_ERR_CAP, "out_cap (%zu) is below the candidates' bound (%llu)", out_cap,
+                    (unsigned long long)bound);
+    if (bound && !out) return fail(DGX_ERR_ARG, "null argument");
+    if (bound == 0) { *out_len = 0; return DGX_OK; }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += bound;
+    int rc;
+    dgx_str_column D = *col;  // one copy of each column array
+    uint64_t *d_uid, *d_voff, *d_boff;
+    if ((rc = upload_list(l, col->uid, col->n, &d_uid)) || (rc = upload_list(l, col->val_off, col->n + 1, &d_voff)) ||
+        (rc = upload_list(l, col->byte_off, col->nvals + 1, &d_boff)))
+        return rc;
+    void* b;
+    if ((rc = l->ws.alloc(col->nbytes + 16, &b))) return rc;
+    if (col->nbytes) CK(cudaMemcpyAsync(b, col->bytes, col->nbytes, cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += col->nbytes;
+    D.uid = d_uid;
+    D.val_off = d_voff;
+    D.byte_off = d_boff;
+    D.bytes = (const uint8_t*)b;
+    void* p;
+    if ((rc = l->ws.alloc((bound + 10) * sizeof(uint64_t), &p))) return rc;  // the length word, then the values
+    uint64_t* d_out = (uint64_t*)p;
+    if (use_uids) {
+        uint64_t* d_uids;
+        if ((rc = upload_list(l, uids, nuids, &d_uids))) return rc;
+        if ((rc = fz_run(l, Q, d_uids, nullptr, bound, D, d_out + 8, d_out))) return rc;
+        if ((rc = finish_to_host(l, d_out, d_out + 8, bound, out, out_cap, out_len))) *out_len = 0;
+        return rc;
+    }
+    PackSet ps(l, refs, npacks);  // nil / empty packs are packs of no blocks
+    if (ps.rc) return ps.rc;
+    const std::vector<const dgx_dev_pack*> rows = ps.rows();
+    uint64_t *d_mut = nullptr, *d_lists, *cand, *cand_len;
+    const uint8_t* d_flags = nullptr;
+    if (npacks && (rc = upload_mut_layers(l, mut_uids, mut_flags, nmut, &d_mut, &d_flags))) return rc;
+    if ((rc = upload_list(l, lists, nlist, &d_lists))) return rc;
+    if ((rc = fz_trigram_candidates(l, T, rows.data(), npacks, d_mut, d_flags, mut_off, d_lists, list_off, nlists,
+                                    after_uid, &cand, &cand_len)))
+        return rc;
+    if ((rc = fz_run(l, Q, cand, cand_len, bound, D, d_out + 8, d_out))) return rc;
+    if ((rc = ps.synced(finish_to_host(l, d_out, d_out + 8, bound, out, out_cap, out_len)))) *out_len = 0;
+    return rc;
 }
 
 extern "C" uint64_t dgx_merge_matrix_overflows(const dgx_lane* l) { return l ? l->xm_overflows : g_xm_overflows.load(); }

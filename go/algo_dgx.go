@@ -1081,3 +1081,75 @@ func OrderByVar(m MathLeaf, desc bool, dest []uint64, rows []*pb.List, count, of
 	}
 	return res, destOut[:n], true
 }
+
+// dgxMinMatch: below this many candidates a match() stays in Go (handleMatchFunction).  The C21 record
+// (profiles/h100_c21_match.json) times the library against a C restatement of that loop, not against Go, so this is
+// the dgxMinMergeMatrix bound until a Go comparison sets it.
+const dgxMinMatch = dgxMinMergeMatrix
+
+// StrColumn is a predicate's string values as handleMatchFunction reads them at ReadTs: Uids strictly ascending,
+// Vals[i] the values of Uids[i] from the same choice Go's loop makes (pl.ValueForTag(lang) with a lang,
+// pl.AllUntaggedValues for a list predicate, pl.Value otherwise); a uid whose read is ErrNoValue is left out.
+type StrColumn struct {
+	Uids []uint64
+	Vals [][][]byte
+}
+
+// MatchFuzzy runs handleMatchFunction's candidate loop (worker/task.go:1526-1620) in one call: the candidates are
+// uids when it is not empty (the filter's UidList), otherwise the union of rows, uidsForMatch's pl.Uids reads of the
+// query's trigram tokens (worker/match.go:72-100), and a candidate is kept when one of its values passes
+// matchFuzzy(query, val, max).  It returns the kept uids, the task's one UidMatrix row.  ok == false -- max outside
+// int32 or negative, a query above DGX_MATCH_MAX_RUNES runes, fewer than dgxMinMatch candidates, sizes outside the
+// library's bounds (DGX_ERR_ARG / DGX_ERR_CAP) or any other library error -- means the caller keeps Go's loop.
+func MatchFuzzy(col *StrColumn, query string, max int64, uids []uint64, rows [][]uint64) ([]uint64, bool) {
+	bound := len(uids)
+	if bound == 0 {
+		for _, r := range rows {
+			bound += len(r)
+		}
+	}
+	if bound < dgxMinMatch || len(col.Uids) != len(col.Vals) {
+		return nil, false
+	}
+	valOff, byteOff := make([]uint64, 1, len(col.Uids)+1), make([]uint64, 1, len(col.Uids)+1)
+	var data []byte
+	for _, vs := range col.Vals {
+		for _, v := range vs {
+			data = append(data, v...)
+			byteOff = append(byteOff, uint64(len(data)))
+		}
+		valOff = append(valOff, uint64(len(byteOff)-1))
+	}
+	var frees []func()
+	defer func() {
+		for _, f := range frees {
+			f()
+		}
+	}()
+	// the column struct holds pointers, so it and every array it names live in C memory (cgo's pointer rules)
+	pu, fu := cArray(col.Uids)
+	pv, fv := cArray(valOff)
+	pbo, fbo := cArray(byteOff)
+	pd, fd := cArray(data)
+	pq, fq := cArray([]byte(query))
+	frees = append(frees, fu, fv, fbo, fd, fq)
+	pc, fc := cArray([]C.dgx_str_column{{uid: (*C.uint64_t)(pu), val_off: (*C.uint64_t)(pv),
+		byte_off: (*C.uint64_t)(pbo), bytes: (*C.uint8_t)(pd), n: C.size_t(len(col.Uids)),
+		nvals: C.size_t(len(byteOff) - 1), nbytes: C.size_t(len(data))}})
+	frees = append(frees, fc)
+	lists, listOff := make([]uint64, 0, bound+1), make([]uint64, 1, len(rows)+1)
+	if len(uids) == 0 {
+		for _, r := range rows {
+			lists = append(lists, r...)
+			listOff = append(listOff, uint64(len(lists)))
+		}
+	}
+	out := make([]uint64, bound+1)
+	var n C.size_t
+	if C.dgx_match(nil, 0, nil, nil, nil, u64ptr(lists), u64ptr(listOff), C.size_t(len(listOff)-1), 0,
+		u64ptr(uids), C.size_t(len(uids)), (*C.dgx_str_column)(pc), (*C.uint8_t)(pq), C.size_t(len(query)), C.int64_t(max),
+		u64ptr(out), C.size_t(bound), &n) != C.DGX_OK {
+		return nil, false
+	}
+	return out[:n:n], true
+}

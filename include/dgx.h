@@ -739,6 +739,46 @@ int dgx_var_order(const dgx_math_leaf* var, int desc, const uint64_t* dest, size
                   const uint64_t* v_off, size_t nrows, int32_t count, int32_t offset, uint64_t* out, uint64_t* out_off,
                   size_t out_cap, uint64_t* dest_out, size_t dest_cap, size_t* dest_len);
 
+/* A string value column: the values Go's loop reads at ReadTs for one predicate, built by the caller.  uid[0 .. n) are
+ * strictly ascending, the uids that have a value; uid i owns values val_off[i] .. val_off[i+1) (n + 1 offsets,
+ * val_off[0] == 0, val_off[n] == nvals); value j is bytes[byte_off[j] .. byte_off[j+1]) (nvals + 1 offsets,
+ * byte_off[0] == 0, byte_off[nvals] == nbytes), any bytes, valid UTF-8 or not.  A uid that is absent has no value
+ * (posting.ErrNoValue); a uid with several values is a list predicate's.  The column may hold more uids than a call's
+ * candidates: one column per predicate can stay resident across calls until the predicate changes. */
+typedef struct dgx_str_column {
+    const uint64_t* uid;
+    const uint64_t* val_off;
+    const uint64_t* byte_off;
+    const uint8_t* bytes;
+    size_t n;
+    size_t nvals;
+    size_t nbytes;
+} dgx_str_column;
+
+/* The longest query dgx_match takes, in runes. */
+#define DGX_MATCH_MAX_RUNES 4096
+
+/* match(attr, query, max) (worker/task.go handleMatchFunction :1526-1620, uidsForMatch and matchFuzzy /
+ * levenshteinDistance in worker/match.go :24-100).  The candidates are uids[0 .. nuids) when nuids > 0 (the filter's
+ * UidList, strictly ascending); otherwise the union of every trigram row, the leaves taken exactly as
+ * dgx_trigram_query takes them (refs / npacks with their layers, list leaves, after_uid) under one OR: uidsForMatch's
+ * List.Uids reads with First = MaxInt32 and algo.MergeSorted.  No leaf (a query shorter than 3 bytes) is no candidate.
+ * A candidate is kept when one of its values in col is not empty and lies within max edits of the query, the
+ * unit-cost edit distance between Go's []rune conversions of both (an invalid UTF-8 byte is one U+FFFD, equal to a
+ * genuine U+FFFD).  Writes the kept candidates in ascending order to out (*out_len values).
+ * DGX_ERR_ARG before anything is copied: max < 0 or above 2^31 - 1; a query of more than DGX_MATCH_MAX_RUNES runes;
+ * nuids, col->n, col->nvals, col->nbytes or the leaves' bounds of 2^32 or more; column offsets not starting at 0,
+ * decreasing or not ending at nvals / nbytes; a null array that is needed; the layer errors of
+ * dgx_list_uids_unfiltered_rows, a DGX_MUT_VALUE entry included.  DGX_ERR_CAP before anything is copied: out_cap
+ * below the candidates' bound (nuids, or the sum of the leaves' bounds).  DGX_ERR_ARG after the kernels, with
+ * nothing written but *out_len = 0: candidates or column uids not strictly ascending.
+ * Launches: 5, after the trigram stages of dgx_trigram_query for one OR node in the trigram branch, whatever the
+ * candidates, the column, the value lengths and max (DESIGN section 3.17). */
+int dgx_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids, const uint8_t* mut_flags,
+              const uint64_t* mut_off, const uint64_t* lists, const uint64_t* list_off, size_t nlists,
+              uint64_t after_uid, const uint64_t* uids, size_t nuids, const dgx_str_column* col, const uint8_t* query,
+              size_t query_len, int64_t max, uint64_t* out, size_t out_cap, size_t* out_len);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -1059,6 +1099,23 @@ int dgx_dev_var_order(dgx_lane* lane, const dgx_math_leaf* var, int desc, const 
                       const uint64_t* d_ndest, const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows,
                       size_t v_cap, int32_t count, int32_t offset, uint64_t* d_out, uint64_t* d_out_off,
                       size_t out_cap, uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_dest_len);
+/* Device form of dgx_match: packs from dgx_dev_pack_upload; the layers, list leaves, d_uids, col's arrays and the
+ * outputs are device memory; mut_off, list_off and the query stay in host memory, as in dgx_dev_trigram_query.  The
+ * caller picks the branch: use_uids != 0 takes d_uids, whose count is the low 32 bits of the device word d_nuids (at
+ * most nuids, the room; d_nuids NULL: exactly nuids), so dgx_dev_sg_filter's D1, dgx_dev_merge_sorted_matrix,
+ * dgx_dev_trigram_query or a previous dgx_dev_match feed it without a host read.  Go's query layer never sends an
+ * empty UidList to a filter, so here an empty list is an empty result.  use_uids == 0 takes the trigram leaves.  The
+ * bound is nuids or the sum of the leaves' bounds: out_cap below it is DGX_ERR_CAP at the call, as every argument
+ * error of the host form is DGX_ERR_ARG there, except the column's offsets, which are checked on the device.
+ * d_out_len is one device uint64.  The order and offset checks, a count word past its room and a DGX_MUT_VALUE entry
+ * are found on the device: a refused call writes *d_out_len = 0 and nothing else, and surfaces as DGX_ERR_ARG at the
+ * next dgx_lane_sync.  A bound of 0 writes a zero length without a launch.  Asynchronous on the lane; launches as the
+ * host form's. */
+int dgx_dev_match(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t npacks, const uint64_t* d_mut_uids,
+                  const uint8_t* d_mut_flags, const uint64_t* mut_off, const uint64_t* d_lists,
+                  const uint64_t* list_off, size_t nlists, uint64_t after_uid, int use_uids, const uint64_t* d_uids,
+                  size_t nuids, const uint64_t* d_nuids, const dgx_str_column* col, const uint8_t* query,
+                  size_t query_len, int64_t max, uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

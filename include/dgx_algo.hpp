@@ -668,6 +668,41 @@ inline OrderResult OrderByVar(const MathMap& m, bool desc, const pb::List& dest,
     return detail::order_by_var(leaf, desc, dest, rows, count, offset);
 }
 
+// A predicate's string values for MatchFuzzy: uids strictly ascending, vals[i] the values of uids[i] as Go's match
+// loop reads them (Value, ValueForTag or AllUntaggedValues); a uid without a value is left out.
+struct StrColumn {
+    std::vector<uint64_t> uids;
+    std::vector<std::vector<std::string>> vals;
+};
+
+// match(attr, query, max) (worker/task.go handleMatchFunction, worker/match.go uidsForMatch / matchFuzzy) in one
+// dgx_match call: the candidates are uids when it is not empty (the filter's UidList), otherwise the union of rows,
+// the query's trigram rows as pl.Uids read them; a candidate is kept when one of its values is within max edits of
+// the query over Go's []rune conversion.  Returns the kept candidates.
+inline pb::List MatchFuzzy(const StrColumn& col, const std::string& query, int64_t max, const pb::List& uids,
+                           const std::vector<pb::List>& rows = {}) {
+    if (col.uids.size() != col.vals.size()) throw Error(DGX_ERR_ARG, "one list of values per uid");
+    std::vector<uint64_t> val_off{0}, byte_off{0};
+    std::string data;
+    for (const auto& vs : col.vals) {
+        for (const std::string& v : vs) { data += v; byte_off.push_back(data.size()); }
+        val_off.push_back(byte_off.size() - 1);
+    }
+    const dgx_str_column c{col.uids.data(), val_off.data(), byte_off.data(), (const uint8_t*)data.data(),
+                           col.uids.size(), byte_off.size() - 1, data.size()};
+    std::vector<uint64_t> lists, list_off{0};
+    if (uids.Uids.empty())
+        for (const pb::List& r : rows) { lists.insert(lists.end(), r.Uids.begin(), r.Uids.end()); list_off.push_back(lists.size()); }
+    const size_t bound = uids.Uids.empty() ? lists.size() : uids.Uids.size();
+    std::vector<uint64_t> out(std::max<size_t>(bound, 1));
+    size_t n = 0;
+    check(dgx_match(nullptr, 0, nullptr, nullptr, nullptr, lists.data(), list_off.data(), list_off.size() - 1, 0,
+                    uids.Uids.data(), uids.Uids.size(), &c, (const uint8_t*)query.data(), query.size(), max,
+                    out.data(), bound, &n));
+    out.resize(n);
+    return pb::List(out);
+}
+
 }  // namespace algo
 
 // Wire-format adjacency (dgx_wire_*, host only): the bytes proto.Unmarshal sees at posting/list.go:1045 and

@@ -146,6 +146,7 @@ def main():
     ap.add_argument("--c18-only", action="store_true", help="only the C18 math() rows")
     ap.add_argument("--c19-only", action="store_true", help="only the C19 @filter and first / offset rows")
     ap.add_argument("--c20-only", action="store_true", help="only the C20 orderasc / orderdesc by a value variable rows")
+    ap.add_argument("--c21-only", action="store_true", help="only the C21 match() rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -177,9 +178,11 @@ def main():
         rows = c19_rows(Lane())
     elif args.c20_only:
         rows = c20_rows(Lane())
+    elif args.c21_only:
+        rows = c21_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only or args.c20_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only or args.c20_only or args.c21_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -2052,6 +2055,93 @@ def c20_rows(L):
                              "values": int(M), "check": bool(ok), "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del d_k, d_w, d_dest, d_v, d_off, d_out, d_oo, d_do, d_len
+    return out_rows
+
+
+def c21_rows(L):
+    """C21 "match()": handleMatchFunction's candidates tested against a string value column.  C21a: a name-like column
+    of 1e7 uids (5-20 bytes, some multi-byte), a UidList of 3e6 of them, "alice" with max 2 (short tier).  C21b: the
+    trigram branch, 6 synthetic trigram rows (list leaves) over C21a's column whose union is about 1e6 candidates, an
+    8-byte query, max 3.  C21c: 1e5 text values of 1-4 KB, a 40-rune query, max 8: the short tier, where the length
+    shortcut decides every pair.  C21e: 1e5 values each up to 30 edits from a 110-rune (120-byte) query, max 20:
+    the long tier (warp per pair), every pair decided by the distance.  C21d: TestMatchFuncWithAfterWithValidUid's
+    size (launch-bound).  Legs: (1) the device form on resident inputs (CUDA events; the column, candidates or rows
+    already on the device), (2) the host form with its copies (wall clock), (3) the line-by-line restatement
+    (tests/match_oracle.c) on 1 thread -- C, not Go.  Every leg is checked against the restatement."""
+    import gen_match as gm
+    import match_cases as mc
+    import match_oracle as mo
+    from dgraph_b200 import algo
+
+    U64 = np.uint64
+    rng = np.random.default_rng(21)
+
+    def up(x, dt=U64):
+        x = np.concatenate([np.ascontiguousarray(x, dt), np.zeros(1, dt)])
+        return torch.from_numpy(x.view(np.int64) if dt == U64 else x).to(DEV)
+
+    names = gm.name_column(rng, 10_000_000)
+    cands = np.sort(rng.choice(names.uid, 3_000_000, replace=False))
+    rows = [np.sort(rng.choice(names.uid, 170_000, replace=False)) for _ in range(6)]
+    text = gm.text_column(rng, 100_000, 1024, 4096)
+    q40 = "the graph caf\u00e9 query node \u20ac index abc edge of a graph"[:40]
+    q120 = ("graph query node caf\u00e9 \u20ac edge " * 6).encode()[:120]
+    near = gm.text_column(rng, 100_000, 0, 0, base=q120, edits=30)
+    g, cols = mc.golden()
+    gu, gv = cols["name"]
+    small = mc.column(gu, gv)
+    ali = np.array(sorted(u for u, (v,) in zip(gu, gv) if b"Ali" in v and u > 0x2710), U64)
+    work = [("C21a", names, "alice", 2, cands, []), ("C21b", names, "aliceros", 3, None, rows),
+            ("C21c", text, q40, 8, text.uid, []), ("C21e", near, q120, 20, near.uid, []),
+            ("C21d", small, "Ali", 5, None, [ali])]
+    out_rows = []
+    for name, col, query, mx, uids, leaves in work:
+        t0 = time.perf_counter()
+        want = mo.match(col, query, mx, uids=uids, leaves=leaves)
+        t_or = (time.perf_counter() - t0) * 1e3
+        dt = [up(col.uid), up(col.val_off), up(col.byte_off), up(col.bytes, np.uint8)]
+        dcol = _lib.StrColumn(dt[0].data_ptr(), dt[1].data_ptr(), dt[2].data_ptr(), dt[3].data_ptr(), col.uid.size,
+                              int(col.byte_off.size - 1), int(col.byte_off[-1]))
+        if uids is not None:
+            d_u = up(uids)
+            cap = int(uids.size)
+            kw = dict(d_uids=d_u.data_ptr(), nuids=cap)
+        else:
+            lo = np.zeros(len(leaves) + 1, U64)
+            np.cumsum([r.size for r in leaves], out=lo[1:])
+            d_l = up(np.concatenate(leaves))
+            cap = int(lo[-1])
+            kw = dict(d_lists=d_l.data_ptr(), list_off=lo)
+        d_out = torch.empty(cap + 1, dtype=torch.int64, device=DEV)
+        d_len = torch.empty(1, dtype=torch.int64, device=DEV)
+
+        def dev():
+            algo.dev_match(L.h, dcol, query, mx, d_out.data_ptr(), cap, d_len.data_ptr(), **kw)
+        ms_dev, _ = timeit(dev, warm=2, reps=10)
+        L.sync()
+        k = int(d_len.cpu().numpy()[0])
+        ok_dev = np.array_equal(d_out[:k].cpu().numpy().view(U64), want)
+        host_kw = dict(uids=uids) if uids is not None else dict(leaves=leaves)
+        algo.MatchFuzzy(col, query, mx, **host_kw)
+        ts = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            got = algo.MatchFuzzy(col, query, mx, **host_kw)
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ok_host = np.array_equal(got.Uids, want)
+        nv = int(col.byte_off.size - 1)
+        full = (f"{name}: column of {col.uid.size} uids, {nv} values, {int(col.byte_off[-1])} bytes; "
+                f"{'UidList of %d' % cap if uids is not None else '%d trigram rows, %d uids' % (len(leaves), cap)}; "
+                f"query of {len(gm.runes(query.encode() if isinstance(query, str) else query))} runes, max {mx}; "
+                f"kept {want.size}")
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev, "CUDA events, median of 10 after 2 warm"),
+                                    ("host form", float(np.median(ts)), ok_host, "wall clock, median of 3 after 1 warm"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, True, "orc_match, wall clock, one run; "
+                                     "the reference the other legs are checked against")):
+            out_rows.append({"op": "MatchFuzzy", "workload": name, "leg": leg, "config": full, "ms": round(ms, 4),
+                             "candidates": cap, "check": bool(ok), "timing": timing})
+            print(json.dumps(out_rows[-1]), flush=True)
+        del dt, d_out, d_len
     return out_rows
 
 
