@@ -160,6 +160,11 @@ SYMBOLS = {
                              C.c_int32, _vp, _sz, _szp, _vp, _vp, _sz, _vp]),
     "dgx_match": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz, C.POINTER(StrColumn), _vp,
                          _sz, C.c_int64, _vp, _sz, _szp]),
+    "dgx_regex_compile": (_int, [_vp, _sz, _int, C.POINTER(_vp)]),
+    "dgx_regex_free": (None, [_vp]),
+    "dgx_regex_tables": (_int, [_vp, _szp, _szp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp)]),
+    "dgx_regex_match": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz,
+                               C.POINTER(StrColumn), _vp, _vp, _sz, _szp]),
     "dgx_var_order": (_int, [C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _sz, C.c_int32, C.c_int32, _vp, _vp, _sz,
                              _vp, _sz, _szp]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
@@ -214,6 +219,8 @@ SYMBOLS = {
                                  _sz, _sz, C.c_int32, C.c_int32, _vp, _sz, _vp, _vp, _vp, _sz, _vp]),
     "dgx_dev_match": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _int, _vp, _sz, _vp,
                              C.POINTER(StrColumn), _vp, _sz, C.c_int64, _vp, _sz, _vp]),
+    "dgx_dev_regex_match": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _int, _vp, _sz, _vp,
+                                   C.POINTER(StrColumn), _vp, _vp, _sz, _vp]),
     "dgx_dev_var_order": (_int, [_vp, C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _vp, _sz, _sz, C.c_int32,
                                  C.c_int32, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),

@@ -1044,6 +1044,75 @@ def dev_match(lane, dcol: "_lib.StrColumn", query, threshold: int, d_out: int, o
                                          C.byref(dcol), _p(q), qlen, threshold, d_out, out_cap, d_out_len))
 
 
+class RegexProg:
+    """regexp()'s pattern compiled for MatchRegex (dgx_regex_compile): Go's "(?m)" + pattern as codesearch matches it,
+    one line at a time, as a byte DFA.  fold: the /i modifier.  Raises DgxError (DGX_ERR_ARG) for a pattern outside the
+    compiled subset or one Go rejects, and (DGX_ERR_CAP) for a DFA past DGX_REGEX_MAX_STATES states; a caller then
+    keeps its own matcher."""
+
+    def __init__(self, pattern, fold: bool = False):
+        p = pattern.encode() if isinstance(pattern, str) else bytes(pattern)
+        buf = np.frombuffer(p + b"\0", np.uint8)
+        h = C.c_void_p()
+        _lib.check(_lib.load().dgx_regex_compile(_p(buf), len(p), 1 if fold else 0, C.byref(h)))
+        self.handle = h.value
+
+    def __del__(self):
+        if getattr(self, "handle", None):
+            _lib.load().dgx_regex_free(self.handle)
+            self.handle = None
+
+    def tables(self):
+        """(cls[256], trans[nstates, nclasses], term[nstates]) copies of the compiled tables."""
+        ns, nc = C.c_size_t(), C.c_size_t()
+        cp, tp, mp = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        _lib.check(_lib.load().dgx_regex_tables(self.handle, C.byref(ns), C.byref(nc), C.byref(cp), C.byref(tp),
+                                                C.byref(mp)))
+        n, k = ns.value, nc.value
+        cls = np.ctypeslib.as_array(C.cast(cp, C.POINTER(C.c_uint8)), (256,)).copy()
+        trans = np.ctypeslib.as_array(C.cast(tp, C.POINTER(C.c_uint16)), (n * k,)).reshape(n, k).copy()
+        term = np.ctypeslib.as_array(C.cast(mp, C.POINTER(C.c_uint8)), (n,)).copy()
+        return cls, trans, term
+
+
+def MatchRegex(col: StrColumn, prog: RegexProg, uids=None, leaves=(), afterUID: int = 0, keys=None) -> List:
+    """regexp(attr, /pattern/) (worker/task.go handleRegexFunction, matchRegex) in ONE call (dgx_regex_match): the
+    candidates' values tested on the device with the compiled program.  Candidates as MatchFuzzy takes them: uids (the
+    filter's UidList) when not empty, otherwise the union of leaves read from afterUID.  Returns the kept candidates."""
+    u = np.zeros(0, np.uint64) if uids is None else _u64(uids.Uids if isinstance(uids, List) else uids)
+    pack_ids = [j for j, lf in enumerate(leaves) if isinstance(lf, tuple)]
+    list_ids = [j for j, lf in enumerate(leaves) if not isinstance(lf, tuple)]
+    packs = [leaves[j][0] for j in pack_ids]
+    mut_uids, mut_flags, mut_off = _mut_csr([leaves[j][1] for j in pack_ids])
+    arrs = [_u64(leaves[j].Uids if isinstance(leaves[j], List) else leaves[j]) for j in list_ids]
+    list_off = np.zeros(len(arrs) + 1, dtype=np.uint64)
+    np.cumsum([a.size for a in arrs], out=list_off[1:])
+    lists = np.concatenate(arrs) if int(list_off[-1]) else np.zeros(1, np.uint64)
+    refs, keep = _refs_of(packs, [keys[j] for j in pack_ids] if keys is not None else None)
+    cap = u.size if u.size else sum((_exact(p) if p is not None else 0) + int(mut_off[k + 1] - mut_off[k])
+                                    for k, p in enumerate(packs)) + int(list_off[-1])
+    cs = col.struct()
+    out = np.empty(max(cap, 1), dtype=np.uint64)
+    n = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_regex_match(refs, len(packs), _p(mut_uids), _p(mut_flags), _p(mut_off), _p(lists),
+                                           _p(list_off), len(arrs), afterUID, _p(u) if u.size else None, u.size,
+                                           C.byref(cs), prog.handle, _p(out), cap, C.byref(n)))
+    return List(out[: n.value].copy())
+
+
+def dev_match_regex(lane, dcol: "_lib.StrColumn", prog: RegexProg, d_out: int, out_cap: int, d_out_len: int,
+                    d_uids: int | None = None, nuids: int = 0, d_nuids: int | None = None, packs=(), d_mut_uids=None,
+                    d_mut_flags=None, mut_off=None, d_lists=None, list_off=None, afterUID: int = 0) -> None:
+    """The lane form of MatchRegex (dgx_dev_regex_match), asynchronous, with dev_match's arguments and prog in place of
+    the query and threshold."""
+    tab = (C.c_void_p * max(len(packs), 1))(*packs)
+    mo = np.zeros(1, np.uint64) if mut_off is None else np.ascontiguousarray(np.asarray(mut_off, np.uint64))
+    lo = np.zeros(1, np.uint64) if list_off is None else np.ascontiguousarray(np.asarray(list_off, np.uint64))
+    _lib.check(_lib.load().dgx_dev_regex_match(lane, tab, len(packs), d_mut_uids, d_mut_flags, _p(mo), d_lists,
+                                               _p(lo), lo.size - 1, afterUID, int(d_uids is not None), d_uids, nuids,
+                                               d_nuids, C.byref(dcol), prog.handle, d_out, out_cap, d_out_len))
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

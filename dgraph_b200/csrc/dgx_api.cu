@@ -48,6 +48,8 @@
 #include "sg_filter_kernel.cuh"
 #include "var_order_kernel.cuh"
 #include "match_kernel.cuh"
+#include "regex_kernel.cuh"
+#include "regex_compile.hpp"
 #include "wire.hpp"
 #include "ws_layout.hpp"
 
@@ -558,7 +560,7 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
         if (flag & kLaneErrMatch)
             return fail(DGX_ERR_ARG, "a match() input is malformed (candidates or column uids not strictly ascending, "
                                      "column offsets not starting at 0, decreasing or not ending at nvals / nbytes, or "
-                                     "a length word past its room)");
+                                     "a length word past its room; regexp()'s value test shares these checks)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -6288,15 +6290,14 @@ static int fz_trigram_candidates(dgx_lane* l, const TgPlan& T, const dgx_dev_pac
                         *cand_len);
 }
 
-extern "C" int dgx_dev_match(dgx_lane* l, const dgx_dev_pack* const* packs, size_t npacks, const uint64_t* d_mut_uids,
-                             const uint8_t* d_mut_flags, const uint64_t* mut_off, const uint64_t* d_lists,
-                             const uint64_t* list_off, size_t nlists, uint64_t after_uid, int use_uids,
-                             const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids, const dgx_str_column* col,
-                             const uint8_t* query, size_t query_len, int64_t max, uint64_t* d_out, size_t out_cap,
-                             uint64_t* d_out_len) {
-    if (!l || !d_out_len) return fail(DGX_ERR_ARG, "null argument");
-    FzQuery Q;
-    if (int rc = fz_query(query, query_len, max, &Q)) return rc;
+// The candidates of a value-column test (match(), regexp()) on the lane, then run(l, cand, cand_len, bound, col, d_out,
+// d_out_len), the test's own stages.  The argument checks and refusals are dgx_dev_match's.
+template <class Run>
+static int str_test_dev(dgx_lane* l, const dgx_dev_pack* const* packs, size_t npacks, const uint64_t* d_mut_uids,
+                        const uint8_t* d_mut_flags, const uint64_t* mut_off, const uint64_t* d_lists,
+                        const uint64_t* list_off, size_t nlists, uint64_t after_uid, int use_uids,
+                        const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids, const dgx_str_column* col,
+                        uint64_t* d_out, size_t out_cap, uint64_t* d_out_len, const Run& run) {
     if (int rc = fz_check_column(col, false)) return rc;
     TgPlan T;
     FzTree tree(npacks + nlists);
@@ -6331,22 +6332,20 @@ extern "C" int dgx_dev_match(dgx_lane* l, const dgx_dev_pack* const* packs, size
         cand = c;
         cand_len = cl;
     }
-    if (int rc = fz_run(l, Q, cand, cand_len, bound, *col, d_out, d_out_len)) return rc;
+    if (int rc = run(l, cand, cand_len, bound, *col, d_out, d_out_len)) return rc;
     g_stats.uids_in += bound;
     l->note_output(d_out, out_cap * sizeof(uint64_t));
     return DGX_OK;
 }
 
-extern "C" int dgx_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids, const uint8_t* mut_flags,
+// The host form's driver: dgx_match's checks, uploads and branches around run.
+template <class Run>
+static int str_test_host(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids, const uint8_t* mut_flags,
                          const uint64_t* mut_off, const uint64_t* lists, const uint64_t* list_off, size_t nlists,
                          uint64_t after_uid, const uint64_t* uids, size_t nuids, const dgx_str_column* col,
-                         const uint8_t* query, size_t query_len, int64_t max, uint64_t* out, size_t out_cap,
-                         size_t* out_len) {
-    if (!out_len) return fail(DGX_ERR_ARG, "null out_len");
-    FzQuery Q;
-    if (int rc = fz_query(query, query_len, max, &Q)) return rc;
+                         uint64_t* out, size_t out_cap, size_t* out_len, const Run& run) {
     if (int rc = fz_check_column(col, true)) return rc;
-    const bool use_uids = nuids > 0;  // handleMatchFunction: a non-empty UidList is the candidates
+    const bool use_uids = nuids > 0;  // handleMatchFunction / handleRegexFunction: a non-empty UidList is the candidates
     TgPlan T;
     FzTree tree(npacks + nlists);
     uint64_t bound, nmut = 0, nlist = 0;
@@ -6394,7 +6393,7 @@ extern "C" int dgx_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t
     if (use_uids) {
         uint64_t* d_uids;
         if ((rc = upload_list(l, uids, nuids, &d_uids))) return rc;
-        if ((rc = fz_run(l, Q, d_uids, nullptr, bound, D, d_out + 8, d_out))) return rc;
+        if ((rc = run(l, d_uids, nullptr, bound, D, d_out + 8, d_out))) return rc;
         if ((rc = finish_to_host(l, d_out, d_out + 8, bound, out, out_cap, out_len))) *out_len = 0;
         return rc;
     }
@@ -6408,9 +6407,179 @@ extern "C" int dgx_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t
     if ((rc = fz_trigram_candidates(l, T, rows.data(), npacks, d_mut, d_flags, mut_off, d_lists, list_off, nlists,
                                     after_uid, &cand, &cand_len)))
         return rc;
-    if ((rc = fz_run(l, Q, cand, cand_len, bound, D, d_out + 8, d_out))) return rc;
+    if ((rc = run(l, cand, cand_len, bound, D, d_out + 8, d_out))) return rc;
     if ((rc = ps.synced(finish_to_host(l, d_out, d_out + 8, bound, out, out_cap, out_len)))) *out_len = 0;
     return rc;
+}
+
+extern "C" int dgx_dev_match(dgx_lane* l, const dgx_dev_pack* const* packs, size_t npacks, const uint64_t* d_mut_uids,
+                             const uint8_t* d_mut_flags, const uint64_t* mut_off, const uint64_t* d_lists,
+                             const uint64_t* list_off, size_t nlists, uint64_t after_uid, int use_uids,
+                             const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids, const dgx_str_column* col,
+                             const uint8_t* query, size_t query_len, int64_t max, uint64_t* d_out, size_t out_cap,
+                             uint64_t* d_out_len) {
+    if (!l || !d_out_len) return fail(DGX_ERR_ARG, "null argument");
+    FzQuery Q;
+    if (int rc = fz_query(query, query_len, max, &Q)) return rc;
+    return str_test_dev(l, packs, npacks, d_mut_uids, d_mut_flags, mut_off, d_lists, list_off, nlists, after_uid,
+                        use_uids, d_uids, nuids, d_nuids, col, d_out, out_cap, d_out_len,
+                        [&](dgx_lane* ln, const uint64_t* c, const uint64_t* cl, uint64_t bound,
+                            const dgx_str_column& D, uint64_t* o, uint64_t* ol) {
+                            return fz_run(ln, Q, c, cl, bound, D, o, ol);
+                        });
+}
+
+extern "C" int dgx_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids, const uint8_t* mut_flags,
+                         const uint64_t* mut_off, const uint64_t* lists, const uint64_t* list_off, size_t nlists,
+                         uint64_t after_uid, const uint64_t* uids, size_t nuids, const dgx_str_column* col,
+                         const uint8_t* query, size_t query_len, int64_t max, uint64_t* out, size_t out_cap,
+                         size_t* out_len) {
+    if (!out_len) return fail(DGX_ERR_ARG, "null out_len");
+    FzQuery Q;
+    if (int rc = fz_query(query, query_len, max, &Q)) return rc;
+    return str_test_host(refs, npacks, mut_uids, mut_flags, mut_off, lists, list_off, nlists, after_uid, uids, nuids,
+                         col, out, out_cap, out_len,
+                         [&](dgx_lane* ln, const uint64_t* c, const uint64_t* cl, uint64_t bound,
+                             const dgx_str_column& D, uint64_t* o, uint64_t* ol) {
+                             return fz_run(ln, Q, c, cl, bound, D, o, ol);
+                         });
+}
+
+// ---------------------------------------------------------------------------
+// regexp(): handleRegexFunction's candidates tested with matchRegex against a string value column (regex_kernel.cuh)
+// ---------------------------------------------------------------------------
+static_assert(rx::kMaxStates == DGX_REGEX_MAX_STATES, "include/dgx.h states the state cap");
+static_assert(rx::kTermAbsorb == RX_ABSORB && rx::kTermAccept == RX_ACCEPT && rx::kStartText == RX_START,
+              "regex_kernel.cuh reads the compiler's state numbering");
+
+struct dgx_regex_prog {
+    rx::Prog p;
+};
+
+extern "C" int dgx_regex_compile(const char* pattern, size_t len, int flags, dgx_regex_prog** prog) {
+    if (!prog || (len && !pattern)) return fail(DGX_ERR_ARG, "null argument");
+    *prog = nullptr;
+    if (flags & ~DGX_REGEX_FOLD) return fail(DGX_ERR_ARG, "unknown regex flags %d", flags);
+    dgx_regex_prog* r = new dgx_regex_prog;
+    const int rc = rx::compile((const uint8_t*)pattern, len, (flags & DGX_REGEX_FOLD) != 0, &r->p);
+    if (rc != rx::kOK) delete r;
+    if (rc == rx::kRefuse) return fail(DGX_ERR_ARG, "the pattern is outside the compiled subset or invalid");
+    if (rc == rx::kTooBig)
+        return fail(DGX_ERR_CAP, "the pattern's DFA exceeds %d states (or its byte NFA %d nodes)", rx::kMaxStates,
+                    rx::kMaxNfa);
+    *prog = r;
+    return DGX_OK;
+}
+
+extern "C" void dgx_regex_free(dgx_regex_prog* prog) { delete prog; }
+
+extern "C" int dgx_regex_tables(const dgx_regex_prog* prog, size_t* nstates, size_t* nclasses, const uint8_t** cls,
+                                const uint16_t** trans, const uint8_t** term) {
+    if (!prog || !nstates || !nclasses || !cls || !trans || !term) return fail(DGX_ERR_ARG, "null argument");
+    *nstates = prog->p.nstates;
+    *nclasses = prog->p.nclasses;
+    *cls = prog->p.cls;
+    *trans = prog->p.trans.data();
+    *term = prog->p.term.data();
+    return DGX_OK;
+}
+
+// The test of ccap candidate slots on the lane: 5 launches whatever the candidates, the column, the value lengths and
+// the program.  Workspace: the program's tables, 8 per column value (the warp tier's queue) and about 33 per candidate
+// slot.  col's arrays are device memory.
+static int rx_run(dgx_lane* l, const rx::Prog& R, const uint64_t* cand, const uint64_t* cand_len, uint64_t ccap,
+                  const dgx_str_column& col, uint64_t* d_out, uint64_t* d_out_len) {
+    RxParams P{};
+    FzParams& F = P.F;
+    unsigned char *h_cls, *h_term;
+    uint16_t* h_trans;
+    u64* status;
+    u32* tickets;
+    const uint64_t st = scan_tiles(ccap), kt = (ccap + CP_TILE - 1) / CP_TILE;
+    WsCarve ws(l);
+    ws.copied(&P.cls, &h_cls, 256);
+    ws.copied(&P.trans, &h_trans, R.trans.size());
+    ws.copied(&P.term, &h_term, R.term.size());
+    if (int rc = ws.stage()) return rc;
+    memcpy(h_cls, R.cls, 256);
+    memcpy(h_trans, R.trans.data(), R.trans.size() * sizeof(uint16_t));
+    memcpy(h_term, R.term.data(), R.term.size());
+    ws.zeroed(&F.words, 4);
+    ws.zeroed(&tickets, 4);
+    ws.zeroed(&status, st + kt);
+    ws.zeroed(&F.keep, ccap);
+    ws.plain(&F.cnt, ccap);
+    ws.plain(&F.vlo, ccap);
+    ws.plain(&F.pair_off, ccap + 1);
+    ws.plain(&F.longq, std::max<size_t>(col.nvals, 1));
+    if (int rc = ws.commit()) return rc;
+    F.cand = (const u64*)cand;
+    F.cand_len = (const u64*)cand_len;
+    F.ccap = ccap;
+    F.uid = (const u64*)col.uid;
+    F.val_off = (const u64*)col.val_off;
+    F.byte_off = (const u64*)col.byte_off;
+    F.bytes = col.bytes;
+    F.n = col.n;
+    F.nvals = col.nvals;
+    F.nbytes = col.nbytes;
+    F.err = l->d_err;
+    P.nstates = R.nstates;
+    P.nclasses = R.nclasses;
+    P.warp = R.nstates <= (uint32_t)RX_WARP_STATES;
+    const size_t smem = ((size_t)R.nstates * R.nclasses * 2 + 15) / 16 * 16 + 256 + R.nstates;
+    const unsigned tgrid = (unsigned)std::min<uint64_t>(gb_grid(col.nvals), 8ull * g_num_sms);
+    fz_lookup_kernel<<<gb_grid(std::max<uint64_t>({ccap, col.n + 1, col.nvals + 1})), 256, 0, l->stream>>>(F);
+    scan_u64_kernel<<<(unsigned)st, EN_NT, 0, l->stream>>>(F.cnt, F.pair_off, F.words + FZ_W_N, ccap, status, tickets,
+                                                            F.words + FZ_W_PAIRS);
+    if (R.trans.size() * 2 <= RX_SMEM_TABLE && smem <= 48 * 1024)
+        rx_test_kernel<true><<<tgrid, RX_NT, smem, l->stream>>>(P);
+    else
+        rx_test_kernel<false><<<tgrid, RX_NT, 0, l->stream>>>(P);
+    rx_long_kernel<<<(unsigned)(2 * g_num_sms), RX_NT, 0, l->stream>>>(P);
+    CompactParams K;
+    K.v = (const u64*)cand;
+    K.keep = F.keep;
+    K.m = ccap;
+    K.out = (u64*)d_out;
+    K.out_cap = ccap;
+    K.out_len = (u64*)d_out_len;
+    K.status = status + st;
+    K.ticket = tickets + 1;
+    K.err = l->d_err;
+    compact_kernel<<<(unsigned)kt, CP_NT, 0, l->stream>>>(K);
+    CK(cudaGetLastError());
+    count_launches(l, 5);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_regex_match(dgx_lane* l, const dgx_dev_pack* const* packs, size_t npacks,
+                                   const uint64_t* d_mut_uids, const uint8_t* d_mut_flags, const uint64_t* mut_off,
+                                   const uint64_t* d_lists, const uint64_t* list_off, size_t nlists, uint64_t after_uid,
+                                   int use_uids, const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids,
+                                   const dgx_str_column* col, const dgx_regex_prog* prog, uint64_t* d_out,
+                                   size_t out_cap, uint64_t* d_out_len) {
+    if (!l || !d_out_len || !prog) return fail(DGX_ERR_ARG, "null argument");
+    return str_test_dev(l, packs, npacks, d_mut_uids, d_mut_flags, mut_off, d_lists, list_off, nlists, after_uid,
+                        use_uids, d_uids, nuids, d_nuids, col, d_out, out_cap, d_out_len,
+                        [&](dgx_lane* ln, const uint64_t* c, const uint64_t* cl, uint64_t bound,
+                            const dgx_str_column& D, uint64_t* o, uint64_t* ol) {
+                            return rx_run(ln, prog->p, c, cl, bound, D, o, ol);
+                        });
+}
+
+extern "C" int dgx_regex_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids,
+                               const uint8_t* mut_flags, const uint64_t* mut_off, const uint64_t* lists,
+                               const uint64_t* list_off, size_t nlists, uint64_t after_uid, const uint64_t* uids,
+                               size_t nuids, const dgx_str_column* col, const dgx_regex_prog* prog, uint64_t* out,
+                               size_t out_cap, size_t* out_len) {
+    if (!out_len || !prog) return fail(DGX_ERR_ARG, "null argument");
+    return str_test_host(refs, npacks, mut_uids, mut_flags, mut_off, lists, list_off, nlists, after_uid, uids, nuids,
+                         col, out, out_cap, out_len,
+                         [&](dgx_lane* ln, const uint64_t* c, const uint64_t* cl, uint64_t bound,
+                             const dgx_str_column& D, uint64_t* o, uint64_t* ol) {
+                             return rx_run(ln, prog->p, c, cl, bound, D, o, ol);
+                         });
 }
 
 extern "C" uint64_t dgx_merge_matrix_overflows(const dgx_lane* l) { return l ? l->xm_overflows : g_xm_overflows.load(); }

@@ -1111,6 +1111,24 @@ func MatchFuzzy(col *StrColumn, query string, max int64, uids []uint64, rows [][
 	if bound < dgxMinMatch || len(col.Uids) != len(col.Vals) {
 		return nil, false
 	}
+	pc, free := cStrColumn(col)
+	defer free()
+	pq, fq := cArray([]byte(query))
+	defer fq()
+	lists, listOff := candidateRows(uids, rows, bound)
+	out := make([]uint64, bound+1)
+	var n C.size_t
+	if C.dgx_match(nil, 0, nil, nil, nil, u64ptr(lists), u64ptr(listOff), C.size_t(len(listOff)-1), 0,
+		u64ptr(uids), C.size_t(len(uids)), (*C.dgx_str_column)(pc), (*C.uint8_t)(pq), C.size_t(len(query)), C.int64_t(max),
+		u64ptr(out), C.size_t(bound), &n) != C.DGX_OK {
+		return nil, false
+	}
+	return out[:n:n], true
+}
+
+// cStrColumn copies col into C memory as a dgx_str_column: the struct holds pointers, so it and every array it names
+// live in C memory (cgo's pointer rules).  The caller calls free when the library is done with it.
+func cStrColumn(col *StrColumn) (unsafe.Pointer, func()) {
 	valOff, byteOff := make([]uint64, 1, len(col.Uids)+1), make([]uint64, 1, len(col.Uids)+1)
 	var data []byte
 	for _, vs := range col.Vals {
@@ -1120,23 +1138,19 @@ func MatchFuzzy(col *StrColumn, query string, max int64, uids []uint64, rows [][
 		}
 		valOff = append(valOff, uint64(len(byteOff)-1))
 	}
-	var frees []func()
-	defer func() {
-		for _, f := range frees {
-			f()
-		}
-	}()
-	// the column struct holds pointers, so it and every array it names live in C memory (cgo's pointer rules)
 	pu, fu := cArray(col.Uids)
 	pv, fv := cArray(valOff)
 	pbo, fbo := cArray(byteOff)
 	pd, fd := cArray(data)
-	pq, fq := cArray([]byte(query))
-	frees = append(frees, fu, fv, fbo, fd, fq)
 	pc, fc := cArray([]C.dgx_str_column{{uid: (*C.uint64_t)(pu), val_off: (*C.uint64_t)(pv),
 		byte_off: (*C.uint64_t)(pbo), bytes: (*C.uint8_t)(pd), n: C.size_t(len(col.Uids)),
 		nvals: C.size_t(len(byteOff) - 1), nbytes: C.size_t(len(data))}})
-	frees = append(frees, fc)
+	return pc, func() { fc(); fd(); fbo(); fv(); fu() }
+}
+
+// candidateRows lays rows out as list leaves when uids is empty (the trigram branch), as dgx_match and
+// dgx_regex_match take them.
+func candidateRows(uids []uint64, rows [][]uint64, bound int) ([]uint64, []uint64) {
 	lists, listOff := make([]uint64, 0, bound+1), make([]uint64, 1, len(rows)+1)
 	if len(uids) == 0 {
 		for _, r := range rows {
@@ -1144,11 +1158,48 @@ func MatchFuzzy(col *StrColumn, query string, max int64, uids []uint64, rows [][
 			listOff = append(listOff, uint64(len(lists)))
 		}
 	}
+	return lists, listOff
+}
+
+// dgxMinRegex: below this many candidates a regexp() stays in Go (handleRegexFunction).  No C22 record times the
+// library against Go's loop yet, so this is the dgxMinMatch bound until one sets it.
+const dgxMinRegex = dgxMinMatch
+
+// MatchRegex is handleRegexFunction's value loop (worker/task.go:1240-1356, matchRegex :1809-1811) in one
+// dgx_regex_match call: pattern is the regexp's pattern as cregexp.Compile takes it before the "(?m)" prefix, fold the
+// i modifier.  The candidates are uids when not empty (the @filter branch's UidList), otherwise the union of rows,
+// uidsForRegex's result.  Returns the kept candidates and true; false -- a pattern outside the compiled subset
+// (DGX_ERR_ARG), a DFA past DGX_REGEX_MAX_STATES (DGX_ERR_CAP), fewer than dgxMinRegex candidates, or any other
+// library error -- means the caller keeps cregexp and Go's loop.  The caller then intersects every UidMatrix row with
+// the result as before.
+func MatchRegex(col *StrColumn, pattern string, fold bool, uids []uint64, rows [][]uint64) ([]uint64, bool) {
+	bound := len(uids)
+	if bound == 0 {
+		for _, r := range rows {
+			bound += len(r)
+		}
+	}
+	if bound < dgxMinRegex || len(col.Uids) != len(col.Vals) {
+		return nil, false
+	}
+	pp, fp := cArray([]byte(pattern))
+	defer fp()
+	flags := C.int(0)
+	if fold {
+		flags = C.DGX_REGEX_FOLD
+	}
+	var prog *C.dgx_regex_prog
+	if C.dgx_regex_compile((*C.char)(pp), C.size_t(len(pattern)), flags, &prog) != C.DGX_OK {
+		return nil, false
+	}
+	defer C.dgx_regex_free(prog)
+	pc, free := cStrColumn(col)
+	defer free()
+	lists, listOff := candidateRows(uids, rows, bound)
 	out := make([]uint64, bound+1)
 	var n C.size_t
-	if C.dgx_match(nil, 0, nil, nil, nil, u64ptr(lists), u64ptr(listOff), C.size_t(len(listOff)-1), 0,
-		u64ptr(uids), C.size_t(len(uids)), (*C.dgx_str_column)(pc), (*C.uint8_t)(pq), C.size_t(len(query)), C.int64_t(max),
-		u64ptr(out), C.size_t(bound), &n) != C.DGX_OK {
+	if C.dgx_regex_match(nil, 0, nil, nil, nil, u64ptr(lists), u64ptr(listOff), C.size_t(len(listOff)-1), 0,
+		u64ptr(uids), C.size_t(len(uids)), (*C.dgx_str_column)(pc), prog, u64ptr(out), C.size_t(bound), &n) != C.DGX_OK {
 		return nil, false
 	}
 	return out[:n:n], true

@@ -779,6 +779,46 @@ int dgx_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids,
               uint64_t after_uid, const uint64_t* uids, size_t nuids, const dgx_str_column* col, const uint8_t* query,
               size_t query_len, int64_t max, uint64_t* out, size_t out_cap, size_t* out_len);
 
+/* regexp()'s pattern compiled for dgx_regex_match: a line-oriented byte DFA (DESIGN section 3.18).  It restates
+ * codesearch's matcher over "(?m)" + pattern as Go's regexp/syntax parses it with Perl flags, for this subset:
+ * literals and escapes (punctuation, \a \f \t \n \r \v, \xHH, \x{H..}), '.', bracket classes with ranges, negation,
+ * \d \s \w \D \S \W and [:name:] / [:^name:] inside, the same Perl classes outside, groups ( ), (?: ), flag groups
+ * (?flags) and (?flags: ) over i m s U with '-', alternation, * + ? and their lazy forms, {n} {n,} {n,m} up to 1000
+ * (nested counts multiplying to at most 1000, as Go requires), ^ $ \A \z; under (?-m) ^ and $ are \A and \z, as
+ * Go's OneLine makes them.  Under (?i) (or DGX_REGEX_FOLD, the /i
+ * modifier) ASCII letters fold, with K U+212A and long s U+017F in the orbits of k and s; a folded literal or class item
+ * holding any other non-ASCII rune is outside the subset.  A rune matches only its own well-formed UTF-8 bytes: an
+ * invalid byte matches nothing, not even '.' or a negated class.  Everything else -- \p{..}, \b, \B, \Q..\E, octal
+ * escapes, named groups, a '{' that is not a repeat count, stacked repetition operators, invalid UTF-8 in the pattern,
+ * and every pattern Go rejects -- is DGX_ERR_ARG, so a caller can keep its own matcher for it.  A DFA of more than
+ * DGX_REGEX_MAX_STATES states, a byte NFA past its own bound, or a construction past its work bound (which keeps the
+ * host's compile time to tens of milliseconds before a caller falls back) is DGX_ERR_CAP.  The program is host memory,
+ * immutable and shareable between threads and calls; dgx_regex_free releases it. */
+#define DGX_REGEX_FOLD 1
+#define DGX_REGEX_MAX_STATES 4096
+typedef struct dgx_regex_prog dgx_regex_prog;
+int dgx_regex_compile(const char* pattern, size_t len, int flags, dgx_regex_prog** prog);
+void dgx_regex_free(dgx_regex_prog* prog);
+/* The compiled tables, read-only and owned by prog: cls[256] maps a byte to its class, trans[s * nclasses + c] is the
+ * next state, term[s] has bit 1 when s absorbs (0 dead, 1 accept) and bit 2 when a value ending in s matches.  A value
+ * starts in state 2; '\n' leads every live state to 3, a later line's start, or to 0 / 1. */
+int dgx_regex_tables(const dgx_regex_prog* prog, size_t* nstates, size_t* nclasses, const uint8_t** cls,
+                     const uint16_t** trans, const uint8_t** term);
+
+/* regexp(attr, /pattern/) (worker/task.go handleRegexFunction :1240-1356, matchRegex :1809-1811) over a string value
+ * column.  The candidates are uids[0 .. nuids) when nuids > 0 (the filter's UidList, strictly ascending); otherwise
+ * the union of the leaves, taken exactly as dgx_match takes them (uidsForRegex's trigram rows: the caller passes the
+ * query's leaves; dgx_trigram_query evaluates a whole AND/OR tree, whose result is a UidList for this call).  A
+ * candidate is kept when one of its values in col is not empty and prog matches it: some line of the value holds a
+ * match, the first line only when it is not empty (codesearch reports that match at offset 0, which matchRegex counts
+ * as none).  Writes the kept candidates in ascending order to out (*out_len values).  Refusals as dgx_match's, with
+ * prog in place of the query: a null prog is DGX_ERR_ARG.  Launches: 5, after the trigram stages in the trigram
+ * branch, whatever the candidates, the column, the value lengths and the program (DESIGN section 3.18). */
+int dgx_regex_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut_uids, const uint8_t* mut_flags,
+                    const uint64_t* mut_off, const uint64_t* lists, const uint64_t* list_off, size_t nlists,
+                    uint64_t after_uid, const uint64_t* uids, size_t nuids, const dgx_str_column* col,
+                    const dgx_regex_prog* prog, uint64_t* out, size_t out_cap, size_t* out_len);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -1116,6 +1156,16 @@ int dgx_dev_match(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t npack
                   const uint64_t* list_off, size_t nlists, uint64_t after_uid, int use_uids, const uint64_t* d_uids,
                   size_t nuids, const uint64_t* d_nuids, const dgx_str_column* col, const uint8_t* query,
                   size_t query_len, int64_t max, uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
+/* Device form of dgx_regex_match, with dgx_dev_match's arguments and rules (use_uids, d_nuids, the device-side
+ * refusals surfacing at dgx_lane_sync), prog in place of the query.  The program's tables are copied with the call's
+ * workspace, so a device chain of dgx_dev_trigram_query, dgx_dev_sg_filter, dgx_dev_match or dgx_dev_regex_match
+ * outputs feeds it with no host read.  col's arrays need no padding or alignment: no byte outside
+ * [bytes, bytes + nbytes) is read. */
+int dgx_dev_regex_match(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t npacks, const uint64_t* d_mut_uids,
+                        const uint8_t* d_mut_flags, const uint64_t* mut_off, const uint64_t* d_lists,
+                        const uint64_t* list_off, size_t nlists, uint64_t after_uid, int use_uids,
+                        const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids, const dgx_str_column* col,
+                        const dgx_regex_prog* prog, uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

@@ -675,30 +675,80 @@ struct StrColumn {
     std::vector<std::vector<std::string>> vals;
 };
 
+namespace detail {
+// A StrColumn as the flat arrays of dgx_str_column; `c` points into this object, so it is neither copied nor moved.
+struct StrColumnCsr {
+    std::vector<uint64_t> val_off{0}, byte_off{0};
+    std::string data;
+    dgx_str_column c{};
+    explicit StrColumnCsr(const StrColumn& col) {
+        if (col.uids.size() != col.vals.size()) throw Error(DGX_ERR_ARG, "one list of values per uid");
+        for (const auto& vs : col.vals) {
+            for (const std::string& v : vs) { data += v; byte_off.push_back(data.size()); }
+            val_off.push_back(byte_off.size() - 1);
+        }
+        c = dgx_str_column{col.uids.data(), val_off.data(), byte_off.data(), (const uint8_t*)data.data(),
+                           col.uids.size(), byte_off.size() - 1, data.size()};
+    }
+    StrColumnCsr(const StrColumnCsr&) = delete;
+    StrColumnCsr& operator=(const StrColumnCsr&) = delete;
+};
+// The candidates as dgx_match / dgx_regex_match take them: uids when not empty, otherwise rows as list leaves.
+struct Candidates {
+    std::vector<uint64_t> lists, list_off{0};
+    size_t bound;
+    Candidates(const pb::List& uids, const std::vector<pb::List>& rows) {
+        if (uids.Uids.empty())
+            for (const pb::List& r : rows) { lists.insert(lists.end(), r.Uids.begin(), r.Uids.end()); list_off.push_back(lists.size()); }
+        bound = uids.Uids.empty() ? lists.size() : uids.Uids.size();
+    }
+};
+}  // namespace detail
+
 // match(attr, query, max) (worker/task.go handleMatchFunction, worker/match.go uidsForMatch / matchFuzzy) in one
 // dgx_match call: the candidates are uids when it is not empty (the filter's UidList), otherwise the union of rows,
 // the query's trigram rows as pl.Uids read them; a candidate is kept when one of its values is within max edits of
 // the query over Go's []rune conversion.  Returns the kept candidates.
 inline pb::List MatchFuzzy(const StrColumn& col, const std::string& query, int64_t max, const pb::List& uids,
                            const std::vector<pb::List>& rows = {}) {
-    if (col.uids.size() != col.vals.size()) throw Error(DGX_ERR_ARG, "one list of values per uid");
-    std::vector<uint64_t> val_off{0}, byte_off{0};
-    std::string data;
-    for (const auto& vs : col.vals) {
-        for (const std::string& v : vs) { data += v; byte_off.push_back(data.size()); }
-        val_off.push_back(byte_off.size() - 1);
-    }
-    const dgx_str_column c{col.uids.data(), val_off.data(), byte_off.data(), (const uint8_t*)data.data(),
-                           col.uids.size(), byte_off.size() - 1, data.size()};
-    std::vector<uint64_t> lists, list_off{0};
-    if (uids.Uids.empty())
-        for (const pb::List& r : rows) { lists.insert(lists.end(), r.Uids.begin(), r.Uids.end()); list_off.push_back(lists.size()); }
-    const size_t bound = uids.Uids.empty() ? lists.size() : uids.Uids.size();
-    std::vector<uint64_t> out(std::max<size_t>(bound, 1));
+    const detail::StrColumnCsr c(col);
+    const detail::Candidates k(uids, rows);
+    std::vector<uint64_t> out(std::max<size_t>(k.bound, 1));
     size_t n = 0;
-    check(dgx_match(nullptr, 0, nullptr, nullptr, nullptr, lists.data(), list_off.data(), list_off.size() - 1, 0,
-                    uids.Uids.data(), uids.Uids.size(), &c, (const uint8_t*)query.data(), query.size(), max,
-                    out.data(), bound, &n));
+    check(dgx_match(nullptr, 0, nullptr, nullptr, nullptr, k.lists.data(), k.list_off.data(), k.list_off.size() - 1, 0,
+                    uids.Uids.data(), uids.Uids.size(), &c.c, (const uint8_t*)query.data(), query.size(), max,
+                    out.data(), k.bound, &n));
+    out.resize(n);
+    return pb::List(out);
+}
+
+// A regexp() pattern compiled once (dgx_regex_compile; fold is the /i modifier).  Throws Error with DGX_ERR_ARG for a
+// pattern outside the compiled subset or one Go rejects, DGX_ERR_CAP past DGX_REGEX_MAX_STATES: keep Go's matcher then.
+class RegexProg {
+  public:
+    explicit RegexProg(const std::string& pattern, bool fold = false) {
+        check(dgx_regex_compile(pattern.data(), pattern.size(), fold ? DGX_REGEX_FOLD : 0, &p_));
+    }
+    ~RegexProg() { dgx_regex_free(p_); }
+    RegexProg(const RegexProg&) = delete;
+    RegexProg& operator=(const RegexProg&) = delete;
+    const dgx_regex_prog* get() const { return p_; }
+
+  private:
+    dgx_regex_prog* p_ = nullptr;
+};
+
+// regexp(attr, /pattern/) (worker/task.go handleRegexFunction, matchRegex) in one dgx_regex_match call: the
+// candidates as MatchFuzzy takes them, kept when one of their values matches prog.  Returns the kept candidates.
+inline pb::List MatchRegex(const StrColumn& col, const RegexProg& prog, const pb::List& uids,
+                           const std::vector<pb::List>& rows = {}) {
+    const detail::StrColumnCsr c(col);
+    const detail::Candidates k(uids, rows);
+    std::vector<uint64_t> out(std::max<size_t>(k.bound, 1));
+    size_t n = 0;
+    check(dgx_regex_match(nullptr, 0, nullptr, nullptr, nullptr, k.lists.data(), k.list_off.data(),
+                          k.list_off.size() - 1, 0, uids.Uids.data(), uids.Uids.size(), &c.c, prog.get(), out.data(),
+                          k.bound, &n));
     out.resize(n);
     return pb::List(out);
 }
