@@ -94,6 +94,21 @@ class StrColumn(C.Structure):
                 ("n", C.c_size_t), ("nvals", C.c_size_t), ("nbytes", C.c_size_t)]
 
 
+class ValColumn(C.Structure):
+    """dgx_val_column (include/dgx.h): a predicate's values converted to one type, uid i owning values val_off[i] ..
+    val_off[i+1), as words (and nanoseconds) or, for DGX_VAL_STRING, a referenced StrColumn; an optional bad byte per
+    value."""
+    _fields_ = [("type", C.c_int), ("uid", C.c_void_p), ("val_off", C.c_void_p), ("word", C.c_void_p),
+                ("nsec", C.c_void_p), ("bad", C.c_void_p), ("str", C.POINTER(StrColumn)), ("n", C.c_size_t),
+                ("nvals", C.c_size_t)]
+
+
+class ValArgs(C.Structure):
+    """dgx_val_args (include/dgx.h): a compare function's arguments, words (and nanoseconds) or string byte ranges."""
+    _fields_ = [("word", C.c_void_p), ("nsec", C.c_void_p), ("bytes", C.c_void_p), ("byte_off", C.c_void_p),
+                ("n", C.c_size_t)]
+
+
 class SgFilterTree(C.Structure):
     """dgx_sg_filter_tree (include/dgx.h): a subgraph's @filter tree, node 0 the root, parents below their children."""
     _fields_ = [("nnodes", C.c_size_t), ("op", C.c_void_p), ("parent", C.c_void_p), ("leaf", C.c_void_p)]
@@ -165,6 +180,8 @@ SYMBOLS = {
     "dgx_regex_tables": (_int, [_vp, _szp, _szp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp)]),
     "dgx_regex_match": (_int, [C.POINTER(PackRef), _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _vp, _sz,
                                C.POINTER(StrColumn), _vp, _vp, _sz, _szp]),
+    "dgx_compare_uids": (_int, [_int, C.POINTER(ValArgs), C.POINTER(ValColumn), _vp, _sz, _vp, _sz, _szp, _vp]),
+    "dgx_compare_rows": (_int, [_int, C.POINTER(ValArgs), C.POINTER(ValColumn), _vp, _vp, _sz, _vp, _vp, _vp, _sz]),
     "dgx_var_order": (_int, [C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _sz, C.c_int32, C.c_int32, _vp, _vp, _sz,
                              _vp, _sz, _szp]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
@@ -221,6 +238,10 @@ SYMBOLS = {
                              C.POINTER(StrColumn), _vp, _sz, C.c_int64, _vp, _sz, _vp]),
     "dgx_dev_regex_match": (_int, [_vp, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _u64, _int, _vp, _sz, _vp,
                                    C.POINTER(StrColumn), _vp, _vp, _sz, _vp]),
+    "dgx_dev_compare_uids": (_int, [_vp, _int, C.POINTER(ValArgs), C.POINTER(ValColumn), _vp, _sz, _vp, _vp, _sz,
+                                    _vp, _vp]),
+    "dgx_dev_compare_rows": (_int, [_vp, _int, C.POINTER(ValArgs), C.POINTER(ValColumn), _vp, _vp, _sz, _sz, _vp,
+                                    _vp, _vp, _sz]),
     "dgx_dev_var_order": (_int, [_vp, C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _vp, _sz, _sz, C.c_int32,
                                  C.c_int32, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),

@@ -1113,6 +1113,175 @@ def dev_match_regex(lane, dcol: "_lib.StrColumn", prog: RegexProg, d_out: int, o
                                                d_nuids, C.byref(dcol), prog.handle, d_out, out_cap, d_out_len))
 
 
+VAL_DATETIME, VAL_STRING = 5, 6  # DGX_VAL_* of a typed value column
+CMP_OPS = {"le": 0, "ge": 1, "lt": 2, "gt": 3, "eq": 4, "between": 5}  # DGX_SGF_CMP_*
+CMP_NO_ARG = 0xFFFFFFFF  # compare_rows' row_arg: the row passes unchanged
+
+
+def _addr(a):
+    return None if a is None else a.ctypes.data
+
+
+def _val_words(typ: int, vals) -> tuple:
+    """(words, nsec) of values of one type: int, float, bool or (unix seconds, nanoseconds)."""
+    if typ == VAL_INT64:
+        return np.asarray([int(v) for v in vals], np.int64).view(np.uint64), None
+    if typ == VAL_FLOAT64:
+        return np.asarray([float(v) for v in vals], np.float64).view(np.uint64), None
+    if typ == VAL_BOOL:
+        return np.asarray([1 if v else 0 for v in vals], np.uint64), None
+    if typ == VAL_DATETIME:
+        return (np.asarray([int(v[0]) for v in vals], np.int64).view(np.uint64),
+                np.asarray([int(v[1]) for v in vals], np.uint32))
+    raise ValueError(f"type {typ} has no words")
+
+
+class ValColumn:
+    """A typed value column (dgx_val_column): a predicate's values converted to its schema type, as Go's compare loops
+    read them.  typ: VAL_INT64, VAL_FLOAT64, VAL_BOOL, VAL_DATETIME or VAL_STRING.  uids: strictly ascending;
+    values[i]: the values of uids[i], each an int, a float, a bool, a (unix seconds, nanoseconds) pair or bytes / str
+    by type.  bad: optional, per uid the list of flags of its values whose conversion failed or gave nil."""
+
+    def __init__(self, typ: int, uids, values, bad=None):
+        self.type = typ
+        flat = [v for vs in values for v in vs]
+        if typ == VAL_STRING:
+            self.str = StrColumn(uids, values)
+            self.uid, self.val_off = self.str.uid, self.str.val_off
+            self.word = self.nsec = None
+        else:
+            self.str = None
+            self.uid = np.ascontiguousarray(np.asarray(uids, np.uint64).reshape(-1))
+            if len(values) != self.uid.size:
+                raise ValueError("one list of values per uid")
+            self.val_off = np.zeros(self.uid.size + 1, np.uint64)
+            np.cumsum([len(vs) for vs in values], out=self.val_off[1:])
+            w, ns = _val_words(typ, flat)
+            self.word = w if w.size else np.zeros(1, np.uint64)
+            self.nsec = None if ns is None else (ns if ns.size else np.zeros(1, np.uint32))
+        self.bad = None if bad is None else np.asarray([1 if b else 0 for bs in bad for b in bs] or [0], np.uint8)
+
+    @classmethod
+    def from_arrays(cls, typ: int, uid=None, val_off=None, word=None, nsec=None, bad=None, str_col=None):
+        c = cls.__new__(cls)
+        c.type, c.str = typ, str_col
+        if typ == VAL_STRING:
+            c.uid, c.val_off = str_col.uid, str_col.val_off
+        else:
+            c.uid, c.val_off = (np.ascontiguousarray(np.asarray(a, np.uint64)) for a in (uid, val_off))
+        c.word = None if word is None else np.ascontiguousarray(np.asarray(word).view(np.uint64))
+        c.nsec = None if nsec is None else np.ascontiguousarray(np.asarray(nsec, np.uint32))
+        c.bad = None if bad is None else np.ascontiguousarray(np.asarray(bad, np.uint8))
+        return c
+
+    def struct(self) -> "_lib.ValColumn":
+        n, nv = self.uid.size, int(self.val_off[-1])
+        if self.type == VAL_STRING:
+            self._s = self.str.struct()
+            return _lib.ValColumn(self.type, None, None, None, None, _addr(self.bad), C.pointer(self._s), 0, 0)
+        return _lib.ValColumn(self.type, self.uid.ctypes.data if n else None, self.val_off.ctypes.data,
+                              _addr(self.word), _addr(self.nsec), _addr(self.bad), None, n, nv)
+
+
+class ValArgs:
+    """A compare function's arguments (dgx_val_args) of one type, as ValColumn takes values."""
+
+    def __init__(self, typ: int, args):
+        args = list(args)
+        self.n = len(args)
+        if typ == VAL_STRING:
+            bs = [a.encode() if isinstance(a, str) else bytes(a) for a in args]
+            self.off = np.zeros(len(bs) + 1, np.uint64)
+            np.cumsum([len(b) for b in bs], out=self.off[1:])
+            self.bytes = np.frombuffer(b"".join(bs) + b"\0", np.uint8).copy()
+            self.word = self.nsec = None
+        else:
+            w, ns = _val_words(typ, args)
+            self.word = w if w.size else np.zeros(1, np.uint64)
+            self.nsec = ns
+            self.bytes = self.off = None
+
+    def struct(self) -> "_lib.ValArgs":
+        return _lib.ValArgs(_addr(self.word), _addr(self.nsec), _addr(self.bytes), _addr(self.off), self.n)
+
+
+def _cmp_op(op) -> int:
+    return CMP_OPS[op] if isinstance(op, str) else int(op)
+
+
+def CompareUids(col: ValColumn, op, args, uids, counts: bool = False):
+    """eq / le / lt / ge / gt / between over a UidList (worker/task.go handleValuePostings, compareAttrFn branch) in ONE
+    call (dgx_compare_uids): candidate uids[i] is kept when one of its values in col passes types.CompareVals(op, v,
+    arg) (CompareBetween for between; eq: any argument).  args: a ValArgs or values of col's type.  Returns the kept
+    candidates as a List, and with counts=True also Go's row lengths (matching values per candidate, np.uint32).  A
+    candidate with a bad value raises DgxError (DGX_ERR_ARG), where Go returns the conversion error."""
+    a = args if isinstance(args, ValArgs) else ValArgs(col.type, args)
+    u = _u64(uids.Uids if isinstance(uids, List) else uids)
+    cs, ast = col.struct(), a.struct()
+    out = np.empty(max(u.size, 1), np.uint64)
+    cnt = np.zeros(max(u.size, 1), np.uint32)
+    n = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_compare_uids(_cmp_op(op), C.byref(ast), C.byref(cs), _p(u) if u.size else None, u.size,
+                                            _p(out), u.size, C.byref(n), _p(cnt) if counts else None))
+    res = List(out[: n.value].copy())
+    return (res, cnt[: u.size].copy()) if counts else res
+
+
+def CompareRowArgs(op, nrows: int, neq: int = 1, first_is_ineq: bool = False) -> np.ndarray:
+    """row_arg for CompareRows from handleCompareFunction's three cases (worker/task.go :1491-1520): eq pairs row r
+    with eqTokens[r] (neq of them; Go indexes past them otherwise, which raises ValueError here), between filters
+    rows 0 and nrows - 1 against the pair, any other op row 0 when tokens[0] == ineqValueToken[0]."""
+    ra = np.full(nrows, CMP_NO_ARG, np.uint32)
+    name = op if isinstance(op, str) else {v: k for k, v in CMP_OPS.items()}[int(op)]
+    if name == "eq":
+        if nrows > neq:
+            raise ValueError(f"eq over {nrows} index rows and {neq} eqTokens: Go indexes past eqTokens")
+        ra[:] = np.arange(nrows, dtype=np.uint32)
+    elif name == "between":
+        if nrows:
+            ra[0] = ra[nrows - 1] = 0
+    elif first_is_ineq and nrows:
+        ra[0] = 0
+    return ra
+
+
+def CompareRows(col: ValColumn, op, args, rows, row_arg) -> list:
+    """handleCompareFunction's filterRow over the index rows (worker/task.go :1395-1520) in ONE call
+    (dgx_compare_rows): row r stays as it is when row_arg[r] is CMP_NO_ARG, otherwise keeps the uids with a value in
+    col passing op against argument row_arg[r] (between: row_arg[r] and the next); a bad value never passes.  Rows
+    need not ascend.  Returns the filtered rows."""
+    a = args if isinstance(args, ValArgs) else ValArgs(col.type, args)
+    v, v_off = _csr_u64(rows)
+    ra = np.ascontiguousarray(np.asarray(row_arg, np.uint32))
+    nrows, M = len(rows), int(v_off[-1])
+    cs, ast = col.struct(), a.struct()
+    out = np.empty(max(M, 1), np.uint64)
+    out_off = np.zeros(nrows + 1, np.uint64)
+    _lib.check(_lib.load().dgx_compare_rows(_cmp_op(op), C.byref(ast), C.byref(cs), _p(v), _p(v_off), nrows,
+                                            _p(ra) if nrows else None, _p(out), _p(out_off), M))
+    return [out[int(out_off[i]):int(out_off[i + 1])].copy() for i in range(nrows)]
+
+
+def dev_compare_uids(lane, dcol: "_lib.ValColumn", op, args: ValArgs, d_uids: int, nuids: int, d_out: int,
+                     out_cap: int, d_out_len: int, d_nuids: int | None = None, d_counts: int | None = None) -> None:
+    """The lane form of CompareUids (dgx_dev_compare_uids), asynchronous: dcol is a ValColumn struct whose arrays are
+    device memory (a resident column), args stay on the host, the other pointers are device addresses; the count is
+    nuids or the low 32 bits of the device word d_nuids.  Refusals found on the device surface at dgx_lane_sync."""
+    ast = args.struct()
+    _lib.check(_lib.load().dgx_dev_compare_uids(lane, _cmp_op(op), C.byref(ast), C.byref(dcol), d_uids, nuids,
+                                                d_nuids, d_out, out_cap, d_out_len, d_counts))
+
+
+def dev_compare_rows(lane, dcol: "_lib.ValColumn", op, args: ValArgs, d_v: int, d_v_off: int, nrows: int, v_cap: int,
+                     row_arg, d_out: int, d_out_off: int, out_cap: int) -> None:
+    """The lane form of CompareRows (dgx_dev_compare_rows), asynchronous: the rows calls' (d_out, d_out_off) as they
+    are, v_cap their room; row_arg on the host."""
+    ast = args.struct()
+    ra = np.ascontiguousarray(np.asarray(row_arg, np.uint32))
+    _lib.check(_lib.load().dgx_dev_compare_rows(lane, _cmp_op(op), C.byref(ast), C.byref(dcol), d_v, d_v_off, nrows,
+                                                v_cap, _p(ra) if nrows else None, d_out, d_out_off, out_cap))
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -50,6 +50,7 @@
 #include "match_kernel.cuh"
 #include "regex_kernel.cuh"
 #include "regex_compile.hpp"
+#include "compare_kernel.cuh"
 #include "wire.hpp"
 #include "ws_layout.hpp"
 
@@ -561,6 +562,10 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
             return fail(DGX_ERR_ARG, "a match() input is malformed (candidates or column uids not strictly ascending, "
                                      "column offsets not starting at 0, decreasing or not ending at nvals / nbytes, or "
                                      "a length word past its room; regexp()'s value test shares these checks)");
+        if (flag & kLaneErrCompare)
+            return fail(DGX_ERR_ARG, "a compare function's input is refused (candidates or column uids not strictly "
+                                     "ascending, column or row offsets malformed, a length word past its room, or a "
+                                     "candidate's value whose conversion failed)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -6256,6 +6261,7 @@ static int fz_run(dgx_lane* l, const FzQuery& Q, const uint64_t* cand, const uin
     P.m = Q.m;
     P.max = Q.max;
     P.err = l->d_err;
+    P.err_bit = kLaneErrMatch;
     fz_lookup_kernel<<<gb_grid(std::max<uint64_t>({ccap, col.n + 1, col.nvals + 1})), 256, 0, l->stream>>>(P);
     scan_u64_kernel<<<(unsigned)st, EN_NT, 0, l->stream>>>(P.cnt, P.pair_off, P.words + FZ_W_N, ccap, status, tickets,
                                                             P.words + FZ_W_PAIRS);
@@ -6524,6 +6530,7 @@ static int rx_run(dgx_lane* l, const rx::Prog& R, const uint64_t* cand, const ui
     F.nvals = col.nvals;
     F.nbytes = col.nbytes;
     F.err = l->d_err;
+    F.err_bit = kLaneErrMatch;
     P.nstates = R.nstates;
     P.nclasses = R.nclasses;
     P.warp = R.nstates <= (uint32_t)RX_WARP_STATES;
@@ -6580,6 +6587,432 @@ extern "C" int dgx_regex_match(const dgx_pack_ref* refs, size_t npacks, const ui
                              const dgx_str_column& D, uint64_t* o, uint64_t* ol) {
                              return rx_run(ln, prog->p, c, cl, bound, D, o, ol);
                          });
+}
+
+// ---------------------------------------------------------------------------
+// The compare functions eq / le / lt / ge / gt / between over a typed value column (compare_kernel.cuh)
+// ---------------------------------------------------------------------------
+static_assert(CMP_LE == DGX_SGF_CMP_LE && CMP_GE == DGX_SGF_CMP_GE && CMP_LT == DGX_SGF_CMP_LT &&
+                  CMP_GT == DGX_SGF_CMP_GT && CMP_EQ == DGX_SGF_CMP_EQ && CMP_BETWEEN == DGX_SGF_CMP_BETWEEN,
+              "compare_kernel.cuh reads include/dgx.h's op codes");
+static_assert(CMP_INT == DGX_VAL_INT64 && CMP_FLOAT == DGX_VAL_FLOAT64 && CMP_BOOL == DGX_VAL_BOOL &&
+                  CMP_TIME == DGX_VAL_DATETIME && CMP_STR == DGX_VAL_STRING,
+              "compare_kernel.cuh reads include/dgx.h's type codes");
+constexpr uint32_t kNsecPerSec = 1000000000u;
+
+// The arguments as the kernels read them: in the caller's order, or (eq on the value path) sorted and deduplicated
+// under Equal, NaN dropped and -0 folded to +0.
+struct CmpArgs {
+    std::vector<uint64_t> word;
+    std::vector<uint32_t> nsec;
+    std::vector<uint8_t> bytes;
+    std::vector<uint64_t> off;  // n + 1 byte offsets (strings)
+    size_t n = 0;
+};
+
+static int cmp_args(int op, int type, const dgx_val_args* a, bool eq_set, CmpArgs* A) {
+    if (op < DGX_SGF_CMP_LE || op > DGX_SGF_CMP_BETWEEN) return fail(DGX_ERR_ARG, "unknown compare op %d", op);
+    if (!a) return fail(DGX_ERR_ARG, "null arguments");
+    const size_t n = a->n;
+    if (n >= kFz32) return fail(DGX_ERR_ARG, "%zu arguments: at most 2^32 - 1", n);
+    if (op == DGX_SGF_CMP_BETWEEN && n != 2) return fail(DGX_ERR_ARG, "between takes 2 arguments, not %zu", n);
+    if (op == DGX_SGF_CMP_EQ && n < 1) return fail(DGX_ERR_ARG, "eq takes at least 1 argument");
+    if (op < DGX_SGF_CMP_EQ && n != 1) return fail(DGX_ERR_ARG, "op %d takes 1 argument, not %zu", op, n);
+    std::vector<size_t> idx(n);
+    for (size_t k = 0; k < n; ++k) idx[k] = k;
+    if (type == DGX_VAL_STRING) {
+        if (!a->byte_off) return fail(DGX_ERR_ARG, "null argument byte offsets");
+        if (int rc = check_offsets("args byte_off", a->byte_off, n, kFz32)) return rc;
+        if (a->byte_off[n] && !a->bytes) return fail(DGX_ERR_ARG, "null argument bytes");
+        auto sv = [&](size_t k) {
+            return std::string((const char*)a->bytes + a->byte_off[k], (size_t)(a->byte_off[k + 1] - a->byte_off[k]));
+        };
+        if (eq_set) {
+            std::vector<std::string> s(n);
+            for (size_t k = 0; k < n; ++k) s[k] = sv(k);
+            std::sort(idx.begin(), idx.end(), [&](size_t x, size_t y) { return s[x] < s[y]; });  // bytewise, unsigned
+            idx.erase(std::unique(idx.begin(), idx.end(), [&](size_t x, size_t y) { return s[x] == s[y]; }), idx.end());
+        }
+        A->off.push_back(0);
+        for (size_t k : idx) {
+            const std::string s = sv(k);
+            A->bytes.insert(A->bytes.end(), s.begin(), s.end());
+            A->off.push_back(A->bytes.size());
+        }
+        A->word.assign(idx.size(), 0);
+        A->n = idx.size();
+        return DGX_OK;
+    }
+    if (!a->word) return fail(DGX_ERR_ARG, "null argument words");
+    if (type == DGX_VAL_DATETIME) {
+        if (!a->nsec) return fail(DGX_ERR_ARG, "null argument nanoseconds");
+        for (size_t k = 0; k < n; ++k)
+            if (a->nsec[k] >= kNsecPerSec) return fail(DGX_ERR_ARG, "argument %zu has %u nanoseconds", k, a->nsec[k]);
+    }
+    auto key = [&](size_t k) -> uint64_t {  // a total order's key under Equal (NaN dropped before)
+        uint64_t w = a->word[k];
+        if (type == DGX_VAL_INT64 || type == DGX_VAL_DATETIME) return w ^ (uint64_t(1) << 63);
+        if (type == DGX_VAL_BOOL) return w != 0;
+        double d;
+        memcpy(&d, &w, 8);
+        if (d == 0) return uint64_t(1) << 63;  // -0 and +0
+        return (w >> 63) ? ~w : w | (uint64_t(1) << 63);
+    };
+    auto less = [&](size_t x, size_t y) {
+        const uint64_t kx = key(x), ky = key(y);
+        return kx != ky ? kx < ky : (type == DGX_VAL_DATETIME && a->nsec[x] < a->nsec[y]);
+    };
+    auto same = [&](size_t x, size_t y) { return !less(x, y) && !less(y, x); };
+    if (eq_set) {
+        if (type == DGX_VAL_FLOAT64)
+            idx.erase(std::remove_if(idx.begin(), idx.end(), [&](size_t k) {
+                          double d;
+                          memcpy(&d, &a->word[k], 8);
+                          return d != d;
+                      }), idx.end());
+        std::sort(idx.begin(), idx.end(), less);
+        idx.erase(std::unique(idx.begin(), idx.end(), same), idx.end());
+    }
+    for (size_t k : idx) {
+        uint64_t w = a->word[k];
+        if (eq_set && type == DGX_VAL_FLOAT64 && key(k) == uint64_t(1) << 63) w = 0;  // -0 folded to +0
+        if (eq_set && type == DGX_VAL_BOOL) w = w != 0;
+        A->word.push_back(w);
+        A->nsec.push_back(type == DGX_VAL_DATETIME ? a->nsec[k] : 0);
+    }
+    A->off.assign(1, 0);
+    A->n = idx.size();
+    return DGX_OK;
+}
+
+// The column's checks before anything is copied; the host form also checks its offsets (the device form's are checked
+// by fz_lookup_kernel).  S receives the column as match()'s lookup reads it.
+static int cmp_check_column(const dgx_val_column* c, bool host, dgx_str_column* S) {
+    if (!c) return fail(DGX_ERR_ARG, "null column");
+    const int t = c->type;
+    if (t != DGX_VAL_INT64 && t != DGX_VAL_FLOAT64 && t != DGX_VAL_BOOL && t != DGX_VAL_DATETIME && t != DGX_VAL_STRING)
+        return fail(DGX_ERR_ARG, "type %d is not compared on the device", t);
+    if (t == DGX_VAL_STRING) {
+        if (!c->str) return fail(DGX_ERR_ARG, "null string column");
+        *S = *c->str;
+        return fz_check_column(c->str, host);
+    }
+    if (c->n >= kFz32 || c->nvals >= kFz32)
+        return fail(DGX_ERR_ARG, "column sizes are 32-bit: n %zu, nvals %zu", c->n, c->nvals);
+    if (!c->val_off || (c->n && !c->uid) || (c->nvals && !c->word) || (t == DGX_VAL_DATETIME && c->nvals && !c->nsec))
+        return fail(DGX_ERR_ARG, "null column array");
+    *S = dgx_str_column{c->uid, c->val_off, nullptr, nullptr, c->n, c->nvals, 0};
+    if (!host) return DGX_OK;
+    if (int rc = check_offsets("val_off", c->val_off, c->n, kFz32)) return rc;
+    if (c->val_off[c->n] != c->nvals)
+        return fail(DGX_ERR_ARG, "val_off[n] is %llu, not nvals (%zu)", (unsigned long long)c->val_off[c->n], c->nvals);
+    return DGX_OK;
+}
+
+// The call's parameters common to both paths: the column (device arrays) and the arguments, copied with the workspace.
+static void cmp_bind(CmpParams& P, int op, const dgx_val_column& col, const dgx_str_column& S, dgx_lane* l) {
+    FzParams& F = P.F;
+    F.uid = (const u64*)S.uid;
+    F.val_off = (const u64*)S.val_off;
+    F.byte_off = (const u64*)S.byte_off;
+    F.bytes = S.bytes;
+    F.n = S.n;
+    F.nvals = S.nvals;
+    F.nbytes = S.nbytes;
+    F.err = l->d_err;
+    F.err_bit = kLaneErrCompare;
+    P.type = (u32)col.type;
+    P.op = (u32)op;
+    P.word = (const u64*)col.word;
+    P.nsec = col.nsec;
+    P.bad = col.bad;
+}
+static void cmp_declare_args(WsCarve& ws, CmpParams& P, const CmpArgs& A, uint64_t** hw, uint32_t** hn, uint8_t** hb,
+                             uint64_t** ho) {
+    ws.copied(&P.aword, hw, std::max<size_t>(A.word.size(), 1));
+    ws.copied(&P.ansec, hn, std::max<size_t>(A.nsec.size(), 1));
+    ws.copied(&P.aoff, ho, A.off.size());
+    ws.copied(&P.abytes, hb, A.bytes.size() + 16);
+}
+static void cmp_fill_args(CmpParams& P, const CmpArgs& A, uint64_t* hw, uint32_t* hn, uint8_t* hb, uint64_t* ho) {
+    hw[0] = 0;
+    hn[0] = 0;
+    if (!A.word.empty()) memcpy(hw, A.word.data(), A.word.size() * 8);
+    if (!A.nsec.empty()) memcpy(hn, A.nsec.data(), A.nsec.size() * 4);
+    memcpy(ho, A.off.data(), A.off.size() * 8);
+    memset(hb, 0, A.bytes.size() + 16);
+    if (!A.bytes.empty()) memcpy(hb, A.bytes.data(), A.bytes.size());
+    P.nargs = (u32)A.n;
+}
+
+// The value path on the lane for ccap candidate slots: 5 launches whatever the candidates, the column and the
+// arguments.  Workspace: the arguments and about 37 bytes per candidate slot (value counts, first values, pair
+// offsets, hits, keep flags, the look-back words).
+static int cmp_uids_run(dgx_lane* l, int op, const CmpArgs& A, const dgx_val_column& col, const dgx_str_column& S,
+                        const uint64_t* cand, const uint64_t* cand_len, uint64_t ccap, uint64_t* d_out,
+                        uint64_t* d_out_len, uint32_t* d_counts) {
+    CmpParams P{};
+    FzParams& F = P.F;
+    uint64_t *hw, *ho;
+    uint32_t* hn;
+    uint8_t* hb;
+    u64* status;
+    u32* tickets;
+    const uint64_t st = scan_tiles(ccap), kt = (ccap + CP_TILE - 1) / CP_TILE;
+    WsCarve ws(l);
+    cmp_declare_args(ws, P, A, &hw, &hn, &hb, &ho);
+    if (int rc = ws.stage()) return rc;
+    cmp_fill_args(P, A, hw, hn, hb, ho);
+    ws.zeroed(&F.words, 4);
+    ws.zeroed(&tickets, 4);
+    ws.zeroed(&status, st + kt);
+    ws.zeroed(&F.keep, ccap);
+    ws.zeroed(&P.hits, ccap);
+    ws.plain(&F.cnt, ccap);
+    ws.plain(&F.vlo, ccap);
+    ws.plain(&F.pair_off, ccap + 1);
+    if (int rc = ws.commit()) return rc;
+    cmp_bind(P, op, col, S, l);
+    F.cand = (const u64*)cand;
+    F.cand_len = (const u64*)cand_len;
+    F.ccap = ccap;
+    P.counts = d_counts;
+    const unsigned tgrid = (unsigned)std::min<uint64_t>(gb_grid(S.nvals), 8ull * g_num_sms);
+    fz_lookup_kernel<<<gb_grid(std::max<uint64_t>({ccap, S.n + 1, S.nvals + 1})), 256, 0, l->stream>>>(F);
+    scan_u64_kernel<<<(unsigned)st, EN_NT, 0, l->stream>>>(F.cnt, F.pair_off, F.words + FZ_W_N, ccap, status, tickets,
+                                                            F.words + FZ_W_PAIRS);
+    cmp_pairs_kernel<<<tgrid, CMP_NT, 0, l->stream>>>(P);
+    cmp_finish_kernel<<<gb_grid(ccap), CMP_NT, 0, l->stream>>>(P);
+    CompactParams K;
+    K.v = (const u64*)cand;
+    K.keep = F.keep;
+    K.m = ccap;
+    K.out = (u64*)d_out;
+    K.out_cap = ccap;
+    K.out_len = (u64*)d_out_len;
+    K.status = status + st;
+    K.ticket = tickets + 1;
+    K.err = l->d_err;
+    compact_kernel<<<(unsigned)kt, CP_NT, 0, l->stream>>>(K);
+    CK(cudaGetLastError());
+    count_launches(l, 5);
+    return DGX_OK;
+}
+
+// The index path on the lane: 4 launches whatever the rows, the column and the arguments.  Workspace: the arguments,
+// 4 bytes per row and 16 per value slot (keep flags and their scan).
+static int cmp_rows_run(dgx_lane* l, int op, const CmpArgs& A, const dgx_val_column& col, const dgx_str_column& S,
+                        const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows, uint64_t v_cap,
+                        const uint32_t* row_arg, uint64_t* d_out, uint64_t* d_out_off) {
+    CmpParams P{};
+    FzParams& F = P.F;
+    uint64_t *hw, *ho;
+    uint32_t *hn, *hra;
+    uint8_t* hb;
+    u64* status;
+    u32* tickets;
+    const uint64_t tiles = scan_tiles(v_cap);
+    WsCarve ws(l);
+    cmp_declare_args(ws, P, A, &hw, &hn, &hb, &ho);
+    ws.copied(&P.row_arg, &hra, nrows);
+    if (int rc = ws.stage()) return rc;
+    cmp_fill_args(P, A, hw, hn, hb, ho);
+    memcpy(hra, row_arg, nrows * sizeof(uint32_t));
+    ws.zeroed(&F.words, 4);
+    ws.zeroed(&tickets, 2);
+    ws.zeroed(&status, tiles);
+    ws.plain(&P.flag, std::max<uint64_t>(v_cap, 1));
+    ws.plain(&P.pos, v_cap + 1);
+    if (int rc = ws.commit()) return rc;
+    cmp_bind(P, op, col, S, l);
+    F.ccap = 0;  // the lookup checks the column alone
+    P.v = (const u64*)d_v;
+    P.v_off = (const u64*)d_v_off;
+    P.nrows = nrows;
+    P.v_cap = v_cap;
+    P.out = (u64*)d_out;
+    P.out_off = (u64*)d_out_off;
+    const uint64_t nt = std::max<uint64_t>(v_cap, nrows + 1);
+    fz_lookup_kernel<<<gb_grid(std::max<uint64_t>(S.n + 1, S.nvals + 1)), 256, 0, l->stream>>>(F);
+    cmp_rows_kernel<<<gb_grid(nt), CMP_NT, 0, l->stream>>>(P);
+    scan_u64_kernel<<<(unsigned)tiles, EN_NT, 0, l->stream>>>(P.flag, P.pos, F.words + CMP_W_M, v_cap, status, tickets,
+                                                                nullptr);
+    cmp_place_kernel<<<gb_grid(nt), CMP_NT, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 4);
+    return DGX_OK;
+}
+
+// A host array's device copy in the lane's workspace (nothing for bytes == 0).
+static int upload_bytes(dgx_lane* l, const void* h, size_t bytes, void** d) {
+    if (int rc = l->ws.alloc(bytes + 16, d)) return rc;
+    if (bytes) CK(cudaMemcpyAsync(*d, h, bytes, cudaMemcpyHostToDevice, l->stream));
+    g_stats.h2d += bytes;
+    return DGX_OK;
+}
+
+// The host form's column copy: every array the type needs, with the view match()'s lookup reads.
+static int cmp_upload_column(dgx_lane* l, const dgx_val_column* c, dgx_val_column* D, dgx_str_column* S,
+                             dgx_str_column* DS) {
+    *D = *c;
+    const dgx_str_column& H = c->type == DGX_VAL_STRING ? *c->str : *S;
+    uint64_t *d_uid, *d_voff;
+    int rc;
+    if ((rc = upload_list(l, H.uid, H.n, &d_uid)) || (rc = upload_list(l, H.val_off, H.n + 1, &d_voff))) return rc;
+    void* p;
+    if (c->bad) {
+        if ((rc = upload_bytes(l, c->bad, H.nvals, &p))) return rc;
+        D->bad = (const uint8_t*)p;
+    }
+    *DS = H;
+    DS->uid = d_uid;
+    DS->val_off = d_voff;
+    if (c->type == DGX_VAL_STRING) {
+        uint64_t* d_boff;
+        if ((rc = upload_list(l, H.byte_off, H.nvals + 1, &d_boff))) return rc;
+        if ((rc = upload_bytes(l, H.bytes, H.nbytes, &p))) return rc;
+        DS->byte_off = d_boff;
+        DS->bytes = (const uint8_t*)p;
+        return DGX_OK;
+    }
+    if ((rc = upload_bytes(l, c->word, H.nvals * 8, &p))) return rc;
+    D->word = (const uint64_t*)p;
+    if (c->type == DGX_VAL_DATETIME) {
+        if ((rc = upload_bytes(l, c->nsec, H.nvals * 4, &p))) return rc;
+        D->nsec = (const uint32_t*)p;
+    }
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_compare_uids(dgx_lane* l, int op, const dgx_val_args* args, const dgx_val_column* col,
+                                    const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids, uint64_t* d_out,
+                                    size_t out_cap, uint64_t* d_out_len, uint32_t* d_counts) {
+    if (!l || !d_out_len) return fail(DGX_ERR_ARG, "null argument");
+    dgx_str_column S;
+    if (int rc = cmp_check_column(col, false, &S)) return rc;
+    CmpArgs A;
+    if (int rc = cmp_args(op, col->type, args, op == DGX_SGF_CMP_EQ, &A)) return rc;
+    if (nuids >= kFz32) return fail(DGX_ERR_ARG, "nuids %zu: at most 2^32 - 1", nuids);
+    if (out_cap < nuids) return fail(DGX_ERR_CAP, "out_cap (%zu) is below nuids (%zu)", out_cap, nuids);
+    if (nuids && (!d_uids || !d_out)) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_out_len, sizeof(uint64_t));
+    if (nuids == 0) {
+        CK(cudaMemsetAsync(d_out_len, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = cmp_uids_run(l, op, A, *col, S, d_uids, d_nuids, nuids, d_out, d_out_len, d_counts)) return rc;
+    g_stats.uids_in += nuids;
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    if (d_counts) l->note_output(d_counts, nuids * sizeof(uint32_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_compare_uids(int op, const dgx_val_args* args, const dgx_val_column* col, const uint64_t* uids,
+                                size_t nuids, uint64_t* out, size_t out_cap, size_t* out_len, uint32_t* counts) {
+    if (!out_len) return fail(DGX_ERR_ARG, "null out_len");
+    dgx_str_column S;
+    if (int rc = cmp_check_column(col, true, &S)) return rc;
+    CmpArgs A;
+    if (int rc = cmp_args(op, col->type, args, op == DGX_SGF_CMP_EQ, &A)) return rc;
+    if (nuids >= kFz32) return fail(DGX_ERR_ARG, "nuids %zu: at most 2^32 - 1", nuids);
+    if (out_cap < nuids) return fail(DGX_ERR_CAP, "out_cap (%zu) is below nuids (%zu)", out_cap, nuids);
+    if (nuids && (!uids || !out)) return fail(DGX_ERR_ARG, "null argument");
+    if (nuids == 0) { *out_len = 0; return DGX_OK; }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += nuids;
+    int rc;
+    dgx_val_column D;
+    dgx_str_column DS;
+    if ((rc = cmp_upload_column(l, col, &D, &S, &DS))) return rc;
+    uint64_t* d_uids;
+    void* p;
+    if ((rc = upload_list(l, uids, nuids, &d_uids))) return rc;
+    if ((rc = l->ws.alloc((nuids + 10) * sizeof(uint64_t), &p))) return rc;  // the length word, then the values
+    uint64_t* d_out = (uint64_t*)p;
+    uint32_t* d_counts = nullptr;
+    if (counts && (rc = l->ws.alloc(nuids * sizeof(uint32_t), (void**)&d_counts))) return rc;
+    if ((rc = cmp_uids_run(l, op, A, D, DS, d_uids, nullptr, nuids, d_out + 8, d_out, d_counts))) return rc;
+    if ((rc = finish_to_host(l, d_out, d_out + 8, nuids, out, out_cap, out_len))) {
+        *out_len = 0;
+        return rc;
+    }
+    if (counts) {
+        CK(cudaMemcpyAsync(counts, d_counts, nuids * sizeof(uint32_t), cudaMemcpyDeviceToHost, l->stream));
+        CK(cudaStreamSynchronize(l->stream));
+        g_stats.d2h += nuids * sizeof(uint32_t);
+    }
+    return DGX_OK;
+}
+
+static int cmp_check_row_args(const CmpArgs& A, int op, const uint32_t* row_arg, size_t nrows) {
+    if (nrows && !row_arg) return fail(DGX_ERR_ARG, "null row_arg");
+    const uint64_t need = op == DGX_SGF_CMP_BETWEEN ? 2 : 1;
+    for (size_t r = 0; r < nrows; ++r)
+        if (row_arg[r] != CMP_NO_ARG && (uint64_t)row_arg[r] + need > A.n)
+            return fail(DGX_ERR_ARG, "row_arg[%zu] is %u: past the %zu arguments", r, row_arg[r], A.n);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_compare_rows(dgx_lane* l, int op, const dgx_val_args* args, const dgx_val_column* col,
+                                    const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows, size_t v_cap,
+                                    const uint32_t* row_arg, uint64_t* d_out, uint64_t* d_out_off, size_t out_cap) {
+    if (!l || !d_out_off) return fail(DGX_ERR_ARG, "null argument");
+    dgx_str_column S;
+    if (int rc = cmp_check_column(col, false, &S)) return rc;
+    CmpArgs A;
+    if (int rc = cmp_args(op, col->type, args, false, &A)) return rc;
+    if (int rc = cmp_check_row_args(A, op, row_arg, nrows)) return rc;
+    if (nrows >= kFz32 || v_cap >= kFz32) return fail(DGX_ERR_ARG, "nrows %zu, v_cap %zu: below 2^32", nrows, v_cap);
+    if (out_cap < v_cap) return fail(DGX_ERR_CAP, "out_cap (%zu) is below v_cap (%zu)", out_cap, v_cap);
+    if (!d_v_off || (v_cap && (!d_v || !d_out))) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    if (nrows == 0) {
+        CK(cudaMemsetAsync(d_out_off, 0, sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = cmp_rows_run(l, op, A, *col, S, d_v, d_v_off, nrows, v_cap, row_arg, d_out, d_out_off)) return rc;
+    g_stats.uids_in += v_cap;
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_compare_rows(int op, const dgx_val_args* args, const dgx_val_column* col, const uint64_t* v,
+                                const uint64_t* v_off, size_t nrows, const uint32_t* row_arg, uint64_t* out,
+                                uint64_t* out_off, size_t out_cap) {
+    if (!out_off || !v_off) return fail(DGX_ERR_ARG, "null argument");
+    dgx_str_column S;
+    if (int rc = cmp_check_column(col, true, &S)) return rc;
+    CmpArgs A;
+    if (int rc = cmp_args(op, col->type, args, false, &A)) return rc;
+    if (int rc = cmp_check_row_args(A, op, row_arg, nrows)) return rc;
+    if (nrows >= kFz32) return fail(DGX_ERR_ARG, "nrows %zu: at most 2^32 - 1", nrows);
+    if (int rc = check_offsets("v_off", v_off, nrows, kFz32)) return rc;
+    const uint64_t m = v_off[nrows];
+    if (out_cap < m) return fail(DGX_ERR_CAP, "out_cap (%zu) is below v_off[nrows] (%llu)", out_cap, (unsigned long long)m);
+    if (m && (!v || !out)) return fail(DGX_ERR_ARG, "null argument");
+    if (nrows == 0) { out_off[0] = 0; return DGX_OK; }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += m;
+    int rc;
+    dgx_val_column D;
+    dgx_str_column DS;
+    if ((rc = cmp_upload_column(l, col, &D, &S, &DS))) return rc;
+    uint64_t *d_v, *d_voff, *d_out, *d_off;
+    if ((rc = upload_list(l, v, m, &d_v)) || (rc = upload_list(l, v_off, nrows + 1, &d_voff))) return rc;
+    if ((rc = l->ws.alloc((m + nrows + 2) * sizeof(uint64_t), (void**)&d_out))) return rc;
+    d_off = d_out + m + 1;
+    if ((rc = cmp_rows_run(l, op, A, D, DS, d_v, d_voff, nrows, m, row_arg, d_out, d_off))) return rc;
+    return batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap);
 }
 
 extern "C" uint64_t dgx_merge_matrix_overflows(const dgx_lane* l) { return l ? l->xm_overflows : g_xm_overflows.load(); }

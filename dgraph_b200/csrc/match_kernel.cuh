@@ -6,7 +6,8 @@
 // candidate is kept when one of its values lies within max edits of the query, distances taken over Go's []rune
 // conversion (an invalid UTF-8 byte is one U+FFFD).  The device runs:
 //   fz_lookup_kernel   thread per candidate: its value range in the column (binary search), the order checks of the
-//                      candidates and of the column (uids strictly ascending, offsets ascending and closed)
+//                      candidates and of the column (uids strictly ascending, offsets ascending and closed; byte
+//                      offsets only when the column has them, so compare_kernel.cuh's typed columns share it)
 //   scan_u64_kernel    value counts -> pair offsets: the (candidate, value) pairs flattened, so a hub's 10^4 list
 //                      values spread over 10^4 threads
 //   fz_test_kernel     thread per pair: an empty value fails; a query of more than 64 runes queues the pair for the
@@ -57,12 +58,13 @@ struct FzParams {
     unsigned char* keep;  // ccap
     u64* longq;  // nvals: (candidate << 32) | value of a queued pair
     int* err;
+    int err_bit;  // the lane error bit a refusal raises (kLaneErrMatch for match() and regexp())
 };
 constexpr int FZ_W_N = 0, FZ_W_PAIRS = 1, FZ_W_LONG = 2, FZ_W_BAD = 3;
 
 __device__ __forceinline__ void fz_refuse(const FzParams& P) {
     atomicExch((unsigned long long*)(P.words + FZ_W_BAD), 1ull);
-    atomicOr(P.err, kLaneErrMatch);
+    atomicOr(P.err, P.err_bit);
 }
 
 // utf8.DecodeRuneInString over p[i .. len): the rune and its width; anything Go does not accept is (U+FFFD, 1).
@@ -138,13 +140,14 @@ __global__ void __launch_bounds__(256) fz_lookup_kernel(const FzParams P) {
     if (t == 0) {
         P.words[FZ_W_N] = nc;
         if (raw > P.ccap) fz_refuse(P);
-        if (P.val_off[0] != 0 || P.val_off[P.n] != P.nvals || P.byte_off[0] != 0 || P.byte_off[P.nvals] != P.nbytes)
+        if (P.val_off[0] != 0 || P.val_off[P.n] != P.nvals ||
+            (P.byte_off && (P.byte_off[0] != 0 || P.byte_off[P.nvals] != P.nbytes)))
             fz_refuse(P);
     }
     if (t < P.n) {
         if ((t > 0 && P.uid[t - 1] >= P.uid[t]) || P.val_off[t] > P.val_off[t + 1]) fz_refuse(P);
     }
-    if (t < P.nvals && P.byte_off[t] > P.byte_off[t + 1]) fz_refuse(P);
+    if (P.byte_off && t < P.nvals && P.byte_off[t] > P.byte_off[t + 1]) fz_refuse(P);
     if (t < P.ccap) {
         u64 c = 0, lo = 0;
         if (t < nc) {

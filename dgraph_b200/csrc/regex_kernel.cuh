@@ -46,11 +46,11 @@ struct RxSpan {
     u64 lo, hi;      // the value's byte offsets from seg
     u64 clo, chi;    // the column's
 };
-__device__ __forceinline__ RxSpan rx_span(const RxParams& P, u64 b0, u64 len) {
-    const uintptr_t a = (uintptr_t)P.F.bytes;
+__device__ __forceinline__ RxSpan rx_span(const unsigned char* bytes, u64 nbytes, u64 b0, u64 len) {
+    const uintptr_t a = (uintptr_t)bytes;
     const uintptr_t base = a & ~(uintptr_t)15;
     const u64 off = (u64)(a - base);
-    return RxSpan{(const uint4*)base, off + b0, off + b0 + len, off, off + P.F.nbytes};
+    return RxSpan{(const uint4*)base, off + b0, off + b0 + len, off, off + nbytes};
 }
 __device__ __forceinline__ uint4 rx_load(const RxSpan& sp, u64 g) {
     if (g * 16 >= sp.clo && g * 16 + 16 <= sp.chi) return __ldg(sp.seg + g);
@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(RX_NT) rx_test_kernel(const RxParams P) {
             F.longq[atomicAdd((unsigned long long*)(F.words + FZ_W_LONG), 1ull)] = (c << 32) | (j - F.vlo[c]);
             continue;
         }
-        const RxSpan sp = rx_span(P, b0, len);
+        const RxSpan sp = rx_span(F.bytes, F.nbytes, b0, len);
         u32 s = RX_START;
         for (u64 q = sp.lo & ~15ull; q < sp.hi && !(tab.term[s] & RX_ABSORB); q += 16)
             s = rx_seg(tab, rx_load(sp, q / 16), q, sp.lo, sp.hi, s);
@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(RX_NT, 1) rx_long_kernel(const RxParams P) {
     for (u32 q = blockIdx.x * (RX_NT / 32) + wid; q < nq; q += nwarps) {
         const u64 e = F.longq[q], c = e >> 32, j = F.vlo[c] + (e & 0xFFFFFFFFull);
         const u64 b0 = F.byte_off[j], len = F.byte_off[j + 1] - b0;
-        const RxSpan sp = rx_span(P, b0, len);
+        const RxSpan sp = rx_span(F.bytes, F.nbytes, b0, len);
         const u64 g0 = sp.lo / 16, nseg = (sp.hi + 15) / 16 - g0, per = (nseg + 31) / 32;
         const u64 s0 = g0 + (u64)lane * per, s1 = min(s0 + per, g0 + nseg);
         // lane 0 starts at the text's start: one walk; every other lane a vector over all states until it converges

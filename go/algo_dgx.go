@@ -1204,3 +1204,176 @@ func MatchRegex(col *StrColumn, pattern string, fold bool, uids []uint64, rows [
 	}
 	return out[:n:n], true
 }
+
+// dgxMinCompare: below this many candidates (or index-row values) a compare function stays in Go.  No C23 record times
+// the library against Go's loops yet, so this is the dgxMinMergeMatrix bound, as dgxMinMatch is, until one sets it.
+const dgxMinCompare = dgxMinMergeMatrix
+
+// The types of a ValColumn beyond ValInt64 / ValFloat64 / ValBool, and the compare ops (DGX_SGF_CMP_*).
+const (
+	ValDateTime = C.DGX_VAL_DATETIME
+	ValString   = C.DGX_VAL_STRING
+	CmpLE       = C.DGX_SGF_CMP_LE
+	CmpGE       = C.DGX_SGF_CMP_GE
+	CmpLT       = C.DGX_SGF_CMP_LT
+	CmpGT       = C.DGX_SGF_CMP_GT
+	CmpEQ       = C.DGX_SGF_CMP_EQ
+	CmpBetween  = C.DGX_SGF_CMP_BETWEEN
+)
+
+// ValColumn is a predicate's values converted to its schema type as Go's compare loops read them (types.Convert of
+// each stored value): Uids strictly ascending; for Type ValString the values of Uids[i] are Str.Vals[i] (Str.Uids is
+// Uids), otherwise Words[i] (int64, float64 bits, bool 0 / 1, or a datetime's Unix seconds with Nsec[i] its
+// nanoseconds).  Bad[i][j], when Bad is set, marks a value whose conversion failed or gave nil.
+type ValColumn struct {
+	Type  int
+	Uids  []uint64
+	Words [][]uint64
+	Nsec  [][]uint32
+	Str   *StrColumn
+	Bad   [][]bool
+}
+
+// ValArgs are a compare function's arguments (srcFn.eqTokens) of the column's type: Words (and Nsec) or Strs.
+type ValArgs struct {
+	Words []uint64
+	Nsec  []uint32
+	Strs  [][]byte
+}
+
+// cValCall copies col and args into C memory as a dgx_val_column and a dgx_val_args (cgo's pointer rules), the
+// string values through cStrColumn, the helper MatchFuzzy uses.  The caller calls free when the library is done.
+func cValCall(col *ValColumn, args *ValArgs) (unsafe.Pointer, unsafe.Pointer, func()) {
+	var frees []func()
+	keep := func(p unsafe.Pointer, f func()) unsafe.Pointer { frees = append(frees, f); return p }
+	valOff := []uint64{0}
+	var words []uint64
+	var nsec []uint32
+	var bad []uint8
+	var str unsafe.Pointer
+	for i := range col.Uids {
+		k := 0
+		if col.Type == ValString {
+			k = len(col.Str.Vals[i])
+		} else {
+			k = len(col.Words[i])
+			words = append(words, col.Words[i]...)
+			if col.Type == ValDateTime {
+				nsec = append(nsec, col.Nsec[i]...)
+			}
+		}
+		if col.Bad != nil {
+			for _, b := range col.Bad[i] {
+				if b {
+					bad = append(bad, 1)
+				} else {
+					bad = append(bad, 0)
+				}
+			}
+		}
+		valOff = append(valOff, valOff[len(valOff)-1]+uint64(k))
+	}
+	if col.Type == ValString {
+		str = keep(cStrColumn(col.Str))
+	}
+	var pbad unsafe.Pointer
+	if col.Bad != nil {
+		pbad = keep(cArray(bad))
+	}
+	pc := keep(cArray([]C.dgx_val_column{{_type: C.int(col.Type), uid: (*C.uint64_t)(keep(cArray(col.Uids))),
+		val_off: (*C.uint64_t)(keep(cArray(valOff))), word: (*C.uint64_t)(keep(cArray(words))),
+		nsec: (*C.uint32_t)(keep(cArray(nsec))), bad: (*C.uint8_t)(pbad), str: (*C.dgx_str_column)(str),
+		n: C.size_t(len(col.Uids)), nvals: C.size_t(valOff[len(valOff)-1])}}))
+	argOff := []uint64{0}
+	var argBytes []byte
+	for _, s := range args.Strs {
+		argBytes = append(argBytes, s...)
+		argOff = append(argOff, uint64(len(argBytes)))
+	}
+	n := len(args.Words)
+	if col.Type == ValString {
+		n = len(args.Strs)
+	}
+	pa := keep(cArray([]C.dgx_val_args{{word: (*C.uint64_t)(keep(cArray(args.Words))),
+		nsec: (*C.uint32_t)(keep(cArray(args.Nsec))), bytes: (*C.uint8_t)(keep(cArray(argBytes))),
+		byte_off: (*C.uint64_t)(keep(cArray(argOff))), n: C.size_t(n)}}))
+	return pc, pa, func() {
+		for i := len(frees) - 1; i >= 0; i-- {
+			frees[i]()
+		}
+	}
+}
+
+// CompareUids is handleValuePostings' compareAttrFn branch (worker/task.go:540-575) in one dgx_compare_uids call:
+// op is CmpLE .. CmpEQ or CmpBetween, uids the task's UidList.  It returns the kept uids (the merged DestUIDs) and,
+// per candidate, Go's row length (UidList[i] appended once per matching value).  ok == false -- fewer than
+// dgxMinCompare candidates, sizes or types outside the library's bounds, a candidate's bad value (Go returns the
+// conversion error; the caller's loop then reports it) or any other library error -- means the caller keeps Go's loop.
+func CompareUids(col *ValColumn, op int, args *ValArgs, uids []uint64) ([]uint64, []uint32, bool) {
+	if len(uids) < dgxMinCompare {
+		return nil, nil, false
+	}
+	pc, pa, free := cValCall(col, args)
+	defer free()
+	out := make([]uint64, len(uids)+1)
+	counts := make([]uint32, len(uids)+1)
+	var n C.size_t
+	if C.dgx_compare_uids(C.int(op), (*C.dgx_val_args)(pa), (*C.dgx_val_column)(pc), u64ptr(uids), C.size_t(len(uids)),
+		u64ptr(out), C.size_t(len(uids)), &n, (*C.uint32_t)(unsafe.Pointer(&counts[0]))) != C.DGX_OK {
+		return nil, nil, false
+	}
+	return out[:n:n], counts[:len(uids):len(uids)], true
+}
+
+// CompareRowArgs builds row_arg from handleCompareFunction's three cases (worker/task.go:1487-1520): eq pairs row r
+// with eqTokens[r] (ok == false where Go would index past eqTokens), between filters rows 0 and nrows - 1, another op
+// row 0 when tokens[0] == ineqValueToken[0].
+func CompareRowArgs(op, nrows, nEqTokens int, firstIsIneq bool) ([]uint32, bool) {
+	ra := make([]uint32, nrows)
+	for r := range ra {
+		ra[r] = ^uint32(0)
+	}
+	switch {
+	case op == CmpEQ:
+		if nrows > nEqTokens {
+			return nil, false
+		}
+		for r := range ra {
+			ra[r] = uint32(r)
+		}
+	case op == CmpBetween:
+		if nrows > 0 {
+			ra[0], ra[nrows-1] = 0, 0
+		}
+	case firstIsIneq && nrows > 0:
+		ra[0] = 0
+	}
+	return ra, true
+}
+
+// CompareRows is handleCompareFunction's filterRow calls (worker/task.go:1395-1520) in one dgx_compare_rows call over
+// the index uid matrix rows, row_arg from CompareRowArgs.  It returns the filtered rows; ok == false -- fewer than
+// dgxMinCompare values or any library error -- means the caller keeps Go's filterRow loop.
+func CompareRows(col *ValColumn, op int, args *ValArgs, rows []*pb.List, rowArg []uint32) ([][]uint64, bool) {
+	m := varValues(rows)
+	if m < dgxMinCompare || len(rowArg) != len(rows) || len(rows) == 0 {
+		return nil, false
+	}
+	pc, pa, free := cValCall(col, args)
+	defer free()
+	pv, pvo, _, fv := varFlat(rows)
+	defer fv()
+	pr, fr := cArray(rowArg)
+	defer fr()
+	out := make([]uint64, m+1)
+	outOff := make([]uint64, len(rows)+1)
+	if C.dgx_compare_rows(C.int(op), (*C.dgx_val_args)(pa), (*C.dgx_val_column)(pc), (*C.uint64_t)(pv),
+		(*C.uint64_t)(pvo), C.size_t(len(rows)), (*C.uint32_t)(pr), u64ptr(out), u64ptr(outOff), C.size_t(m)) != C.DGX_OK {
+		return nil, false
+	}
+	res := make([][]uint64, len(rows))
+	for r := range rows {
+		res[r] = out[outOff[r]:outOff[r+1]:outOff[r+1]]
+	}
+	return res, true
+}

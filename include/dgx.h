@@ -819,6 +819,80 @@ int dgx_regex_match(const dgx_pack_ref* refs, size_t npacks, const uint64_t* mut
                     uint64_t after_uid, const uint64_t* uids, size_t nuids, const dgx_str_column* col,
                     const dgx_regex_prog* prog, uint64_t* out, size_t out_cap, size_t* out_len);
 
+/* A typed value column: the values of one predicate converted to its schema type, as Go's compare loops read them
+ * (types.Convert of each stored value).  The layout is dgx_str_column's: uid[0 .. n) strictly ascending, uid i owning
+ * values val_off[i] .. val_off[i+1) (n + 1 offsets, val_off[0] == 0, val_off[n] == nvals), several values per uid for a
+ * list predicate, every count below 2^32.  type picks the value's form:
+ *   DGX_VAL_INT64     word[j] is the int64
+ *   DGX_VAL_FLOAT64   word[j] is the IEEE binary64 pattern
+ *   DGX_VAL_BOOL      word[j] != 0 is true
+ *   DGX_VAL_DATETIME  word[j] is the instant's Unix seconds (int64, negative before 1970), nsec[j] its nanoseconds
+ *                     (below 10^9); the location is not part of the value, as time.Time.Before / Equal ignore it
+ *   DGX_VAL_STRING    str is the column (a dgx_str_column, shared with match() and regexp()): uid, val_off, word,
+ *                     nsec, n and nvals are unused and str's are taken
+ * bad, when set, holds one byte per value: nonzero when the value's conversion to the schema type failed or gave nil. */
+#define DGX_VAL_DATETIME 5
+#define DGX_VAL_STRING 6
+typedef struct dgx_val_column {
+    int type;
+    const uint64_t* uid;
+    const uint64_t* val_off;
+    const uint64_t* word;
+    const uint32_t* nsec;
+    const uint8_t* bad;
+    const dgx_str_column* str;
+    size_t n;
+    size_t nvals;
+} dgx_val_column;
+/* A compare function's arguments, converted to the column's type (convertValue): n values given as a column's values
+ * are (word[k], nsec[k] for DATETIME), or for DGX_VAL_STRING the bytes bytes[byte_off[k] .. byte_off[k+1)).  Host
+ * memory in both forms. */
+typedef struct dgx_val_args {
+    const uint64_t* word;
+    const uint32_t* nsec;
+    const uint8_t* bytes;
+    const uint64_t* byte_off;
+    size_t n;
+} dgx_val_args;
+/* between(v, a, b): the compare op code past DGX_SGF_CMP_EQ.  dgx_sg_filter does not take it. */
+#define DGX_SGF_CMP_BETWEEN 5
+
+/* The compare functions eq / le / lt / ge / gt / between on the value path (worker/task.go handleValuePostings,
+ * compareAttrFn branch :540-575, with types.CompareVals / CompareBetween, types/compare.go): candidate uids[i] (the
+ * filter's UidList, strictly ascending) is tested against each of its values in col.  op is DGX_SGF_CMP_LE .. EQ or
+ * DGX_SGF_CMP_BETWEEN; args holds 1 argument (le, lt, ge, gt), at least 1 (eq: a value equal to any one matches) or
+ * exactly 2 (between a and b).  Go's rules: ge is !Less(v, a), le !Less(a, v), gt Less(a, v), lt Less(v, a), eq
+ * Equal(v, a), between ge(v, a) && le(v, b), each false where Less / Equal returns an error.  So for float64 a NaN value
+ * passes ge, le and between but not gt, lt or eq, a NaN argument makes ge / le true and gt / lt / eq false, and -0
+ * equals +0; a bool passes eq only; strings compare bytewise, unsigned, a proper prefix less.  Writes the candidates
+ * with at least one matching value in ascending order to out (*out_len values) and, when counts is set, counts[i] the
+ * number of uids[i]'s matching values (the length of Go's result row i: a list value matching appends the uid once).
+ * DGX_ERR_ARG before anything is copied: an unknown op or type, a wrong argument count, a DATETIME argument's
+ * nanoseconds of 10^9 or more, nuids or the column's sizes of 2^32 or more, column offsets not starting at 0,
+ * decreasing or not ending at nvals / nbytes, a null array that is needed.  DGX_ERR_CAP before anything is copied:
+ * out_cap below nuids.  DGX_ERR_ARG after the kernels, with nothing written but *out_len = 0: candidates or column
+ * uids not strictly ascending, or a candidate owning a bad value or a DATETIME value's nanoseconds of 10^9 or more (Go
+ * returns the conversion error); such values of uids that are not candidates are not read.  nuids == 0 writes
+ * *out_len = 0 and needs no device.  Launches: 5, whatever the candidates, the column, the values and the arguments
+ * (DESIGN section 3.19). */
+int dgx_compare_uids(int op, const dgx_val_args* args, const dgx_val_column* col, const uint64_t* uids, size_t nuids,
+                     uint64_t* out, size_t out_cap, size_t* out_len, uint32_t* counts);
+/* The compare functions on the index path (worker/task.go handleCompareFunction :1358-1524): the uid matrix
+ * v[v_off[r] .. v_off[r+1]) of the index rows, rows in any order, filtered row by row.  row_arg[r] == UINT32_MAX
+ * keeps row r as it is; otherwise a value of row r is kept when one of its values in col passes op against argument
+ * row_arg[r] (between: arguments row_arg[r] and row_arg[r] + 1), a bad value (or an absent uid) never passing.  Go's
+ * three cases are: eq, row r against eqTokens[r]; between, rows 0 and nrows - 1 against the pair; any other op, row 0
+ * when tokens[0] == ineqValueToken[0].  Writes the kept values in row order to out and nrows + 1 offsets to out_off.
+ * DGX_ERR_ARG before anything is copied: op, type and argument rules as dgx_compare_uids's (any argument count for eq,
+ * 2 for between), a row_arg past the arguments, nrows, v_off[nrows] or the column's sizes of 2^32 or more, v_off not
+ * starting at 0 or decreasing, the column's offsets, a null array that is needed.  DGX_ERR_CAP: out_cap below
+ * v_off[nrows].  DGX_ERR_ARG after the kernels, with every offset 0 and no value written: column uids not strictly
+ * ascending.  nrows == 0 writes out_off[0] = 0 and needs no device.  Launches: 4, whatever the rows, the column and the
+ * arguments (DESIGN section 3.19). */
+int dgx_compare_rows(int op, const dgx_val_args* args, const dgx_val_column* col, const uint64_t* v,
+                     const uint64_t* v_off, size_t nrows, const uint32_t* row_arg, uint64_t* out, uint64_t* out_off,
+                     size_t out_cap);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -1166,6 +1240,26 @@ int dgx_dev_regex_match(dgx_lane* lane, const dgx_dev_pack* const* packs, size_t
                         const uint64_t* list_off, size_t nlists, uint64_t after_uid, int use_uids,
                         const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids, const dgx_str_column* col,
                         const dgx_regex_prog* prog, uint64_t* d_out, size_t out_cap, uint64_t* d_out_len);
+/* Device form of dgx_compare_uids: col is a host struct whose arrays (its str's included) are device memory, args stay
+ * in host memory, d_uids and the outputs are device memory.  The candidate count is the low 32 bits of the device word
+ * d_nuids (at most nuids, the room; d_nuids NULL: exactly nuids), so the outputs of dgx_dev_sg_filter,
+ * dgx_dev_merge_sorted_matrix, dgx_dev_match or a previous dgx_dev_compare_uids feed it without a host read.  The bound
+ * is nuids: out_cap below it is DGX_ERR_CAP at the call, as every argument error of the host form is DGX_ERR_ARG there,
+ * except the column's offsets, which are checked on the device.  d_out_len is one device uint64; d_counts, when set,
+ * room for nuids uint32.  The order and offset checks, a count word past its room and a candidate's bad value are found
+ * on the device: a refused call writes *d_out_len = 0 and nothing else, and surfaces as DGX_ERR_ARG at the next
+ * dgx_lane_sync.  nuids == 0 writes a zero length without a launch.  Asynchronous on the lane; 5 launches. */
+int dgx_dev_compare_uids(dgx_lane* lane, int op, const dgx_val_args* args, const dgx_val_column* col,
+                         const uint64_t* d_uids, size_t nuids, const uint64_t* d_nuids, uint64_t* d_out,
+                         size_t out_cap, uint64_t* d_out_len, uint32_t* d_counts);
+/* Device form of dgx_compare_rows: col as in dgx_dev_compare_uids, args and row_arg in host memory, d_v, d_v_off and
+ * the outputs device memory, so the rows calls' (d_out, d_out_off) feed it as they are.  v_cap is the room of d_v
+ * (d_v_off[nrows] must not pass it); out_cap below v_cap is DGX_ERR_CAP at the call.  v_off and the column are checked
+ * on the device: a refused call writes nrows + 1 zero offsets and no value, and surfaces as DGX_ERR_ARG at the next
+ * dgx_lane_sync.  nrows == 0 writes a zero offset without a launch.  Asynchronous on the lane; 4 launches. */
+int dgx_dev_compare_rows(dgx_lane* lane, int op, const dgx_val_args* args, const dgx_val_column* col,
+                         const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows, size_t v_cap,
+                         const uint32_t* row_arg, uint64_t* d_out, uint64_t* d_out_off, size_t out_cap);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

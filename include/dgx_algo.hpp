@@ -15,6 +15,7 @@
 
 #include <algorithm>
 #include <cstdint>
+#include <memory>
 #include <numeric>
 #include <stdexcept>
 #include <string>
@@ -720,6 +721,95 @@ inline pb::List MatchFuzzy(const StrColumn& col, const std::string& query, int64
                     out.data(), k.bound, &n));
     out.resize(n);
     return pb::List(out);
+}
+
+// A predicate's values converted to one type for CompareUids / CompareRows (dgx_val_column): type is DGX_VAL_INT64,
+// DGX_VAL_FLOAT64 (IEEE bits), DGX_VAL_BOOL, DGX_VAL_DATETIME (Unix seconds in words, nanoseconds in nsec) or
+// DGX_VAL_STRING (strs); uids strictly ascending, the values of uids[i] at index i; bad, when not empty, flags the
+// values whose conversion failed or gave nil.
+struct ValColumn {
+    int type = DGX_VAL_INT64;
+    std::vector<uint64_t> uids;
+    std::vector<std::vector<uint64_t>> words;
+    std::vector<std::vector<uint32_t>> nsec;
+    std::vector<std::vector<std::string>> strs;
+    std::vector<std::vector<uint8_t>> bad;
+};
+// A compare function's arguments of the column's type: words (and nsec) or strs.
+struct ValArgs {
+    std::vector<uint64_t> words;
+    std::vector<uint32_t> nsec;
+    std::vector<std::string> strs;
+};
+
+namespace detail {
+// A ValColumn and its arguments as dgx_val_column / dgx_val_args; the structs point into this object.
+struct ValCall {
+    std::vector<uint64_t> val_off{0}, word, arg_off{0};
+    std::vector<uint32_t> nsec;
+    std::vector<uint8_t> bad;
+    std::string arg_bytes;
+    StrColumn sc;
+    std::unique_ptr<StrColumnCsr> str;
+    dgx_val_column c{};
+    dgx_val_args a{};
+    ValCall(const ValColumn& col, const ValArgs& args) {
+        const bool is_str = col.type == DGX_VAL_STRING;
+        const size_t n = col.uids.size();
+        if ((is_str ? col.strs.size() : col.words.size()) != n) throw Error(DGX_ERR_ARG, "one list of values per uid");
+        for (size_t i = 0; i < n; ++i) {
+            const size_t k = is_str ? col.strs[i].size() : col.words[i].size();
+            if (!is_str) word.insert(word.end(), col.words[i].begin(), col.words[i].end());
+            if (col.type == DGX_VAL_DATETIME) nsec.insert(nsec.end(), col.nsec[i].begin(), col.nsec[i].end());
+            if (!col.bad.empty()) bad.insert(bad.end(), col.bad[i].begin(), col.bad[i].end());
+            val_off.push_back(val_off.back() + k);
+        }
+        if (is_str) {
+            sc = StrColumn{col.uids, col.strs};
+            str.reset(new StrColumnCsr(sc));
+        }
+        c = dgx_val_column{col.type, col.uids.data(), val_off.data(), word.data(), nsec.data(),
+                           col.bad.empty() ? nullptr : bad.data(), is_str ? &str->c : nullptr, n, val_off.back()};
+        for (const std::string& s : args.strs) { arg_bytes += s; arg_off.push_back(arg_bytes.size()); }
+        a = dgx_val_args{args.words.data(), args.nsec.data(), (const uint8_t*)arg_bytes.data(), arg_off.data(),
+                         is_str ? args.strs.size() : args.words.size()};
+    }
+    ValCall(const ValCall&) = delete;
+    ValCall& operator=(const ValCall&) = delete;
+};
+}  // namespace detail
+
+// eq / le / lt / ge / gt / between (op DGX_SGF_CMP_*) over the filter's UidList (worker/task.go handleValuePostings,
+// compareAttrFn branch) in one dgx_compare_uids call: the candidates with a value passing types.CompareVals, and in
+// *counts, when given, Go's row lengths.  A candidate's bad value throws Error(DGX_ERR_ARG), Go's conversion error.
+inline pb::List CompareUids(const ValColumn& col, int op, const ValArgs& args, const pb::List& uids,
+                            std::vector<uint32_t>* counts = nullptr) {
+    const detail::ValCall v(col, args);
+    std::vector<uint64_t> out(std::max<size_t>(uids.Uids.size(), 1));
+    std::vector<uint32_t> cnt(std::max<size_t>(uids.Uids.size(), 1));
+    size_t n = 0;
+    check(dgx_compare_uids(op, &v.a, &v.c, uids.Uids.data(), uids.Uids.size(), out.data(), uids.Uids.size(), &n,
+                           counts ? cnt.data() : nullptr));
+    out.resize(n);
+    if (counts) { cnt.resize(uids.Uids.size()); *counts = cnt; }
+    return pb::List(out);
+}
+
+// handleCompareFunction's filterRow over the index rows (worker/task.go :1395-1520) in one dgx_compare_rows call:
+// row r unchanged when row_arg[r] is UINT32_MAX, otherwise filtered by value against argument row_arg[r].
+inline std::vector<pb::List> CompareRows(const ValColumn& col, int op, const ValArgs& args,
+                                         const std::vector<pb::List>& rows, const std::vector<uint32_t>& row_arg) {
+    const detail::ValCall v(col, args);
+    if (row_arg.size() != rows.size()) throw Error(DGX_ERR_ARG, "one row_arg per row");
+    std::vector<uint64_t> flat, off{0};
+    for (const pb::List& r : rows) { flat.insert(flat.end(), r.Uids.begin(), r.Uids.end()); off.push_back(flat.size()); }
+    std::vector<uint64_t> out(std::max<size_t>(flat.size(), 1)), out_off(rows.size() + 1);
+    check(dgx_compare_rows(op, &v.a, &v.c, flat.data(), off.data(), rows.size(), row_arg.data(), out.data(),
+                           out_off.data(), flat.size()));
+    std::vector<pb::List> res;
+    for (size_t r = 0; r < rows.size(); ++r)
+        res.push_back(pb::List(std::vector<uint64_t>(out.begin() + out_off[r], out.begin() + out_off[r + 1])));
+    return res;
 }
 
 // A regexp() pattern compiled once (dgx_regex_compile; fold is the /i modifier).  Throws Error with DGX_ERR_ARG for a

@@ -147,6 +147,7 @@ def main():
     ap.add_argument("--c19-only", action="store_true", help="only the C19 @filter and first / offset rows")
     ap.add_argument("--c20-only", action="store_true", help="only the C20 orderasc / orderdesc by a value variable rows")
     ap.add_argument("--c21-only", action="store_true", help="only the C21 match() rows")
+    ap.add_argument("--c23-only", action="store_true", help="only the C23 compare function rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -180,9 +181,11 @@ def main():
         rows = c20_rows(Lane())
     elif args.c21_only:
         rows = c21_rows(Lane())
+    elif args.c23_only:
+        rows = c23_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only or args.c20_only or args.c21_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only or args.c20_only or args.c21_only or args.c23_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -2142,6 +2145,209 @@ def c21_rows(L):
                              "candidates": cap, "check": bool(ok), "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del dt, d_out, d_len
+    return out_rows
+
+
+def c23_rows(L):
+    """C23 "the compare functions": eq / le / lt / ge / gt / between over a typed value column.  C23a: an int64 column
+    of 1e8 uids, a UidList of 2e7, ge keeping about half.  C23b: a float list predicate, 1e7 uids of 1-8 values with
+    NaNs mixed in, between.  C23c: C21a's 1e7-uid name column with 3e6 candidates: eq with 1 argument, eq with 1 000
+    arguments, and ge.  C23d: ge at root on a float index of 1e7 values in about 1e4 buckets, as the device chain (the
+    rows resident -> row 0 filtered by dgx_dev_compare_rows -> dgx_dev_merge_sorted_matrix), beside the same chain
+    without the filter.  C23e: TestFilterNonIndexedPredicate's size (launch-bound).  C23f: a UidList of 9 against
+    C23a's resident column: the whole-column check every value-column call pays (DESIGN section 3.17).  C23d's legs
+    start from the index rows resident on the device; the rows read before them is not timed.  Legs: (1) the
+    device form on resident inputs (CUDA events), (2) the host form with its copies (wall clock), (3) the line-by-line
+    restatement (tests/compare_oracle.c) on 1 thread -- C, not Go.  Every leg is checked against the restatement.
+    Algorithmic bytes: candidates read and written (16 per candidate), each tested value's word or bytes, and the
+    column's uid and val_off arrays, which every call reads whole for its checks.  For C23a, C23b and C23c's one-argument
+    eq, each kernel's time (torch.profiler, a run of its own) is set against the bytes that kernel must move."""
+    import compare_oracle as co
+    import gen_match as gm
+    from dgraph_b200 import algo
+
+    U64 = np.uint64
+    rng = np.random.default_rng(23)
+
+    def kernel_times(fn, reps=5):
+        """Mean device time per call of each named kernel, from torch.profiler with CUDA activities."""
+        from torch.profiler import ProfilerActivity, profile
+
+        fn()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                fn()
+            torch.cuda.synchronize()
+        t = {}
+        for e in prof.key_averages():
+            for k in ("fz_lookup_kernel", "scan_u64_kernel", "cmp_pairs_kernel", "cmp_finish_kernel",
+                      "compact_kernel", "cmp_rows_kernel", "cmp_place_kernel"):
+                if k in e.key:
+                    us = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
+                    t[k] = t.get(k, 0.0) + us / 1e3 / reps
+        return t
+    peak, _ = peak_gbs()
+
+    def up(x, dt=U64):
+        x = np.concatenate([np.ascontiguousarray(x, dt), np.zeros(1, dt)])
+        return torch.from_numpy(x.view(np.int64) if dt == U64 else x.view(np.int32) if dt == np.uint32 else x).to(DEV)
+
+    def dev_col(col):
+        keep = []
+
+        def d(a, dt=U64):
+            if a is None:
+                return None
+            t = up(a, dt)
+            keep.append(t)
+            return t.data_ptr()
+        if col.type == algo.VAL_STRING:
+            s = col.str
+            sc = _lib.StrColumn(d(s.uid), d(s.val_off), d(s.byte_off), d(s.bytes, np.uint8), s.uid.size,
+                                int(s.byte_off.size - 1), int(s.byte_off[-1]))
+            keep.append(sc)
+            return _lib.ValColumn(col.type, None, None, None, None, None, C.pointer(sc), 0, 0), keep
+        return _lib.ValColumn(col.type, d(col.uid), d(col.val_off), d(col.word), d(col.nsec, np.uint32), None, None,
+                              col.uid.size, int(col.val_off[-1])), keep
+
+    n = 100_000_000
+    a_uid = np.arange(1, 2 * n, 2, dtype=U64)
+    a_col = algo.ValColumn.from_arrays(algo.VAL_INT64, a_uid, np.arange(n + 1, dtype=U64),
+                                       rng.integers(-10 ** 9, 10 ** 9, n).astype(np.int64))
+    a_cands = np.sort(rng.choice(a_uid, 20_000_000, replace=False))
+    nb = 10_000_000
+    b_cnt = rng.integers(1, 9, nb)
+    b_words = rng.normal(0, 100, int(b_cnt.sum()))
+    b_words[rng.random(b_words.size) < 0.05] = np.nan
+    b_off = np.zeros(nb + 1, U64)
+    np.cumsum(b_cnt, out=b_off[1:])
+    b_uid = np.arange(1, nb + 1, dtype=U64)
+    b_col = algo.ValColumn.from_arrays(algo.VAL_FLOAT64, b_uid, b_off, b_words)
+    names = gm.name_column(rng, 10_000_000)
+    c_col = algo.ValColumn.from_arrays(algo.VAL_STRING, str_col=names)
+    c_cands = np.sort(rng.choice(names.uid, 3_000_000, replace=False))
+    stored = [bytes(names.bytes[int(names.byte_off[j]):int(names.byte_off[j + 1])])
+              for j in rng.integers(0, names.byte_off.size - 1, 1000)]
+    e_col = algo.ValColumn(algo.VAL_INT64, np.arange(1, 22), [[int(x)] for x in rng.integers(0, 100, 21)])
+    work = [("C23a", a_col, "ge", [0], a_cands), ("C23b", b_col, "between", [-50.0, 50.0], b_uid),
+            ("C23c eq 1", c_col, "eq", [b"alice"], c_cands), ("C23c eq 1000", c_col, "eq", stored, c_cands),
+            ("C23c ge", c_col, "ge", [b"m"], c_cands), ("C23e", e_col, "ge", [50], np.arange(1, 22, dtype=U64)),
+            ("C23f", a_col, "ge", [0], np.sort(rng.choice(a_uid, 9, replace=False)))]
+    out_rows = []
+    dcols = {}
+    for name, col, op, args, cands in work:
+        t0 = time.perf_counter()
+        want = co.compare_uids(col, op, args, cands)
+        t_or = (time.perf_counter() - t0) * 1e3
+        if id(col) not in dcols:
+            dcols = {id(col): dev_col(col)}
+        dcol, _ = dcols[id(col)]
+        a = algo.ValArgs(col.type, args)
+        nc = int(cands.size)
+        d_u = up(cands)
+        d_out = torch.empty(nc + 1, dtype=torch.int64, device=DEV)
+        d_len = torch.empty(1, dtype=torch.int64, device=DEV)
+        d_cnt = torch.empty(nc + 1, dtype=torch.int32, device=DEV)
+
+        def dev():
+            algo.dev_compare_uids(L.h, dcol, op, a, d_u.data_ptr(), nc, d_out.data_ptr(), nc, d_len.data_ptr(),
+                                  d_counts=d_cnt.data_ptr())
+        ms_dev, _ = timeit(dev, warm=2, reps=10)
+        L.sync()
+        k = int(d_len.cpu().numpy()[0])
+        ok_dev = np.array_equal(d_out[:k].cpu().numpy().view(U64), want[0]) and \
+            np.array_equal(d_cnt[:nc].cpu().numpy().view(np.uint32), want[1])
+        algo.CompareUids(col, op, a, cands)
+        ts = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            got, cnt = algo.CompareUids(col, op, a, cands, counts=True)
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ok_host = np.array_equal(got.Uids, want[0]) and np.array_equal(cnt, want[1])
+        ncol = col.uid.size
+        lo = np.searchsorted(col.uid, cands)
+        hit = (lo < ncol) & (col.uid[np.minimum(lo, ncol - 1)] == cands)
+        pairs = int((col.val_off[lo[hit] + 1] - col.val_off[lo[hit]]).sum())
+        vbytes = pairs * 8 if col.type != algo.VAL_STRING else int(
+            (col.str.byte_off[col.val_off[lo[hit] + 1].astype(np.int64)] -
+             col.str.byte_off[col.val_off[lo[hit]].astype(np.int64)]).sum()) + pairs * 16
+        abytes = 16 * nc + vbytes + 16 * ncol
+        full = (f"{name}: {op} with {len(args)} argument(s); column of {ncol} uids, {int(col.val_off[-1])} values; "
+                f"UidList of {nc}; {pairs} (candidate, value) pairs; kept {want[0].size}")
+        kernels = None
+        if name in ("C23a", "C23b", "C23c eq 1"):  # each kernel's time and share of peak, in a profiled run of its own
+            kt = kernel_times(dev)
+            kb = {"fz_lookup_kernel": 16 * ncol + 24 * nc, "scan_u64_kernel": 16 * nc,
+                  "cmp_pairs_kernel": vbytes + 20 * nc, "cmp_finish_kernel": 9 * nc,
+                  "compact_kernel": 9 * nc + 8 * int(want[0].size)}
+            kernels = {k: {"ms": round(kt[k], 4), "algorithmic_bytes": b,
+                           "frac_of_hbm_peak": round(b / (kt[k] * 1e-3) / 1e9 / peak, 4)}
+                       for k, b in kb.items() if kt.get(k)}
+        for leg, ms, ok, timing in (("device form, resident", ms_dev, ok_dev, "CUDA events, median of 10 after 2 warm"),
+                                    ("host form", float(np.median(ts)), ok_host, "wall clock, median of 3 after 1 warm"),
+                                    ("restatement, 1 thread (C, not Go)", t_or, True, "orc_compare_uids, wall clock, "
+                                     "one run; the reference the other legs are checked against")):
+            r = {"op": "CompareUids", "workload": name, "leg": leg, "config": full, "ms": round(ms, 4),
+                 "candidates": nc, "check": bool(ok), "timing": timing}
+            if leg.startswith("device"):
+                gbs = abytes / (ms * 1e-3) / 1e9
+                r.update({"algorithmic_bytes": abytes, "algorithmic_GBps": round(gbs, 1),
+                          "frac_of_hbm_peak": round(gbs / peak, 4)})
+                if kernels:
+                    r["kernels"] = kernels
+            out_rows.append(r)
+            print(json.dumps(r), flush=True)
+        del d_u, d_out, d_len, d_cnt
+    dcols.clear()
+    # C23d: ge at root on a float index: rows are the buckets int64(f) of 1e7 values, row 0 the bucket of the argument
+    nd = 10_000_000
+    vals = rng.uniform(0, 10_000, nd)
+    d_uid = np.arange(1, nd + 1, dtype=U64)
+    d_col = algo.ValColumn.from_arrays(algo.VAL_FLOAT64, d_uid, np.arange(nd + 1, dtype=U64), vals)
+    arg = 2500.5
+    bk = vals.astype(np.int64)
+    order = np.lexsort((d_uid, bk))
+    keys, starts = np.unique(bk[order], return_index=True)
+    sel = keys >= int(arg)
+    rows_v = d_uid[order][starts[sel][0]:]
+    off = np.concatenate([starts[sel] - starts[sel][0], [rows_v.size]]).astype(U64)
+    nrows = int(sel.sum())
+    ra = algo.CompareRowArgs("ge", nrows, 1, True)
+    want_rows = co.compare_rows(d_col, "ge", [arg], [rows_v[int(off[r]):int(off[r + 1])] for r in range(nrows)], ra)
+    want = np.unique(np.concatenate(want_rows))
+    dcol, keep = dev_col(d_col)
+    a = algo.ValArgs(algo.VAL_FLOAT64, [arg])
+    M = rows_v.size
+    dv, doff = up(rows_v), up(off)
+    fo, foo = torch.empty(M + 1, dtype=torch.int64, device=DEV), torch.empty(nrows + 1, dtype=torch.int64, device=DEV)
+    dest, dlen = torch.empty(M + 1, dtype=torch.int64, device=DEV), torch.empty(1, dtype=torch.int64, device=DEV)
+    lib = _lib.load()
+
+    def chain():
+        algo.dev_compare_rows(L.h, dcol, "ge", a, dv.data_ptr(), doff.data_ptr(), nrows, M, ra, fo.data_ptr(),
+                              foo.data_ptr(), M)
+        _lib.check(lib.dgx_dev_merge_sorted_matrix(L.h, fo.data_ptr(), foo.data_ptr(), nrows, M, dest.data_ptr(), M,
+                                                   dlen.data_ptr()))
+
+    def merge_only():
+        _lib.check(lib.dgx_dev_merge_sorted_matrix(L.h, dv.data_ptr(), doff.data_ptr(), nrows, M, dest.data_ptr(), M,
+                                                   dlen.data_ptr()))
+    ms_m, _ = timeit(merge_only, warm=2, reps=10)
+    L.sync()
+    ms_c, _ = timeit(chain, warm=2, reps=10)
+    L.sync()
+    k = int(dlen.cpu().numpy()[0])
+    ok = np.array_equal(dest[:k].cpu().numpy().view(U64), want)
+    full = (f"C23d: ge({arg}) at root on a float index of {nd} values in {keys.size} buckets; the {nrows} index rows "
+            f"({M} uids) already resident, as the rows read leaves them (the read itself is not timed); row 0 of "
+            f"{int(off[1])} filtered; DestUIDs {want.size}")
+    for leg, ms, okk in (("device chain: rows -> compare_rows -> merge_sorted_matrix", ms_c, ok),
+                         ("device chain without the filter: rows -> merge_sorted_matrix", ms_m, True)):
+        r = {"op": "CompareRows", "workload": "C23d", "leg": leg, "config": full, "ms": round(ms, 4), "check": bool(okk),
+             "timing": "CUDA events, median of 10 after 2 warm"}
+        out_rows.append(r)
+        print(json.dumps(r), flush=True)
     return out_rows
 
 
