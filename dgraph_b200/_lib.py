@@ -184,6 +184,8 @@ SYMBOLS = {
     "dgx_compare_rows": (_int, [_int, C.POINTER(ValArgs), C.POINTER(ValColumn), _vp, _vp, _sz, _vp, _vp, _vp, _sz]),
     "dgx_var_order": (_int, [C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _sz, C.c_int32, C.c_int32, _vp, _vp, _sz,
                              _vp, _sz, _szp]),
+    "dgx_pred_order": (_int, [C.POINTER(ValColumn), _int, _vp, _sz, _vp, _vp, _sz, C.c_int32, C.c_int32, _vp, _vp,
+                              _sz, _vp, _sz, _szp]),
     "dgx_groupby_uid": (_int, [_vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _szp, _szp]),
     "dgx_pack_seek": (_int, [C.POINTER(PackView), _int, _u64, _int, _sz, _vp, _sz, _szp, _szp]),
     "dgx_encode_bound": (None, [_sz, C.c_uint32, _szp, _szp]),
@@ -244,6 +246,8 @@ SYMBOLS = {
                                     _vp, _vp, _sz]),
     "dgx_dev_var_order": (_int, [_vp, C.POINTER(MathLeaf), _int, _vp, _sz, _vp, _vp, _vp, _sz, _sz, C.c_int32,
                                  C.c_int32, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "dgx_dev_pred_order": (_int, [_vp, C.POINTER(ValColumn), _int, _vp, _sz, _vp, _vp, _vp, _sz, _sz, C.c_int32,
+                                  C.c_int32, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_dev_groupby_uid": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _sz, _sz, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "dgx_merge_matrix_overflows": (_u64, [_vp]),
     "dgx_filter_tail_queries": (_u64, [_vp]),

@@ -1282,6 +1282,42 @@ def dev_compare_rows(lane, dcol: "_lib.ValColumn", op, args: ValArgs, d_v: int, 
                                                 v_cap, _p(ra) if nrows else None, d_out, d_out_off, out_cap))
 
 
+def OrderByPred(col: ValColumn, desc: bool, dest, rows, count: int = 0, offset: int = 0):
+    """orderasc / orderdesc by a predicate without its index (query/query.go applyOrderAndPagination's predicate
+    branch with worker/sort.go sortWithoutIndex: sortByValue, paginate) in ONE call (dgx_pred_order), in Go's exact
+    order, ties included.
+
+    col: the predicate's ValColumn (VAL_INT64, VAL_FLOAT64, VAL_DATETIME or VAL_STRING, one value per uid; a bad value
+    counts as none); desc: orderdesc; dest: the node's DestUIDs; rows: its uid matrix (strictly ascending rows);
+    count / offset: the SortMessage's Count (already 1000 for 0, as the query layer sets it) and Offset.  Each row is
+    its dest uids with a value sorted by value, then those without one in row order, cut by x.PageRange.  Returns
+    (rows, dest): the ordered and paged rows and the new DestUIDs as a List.  A bool column, a negative count and a
+    list predicate's column raise DgxError (DGX_ERR_ARG), where Go returns an error."""
+    d = _u64(dest.Uids if isinstance(dest, List) else dest)
+    v, v_off = _csr_u64(rows)
+    nrows, M = len(rows), int(v_off[-1])
+    cs = col.struct()
+    out = np.empty(max(M, 1), np.uint64)
+    out_off = np.zeros(nrows + 1, np.uint64)
+    dout = np.empty(max(d.size, 1), np.uint64)
+    n = C.c_size_t(0)
+    _lib.check(_lib.load().dgx_pred_order(C.byref(cs), int(bool(desc)), _p(d), d.size, _p(v), _p(v_off), nrows,
+                                          count, offset, _p(out), _p(out_off), M, _p(dout), d.size, C.byref(n)))
+    return [out[int(out_off[i]):int(out_off[i + 1])].copy() for i in range(nrows)], List(dout[:n.value].copy())
+
+
+def dev_order_by_pred(lane, dcol: "_lib.ValColumn", desc: bool, d_dest: int, ndest: int, d_v: int, d_v_off: int,
+                      nrows: int, v_cap: int, d_out: int, d_out_off: int, out_cap: int, d_dest_out: int,
+                      dest_cap: int, d_dest_len: int, count: int = 0, offset: int = 0,
+                      d_ndest: int | None = None) -> None:
+    """The lane form of OrderByPred (dgx_dev_pred_order), asynchronous: dcol is a ValColumn struct whose arrays are
+    device memory (a resident column), every other pointer a device address; |dest| is ndest or the low 32 bits of
+    the device word d_ndest.  Refusals found on the device surface at dgx_lane_sync."""
+    _lib.check(_lib.load().dgx_dev_pred_order(lane, C.byref(dcol), int(bool(desc)), d_dest, ndest, d_ndest, d_v,
+                                              d_v_off, nrows, v_cap, count, offset, d_out, d_out_off, out_cap,
+                                              d_dest_out, dest_cap, d_dest_len))
+
+
 def _exact(p) -> int:
     from .codec import ExactLen
 

@@ -51,6 +51,7 @@
 #include "regex_kernel.cuh"
 #include "regex_compile.hpp"
 #include "compare_kernel.cuh"
+#include "pred_order_kernel.cuh"
 #include "wire.hpp"
 #include "ws_layout.hpp"
 
@@ -566,6 +567,11 @@ extern "C" int dgx_lane_sync(dgx_lane* l) {
             return fail(DGX_ERR_ARG, "a compare function's input is refused (candidates or column uids not strictly "
                                      "ascending, column or row offsets malformed, a length word past its room, or a "
                                      "candidate's value whose conversion failed)");
+        if (flag & kLaneErrPredOrder)
+            return fail(DGX_ERR_ARG, "an order-by-predicate input is refused (dest, a row or column uids not strictly "
+                                     "ascending, row or column offsets malformed, a length word past its room, a "
+                                     "row uid owning several values, which Go refuses as a list predicate, or a "
+                                     "datetime value's nanoseconds of 10^9 or more)");
         if (flag & kLaneErrMut)
             return fail(DGX_ERR_ARG, "a mutable layer is malformed (entries not strictly ascending, uid 0 or unknown "
                                      "flags) or a probe / iterate / unfiltered row's pack starts at uid 0");
@@ -7013,6 +7019,258 @@ extern "C" int dgx_compare_rows(int op, const dgx_val_args* args, const dgx_val_
     d_off = d_out + m + 1;
     if ((rc = cmp_rows_run(l, op, A, D, DS, d_v, d_voff, nrows, m, row_arg, d_out, d_off))) return rc;
     return batch_to_host(l, d_out, d_off, nrows, out, out_off, out_cap);
+}
+
+// ---------------------------------------------------------------------------
+// orderasc / orderdesc by a predicate without its index: sortWithoutIndex's value sort over a typed value column,
+// nulls last, paged (pred_order_kernel.cuh)
+// ---------------------------------------------------------------------------
+
+// The column's checks both forms make before anything is copied: the four sortable types, then compare's checks.
+static int po_check_column(const dgx_val_column* c, bool host, dgx_str_column* S) {
+    if (!c) return fail(DGX_ERR_ARG, "null column");
+    const int t = c->type;
+    if (t != DGX_VAL_INT64 && t != DGX_VAL_FLOAT64 && t != DGX_VAL_DATETIME && t != DGX_VAL_STRING)
+        return fail(DGX_ERR_ARG, "type %d is not ordered on the device (int64, float64, datetime or string)", t);
+    return cmp_check_column(c, host, S);
+}
+
+// The datetime key sort's passes: the nanoseconds, then the seconds.
+static uint32_t po_key_passes(int type) { return type == DGX_VAL_DATETIME ? PO_NS_PASSES + VO_KEY_PASSES : VO_KEY_PASSES; }
+
+// The whole call on the lane: 38 + 3 P_r launches (51 + 3 P_r for datetime).  Workspace: words, tickets and the
+// look-back words, zeroed; per value slot of v_cap about 140 bytes (U and W flags and their scans 32, value index 4,
+// N 8, W's uids, words, extras and rows 28, keys 16, radix keys and payloads 24, pair slots 4, the radix hist); per
+// row 44; 16 per dest slot.
+static int po_run(dgx_lane* l, const dgx_val_column& col, const dgx_str_column& S, int desc, const uint64_t* dest,
+                  const uint64_t* dlen, uint64_t dcap, const uint64_t* v, const uint64_t* v_off, uint64_t nrows,
+                  uint64_t v_cap, int32_t count, int32_t offset, uint64_t* out, uint64_t* out_off,
+                  uint64_t* dest_out, uint64_t* dest_len) {
+    const uint64_t vc = std::max<uint64_t>(v_cap, 1), tv = scan_tiles(vc), tr = scan_tiles(nrows), td = scan_tiles(dcap);
+    const uint64_t tiles = (vc + GB_TILE - 1) / GB_TILE, hn = (uint64_t)GB_RADIX * tiles, th = scan_tiles(hn);
+    const uint32_t pr = vo_row_passes(nrows), kp = po_key_passes(col.type);
+    PoParams P{};
+    FzParams& F = P.F;
+    u64 *status, *ek[2], *hist, *hoff;
+    u32 *tickets, *ep[2];
+    WsCarve ws(l);
+    ws.zeroed(&P.bad, 4);
+    ws.zeroed(&P.words, VO_WORDS);
+    ws.zeroed(&F.words, 4);
+    ws.zeroed(&tickets, 32);
+    ws.zeroed(&status, 2 * tv + (kp + pr) * th + tr + td);
+    ws.zeroed(&P.rflag, nrows);
+    ws.zeroed(&P.mark, dcap);
+    ws.plain(&P.uf, vc);
+    ws.plain(&P.ux, vc + 1);
+    ws.plain(&P.wf, vc);
+    ws.plain(&P.wx, vc + 1);
+    ws.plain(&P.N, vc);
+    ws.plain(&P.wuid, vc);
+    ws.plain(&P.wword, vc);
+    ws.plain(&P.wext, vc);
+    ws.plain(&P.okey, vc);
+    ws.plain(&P.okey2, vc);
+    ws.plain(&ek[0], vc);
+    ws.plain(&ek[1], vc);
+    ws.plain(&hist, hn);
+    ws.plain(&hoff, hn + 1);
+    ws.plain(&P.uoff, nrows + 1);
+    ws.plain(&P.woff, nrows + 1);
+    ws.plain(&P.plen, nrows);
+    ws.plain(&P.po, nrows + 1);
+    ws.plain(&P.mx, dcap + 1);
+    ws.plain(&P.vj, vc);
+    ws.plain(&P.wrow, vc);
+    ws.plain(&ep[0], vc);
+    ws.plain(&ep[1], vc);
+    ws.plain(&P.pairs, vc);
+    ws.plain(&P.longrows, nrows);
+    ws.plain(&P.pstart, nrows);
+    if (int rc = ws.commit()) return rc;
+    F.uid = (const u64*)S.uid;
+    F.val_off = (const u64*)S.val_off;
+    F.byte_off = (const u64*)S.byte_off;
+    F.bytes = S.bytes;
+    F.n = S.n;
+    F.nvals = S.nvals;
+    F.nbytes = S.nbytes;
+    F.err = l->d_err;
+    F.err_bit = kLaneErrPredOrder;
+    F.ccap = 0;  // the lookup checks the column alone
+    P.type = (u32)col.type;
+    P.desc = desc != 0;
+    P.word = (const u64*)col.word;
+    P.nsec = col.nsec;
+    P.vbad = col.bad;
+    P.dest = (const u64*)dest;
+    P.dlen = (const u64*)dlen;
+    P.dcap = dcap;
+    P.v = (const u64*)v;
+    P.v_off = (const u64*)v_off;
+    P.nrows = nrows;
+    P.v_cap = v_cap;
+    P.count = count;
+    P.offset = offset;
+    P.tiles = tiles;
+    P.err = l->d_err;
+    P.ticket = tickets + 31;
+    P.ek = ek[0];
+    P.ep = ep[0];
+    P.out = (u64*)out;
+    P.out_off = (u64*)out_off;
+    P.dest_out = (u64*)dest_out;
+    P.dest_len = (u64*)dest_len;
+    u32* ticket = tickets;
+    auto scan = [&](const u64* in, u64* o, const u64* n_word, uint64_t n, u64* total) {
+        const uint64_t t = scan_tiles(n);
+        scan_u64_kernel<<<(unsigned)t, EN_NT, 0, l->stream>>>(in, o, n_word, n, status, ticket, total);
+        status += t;
+        ticket += 1;
+    };
+    fz_lookup_kernel<<<gb_grid(std::max<uint64_t>(S.n + 1, S.nvals + 1)), 256, 0, l->stream>>>(F);
+    po_check_kernel<<<gb_grid(std::max<uint64_t>({dcap, nrows + 1, v_cap})), 256, 0, l->stream>>>(P);
+    po_gather_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P);
+    scan(P.uf, P.ux, P.words + VO_W_M, vc, nullptr);
+    scan(P.wf, P.wx, P.words + VO_W_M, vc, P.words + VO_W_W);
+    po_compact_kernel<<<gb_grid(std::max<uint64_t>(v_cap, nrows + 1)), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 6);
+    // W by key (the result is back in buffer c after an even number of passes): a datetime by its nanoseconds, then
+    // stably by its seconds; then stably by row
+    int c = 0;
+    auto sort = [&](uint32_t passes) {
+        u64* const k[2] = {ek[c], ek[c ^ 1]};
+        u32* const p[2] = {ep[c], ep[c ^ 1]};
+        const int rc = gb_sort(l, tiles, P.bad, P.words + VO_W_H, k, p, P.words + VO_W_W, passes, hist, hoff, status,
+                               ticket);
+        c ^= (int)(passes & 1);
+        return rc;
+    };
+    if (col.type == DGX_VAL_DATETIME) {
+        if (int rc = sort(PO_NS_PASSES)) return rc;
+        po_rekey_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P, P.okey, ep[c], ek[c ^ 1], ep[c ^ 1]);
+        CK(cudaGetLastError());
+        count_launches(l, 1);
+        c ^= 1;
+    }
+    if (int rc = sort(VO_KEY_PASSES)) return rc;
+    po_rekey_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P, nullptr, ep[c], ek[c ^ 1], ep[c ^ 1]);
+    c ^= 1;
+    if (int rc = sort(pr)) return rc;
+    P.S = ep[c];
+    po_tier_kernel<<<gb_grid(v_cap), 256, 0, l->stream>>>(P);
+    po_rows_kernel<<<gb_grid(nrows), 256, 0, l->stream>>>(P);
+    vo_cta_kernel<<<(unsigned)(2 * g_num_sms), VO_NT, 0, l->stream>>>(P);
+    scan(P.plen, P.po, P.words + VO_W_R, nrows, nullptr);
+    po_write_kernel<<<gb_grid(std::max<uint64_t>(v_cap, nrows + 1)), 256, 0, l->stream>>>(P);
+    scan(P.mark, P.mx, P.words + VO_W_ND, dcap, nullptr);
+    vo_dest_kernel<<<gb_grid(dcap), 256, 0, l->stream>>>(P);
+    CK(cudaGetLastError());
+    count_launches(l, 8);
+    return DGX_OK;
+}
+
+// The arguments both forms refuse before anything is copied.
+static int po_check_args(int32_t count, uint64_t ndest, uint64_t nrows) {
+    if (count < 0) return fail(DGX_ERR_ARG, "count %d: processSort refuses a negative count", count);
+    if (ndest >= kVoMax || nrows >= kVoMax)
+        return fail(DGX_ERR_ARG, "sizes are 32-bit: ndest %llu, nrows %llu", (unsigned long long)ndest,
+                    (unsigned long long)nrows);
+    return DGX_OK;
+}
+
+extern "C" int dgx_dev_pred_order(dgx_lane* l, const dgx_val_column* col, int desc, const uint64_t* d_dest,
+                                  size_t ndest, const uint64_t* d_ndest, const uint64_t* d_v, const uint64_t* d_v_off,
+                                  size_t nrows, size_t v_cap, int32_t count, int32_t offset, uint64_t* d_out,
+                                  uint64_t* d_out_off, size_t out_cap, uint64_t* d_dest_out, size_t dest_cap,
+                                  uint64_t* d_dest_len) {
+    if (!l || !d_dest_len || !d_v_off || !d_out_off) return fail(DGX_ERR_ARG, "null argument");
+    dgx_str_column S;
+    if (int rc = po_check_column(col, false, &S)) return rc;
+    if (int rc = po_check_args(count, ndest, nrows)) return rc;
+    if (v_cap >= kVoMax) return fail(DGX_ERR_ARG, "v_cap %zu: at most 2^32 - 1", v_cap);
+    if ((ndest && !d_dest) || (v_cap && !d_v)) return fail(DGX_ERR_ARG, "null argument");
+    if (out_cap < v_cap || dest_cap < ndest)
+        return fail(DGX_ERR_CAP, "out_cap %zu / dest_cap %zu below the bounds %zu / %zu", out_cap, dest_cap, v_cap,
+                    ndest);
+    if ((v_cap && !d_out) || (ndest && !d_dest_out)) return fail(DGX_ERR_ARG, "null argument");
+    if (int rc = lane_begin_op(l)) return rc;
+    g_stats.calls += 1;
+    l->note_output(d_dest_len, sizeof(uint64_t));
+    l->note_output(d_out_off, (nrows + 1) * sizeof(uint64_t));
+    if (ndest == 0 || nrows == 0) {  // no dest value or no row: every row is empty, so is the new dest
+        CK(cudaMemsetAsync(d_dest_len, 0, sizeof(uint64_t), l->stream));
+        CK(cudaMemsetAsync(d_out_off, 0, (nrows + 1) * sizeof(uint64_t), l->stream));
+        return DGX_OK;
+    }
+    if (int rc = po_run(l, *col, S, desc, d_dest, d_ndest, ndest, d_v, d_v_off, nrows, v_cap, count, offset, d_out,
+                        d_out_off, d_dest_out, d_dest_len))
+        return rc;
+    g_stats.uids_in += ndest + v_cap;
+    l->note_output(d_out, out_cap * sizeof(uint64_t));
+    l->note_output(d_dest_out, dest_cap * sizeof(uint64_t));
+    return DGX_OK;
+}
+
+extern "C" int dgx_pred_order(const dgx_val_column* col, int desc, const uint64_t* dest, size_t ndest,
+                              const uint64_t* v, const uint64_t* v_off, size_t nrows, int32_t count, int32_t offset,
+                              uint64_t* out, uint64_t* out_off, size_t out_cap, uint64_t* dest_out, size_t dest_cap,
+                              size_t* dest_len) {
+    if (!dest_len || !v_off || !out_off) return fail(DGX_ERR_ARG, "null argument");
+    int rc;
+    dgx_str_column S;
+    if ((rc = po_check_column(col, true, &S))) return rc;
+    if ((rc = po_check_args(count, ndest, nrows))) return rc;
+    if ((rc = check_offsets("v_off", v_off, nrows, kVoMax))) return rc;
+    const uint64_t m = v_off[nrows];
+    if ((ndest && !dest) || (m && !v)) return fail(DGX_ERR_ARG, "null argument");
+    if (out_cap < m || dest_cap < ndest)
+        return fail(DGX_ERR_CAP, "out_cap %zu / dest_cap %zu below the bounds %llu / %zu", out_cap, dest_cap,
+                    (unsigned long long)m, ndest);
+    if ((m && !out) || (ndest && !dest_out)) return fail(DGX_ERR_ARG, "null argument");
+    if (ndest == 0 || nrows == 0) {  // no dest value or no row: every row is empty, so is the new dest
+        *dest_len = 0;
+        memset(out_off, 0, (nrows + 1) * sizeof(uint64_t));
+        return DGX_OK;
+    }
+    LaneLease lease;
+    if (lease.rc) return lease.rc;
+    dgx_lane* l = lease.l;
+    g_stats.calls += 1;
+    g_stats.uids_in += ndest + m;
+    dgx_val_column D;
+    dgx_str_column DS;
+    if ((rc = cmp_upload_column(l, col, &D, &S, &DS))) return rc;
+    uint64_t *d_dest, *d_v, *d_v_off;
+    if ((rc = upload_list(l, dest, ndest, &d_dest)) || (rc = upload_list(l, v, m, &d_v)) ||
+        (rc = upload_list(l, v_off, nrows + 1, &d_v_off)))
+        return rc;
+    uint64_t *o_len, *o_dest, *o_out, *o_off;
+    WsCarve o(l);
+    o.plain(&o_len, 1);
+    o.plain(&o_dest, ndest);
+    o.plain(&o_out, m);
+    o.plain(&o_off, nrows + 1);
+    if ((rc = o.commit())) return rc;
+    if ((rc = po_run(l, D, DS, desc, d_dest, nullptr, ndest, d_v, d_v_off, nrows, m, count, offset, o_out, o_off,
+                     o_dest, o_len)))
+        return rc;
+    CK(cudaMemcpyAsync(l->h_word, o_len, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaMemcpyAsync(l->h_word + 1, o_off + nrows, sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if ((rc = dgx_lane_sync(l))) {
+        *dest_len = 0;
+        return rc;
+    }
+    const uint64_t DN = l->h_word[0], K = l->h_word[1];
+    *dest_len = DN;
+    CK(cudaMemcpyAsync(out_off, o_off, (nrows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (DN) CK(cudaMemcpyAsync(dest_out, o_dest, DN * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    if (K) CK(cudaMemcpyAsync(out, o_out, K * sizeof(uint64_t), cudaMemcpyDeviceToHost, l->stream));
+    CK(cudaStreamSynchronize(l->stream));
+    g_stats.d2h += (DN + K + nrows + 3) * sizeof(uint64_t);
+    g_stats.uids_out += DN + K;
+    return DGX_OK;
 }
 
 extern "C" uint64_t dgx_merge_matrix_overflows(const dgx_lane* l) { return l ? l->xm_overflows : g_xm_overflows.load(); }

@@ -192,16 +192,23 @@ struct VoRow {
     }
 };
 
+// W of row-start b0 as the sort reads it
+__device__ __forceinline__ VoRow vo_row(const VoParams& P, u64 b0) {
+    return VoRow{P.wtag + b0, P.wword + b0, P.wuid + b0, P.desc != 0};
+}
+
 // ---- Go's pdqsort (sort/zsortinterface.go), one thread -------------------------------------------------------------
 
 __device__ __forceinline__ int vo_bits_len(u64 x) { return x ? 64 - __clzll((long long)x) : 0; }
 
-__device__ __forceinline__ void vo_insertion_sort(const VoRow& d, long a, long b) {
+template <class Row>
+__device__ __forceinline__ void vo_insertion_sort(const Row& d, long a, long b) {
     for (long i = a + 1; i < b; i++)
         for (long j = i; j > a && d.less(j, j - 1); j--) d.swap(j, j - 1);
 }
 
-__device__ __forceinline__ void vo_sift_down(const VoRow& d, long lo, long hi, long first) {
+template <class Row>
+__device__ __forceinline__ void vo_sift_down(const Row& d, long lo, long hi, long first) {
     long root = lo;
     for (;;) {
         long child = 2 * root + 1;
@@ -213,7 +220,8 @@ __device__ __forceinline__ void vo_sift_down(const VoRow& d, long lo, long hi, l
     }
 }
 
-__device__ __forceinline__ void vo_heap_sort(const VoRow& d, long a, long b) {
+template <class Row>
+__device__ __forceinline__ void vo_heap_sort(const Row& d, long a, long b) {
     const long first = a, lo = 0, hi = b - a;
     for (long i = (hi - 1) / 2; i >= 0; i--) vo_sift_down(d, i, hi, first);
     for (long i = hi - 1; i >= 0; i--) {
@@ -223,7 +231,8 @@ __device__ __forceinline__ void vo_heap_sort(const VoRow& d, long a, long b) {
 }
 
 // partition with the pivot already swapped to a: returns mid, sets *already
-__device__ __forceinline__ long vo_partition(const VoRow& d, long a, long b, bool* already) {
+template <class Row>
+__device__ __forceinline__ long vo_partition(const Row& d, long a, long b, bool* already) {
     long i = a + 1, j = b - 1;
     while (i <= j && d.less(i, a)) i++;
     while (i <= j && !d.less(j, a)) j--;
@@ -247,7 +256,8 @@ __device__ __forceinline__ long vo_partition(const VoRow& d, long a, long b, boo
 }
 
 // partitionEqual with the pivot already swapped to a
-__device__ __forceinline__ long vo_partition_equal(const VoRow& d, long a, long b) {
+template <class Row>
+__device__ __forceinline__ long vo_partition_equal(const Row& d, long a, long b) {
     long i = a + 1, j = b - 1;
     for (;;) {
         while (i <= j && !d.less(a, i)) i++;
@@ -260,7 +270,8 @@ __device__ __forceinline__ long vo_partition_equal(const VoRow& d, long a, long 
     return i;
 }
 
-__device__ __forceinline__ bool vo_partial_insertion_sort(const VoRow& d, long a, long b) {
+template <class Row>
+__device__ __forceinline__ bool vo_partial_insertion_sort(const Row& d, long a, long b) {
     constexpr int kMaxSteps = 5;
     constexpr long kShortestShifting = 50;
     long i = a + 1;
@@ -285,7 +296,8 @@ __device__ __forceinline__ bool vo_partial_insertion_sort(const VoRow& d, long a
     return false;
 }
 
-__device__ __forceinline__ void vo_break_patterns(const VoRow& d, long a, long b) {
+template <class Row>
+__device__ __forceinline__ void vo_break_patterns(const Row& d, long a, long b) {
     const long length = b - a;
     if (length >= 8) {
         u64 random = (u64)length;  // xorshift seeded by the length
@@ -302,7 +314,8 @@ __device__ __forceinline__ void vo_break_patterns(const VoRow& d, long a, long b
     }
 }
 
-__device__ __forceinline__ void vo_order2(const VoRow& d, long& a, long& b, int& swaps) {
+template <class Row>
+__device__ __forceinline__ void vo_order2(const Row& d, long& a, long& b, int& swaps) {
     if (d.less(b, a)) {
         swaps++;
         const long t = a;
@@ -311,7 +324,8 @@ __device__ __forceinline__ void vo_order2(const VoRow& d, long& a, long& b, int&
     }
 }
 
-__device__ __forceinline__ long vo_median(const VoRow& d, long a, long b, long c, int& swaps) {
+template <class Row>
+__device__ __forceinline__ long vo_median(const Row& d, long a, long b, long c, int& swaps) {
     vo_order2(d, a, b, swaps);
     vo_order2(d, b, c, swaps);
     vo_order2(d, a, b, swaps);
@@ -320,7 +334,8 @@ __device__ __forceinline__ long vo_median(const VoRow& d, long a, long b, long c
 
 constexpr int VO_HINT_UNKNOWN = 0, VO_HINT_INC = 1, VO_HINT_DEC = 2;
 
-__device__ __forceinline__ long vo_choose_pivot(const VoRow& d, long a, long b, int& hint) {
+template <class Row>
+__device__ __forceinline__ long vo_choose_pivot(const Row& d, long a, long b, int& hint) {
     constexpr long kShortestNinther = 50;
     constexpr int kMaxSwaps = 4 * 3;
     const long l = b - a;
@@ -338,7 +353,8 @@ __device__ __forceinline__ long vo_choose_pivot(const VoRow& d, long a, long b, 
     return j;
 }
 
-__device__ __forceinline__ void vo_reverse_range(const VoRow& d, long a, long b) {
+template <class Row>
+__device__ __forceinline__ void vo_reverse_range(const Row& d, long a, long b) {
     long i = a, j = b - 1;
     while (i < j) {
         d.swap(i, j);
@@ -359,7 +375,8 @@ constexpr int VO_DONE = 0, VO_PART = 1, VO_PART_EQUAL = 2;
 
 // Runs the loop until it needs a partition of [f.a, f.b) (the pivot already swapped to f.a): VO_PART or
 // VO_PART_EQUAL; VO_DONE when the sort has finished.
-__device__ __forceinline__ int vo_advance(const VoRow& d, VoFrame& f, VoFrame* st, int& top) {
+template <class Row>
+__device__ __forceinline__ int vo_advance(const Row& d, VoFrame& f, VoFrame* st, int& top) {
     for (;;) {
         const long a = f.a, b = f.b, length = b - a;
         bool ret = false;
@@ -417,7 +434,8 @@ __device__ __forceinline__ void vo_after(VoFrame& f, VoFrame* st, int& top, int 
 }
 
 // sort.Sort on one thread
-__device__ __forceinline__ void vo_sort_thread(const VoRow& d, long n) {
+template <class Row>
+__device__ __forceinline__ void vo_sort_thread(const Row& d, long n) {
     if (n <= 1) return;
     VoFrame st[VO_STACK_THREAD];
     int top = 0;
@@ -596,8 +614,9 @@ __device__ __forceinline__ u32 vo_block_rank(bool g, u32* total) {
 // when Less(i, a) (partition) or !Less(a, i) (partitionEqual); with m of them, the left part is [a + 1, a + m].  Go's
 // Hoare loop swaps the k-th entry of the left part that goes right, counted from the left, with the k-th entry of the
 // right part that goes left, counted from the right.  Returns mid (before partition's final swap) and the pair count.
-__device__ __forceinline__ void vo_coop_partition(const VoRow& d, long a, long b, bool eq, u32* pairs, long* mid, u64* npairs) {
-    const VoVal pv = d.at(a);
+template <class Row>
+__device__ __forceinline__ void vo_coop_partition(const Row& d, long a, long b, bool eq, u32* pairs, long* mid, u64* npairs) {
+    const auto pv = d.at(a);
     auto left = [&](long i) { return eq ? !vo_Less(pv, d.at(i), d.desc) : vo_Less(d.at(i), pv, d.desc); };
     u64 c = 0;
     for (long i = a + 1 + threadIdx.x; i < b; i += VO_NT) c += left(i);
@@ -629,7 +648,8 @@ __device__ __forceinline__ void vo_coop_partition(const VoRow& d, long a, long b
 // Fixed grid of VO_NT-thread CTAs: each pulls long tier-2 rows from the counter and runs Go's pdqsort over it, thread 0
 // driving the loop and the whole CTA computing each partition.  Like vo_rows_kernel it declares one CTA per SM as its
 // minimum: with the default occupancy target ptxas spills the inlined pdqsort at 40 registers.
-__global__ void __launch_bounds__(VO_NT, 1) vo_cta_kernel(const VoParams P) {
+template <class Params>
+__global__ void __launch_bounds__(VO_NT, 1) vo_cta_kernel(const Params P) {
     __shared__ VoFrame s_f;
     __shared__ VoFrame s_st[VO_STACK_CTA];
     __shared__ int s_top, s_kind;
@@ -643,7 +663,7 @@ __global__ void __launch_bounds__(VO_NT, 1) vo_cta_kernel(const VoParams P) {
         if (i >= nlong) return;
         const u32 r = P.longrows[i];
         const u64 b0 = P.woff[r], n = P.woff[r + 1] - b0;
-        const VoRow d{P.wtag + b0, P.wword + b0, P.wuid + b0, P.desc != 0};
+        const auto d = vo_row(P, b0);
         if (threadIdx.x == 0) {
             s_f = VoFrame{0, (u32)n, vo_bits_len(n), 1, 1};
             s_top = 0;
@@ -684,7 +704,8 @@ __global__ void __launch_bounds__(256) vo_write_kernel(const VoParams P) {
 }
 
 // Grid over dcap threads.
-__global__ void __launch_bounds__(256) vo_dest_kernel(const VoParams P) {
+template <class Params>
+__global__ void __launch_bounds__(256) vo_dest_kernel(const Params P) {
     const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (*P.bad) {
         if (t == 0) *P.dest_len = 0;

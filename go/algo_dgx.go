@@ -1082,6 +1082,65 @@ func OrderByVar(m MathLeaf, desc bool, dest []uint64, rows []*pb.List, count, of
 	return res, destOut[:n], true
 }
 
+// dgxMinPredOrder: below this many dest values plus row values a node's order by a predicate stays in Go
+// (applyOrderAndPagination's predicate branch).  No measurement of the call exists yet, so this is the
+// dgxMinMergeMatrix bound until one sets it.
+const dgxMinPredOrder = dgxMinMergeMatrix
+
+// OrderByPred runs applyOrderAndPagination's predicate branch for a predicate whose sortWithIndex fails before it
+// reads (no index, or no sortable tokenizer: worker/sort.go:210-240), so that processSort's answer is always
+// sortWithoutIndex's (worker/sort.go:139-187, sortByValue, paginate), in one dgx_pred_order call.  col holds the
+// predicate's values as fetchValue reads them (ValueFor at ReadTs, types.Convert to the schema type, a failed
+// conversion marked Bad, an absent value left out); order is sg.Params.Order; sortable reports whether sortWithIndex
+// could run; isList the schema's list flag; dest is sg.DestUIDs, rows the matrix updateUidMatrix left, count (already
+// 1000 for 0) / offset the SortMessage's.  It returns the new rows and DestUIDs.  ok == false -- a sortable index (the
+// answer is then a race with the indexed sort), more than one order key (multiSort), Langs, FacetsOrder, a list
+// predicate, a type other than int64, float64, datetime and string (bool keeps Go's error and its all-null case),
+// sizes outside the library's bounds, below dgxMinPredOrder values, or any library error -- means the caller keeps
+// SortOverNetwork.  The facets reorder after the sort stays in Go.
+func OrderByPred(col *ValColumn, order []*pb.Order, sortable, isList, facetsOrder bool, dest []uint64,
+	rows []*pb.List, count, offset int) ([][]uint64, []uint64, bool) {
+	if sortable || len(order) != 1 || len(order[0].Langs) > 0 || facetsOrder || isList || count < 0 ||
+		count != int(int32(count)) || offset != int(int32(offset)) {
+		return nil, nil, false
+	}
+	switch col.Type {
+	case ValInt64, ValFloat64, ValDateTime, ValString:
+	default:
+		return nil, nil, false
+	}
+	mv, nrows := totalUids(rows), len(rows)
+	if len(dest)+mv < dgxMinPredOrder {
+		return nil, nil, false
+	}
+	pc, _, free := cValCall(col, &ValArgs{})
+	defer free()
+	v, vOff := make([]uint64, 0, mv+1), make([]uint64, 1, nrows+1)
+	for _, r := range rows {
+		if r != nil {
+			v = append(v, r.Uids...)
+		}
+		vOff = append(vOff, uint64(len(v)))
+	}
+	d := append(make([]uint64, 0, len(dest)+1), dest...)
+	destOut, out, outOff := make([]uint64, len(dest)+1), make([]uint64, mv+1), make([]uint64, nrows+1)
+	var n C.size_t
+	isDesc := C.int(0)
+	if order[0].Desc {
+		isDesc = 1
+	}
+	if C.dgx_pred_order((*C.dgx_val_column)(pc), isDesc, u64ptr(d), C.size_t(len(dest)), u64ptr(v), u64ptr(vOff),
+		C.size_t(nrows), C.int32_t(count), C.int32_t(offset), u64ptr(out), u64ptr(outOff), C.size_t(mv),
+		u64ptr(destOut), C.size_t(len(dest)), &n) != C.DGX_OK {
+		return nil, nil, false
+	}
+	res := make([][]uint64, nrows)
+	for i := range res {
+		res[i] = out[outOff[i]:outOff[i+1]:outOff[i+1]]
+	}
+	return res, destOut[:n], true
+}
+
 // dgxMinMatch: below this many candidates a match() stays in Go (handleMatchFunction).  The C21 record
 // (profiles/h100_c21_match.json) times the library against a C restatement of that loop, not against Go, so this is
 // the dgxMinMergeMatrix bound until a Go comparison sets it.

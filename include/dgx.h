@@ -893,6 +893,37 @@ int dgx_compare_rows(int op, const dgx_val_args* args, const dgx_val_column* col
                      const uint64_t* v_off, size_t nrows, const uint32_t* row_arg, uint64_t* out, uint64_t* out_off,
                      size_t out_cap);
 
+/* orderasc / orderdesc by a predicate whose values have no sortable index (query/query.go applyOrderAndPagination
+ * :2511-2592, predicate branch, with worker/sort.go sortWithoutIndex :139-187: sortByValue :775-822, fetchValue and
+ * paginate :740-773), in Go's exact order.  processSort returns sortWithoutIndex's answer whenever sortWithIndex
+ * fails before reading, that is for a predicate with no index or no sortable tokenizer; for an indexed predicate its
+ * answer is a race with the indexed sort, which this call does not restate.  dest, v and v_off are dgx_var_order's:
+ * the node's DestUIDs (strictly ascending) and its uid matrix (strictly ascending rows, v_off[0] == 0).  col is the
+ * predicate's typed value column (dgx_val_column) of type DGX_VAL_INT64, DGX_VAL_FLOAT64, DGX_VAL_DATETIME or
+ * DGX_VAL_STRING, one value per uid (Go refuses to sort by a list predicate).
+ * Each row keeps, in row order, its uids in dest (U).  W is U's uids with a value, N the rest: a uid absent from the
+ * column, owning no value, or whose value is marked bad (fetchValue's error: no value, or a failed conversion).  The
+ * row becomes W sorted by types.Sort(values, &uids, []bool{desc}, ""): sort.Sort(byValue), Go's pdqsort with its tie
+ * order, under byValue.Less (equal values are not less; otherwise types.less, negated for desc: int64 <, float64 < with
+ * -0 equal to +0 and a NaN neither less nor equal, datetime the instant, strings bytewise and unsigned with a proper
+ * prefix less), followed by N in row order, unsorted; then it is cut to x.PageRange(count, offset, |U|).  The query
+ * layer replaces a count of 0 with 1000 before processSort; this call applies the count it is given.  The new dest is
+ * the dest values some row still holds.  Writes the rows to out / out_off (nrows + 1 offsets) and the new dest to
+ * dest_out (*dest_len values).
+ * DGX_ERR_ARG before anything is copied: a null column, DGX_VAL_BOOL (SortWithFacet refuses a bool as not sortable)
+ * or an unknown type, count < 0 (processSort refuses it), ndest, nrows, v_off[nrows] or the column's sizes of 2^32 or
+ * more, v_off or the column's offsets not starting at 0 or decreasing (and not ending at nvals / nbytes), a null
+ * array that is needed.  DGX_ERR_CAP before anything is copied: out_cap below v_off[nrows] or dest_cap below ndest.
+ * DGX_ERR_ARG after the kernels, with nothing written but *dest_len = 0: dest, a row or the column's uids not strictly
+ * ascending, a U uid owning more than one value, or a U uid's datetime value with nanoseconds of 10^9 or more.  Bad
+ * values, and the values of uids outside U, are not otherwise read.  ndest == 0 or nrows == 0 writes zero offsets and
+ * *dest_len = 0 and needs no device.
+ * Launches: 38 + 3 ceil(b_r / 8) for int64, float64 and string columns and 51 + 3 ceil(b_r / 8) for datetime, b_r the
+ * bit width of nrows - 1 (DESIGN section 3.20), whatever the values, ties, column size and the rows' tiers. */
+int dgx_pred_order(const dgx_val_column* col, int desc, const uint64_t* dest, size_t ndest, const uint64_t* v,
+                   const uint64_t* v_off, size_t nrows, int32_t count, int32_t offset, uint64_t* out, uint64_t* out_off,
+                   size_t out_cap, uint64_t* dest_out, size_t dest_cap, size_t* dest_len);
+
 /* codec.Decoder positioned calls (codec/codec.go:154-384), one call each, computed on the device:
  *   kind 0 Decoder.Seek(uid, whence)          :279-337   whence 0 = SeekStart (>= uid), 1 = SeekCurrent (> uid)
  *   kind 1 Decoder.SeekToBlock(uid, whence)   :219-271   resumes the base search at block_idx
@@ -1260,6 +1291,20 @@ int dgx_dev_compare_uids(dgx_lane* lane, int op, const dgx_val_args* args, const
 int dgx_dev_compare_rows(dgx_lane* lane, int op, const dgx_val_args* args, const dgx_val_column* col,
                          const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows, size_t v_cap,
                          const uint32_t* row_arg, uint64_t* d_out, uint64_t* d_out_off, size_t out_cap);
+/* Device form of dgx_pred_order, with dgx_dev_var_order's rules: col is a host struct whose arrays (its str's
+ * included) are device memory, d_dest, the rows and the outputs are device memory, so dgx_dev_sg_filter's new dest
+ * and rows and a resident column feed it without a host read.  |dest| is ndest, or the low 32 bits of the device word
+ * d_ndest when it is set (at most ndest).  v_cap is the room of d_v (d_v_off[nrows] must not pass it).  The bounds are
+ * v_cap and ndest: out_cap or dest_cap below them is DGX_ERR_CAP at the call, as every argument error of the host form
+ * is DGX_ERR_ARG there, except the offsets of v_off and the column, which are checked on the device.  d_dest_len is
+ * one device uint64.  The order and offset checks, a length word past its room, a list value and a datetime's
+ * nanoseconds run on the device: a refused call writes *d_dest_len = 0 and nothing else, and surfaces as DGX_ERR_ARG
+ * at the next dgx_lane_sync.  ndest == 0 or nrows == 0 writes zero offsets and length without a launch.  Asynchronous
+ * on the lane; launches as the host form's. */
+int dgx_dev_pred_order(dgx_lane* lane, const dgx_val_column* col, int desc, const uint64_t* d_dest, size_t ndest,
+                       const uint64_t* d_ndest, const uint64_t* d_v, const uint64_t* d_v_off, size_t nrows,
+                       size_t v_cap, int32_t count, int32_t offset, uint64_t* d_out, uint64_t* d_out_off,
+                       size_t out_cap, uint64_t* d_dest_out, size_t dest_cap, uint64_t* d_dest_len);
 /* Buckets of the matrix merges that were too large for shared memory and took the slower global-memory sort: of this
  * lane as of its last dgx_lane_sync, or of the whole process for lane == NULL.  Results do not depend on it. */
 uint64_t dgx_merge_matrix_overflows(const dgx_lane* lane);

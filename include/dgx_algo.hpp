@@ -812,6 +812,28 @@ inline std::vector<pb::List> CompareRows(const ValColumn& col, int op, const Val
     return res;
 }
 
+// orderasc / orderdesc by a predicate with no sortable index (query/query.go applyOrderAndPagination's predicate
+// branch with worker/sort.go sortWithoutIndex) in one dgx_pred_order call, in Go's exact order, ties included: each
+// row's dest uids with a value sorted by it, then those without one (absent, or bad) in row order, cut by
+// x.PageRange(count, offset, |row|).  col: DGX_VAL_INT64, DGX_VAL_FLOAT64, DGX_VAL_DATETIME or DGX_VAL_STRING, one
+// value per uid.  A bool column, a negative count or a list value throws Error(DGX_ERR_ARG), where Go errs.
+inline OrderResult OrderByPred(const ValColumn& col, bool desc, const pb::List& dest, const std::vector<pb::List>& rows,
+                               int32_t count = 0, int32_t offset = 0) {
+    const detail::ValCall c(col, ValArgs{});
+    std::vector<uint64_t> v, v_off{0};
+    for (const pb::List& r : rows) { v.insert(v.end(), r.Uids.begin(), r.Uids.end()); v_off.push_back(v.size()); }
+    const size_t nd = dest.Uids.size(), nrows = rows.size();
+    std::vector<uint64_t> out(std::max<size_t>(v.size(), 1)), out_off(nrows + 1), dout(std::max<size_t>(nd, 1));
+    size_t n = 0;
+    check(dgx_pred_order(&c.c, desc ? 1 : 0, dest.Uids.data(), nd, v.data(), v_off.data(), nrows, count, offset,
+                         out.data(), out_off.data(), v.size(), dout.data(), nd, &n));
+    OrderResult res;
+    for (size_t r = 0; r < nrows; ++r)
+        res.rows.emplace_back(std::vector<uint64_t>(out.begin() + out_off[r], out.begin() + out_off[r + 1]));
+    res.dest = pb::List(std::vector<uint64_t>(dout.begin(), dout.begin() + n));
+    return res;
+}
+
 // A regexp() pattern compiled once (dgx_regex_compile; fold is the /i modifier).  Throws Error with DGX_ERR_ARG for a
 // pattern outside the compiled subset or one Go rejects, DGX_ERR_CAP past DGX_REGEX_MAX_STATES: keep Go's matcher then.
 class RegexProg {

@@ -148,6 +148,7 @@ def main():
     ap.add_argument("--c20-only", action="store_true", help="only the C20 orderasc / orderdesc by a value variable rows")
     ap.add_argument("--c21-only", action="store_true", help="only the C21 match() rows")
     ap.add_argument("--c23-only", action="store_true", help="only the C23 compare function rows")
+    ap.add_argument("--c24-only", action="store_true", help="only the C24 orderasc / orderdesc by a predicate rows")
     args = ap.parse_args()
     if args.c6_only:
         rows = c6_rows(Lane())
@@ -183,9 +184,11 @@ def main():
         rows = c21_rows(Lane())
     elif args.c23_only:
         rows = c23_rows(Lane())
+    elif args.c24_only:
+        rows = c24_rows(Lane())
     else:
         rows = run(Lane(), 10 if args.small else 1, quick=False)
-    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only or args.c20_only or args.c21_only or args.c23_only:  # the card and its power limit, read in the same run as the numbers
+    if args.c6_only or args.c7_only or args.c8_only or args.c9_only or args.c10_only or args.c11_only or args.c12_only or args.c13_only or args.c14_only or args.c15_only or args.c16_only or args.c17_only or args.c18_only or args.c19_only or args.c20_only or args.c21_only or args.c23_only or args.c24_only:  # the card and its power limit, read in the same run as the numbers
         import subprocess
 
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -2596,6 +2599,118 @@ def c15_rows(L):
                              "values": m, "launches": launches, "check": bool(ok), "timing": timing})
             print(json.dumps(out_rows[-1]), flush=True)
         del keep
+    return out_rows
+
+
+
+def c24_rows(L):
+    """C24 "orderasc / orderdesc by a predicate without its index" (dgx_pred_order).  C24a: 10 000 rows of about 1e7
+    values over an int64 column of 1e7 uids with 10 % absent, distinct values (tier 1).  C24b: the same matrix over a
+    string column of 10^4 distinct names (tied rows, tier 2 on threads).  C24c: one row of 3e6 uids over datetimes at
+    second resolution with 10^5 distinct instants (the CTA tier).  C24d: one row of 3e6 distinct strings sharing their
+    first 8 bytes (tier 2 on a CTA, byte comparisons).  C24e: a reference test's size (launch-bound).  Every call pages
+    with count 1000, the query layer's default.  Legs: (1) the device form on resident inputs (CUDA events), (2) the
+    host form with its copies (wall clock), (3) the line-by-line restatement (tests/pred_order_oracle.c) on 1 thread --
+    C, not Go.  Every leg is checked against the restatement."""
+    import pred_order_oracle as po
+    from dgraph_b200 import algo
+
+    U64 = np.uint64
+    rng = np.random.default_rng(24)
+
+    def up(x, dt=U64):
+        x = np.concatenate([np.ascontiguousarray(x, dt), np.zeros(1, dt)])
+        return torch.from_numpy(x.view(np.int64) if dt == U64 else x.view(np.int32) if dt == np.uint32 else x).to(DEV)
+
+    def dev_col(col):
+        keep = []
+
+        def d(a, dt=U64):
+            if a is None:
+                return None
+            t = up(a, dt)
+            keep.append(t)
+            return t.data_ptr()
+        if col.type == algo.VAL_STRING:
+            s = col.str
+            sc = _lib.StrColumn(d(s.uid), d(s.val_off), d(s.byte_off), d(s.bytes, np.uint8), s.uid.size,
+                                int(s.byte_off.size - 1), int(s.byte_off[-1]))
+            keep.append(sc)
+            return _lib.ValColumn(col.type, None, None, None, None, None, C.pointer(sc), 0, 0), keep
+        return _lib.ValColumn(col.type, d(col.uid), d(col.val_off), d(col.word), d(col.nsec, np.uint32), None, None,
+                              col.uid.size, int(col.val_off[-1])), keep
+
+    def str_col(uids, width, codes, prefix=b""):
+        """A string column of fixed-width values prefix + the decimal code, built as arrays."""
+        w = len(prefix) + width
+        txt = np.char.zfill(codes.astype(str), width).astype("S%d" % width)
+        buf = np.frombuffer(b"".join([prefix + x for x in txt.tolist()]), np.uint8)
+        boff = np.arange(uids.size + 1, dtype=U64) * U64(w)
+        sc = algo.StrColumn.from_csr(uids, np.arange(uids.size + 1, dtype=U64), boff, buf)
+        return algo.ValColumn.from_arrays(algo.VAL_STRING, str_col=sc)
+
+    nu = 10_000_000
+    uids = np.arange(1, nu + 1, dtype=U64)
+    present = np.sort(uids[rng.random(nu) < 0.9])
+    a_col = algo.ValColumn.from_arrays(algo.VAL_INT64, present, np.arange(present.size + 1, dtype=U64),
+                                       rng.permutation(present.size).astype(np.int64) * 7 - 10 ** 6)
+    rows = []
+    for _ in range(10_000):
+        k = int(rng.integers(800, 1200))
+        s0 = int(rng.integers(0, nu - 4 * k))
+        rows.append(uids[s0:s0 + 4 * k:4][:k].copy())
+    b_col = str_col(present, 5, rng.integers(0, 10_000, present.size), b"name")
+    n3 = 3_000_000
+    u3 = np.arange(1, n3 + 1, dtype=U64)
+    c_col = algo.ValColumn.from_arrays(algo.VAL_DATETIME, u3, np.arange(n3 + 1, dtype=U64),
+                                       (rng.integers(0, 100_000, n3) * 3600 - 10 ** 9).astype(np.int64),
+                                       np.zeros(n3, np.uint32))
+    d_col = str_col(u3, 9, rng.permutation(n3), b"prefix00")
+    e_col = algo.ValColumn(algo.VAL_STRING, [23, 24, 25, 31, 101],
+                           [["Zambo Alice"], ["John Alice"], ["Bob Joe"], ["Allan Matt"], ["John Oliver"]])
+    e_row = np.array([23, 24, 25, 31, 101], U64)
+    work = [("C24a", a_col, False, uids, rows), ("C24b", b_col, False, uids, rows), ("C24c", c_col, True, u3, [u3]),
+            ("C24d", d_col, False, u3, [u3]), ("C24e", e_col, False, e_row, [e_row])]
+    count, offset = 1000, 0
+    out_rows = []
+    for name, col, desc, dest, rws in work:
+        t0 = time.perf_counter()
+        want_rows, want_dest = po.pred_order(col, desc, dest, rws, count, offset)
+        t_or = (time.perf_counter() - t0) * 1e3
+        dcol, keep = dev_col(col)
+        v = np.concatenate(rws)
+        v_off = np.zeros(len(rws) + 1, U64)
+        np.cumsum([r.size for r in rws], out=v_off[1:])
+        nr, m, nd = len(rws), int(v.size), int(dest.size)
+        d_d, d_v, d_vo = up(dest), up(v), up(v_off)
+        d_out = torch.empty(m + 1, dtype=torch.int64, device=DEV)
+        d_off = torch.empty(nr + 1, dtype=torch.int64, device=DEV)
+        d_dest = torch.empty(nd + 1, dtype=torch.int64, device=DEV)
+        d_len = torch.empty(1, dtype=torch.int64, device=DEV)
+
+        def dev():
+            algo.dev_order_by_pred(L.h, dcol, desc, d_d.data_ptr(), nd, d_v.data_ptr(), d_vo.data_ptr(), nr, m,
+                                   d_out.data_ptr(), d_off.data_ptr(), m, d_dest.data_ptr(), nd, d_len.data_ptr(),
+                                   count, offset)
+        ms_dev, _ = timeit(dev, warm=1, reps=5)
+        L.sync()
+        off = d_off.cpu().numpy().view(U64)
+        out = d_out.cpu().numpy().view(U64)
+        k = int(d_len.cpu().numpy()[0])
+        ok_dev = all(np.array_equal(out[int(off[i]):int(off[i + 1])], want_rows[i]) for i in range(nr)) and \
+            np.array_equal(d_dest[:k].cpu().numpy().view(U64), want_dest)
+        del keep
+        t0 = time.perf_counter()
+        h_rows, h_dest = algo.OrderByPred(col, desc, dest, rws, count, offset)
+        ms_host = (time.perf_counter() - t0) * 1e3
+        ok_host = all(np.array_equal(a, b) for a, b in zip(h_rows, want_rows)) and \
+            np.array_equal(h_dest.Uids, want_dest)
+        r = {"op": name, "type": int(col.type), "rows": nr, "values": m, "dest": nd, "desc": desc, "count": count,
+             "ms_resident": ms_dev, "ms_host_form": ms_host, "ms_restatement_1_thread": t_or,
+             "check_resident": bool(ok_dev), "check_host_form": bool(ok_host)}
+        if not QUIET:
+            print(json.dumps(r), flush=True)
+        out_rows.append(r)
     return out_rows
 
 
